@@ -1,11 +1,11 @@
 #!/usr/bin/env python
-"""bench.py — agent-env-steps/sec of the 5x5 large_grid MA2C hot path on N B200s (one node).
+"""bench.py — agent-env-steps/sec of the 5x5 large_grid MA2C hot path on N H100s (one node).
 
 Contract: `python bench.py --gpus N --steps K --warmup W` (N>1: launched by torchrun, one rank
 per GPU).  Prints ONE JSON line on rank 0.
 
 Workload (BASELINE.json configs[2]): 5x5 large_grid, MA2C observation layout (n_s in {32,42,52},
-fingerprints), `--replicas` (default 8192) lock-stepped env replicas PER GPU ("weak" scaling),
+fingerprints), `--replicas` (default 4096) lock-stepped env replicas PER GPU ("weak" scaling),
 synthetic demand of the named grid (large_grid/data/build_file.py flows 1100/925), replica r of
 rank k seeded with seed0 + k*R + r.
 
@@ -74,11 +74,10 @@ def parse():
     p.add_argument("--impl", default="ours", choices=["ours", "reference"])
     p.add_argument("--scenario", default="large_grid", choices=["large_grid", "real_net"],
                    help="large_grid = BASELINE configs[2] (headline); real_net = configs[3] (Monaco MA2C, 2048 replicas)")
-    p.add_argument("--replicas", type=int, default=None, help="env replicas per GPU (default 8192 grid / 2048 Monaco)")
+    p.add_argument("--replicas", type=int, default=None, help="env replicas per GPU (default 4096 grid / 2048 Monaco: the rollout's bf16 activation store and the update buffers fit an 80 GB H100)")
     p.add_argument("--burnin", type=int, default=240)
     p.add_argument("--mode", default=None, choices=[None, "sim", "train"])
-    p.add_argument("--chunk", type=int, default=4096,
-                   help="replicas per update chunk (4096: 1600 BPTT work items = 10.8 waves of 148 CTAs; 1024: 2.7 waves)")
+    p.add_argument("--chunk", type=int, default=1024, help="replicas per update chunk (1024: 400 BPTT work items)")
     p.add_argument("--fp32-gemm", action="store_true", help="plain fp32 (no TF32 tensor cores) in the learner GEMMs")
     p.add_argument("--seed", type=int, default=12)
     p.add_argument("--no-cpu-baseline", action="store_true")
@@ -87,6 +86,8 @@ def parse():
     p.add_argument("--agent", default="ma2c", choices=["ma2c", "ia2c"],
                    help="ma2c = BASELINE configs[2] (the headline workload); ia2c with --policy fc = configs[1]")
     p.add_argument("--policy", default="lstm", choices=["lstm", "fc"], help="fc = FcACPolicy (agents/policies.py:214-256)")
+    p.add_argument("--dump-outputs", default=None, metavar="DIR",
+                   help="after the timed steps, write what the timed path computed in its last step as DIR/<name>.npy")
     p.add_argument("--e2e-parts", type=int, default=4,
                    help="replica ranges of the host-buffer (e2e) loop, one stream each (1: single blocking tsc_step_host)")
     return p.parse_args()
@@ -121,6 +122,24 @@ def algorithmic_bytes(net, v_live):
     """BASELINE.md §3: B_step = 2*V*16 + 2*L*8 + 2*A*4 + 4*A + 4*sum(N_s) + 4*A + 4 + 1."""
     L, A = net.n_lanes, net.n_nodes
     return 2 * v_live * 16 + 2 * L * 8 + 2 * A * 4 + 4 * A + 4 * net.n_obs + 4 * A + 4 + 1
+
+
+def dump_outputs(out_dir, arrays, max_elems=3 << 20, budget_bytes=64 << 20):
+    """Write each array as out_dir/<name>.npy (float64 stays float64, everything else becomes float32), at most
+    `budget_bytes` of array data in all.  An array of more than `max_elems` elements, or more than what is left of the
+    budget, is replaced by the same fixed sample of its elements in every run (seeded indices, ascending)."""
+    os.makedirs(out_dir, exist_ok=True)
+    left = budget_bytes - 4096 * len(arrays)                   # room for the .npy headers
+    for name, a in arrays.items():
+        a = a.detach().cpu().numpy() if hasattr(a, "detach") else np.asarray(a)
+        a = a.astype(np.float64 if a.dtype == np.float64 else np.float32)
+        cap = min(max_elems, left // a.itemsize)
+        if cap <= 0:
+            raise ValueError("--dump-outputs: no budget left for %s" % name)
+        if a.size > cap:
+            a = a.ravel()[np.sort(np.random.default_rng(0).choice(a.size, cap, replace=False))]
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+        left -= a.nbytes
 
 
 # ------------------------------------------------------------------------------------------------
@@ -229,7 +248,7 @@ def main():
     if args.scenario == "real_net":
         args.agent = "ma2c"
     if args.replicas is None:
-        args.replicas = 2048 if args.scenario == "real_net" else 8192
+        args.replicas = 2048 if args.scenario == "real_net" else 4096
     net, par, n_step, reward_norm = build_scenario(args)
     cores = usable_cpus()
     wl = workload_name(args.replicas, mode, args.agent, args.policy, args.scenario)
@@ -307,10 +326,12 @@ def main():
         fp = torch.rand(R, net.n_nodes, net.max_na, device=dev, generator=gen)
         sim_events = []
 
+        last_sim = {}
+
         def one_step(i):
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
-            sim.step(acts[i % n_act_sets], fp)
+            last_sim["out"] = sim.step(acts[i % n_act_sets], fp)
             e1.record()
             sim_events.append((e0, e1))
 
@@ -343,6 +364,13 @@ def main():
     t_end.record()
     barrier()
     total_ms = t_start.elapsed_time(t_end)
+    if args.dump_outputs and rank == 0:
+        if trainer is not None:
+            m = trainer.model
+            outs = {"pi": m.pi, "value": m.val, "action": m.act, "params": m.P}
+        else:
+            outs = dict(zip(("obs", "reward", "global_reward", "done"), last_sim["out"]))
+        dump_outputs(args.dump_outputs, outs)
     evs = trainer.sim_events if trainer is not None else sim_events
     kern_ms = float(np.mean([a.elapsed_time(b) for a, b in evs]))
     update_ms = None
@@ -458,36 +486,16 @@ def main():
     if os.path.exists(peaks_path):
         peak, peak_src = float(json.load(open(peaks_path))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     else:
-        peak, peak_src = 6650.0, "fallback (B200_PROFILING.md)"
+        peak, peak_src = 3350.0, "H100 SXM data sheet (3.35 TB/s), not measured"
     alg_bytes = algorithmic_bytes(net, v_live) * R
     achieved = alg_bytes / (kern_ms * 1e-3) / 1e9
-    traffic, issue = None, None
-    prof = None
-    for name in ("r02_sim_kernel_traffic.json", "r01_sim_kernel_traffic.json"):      # newest ncu capture of the kernel
-        tr_path = os.path.join(ROOT, "profiles", name)
-        if os.path.exists(tr_path):
-            prof = json.load(open(tr_path))
-            break
-    if prof is not None and args.scenario == "large_grid" and prof.get("grid") == R:
-        traffic = prof.get("dram_bytes_per_launch")
-        if prof.get("warp_inst_per_launch"):
-            # second roofline of the same kernel: instruction issue (what actually bounds it).  Warp instructions per
-            # launch come from the committed ncu capture (smsp__inst_executed.sum); the rate uses the launch duration
-            # measured live here; peak = 148 SMs x 4 warp schedulers x 1 instruction / cycle x the sampled SM clock.
-            clk = (sampler.summary().get("sm_mhz") or 1965) * 1e6
-            issue_peak = 148 * 4 * clk
-            issue_rate = float(prof["warp_inst_per_launch"]) / (kern_ms * 1e-3)
-            issue = {"bound": "issue", "achieved": issue_rate / 1e9, "peak": issue_peak / 1e9, "unit": "G warp-inst/s",
-                     "frac": issue_rate / issue_peak, "warp_inst_per_launch": prof["warp_inst_per_launch"],
-                     "source": prof.get("source")}
     roofline = {"bound": "hbm", "kernel": "tsc_step_kernel", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                "frac": achieved / peak, "traffic": traffic, "peak_source": peak_src,
+                "frac": achieved / peak, "peak_source": peak_src,
                 "algorithmic_bytes_per_launch": alg_bytes, "mean_live_vehicles_per_replica": v_live,
                 "kernel_ms_per_launch": kern_ms, "share_of_step": kern_ms * args.steps / total_ms,
-                "issue": issue,
-                "note": "SURVEY 8(d) names HBM as the bound, so `frac` is against the measured copy bandwidth; the kernel is "
-                        "in fact instruction-issue-bound (five fused simulated seconds of Krauss updates per 24-32 B of "
-                        "state per vehicle) - see `issue` and DESIGN.md section 5"}
+                "note": "SURVEY 8(d) names HBM as the bound, so `frac` is against HBM bandwidth; the kernel moves little "
+                        "data per instruction (five fused simulated seconds of Krauss updates per 8 B of state per "
+                        "vehicle), see DESIGN.md section 5"}
     cb = None
     if not args.no_cpu_baseline:
         cb, _, _, _ = cpu_reference(net, par, args, cores, n_step, mode, budget_s=args.cpu_budget)
@@ -499,7 +507,7 @@ def main():
             "config": {"workload": wl, "scenario": args.scenario, "replicas_per_gpu": R, "agents": net.n_nodes,
                        "burnin_control_steps": args.burnin, "mode": mode, "n_step": n_step,
                        "updates_in_timed_region": n_updates_timed, "update_chunk_replicas": args.chunk, "untimed_alignment_steps": align_steps,
-                       "learner_gemm_library": "none: own tcgen05 kernels for the forward, BPTT, dX and all weight gradients; "
+                       "learner_gemm_library": "none: own wgmma kernels for the forward, BPTT, dX and all weight gradients; "
                                                "own SIMT kernels for loss / heads / optimizer"
                        if mode == "train" else None,
                        "l2": "inputs larger than L2: %.0f MB of replica state per GPU is streamed every step"

@@ -25,7 +25,7 @@ SYMBOLS = ["tsc_last_error", "tsc_create", "tsc_destroy", "tsc_reset", "tsc_set_
 
 
 def build_native(force: bool = False, verbose: bool = False) -> str:
-    """Compile csrc/*.cu for sm_100a with nvcc (cross-compiles without a GPU)."""
+    """Compile csrc/*.cu for sm_90a (H100) with nvcc (cross-compiles without a GPU)."""
     cmd = ["make", "-C", CSRC] + (["-B"] if force else [])
     out = subprocess.run(cmd, capture_output=True, text=True)
     if out.returncode != 0:

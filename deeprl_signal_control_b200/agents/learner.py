@@ -11,8 +11,8 @@ Device-side counterpart of reference agents/models.py (IA2C/MA2C) + agents/polic
 Replicas share the weights: the gradient is the mean over replicas (and over ranks: one
 `all_reduce(SUM)` of the flat gradient per update, then identical updates everywhere).
 
-Shipping path (`use_tc`, the default): every kernel is hand-written — the fused tcgen05 forward
-(csrc/tsc_policy_tc.cu: fc front end, gate GEMM, LSTM cell, heads, sampling, bf16 activation store), the tcgen05
+Shipping path (`use_tc`, the default): every kernel is hand-written — the fused wgmma forward
+(csrc/tsc_policy_tc.cu: fc front end, gate GEMM, LSTM cell, heads, sampling, bf16 activation store), the wgmma
 update (BPTT with TMA operand copies, dX = dZ.Wx^T, LSTM and fc weight gradients) and the SIMT kernels of
 csrc/tsc_learn.cu (loss / head gradients, returns, clip + RMSProp).  No library GEMM runs on it.
 `use_tc=False` selects the plain fp32 twin kernels (fc_embed, lstm_seq_fwd / bwd, heads, fc_bwd) that the reference
@@ -103,8 +103,8 @@ class BatchedA2C:
                               device=self.dev)
         self.Wt = torch.zeros(U, 32, L.h, 8, dtype=torch.bfloat16, device=self.dev)    # Wh^T image for the BPTT MMA
         self.Wxt = torch.zeros(U, 32, L.dx, 8, dtype=torch.bfloat16, device=self.dev)  # Wx^T image: dX fused into the BPTT
-        # measured (R = 8192, 1 x B200): fusing dX into the BPTT step lengthens the serial per-step chain (update 72.5 ->
-        # 92.5 ms), so the default keeps dX as a separate product; `dx_fused = True` selects the fused kernel (tested)
+        # fusing dX into the BPTT step lengthens its serial per-step chain, so the default keeps dX as a separate
+        # product; `dx_fused = True` selects the fused kernel (tested)
         self.dx_fused = False
         self.dx_fusable = self.use_tc and L.dx % 32 == 0 and L.dx <= 256
         # stand-alone dX = dZ . Wx^T kernel (tscl_dx_tc); False falls back to the library GEMM (A/B measurements only)
@@ -409,7 +409,7 @@ class BatchedA2C:
                 self.gv["wx"].baddbmm_(X.transpose(1, 2), dZ)
                 self.gv["wh"].baddbmm_(Hp.transpose(1, 2), dZ)
                 self.gv["bl"].add_(dZ.sum(dim=1))
-            # dX = dZ . Wx^T: own warp-specialised tcgen05 kernel on the shipping path (tscl_dx_tc); a library GEMM only on
+            # dX = dZ . Wx^T: own warp-specialised wgmma kernel on the shipping path (tscl_dx_tc); a library GEMM only on
             # the fp32 twin path, for dx > 224 and under TSC_DX_LIBRARY=1 (A/B measurements)
             if all_tc and not fuse_dx and self.dx_own:
                 _lib.check(lib.tscl_dx_tc(self._h, _p(dZb), _p(self.Wxt), _p(dXb), C.c_int64(M), st()))

@@ -25,7 +25,7 @@ from .learner import BatchedA2C, _p
 class BatchedFcA2C(BatchedA2C):
     def __init__(self, layout: PolicyLayout, n_replicas: int, n_step: int, **kw):
         assert not layout.recurrent, "BatchedFcA2C needs PolicyLayout(recurrent=False)"
-        kw["use_tc"] = False               # the fused tcgen05 forward / BPTT kernels are LSTM-specific
+        kw["use_tc"] = False               # the fused tensor-core forward / BPTT kernels are LSTM-specific
         kw["store_acts"] = False
         super().__init__(layout, n_replicas, n_step, **kw)
         self.fc_bwd_tc = layout.fc_bwd_tc_ok      # front-end weight gradients on the tensor cores (fp32 inputs)

@@ -1,4 +1,4 @@
-// tsc_learn.cu — hand-written sm_100a kernels of the per-intersection A2C learner + C ABI
+// tsc_learn.cu — hand-written sm_90a (H100) kernels of the per-intersection A2C learner + C ABI
 // (include/tsc_learn.h).  fp32 storage and arithmetic (the reference is fp32 TF1).
 //
 //   fc_embed_kernel       relu(fc) front end of all 2A networks            agents/policies.py:191-201
@@ -16,6 +16,8 @@
 #include <stdint.h>
 
 #include <string>
+#include <map>
+#include <mutex>
 #include <vector>
 
 #include "../../include/tsc_learn.h"
@@ -46,6 +48,8 @@ struct tscl_handle {
   std::vector<void*> owned;
   int max_in = 0;      // max n_wave + n_wait + n_fp
   int max_fcw = 0;     // max fc weight floats of a unit (incl. biases)
+  std::map<void*, float*> acc_tiles;   // accumulator tiles of the tensor-core kernels, per stream (tscl_acc_tiles)
+  std::mutex acc_mu;
 };
 
 __device__ __forceinline__ float sigmoidf_(float x) { return 1.0f / (1.0f + __expf(-x)); }
@@ -331,7 +335,7 @@ __global__ void returns_kernel(const float* __restrict__ rew, const float* __res
 #define HL_GX 96
 #define HL_LD 68                       // row pitch in floats: 16-byte aligned rows, conflict-free 128-bit row-owner accesses
 #define HL_DL 12                       // dlog (8) | dv | pad
-// Shared-memory traffic bounds this kernel (ncu: short scoreboard 6.3, mio throttle 3.3 per issue): rows and the head
+// Shared-memory traffic bounds this kernel: rows and the head
 // weights are therefore moved with 128-bit accesses only (Wp padded to 8 logits per hidden unit = two broadcast loads).
 __global__ void __launch_bounds__(128)
 heads_loss_kernel(const DDims d, const float* __restrict__ P, const float* __restrict__ Hm,
@@ -379,10 +383,9 @@ heads_loss_kernel(const DDims d, const float* __restrict__ P, const float* __res
       for (int k4 = 0; k4 < H64 / 4; ++k4) myH4[k4] = __ldg(p4 + k4);
     }
   };
-  auto st8 = [](float* p, const float* v) {      // 256-bit store: one full sector per thread and instruction
-    asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "r"(__float_as_uint(v[0])),
-                 "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])), "r"(__float_as_uint(v[3])), "r"(__float_as_uint(v[4])),
-                 "r"(__float_as_uint(v[5])), "r"(__float_as_uint(v[6])), "r"(__float_as_uint(v[7])) : "memory");
+  auto st8 = [](float* p, const float* v) {      // one 32-byte sector per thread: two 128-bit stores
+    reinterpret_cast<float4*>(p)[0] = make_float4(v[0], v[1], v[2], v[3]);
+    reinterpret_cast<float4*>(p)[1] = make_float4(v[4], v[5], v[6], v[7]);
   };
   for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
     const int64_t m = tile * 128 + tid;
@@ -651,7 +654,7 @@ fc_bwd_kernel(const DDims d, const float* __restrict__ obs, const float* __restr
       const int rows = (M - m0) < FB_ROWS ? (int)(M - m0) : FB_ROWS;
       const int64_t o0 = ((int64_t)u * M + m0) * dx + col;
       // rows in groups of 8: all 16 global loads of a group are issued before they are consumed
-      // (16-row groups were measured 2x slower: register pressure)
+      // (16-row groups need too many registers)
       for (int r0 = 0; r0 < rows; r0 += 8) {
         float g[8];
 #pragma unroll
@@ -937,6 +940,14 @@ fc_hidden_wgrad_kernel(const DDims d, const float* __restrict__ X, const float* 
 struct DDimsTC;
 const DDimsTC* tscl_dims_of(tscl_handle* h) { return reinterpret_cast<const DDimsTC*>(&h->d); }
 int tscl_device_of(tscl_handle* h) { return h->device; }
+// `bytes` of device memory for the accumulator tiles of kernels launched on `stream`; allocated on first use, freed with
+// the handle (every caller asks for the same size)
+float* tscl_acc_tiles(tscl_handle* h, void* stream, size_t bytes) {
+  std::lock_guard<std::mutex> lock(h->acc_mu);
+  float*& p = h->acc_tiles[stream];
+  if (!p && cudaMalloc(&p, bytes) != cudaSuccess) p = nullptr;
+  return p;
+}
 
 // ================================================================================================
 template <class T>
@@ -998,6 +1009,7 @@ extern "C" int tscl_destroy(tscl_handle* h) {
   if (!h) return 0;
   cudaSetDevice(h->device);
   for (void* p : h->owned) cudaFree(p);
+  for (auto& e : h->acc_tiles) cudaFree(e.second);
   delete h;
   return 0;
 }
@@ -1144,7 +1156,9 @@ extern "C" int tscl_unpack_store(tscl_handle* h, const void* st_x, const void* s
   if (!h || !st_x || T <= 0 || rc <= 0) return tsc_set_error("tscl_unpack_store: bad argument");
   LCK(cudaSetDevice(h->device));
   const int64_t rows = (int64_t)2 * h->d.A * T * rc;
-  unpack_store_kernel<<<148 * 8, 256, 0, (cudaStream_t)stream>>>(
+  int n_sm = 0;
+  LCK(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, h->device));
+  unpack_store_kernel<<<n_sm * 8, 256, 0, (cudaStream_t)stream>>>(
       (const uint4*)st_x, (const uint4*)st_g, (const uint4*)st_c, (const uint4*)st_h, (float4*)X, (float4*)ZG, (float4*)Cc,
       (float4*)H, (float4*)Hp, h0, done, rows * h->d.dx / 8, rows * G4 / 8, rows * H64 / 8, T, rc, ld_state, r0);
   LCK(cudaGetLastError());
@@ -1170,7 +1184,7 @@ extern "C" int tscl_clip_rmsprop(tscl_handle* h, float* params, float* grads, fl
 
 // ------------------------------------------------------------------------------------------------
 // Host-buffer (e2e) loop helpers: one call per replica range and control step replaces a dozen framework-level
-// copies / elementwise launches (the host loop was issue-bound: 0.22 ms of Python per range and step).
+// copies / elementwise launches (a host loop of Python-level copies is bound by launch issue).
 //   tscl_host_transition: observations host -> rollout slot, rewards host -> normalised / clipped rollout slot
 //   (envs/env.py reward hand-over + agents/models.py:222-229 `add_transition`, utils.py reward_norm / reward_clip),
 //   global rewards host -> running episode sum (utils.py:296-305).

@@ -1,19 +1,17 @@
-// tsc_policy_tc.cu — fused per-control-step policy forward on the 5th-gen tensor cores (sm_100a).
+// tsc_policy_tc.cu — fused per-control-step policy forward and the learner's GEMMs on the Hopper tensor cores (sm_90a).
 //
-// One persistent CTA (256 threads, 1 per SM, ~223 KB smem) walks (unit, 128-replica tile) work items:
-//   1. SIMT fc front end (agents/policies.py:191-201): relu(fc) of the observation slice, written as
-//      bf16 straight into the A-operand tile in shared memory (UMMA K-major, no swizzle), followed by
-//      the previous hidden state h (masked by the pre-decision done flag, agents/utils.py:104-105);
-//   2. one elected thread issues K/16 `tcgen05.mma.cta_group::1.kind::f16` (M=128, N=256, bf16 x bf16
-//      -> fp32) against the packed [Wx;Wh] operand that stays resident in shared memory; the
-//      accumulator lives in TMEM (256 columns); completion via tcgen05.commit -> mbarrier;
-//   3. epilogue: every thread owns one replica row (TMEM lane) and 32 hidden units: tcgen05.ld of the
-//      four gate pre-activations, bias, LSTM cell (agents/utils.py:106-113), state write-back, head
-//      dot products (agents/policies.py:18-26), then softmax / value / categorical sample
-//      (utils.py:155-157) for the row.
+// One persistent CTA (1 per SM, up to ~223 KB smem) walks (unit, 128-replica tile) work items:
+//   1. fc front end (agents/policies.py:191-201): relu(fc) of the observation slice, written as bf16 straight into
+//      the A-operand tile in shared memory (K-major, no swizzle), followed by the previous hidden state h (masked by
+//      the pre-decision done flag, agents/utils.py:104-105);
+//   2. warps 0-7 (two warpgroups, 64 rows each) run wgmma.mma_async m64nNk16 (bf16 x bf16 -> fp32) against the packed
+//      [Wx;Wh] operand that stays resident in shared memory, and store the accumulators to the CTA's accumulator tile;
+//   3. epilogue: every thread owns one replica row and a group of hidden units: the four gate pre-activations, bias,
+//      LSTM cell (agents/utils.py:106-113), state write-back, head dot products (agents/policies.py:18-26), then
+//      softmax / value / categorical sample (utils.py:155-157) for the row.
 // Replaces per step: fc_embed_kernel + library GEMM + lstm_seq_fwd_kernel(T=1) + heads_kernel.
 //
-// Operand layouts (bytes, 16-byte "core rows", no swizzle; cute canonical ((8,n),2):((1,SBO),LBO)):
+// Operand layouts (bytes, 16-byte "core rows", no swizzle; canonical ((8,n),2):((1,SBO),LBO)):
 //   A tile  [KC][128 rows][16 B]   : LBO = 2048 (next K chunk of 8 bf16), SBO = 128 (next 8 rows)
 //   B tile  [KC][256 cols][16 B]   : LBO = 4096,                          SBO = 128
 #include <cuda.h>
@@ -42,6 +40,7 @@ struct DDimsTC {   // mirror of DDims in tsc_learn.cu (kept in sync by tscl_hand
 };
 const DDimsTC* tscl_dims_of(tscl_handle* h);   // defined in tsc_learn.cu
 int tscl_device_of(tscl_handle* h);
+float* tscl_acc_tiles(tscl_handle* h, void* stream, size_t bytes);   // defined in tsc_learn.cu
 
 #define TC_M 128
 #define TC_N 256
@@ -55,9 +54,22 @@ int tscl_device_of(tscl_handle* h);
 
 // ---------------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+// ---- Hopper tensor cores ------------------------------------------------------------------------------
+// wgmma.mma_async: a warpgroup (4 warps) computes a 64-row slab of a product whose operands sit in shared memory,
+// described by matrix descriptors (core matrices of 8 rows x 16 bytes).  The two warpgroups of warps 0-7 cover the
+// 128 rows of a tile.  Their fp32 accumulator fragments are stored to the CTA's accumulator tile, 128 rows x ACC_COLS
+// fp32 in global memory (one tile per CTA and stream, see acc_tiles(); the tile of a CTA is written and read back by
+// the same SM within microseconds, so the round trip normally stays in L1/L2), which the row-per-thread epilogues read
+// back at address (row base << 16) + column, row = row base + lane.  This keeps the epilogues' thread = row mapping;
+// an epilogue that works on the wgmma register fragments directly would save the round trip (DESIGN.md §5).
+#define ACC_COLS 512
 __device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
   return (uint64_t)((saddr >> 4) & 0x3FFFu) | ((uint64_t)((lbo >> 4) & 0x3FFFu) << 16) |
-         ((uint64_t)((sbo >> 4) & 0x3FFFu) << 32) | (1ull << 46);   // version = 1 (Blackwell), no swizzle
+         ((uint64_t)((sbo >> 4) & 0x3FFFu) << 32);   // layout type 0: no swizzle
+}
+// the same operand `n` rows / columns further along M or N (n a multiple of 8): core-matrix groups are SBO apart
+__device__ __forceinline__ uint64_t desc_adv_mn(uint64_t desc, int n) {
+  return desc + ((desc >> 32) & 0x3FFFu) * (uint64_t)(n >> 3);
 }
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
@@ -69,31 +81,93 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
                  : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
   } while (!ok);
 }
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accum) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(accum) : "memory");
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n16(float (&d)[8], uint64_t da, uint64_t db, uint32_t accum) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, %11, %12;\n\t}"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+               : "l"(da), "l"(db), "r"(accum), "n"(TA), "n"(TB) : "memory");
 }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n32(float (&d)[16], uint64_t da, uint64_t db, uint32_t accum) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, %19, %20;\n\t}"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+               : "l"(da), "l"(db), "r"(accum), "n"(TA), "n"(TB) : "memory");
 }
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float* v) {
-  uint32_t r[16];
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                 "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-               : "r"(taddr));
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t da, uint64_t db, uint32_t accum) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, %35, %36;\n\t}"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+               : "l"(da), "l"(db), "r"(accum), "n"(TA), "n"(TB) : "memory");
+}
+
+// one NC-column chunk of D[128 x N] = sum_ks A_ks . B_ks into columns col0 + c .. of the accumulator tile
+// (accum: add to what the tile holds).  descs(ks, da, db) gives the descriptors of the whole 128-row A tile and of B.
+template <int NC, int TA, int TB, class F>
+__device__ __forceinline__ void wg_mma_chunk(float* tile, int col0, int c, int KS, bool accum, const F& descs) {
+  constexpr int NR = NC / 2;
+  const int tid = threadIdx.x, g = tid >> 7, lane = tid & 31;
+  const int row = g * 64 + ((tid >> 5) & 3) * 16 + (lane >> 2);
+  float* p0 = tile + (size_t)row * ACC_COLS + col0 + c + 2 * (lane & 3);
+  float* p1 = p0 + 8 * ACC_COLS;
+  float dd[NR];
 #pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, float* v) {
-  uint32_t r[8];
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr));
+  for (int j = 0; j < NR / 4; ++j) {
+    float2 x = make_float2(0.f, 0.f), y = x;
+    if (accum) { x = *reinterpret_cast<const float2*>(p0 + 8 * j); y = *reinterpret_cast<const float2*>(p1 + 8 * j); }
+    dd[4 * j] = x.x; dd[4 * j + 1] = x.y; dd[4 * j + 2] = y.x; dd[4 * j + 3] = y.y;
+  }
+  asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+  for (int ks = 0; ks < KS; ++ks) {
+    uint64_t da, db;
+    descs(ks, da, db);
+    da = desc_adv_mn(da, 64 * g);
+    db = desc_adv_mn(db, c);
+    const uint32_t acc = (accum || ks > 0) ? 1u : 0u;
+    if constexpr (NC == 64) wgmma_n64<TA, TB>(dd, da, db, acc);
+    else if constexpr (NC == 32) wgmma_n32<TA, TB>(dd, da, db, acc);
+    else wgmma_n16<TA, TB>(dd, da, db, acc);
+  }
+  asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+  asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
 #pragma unroll
-  for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[i]);
+  for (int i = 0; i < NR; ++i) asm volatile("" : "+f"(dd[i])::"memory");
+#pragma unroll
+  for (int j = 0; j < NR / 4; ++j) {
+    *reinterpret_cast<float2*>(p0 + 8 * j) = make_float2(dd[4 * j], dd[4 * j + 1]);
+    *reinterpret_cast<float2*>(p1 + 8 * j) = make_float2(dd[4 * j + 2], dd[4 * j + 3]);
+  }
+}
+// D[128 x N] (N a multiple of 16) into tile columns col0 .. col0 + N; executed by all threads of warps 0-7.
+// TA / TB: 0 = K-major, 1 = MN-major operand.
+template <int TA, int TB, class F>
+__device__ __forceinline__ void wg_mma(float* tile, int col0, int N, int KS, bool accum, const F& descs) {
+  int c = 0;
+  for (; c + 64 <= N; c += 64) wg_mma_chunk<64, TA, TB>(tile, col0, c, KS, accum, descs);
+  if (c + 32 <= N) { wg_mma_chunk<32, TA, TB>(tile, col0, c, KS, accum, descs); c += 32; }
+  if (c + 16 <= N) wg_mma_chunk<16, TA, TB>(tile, col0, c, KS, accum, descs);
+}
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
+}
+// warps 0-7 have stored their fragments: publish them to the CTA and arrive (once) on `bar`
+__device__ __forceinline__ void wg_mma_done(uint32_t bar) {
+  __threadfence_block();
+  asm volatile("bar.sync 1, 256;" ::: "memory");
+  if (threadIdx.x == 0) mbar_arrive(bar);
+}
+// 16 / 8 consecutive accumulator columns of row (addr >> 16) + lane
+__device__ __forceinline__ void acc_ld16(const float* tile, uint32_t addr, float* v) {
+  const float4* p = reinterpret_cast<const float4*>(tile + (size_t)((addr >> 16) + (threadIdx.x & 31)) * ACC_COLS + (addr & 0xFFFFu));
+#pragma unroll
+  for (int i = 0; i < 4; ++i) { const float4 x = p[i]; v[4 * i] = x.x; v[4 * i + 1] = x.y; v[4 * i + 2] = x.z; v[4 * i + 3] = x.w; }
+}
+__device__ __forceinline__ void acc_ld8(const float* tile, uint32_t addr, float* v) {
+  const float4* p = reinterpret_cast<const float4*>(tile + (size_t)((addr >> 16) + (threadIdx.x & 31)) * ACC_COLS + (addr & 0xFFFFu));
+#pragma unroll
+  for (int i = 0; i < 2; ++i) { const float4 x = p[i]; v[4 * i] = x.x; v[4 * i + 1] = x.y; v[4 * i + 2] = x.z; v[4 * i + 3] = x.w; }
 }
 
 __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
@@ -117,6 +191,15 @@ __device__ __forceinline__ uint32_t pmix32(uint32_t h) {
 }
 
 // ---------------------------------------------------------------------------------------------------
+// Accumulator tiles of the tensor-core kernels: one [128][ACC_COLS] fp32 tile per CTA, grids of at most two CTAs per SM
+// (tscl_acc_tiles: owned by the handle, one set per stream, so that kernels running concurrently on different streams
+// never share one)
+static float* acc_tiles(tscl_handle* h, void* stream) {
+  int n_sm = 0;
+  if (cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, tscl_device_of(h)) != cudaSuccess) return nullptr;
+  return tscl_acc_tiles(h, stream, (size_t)2 * n_sm * TC_M * ACC_COLS * sizeof(float));
+}
+
 // per-unit stride of the packed image: main [KC][256][8] followed by the fc image [8][dx][8]
 __host__ __device__ inline int64_t wp_stride(int dx) { return (int64_t)((dx + TC_H) / 8) * TC_N * 8 + (int64_t)8 * dx * 8; }
 
@@ -162,6 +245,7 @@ __global__ void pack_fc_kernel(const DDimsTC d, const float* __restrict__ P, __n
 }
 
 struct StepTC {
+  float* acc;                // accumulator tiles, one [128][ACC_COLS] fp32 tile per CTA (acc_tiles)
   const float* P;
   const __nv_bfloat16* Wp;
   const float* obs;        // [R][n_obs]
@@ -203,24 +287,16 @@ policy_step_tc_kernel(const DDimsTC d, const StepTC a) {
   float* sBo = sWo + TC_H * 8;                                  // [8]
   float* sBias = sBo + 8;                                       // [256]
   uint64_t* sBar = reinterpret_cast<uint64_t*>(sBias + TC_N);   // mbarrier
-  uint32_t* sTmem = reinterpret_cast<uint32_t*>(sBar + 1);      // TMEM base address
   float* sRed = sStage;
 
   const uint32_t bar = smem_u32(sBar);
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(sTmem)), "r"(256));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
   if (tid == 0) {
     mbar_init(bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem = *sTmem;
+  float* const acc = a.acc + (size_t)blockIdx.x * TC_M * ACC_COLS;
   // instruction descriptor: D=f32, A=B=bf16, K-major both, N=256, M=128
-  const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(TC_N >> 3) << 17) | ((uint32_t)(TC_M >> 4) << 24);
 
   const int64_t n_tiles = (a.R + TC_M - 1) / TC_M;
   const int64_t n_items = n_tiles * 2 * d.A;
@@ -330,29 +406,22 @@ policy_step_tc_kernel(const DDimsTC d, const StepTC a) {
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     __syncthreads();
     // ---- 2. MMA: D[128 x 256] = A[128 x K] . B[K x 256] ----
-    if (warp == 0) {
-      if (lane == 0) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t aA = smem_u32(sA), aB = smem_u32(sB);
-        for (int ks = 0; ks < KS; ++ks) {
-          uint64_t da, db;
-          if (!a.swap_lbo_sbo) {
-            da = make_desc(aA + ks * 2 * 2048, 2048, 128);
-            db = make_desc(aB + ks * 2 * 4096, 4096, 128);
-          } else {
-            da = make_desc(aA + ks * 2 * 2048, 128, 2048);
-            db = make_desc(aB + ks * 2 * 4096, 128, 4096);
-          }
-          umma_bf16(tmem, da, db, idesc, ks > 0 ? 1u : 0u);
+    if (warp < 8) {
+      const uint32_t aA = smem_u32(sA), aB = smem_u32(sB);
+      wg_mma<0, 0>(acc, 0, TC_N, KS, false, [&](int ks, uint64_t& da, uint64_t& db) {
+        if (!a.swap_lbo_sbo) {
+          da = make_desc(aA + ks * 2 * 2048, 2048, 128);
+          db = make_desc(aB + ks * 2 * 4096, 4096, 128);
+        } else {
+          da = make_desc(aA + ks * 2 * 2048, 128, 2048);
+          db = make_desc(aB + ks * 2 * 4096, 128, 4096);
         }
-        umma_commit(bar);
-      }
-      __syncwarp();
+      });
+      wg_mma_done(bar);
     }
     mbar_wait(bar, parity);
     parity ^= 1;
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    // ---- 3. epilogue: thread = (row = TMEM lane, 32 hidden units) ----
+    // ---- 3. epilogue: thread = (row of the accumulator tile, 32 hidden units) ----
     {
       const int q = warp & 3, half = warp >> 2;
       const int row = q * 32 + lane;
@@ -365,9 +434,8 @@ policy_step_tc_kernel(const DDimsTC d, const StepTC a) {
 #pragma unroll
       for (int jb = 0; jb < 2; ++jb) {
         float zi[16], zf[16], zo[16], zu[16];
-        const uint32_t tbase = tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(half * 32 + jb * 16);
-        tmem_ld16(tbase, zi); tmem_ld16(tbase + 64, zf); tmem_ld16(tbase + 128, zo); tmem_ld16(tbase + 192, zu);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+        const uint32_t tbase = ((uint32_t)(q * 32) << 16) + (uint32_t)(half * 32 + jb * 16);
+        acc_ld16(acc, tbase, zi); acc_ld16(acc, tbase + 64, zf); acc_ld16(acc, tbase + 128, zo); acc_ld16(acc, tbase + 192, zu);
         if (a.zdbg && valid) {
           float* z = a.zdbg + ((int64_t)u * a.R + r) * TC_N + half * 32 + jb * 16;
 #pragma unroll
@@ -406,8 +474,7 @@ policy_step_tc_kernel(const DDimsTC d, const StepTC a) {
           }
         }
       }
-      // all TMEM reads of this tile are done before the next tile's MMA may overwrite the accumulator
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+      // all accumulator reads of this tile are done before the next tile's MMA may overwrite the accumulator
       __syncthreads();     // also: sStage (aliased by sRed) is free
       if (half == 1) {
 #pragma unroll
@@ -448,7 +515,6 @@ policy_step_tc_kernel(const DDimsTC d, const StepTC a) {
     }
   }
   __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(256));
 }
 
 // ===================================================================================================
@@ -491,6 +557,8 @@ extern "C" int tscl_policy_step(tscl_handle* h, const float* params, const void*
   const int64_t n_items = ((R + TC_M - 1) / TC_M) * 2 * d.A;
   const int grid = (int)(n_items < n_sm ? n_items : n_sm);
   StepTC a;
+  a.acc = acc_tiles(h, stream);
+  if (!a.acc) return tsc_set_error("accumulator tiles: cudaMalloc failed");
   a.P = params; a.Wp = (const __nv_bfloat16*)wpack_bf16; a.obs = obs; a.c_in = c_in; a.h_in = h_in; a.c_out = c_out;
   a.h_out = h_out; a.pi = pi; a.val = val; a.act = act; a.zdbg = zdbg; a.R = R; a.done = done;
   a.swap_lbo_sbo = swap_lbo_sbo; a.seed_lo = (uint32_t)seed; a.seed_hi = (uint32_t)(seed >> 32);
@@ -505,9 +573,9 @@ extern "C" int tscl_policy_step(tscl_handle* h, const float* params, const void*
 // v2: the fc front end also runs on the tensor cores.
 //   A0 = observation slice tile [128 x 64] (wave32|fp16|wait16, bf16) staged in the LAST 8 K-chunks of the A tile,
 //   B0 = block-diagonal fc weights [64 x dx] staged in the FIRST chunks of the A tile (both regions are dead
-//        until the fc result is written / the h part is loaded), D0 = TMEM columns 256..256+dx;
-//   TMEM -> registers -> (+bias, relu, bf16) -> A tile chunks 0..dx/8, then h_prev -> last 8 chunks, then the
-//   gate MMA and the epilogue exactly as in v1.  Two tcgen05.commit per tile on one mbarrier.
+//        until the fc result is written / the h part is loaded), D0 = accumulator columns 256..256+dx;
+//   accumulator tile -> (+bias, relu, bf16) -> A tile chunks 0..dx/8, then h_prev -> last 8 chunks, then the
+//   gate MMA and the epilogue exactly as in v1.  Two MMA completions per tile on one mbarrier.
 // NT = 256: thread = (replica row, 32 hidden units); NT = 512: thread = (replica row, 16 hidden units) — twice the warps
 // per SM for the latency-bound staging / epilogue phases (one CTA per SM either way: the weight operand fills shared
 // memory), same arithmetic per element, so both variants produce identical bits.
@@ -532,22 +600,13 @@ policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
   float* sBias = sBo + 8;                                       // [256]  lstm bias
   float* sBias0 = sBias + TC_N;                                 // [256]  fc biases
   uint64_t* sBar = reinterpret_cast<uint64_t*>(sBias0 + TC_N);
-  uint32_t* sTmem = reinterpret_cast<uint32_t*>(sBar + 2);
   const uint32_t bar = smem_u32(sBar), bar_fc = smem_u32(sBar + 1);   // MMA completion; fc-weight bulk copy landed
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(sTmem)), "r"(512));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
   if (tid == 0) {
     mbar_init(bar, 1); mbar_init(bar_fc, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem = *sTmem;
-  const uint32_t idesc1 = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(TC_N >> 3) << 17) | ((uint32_t)(TC_M >> 4) << 24);
-  const uint32_t idesc0 = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(d.dx >> 3) << 17) | ((uint32_t)(TC_M >> 4) << 24);
+  float* const acc = a.acc + (size_t)blockIdx.x * TC_M * ACC_COLS;
   const int64_t n_tiles = (a.R + TC_M - 1) / TC_M;
   const int64_t ld = a.ld > 0 ? a.ld : a.R;
   const int64_t n_items = n_tiles * 2 * d.A;
@@ -575,7 +634,7 @@ policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
     // NT = 512: no block-wide barrier here.  Warps 0-3 may still be in the previous tile's head softmax / sampling (they read
     // sRed, sRed2 = sA + 32 KB, sBo) while warps 4-15 already fetch and stage this tile's observation slice (last 8 chunks
     // of sA) and the fc-weight block (first 28 KB of sA); the barrier after the staging retires the previous tile.
-    if (NT != 512 || u != cur_u) __syncthreads();      // previous tile fully retired (sRed, sA, sBo, TMEM readers)
+    if (NT != 512 || u != cur_u) __syncthreads();      // previous tile fully retired (sRed, sA, sBo, accumulator readers)
     if (u != cur_u) {
       cur_u = u;
       const uint4* src = reinterpret_cast<const uint4*>(Wu);
@@ -624,7 +683,7 @@ policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
       // fc weights (one contiguous 8 * dx * 16-byte block of the packed image) by ONE bulk copy (TMA unit, completion on
       // bar_fc): it overlaps the observation staging below; only the MMA-issuing thread waits for it
       // NT = 512: the copy for every tile but the CTA's first was issued right after the previous tile's gate MMA had
-      // completed (the whole epilogue hides its ~3 k cycles)
+      // completed (the whole epilogue hides it)
       if (tid == NT - 1 && (NT != 512 || it == it_lo)) {
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // earlier generic-proxy stores to the A tile precede this async write
         mbar_expect_tx(bar_fc, (uint32_t)(8 * d.dx * 16));
@@ -682,19 +741,14 @@ policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     __syncthreads();
     PROF_MARK(1);      // staging: fc weights + observation slice
-    // ---- 2. MMA0: D0[128 x dx] = A0[128 x 64] . B0[64 x dx]  (TMEM columns 256..) ----
-    if (warp == 0) {
-      if (lane == 0) {
-        mbar_wait(bar_fc, par_fc);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        for (int ks = 0; ks < 4; ++ks) {
-          const uint64_t da = make_desc(aA + (KC - 8 + 2 * ks) * 2048, 2048, 128);
-          const uint64_t db = make_desc(aA + ks * 2 * (d.dx * 16), d.dx * 16, 128);
-          umma_bf16(tmem + 256, da, db, idesc0, ks > 0 ? 1u : 0u);
-        }
-        umma_commit(bar);
-      }
-      __syncwarp();
+    // ---- 2. MMA0: D0[128 x dx] = A0[128 x 64] . B0[64 x dx]  (accumulator columns 256..) ----
+    if (warp < 8) {
+      mbar_wait(bar_fc, par_fc);
+      wg_mma<0, 0>(acc, 256, d.dx, 4, false, [&](int ks, uint64_t& da, uint64_t& db) {
+        da = make_desc(aA + (KC - 8 + 2 * ks) * 2048, 2048, 128);
+        db = make_desc(aA + ks * 2 * (d.dx * 16), d.dx * 16, 128);
+      });
+      wg_mma_done(bar);
     }
     par_fc ^= 1;
     // h_{t-1} of this thread's (row, hidden-unit group): requested before the MMA wait, staged after the relu epilogue
@@ -708,7 +762,6 @@ policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
     }
     mbar_wait(bar, parity);
     parity ^= 1;
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
     PROF_MARK(2);      // MMA0 issue + wait
     // ---- 3. X = relu(D0 + b) as bf16 -> A tile chunks 0..dx/8 ; h_prev -> last 8 chunks ----
     {
@@ -719,10 +772,9 @@ policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
       const int64_t m = st ? store_row(row) : 0;
       const int cend = (hw + 1) * ncol;
       for (int c0 = hw * ncol; c0 < cend;) {
-        if (NT == 512 && (c0 & 15) == 0 && c0 + 16 <= cend) {      // 16 columns: one 256-bit store of the activation row
+        if (NT == 512 && (c0 & 15) == 0 && c0 + 16 <= cend) {      // 16 columns: two 128-bit stores of the activation row
           float z[16];
-          tmem_ld16(tmem + ((uint32_t)(q * 32) << 16) + 256u + (uint32_t)c0, z);
-          asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+          acc_ld16(acc, ((uint32_t)(q * 32) << 16) + 256u + (uint32_t)c0, z);
           __align__(32) __nv_bfloat16 v[16];
 #pragma unroll
           for (int e = 0; e < 16; ++e) v[e] = __float2bfloat16_rn(fmaxf(z[e] + sBias0[c0 + e], 0.f));
@@ -730,14 +782,13 @@ policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
           *reinterpret_cast<uint4*>(sA + (size_t)((c0 >> 3) + 1) * 2048 + row * 16) = *reinterpret_cast<const uint4*>(v + 8);
           if (st) {
             const uint4 x = reinterpret_cast<const uint4*>(v)[0], y = reinterpret_cast<const uint4*>(v)[1];
-            asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(a.st_x + (m * d.dx + c0)), "r"(x.x), "r"(x.y),
-                         "r"(x.z), "r"(x.w), "r"(y.x), "r"(y.y), "r"(y.z), "r"(y.w) : "memory");
+            reinterpret_cast<uint4*>(a.st_x + (m * d.dx + c0))[0] = x;
+            reinterpret_cast<uint4*>(a.st_x + (m * d.dx + c0))[1] = y;
           }
           c0 += 16;
         } else {
           float z[8];
-          tmem_ld8(tmem + ((uint32_t)(q * 32) << 16) + 256u + (uint32_t)c0, z);
-          asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+          acc_ld8(acc, ((uint32_t)(q * 32) << 16) + 256u + (uint32_t)c0, z);
           __align__(16) __nv_bfloat16 v[8];
 #pragma unroll
           for (int e = 0; e < 8; ++e) v[e] = __float2bfloat16_rn(fmaxf(z[e] + sBias0[c0 + e], 0.f));
@@ -758,20 +809,16 @@ policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
         *reinterpret_cast<uint4*>(sA + (size_t)(KCX + half * (HPT / 8) + c8) * 2048 + row * 16) = *reinterpret_cast<const uint4*>(v);
       }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     __syncthreads();
     PROF_MARK(3);      // relu epilogue of the fc GEMM (+ st_x) and h staging
     // ---- 4. MMA1: gates D1[128 x 256] = [X | h][128 x K] . [Wx;Wh][K x 256] ----
-    if (warp == 0) {
-      if (lane == 0) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        for (int ks = 0; ks < KS; ++ks)
-          umma_bf16(tmem, make_desc(aA + ks * 2 * 2048, 2048, 128), make_desc(aB + ks * 2 * 4096, 4096, 128), idesc1,
-                    ks > 0 ? 1u : 0u);
-        umma_commit(bar);
-      }
-      __syncwarp();
+    if (warp < 8) {
+      wg_mma<0, 0>(acc, 0, TC_N, KS, false, [&](int ks, uint64_t& da, uint64_t& db) {
+        da = make_desc(aA + ks * 2 * 2048, 2048, 128);
+        db = make_desc(aB + ks * 2 * 4096, 4096, 128);
+      });
+      wg_mma_done(bar);
     }
     float cpre[16];        // c_{t-1} of this thread's 16 hidden units (NT = 512): in flight while the gate MMA runs
     if constexpr (NT == 512) {
@@ -779,13 +826,9 @@ policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
       if (r < a.R && !a.done) {
         const float* cp = a.c_in + ((int64_t)u * ld + r) * TC_H + (warp >> 2) * HPT;
 #pragma unroll
-        for (int e8 = 0; e8 < 2; ++e8) {      // 256-bit loads: one full sector per thread and instruction
-          uint32_t w[8];
-          asm volatile("ld.global.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                       : "=r"(w[0]), "=r"(w[1]), "=r"(w[2]), "=r"(w[3]), "=r"(w[4]), "=r"(w[5]), "=r"(w[6]), "=r"(w[7])
-                       : "l"(cp + 8 * e8));
-#pragma unroll
-          for (int e = 0; e < 8; ++e) cpre[8 * e8 + e] = __uint_as_float(w[e]);
+        for (int e4 = 0; e4 < 4; ++e4) {
+          const float4 x = reinterpret_cast<const float4*>(cp)[e4];
+          cpre[4 * e4] = x.x; cpre[4 * e4 + 1] = x.y; cpre[4 * e4 + 2] = x.z; cpre[4 * e4 + 3] = x.w;
         }
       } else {
 #pragma unroll
@@ -794,7 +837,6 @@ policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
     }
     mbar_wait(bar, parity);
     parity ^= 1;
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
     if (NT == 512 && tid == NT - 1 && it + 1 < it_hi) {
       // the A tile is dead: fetch the NEXT tile's fc-weight block now (its unit may differ)
       const int un = (int)((it + 1) / n_tiles);
@@ -857,9 +899,8 @@ policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
 #pragma unroll
       for (int jb = 0; jb < HPT / 16; ++jb) {
         float zi[16], zf[16], zo[16], zu[16];
-        const uint32_t tbase = tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(half * HPT + jb * 16);
-        tmem_ld16(tbase, zi); tmem_ld16(tbase + 64, zf); tmem_ld16(tbase + 128, zo); tmem_ld16(tbase + 192, zu);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+        const uint32_t tbase = ((uint32_t)(q * 32) << 16) + (uint32_t)(half * HPT + jb * 16);
+        acc_ld16(acc, tbase, zi); acc_ld16(acc, tbase + 64, zf); acc_ld16(acc, tbase + 128, zo); acc_ld16(acc, tbase + 192, zu);
         if (a.zdbg && valid) {
           float* z = a.zdbg + ((int64_t)u * ld + r) * TC_N + half * HPT + jb * 16;
 #pragma unroll
@@ -895,16 +936,13 @@ policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
           for (int jj = 0; jj < 8; ++jj) lg[jj] = fmaf(hn[e], sWo[j * 8 + jj], lg[jj]);
         }
         if constexpr (NT == 512) {
-          // Stores: a thread owns (row, 16 hidden units), i.e. 32-byte pieces of its row.  They leave as 256-bit stores
-          // (STG.256: one full 32-byte sector per thread and instruction, 14 instructions per thread and tile) straight
-          // from the registers, interleaved with the other warps' cell math.  Measured alternatives: 16-byte row-owner
-          // stores (28 half-sector instructions: the LSU was ~half of the kernel), a SIMT copy-out through XOR-swizzled
-          // shared memory (coalesced, but 4 staging passes with 8 block-wide barriers: 16 k cycles per tile) and the same
-          // passes handed to the copy engine row by row (cp.async.bulk, 128-512 B each: slower still).
+          // Stores: a thread owns (row, 16 hidden units), i.e. 32-byte pieces of its row.  They leave as pairs of 128-bit stores
+          // (one full 32-byte sector per thread) straight from the registers, interleaved with the
+          // other warps' cell math.  Alternatives: a SIMT copy-out through XOR-swizzled shared memory (coalesced, but 4
+          // staging passes with 8 block-wide barriers) or the same passes handed to the copy engine row by row.
           auto st32 = [](void* p, const void* v) {
             const uint4 x = reinterpret_cast<const uint4*>(v)[0], y = reinterpret_cast<const uint4*>(v)[1];
-            asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "r"(x.x), "r"(x.y), "r"(x.z), "r"(x.w),
-                         "r"(y.x), "r"(y.y), "r"(y.z), "r"(y.w) : "memory");
+            reinterpret_cast<uint4*>(p)[0] = x; reinterpret_cast<uint4*>(p)[1] = y;
           };
           if (valid) {
             if (a.st_g) {
@@ -950,7 +988,6 @@ policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
         }
         }
       }
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
       if (half == 1) {
 #pragma unroll
         for (int j = 0; j < 8; ++j) sRed[row * 8 + j] = lg[j];
@@ -968,334 +1005,6 @@ policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
     for (int i = 0; i < 16; ++i) atomicAdd(a.prof + i, (unsigned long long)pt[i]);
 #undef PROF_MARK
   __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512));
-}
-
-// ===================================================================================================
-// v3: the same fused step with the weight operand STREAMED instead of resident, so that TWO CTAs share an SM and
-// overlap each other's serial phases (v2 holds the 147 KB [Wx;Wh] image in shared memory: one CTA per SM, every
-// latency exposed).
-//   * [Wx;Wh] of the current unit stays in L2 (7.4 MB for all 50 units); its 18 K-slabs of 8 KB travel through a
-//     4-stage ring in shared memory by cp.async.bulk (TMA unit, mbarrier complete_tx), issued and consumed by ONE
-//     thread, which also issues the tcgen05.mma of each slab and commits it to the slab's "empty" barrier;
-//     the first slabs of the NEXT work item and its fc-weight block are prefetched while the current item is in its
-//     epilogue;
-//   * TMEM: 256 columns per CTA (two CTAs = 512): the fc accumulator D0 (dx columns) and the gate accumulator D1 (256)
-//     share them, D0 is dead once X has been written to the A tile;
-//   * shared memory 112 KB per CTA: A tile 72 KB | ring 32 KB | biases, head weights, partial head sums.
-// Arithmetic per element is identical to v2: the two kernels produce the same bits.
-#define V3_NSTG 4
-#define V3_SLAB 8192
-__global__ void __launch_bounds__(256, 2)
-policy_step_tc3_kernel(const DDimsTC d, const StepTC a) {
-  constexpr int NT = 256, NG = 2, HPT = 32;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int K = d.dx + TC_H, KC = K / 8, KS = K / 16, KCX = d.dx / 8;
-  unsigned char* sA = tc_smem;                                  // KC * 2048
-  unsigned char* sR = sA + (size_t)KC * 2048;                   // ring: V3_NSTG * 8192
-  float* sRed = reinterpret_cast<float*>(sR + V3_NSTG * V3_SLAB);   // [128][8]
-  float* sWo = sRed + TC_M * 8;                                 // [64][8]
-  float* sBo = sWo + TC_H * 8;                                  // [8]
-  float* sBias = sBo + 8;                                       // [256]  lstm bias
-  float* sBias0 = sBias + TC_N;                                 // [256]  fc biases
-  uint64_t* sBar = reinterpret_cast<uint64_t*>(sBias0 + TC_N);  // [0] mma done, [1] fc weights landed, [2..5] full, [6..9] empty
-  uint32_t* sTmem = reinterpret_cast<uint32_t*>(sBar + 2 + 2 * V3_NSTG);
-  const uint32_t bar_mma = smem_u32(sBar), bar_fc = smem_u32(sBar + 1);
-  const uint32_t bar_full = smem_u32(sBar + 2), bar_empty = smem_u32(sBar + 2 + V3_NSTG);
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(sTmem)), "r"(256));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  if (tid == 0) {
-    mbar_init(bar_mma, 1); mbar_init(bar_fc, 1);
-    for (int s = 0; s < V3_NSTG; ++s) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, 1); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem = *sTmem;
-  const uint32_t idesc1 = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(TC_N >> 3) << 17) | ((uint32_t)(TC_M >> 4) << 24);
-  const uint32_t idesc0 = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(d.dx >> 3) << 17) | ((uint32_t)(TC_M >> 4) << 24);
-  const int64_t n_tiles = (a.R + TC_M - 1) / TC_M;
-  const int64_t ld = a.ld > 0 ? a.ld : a.R;
-  const int64_t n_items = n_tiles * 2 * d.A;
-  const int64_t it_lo = n_items * blockIdx.x / gridDim.x, it_hi = n_items * (blockIdx.x + 1) / gridDim.x;
-  int cur_u = -1;
-  uint32_t par_mma = 0, par_fc = 0;
-  uint32_t n_issue = 0, n_cons = 0;            // thread 0: slabs issued / consumed since the kernel started
-  int nw = 0, nt = 0, nf = 0, ooff = 0, na = 0;
-  const uint32_t aA = smem_u32(sA), aR = smem_u32(sR);
-  const uint32_t fc_bytes = (uint32_t)(8 * d.dx * 16);
-
-  // thread 0 only: stream slab `ks` of unit `u` into the next ring stage (waits until the MMA that last read it is done)
-  auto issue_slab = [&](int u, int ks) {
-    const uint32_t s = n_issue % V3_NSTG, k = n_issue / V3_NSTG;
-    if (k > 0) mbar_wait(bar_empty + 8 * s, (k - 1) & 1);
-    mbar_expect_tx(bar_full + 8 * s, V3_SLAB);
-    bulk_g2s(aR + s * V3_SLAB, reinterpret_cast<const unsigned char*>(a.Wp + (int64_t)u * wp_stride(d.dx)) + (size_t)ks * V3_SLAB,
-             V3_SLAB, bar_full + 8 * s);
-    ++n_issue;
-  };
-  const int n_pre = KS < V3_NSTG ? KS : V3_NSTG;
-  if (tid == 0 && it_lo < it_hi) {             // first work item: fc weights + the first slabs
-    const int u0 = (int)(it_lo / n_tiles);
-    mbar_expect_tx(bar_fc, fc_bytes);
-    bulk_g2s(aA, reinterpret_cast<const unsigned char*>(a.Wp + (int64_t)u0 * wp_stride(d.dx)) + (size_t)KC * 4096, fc_bytes, bar_fc);
-    for (int ks = 0; ks < n_pre; ++ks) issue_slab(u0, ks);
-  }
-
-  for (int64_t it = it_lo; it < it_hi; ++it) {
-    const int u = (int)(it / n_tiles);
-    const int64_t r0 = (it - (int64_t)u * n_tiles) * TC_M;
-    const int ag = u >> 1;
-    const int64_t st_c0 = (a.row0 + r0) / a.rc, st_rin0 = (a.row0 + r0) - st_c0 * a.rc;
-    auto store_row = [&](int row) -> int64_t {
-      int64_t c = st_c0, rin = st_rin0 + row;
-      while (rin >= a.rc) { rin -= a.rc; ++c; }
-      return ((c * (2 * d.A) + u) * a.T + a.t) * a.rc + rin;
-    };
-    if (u != cur_u) {      // per-unit constants (sRed / sWo / biases are not touched by the async copies in flight)
-      __syncthreads();     // previous item's epilogue has finished reading them
-      cur_u = u;
-      nw = d.n_wave[ag]; nt = d.n_wait[ag]; nf = d.ff > 0 ? d.n_fp[ag] : 0;
-      ooff = d.obs_off[ag]; na = d.n_a[ag];
-      for (int i = tid; i < TC_H * 8; i += NT) {
-        const int k = i >> 3, j = i & 7;
-        sWo[i] = j < d.max_na ? a.P[d.off_wo + ((int64_t)u * TC_H + k) * d.max_na + j] : 0.f;
-      }
-      if (tid < 8) sBo[tid] = tid < d.max_na ? a.P[d.off_bo + (int64_t)u * d.max_na + tid] : 0.f;
-      for (int i = tid; i < TC_N; i += NT) {
-        sBias[i] = a.P[d.off_bl + (int64_t)u * TC_N + i];
-        float b0 = 0.f;
-        if (i < d.fw) b0 = a.P[d.off_fcw_b[u] + i];
-        else if (i < d.fw + d.ff) b0 = a.P[d.off_fcf_b[u] + (i - d.fw)];
-        else if (i < d.dx) b0 = a.P[d.off_fct_b[u] + (i - d.fw - d.ff)];
-        sBias0[i] = b0;
-      }
-    }
-    if (it + 1 < it_hi) {      // L2 prefetch of the next item's observation slice and state rows
-      const int un = (int)((it + 1) / n_tiles);
-      const int64_t rn = ((it + 1) - (int64_t)un * n_tiles) * TC_M + (tid / NG);
-      if (rn < a.R) {
-        const int an = un >> 1;
-        asm volatile("prefetch.global.L2 [%0];" ::"l"(a.obs + rn * d.n_obs + d.obs_off[an] + (tid % NG) * 32));
-        const int64_t so = ((int64_t)un * ld + rn) * TC_H + (tid % NG) * 32;
-        asm volatile("prefetch.global.L2 [%0];" ::"l"(a.c_in + so));
-        asm volatile("prefetch.global.L2 [%0];" ::"l"(a.h_in + so));
-      }
-    }
-    // ---- 1. observation slice -> last 8 chunks of the A tile (the fc weights arrive by bulk copy in chunks 0..) ----
-#pragma unroll
-    for (int p = 0; p < 1024 / NT; ++p) {
-      const int pair = p * NT + tid;
-      const int row = pair & 127, ch = pair >> 7;
-      const int64_t r = r0 + row;
-      __align__(16) __nv_bfloat16 v[8];
-#pragma unroll
-      for (int e = 0; e < 8; ++e) {
-        const int c = ch * 8 + e;
-        int src = -1;
-        if (c < d.kw) { if (c < nw) src = c; }
-        else if (c < d.kw + TC_KF) { if (c - d.kw < nf) src = nw + nt + (c - d.kw); }
-        else { if (c - d.kw - TC_KF < nt) src = nw + (c - d.kw - TC_KF); }
-        float x = 0.f;
-        if (src >= 0 && r < a.R) x = __ldg(a.obs + r * d.n_obs + ooff + src);
-        v[e] = __float2bfloat16_rn(x);
-      }
-      *reinterpret_cast<uint4*>(sA + (size_t)(KC - 8 + ch) * 2048 + row * 16) = *reinterpret_cast<const uint4*>(v);
-    }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    __syncthreads();
-    // ---- 2. MMA0: D0[128 x dx] = A0[128 x 64] . B0[64 x dx]  (TMEM columns 0..dx) ----
-    if (tid == 0) {
-      mbar_wait(bar_fc, par_fc);               // fc weights of this item have landed in chunks 0..
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      for (int ks = 0; ks < 4; ++ks) {
-        const uint64_t da = make_desc(aA + (KC - 8 + 2 * ks) * 2048, 2048, 128);
-        const uint64_t db = make_desc(aA + ks * 2 * (d.dx * 16), d.dx * 16, 128);
-        umma_bf16(tmem, da, db, idesc0, ks > 0 ? 1u : 0u);
-      }
-      umma_commit(bar_mma);
-    }
-    par_fc ^= 1;
-    mbar_wait(bar_mma, par_mma);
-    par_mma ^= 1;
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    // ---- 3. X = relu(D0 + b) as bf16 -> A tile chunks 0..dx/8 ; h_prev -> the 8 chunks after them ----
-    {
-      const int q = warp & 3, hw = warp >> 2;
-      const int row = q * 32 + lane;
-      const int ncol = d.dx / NG;
-      const bool st = a.st_x && r0 + row < a.R;
-      const int64_t m = st ? store_row(row) : 0;
-      for (int c0 = hw * ncol; c0 < (hw + 1) * ncol; c0 += 8) {
-        float z[8];
-        tmem_ld8(tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)c0, z);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        __align__(16) __nv_bfloat16 v[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) v[e] = __float2bfloat16_rn(fmaxf(z[e] + sBias0[c0 + e], 0.f));
-        *reinterpret_cast<uint4*>(sA + (size_t)(c0 >> 3) * 2048 + row * 16) = *reinterpret_cast<const uint4*>(v);
-        if (st) *reinterpret_cast<uint4*>(a.st_x + (m * d.dx + c0)) = *reinterpret_cast<const uint4*>(v);
-      }
-    }
-    {
-      const int row = tid / NG, half = tid % NG;
-      const int64_t r = r0 + row;
-      const bool live = r < a.R && !a.done;
-      const float4* hp = reinterpret_cast<const float4*>(a.h_in + ((int64_t)u * ld + (r < a.R ? r : 0)) * TC_H + half * HPT);
-#pragma unroll
-      for (int c8 = 0; c8 < HPT / 8; ++c8) {
-        __align__(16) __nv_bfloat16 v[8];
-        float4 x0 = make_float4(0.f, 0.f, 0.f, 0.f), x1 = x0;
-        if (live) { x0 = hp[2 * c8]; x1 = hp[2 * c8 + 1]; }
-        v[0] = __float2bfloat16_rn(x0.x); v[1] = __float2bfloat16_rn(x0.y); v[2] = __float2bfloat16_rn(x0.z); v[3] = __float2bfloat16_rn(x0.w);
-        v[4] = __float2bfloat16_rn(x1.x); v[5] = __float2bfloat16_rn(x1.y); v[6] = __float2bfloat16_rn(x1.z); v[7] = __float2bfloat16_rn(x1.w);
-        *reinterpret_cast<uint4*>(sA + (size_t)(KCX + half * (HPT / 8) + c8) * 2048 + row * 16) = *reinterpret_cast<const uint4*>(v);
-      }
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    __syncthreads();
-    // ---- 4. MMA1: gates D1[128 x 256] = [X | h][128 x K] . [Wx;Wh][K x 256], B slabs through the ring ----
-    if (tid == 0) {
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      for (int ks = 0; ks < KS; ++ks) {
-        const uint32_t s = n_cons % V3_NSTG, k = n_cons / V3_NSTG;
-        mbar_wait(bar_full + 8 * s, k & 1);
-        umma_bf16(tmem, make_desc(aA + ks * 2 * 2048, 2048, 128), make_desc(aR + s * V3_SLAB, 4096, 128), idesc1,
-                  ks > 0 ? 1u : 0u);
-        umma_commit(bar_empty + 8 * s);
-        ++n_cons;
-        if (ks >= 1 && ks - 1 + V3_NSTG < KS) issue_slab(u, ks - 1 + V3_NSTG);   // refill the stage MMA(ks-1) has left
-      }
-      umma_commit(bar_mma);
-    }
-    mbar_wait(bar_mma, par_mma);
-    par_mma ^= 1;
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    if (tid == 0 && it + 1 < it_hi) {          // the A tile and the ring are free: start the next item's operands now
-      const int un = (int)((it + 1) / n_tiles);
-      mbar_expect_tx(bar_fc, fc_bytes);
-      bulk_g2s(aA, reinterpret_cast<const unsigned char*>(a.Wp + (int64_t)un * wp_stride(d.dx)) + (size_t)KC * 4096, fc_bytes, bar_fc);
-      for (int ks = 0; ks < n_pre; ++ks) issue_slab(un, ks);
-    }
-    // ---- 5. epilogue (as v2, NT = 256) ----
-    {
-      const int q = warp & 3, half = warp >> 2;
-      const int row = q * 32 + lane;
-      const int64_t r = r0 + row;
-      const bool valid = r < a.R;
-      const int64_t srow = ((int64_t)u * ld + (valid ? r : 0)) * TC_H + half * HPT;
-      float lg[8];
-#pragma unroll
-      for (int j = 0; j < 8; ++j) lg[j] = 0.f;
-#pragma unroll 1
-      for (int jb = 0; jb < HPT / 16; ++jb) {
-        float zi[16], zf[16], zo[16], zu[16];
-        const uint32_t tbase = tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(half * HPT + jb * 16);
-        tmem_ld16(tbase, zi); tmem_ld16(tbase + 64, zf); tmem_ld16(tbase + 128, zo); tmem_ld16(tbase + 192, zu);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        float cprev[16];
-        if (valid && !a.done) {
-          const float4* cp = reinterpret_cast<const float4*>(a.c_in + srow + jb * 16);
-#pragma unroll
-          for (int e4 = 0; e4 < 4; ++e4) {
-            const float4 x = cp[e4];
-            cprev[4 * e4] = x.x; cprev[4 * e4 + 1] = x.y; cprev[4 * e4 + 2] = x.z; cprev[4 * e4 + 3] = x.w;
-          }
-        } else {
-#pragma unroll
-          for (int e = 0; e < 16; ++e) cprev[e] = 0.f;
-        }
-        float cn[16], hn[16];
-        __align__(16) __nv_bfloat16 gbuf[4][16];
-#pragma unroll
-        for (int e = 0; e < 16; ++e) {
-          const int j = half * HPT + jb * 16 + e;
-          const float gi = sigm(zi[e] + sBias[j]), gf = sigm(zf[e] + sBias[64 + j]);
-          const float go = sigm(zo[e] + sBias[128 + j]), gu = tanh_fast(zu[e] + sBias[192 + j]);
-          cn[e] = gf * cprev[e] + gi * gu;
-          hn[e] = go * tanh_fast(cn[e]);
-          gbuf[0][e] = __float2bfloat16_rn(gi); gbuf[1][e] = __float2bfloat16_rn(gf);
-          gbuf[2][e] = __float2bfloat16_rn(go); gbuf[3][e] = __float2bfloat16_rn(gu);
-#pragma unroll
-          for (int jj = 0; jj < 8; ++jj) lg[jj] = fmaf(hn[e], sWo[j * 8 + jj], lg[jj]);
-        }
-        if (valid && a.st_g) {
-          const int64_t m = store_row((int)(r - r0));
-          const int jo = half * HPT + jb * 16;
-#pragma unroll
-          for (int g = 0; g < 4; ++g) {
-            uint4* o = reinterpret_cast<uint4*>(a.st_g + m * TC_N + g * 64 + jo);
-            o[0] = *reinterpret_cast<const uint4*>(&gbuf[g][0]); o[1] = *reinterpret_cast<const uint4*>(&gbuf[g][8]);
-          }
-          __align__(16) __nv_bfloat16 cb[16], hb[16];
-#pragma unroll
-          for (int e = 0; e < 16; ++e) { cb[e] = __float2bfloat16_rn(cn[e]); hb[e] = __float2bfloat16_rn(hn[e]); }
-          uint4* oc = reinterpret_cast<uint4*>(a.st_c + m * TC_H + jo);
-          uint4* oh = reinterpret_cast<uint4*>(a.st_h + m * TC_H + jo);
-          oc[0] = *reinterpret_cast<const uint4*>(cb); oc[1] = *reinterpret_cast<const uint4*>(cb + 8);
-          oh[0] = *reinterpret_cast<const uint4*>(hb); oh[1] = *reinterpret_cast<const uint4*>(hb + 8);
-        }
-        if (valid) {
-          float4* co = reinterpret_cast<float4*>(a.c_out + srow + jb * 16);
-          float4* ho = reinterpret_cast<float4*>(a.h_out + srow + jb * 16);
-#pragma unroll
-          for (int e4 = 0; e4 < 4; ++e4) {
-            co[e4] = make_float4(cn[4 * e4], cn[4 * e4 + 1], cn[4 * e4 + 2], cn[4 * e4 + 3]);
-            ho[e4] = make_float4(hn[4 * e4], hn[4 * e4 + 1], hn[4 * e4 + 2], hn[4 * e4 + 3]);
-          }
-        }
-      }
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      if (half == 1) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) sRed[row * 8 + j] = lg[j];
-      }
-      __syncthreads();       // also: every thread is done with TMEM -> the next item's MMA0 may overwrite D
-      if (half == 0 && valid) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) lg[j] += sRed[row * 8 + j] + sBo[j];
-        if ((u & 1) == 0) {
-          float mx = -1e30f;
-#pragma unroll
-          for (int j = 0; j < 8; ++j) if (j < na) mx = fmaxf(mx, lg[j]);
-          float s = 0.f;
-#pragma unroll
-          for (int j = 0; j < 8; ++j) { lg[j] = j < na ? __expf(lg[j] - mx) : 0.f; s += lg[j]; }
-          const float inv = 1.0f / s;
-          float* po = a.pi + ((int64_t)r * d.A + ag) * d.max_na;
-#pragma unroll
-          for (int j = 0; j < 8; ++j) if (j < d.max_na) po[j] = lg[j] * inv;
-          if (a.act) {
-            uint32_t hsh = pmix32(a.seed_lo ^ (a.step * 0x9E3779B1U));
-            hsh = pmix32(hsh ^ a.seed_hi ^ ((uint32_t)(a.replica0 + r) * 0x85EBCA77U));
-            hsh = pmix32(hsh ^ ((uint32_t)ag * 0xC2B2AE3DU));
-            const float uu = (float)(hsh >> 8) * (1.0f / 16777216.0f);
-            float cum = 0.f;
-            int pick = na - 1;
-            bool found = false;
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-              if (j < na) { cum += lg[j] * inv; if (!found && uu < cum) { pick = j; found = true; } }
-            a.act[(int64_t)r * d.A + ag] = pick;
-          }
-        } else {
-          a.val[(int64_t)r * d.A + ag] = lg[0];
-        }
-      }
-      __syncthreads();       // sRed is rewritten by the next item's epilogue only, but its head reads must finish first
-    }
-  }
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(256));
-}
-
-static size_t tc3_smem_bytes(int K) {
-  const int KC = K / 8;
-  return (size_t)KC * 2048 + V3_NSTG * V3_SLAB + (TC_M * 8 + TC_H * 8 + 8 + TC_N + TC_N) * 4 + (2 + 2 * V3_NSTG) * 8 + 16;
 }
 
 static size_t tc2_smem_bytes(int K) {
@@ -1338,27 +1047,18 @@ extern "C" int tscl_policy_step_v2r(tscl_handle* h, const float* params, const v
   const int64_t n_items = ((R + TC_M - 1) / TC_M) * 2 * d.A;
   const int grid = (int)(n_items < n_sm ? n_items : n_sm);
   StepTC a;
+  a.acc = acc_tiles(h, stream);
+  if (!a.acc) return tsc_set_error("accumulator tiles: cudaMalloc failed");
   a.P = params; a.Wp = (const __nv_bfloat16*)wpack_bf16; a.obs = obs; a.c_in = c_in; a.h_in = h_in; a.c_out = c_out;
   a.h_out = h_out; a.pi = pi; a.val = val; a.act = act; a.zdbg = zdbg; a.R = R; a.done = done; a.swap_lbo_sbo = 0;
   a.seed_lo = (uint32_t)seed; a.seed_hi = (uint32_t)(seed >> 32); a.step = (uint32_t)step; a.replica0 = replica0;
   a.st_x = (__nv_bfloat16*)st_x; a.st_g = (__nv_bfloat16*)st_g; a.st_c = (__nv_bfloat16*)st_c; a.st_h = (__nv_bfloat16*)st_h;
   a.t = t; a.T = T > 0 ? T : 1; a.rc = rc > 0 ? rc : R; a.ld = ld_state; a.row0 = ld_state > 0 ? row0 : 0;
   a.prof = g_policy_prof;
-  // default: the resident-weight kernel v2 (512 threads; TSC_POLICY_THREADS=256 = its round-1 thread mapping).
-  // TSC_POLICY_V3=1 selects the streamed-weight two-CTA-per-SM kernel: measured 1.404 vs 1.342 ms of rollout per control
-  // step at R = 8192 (policy kernel ~0.63 vs 0.57 ms), i.e. slower, so it is not the default
-  static const int pol_v3 = []() { const char* e = getenv("TSC_POLICY_V3"); return e ? atoi(e) : 0; }();
+  // 512 threads (thread = row and 16 hidden units) where the copy-out staging fits the A-tile region, else 256;
+  // TSC_POLICY_THREADS=256 selects the 256-thread mapping for experiments
   static const int pol_threads = []() { const char* e = getenv("TSC_POLICY_THREADS"); return e && atoi(e) == 256 ? 256 : 512; }();
-  if (pol_v3 && !zdbg) {
-    const size_t smem3 = tc3_smem_bytes(K);
-    static int attr3_dev = -1;
-    if (attr3_dev != tscl_device_of(h)) {
-      PCK(cudaFuncSetAttribute(policy_step_tc3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem3));
-      attr3_dev = tscl_device_of(h);
-    }
-    const int grid3 = (int)(n_items < 2 * n_sm ? n_items : 2 * n_sm);       // two CTAs per SM
-    policy_step_tc3_kernel<<<grid3, 256, smem3, (cudaStream_t)stream>>>(d, a);
-  } else if (a.prof && wide_tile) policy_step_tc2_kernel<512, true><<<grid, 512, smem, (cudaStream_t)stream>>>(d, a);
+  if (a.prof && wide_tile) policy_step_tc2_kernel<512, true><<<grid, 512, smem, (cudaStream_t)stream>>>(d, a);
   else if (pol_threads == 512 && wide_tile) policy_step_tc2_kernel<512, false><<<grid, 512, smem, (cudaStream_t)stream>>>(d, a);
   else policy_step_tc2_kernel<256, false><<<grid, 256, smem, (cudaStream_t)stream>>>(d, a);
   PCK(cudaGetLastError());
@@ -1379,8 +1079,8 @@ extern "C" int tscl_policy_step_v2(tscl_handle* h, const float* params, const vo
 // One CTA walks (unit, 128-replica tile) items; for t = T-1 .. 0:
 //   thread = (replica row, 32 hidden units): cell backward from gate activations, c_t, c_{t-1} and the
 //   incoming dh / dc  ->  dz (4 x 32) written fp32 in place over the gates (operand of the weight-gradient
-//   GEMMs) and as bf16 into the A tile [128 x 256];  tcgen05.mma  D[128 x 64] = dz . Wh^T  (K = 256, N = 64)
-//   -> TMEM -> the thread's 32 columns = dh_{t-1} carry.  dc / dh carries stay in registers.
+//   GEMMs) and as bf16 into the A tile [128 x 256];  wgmma  D[128 x 64] = dz . Wh^T  (K = 256, N = 64)
+//   -> accumulator tile -> the thread's 32 columns = dh_{t-1} carry.  dc / dh carries stay in registers.
 #define BW_KC 32            // 256 / 8 K-chunks
 __global__ void pack_wht_kernel(const DDimsTC d, const float* __restrict__ P, __nv_bfloat16* __restrict__ Wt) {
   const int u = blockIdx.y;
@@ -1407,6 +1107,7 @@ __global__ void pack_wxt_kernel(const DDimsTC d, const float* __restrict__ P, __
   }
 }
 struct BwdTC {
+  float* acc;                // accumulator tiles, one [128][ACC_COLS] fp32 tile per CTA (acc_tiles)
   const __nv_bfloat16* Wxt;  // optional [2A][32][dx][8] (tscl_pack_wxt): with dXb, dX = dZ . Wx^T is fused into the step
   __nv_bfloat16* dXb;        // optional [2A][T*Rc][dx] bf16
   const __nv_bfloat16* Wt;   // [2A][32][64][8]
@@ -1439,30 +1140,20 @@ lstm_bwd_tc_kernel(const DDimsTC d, const BwdTC a) {
   unsigned char* sB = tc_smem;                       // 32 * 1024  : Wh^T image
   unsigned char* sA = sB + BW_KC * 1024;             // 32 * 2048  : dz tile
   uint64_t* sBar = reinterpret_cast<uint64_t*>(sA + BW_KC * 2048);
-  uint32_t* sTmem = reinterpret_cast<uint32_t*>(sBar + 1);
   unsigned char* sBx = sA + BW_KC * 2048 + 16;       // 32 * dx * 16 : Wx^T image (only when fuse_dx)
   const uint32_t bar = smem_u32(sBar);
-  const uint32_t tmem_cols = fuse_dx ? 512u : 64u;   // D1 (dh) in columns 0..63, D2 (dX) in columns 64..64+dx
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(sTmem)), "r"(tmem_cols));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
   if (tid == 0) {
     mbar_init(bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem = *sTmem;
-  const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(TC_H >> 3) << 17) | ((uint32_t)(TC_M >> 4) << 24);
-  const uint32_t idesc_x = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(dx >> 3) << 17) | ((uint32_t)(TC_M >> 4) << 24);
+  float* const acc = a.acc + (size_t)blockIdx.x * TC_M * ACC_COLS;
   const uint32_t aA = smem_u32(sA), aB = smem_u32(sB), aBx = smem_u32(sBx);
   const int64_t n_tiles = (a.Rc + TC_M - 1) / TC_M;
   const int64_t n_items = n_tiles * 2 * d.A;
   int cur_u = -1;
   uint32_t parity = 0;
-  const int q = warp & 3, qt = warp >> 2;            // TMEM lane quadrant, hidden-unit group
+  const int q = warp & 3, qt = warp >> 2;            // row quadrant of the accumulator tile, hidden-unit group
   const int row = q * 32 + lane, jq = qt * HPT;
   auto bf8 = [](const uint4 v, float* o) {
     const uint32_t w[4] = {v.x, v.y, v.z, v.w};
@@ -1573,33 +1264,28 @@ lstm_bwd_tc_kernel(const DDimsTC d, const BwdTC a) {
       }
       const bool need_dh = keep != 0.f && t > 0;
       if (need_dh || fuse_dx) {
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
         __syncthreads();
-        if (warp == 0) {
-          if (lane == 0) {
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            if (need_dh)
-              for (int ks = 0; ks < 16; ++ks)
-                umma_bf16(tmem, make_desc(aA + ks * 2 * 2048, 2048, 128), make_desc(aB + ks * 2 * 1024, 1024, 128), idesc,
-                          ks > 0 ? 1u : 0u);
-            if (fuse_dx)      // same A tile, B = Wx^T image: chunk stride dx * 16 B, 8-row groups 128 B apart
-              for (int ks = 0; ks < 16; ++ks)
-                umma_bf16(tmem + 64u, make_desc(aA + ks * 2 * 2048, 2048, 128),
-                          make_desc(aBx + (uint32_t)(ks * 2 * dx * 16), (uint32_t)(dx * 16), 128), idesc_x, ks > 0 ? 1u : 0u);
-            umma_commit(bar);
-          }
-          __syncwarp();
+        if (warp < 8) {
+          if (need_dh)
+            wg_mma<0, 0>(acc, 0, TC_H, 16, false, [&](int ks, uint64_t& da, uint64_t& db) {
+              da = make_desc(aA + ks * 2 * 2048, 2048, 128);
+              db = make_desc(aB + ks * 2 * 1024, 1024, 128);
+            });
+          if (fuse_dx)      // same A tile, B = Wx^T image: chunk stride dx * 16 B, 8-row groups 128 B apart
+            wg_mma<0, 0>(acc, 64, dx, 16, false, [&](int ks, uint64_t& da, uint64_t& db) {
+              da = make_desc(aA + ks * 2 * 2048, 2048, 128);
+              db = make_desc(aBx + (uint32_t)(ks * 2 * dx * 16), (uint32_t)(dx * 16), 128);
+            });
+          wg_mma_done(bar);
         }
         mbar_wait(bar, parity);
         parity ^= 1;
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
         if (need_dh) {
           float dhp[HPT];
 #pragma unroll
           for (int c16 = 0; c16 < HPT / 16; ++c16)
-            tmem_ld16(tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(jq + c16 * 16), dhp + c16 * 16);
-          asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+            acc_ld16(acc, ((uint32_t)(q * 32) << 16) + (uint32_t)(jq + c16 * 16), dhp + c16 * 16);
 #pragma unroll
           for (int e = 0; e < HPT; ++e) dhc[e] = dhp[e] * keep;
         } else {
@@ -1610,8 +1296,7 @@ lstm_bwd_tc_kernel(const DDimsTC d, const BwdTC a) {
           const int per = dx / NQ;
           for (int c8 = 0; c8 < per; c8 += 8) {
             float xv[8];
-            tmem_ld8(tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(64 + qt * per + c8), xv);
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+            acc_ld8(acc, ((uint32_t)(q * 32) << 16) + (uint32_t)(64 + qt * per + c8), xv);
             if (valid) {
               __align__(16) __nv_bfloat16 v[8];
 #pragma unroll
@@ -1626,26 +1311,23 @@ lstm_bwd_tc_kernel(const DDimsTC d, const BwdTC a) {
       }
     }
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(tmem_cols));
 }
 
 // ---------------------------------------------------------------------------------------------------
 // BPTT, staged variant (the activation-store path of the training loop: gates / c from the bf16 store, dZ written as
 // bf16).  Same arithmetic as lstm_bwd_tc_kernel<512>; what changes is how the operands reach the threads.  There a
 // thread owns (row, 16 hidden units) and loads its 16-byte pieces straight from global memory, 128-512 B apart between
-// the lanes of a warp (32 sectors per load instruction: lg_throttle 3.5 and long_scoreboard 10 warps per issue in
-// profiles/r02).  Here each step's tile — gates [128 x 512 B], c_{t-1} [128 x 128 B], dH [128 x 256 B] — is fetched by
+// the lanes of a warp (32 sectors per load instruction).  Here each step's tile — gates [128 x 512 B], c_{t-1} [128 x 128 B], dH [128 x 256 B] — is fetched by
 // coalesced 16-byte cp.async (one row segment per warp instruction) into XOR-swizzled shared memory one step AHEAD
 // (issued as soon as every thread has taken step t's operands into registers, landing while step t's cell math, MMA
-// and TMEM read-back run), and the threads pick their pieces from there without bank conflicts.
+// and accumulator read-back run), and the threads pick their pieces from there without bank conflicts.
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
 }
 // TMA = true: the per-step operand tile (gates 64 KB, dH 32 KB, c 16 KB) arrives by SEVEN cp.async.bulk.tensor copies issued
-// by one thread (hardware 128-byte swizzle = the pattern the readers use) instead of 14 cp.async per thread: the phase
-// profile showed the issue of those 7168 16-byte copies blocking every warp for 7.9 k of the 17 k cycles of a step.
+// by one thread (hardware 128-byte swizzle = the pattern the readers use) instead of 14 cp.async per thread, whose issue
+// (7168 16-byte copies per step) blocks every warp.
 template <bool PROF, bool TMA>
 __global__ void __launch_bounds__(512, 1)
 lstm_bwd_tc_staged_kernel(const DDimsTC d, const BwdTC a, const __grid_constant__ CUtensorMap mapG,
@@ -1661,29 +1343,21 @@ lstm_bwd_tc_staged_kernel(const DDimsTC d, const BwdTC a, const __grid_constant_
   unsigned char* sC0 = sG + 128 * 512;               // 16 KB x 2 : c ring, [128][8 chunks ^ (row & 7)]
   unsigned char* sD = sC0 + 2 * 128 * 128;           // 32 KB : dH fp32 [128][16 chunks ^ (row & 15)]; TMA: 2 boxes of 32 floats
   uint64_t* sBar = reinterpret_cast<uint64_t*>(sD + 128 * 256);
-  uint32_t* sTmem = reinterpret_cast<uint32_t*>(sBar + 2);
   const uint32_t bar = smem_u32(sBar), ldbar = bar + 8;
   uint32_t ldpar = 0;
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(sTmem)), "r"(64));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
   if (tid == 0) {
     mbar_init(bar, 1); mbar_init(ldbar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem = *sTmem;
-  const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(TC_H >> 3) << 17) | ((uint32_t)(TC_M >> 4) << 24);
+  float* const acc = a.acc + (size_t)blockIdx.x * TC_M * ACC_COLS;
   const uint32_t aA = smem_u32(sA), aB = smem_u32(sB);
   const uint32_t aG = smem_u32(sG), aC = smem_u32(sC0), aD = smem_u32(sD);
   const int64_t n_tiles = (a.Rc + TC_M - 1) / TC_M;
   const int64_t n_items = n_tiles * 2 * d.A;
   int cur_u = -1;
   uint32_t parity = 0;
-  const int q = warp & 3, qt = warp >> 2;            // TMEM lane quadrant, hidden-unit group (16 units)
+  const int q = warp & 3, qt = warp >> 2;            // row quadrant of the accumulator tile, hidden-unit group (16 units)
   const int row = q * 32 + lane, jq = qt * HPT;
   auto bf8 = [](const uint4 v, float* o) {
     const uint32_t w[4] = {v.x, v.y, v.z, v.w};
@@ -1838,40 +1512,34 @@ lstm_bwd_tc_staged_kernel(const DDimsTC d, const BwdTC a, const __grid_constant_
           zpk[g][jb] = *reinterpret_cast<const uint4*>(v);
         }
       }
-      if (valid) {      // dZ of this thread's 16 hidden units: one 256-bit store (a full sector) per gate
+      if (valid) {      // dZ of this thread's 16 hidden units: two 128-bit stores (a full sector) per gate
 #pragma unroll
         for (int g = 0; g < 4; ++g) {
           const uint4 x = zpk[g][0], y = zpk[g][1];
-          asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(a.dZb + m * TC_N + g * 64 + jq), "r"(x.x),
-                       "r"(x.y), "r"(x.z), "r"(x.w), "r"(y.x), "r"(y.y), "r"(y.z), "r"(y.w) : "memory");
+          reinterpret_cast<uint4*>(a.dZb + m * TC_N + g * 64 + jq)[0] = x;
+          reinterpret_cast<uint4*>(a.dZb + m * TC_N + g * 64 + jq)[1] = y;
         }
       }
       BP_MARK(1);                                   // second sub-batch: cell backward, dZ stores
       if (keep != 0.f && t > 0) {
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
         __syncthreads();
         BP_MARK(2);                                 // barrier before the MMA
-        if (warp == 0) {
-          if (lane == 0) {
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            for (int ks = 0; ks < 16; ++ks)
-              umma_bf16(tmem, make_desc(aA + ks * 2 * 2048, 2048, 128), make_desc(aB + ks * 2 * 1024, 1024, 128), idesc,
-                        ks > 0 ? 1u : 0u);
-            umma_commit(bar);
-          }
-          __syncwarp();
+        if (warp < 8) {
+          wg_mma<0, 0>(acc, 0, TC_H, 16, false, [&](int ks, uint64_t& da, uint64_t& db) {
+            da = make_desc(aA + ks * 2 * 2048, 2048, 128);
+            db = make_desc(aB + ks * 2 * 1024, 1024, 128);
+          });
+          wg_mma_done(bar);
         }
         mbar_wait(bar, parity);
         parity ^= 1;
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
         BP_MARK(3);                                 // MMA issue + commit + wait
         float dhp[HPT];
-        tmem_ld16(tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)jq, dhp);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+        acc_ld16(acc, ((uint32_t)(q * 32) << 16) + (uint32_t)jq, dhp);
 #pragma unroll
         for (int e = 0; e < HPT; ++e) dhc[e] = dhp[e] * keep;
-        BP_MARK(4);                                 // TMEM read-back
+        BP_MARK(4);                                 // accumulator read-back
       } else {
 #pragma unroll
         for (int e = 0; e < HPT; ++e) dhc[e] = 0.f;
@@ -1882,9 +1550,7 @@ lstm_bwd_tc_staged_kernel(const DDimsTC d, const BwdTC a, const __grid_constant_
     for (int i = 0; i < 8; ++i) atomicAdd(a.prof + i, (unsigned long long)bp[i]);
 #undef BP_MARK
   asm volatile("cp.async.wait_group 0;" ::: "memory");
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(64));
 }
 
 // 2-D tiled tensor map (row-major [rows][cols], box = box_cols x box_rows, inner box = 128 bytes, 128-byte swizzle) through the
@@ -1957,16 +1623,18 @@ extern "C" int tscl_lstm_seq_bwd_tc_dx(tscl_handle* h, const void* wt_bf16, floa
   int n_sm = 0;
   PCK(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, tscl_device_of(h)));
   const int64_t n_items = ((Rc + TC_M - 1) / TC_M) * 2 * d.A;
-  // 96 KB smem: two 512-thread CTAs per SM when registers allow; the fused-dX variant (up to 211 KB, 512 TMEM columns) is
+  // 96 KB smem: two 512-thread CTAs per SM when registers allow; the fused-dX variant (up to 211 KB) is
   // one CTA per SM
   const int64_t max_ctas = dx_bf16 ? n_sm : 2 * n_sm;
   const int grid = (int)(n_items < max_ctas ? n_items : max_ctas);
   BwdTC a;
+  a.acc = acc_tiles(h, stream);
+  if (!a.acc) return tsc_set_error("accumulator tiles: cudaMalloc failed");
   a.Wt = (const __nv_bfloat16*)wt_bf16; a.ZG = ZG; a.C = C; a.dH = dH; a.c0 = c0; a.done = done; a.T = T; a.Rc = Rc;
   a.ld_state = ld_state; a.r0 = r0; a.Gb = (const __nv_bfloat16*)gates_bf16; a.Cb = (const __nv_bfloat16*)c_bf16; a.dZb = (__nv_bfloat16*)dz_bf16;
   a.Wxt = (const __nv_bfloat16*)wxt_bf16; a.dXb = (__nv_bfloat16*)dx_bf16;
-  // measured (R = 8192, 1 x B200): the one-CTA-per-SM 512-thread variant 2.097 ms per control step, the two-CTA 256-thread
-  // variant 2.144 ms; TSC_BPTT_THREADS=256 selects the latter for experiments
+  // default: the one-CTA-per-SM 512-thread variant; TSC_BPTT_THREADS=256 selects the two-CTA-per-SM 256-thread variant
+  // for experiments (same arithmetic, same bits)
   static const int bw_threads = []() { const char* e = getenv("TSC_BPTT_THREADS"); return e && atoi(e) == 256 ? 256 : 512; }();
   // staged variant (coalesced cp.async into swizzled shared memory one step ahead): store path without fused dX
   static const int bw_staged = []() { const char* e = getenv("TSC_BPTT_STAGED"); return e ? atoi(e) : 1; }();
@@ -2009,8 +1677,8 @@ extern "C" int tscl_lstm_seq_bwd_tc_dx(tscl_handle* h, const void* wt_bf16, floa
 //   dW[k][c] = sum_m In[m][k] * dXm[m][c],   dXm = dX * (X > 0),   m = (t, replica) rows of one chunk
 // is a GEMM whose reduction index is the ROW index, so both operands are staged MN-major: the row-major global
 // data lands as [col/8][128 rows][8 cols] bf16 without a transposition, and
-//   D[dX column (two M = 128 halves)][64 input slots] += A^T B      (tcgen05.mma, a_major = b_major = MN, K = 128 rows)
-// accumulates in TMEM over all tiles of a unit.  A spare input slot holds 1.0: its D column is the bias gradient.
+//   D[dX column (two M = 128 halves)][64 input slots] += A^T B      (wgmma, A and B MN-major, K = 128 rows)
+// accumulates in the accumulator tile over all tiles of a unit.  A spare input slot holds 1.0: its D column is the bias gradient.
 // Persistent: CTA b owns the tile range [b NT / grid, (b + 1) NT / grid) of the (unit, tile) list and flushes its
 // accumulator with atomics whenever the unit changes (<= 3 flushes per CTA).
 #define FBT_ROWS 128
@@ -2020,6 +1688,7 @@ extern "C" int tscl_lstm_seq_bwd_tc_dx(tscl_handle* h, const void* wt_bf16, floa
 #define FBT_STAGE (FBT_A_BYTES + FBT_B_BYTES)
 #define FBT_THREADS 512
 struct FcBwdTC {
+  float* acc;                // accumulator tiles, one [128][ACC_COLS] fp32 tile per CTA (acc_tiles)
   const float* obs;            // rows as tscl_fc_embed
   const float* X;              // [2A][M][dx] fp32 activations, or
   const __nv_bfloat16* Xb;     // [2A][M][dx] bf16 activations (one chunk of the activation store)
@@ -2034,23 +1703,14 @@ __global__ void __launch_bounds__(FBT_THREADS, 1)
 fc_bwd_tc_kernel(const DDimsTC d, const FcBwdTC a) {
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   uint64_t* sBar = reinterpret_cast<uint64_t*>(tc_smem + 2 * FBT_STAGE);
-  uint32_t* sTmem = reinterpret_cast<uint32_t*>(sBar + 2);
   const uint32_t bar0 = smem_u32(sBar);
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(sTmem)), "r"(128));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
   if (tid == 0) {
     mbar_init(bar0, 1); mbar_init(bar0 + 8, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem = *sTmem;
+  float* const acc = a.acc + (size_t)blockIdx.x * TC_M * ACC_COLS;
   // bf16 x bf16 -> f32, A and B MN-major, N = 64, M = 128
-  const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | (1u << 16) | ((uint32_t)(64 >> 3) << 17) |
-                         ((uint32_t)(128 >> 4) << 24);
   const uint32_t lbo = a.variant ? FBT_SBO : 128, sbo = a.variant ? 128 : FBT_SBO;
   const int dx = d.dx, ng = dx >> 3, n_items = FBT_ROWS * ng;
   const uint32_t ng_magic = (1u << 20) / (uint32_t)ng + 1u;      // i / ng == (i * magic) >> 20 for i < 4096, ng <= 32
@@ -2066,13 +1726,11 @@ fc_bwd_tc_kernel(const DDimsTC d, const FcBwdTC a) {
   auto flush = [&](int u) {
     if (pend0) { mbar_wait(bar0, ph0); ph0 ^= 1; pend0 = false; }
     if (pend1) { mbar_wait(bar0 + 8, ph1); ph1 ^= 1; pend1 = false; }
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
     const int q = warp & 3, cgp = warp >> 2, mh = cgp >> 1, k0 = (cgp & 1) * 32;
     const int c = mh * 128 + q * 32 + lane;
     float v[32];
-    const uint32_t tb = tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(mh * 64 + k0);
-    tmem_ld16(tb, v); tmem_ld16(tb + 16, v + 16);
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+    const uint32_t tb = ((uint32_t)(q * 32) << 16) + (uint32_t)(mh * 64 + k0);
+    acc_ld16(acc, tb, v); acc_ld16(acc, tb + 16, v + 16);
     if (c < dx) {
       int64_t wo, bo; int ld, cc, s0, n;
       if (c < d.fw) { wo = d.off_fcw_w[u]; bo = d.off_fcw_b[u]; ld = d.fw; cc = c; s0 = 0; n = nw; }
@@ -2085,7 +1743,6 @@ fc_bwd_tc_kernel(const DDimsTC d, const FcBwdTC a) {
         if (slot == d.ones_slot) atomicAdd(&a.G[bo + cc], v[e]);
       }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
   };
 
@@ -2254,23 +1911,20 @@ fc_bwd_tc_kernel(const DDimsTC d, const FcBwdTC a) {
       *reinterpret_cast<uint4*>(sB + (size_t)bc * FBT_SBO + row * 16) = *reinterpret_cast<const uint4*>(o);
     }
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    if (tid == 0) {
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+    if (warp < 8) {
       const uint32_t aA = smem_u32(sA), aB = smem_u32(sB);
-#pragma unroll
       for (int mh = 0; mh < 2; ++mh)
-        for (int ks = 0; ks < FBT_ROWS / 16; ++ks)
-          umma_bf16(tmem + mh * 64, make_desc(aA + mh * 16 * FBT_SBO + ks * 256, lbo, sbo),
-                    make_desc(aB + ks * 256, lbo, sbo), idesc, (first && ks == 0) ? 0u : 1u);
-      umma_commit(bar0 + 8 * s);
+        wg_mma<1, 1>(acc, mh * 64, 64, FBT_ROWS / 16, !first, [&](int ks, uint64_t& da, uint64_t& db) {
+          da = make_desc(aA + mh * 16 * FBT_SBO + ks * 256, lbo, sbo);
+          db = make_desc(aB + ks * 256, lbo, sbo);
+        });
+      wg_mma_done(bar0 + 8 * s);
     }
     if (s == 0) pend0 = true; else pend1 = true;
     first = false;
   }
   if (cur_u >= 0) flush(cur_u);
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(128));
 }
 
 extern "C" int tscl_fc_bwd_tc(tscl_handle* h, const float* obs, const float* X, const void* x_bf16, const float* dX,
@@ -2292,6 +1946,8 @@ extern "C" int tscl_fc_bwd_tc(tscl_handle* h, const float* obs, const float* X, 
   const int64_t NT = ((M + FBT_ROWS - 1) / FBT_ROWS) * 2 * d.A;
   const int grid = (int)(NT < n_sm ? NT : n_sm);
   FcBwdTC a;
+  a.acc = acc_tiles(h, stream);
+  if (!a.acc) return tsc_set_error("accumulator tiles: cudaMalloc failed");
   a.obs = obs; a.X = X; a.Xb = (const __nv_bfloat16*)x_bf16; a.dX = dX; a.dXb = (const __nv_bfloat16*)dx_bf16; a.G = grads; a.M = M;
   a.rows_per_t = rows_per_t;
   a.stride_t = stride_t; a.variant = variant;
@@ -2304,13 +1960,14 @@ extern "C" int tscl_fc_bwd_tc(tscl_handle* h, const float* obs, const float* X, 
 // LSTM weight gradients on the tensor cores (replaces two cuBLAS GEMMs, a column reduction and the fp32 unpacking of
 // X / Hp):   dWx += X^T dZ,   dWh += Hp^T dZ,   dbl += 1^T dZ      over the rows m = (t, replica) of one chunk.
 // Same MN-major staging as fc_bwd_tc_kernel.  A = [X | Hp | 1] (dx + 64 + 1 columns = up to three M = 128 blocks),
-// B = one 128-column half of dZ; D[block][128 gate columns] accumulates in TMEM (384 columns).  A CTA owns a
+// B = one 128-column half of dZ; D[block][128 gate columns] accumulates in the accumulator tile (384 columns).  A CTA owns a
 // contiguous tile range of the (unit, half, tile) list and flushes with atomics when (unit, half) changes.
 // Hp is rebuilt from the bf16 activation store: Hp[t] = (1 - done[t]) * (t > 0 ? H[t-1] : h0).
 #define WG_A_CHUNKS 40
 #define WG_Z_CHUNKS 16
 #define WG_STAGE ((WG_A_CHUNKS + WG_Z_CHUNKS) * FBT_SBO)
 struct WGradTC {
+  float* acc;                // accumulator tiles, one [128][ACC_COLS] fp32 tile per CTA (acc_tiles)
   const float* dZ;             // [2A][M][256] fp32, or
   const __nv_bfloat16* dZb;    // [2A][M][256] bf16
   const float* X;              // [2A][M][dx] fp32, or
@@ -2328,24 +1985,15 @@ __global__ void __launch_bounds__(FBT_THREADS, 1)
 wgrad_tc_kernel(const DDimsTC d, const WGradTC a) {
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   uint64_t* sBar = reinterpret_cast<uint64_t*>(tc_smem + 2 * WG_STAGE);
-  uint32_t* sTmem = reinterpret_cast<uint32_t*>(sBar + 2);
   const uint32_t bar0 = smem_u32(sBar);
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(sTmem)), "r"(512));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
   if (tid == 0) {
     mbar_init(bar0, 1); mbar_init(bar0 + 8, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   // never-written A chunks are read by the last M block: keep them finite
   for (int i = tid; i < 2 * WG_STAGE / 16; i += FBT_THREADS) reinterpret_cast<uint4*>(tc_smem)[i] = make_uint4(0, 0, 0, 0);
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem = *sTmem;
-  const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | (1u << 16) | ((uint32_t)(128 >> 3) << 17) |
-                         ((uint32_t)(128 >> 4) << 24);
+  float* const acc = a.acc + (size_t)blockIdx.x * TC_M * ACC_COLS;
   const uint32_t lbo = a.variant ? FBT_SBO : 128, sbo = a.variant ? 128 : FBT_SBO;
   const int dx = d.dx, ng = dx >> 3, n_xitems = FBT_ROWS * ng;
   const int nb = (dx + TC_H + 1 + 127) >> 7;        // M blocks
@@ -2359,16 +2007,14 @@ wgrad_tc_kernel(const DDimsTC d, const WGradTC a) {
   auto flush = [&](int pu) {
     if (pend0) { mbar_wait(bar0, ph0); ph0 ^= 1; pend0 = false; }
     if (pend1) { mbar_wait(bar0 + 8, ph1); ph1 ^= 1; pend1 = false; }
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
     const int u = pu >> 1, nh = pu & 1;
     const int q = warp & 3, cq = warp >> 2;
     const int g0 = nh * 128 + cq * 32;
     for (int b = 0; b < nb; ++b) {
       const int ci = b * 128 + q * 32 + lane;
       float v[32];
-      const uint32_t tb = tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(b * 128 + cq * 32);
-      tmem_ld16(tb, v); tmem_ld16(tb + 16, v + 16);
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+      const uint32_t tb = ((uint32_t)(q * 32) << 16) + (uint32_t)(b * 128 + cq * 32);
+      acc_ld16(acc, tb, v); acc_ld16(acc, tb + 16, v + 16);
       float* dst = nullptr;
       if (ci < dx) dst = a.G + d.off_wx + ((int64_t)u * dx + ci) * TC_N + g0;
       else if (ci < dx + TC_H) dst = a.G + d.off_wh + ((int64_t)u * TC_H + (ci - dx)) * TC_N + g0;
@@ -2378,7 +2024,6 @@ wgrad_tc_kernel(const DDimsTC d, const WGradTC a) {
         for (int e = 0; e < 32; ++e) atomicAdd(dst + e, v[e]);
       }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
   };
 
@@ -2509,22 +2154,20 @@ wgrad_tc_kernel(const DDimsTC d, const WGradTC a) {
     if (tid < FBT_ROWS)
       *reinterpret_cast<uint4*>(sA + (size_t)(ng + 8) * FBT_SBO + tid * 16) = make_uint4(tid < rows_valid ? 0x3f80u : 0u, 0, 0, 0);
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    if (tid == 0) {
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+    if (warp < 8) {
       const uint32_t aA = smem_u32(sA), aZ = smem_u32(sZ);
       for (int b = 0; b < nb; ++b)
-        for (int ks = 0; ks < FBT_ROWS / 16; ++ks)
-          umma_bf16(tmem + b * 128, make_desc(aA + b * 16 * FBT_SBO + ks * 256, lbo, sbo),
-                    make_desc(aZ + ks * 256, lbo, sbo), idesc, (first && ks == 0) ? 0u : 1u);
-      umma_commit(bar0 + 8 * s);
+        wg_mma<1, 1>(acc, b * 128, 128, FBT_ROWS / 16, !first, [&](int ks, uint64_t& da, uint64_t& db) {
+          da = make_desc(aA + b * 16 * FBT_SBO + ks * 256, lbo, sbo);
+          db = make_desc(aZ + ks * 256, lbo, sbo);
+        });
+      wg_mma_done(bar0 + 8 * s);
     }
     if (s == 0) pend0 = true; else pend1 = true;
     first = false;
   }
   if (cur_pu >= 0) flush(cur_pu);
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512));
 }
 
 // All-bf16 variant (the training loop's): 64-row tiles, two smem stages + one register stage.  CTAs 2p and 2p+1 walk the
@@ -2538,13 +2181,8 @@ __global__ void __launch_bounds__(FBT_THREADS, 1)
 wgrad_tc_async_kernel(const DDimsTC d, const WGradTC a) {
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   uint64_t* sBar = reinterpret_cast<uint64_t*>(tc_smem + WGA_STAGES * WGA_STAGE);
-  uint32_t* sTmem = reinterpret_cast<uint32_t*>(sBar + WGA_STAGES);
-  float* sDone = reinterpret_cast<float*>(sTmem + 2);
+  float* sDone = reinterpret_cast<float*>(sBar + WGA_STAGES + 1);
   const uint32_t bar0 = smem_u32(sBar);
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(sTmem)), "r"(512));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
   if (tid == 0) {
     for (int i = 0; i < WGA_STAGES; ++i) mbar_init(bar0 + 8 * i, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -2552,12 +2190,8 @@ wgrad_tc_async_kernel(const DDimsTC d, const WGradTC a) {
   // never-written A chunks are read by the last M block: keep them finite
   for (int i = tid; i < WGA_STAGES * WGA_STAGE / 16; i += FBT_THREADS) reinterpret_cast<uint4*>(tc_smem)[i] = make_uint4(0, 0, 0, 0);
   for (int i = tid; i < a.T; i += FBT_THREADS) sDone[i] = a.done[i];
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem = *sTmem;
-  const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | (1u << 16) | ((uint32_t)(128 >> 3) << 17) |
-                         ((uint32_t)(128 >> 4) << 24);
+  float* const acc = a.acc + (size_t)blockIdx.x * TC_M * ACC_COLS;
   const uint32_t lbo = a.variant ? WGA_SBO : 128, sbo = a.variant ? 128 : WGA_SBO;
   const int dx = d.dx, ng = dx >> 3, n_xitems = WGA_ROWS * ng;
   const uint32_t ng_magic = (1u << 20) / (uint32_t)ng + 1u;      // i / ng == (i * magic) >> 20 for i < 4096, ng <= 32
@@ -2574,15 +2208,13 @@ wgrad_tc_async_kernel(const DDimsTC d, const WGradTC a) {
   };
   auto flush = [&](int u) {
     for (int s = 0; s < WGA_STAGES; ++s) wait_stage(s);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
     const int q = warp & 3, cq = warp >> 2;
     const int g0 = nh * 128 + cq * 32;
     for (int b = 0; b < nb; ++b) {
       const int ci = b * 128 + q * 32 + lane;
       float v[32];
-      const uint32_t tb = tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(b * 128 + cq * 32);
-      tmem_ld16(tb, v); tmem_ld16(tb + 16, v + 16);
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+      const uint32_t tb = ((uint32_t)(q * 32) << 16) + (uint32_t)(b * 128 + cq * 32);
+      acc_ld16(acc, tb, v); acc_ld16(acc, tb + 16, v + 16);
       float* dst = nullptr;
       if (ci < dx) dst = a.G + d.off_wx + ((int64_t)u * dx + ci) * TC_N + g0;
       else if (ci < dx + TC_H) dst = a.G + d.off_wh + ((int64_t)u * TC_H + (ci - dx)) * TC_N + g0;
@@ -2592,7 +2224,6 @@ wgrad_tc_async_kernel(const DDimsTC d, const WGradTC a) {
         for (int e = 0; e < 32; ++e) atomicAdd(dst + e, v[e]);
       }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
   };
 
@@ -2602,7 +2233,7 @@ wgrad_tc_async_kernel(const DDimsTC d, const WGradTC a) {
   int64_t it_t = im0 / a.rc, it_rem = im0 - it_t * a.rc;
   // Register-staged pipeline: the 7 pieces (16 B each: 2 of dZ, <= 4 of X, 1 of Hp) of tile j + 2 are loaded into
   // registers while tile j is multiplied and tile j + 1 sits in the other smem stage; they are stored one iteration
-  // later, when their latency has passed.  (cp.async was measured slower here: LDGSTS keeps its address registers
+  // later, when their latency has passed.  (cp.async is slower here: LDGSTS keeps its address registers
   // reserved until the copy completes, and the allocator's reuse of them stalls the warp for a memory latency.)
   uint4 pv[7];
   int prv = 0;                                   // rows_valid of the tile held in pv
@@ -2680,16 +2311,15 @@ wgrad_tc_async_kernel(const DDimsTC d, const WGradTC a) {
       cur_u = u; first = true;
     }
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    if (tid == 0) {
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+    if (warp < 8) {
       const uint32_t aA = smem_u32(tc_smem + (size_t)s * WGA_STAGE), aZ = aA + WG_A_CHUNKS * WGA_SBO;
       for (int b = 0; b < nb; ++b)
-        for (int ks = 0; ks < WGA_ROWS / 16; ++ks)
-          umma_bf16(tmem + b * 128, make_desc(aA + b * 16 * WGA_SBO + ks * 256, lbo, sbo),
-                    make_desc(aZ + ks * 256, lbo, sbo), idesc, (first && ks == 0) ? 0u : 1u);
-      umma_commit(bar0 + 8 * s);
+        wg_mma<1, 1>(acc, b * 128, 128, WGA_ROWS / 16, !first, [&](int ks, uint64_t& da, uint64_t& db) {
+          da = make_desc(aA + b * 16 * WGA_SBO + ks * 256, lbo, sbo);
+          db = make_desc(aZ + ks * 256, lbo, sbo);
+        });
+      wg_mma_done(bar0 + 8 * s);
     }
     pend |= 1u << s;
     first = false;
@@ -2700,7 +2330,6 @@ wgrad_tc_async_kernel(const DDimsTC d, const WGradTC a) {
     }
   }
   if (cur_u >= 0) flush(cur_u);
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512));
 }
 
 extern "C" int tscl_wgrad_tc(tscl_handle* h, const float* dZ, const void* dz_bf16, const float* X, const void* x_bf16,
@@ -2726,6 +2355,8 @@ extern "C" int tscl_wgrad_tc(tscl_handle* h, const float* dZ, const void* dz_bf1
   const int64_t NT = ((M + FBT_ROWS - 1) / FBT_ROWS) * 4 * d.A;
   const int grid = (int)(NT < n_sm ? NT : n_sm);
   WGradTC a;
+  a.acc = acc_tiles(h, stream);
+  if (!a.acc) return tsc_set_error("accumulator tiles: cudaMalloc failed");
   a.dZ = dZ; a.dZb = (const __nv_bfloat16*)dz_bf16; a.X = X; a.Xb = (const __nv_bfloat16*)x_bf16; a.Hp = Hp; a.Hb = (const __nv_bfloat16*)h_bf16; a.h0 = h0;
   a.done = done; a.G = grads; a.M = M; a.rc = rc; a.ld_state = ld_state; a.r0 = r0; a.T = T; a.variant = variant;
   if (a.dZb && a.Xb && a.Hb && T <= WGA_MAXT) {
@@ -2742,27 +2373,26 @@ extern "C" int tscl_wgrad_tc(tscl_handle* h, const float* dZ, const void* dz_bf1
 // ===================================================================================================
 // dX = dZ . Wx^T  (input gradient of the LSTM's x-projection, agents/utils.py:103-105 differentiated): a streaming GEMM
 // [M x 256] . [256 x dx] per unit, 960 B of HBM traffic per row.  Warp-specialised persistent kernel:
-//   warps 4-7  loaders : 16-byte cp.async of one swizzle atom (128 rows x 64 K, 16 KB) per stage, written in the
-//                        SWIZZLE_128B K-major pattern (chunk ^ (row & 7)); 3 stages, completion signalled two stages late
-//   warp  8    MMA     : 4 x tcgen05.mma (M = 128, N = dx, K = 16) per atom, B = the unit's Wx^T image resident in shared
-//                        memory (fetched by one cp.async.bulk per unit), accumulators double-buffered in TMEM (2 x 256 cols)
-//   warps 0-3  epilogue: tcgen05.ld -> bf16 -> padded row in shared memory -> one cp.async.bulk store per row (448 B),
-//                        drained by the copy engine while the next tile is converted
+//   warps 8-11  loaders : 16-byte cp.async of one swizzle atom (128 rows x 64 K, 16 KB) per stage, written in the
+//                         SWIZZLE_128B K-major pattern (chunk ^ (row & 7)); 3 stages, completion signalled two stages late
+//   warps 0-7   MMA     : two warpgroups (64 rows each), 4 x wgmma (N = dx, K = 16) per atom, B = the unit's Wx^T image
+//                         resident in shared memory (fetched by one cp.async.bulk per unit), accumulators double-buffered
+//                         in the accumulator tile (2 x 256 columns)
+//   warps 12-15 epilogue: accumulator row -> bf16 -> padded row in shared memory -> one cp.async.bulk store per row
+//                         (448 B), drained by the copy engine while the next tile is converted
 // A CTA owns a contiguous range of the (unit, 128-row tile) list, so it changes unit at most twice.
-#define DXK_THREADS 288
+#define DXK_THREADS 512
 #define DXK_STAGES 3
 #define DXK_STAGE_BYTES 16384
 struct DxTC {
+  float* acc;                // accumulator tiles, one [128][ACC_COLS] fp32 tile per CTA (acc_tiles)
   const __nv_bfloat16* dZb;    // [2A][M][256]
   const __nv_bfloat16* Wxt;    // [2A][32][dx][8]  (tscl_pack_wxt)
   __nv_bfloat16* dXb;          // [2A][M][dx]
   int64_t M;
 };
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
 __device__ __forceinline__ uint64_t make_desc_sw128(uint32_t saddr) {      // K-major, 128-byte swizzle, 8-row groups 1024 B apart
-  return (uint64_t)((saddr >> 4) & 0x3FFFu) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) | (2ull << 61);
+  return (uint64_t)((saddr >> 4) & 0x3FFFu) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);   // layout type 1: 128B swizzle
 }
 
 __global__ void __launch_bounds__(DXK_THREADS, 1)
@@ -2773,30 +2403,23 @@ dx_tc_kernel(const DDimsTC d, const DxTC a) {
   unsigned char* sB = sStage + DXK_STAGES * DXK_STAGE_BYTES;
   unsigned char* sOut = sB + (size_t)BW_KC * dx * 16;
   uint64_t* sBar = reinterpret_cast<uint64_t*>(sOut + (size_t)128 * out_stride);
-  uint32_t* sTmem = reinterpret_cast<uint32_t*>(sBar + 12);
   const uint32_t bar_full = smem_u32(sBar), bar_empty = bar_full + 24, bar_accf = bar_full + 48, bar_acce = bar_full + 64,
-                 bar_b = bar_full + 80, bar_d = bar_full + 88;
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(sTmem)), "r"(512));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
+                 bar_b = bar_full + 80;
   if (tid == 0) {
     for (int s = 0; s < DXK_STAGES; ++s) { mbar_init(bar_full + 8 * s, 128); mbar_init(bar_empty + 8 * s, 1); }
     for (int b = 0; b < 2; ++b) { mbar_init(bar_accf + 8 * b, 1); mbar_init(bar_acce + 8 * b, 128); }
-    mbar_init(bar_b, 1); mbar_init(bar_d, 1);
+    mbar_init(bar_b, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem = *sTmem;
+  float* const acc = a.acc + (size_t)blockIdx.x * TC_M * ACC_COLS;
   const int64_t tpu = (a.M + 127) / 128;
   const int64_t NT = tpu * 2 * d.A;
   const int64_t j0 = NT * blockIdx.x / gridDim.x, j1 = NT * (blockIdx.x + 1) / gridDim.x;
 
-  if (warp >= 4 && warp < 8) {
+  if (warp >= 8 && warp < 12) {
     // ---------------- loaders ----------------
-    const int lt = tid - 128;
+    const int lt = tid - 256;
     const uint32_t aS = smem_u32(sStage);
     int64_t it = 0;
     for (int64_t j = j0; j < j1; ++j) {
@@ -2831,49 +2454,41 @@ dx_tc_kernel(const DDimsTC d, const DxTC a) {
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
       mbar_arrive(bar_full + 8 * (int)((it - 1) % DXK_STAGES));
     }
-  } else if (warp == 8) {
-    // ---------------- MMA issuer ----------------
-    if (lane == 0) {
-      const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(dx >> 3) << 17) | ((uint32_t)(TC_M >> 4) << 24);
-      const uint32_t aS = smem_u32(sStage), aB = smem_u32(sB);
-      const uint32_t b_lbo = (uint32_t)dx * 16;
-      int64_t it = 0, tc = 0;
-      int cur_u = -1;
-      uint32_t bph = 0, dph = 0;
-      for (int64_t j = j0; j < j1; ++j, ++tc) {
-        const int u = (int)(j / tpu);
-        if (u != cur_u) {
-          if (cur_u >= 0) {                       // the MMAs in flight still read the previous unit's image
-            umma_commit(bar_d);
-            mbar_wait(bar_d, dph); dph ^= 1;
-          }
-          cur_u = u;
+  } else if (warp < 8) {
+    // ---------------- MMA: warps 0-7, one warpgroup per 64-row half ----------------
+    const uint32_t aS = smem_u32(sStage), aB = smem_u32(sB);
+    const uint32_t b_lbo = (uint32_t)dx * 16;
+    int64_t it = 0, tc = 0;
+    int cur_u = -1;
+    uint32_t bph = 0;
+    for (int64_t j = j0; j < j1; ++j, ++tc) {
+      const int u = (int)(j / tpu);
+      if (u != cur_u) {      // every MMA of the previous unit has completed (wg_mma_done of its last atom)
+        cur_u = u;
+        if (tid == 0) {
           const uint32_t bytes = (uint32_t)BW_KC * dx * 16;
           mbar_expect_tx(bar_b, bytes);
           bulk_g2s(aB, a.Wxt + (int64_t)u * BW_KC * dx * 8, bytes, bar_b);
-          mbar_wait(bar_b, bph); bph ^= 1;
         }
-        const int b = (int)(tc & 1);
-        const int64_t nb = tc >> 1;
-        if (nb > 0) mbar_wait(bar_acce + 8 * b, (uint32_t)((nb - 1) & 1));
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        for (int at = 0; at < 4; ++at, ++it) {
-          const int s = (int)(it % DXK_STAGES);
-          mbar_wait(bar_full + 8 * s, (uint32_t)((it / DXK_STAGES) & 1));
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll
-          for (int k = 0; k < 4; ++k)
-            umma_bf16(tmem + b * 256, make_desc_sw128(aS + s * DXK_STAGE_BYTES + k * 32),
-                      make_desc(aB + (uint32_t)((at * 4 + k) * 2) * b_lbo, b_lbo, 128), idesc, (at | k) ? 1u : 0u);
-          umma_commit(bar_empty + 8 * s);
-        }
-        umma_commit(bar_accf + 8 * b);
+        mbar_wait(bar_b, bph); bph ^= 1;
       }
+      const int b = (int)(tc & 1);
+      const int64_t nb = tc >> 1;
+      if (nb > 0) mbar_wait(bar_acce + 8 * b, (uint32_t)((nb - 1) & 1));
+      for (int at = 0; at < 4; ++at, ++it) {
+        const int s = (int)(it % DXK_STAGES);
+        mbar_wait(bar_full + 8 * s, (uint32_t)((it / DXK_STAGES) & 1));
+        wg_mma<0, 0>(acc, b * 256, dx, 4, at > 0, [&](int k, uint64_t& da, uint64_t& db) {
+          da = make_desc_sw128(aS + s * DXK_STAGE_BYTES + k * 32);
+          db = make_desc(aB + (uint32_t)((at * 4 + k) * 2) * b_lbo, b_lbo, 128);
+        });
+        wg_mma_done(bar_empty + 8 * s);
+      }
+      if (tid == 0) mbar_arrive(bar_accf + 8 * b);
     }
-    __syncwarp();
   } else {
-    // ---------------- epilogue: thread = row (TMEM lane) ----------------
-    const int row = tid;
+    // ---------------- epilogue: warps 12-15, thread = row ----------------
+    const int row = tid - 384;
     unsigned char* my = sOut + (size_t)row * out_stride;
     const uint32_t my_s = smem_u32(my);
     int64_t tc = 0;
@@ -2882,14 +2497,12 @@ dx_tc_kernel(const DDimsTC d, const DxTC a) {
       const int64_t m0 = (j - (int64_t)u * tpu) * 128;
       const int b = (int)(tc & 1);
       mbar_wait(bar_accf + 8 * b, (uint32_t)((tc >> 1) & 1));
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
       asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");      // the previous store of this row has left shared memory
-      const uint32_t tb = tmem + ((uint32_t)(warp * 32) << 16) + (uint32_t)(b * 256);
+      const uint32_t tb = ((uint32_t)((warp - 12) * 32) << 16) + (uint32_t)(b * 256);
       for (int c0 = 0; c0 < dx; c0 += 32) {
         float v[32];
-        tmem_ld16(tb + c0, v);
-        if (c0 + 16 < dx) tmem_ld16(tb + c0 + 16, v + 16);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+        acc_ld16(acc, tb + c0, v);
+        if (c0 + 16 < dx) acc_ld16(acc, tb + c0 + 16, v + 16);
         const int nq = (c0 + 16 < dx) ? 4 : 2;
 #pragma unroll
         for (int qd = 0; qd < 4; ++qd) {
@@ -2901,7 +2514,6 @@ dx_tc_kernel(const DDimsTC d, const DxTC a) {
           }
         }
       }
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
       mbar_arrive(bar_acce + 8 * b);
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
       if (m0 + row < a.M) {
@@ -2912,9 +2524,7 @@ dx_tc_kernel(const DDimsTC d, const DxTC a) {
     }
     asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512));
 }
 
 extern "C" int tscl_dx_tc(tscl_handle* h, const void* dz_bf16, const void* wxt_bf16, void* dx_bf16, int64_t M, void* stream) {
@@ -2934,6 +2544,8 @@ extern "C" int tscl_dx_tc(tscl_handle* h, const void* dz_bf16, const void* wxt_b
   const int64_t NT = ((M + 127) / 128) * 2 * d.A;
   const int grid = (int)(NT < n_sm ? NT : n_sm);
   DxTC a;
+  a.acc = acc_tiles(h, stream);
+  if (!a.acc) return tsc_set_error("accumulator tiles: cudaMalloc failed");
   a.dZb = (const __nv_bfloat16*)dz_bf16; a.Wxt = (const __nv_bfloat16*)wxt_bf16; a.dXb = (__nv_bfloat16*)dx_bf16; a.M = M;
   dx_tc_kernel<<<grid, DXK_THREADS, smem, (cudaStream_t)stream>>>(d, a);
   PCK(cudaGetLastError());

@@ -1,4 +1,4 @@
-// tsc_sim.cu — sm_100a control-step kernel + C ABI (include/tsc.h) of libtsc.
+// tsc_sim.cu — sm_90a (H100) control-step kernel + C ABI (include/tsc.h) of libtsc.
 //
 // One CTA advances ONE road-network replica through one whole control interval
 // (reference envs/env.py:566-631: yellow phase, 2 x 1 s, green phase, 3 x 1 s, detector reads,
@@ -1306,7 +1306,9 @@ extern "C" int tsc_mean_live(tsc_handle* h, double* mean_live) {
   if (!h || !mean_live) return fail("tsc_mean_live: bad argument");
   CK(cudaSetDevice(h->device));
   CK(cudaMemset(h->d_scalar, 0, 8));
-  tsc_live_kernel<<<148, 256>>>(h->args.lane_cnt, h->args.net.lpad, h->args.net.n_lanes, h->R, h->d_scalar);
+  int n_sm = 0;
+  CK(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, h->device));
+  tsc_live_kernel<<<n_sm, 256>>>(h->args.lane_cnt, h->args.net.lpad, h->args.net.n_lanes, h->R, h->d_scalar);
   CK(cudaGetLastError());
   unsigned long long s = 0;
   CK(cudaMemcpy(&s, h->d_scalar, 8, cudaMemcpyDeviceToHost));

@@ -11,7 +11,7 @@ Same constructor arguments, attributes and method names as the reference so that
 
 With `n_replicas == 1` (default) returns exactly the reference's Python types, through the
 host-buffer entry point `tsc_step_host`.  With `n_replicas > 1` the batched methods
-(`reset_batch/step_batch`) return device tensors [R, ...] for the B200 learner.
+(`reset_batch/step_batch`) return device tensors [R, ...] for the device-resident learner.
 There is no SUMO process: `gui` is accepted and ignored, `terminate()` is a no-op.
 """
 from __future__ import annotations

@@ -1,5 +1,5 @@
 /*
- * tsc.h — C ABI of libtsc (traffic-signal-control simulator, B200 / sm_100a).
+ * tsc.h — C ABI of libtsc (traffic-signal-control simulator, H100 / sm_90a).
  *
  * This is the drop-in boundary for the hot path of cts198859/deeprl_signal_control:
  *   TrafficSimulator.step()/reset()            reference envs/env.py:544-631

@@ -1,5 +1,5 @@
 /*
- * tsc_learn.h — C ABI of the per-intersection A2C learner kernels in libtsc (sm_100a).
+ * tsc_learn.h — C ABI of the per-intersection A2C learner kernels in libtsc (sm_90a).
  *
  * Replaces, for R lock-stepped replicas and all A agents at once, the TF1 graphs of the reference:
  *   fc / lstm layers                         agents/utils.py:66-74, 88-116
@@ -13,7 +13,7 @@
  * All pointers are caller-owned DEVICE pointers; `stream` is a cudaStream_t as void*.
  * Every function returns 0 or <0 (message via tsc_last_error()).  The three plain time-batched
  * GEMMs of the update (X.Wx, dZ.Wx^T, X^T.dZ) are NOT in this ABI: the host calls the vendor
- * library for them (DESIGN.md §5) until the tcgen05 kernels replace them.
+ * library for them (DESIGN.md §5) until the tensor-core kernels replace them.
  */
 #ifndef TSC_LEARN_H_
 #define TSC_LEARN_H_
@@ -113,7 +113,7 @@ int tscl_lstm_seq_bwd(tscl_handle* h, const float* params, float* ZG, const floa
 int tscl_fc_bwd(tscl_handle* h, const float* obs, const float* X, const float* dX, int64_t M,
                 int64_t rows_per_t, int64_t stride_t, float* grads, void* stream);
 
-/* The same contraction on the tensor cores (tcgen05, MN-major bf16 operands, fp32 accumulation in TMEM over
+/* The same contraction on the tensor cores (wgmma, MN-major bf16 operands, fp32 accumulation in the accumulator tile over
  * 128-row tiles; replaces the SIMT kernel in the training loop).  Pass the activations either as fp32 `X` or as one
  * chunk of the bf16 activation store `x_bf16` ([2A][M][dx]); `variant` must be 0. */
 int tscl_fc_bwd_tc(tscl_handle* h, const float* obs, const float* X, const void* x_bf16, const float* dX,
@@ -122,7 +122,7 @@ int tscl_fc_bwd_tc(tscl_handle* h, const float* obs, const float* X, const void*
 /* dX likewise as fp32 `dX` or bf16 `dx_bf16` ([2A][M][dx]). */
 
 /* LSTM weight gradients of one chunk on the tensor cores:  grads.wx += X^T dZ, grads.wh += Hp^T dZ, grads.bl += 1^T dZ
- * (rows m = t * rc + r, M = T * rc; bf16 operands, fp32 accumulation in TMEM).  X as fp32 `X` or bf16 `x_bf16`
+ * (rows m = t * rc + r, M = T * rc; bf16 operands, fp32 accumulation).  X as fp32 `X` or bf16 `x_bf16`
  * ([2A][M][dx]); Hp as fp32 `Hp` ([2A][M][h]) or rebuilt from the bf16 store chunk `h_bf16` ([2A][T][rc][h]) as
  * (1 - done[t]) * (t > 0 ? H[t-1] : h0[u][r0 + r]).  `variant` must be 0. */
 int tscl_wgrad_tc(tscl_handle* h, const float* dZ, const void* dz_bf16, const float* X, const void* x_bf16,
@@ -130,7 +130,7 @@ int tscl_wgrad_tc(tscl_handle* h, const float* dZ, const void* dz_bf16, const fl
                   int64_t ld_state, int64_t r0, float* grads, int32_t variant, void* stream);
 /* dZ likewise as fp32 `dZ` or bf16 `dz_bf16` ([2A][M][256], written by tscl_lstm_seq_bwd_tc). */
 
-/* BPTT on the tensor cores (tcgen05): same contract as tscl_lstm_seq_bwd, with the recurrent product dz.Wh^T as
+/* BPTT on the tensor cores (wgmma): same contract as tscl_lstm_seq_bwd, with the recurrent product dz.Wh^T as
  * a bf16 MMA (M=128, N=64, K=256) per step; wt_bf16 [2A][32][64][8] comes from tscl_pack_wht (refresh after
  * every optimizer step).  With gates_bf16 / c_bf16 / dz_bf16 and ZG == NULL (the shipping call) the per-step operand tile
  * of 128 replicas (gates, c, dH: 112 KB) is fetched one step ahead by cp.async.bulk.tensor copies through tensor maps
@@ -140,8 +140,8 @@ int tscl_pack_wht(tscl_handle* h, const float* params, void* wt_bf16, void* stre
 int tscl_lstm_seq_bwd_tc(tscl_handle* h, const void* wt_bf16, float* ZG, const float* C, const float* dH, const float* c0,
                          const float* done, int32_t T, int64_t Rc, int64_t ld_state, int64_t r0,
                          const void* gates_bf16, const void* c_bf16, void* dz_bf16, void* stream);
-/* The same kernel with dX = dZ . Wx^T fused into every step (second tcgen05 product of the same dz tile, M=128, N=dx,
- * K=256, accumulator in TMEM columns 64..64+dx): wxt_bf16 [2A][32][dx][8] from tscl_pack_wxt (refresh after every
+/* The same kernel with dX = dZ . Wx^T fused into every step (second wgmma product of the same dz tile, M=128, N=dx,
+ * K=256, accumulator columns 64..64+dx): wxt_bf16 [2A][32][dx][8] from tscl_pack_wxt (refresh after every
  * optimizer step), dx_bf16 [2A][T*Rc][dx] receives dX as bf16 — one way of replacing the last library GEMM of the update
  * (the shipping one is tscl_dx_tc below)
  * (reference: the tf.gradients chain through agents/utils.py:106, `tf.matmul(x, wx)`).  Both NULL = plain BPTT. */
@@ -166,7 +166,7 @@ int tscl_device_transition(tscl_handle* h, const float* rew_dev, float* rew_hist
 int tscl_memcpy_async(tscl_handle* h, void* dst, const void* src, int64_t bytes, int32_t kind, void* stream);
 /* dX = dZ . Wx^T as a stand-alone streaming product (the shipping path; reference: tf.gradients through
  * `tf.matmul(x, wx)`, agents/utils.py:106): dz_bf16 [2A][M][256], wxt_bf16 from tscl_pack_wxt, dx_bf16 [2A][M][dx] out.
- * Warp-specialised tcgen05 kernel (cp.async loaders -> 128B-swizzled operand stages, TMEM double buffer, bulk-copy stores).
+ * Warp-specialised wgmma kernel (cp.async loaders -> 128B-swizzled operand stages, double-buffered accumulator tiles, bulk-copy stores).
  * dx must be a multiple of 16, <= 224 for the shared-memory budget. */
 int tscl_dx_tc(tscl_handle* h, const void* dz_bf16, const void* wxt_bf16, void* dx_bf16, int64_t M, void* stream);
 /* gates_bf16 / c_bf16 (both or neither): read gate activations and c_t straight from one chunk of the bf16
@@ -184,7 +184,7 @@ int tscl_unpack_store(tscl_handle* h, const void* st_x, const void* st_g, const 
  * device counters while the pointer is set (NULL = off; a separate instantiation of the kernel, the hot one is unchanged). */
 int tscl_debug_policy_prof(void* counters_dev);
 /* same for the staged BPTT kernel: 8 counters (operand wait | smem->regs + cell backward + dZ stores | barrier | MMA + wait |
- * TMEM read-back), summed over CTAs; NULL switches profiling off */
+ * accumulator read-back), summed over CTAs; NULL switches profiling off */
 int tscl_debug_bptt_prof(void* counters_dev);
 
 /* Per-agent clip_by_global_norm(max_norm) + RMSProp step (TF1 semantics).  agent_of [n_params] u8.
@@ -192,11 +192,11 @@ int tscl_debug_bptt_prof(void* counters_dev);
 int tscl_clip_rmsprop(tscl_handle* h, float* params, float* grads, float* ms, const uint8_t* agent_of,
                       float max_norm, float lr, float alpha, float eps, float* norms, void* stream);
 
-/* ---- fused tensor-core policy forward (tcgen05 + TMEM), csrc/tsc_policy_tc.cu -------------------------
+/* ---- fused tensor-core policy forward (wgmma), csrc/tsc_policy_tc.cu -------------------------
  * tscl_pack_weights: per unit, [Wx;Wh] -> bf16 UMMA operand image [(dx+h)/8][4h][8] followed by the
  *   block-diagonal fc image [8][dx][8]; wpack holds 2A such records (call after every optimizer step).
  * tscl_policy_step: one decision for R replicas and all agents in ONE kernel: fc front end, gate GEMM on
- *   the tensor cores (bf16 operands, fp32 accumulate in TMEM), LSTM cell, heads, softmax, sampling.
+ *   the tensor cores (bf16 operands, fp32 accumulation), LSTM cell, heads, softmax, sampling.
  *   Replaces LstmACPolicy.forward / FPLstmACPolicy.forward for a whole batch (agents/policies.py:125-136).
  *   c_in/h_in/c_out/h_out [2A][R][h] (out may alias in); pi [R][A][max_na]; val [R][A]; act [R][A] or NULL;
  *   zdbg [2A][R][4h] raw gate accumulators (debug) or NULL; swap_lbo_sbo: debug switch, pass 0. */
@@ -207,7 +207,7 @@ int tscl_policy_step(tscl_handle* h, const float* params, const void* wpack_bf16
                      int32_t swap_lbo_sbo, void* stream);
 
 /* v2 of the fused forward: the fc front end runs on the tensor cores as well (observation slice tile x
- * block-diagonal fc weights -> TMEM -> relu/bf16 -> A operand).  Same arguments as tscl_policy_step
+ * block-diagonal fc weights -> accumulator -> relu/bf16 -> A operand).  Same arguments as tscl_policy_step
  * (without the descriptor debug switch); needs dx % 32 == 0.  wpack must come from tscl_pack_weights. */
 int tscl_policy_step_v2(tscl_handle* h, const float* params, const void* wpack_bf16, const float* obs, int64_t R,
                         const float* c_in, const float* h_in, float* c_out, float* h_out, float* pi, float* val,

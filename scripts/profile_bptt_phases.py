@@ -28,13 +28,14 @@ _lib.lib().tscl_debug_bptt_prof(C.c_void_p(prof.data_ptr()))
 tr.run(1)                         # the 120th step triggers the update
 torch.cuda.synchronize()
 _lib.lib().tscl_debug_bptt_prof(None)
-p = prof.cpu().numpy().astype(float) / 148
-tot = p.sum()
+n_sm = torch.cuda.get_device_properties(0).multi_processor_count
 n_items = 2 * lay.A * ((chunk + 127) // 128) * ((R + chunk - 1) // chunk)
-steps = n_items * 120 / 148
-print("BPTT: %.0f cycles per CTA per update (%.2f ms at 1.965 GHz), %.0f (tile, step) pairs per CTA = %.0f cycles each"
-      % (tot, tot / 1.965e6, steps, tot / steps))
+n_cta = min(n_items, n_sm)                      # persistent grid of the staged kernel
+p = prof.cpu().numpy().astype(float) / n_cta
+tot = p.sum()
+steps = n_items * 120 / n_cta
+print("BPTT: %.0f cycles per CTA per update, %.0f (tile, step) pairs per CTA = %.0f cycles each" % (tot, steps, tot / steps))
 for nm, v in zip(["wait for step t's operands", "smem -> regs, prefetch issue, cell backward, dZ stores",
-                  "fence + barrier before the MMA", "MMA issue + commit + wait", "TMEM read-back",
+                  "fence + barrier before the MMA", "MMA + fragment store + barrier", "accumulator read-back",
                   "  (of phase 2) smem -> regs + first sub-batch", "  (of phase 2) barrier", "  (of phase 2) operand issue (TMA / cp.async)"], p):
     print("   %-56s %9.0f cycles  %5.1f %%   %.0f per step" % (nm, v, 100 * v / tot, v / steps))

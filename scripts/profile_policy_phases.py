@@ -30,13 +30,14 @@ for store in (True, False):
         m.forward(obs, False)
     torch.cuda.synchronize()
     lib.tscl_debug_policy_prof(None)
-    pa = prof.cpu().numpy().astype(float) / n / 148
+    n_cta = min(((R + 127) // 128) * 2 * lay.A, torch.cuda.get_device_properties(0).multi_processor_count)
+    pa = prof.cpu().numpy().astype(float) / n / n_cta
     p = pa[:7]
     tot = pa.sum()
-    print("activation store %s: %.0f cycles per CTA per launch (%.3f ms at 1.965 GHz)" % (store, tot, tot / 1.965e6))
+    print("activation store %s: %.0f cycles per CTA per launch" % (store, tot))
     for nm, v in zip(names, p):
         print("   %-36s %9.0f cycles  %5.1f %%" % (nm, v, 100 * v / tot))
     del m
-    for nm, v in zip(["  epilogue: TMEM loads + cell math", "  epilogue: X copy-out", "  epilogue: gates copy-out",
+    for nm, v in zip(["  epilogue: accumulator loads + cell math", "  epilogue: X copy-out", "  epilogue: gates copy-out",
                       "  epilogue: c / h fp32 state copy-out", "  epilogue: c | h bf16 copy-out"], pa[8:13]):
         print("   %-36s %9.0f cycles  %5.1f %%" % (nm, v, 100 * v / tot))

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -18,7 +18,7 @@ def pytest_collection_modifyitems(config, items):
     import torch
     if torch.cuda.is_available():
         return
-    skip = pytest.mark.skip(reason="needs a CUDA device (B200): there is no CPU fallback of the product path")
+    skip = pytest.mark.skip(reason="needs a CUDA device (H100): there is no CPU fallback of the product path")
     for item in items:
         if "gpu" in item.keywords:
             item.add_marker(skip)

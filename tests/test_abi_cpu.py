@@ -1,4 +1,4 @@
-"""CPU: the C-ABI shared library builds for sm_100a without a GPU, loads, and exports every function that
+"""CPU: the C-ABI shared library builds for sm_90a without a GPU, loads, and exports every function that
 include/tsc.h and include/tsc_learn.h declare; the Python loader's symbol list is exactly that set; and the product
 path fails loudly without a CUDA device (there is no CPU fallback)."""
 import ctypes as C

@@ -178,7 +178,7 @@ def _fc_layout():
 
 def test_fc_policy_forward_and_gradients_match_oracle():
     """FcACPolicy (agents/policies.py:214-256, BASELINE config 2): forward vs the float64 restatement, gradients vs
-    float64 autograd (rel. 3e-4 of each tensor's max), with the fp32 front-end gradient kernel and the tcgen05 one."""
+    float64 autograd (rel. 3e-4 of each tensor's max), with the fp32 front-end gradient kernel and the wgmma one."""
     from deeprl_signal_control_b200.agents.learner_fc import BatchedFcA2C
     from oracle.learner_ref import a2c_loss, nstep_returns, unit_forward
     lay = _fc_layout()
@@ -232,7 +232,7 @@ def test_fc_policy_forward_and_gradients_match_oracle():
                                torch.from_numpy(m.Adv.cpu().numpy().astype(np.float64)), dones_pre, zeros, zeros, v_coef, beta)
         loss.backward()
         gv, rv = lay.views(G), lay.views(P.grad.numpy())
-        tol = 2e-2 if m.fc_bwd_tc else 3e-4           # the tcgen05 kernel multiplies bf16-rounded operands
+        tol = 2e-2 if m.fc_bwd_tc else 3e-4           # the wgmma kernel multiplies bf16-rounded operands
         for k in gv:
             if rv[k].size == 0 or (m.fc_bwd_tc and not k.startswith("fc")):
                 continue

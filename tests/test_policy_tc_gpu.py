@@ -1,4 +1,4 @@
-"""GPU: the fused tcgen05 policy-forward kernel (tscl_policy_step) vs the fp32 kernels / the oracle.
+"""GPU: the fused wgmma policy-forward kernel (tscl_policy_step) vs the fp32 kernels / the oracle.
 
 The tensor-core path multiplies bf16-rounded operands with fp32 accumulation, so
   * raw gate accumulators are compared with a torch matmul of the SAME bf16-rounded operands
@@ -76,7 +76,7 @@ def _check_v1(m, obs, zdbg, z_ref, Xb, Wx):
         z1 = torch.zeros_like(zdbg)
         _run_tc(m, obs, False, z1, 1)
         err1 = float((z1 - z_ref).abs().max())
-        raise AssertionError("tcgen05 gate GEMM mismatch: max err %.4f (LBO/SBO swapped: %.4f)" % (err0, err1))
+        raise AssertionError("wgmma gate GEMM mismatch: max err %.4f (LBO/SBO swapped: %.4f)" % (err0, err1))
     torch.testing.assert_close(zdbg, z_ref, rtol=1e-3, atol=2e-3)
     # done flag zeroes h and c inside the cell (agents/utils.py:104-105)
     _run_tc(m, obs, True, zdbg, 0)
@@ -178,7 +178,7 @@ def test_update_from_stored_activations_matches_recompute():
 
 
 def test_bptt_tensor_core_kernel_matches_fp32_kernel():
-    """tscl_lstm_seq_bwd_tc (tcgen05 dz.Wh^T, bf16 operands) vs tscl_lstm_seq_bwd (fp32 SIMT) on the same inputs."""
+    """tscl_lstm_seq_bwd_tc (wgmma dz.Wh^T, bf16 operands) vs tscl_lstm_seq_bwd (fp32 SIMT) on the same inputs."""
     from deeprl_signal_control_b200 import _lib
     from deeprl_signal_control_b200.agents.learner import BatchedA2C, _p
     lay = _layout(64)
@@ -223,7 +223,7 @@ def test_bptt_tensor_core_kernel_matches_fp32_kernel():
 
 @pytest.mark.parametrize("ff,use_bf16_x", [(64, True), (0, False), ("monaco", True)])
 def test_fc_weight_gradients_tensor_core_kernel(ff, use_bf16_x):
-    """tscl_fc_bwd_tc (tcgen05, MN-major bf16 operands, reduction over rows) vs
+    """tscl_fc_bwd_tc (wgmma, MN-major bf16 operands, reduction over rows) vs
       * a float64 contraction of the SAME bf16-rounded operands (rtol 2e-3: only summation order differs), and
       * tscl_fc_bwd (fp32 SIMT kernel) within the bf16 operand rounding."""
     from deeprl_signal_control_b200 import _lib
@@ -277,7 +277,7 @@ def test_fc_weight_gradients_tensor_core_kernel(ff, use_bf16_x):
     if worst > 2e-3:                               # diagnose a descriptor-stride mix-up in one GPU run
         G3 = torch.zeros_like(m.G)
         run(1, G3)
-        raise AssertionError("tcgen05 MN-major fc_bwd mismatch: worst rel err %.4f (LBO/SBO swapped: rel-L2 vs fp32 %.4f)"
+        raise AssertionError("wgmma MN-major fc_bwd mismatch: worst rel err %.4f (LBO/SBO swapped: rel-L2 vs fp32 %.4f)"
                              % (worst, float((G3 - G1).norm() / G1.norm())))
     # untouched parameter ranges stay zero, and the fp32 kernel agrees within bf16 operand rounding
     for k in g1:
@@ -289,7 +289,7 @@ def test_fc_weight_gradients_tensor_core_kernel(ff, use_bf16_x):
 
 @pytest.mark.parametrize("ff,from_store", [(64, True), (0, False), ("monaco", True)])
 def test_lstm_weight_gradients_tensor_core_kernel(ff, from_store):
-    """tscl_wgrad_tc: dWx = X^T dZ, dWh = Hp^T dZ, dbl = 1^T dZ (tcgen05, MN-major bf16 operands) vs a float64
+    """tscl_wgrad_tc: dWx = X^T dZ, dWh = Hp^T dZ, dbl = 1^T dZ (wgmma, MN-major bf16 operands) vs a float64
     contraction of the same bf16-rounded operands (rtol 2e-3); Hp rebuilt from the bf16 store with the done mask."""
     from deeprl_signal_control_b200 import _lib
     from deeprl_signal_control_b200.agents.learner import BatchedA2C, _p
@@ -334,7 +334,7 @@ def test_lstm_weight_gradients_tensor_core_kernel(ff, from_store):
         G3 = torch.zeros_like(m.G)
         run(1, G3)
         e3 = float((lay.views(G3)["wx"].double() - wx_ref).abs().max() / wx_ref.abs().max())
-        raise AssertionError("tcgen05 wgrad mismatch: rel errs wx/wh/bl %s (LBO/SBO swapped: wx %.4f)" % (errs, e3))
+        raise AssertionError("wgmma wgrad mismatch: rel errs wx/wh/bl %s (LBO/SBO swapped: wx %.4f)" % (errs, e3))
     # nothing outside wx / wh / bl is touched
     for k, v in gv.items():
         if k not in ("wx", "wh", "bl"):
@@ -343,7 +343,7 @@ def test_lstm_weight_gradients_tensor_core_kernel(ff, from_store):
 
 @pytest.mark.parametrize("ff,M", [(64, 128 * 5 + 37), (0, 300), ("monaco", 4096 + 1), (64, 128 * 400 + 3)])
 def test_dx_kernel_matches_bf16_matmul(ff, M):
-    """tscl_dx_tc (dX = dZ . Wx^T, warp-specialised tcgen05 kernel) vs the same product of the bf16-rounded operands in
+    """tscl_dx_tc (dX = dZ . Wx^T, warp-specialised wgmma kernel) vs the same product of the bf16-rounded operands in
     fp32: products of bf16 values are exact in fp32, so only the summation order and the final bf16 rounding differ."""
     import ctypes as C
     from deeprl_signal_control_b200 import _lib
@@ -358,7 +358,7 @@ def test_dx_kernel_matches_bf16_matmul(ff, M):
     dX = torch.full((U, M, dx), float("nan"), device="cuda", dtype=torch.bfloat16)
     pad = torch.full((1024,), 7.0, device="cuda", dtype=torch.bfloat16)        # canary right behind the output
     st = C.c_void_p(torch.cuda.current_stream().cuda_stream)
-    for _ in range(2):          # second call: the persistent state (barriers, TMEM) is set up afresh every launch
+    for _ in range(2):          # second call: the persistent state (barriers, accumulator tiles) is set up afresh every launch
         _lib.check(_lib.lib().tscl_dx_tc(m._h, C.c_void_p(dZ.data_ptr()), C.c_void_p(m.Wxt.data_ptr()),
                                          C.c_void_p(dX.data_ptr()), C.c_int64(M), st))
     torch.cuda.synchronize()

@@ -172,7 +172,7 @@ def test_single_replica_and_observe_only():
 
 
 def test_many_waves_and_replica_ranges_bit_exact():
-    """R = 2304 replicas = several waves of resident CTAs (4 per SM x 148 SMs = 592): the oracle follows a SAMPLE of
+    """R = 2304 replicas = several waves of resident CTAs (a few per SM x 132 SMs on an H100): the oracle follows a SAMPLE of
     replicas spread over all waves (each replica is independent, so stepping the sample alone is the same computation),
     and the host-buffer range entry point (`tsc_step_host_range`, rep0 > 0) must agree with the device-resident step."""
     from deeprl_signal_control_b200.net.large_grid import build_large_grid

@@ -63,22 +63,20 @@ def test_mini_scenario_runs_in_the_oracle(tmp_path):
     assert m["arrived"] > 250 and bool(d[0])
 
 
-@pytest.mark.skipif(not os.path.exists("/root/reference/real_net/data/in/most.net.xml"), reason="needs the reference checkout")
 def test_monaco_from_files_equals_the_hand_wired_scenario(tmp_path):
-    """most.net.xml + the route file the reference's generator writes (real_net/data/build_file.py:output_flows) +
-    the reference's phase sets and neighbour lists -> the same tables as net/real_net.py's Monaco definition; the
-    tlLogic programs of the net file themselves yield an action set for each of the 28 agents as well."""
-    import types
+    """most.net.xml + the route file the reference's generator writes (real_net/data/build_file.py:output_flows(325),
+    both stored under tests/golden/monaco_sumo) + the reference's phase sets and neighbour lists -> the same tables as
+    net/real_net.py's Monaco definition; the tlLogic programs of the net file themselves yield an action set for each of
+    the 28 agents as well."""
+    import gzip
+    import shutil
     from deeprl_signal_control_b200.net import real_net as rn, sumo_ingest as ing
-    sys.path.insert(0, "/root/reference")
-    for name in ("traci", "sumolib"):
-        sys.modules.setdefault(name, types.ModuleType(name))
-    import importlib
-    bf = importlib.import_module("real_net.data.build_file")
-    rou = tmp_path / "most.rou.xml"
-    rou.write_text(bf.output_flows(325, seed=None))
-    net_file = "/root/reference/real_net/data/in/most.net.xml"
-    a = ing.load_sumo_scenario(net_file, str(rou), tls_phases={n: rn.PHASES[v[0]] for n, v in rn.NODES.items()},
+    gold = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "monaco_sumo")
+    net_file = str(tmp_path / "most.net.xml")
+    with gzip.open(os.path.join(gold, "most.net.xml.gz"), "rb") as fi, open(net_file, "wb") as fo:
+        shutil.copyfileobj(fi, fo)
+    rou = os.path.join(gold, "most.rou.xml")
+    a = ing.load_sumo_scenario(net_file, rou, tls_phases={n: rn.PHASES[v[0]] for n, v in rn.NODES.items()},
                                neighbor_map={k: list(v[1]) for k, v in rn.NODES.items()}, agent="ma2c")
     b = rn.real_net_tables("ma2c")
     # routes (hence lane / link numbering) come in file order there and in FLOWS order here: compare by NAME
