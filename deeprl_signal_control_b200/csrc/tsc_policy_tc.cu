@@ -149,6 +149,32 @@ __device__ __forceinline__ void wg_mma(float* tile, int col0, int N, int KS, boo
   if (c + 32 <= N) { wg_mma_chunk<32, TA, TB>(tile, col0, c, KS, accum, descs); c += 32; }
   if (c + 16 <= N) wg_mma_chunk<16, TA, TB>(tile, col0, c, KS, accum, descs);
 }
+// Register-accumulator form, for products that accumulate over many tiles: issues the KS k-steps of one NC-column slab
+// of this warpgroup into the fragment `dd` (accum: add to what it holds) without committing or waiting.  descs(ks, da, db)
+// gives the descriptors of this warpgroup's 64-row A slab and of the B columns.  The caller brackets a batch of these
+// with wg_fence() and wg_commit(), and reads dd only after wg_wait<0>() (fragment layout: row 16 (warp & 3) + lane / 4
+// (+ 8 for dd[4i + 2], dd[4i + 3]), column 8 i + 2 (lane & 3) (+ 1 for the odd entries)).
+template <int NC, int TA, int TB, class F>
+__device__ __forceinline__ void wg_mma_regs(float (&dd)[NC / 2], int KS, bool accum, const F& descs) {
+  for (int ks = 0; ks < KS; ++ks) {
+    uint64_t da, db;
+    descs(ks, da, db);
+    const uint32_t acc = (accum || ks > 0) ? 1u : 0u;
+    if constexpr (NC == 64) wgmma_n64<TA, TB>(dd, da, db, acc);
+    else if constexpr (NC == 32) wgmma_n32<TA, TB>(dd, da, db, acc);
+    else wgmma_n16<TA, TB>(dd, da, db, acc);
+  }
+}
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accesses of a fragment across a wg_wait (the asm of the wgmma only names it at issue)
+template <int NR>
+__device__ __forceinline__ void wg_frag_fence(float (&dd)[NR]) {
+#pragma unroll
+  for (int i = 0; i < NR; ++i) asm volatile("" : "+f"(dd[i])::"memory");
+}
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
@@ -1677,18 +1703,20 @@ extern "C" int tscl_lstm_seq_bwd_tc_dx(tscl_handle* h, const void* wt_bf16, floa
 //   dW[k][c] = sum_m In[m][k] * dXm[m][c],   dXm = dX * (X > 0),   m = (t, replica) rows of one chunk
 // is a GEMM whose reduction index is the ROW index, so both operands are staged MN-major: the row-major global
 // data lands as [col/8][128 rows][8 cols] bf16 without a transposition, and
-//   D[dX column (two M = 128 halves)][64 input slots] += A^T B      (wgmma, A and B MN-major, K = 128 rows)
-// accumulates in the accumulator tile over all tiles of a unit.  A spare input slot holds 1.0: its D column is the bias gradient.
-// Persistent: CTA b owns the tile range [b NT / grid, (b + 1) NT / grid) of the (unit, tile) list and flushes its
-// accumulator with atomics whenever the unit changes (<= 3 flushes per CTA).
+//   D[dX column (four 64-column slabs)][64 input slots] += A^T B      (wgmma, A and B MN-major, K = 128 rows)
+// Two warpgroups: warpgroup g owns slabs g and g + 2 and keeps their m64n64 fp32 fragments in registers (64 per thread;
+// at 256 threads a thread may use 255) over all tiles of a unit.  A spare input slot holds 1.0: its D column is the bias
+// gradient.  Persistent: CTA b owns the tile range [b NT / grid, (b + 1) NT / grid) of the (unit, tile) list and adds its
+// fragments to G with atomics whenever the unit changes (<= 3 flushes per CTA).  Two smem stages: the first half of tile
+// j + 1 is loaded into registers while the MMAs of tile j run.
 #define FBT_ROWS 128
 #define FBT_SBO 2064                       // chunk stride: 128 rows * 16 B + 16 B pad (conflict-free transposing stores)
 #define FBT_A_BYTES (32 * FBT_SBO)
 #define FBT_B_BYTES (8 * FBT_SBO)
 #define FBT_STAGE (FBT_A_BYTES + FBT_B_BYTES)
-#define FBT_THREADS 512
+#define FBT_THREADS 512                    // the weight-gradient kernels below
+#define FBB_THREADS 256                    // fc_bwd_tc_kernel
 struct FcBwdTC {
-  float* acc;                // accumulator tiles, one [128][ACC_COLS] fp32 tile per CTA (acc_tiles)
   const float* obs;            // rows as tscl_fc_embed
   const float* X;              // [2A][M][dx] fp32 activations, or
   const __nv_bfloat16* Xb;     // [2A][M][dx] bf16 activations (one chunk of the activation store)
@@ -1699,51 +1727,48 @@ struct FcBwdTC {
   int variant;                 // 1: LBO/SBO swapped (descriptor diagnosis)
 };
 
-__global__ void __launch_bounds__(FBT_THREADS, 1)
+__global__ void __launch_bounds__(FBB_THREADS, 1)
 fc_bwd_tc_kernel(const DDimsTC d, const FcBwdTC a) {
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  uint64_t* sBar = reinterpret_cast<uint64_t*>(tc_smem + 2 * FBT_STAGE);
-  const uint32_t bar0 = smem_u32(sBar);
-  if (tid == 0) {
-    mbar_init(bar0, 1); mbar_init(bar0 + 8, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
-  float* const acc = a.acc + (size_t)blockIdx.x * TC_M * ACC_COLS;
-  // bf16 x bf16 -> f32, A and B MN-major, N = 64, M = 128
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
+  // bf16 x bf16 -> f32, A and B MN-major, N = 64, M = 64 per slab
   const uint32_t lbo = a.variant ? FBT_SBO : 128, sbo = a.variant ? 128 : FBT_SBO;
   const int dx = d.dx, ng = dx >> 3, n_items = FBT_ROWS * ng;
   const uint32_t ng_magic = (1u << 20) / (uint32_t)ng + 1u;      // i / ng == (i * magic) >> 20 for i < 4096, ng <= 32
   const int64_t tpu = (a.M + FBT_ROWS - 1) / FBT_ROWS;
   const int64_t NT = tpu * 2 * d.A;
   const int64_t j0 = NT * blockIdx.x / gridDim.x, j1 = NT * (blockIdx.x + 1) / gridDim.x;
-  uint32_t ph0 = 0, ph1 = 0;
-  bool pend0 = false, pend1 = false, first = true;
+  float f0[32], f1[32];                        // slabs wg and wg + 2
+  bool first = true;
   int cur_u = -1, nw = 0, nt = 0, nf = 0, ooff = 0;
   int src[8];                                  // observation index of each of this thread's 8 input slots (-1 none, -2 one)
   const int bc = tid & 7;                      // this thread's B chunk (8 input slots)
 
-  auto flush = [&](int u) {
-    if (pend0) { mbar_wait(bar0, ph0); ph0 ^= 1; pend0 = false; }
-    if (pend1) { mbar_wait(bar0 + 8, ph1); ph1 ^= 1; pend1 = false; }
-    const int q = warp & 3, cgp = warp >> 2, mh = cgp >> 1, k0 = (cgp & 1) * 32;
-    const int c = mh * 128 + q * 32 + lane;
-    float v[32];
-    const uint32_t tb = ((uint32_t)(q * 32) << 16) + (uint32_t)(mh * 64 + k0);
-    acc_ld16(acc, tb, v); acc_ld16(acc, tb + 16, v + 16);
-    if (c < dx) {
-      int64_t wo, bo; int ld, cc, s0, n;
-      if (c < d.fw) { wo = d.off_fcw_w[u]; bo = d.off_fcw_b[u]; ld = d.fw; cc = c; s0 = 0; n = nw; }
-      else if (c < d.fw + d.ff) { wo = d.off_fcf_w[u]; bo = d.off_fcf_b[u]; ld = d.ff; cc = c - d.fw; s0 = d.kw; n = nf; }
-      else { wo = d.off_fct_w[u]; bo = d.off_fct_b[u]; ld = d.ft; cc = c - d.fw - d.ff; s0 = d.kw + TC_KF; n = nt; }
+  // a fragment into G: dX column c = 64 sl + 16 (warp & 3) + lane / 4 (+ 8), input slot 8 i + 2 (lane & 3) (+ 1).
+  // Columns past dx come from A chunks that are never staged: they are dropped here.
+  auto flush_slab = [&](const float (&f)[32], int sl, int u) {
 #pragma unroll
-      for (int e = 0; e < 32; ++e) {
-        const int slot = k0 + e, kin = slot - s0;
-        if (kin >= 0 && kin < n) atomicAdd(&a.G[wo + (int64_t)kin * ld + cc], v[e]);
-        if (slot == d.ones_slot) atomicAdd(&a.G[bo + cc], v[e]);
+    for (int hh = 0; hh < 2; ++hh) {
+      const int c = sl * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * hh;
+      if (c < dx) {
+        int64_t wo, bo; int ld, cc, s0, n;
+        if (c < d.fw) { wo = d.off_fcw_w[u]; bo = d.off_fcw_b[u]; ld = d.fw; cc = c; s0 = 0; n = nw; }
+        else if (c < d.fw + d.ff) { wo = d.off_fcf_w[u]; bo = d.off_fcf_b[u]; ld = d.ff; cc = c - d.fw; s0 = d.kw; n = nf; }
+        else { wo = d.off_fct_w[u]; bo = d.off_fct_b[u]; ld = d.ft; cc = c - d.fw - d.ff; s0 = d.kw + TC_KF; n = nt; }
+#pragma unroll
+        for (int e = 0; e < 16; ++e) {
+          const int slot = 8 * (e >> 1) + 2 * (lane & 3) + (e & 1), kin = slot - s0;
+          const float v = f[4 * (e >> 1) + 2 * hh + (e & 1)];
+          if (kin >= 0 && kin < n) atomicAdd(&a.G[wo + (int64_t)kin * ld + cc], v);
+          if (slot == d.ones_slot) atomicAdd(&a.G[bo + cc], v);
+        }
       }
     }
-    __syncthreads();
+  };
+  auto flush = [&](int u) {
+    wg_wait<0>();
+    wg_frag_fence(f0); wg_frag_fence(f1);
+    flush_slab(f0, wg, u);
+    flush_slab(f1, wg + 2, u);
   };
 
   for (int64_t j = j0; j < j1; ++j) {
@@ -1766,9 +1791,6 @@ fc_bwd_tc_kernel(const DDimsTC d, const FcBwdTC a) {
         src[e] = sidx;
       }
     }
-    // the MMAs that read stage s two tiles ago must have drained it
-    if (s == 0) { if (pend0) { mbar_wait(bar0, ph0); ph0 ^= 1; pend0 = false; } }
-    else { if (pend1) { mbar_wait(bar0 + 8, ph1); ph1 ^= 1; pend1 = false; } }
     unsigned char* sA = tc_smem + (size_t)s * FBT_STAGE;
     unsigned char* sB = sA + FBT_A_BYTES;
     const int rows_valid = (a.M - m0) < FBT_ROWS ? (int)(a.M - m0) : FBT_ROWS;
@@ -1782,14 +1804,14 @@ fc_bwd_tc_kernel(const DDimsTC d, const FcBwdTC a) {
       const int64_t nbytes = (int64_t)rvn * dx * 4;
       if (a.dXb) {
         const char* pd = reinterpret_cast<const char*>(a.dXb + basen);
-        for (int64_t o = (int64_t)tid * 128; o < nbytes / 2; o += FBT_THREADS * 128) asm volatile("prefetch.global.L2 [%0];" ::"l"(pd + o));
+        for (int64_t o = (int64_t)tid * 128; o < nbytes / 2; o += FBB_THREADS * 128) asm volatile("prefetch.global.L2 [%0];" ::"l"(pd + o));
       } else {
         const char* pd = reinterpret_cast<const char*>(a.dX + basen);
-        for (int64_t o = (int64_t)tid * 128; o < nbytes; o += FBT_THREADS * 128) asm volatile("prefetch.global.L2 [%0];" ::"l"(pd + o));
+        for (int64_t o = (int64_t)tid * 128; o < nbytes; o += FBB_THREADS * 128) asm volatile("prefetch.global.L2 [%0];" ::"l"(pd + o));
       }
       if (a.Xb) {
         const char* px = reinterpret_cast<const char*>(a.Xb + basen);
-        for (int64_t o = (int64_t)tid * 128; o < nbytes / 2; o += FBT_THREADS * 128) asm volatile("prefetch.global.L2 [%0];" ::"l"(px + o));
+        for (int64_t o = (int64_t)tid * 128; o < nbytes / 2; o += FBB_THREADS * 128) asm volatile("prefetch.global.L2 [%0];" ::"l"(px + o));
       }
       if (tid < rvn) {
         const int64_t m = m0n + tid;
@@ -1799,43 +1821,47 @@ fc_bwd_tc_kernel(const DDimsTC d, const FcBwdTC a) {
       }
     }
     // ---- B loads first (observation slice of this thread's 8 input slots, 2 rows): their latency overlaps the A staging ----
-    float ov[(FBT_ROWS * 8) / FBT_THREADS][8];
+    uint4 ov[(FBT_ROWS * 8) / FBB_THREADS];      // 8 bf16 each
     {
       const int64_t tq = m0 / a.rows_per_t, rem0 = m0 - tq * a.rows_per_t;      // one division per tile
 #pragma unroll
-      for (int r = 0; r < (FBT_ROWS * 8) / FBT_THREADS; ++r) {
-        const int row = (r * FBT_THREADS + tid) >> 3;
+      for (int r = 0; r < (FBT_ROWS * 8) / FBB_THREADS; ++r) {
+        const int row = (r * FBB_THREADS + tid) >> 3;
+        ov[r] = make_uint4(0, 0, 0, 0);
         if (row < rows_valid) {
           int64_t tt = tq, rem = rem0 + row;
           while (rem >= a.rows_per_t) { rem -= a.rows_per_t; ++tt; }
           const float* op = a.obs + tt * a.stride_t + rem * d.n_obs + ooff;
+          __align__(16) __nv_bfloat16 o[8];
 #pragma unroll
-          for (int e = 0; e < 8; ++e) ov[r][e] = src[e] >= 0 ? __ldg(op + src[e]) : (src[e] == -2 ? 1.0f : 0.f);
-        } else {
-#pragma unroll
-          for (int e = 0; e < 8; ++e) ov[r][e] = 0.f;
+          for (int e = 0; e < 8; ++e) o[e] = __float2bfloat16_rn(src[e] >= 0 ? __ldg(op + src[e]) : (src[e] == -2 ? 1.0f : 0.f));
+          ov[r] = *reinterpret_cast<const uint4*>(o);
         }
       }
     }
-    if (a.dXb && a.Xb) {
-      // ---- A, bf16 in / bf16 out: all loads of the tile in flight at once, relu mask as packed 16-bit integer ops ----
-      uint4 gb[8], xm[8];
+    // ---- A, bf16 in / bf16 out: the loads of half a tile in flight at once, relu mask as packed 16-bit integer ops.
+    //      The first half is loaded before the barrier that frees this stage ----
+    const bool all_bf16 = a.dXb && a.Xb;
+    uint4 gb[8], xm[8];
+    auto load_half = [&](int h) {
 #pragma unroll
       for (int k = 0; k < 8; ++k) {
-        const int i = k * FBT_THREADS + tid;
+        const int i = (8 * h + k) * FBB_THREADS + tid;
         gb[k] = make_uint4(0, 0, 0, 0); xm[k] = make_uint4(0, 0, 0, 0);
         if (i < items_valid) {
           gb[k] = __ldg(reinterpret_cast<const uint4*>(a.dXb + base) + i);
           xm[k] = __ldg(reinterpret_cast<const uint4*>(a.Xb + base) + i);
         }
       }
+    };
+    auto store_half = [&](int h) {
       auto keep2 = [](uint32_t x) -> uint32_t {      // 0xFFFF per 16-bit half where the bf16 value is > 0
         const uint32_t nz = ((x & 0x7FFF7FFFu) + 0x7FFF7FFFu) & ~x & 0x80008000u;
         return (nz >> 15) * 0xFFFFu;
       };
 #pragma unroll
       for (int k = 0; k < 8; ++k) {
-        const int i = k * FBT_THREADS + tid;
+        const int i = (8 * h + k) * FBB_THREADS + tid;
         if (i < n_items) {
           const uint4 o = make_uint4(gb[k].x & keep2(xm[k].x), gb[k].y & keep2(xm[k].y), gb[k].z & keep2(xm[k].z),
                                      gb[k].w & keep2(xm[k].w));
@@ -1843,15 +1869,21 @@ fc_bwd_tc_kernel(const DDimsTC d, const FcBwdTC a) {
           *reinterpret_cast<uint4*>(sA + (size_t)cg * FBT_SBO + row * 16) = o;
         }
       }
+    };
+    if (all_bf16) load_half(0);
+    __syncthreads();      // every warpgroup has waited for its MMAs of tile j - 1: stage s is free
+    if (all_bf16) {
+      store_half(0);
+      if (n_items > 8 * FBB_THREADS) { load_half(1); store_half(1); }
     } else {
       // ---- A: masked dX, 8 columns (one 16 B chunk row) per item; items are contiguous in global memory ----
-      for (int ib = 0; ib < n_items; ib += 4 * FBT_THREADS) {
-        float4 g0[4], g1[4];
-        uint4 xb[4];
-        float4 x0[4], x1[4];
+      for (int ib = 0; ib < n_items; ib += 2 * FBB_THREADS) {
+        float4 g0[2], g1[2];
+        uint4 xb[2];
+        float4 x0[2], x1[2];
   #pragma unroll
-        for (int r = 0; r < 4; ++r) {
-          const int i = ib + r * FBT_THREADS + tid;
+        for (int r = 0; r < 2; ++r) {
+          const int i = ib + r * FBB_THREADS + tid;
           g0[r] = g1[r] = make_float4(0.f, 0.f, 0.f, 0.f);
           xb[r] = make_uint4(0, 0, 0, 0);
           x0[r] = x1[r] = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -1874,8 +1906,8 @@ fc_bwd_tc_kernel(const DDimsTC d, const FcBwdTC a) {
           }
         }
   #pragma unroll
-        for (int r = 0; r < 4; ++r) {
-          const int i = ib + r * FBT_THREADS + tid;
+        for (int r = 0; r < 2; ++r) {
+          const int i = ib + r * FBB_THREADS + tid;
           if (i < n_items) {
             const float gv[8] = {g0[r].x, g0[r].y, g0[r].z, g0[r].w, g1[r].x, g1[r].y, g1[r].z, g1[r].w};
             bool pos[8];
@@ -1903,25 +1935,27 @@ fc_bwd_tc_kernel(const DDimsTC d, const FcBwdTC a) {
     }
     // ---- B: the unit's observation slice scattered into the 64 input slots ----
 #pragma unroll
-    for (int r = 0; r < (FBT_ROWS * 8) / FBT_THREADS; ++r) {
-      const int row = (r * FBT_THREADS + tid) >> 3;
-      __align__(16) __nv_bfloat16 o[8];
-#pragma unroll
-      for (int e = 0; e < 8; ++e) o[e] = __float2bfloat16_rn(ov[r][e]);
-      *reinterpret_cast<uint4*>(sB + (size_t)bc * FBT_SBO + row * 16) = *reinterpret_cast<const uint4*>(o);
+    for (int r = 0; r < (FBT_ROWS * 8) / FBB_THREADS; ++r) {
+      const int row = (r * FBB_THREADS + tid) >> 3;
+      *reinterpret_cast<uint4*>(sB + (size_t)bc * FBT_SBO + row * 16) = ov[r];
     }
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     __syncthreads();
-    if (warp < 8) {
-      const uint32_t aA = smem_u32(sA), aB = smem_u32(sB);
-      for (int mh = 0; mh < 2; ++mh)
-        wg_mma<1, 1>(acc, mh * 64, 64, FBT_ROWS / 16, !first, [&](int ks, uint64_t& da, uint64_t& db) {
-          da = make_desc(aA + mh * 16 * FBT_SBO + ks * 256, lbo, sbo);
-          db = make_desc(aB + ks * 256, lbo, sbo);
-        });
-      wg_mma_done(bar0 + 8 * s);
-    }
-    if (s == 0) pend0 = true; else pend1 = true;
+    // both slabs of each warpgroup are multiplied whatever dx is: rows past dx are never flushed
+    const uint32_t aA = smem_u32(sA), aB = smem_u32(sB);
+    wg_fence();
+    wg_mma_regs<64, 1, 1>(f0, FBT_ROWS / 16, !first, [&](int ks, uint64_t& da, uint64_t& db) {
+      da = make_desc(aA + wg * 8 * FBT_SBO + ks * 256, lbo, sbo);
+      db = make_desc(aB + ks * 256, lbo, sbo);
+    });
+    wg_mma_regs<64, 1, 1>(f1, FBT_ROWS / 16, !first, [&](int ks, uint64_t& da, uint64_t& db) {
+      da = make_desc(aA + (wg + 2) * 8 * FBT_SBO + ks * 256, lbo, sbo);
+      db = make_desc(aB + ks * 256, lbo, sbo);
+    });
+    wg_commit();
+    // wait_group 0, not 1: with a group still in flight across the staging code below (divergent per thread), ptxas
+    // serialises the wgmma of this kernel.  The MMAs of a tile are short next to its staging.
+    wg_wait<0>();
     first = false;
   }
   if (cur_u >= 0) flush(cur_u);
@@ -1935,7 +1969,7 @@ extern "C" int tscl_fc_bwd_tc(tscl_handle* h, const float* obs, const float* X, 
   const DDimsTC& d = *tscl_dims_of(h);
   if ((d.dx % 8) != 0 || d.dx > 256) return tsc_set_error("tscl_fc_bwd_tc: dx must be a multiple of 8, <= 256");
   if (d.kw == 0 || d.ones_slot < 0) return tsc_set_error("tscl_fc_bwd_tc: no free input slot for the bias column (use tscl_fc_bwd)");
-  const size_t smem = 2 * FBT_STAGE + 32;
+  const size_t smem = 2 * FBT_STAGE;
   static int attr_dev = -1;
   if (attr_dev != tscl_device_of(h)) {
     PCK(cudaFuncSetAttribute(fc_bwd_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -1946,12 +1980,10 @@ extern "C" int tscl_fc_bwd_tc(tscl_handle* h, const float* obs, const float* X, 
   const int64_t NT = ((M + FBT_ROWS - 1) / FBT_ROWS) * 2 * d.A;
   const int grid = (int)(NT < n_sm ? NT : n_sm);
   FcBwdTC a;
-  a.acc = acc_tiles(h, stream);
-  if (!a.acc) return tsc_set_error("accumulator tiles: cudaMalloc failed");
   a.obs = obs; a.X = X; a.Xb = (const __nv_bfloat16*)x_bf16; a.dX = dX; a.dXb = (const __nv_bfloat16*)dx_bf16; a.G = grads; a.M = M;
   a.rows_per_t = rows_per_t;
   a.stride_t = stride_t; a.variant = variant;
-  fc_bwd_tc_kernel<<<grid, FBT_THREADS, smem, (cudaStream_t)stream>>>(d, a);
+  fc_bwd_tc_kernel<<<grid, FBB_THREADS, smem, (cudaStream_t)stream>>>(d, a);
   PCK(cudaGetLastError());
   return 0;
 }
@@ -2170,110 +2202,94 @@ wgrad_tc_kernel(const DDimsTC d, const WGradTC a) {
   if (cur_pu >= 0) flush(cur_pu);
 }
 
-// All-bf16 variant (the training loop's): 64-row tiles, two smem stages + one register stage.  CTAs 2p and 2p+1 walk the
-// same (unit, tile) range, one per 128-column half of dZ, so the second reader of an X / Hp tile finds it in L2.
+// All-bf16 variant (the training loop's): 64-row tiles, two smem stages + one register stage, accumulators in registers.
+// The A columns [X | Hp | 1] (dx + 65 <= 320) form nsl 64-column slabs; CTA 5p + k (for nsl = 5) owns slab k of the
+// (unit, tile) range of group p, and its warpgroup q the gate columns 64 q .. 64 q + 63, so every warpgroup holds one
+// m64n64 fragment (32 registers per thread) for as long as the CTA stays on one unit.  The CTAs of a group walk the same
+// range, so the later readers of a dZ tile find it in L2.
 #define WGA_ROWS 64
 #define WGA_SBO (WGA_ROWS * 16 + 16)
-#define WGA_STAGE ((WG_A_CHUNKS + WG_Z_CHUNKS) * WGA_SBO)
+#define WGA_A_CHUNKS 8
+#define WGA_STAGE ((WGA_A_CHUNKS + 32) * WGA_SBO)
 #define WGA_STAGES 2
 #define WGA_MAXT 256
+__host__ __device__ inline int wga_slabs(int dx) { return (dx + TC_H + 1 + 63) >> 6; }
 __global__ void __launch_bounds__(FBT_THREADS, 1)
 wgrad_tc_async_kernel(const DDimsTC d, const WGradTC a) {
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  uint64_t* sBar = reinterpret_cast<uint64_t*>(tc_smem + WGA_STAGES * WGA_STAGE);
-  float* sDone = reinterpret_cast<float*>(sBar + WGA_STAGES + 1);
-  const uint32_t bar0 = smem_u32(sBar);
-  if (tid == 0) {
-    for (int i = 0; i < WGA_STAGES; ++i) mbar_init(bar0 + 8 * i, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  // never-written A chunks are read by the last M block: keep them finite
-  for (int i = tid; i < WGA_STAGES * WGA_STAGE / 16; i += FBT_THREADS) reinterpret_cast<uint4*>(tc_smem)[i] = make_uint4(0, 0, 0, 0);
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wq = warp >> 2;
+  float* sDone = reinterpret_cast<float*>(tc_smem + WGA_STAGES * WGA_STAGE);
   for (int i = tid; i < a.T; i += FBT_THREADS) sDone[i] = a.done[i];
   __syncthreads();
-  float* const acc = a.acc + (size_t)blockIdx.x * TC_M * ACC_COLS;
   const uint32_t lbo = a.variant ? WGA_SBO : 128, sbo = a.variant ? 128 : WGA_SBO;
-  const int dx = d.dx, ng = dx >> 3, n_xitems = WGA_ROWS * ng;
-  const uint32_t ng_magic = (1u << 20) / (uint32_t)ng + 1u;      // i / ng == (i * magic) >> 20 for i < 4096, ng <= 32
-  const int nb = (dx + TC_H + 1 + 127) >> 7;        // M blocks
+  const int dx = d.dx, ng = dx >> 3;
+  const int nsl = wga_slabs(dx);
   const int64_t tpu = (a.M + WGA_ROWS - 1) / WGA_ROWS;
   const int64_t NT = tpu * 2 * d.A;
-  const int npairs = gridDim.x >> 1, pb = blockIdx.x >> 1, nh = blockIdx.x & 1;
-  const int64_t j0 = NT * pb / npairs, j1 = NT * (pb + 1) / npairs;
-  uint32_t pend = 0, phase = 0;                      // bit s: a commit is outstanding on / the wait parity of stage s
+  const int ngrp = gridDim.x / nsl, pb = blockIdx.x / nsl, sl = blockIdx.x - pb * nsl;
+  const int64_t j0 = NT * pb / ngrp, j1 = NT * (pb + 1) / ngrp;
+  // this thread's A piece: 8 columns (chunk cg of [X | Hp | 1 | 0]) of one row
+  const int arow = tid >> 3, cg = sl * 8 + (tid & 7);
+  float f[32];
   bool first = true;
   int cur_u = -1;
-  auto wait_stage = [&](int s) {
-    if (pend & (1u << s)) { mbar_wait(bar0 + 8 * s, (phase >> s) & 1u); phase ^= 1u << s; pend &= ~(1u << s); }
-  };
+  // the fragment into G: A column sl * 64 + 16 (warp & 3) + lane / 4 (+ 8), gate column 64 wq + 8 i + 2 (lane & 3) (+ 1)
   auto flush = [&](int u) {
-    for (int s = 0; s < WGA_STAGES; ++s) wait_stage(s);
-    const int q = warp & 3, cq = warp >> 2;
-    const int g0 = nh * 128 + cq * 32;
-    for (int b = 0; b < nb; ++b) {
-      const int ci = b * 128 + q * 32 + lane;
-      float v[32];
-      const uint32_t tb = ((uint32_t)(q * 32) << 16) + (uint32_t)(b * 128 + cq * 32);
-      acc_ld16(acc, tb, v); acc_ld16(acc, tb + 16, v + 16);
-      float* dst = nullptr;
-      if (ci < dx) dst = a.G + d.off_wx + ((int64_t)u * dx + ci) * TC_N + g0;
-      else if (ci < dx + TC_H) dst = a.G + d.off_wh + ((int64_t)u * TC_H + (ci - dx)) * TC_N + g0;
-      else if (ci == dx + TC_H) dst = a.G + d.off_bl + (int64_t)u * TC_N + g0;
-      if (dst) {
+    wg_wait<0>();
+    wg_frag_fence(f);
 #pragma unroll
-        for (int e = 0; e < 32; ++e) atomicAdd(dst + e, v[e]);
+    for (int hh = 0; hh < 2; ++hh) {
+      const int ci = sl * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * hh;
+      float* dst = nullptr;
+      if (ci < dx) dst = a.G + d.off_wx + ((int64_t)u * dx + ci) * TC_N;
+      else if (ci < dx + TC_H) dst = a.G + d.off_wh + ((int64_t)u * TC_H + (ci - dx)) * TC_N;
+      else if (ci == dx + TC_H) dst = a.G + d.off_bl + (int64_t)u * TC_N;
+      if (dst) {
+        dst += wq * 64 + 2 * (lane & 3);
+#pragma unroll
+        for (int i = 0; i < 8; ++i) { atomicAdd(dst + 8 * i, f[4 * i + 2 * hh]); atomicAdd(dst + 8 * i + 1, f[4 * i + 2 * hh + 1]); }
       }
     }
-    __syncthreads();
   };
 
-  // running position of the NEXT tile to issue: unit, first row, and (t, row within t) of that row
+  // running position of the NEXT tile to load: unit, first row, and (t, row within t) of that row
   int iu = (int)(j0 / tpu);
   int64_t im0 = (j0 - (int64_t)iu * tpu) * WGA_ROWS;
   int64_t it_t = im0 / a.rc, it_rem = im0 - it_t * a.rc;
-  // Register-staged pipeline: the 7 pieces (16 B each: 2 of dZ, <= 4 of X, 1 of Hp) of tile j + 2 are loaded into
-  // registers while tile j is multiplied and tile j + 1 sits in the other smem stage; they are stored one iteration
-  // later, when their latency has passed.  (cp.async is slower here: LDGSTS keeps its address registers
-  // reserved until the copy completes, and the allocator's reuse of them stalls the warp for a memory latency.)
-  uint4 pv[7];
-  int prv = 0;                                   // rows_valid of the tile held in pv
+  // Register-staged pipeline: the 5 pieces (16 B each: 4 of dZ, 1 of A) of tile j + 2 are loaded into registers while
+  // tile j is multiplied and tile j + 1 sits in the other smem stage; they are stored one iteration later, when their
+  // latency has passed.  (cp.async is slower here: LDGSTS keeps its address registers reserved until the copy
+  // completes, and the allocator's reuse of them stalls the warp for a memory latency.)
+  uint4 pv[5];
   auto load_tile = [&]() {
     const int u = iu;
     const int64_t m0 = im0;
     const int rows_valid = (a.M - m0) < WGA_ROWS ? (int)(a.M - m0) : WGA_ROWS;
     const int64_t rowbase = (int64_t)u * a.M + m0;
-    prv = rows_valid;
-#pragma unroll
-    for (int r = 0; r < 2; ++r) {
-      const int i = r * FBT_THREADS + tid, row = i >> 4, g = i & 15;
-      pv[r] = make_uint4(0, 0, 0, 0);
-      if (row < rows_valid) pv[r] = __ldg(reinterpret_cast<const uint4*>(a.dZb + (rowbase + row) * TC_N + nh * 128 + g * 8));
-    }
-    const uint4* xsrc = reinterpret_cast<const uint4*>(a.Xb + rowbase * dx);
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
-      const int i = k * FBT_THREADS + tid;
-      pv[2 + k] = make_uint4(0, 0, 0, 0);
-      if (i < rows_valid * ng) pv[2 + k] = __ldg(xsrc + i);
+      const int i = k * FBT_THREADS + tid, row = i >> 5, g = i & 31;
+      pv[k] = make_uint4(0, 0, 0, 0);
+      if (row < rows_valid) pv[k] = __ldg(reinterpret_cast<const uint4*>(a.dZb + (rowbase + row) * TC_N + g * 8));
     }
-    {
-      const int hrow = tid >> 3, hc = tid & 7;
-      pv[6] = make_uint4(0, 0, 0, 0);
-      if (hrow < rows_valid) {
-        int64_t t = it_t, rem = it_rem + hrow;
+    pv[4] = make_uint4(0, 0, 0, 0);
+    if (arow < rows_valid) {
+      if (cg < ng) pv[4] = __ldg(reinterpret_cast<const uint4*>(a.Xb + (rowbase + arow) * dx) + cg);
+      else if (cg < ng + 8) {
+        const int hc = cg - ng;
+        int64_t t = it_t, rem = it_rem + arow;
         while (rem >= a.rc) { rem -= a.rc; ++t; }
         if (sDone[t] == 0.f) {
-          if (t > 0) pv[6] = __ldg(reinterpret_cast<const uint4*>(a.Hb + (rowbase + hrow - a.rc) * TC_H + hc * 8));
+          if (t > 0) pv[4] = __ldg(reinterpret_cast<const uint4*>(a.Hb + (rowbase + arow - a.rc) * TC_H + hc * 8));
           else {       // first step of the rollout: Hp = h0 (fp32 state)
             const float4* hp = reinterpret_cast<const float4*>(a.h0 + ((int64_t)u * a.ld_state + a.r0 + rem) * TC_H + hc * 8);
             const float4 p = __ldg(hp), qv = __ldg(hp + 1);
             __align__(16) __nv_bfloat16 tt[8] = {__float2bfloat16_rn(p.x), __float2bfloat16_rn(p.y), __float2bfloat16_rn(p.z),
                                                  __float2bfloat16_rn(p.w), __float2bfloat16_rn(qv.x), __float2bfloat16_rn(qv.y),
                                                  __float2bfloat16_rn(qv.z), __float2bfloat16_rn(qv.w)};
-            pv[6] = *reinterpret_cast<const uint4*>(tt);
+            pv[4] = *reinterpret_cast<const uint4*>(tt);
           }
         }
-      }
+      } else if (cg == ng + 8) pv[4].x = 0x3f80u;      // the ones column (bias gradient)
     }
     // advance the running position
     im0 += WGA_ROWS; it_rem += WGA_ROWS;
@@ -2282,23 +2298,13 @@ wgrad_tc_async_kernel(const DDimsTC d, const WGradTC a) {
   };
   auto store_tile = [&](int s) {
     unsigned char* sA = tc_smem + (size_t)s * WGA_STAGE;
-    unsigned char* sZ = sA + (size_t)WG_A_CHUNKS * WGA_SBO;
-#pragma unroll
-    for (int r = 0; r < 2; ++r) {
-      const int i = r * FBT_THREADS + tid, row = i >> 4, g = i & 15;
-      *reinterpret_cast<uint4*>(sZ + (size_t)g * WGA_SBO + row * 16) = pv[r];
-    }
+    unsigned char* sZ = sA + (size_t)WGA_A_CHUNKS * WGA_SBO;
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
       const int i = k * FBT_THREADS + tid;
-      if (i < n_xitems) {
-        const int row = (int)(((uint32_t)i * ng_magic) >> 20), cg = i - row * ng;
-        *reinterpret_cast<uint4*>(sA + (size_t)cg * WGA_SBO + row * 16) = pv[2 + k];
-      }
+      *reinterpret_cast<uint4*>(sZ + (size_t)(i & 31) * WGA_SBO + (i >> 5) * 16) = pv[k];
     }
-    *reinterpret_cast<uint4*>(sA + (size_t)(ng + (tid & 7)) * WGA_SBO + (tid >> 3) * 16) = pv[6];
-    if (tid < WGA_ROWS)
-      *reinterpret_cast<uint4*>(sA + (size_t)(ng + 8) * WGA_SBO + tid * 16) = make_uint4(tid < prv ? 0x3f80u : 0u, 0, 0, 0);
+    *reinterpret_cast<uint4*>(sA + (size_t)(tid & 7) * WGA_SBO + arow * 16) = pv[4];
   };
 
   if (j0 < j1) { load_tile(); store_tile(0); }
@@ -2312,19 +2318,17 @@ wgrad_tc_async_kernel(const DDimsTC d, const WGradTC a) {
     }
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     __syncthreads();
-    if (warp < 8) {
-      const uint32_t aA = smem_u32(tc_smem + (size_t)s * WGA_STAGE), aZ = aA + WG_A_CHUNKS * WGA_SBO;
-      for (int b = 0; b < nb; ++b)
-        wg_mma<1, 1>(acc, b * 128, 128, WGA_ROWS / 16, !first, [&](int ks, uint64_t& da, uint64_t& db) {
-          da = make_desc(aA + b * 16 * WGA_SBO + ks * 256, lbo, sbo);
-          db = make_desc(aZ + ks * 256, lbo, sbo);
-        });
-      wg_mma_done(bar0 + 8 * s);
-    }
-    pend |= 1u << s;
+    const uint32_t aA = smem_u32(tc_smem + (size_t)s * WGA_STAGE), aZ = aA + WGA_A_CHUNKS * WGA_SBO;
+    wg_fence();
+    wg_mma_regs<64, 1, 1>(f, WGA_ROWS / 16, !first, [&](int ks, uint64_t& da, uint64_t& db) {
+      da = make_desc(aA + ks * 256, lbo, sbo);
+      db = make_desc(aZ + wq * 8 * WGA_SBO + ks * 256, lbo, sbo);
+    });
+    wg_commit();
     first = false;
     if (j + 1 < j1) {
-      wait_stage(s ^ 1);            // MMAs of tile j - 1 (issued one iteration ago) have drained the other stage
+      wg_wait<1>();                 // this warpgroup's MMAs of tile j - 1 are done ...
+      __syncthreads();              // ... and every warpgroup's: the other stage is free
       store_tile(s ^ 1);            // tile j + 1, loaded one iteration ago
       if (j + 2 < j1) load_tile();
     }
@@ -2342,7 +2346,7 @@ extern "C" int tscl_wgrad_tc(tscl_handle* h, const float* dZ, const void* dz_bf1
   const DDimsTC& d = *tscl_dims_of(h);
   if ((d.dx % 8) != 0 || d.dx / 8 + 9 > WG_A_CHUNKS) return tsc_set_error("tscl_wgrad_tc: dx must be a multiple of 8, <= 240");
   const size_t smem = 2 * (size_t)WG_STAGE + 32;
-  const size_t smem_async = (size_t)WGA_STAGES * WGA_STAGE + 8 * WGA_STAGES + 8 + 4 * WGA_MAXT;
+  const size_t smem_async = (size_t)WGA_STAGES * WGA_STAGE + 4 * WGA_MAXT;
   static int attr_dev = -1;
   if (attr_dev != tscl_device_of(h)) {
     PCK(cudaFuncSetAttribute(wgrad_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -2355,17 +2359,20 @@ extern "C" int tscl_wgrad_tc(tscl_handle* h, const float* dZ, const void* dz_bf1
   const int64_t NT = ((M + FBT_ROWS - 1) / FBT_ROWS) * 4 * d.A;
   const int grid = (int)(NT < n_sm ? NT : n_sm);
   WGradTC a;
-  a.acc = acc_tiles(h, stream);
-  if (!a.acc) return tsc_set_error("accumulator tiles: cudaMalloc failed");
+  a.acc = nullptr;
   a.dZ = dZ; a.dZb = (const __nv_bfloat16*)dz_bf16; a.X = X; a.Xb = (const __nv_bfloat16*)x_bf16; a.Hp = Hp; a.Hb = (const __nv_bfloat16*)h_bf16; a.h0 = h0;
   a.done = done; a.G = grads; a.M = M; a.rc = rc; a.ld_state = ld_state; a.r0 = r0; a.T = T; a.variant = variant;
   if (a.dZb && a.Xb && a.Hb && T <= WGA_MAXT) {
     const int64_t nt2 = ((M + WGA_ROWS - 1) / WGA_ROWS) * 2 * d.A;
-    int g2 = (int)(nt2 < n_sm / 2 ? nt2 : n_sm / 2) * 2;      // CTA pairs
-    if (g2 < 2) g2 = 2;
+    const int nsl = wga_slabs(d.dx);
+    const int g2 = (int)(nt2 < n_sm / nsl ? nt2 : n_sm / nsl) * nsl;      // groups of nsl CTAs, one per A slab
     wgrad_tc_async_kernel<<<g2, FBT_THREADS, smem_async, (cudaStream_t)stream>>>(d, a);
   }
-  else wgrad_tc_kernel<<<grid, FBT_THREADS, smem, (cudaStream_t)stream>>>(d, a);
+  else {
+    a.acc = acc_tiles(h, stream);
+    if (!a.acc) return tsc_set_error("accumulator tiles: cudaMalloc failed");
+    wgrad_tc_kernel<<<grid, FBT_THREADS, smem, (cudaStream_t)stream>>>(d, a);
+  }
   PCK(cudaGetLastError());
   return 0;
 }
@@ -2374,18 +2381,19 @@ extern "C" int tscl_wgrad_tc(tscl_handle* h, const float* dZ, const void* dz_bf1
 // dX = dZ . Wx^T  (input gradient of the LSTM's x-projection, agents/utils.py:103-105 differentiated): a streaming GEMM
 // [M x 256] . [256 x dx] per unit, 960 B of HBM traffic per row.  Warp-specialised persistent kernel:
 //   warps 8-11  loaders : 16-byte cp.async of one swizzle atom (128 rows x 64 K, 16 KB) per stage, written in the
-//                         SWIZZLE_128B K-major pattern (chunk ^ (row & 7)); 3 stages, completion signalled two stages late
-//   warps 0-7   MMA     : two warpgroups (64 rows each), 4 x wgmma (N = dx, K = 16) per atom, B = the unit's Wx^T image
-//                         resident in shared memory (fetched by one cp.async.bulk per unit), accumulators double-buffered
-//                         in the accumulator tile (2 x 256 columns)
-//   warps 12-15 epilogue: accumulator row -> bf16 -> padded row in shared memory -> one cp.async.bulk store per row
-//                         (448 B), drained by the copy engine while the next tile is converted
+//                         SWIZZLE_128B K-major pattern (chunk ^ (row & 7)); 3 stages, completion signalled one stage late
+//   warps 0-7   MMA     : two warpgroups (64 rows each), 4 x wgmma (N = dx, K = 16) per atom into register fragments
+//                         (dx / 2 fp32 per thread, 168 registers at 384 threads), B = the unit's Wx^T image resident in
+//                         shared memory (fetched by one cp.async.bulk per unit); an atom's stage is released as soon as
+//                         the MMAs of the next atom are issued and its own have completed (wait_group 1)
+//              epilogue : after the tile's 4 atoms, the same warps convert their fragments to bf16 into padded rows in
+//                         shared memory, and one cp.async.bulk store per row (448 B) drains them while the next tile is
+//                         multiplied
 // A CTA owns a contiguous range of the (unit, 128-row tile) list, so it changes unit at most twice.
-#define DXK_THREADS 512
+#define DXK_THREADS 384
 #define DXK_STAGES 3
 #define DXK_STAGE_BYTES 16384
 struct DxTC {
-  float* acc;                // accumulator tiles, one [128][ACC_COLS] fp32 tile per CTA (acc_tiles)
   const __nv_bfloat16* dZb;    // [2A][M][256]
   const __nv_bfloat16* Wxt;    // [2A][32][dx][8]  (tscl_pack_wxt)
   __nv_bfloat16* dXb;          // [2A][M][dx]
@@ -2395,29 +2403,28 @@ __device__ __forceinline__ uint64_t make_desc_sw128(uint32_t saddr) {      // K-
   return (uint64_t)((saddr >> 4) & 0x3FFFu) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);   // layout type 1: 128B swizzle
 }
 
+template <int DXT>
 __global__ void __launch_bounds__(DXK_THREADS, 1)
 dx_tc_kernel(const DDimsTC d, const DxTC a) {
+  constexpr int N64 = DXT / 64, R32 = (DXT % 64) >= 32, R16 = (DXT % 32) >= 16;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int dx = d.dx, row_bytes = dx * 2, out_stride = row_bytes + 16;
+  const int dx = DXT, row_bytes = dx * 2, out_stride = row_bytes + 16;
   unsigned char* sStage = tc_smem;
   unsigned char* sB = sStage + DXK_STAGES * DXK_STAGE_BYTES;
   unsigned char* sOut = sB + (size_t)BW_KC * dx * 16;
   uint64_t* sBar = reinterpret_cast<uint64_t*>(sOut + (size_t)128 * out_stride);
-  const uint32_t bar_full = smem_u32(sBar), bar_empty = bar_full + 24, bar_accf = bar_full + 48, bar_acce = bar_full + 64,
-                 bar_b = bar_full + 80;
+  const uint32_t bar_full = smem_u32(sBar), bar_empty = bar_full + 24, bar_b = bar_full + 48;
   if (tid == 0) {
-    for (int s = 0; s < DXK_STAGES; ++s) { mbar_init(bar_full + 8 * s, 128); mbar_init(bar_empty + 8 * s, 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(bar_accf + 8 * b, 1); mbar_init(bar_acce + 8 * b, 128); }
+    for (int s = 0; s < DXK_STAGES; ++s) { mbar_init(bar_full + 8 * s, 128); mbar_init(bar_empty + 8 * s, 8); }
     mbar_init(bar_b, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
-  float* const acc = a.acc + (size_t)blockIdx.x * TC_M * ACC_COLS;
   const int64_t tpu = (a.M + 127) / 128;
   const int64_t NT = tpu * 2 * d.A;
   const int64_t j0 = NT * blockIdx.x / gridDim.x, j1 = NT * (blockIdx.x + 1) / gridDim.x;
 
-  if (warp >= 8 && warp < 12) {
+  if (warp >= 8) {
     // ---------------- loaders ----------------
     const int lt = tid - 256;
     const uint32_t aS = smem_u32(sStage);
@@ -2437,34 +2444,42 @@ dx_tc_kernel(const DDimsTC d, const DxTC a) {
           cp_async16(aS + s * DXK_STAGE_BYTES + rw * 128 + ((c ^ (rw & 7)) << 4), src0 + rr * TC_N + at * 64 + c * 8);
         }
         asm volatile("cp.async.commit_group;" ::: "memory");
-        if (it >= 2) {
-          asm volatile("cp.async.wait_group 2;" ::: "memory");
+        // one atom of lag, not two: the MMA warps release an atom's stage only once the next atom's MMAs are issued
+        // (wait_group 1), so holding back the atom before that one would close a wait cycle
+        if (it >= 1) {
+          asm volatile("cp.async.wait_group 1;" ::: "memory");
           asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-          mbar_arrive(bar_full + 8 * (int)((it - 2) % DXK_STAGES));
+          mbar_arrive(bar_full + 8 * (int)((it - 1) % DXK_STAGES));
         }
       }
-    }
-    if (it >= 2) {
-      asm volatile("cp.async.wait_group 1;" ::: "memory");
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      mbar_arrive(bar_full + 8 * (int)((it - 2) % DXK_STAGES));
     }
     if (it >= 1) {
       asm volatile("cp.async.wait_group 0;" ::: "memory");
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
       mbar_arrive(bar_full + 8 * (int)((it - 1) % DXK_STAGES));
     }
-  } else if (warp < 8) {
-    // ---------------- MMA: warps 0-7, one warpgroup per 64-row half ----------------
+  } else {
+    // ---------------- MMA + epilogue: warps 0-7, one warpgroup per 64-row half ----------------
+    const int wg = warp >> 2, tl = tid & 127;
     const uint32_t aS = smem_u32(sStage), aB = smem_u32(sB);
     const uint32_t b_lbo = (uint32_t)dx * 16;
-    int64_t it = 0, tc = 0;
-    int cur_u = -1;
+    float f64[N64 > 0 ? N64 : 1][32], f32[16], f16[8];
+    int64_t it = 0;
+    int cur_u = -1, prev_s = 0;
     uint32_t bph = 0;
-    for (int64_t j = j0; j < j1; ++j, ++tc) {
+    // this thread's fragment rows within the tile, and the padded output row it stores (tl < 64)
+    const int fr = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    const uint32_t my_s = smem_u32(sOut + (size_t)(wg * 64 + tl) * out_stride);
+    auto put = [&](int col, float x, float y, int r) {
+      const __nv_bfloat162 v = __floats2bfloat162_rn(x, y);
+      *reinterpret_cast<__nv_bfloat162*>(sOut + (size_t)r * out_stride + col * 2) = v;
+    };
+    for (int64_t j = j0; j < j1; ++j) {
       const int u = (int)(j / tpu);
-      if (u != cur_u) {      // every MMA of the previous unit has completed (wg_mma_done of its last atom)
+      const int64_t m0 = (j - (int64_t)u * tpu) * 128;
+      if (u != cur_u) {      // both warpgroups have waited for every MMA of the previous unit (end of its last tile)
         cur_u = u;
+        asm volatile("bar.sync 1, 256;" ::: "memory");
         if (tid == 0) {
           const uint32_t bytes = (uint32_t)BW_KC * dx * 16;
           mbar_expect_tx(bar_b, bytes);
@@ -2472,57 +2487,76 @@ dx_tc_kernel(const DDimsTC d, const DxTC a) {
         }
         mbar_wait(bar_b, bph); bph ^= 1;
       }
-      const int b = (int)(tc & 1);
-      const int64_t nb = tc >> 1;
-      if (nb > 0) mbar_wait(bar_acce + 8 * b, (uint32_t)((nb - 1) & 1));
       for (int at = 0; at < 4; ++at, ++it) {
         const int s = (int)(it % DXK_STAGES);
         mbar_wait(bar_full + 8 * s, (uint32_t)((it / DXK_STAGES) & 1));
-        wg_mma<0, 0>(acc, b * 256, dx, 4, at > 0, [&](int k, uint64_t& da, uint64_t& db) {
-          da = make_desc_sw128(aS + s * DXK_STAGE_BYTES + k * 32);
-          db = make_desc(aB + (uint32_t)((at * 4 + k) * 2) * b_lbo, b_lbo, 128);
-        });
-        wg_mma_done(bar_empty + 8 * s);
-      }
-      if (tid == 0) mbar_arrive(bar_accf + 8 * b);
-    }
-  } else {
-    // ---------------- epilogue: warps 12-15, thread = row ----------------
-    const int row = tid - 384;
-    unsigned char* my = sOut + (size_t)row * out_stride;
-    const uint32_t my_s = smem_u32(my);
-    int64_t tc = 0;
-    for (int64_t j = j0; j < j1; ++j, ++tc) {
-      const int u = (int)(j / tpu);
-      const int64_t m0 = (j - (int64_t)u * tpu) * 128;
-      const int b = (int)(tc & 1);
-      mbar_wait(bar_accf + 8 * b, (uint32_t)((tc >> 1) & 1));
-      asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");      // the previous store of this row has left shared memory
-      const uint32_t tb = ((uint32_t)((warp - 12) * 32) << 16) + (uint32_t)(b * 256);
-      for (int c0 = 0; c0 < dx; c0 += 32) {
-        float v[32];
-        acc_ld16(acc, tb + c0, v);
-        if (c0 + 16 < dx) acc_ld16(acc, tb + c0 + 16, v + 16);
-        const int nq = (c0 + 16 < dx) ? 4 : 2;
+        const uint32_t a0 = aS + s * DXK_STAGE_BYTES + wg * 8192;
+        const uint32_t b0 = aB + (uint32_t)(at * 8) * b_lbo;
+        wg_fence();
 #pragma unroll
-        for (int qd = 0; qd < 4; ++qd) {
-          if (qd < nq) {
-            __align__(16) __nv_bfloat16 o[8];
-#pragma unroll
-            for (int e = 0; e < 8; ++e) o[e] = __float2bfloat16_rn(v[qd * 8 + e]);
-            *reinterpret_cast<uint4*>(my + (c0 + qd * 8) * 2) = *reinterpret_cast<const uint4*>(o);
-          }
+        for (int q = 0; q < N64; ++q)
+          wg_mma_regs<64, 0, 0>(f64[q], 4, at > 0, [&](int k, uint64_t& da, uint64_t& db) {
+            da = make_desc_sw128(a0 + k * 32);
+            db = make_desc(b0 + (uint32_t)(k * 2) * b_lbo + q * 64 * 16, b_lbo, 128);
+          });
+        if constexpr (R32)
+          wg_mma_regs<32, 0, 0>(f32, 4, at > 0, [&](int k, uint64_t& da, uint64_t& db) {
+            da = make_desc_sw128(a0 + k * 32);
+            db = make_desc(b0 + (uint32_t)(k * 2) * b_lbo + N64 * 64 * 16, b_lbo, 128);
+          });
+        if constexpr (R16)
+          wg_mma_regs<16, 0, 0>(f16, 4, at > 0, [&](int k, uint64_t& da, uint64_t& db) {
+            da = make_desc_sw128(a0 + k * 32);
+            db = make_desc(b0 + (uint32_t)(k * 2) * b_lbo + (N64 * 64 + R32 * 32) * 16, b_lbo, 128);
+          });
+        wg_commit();
+        if (at > 0) {        // the MMAs of the previous atom have completed: release its stage
+          wg_wait<1>();
+          if (lane == 0) mbar_arrive(bar_empty + 8 * prev_s);
         }
+        prev_s = s;
       }
-      mbar_arrive(bar_acce + 8 * b);
+      wg_wait<0>();
+      if (lane == 0) mbar_arrive(bar_empty + 8 * prev_s);
+#pragma unroll
+      for (int q = 0; q < N64; ++q) wg_frag_fence(f64[q]);
+      if constexpr (R32) wg_frag_fence(f32);
+      if constexpr (R16) wg_frag_fence(f16);
+      // ---- epilogue: fragments -> bf16 rows in shared memory -> one bulk store per row ----
+      if (tl < 64) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");      // the previous tile's stores have left
+      asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
+      const int c0 = 2 * (lane & 3);
+#pragma unroll
+      for (int q = 0; q < N64; ++q)
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          put(q * 64 + 8 * i + c0, f64[q][4 * i], f64[q][4 * i + 1], fr);
+          put(q * 64 + 8 * i + c0, f64[q][4 * i + 2], f64[q][4 * i + 3], fr + 8);
+        }
+      if constexpr (R32)
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          put(N64 * 64 + 8 * i + c0, f32[4 * i], f32[4 * i + 1], fr);
+          put(N64 * 64 + 8 * i + c0, f32[4 * i + 2], f32[4 * i + 3], fr + 8);
+        }
+      if constexpr (R16)
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          put(N64 * 64 + R32 * 32 + 8 * i + c0, f16[4 * i], f16[4 * i + 1], fr);
+          put(N64 * 64 + R32 * 32 + 8 * i + c0, f16[4 * i + 2], f16[4 * i + 3], fr + 8);
+        }
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      if (m0 + row < a.M) {
-        __nv_bfloat16* dst = a.dXb + ((int64_t)u * a.M + m0 + row) * dx;
-        asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst), "r"(my_s), "r"(row_bytes) : "memory");
+      asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
+      if (tl < 64) {
+        const int64_t m = m0 + wg * 64 + tl;
+        if (m < a.M) {
+          __nv_bfloat16* dst = a.dXb + ((int64_t)u * a.M + m) * dx;
+          asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst), "r"(my_s), "r"(row_bytes) : "memory");
+        }
+        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
       }
-      asm volatile("cp.async.bulk.commit_group;" ::: "memory");
     }
-    asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+    if (tl < 64) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
   }
   __syncthreads();
 }
@@ -2531,23 +2565,29 @@ extern "C" int tscl_dx_tc(tscl_handle* h, const void* dz_bf16, const void* wxt_b
   if (!h || !dz_bf16 || !wxt_bf16 || !dx_bf16 || M <= 0) return tsc_set_error("tscl_dx_tc: bad argument");
   PCK(cudaSetDevice(tscl_device_of(h)));
   const DDimsTC& d = *tscl_dims_of(h);
-  if (d.dx % 16 != 0 || d.dx > 256 || d.dx < 16) return tsc_set_error("tscl_dx_tc: dx must be a multiple of 16 in [16, 256]");
+  if (d.dx % 16 != 0 || d.dx > 224 || d.dx < 16) return tsc_set_error("tscl_dx_tc: dx must be a multiple of 16 in [16, 224]");
   const size_t smem = (size_t)DXK_STAGES * DXK_STAGE_BYTES + (size_t)BW_KC * d.dx * 16 + (size_t)128 * (d.dx * 2 + 16) + 12 * 8 + 16;
   if (smem > 232448) return tsc_set_error("tscl_dx_tc: shared memory budget exceeded");
+  void (*kern)(const DDimsTC, const DxTC) = nullptr;
+  switch (d.dx) {      // the fragment size of the register accumulators is a compile-time constant
+#define DXK_CASE(n) case n: kern = dx_tc_kernel<n>; break;
+    DXK_CASE(16) DXK_CASE(32) DXK_CASE(48) DXK_CASE(64) DXK_CASE(80) DXK_CASE(96) DXK_CASE(112) DXK_CASE(128)
+    DXK_CASE(144) DXK_CASE(160) DXK_CASE(176) DXK_CASE(192) DXK_CASE(208) DXK_CASE(224)
+#undef DXK_CASE
+  }
   static int attr_dev = -1;
-  if (attr_dev != tscl_device_of(h)) {
-    PCK(cudaFuncSetAttribute(dx_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 232448));
-    attr_dev = tscl_device_of(h);
+  static void (*attr_kern)(const DDimsTC, const DxTC) = nullptr;
+  if (attr_dev != tscl_device_of(h) || attr_kern != kern) {
+    PCK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 232448));
+    attr_dev = tscl_device_of(h); attr_kern = kern;
   }
   int n_sm = 0;
   PCK(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, tscl_device_of(h)));
   const int64_t NT = ((M + 127) / 128) * 2 * d.A;
   const int grid = (int)(NT < n_sm ? NT : n_sm);
   DxTC a;
-  a.acc = acc_tiles(h, stream);
-  if (!a.acc) return tsc_set_error("accumulator tiles: cudaMalloc failed");
   a.dZb = (const __nv_bfloat16*)dz_bf16; a.Wxt = (const __nv_bfloat16*)wxt_bf16; a.dXb = (__nv_bfloat16*)dx_bf16; a.M = M;
-  dx_tc_kernel<<<grid, DXK_THREADS, smem, (cudaStream_t)stream>>>(d, a);
+  kern<<<grid, DXK_THREADS, smem, (cudaStream_t)stream>>>(d, a);
   PCK(cudaGetLastError());
   return 0;
 }
