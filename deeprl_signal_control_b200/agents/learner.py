@@ -98,7 +98,12 @@ class BatchedA2C:
         self.kernel_launches = 0
         # fused tensor-core forward (csrc/tsc_policy_tc.cu): bf16 image of [Wx;Wh], refreshed after every update
         self.use_tc = bool(use_tc) and (L.dx % 16 == 0) and layout.kw > 0    # else: the fp32 kernels
-        self.tc_v2 = self.use_tc and (L.dx % 32 == 0)          # fc front end on the tensor cores too
+        if self.use_tc and L.dx > 224:
+            # the fused forwards keep [Wx;Wh] resident in shared memory: 224 + 64 input rows is the most that fits
+            raise ValueError("the tensor-core policy forward supports dx <= 224 (got %d); use use_tc=False" % L.dx)
+        # fc front end on the tensor cores too; the v2 kernel is instantiated for the shipped fc widths (grid 224,
+        # Monaco 192, IA2C 160), other widths take the v1 kernel
+        self.tc_v2 = self.use_tc and L.dx in (160, 192, 224)
         self.Wp = torch.zeros(U, ((L.dx + L.h) // 8) * 4 * L.h * 8 + 8 * L.dx * 8, dtype=torch.bfloat16,
                               device=self.dev)
         self.Wt = torch.zeros(U, 32, L.h, 8, dtype=torch.bfloat16, device=self.dev)    # Wh^T image for the BPTT MMA

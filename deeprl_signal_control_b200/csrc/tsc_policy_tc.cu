@@ -1,6 +1,7 @@
 // tsc_policy_tc.cu — fused per-control-step policy forward and the learner's GEMMs on the Hopper tensor cores (sm_90a).
 //
-// One persistent CTA (1 per SM, up to ~223 KB smem) walks (unit, 128-replica tile) work items:
+// Policy forward v1 (tscl_policy_step; the shipping v2 kernel, warp-specialised with register accumulators, is described
+// at policy_step_tc2_kernel).  One persistent CTA (1 per SM, up to ~223 KB smem) walks (unit, 128-replica tile) work items:
 //   1. fc front end (agents/policies.py:191-201): relu(fc) of the observation slice, written as bf16 straight into
 //      the A-operand tile in shared memory (K-major, no swizzle), followed by the previous hidden state h (masked by
 //      the pre-decision done flag, agents/utils.py:104-105);
@@ -60,8 +61,8 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)_
 // 128 rows of a tile.  Their fp32 accumulator fragments are stored to the CTA's accumulator tile, 128 rows x ACC_COLS
 // fp32 in global memory (one tile per CTA and stream, see acc_tiles(); the tile of a CTA is written and read back by
 // the same SM within microseconds, so the round trip normally stays in L1/L2), which the row-per-thread epilogues read
-// back at address (row base << 16) + column, row = row base + lane.  This keeps the epilogues' thread = row mapping;
-// an epilogue that works on the wgmma register fragments directly would save the round trip (DESIGN.md §5).
+// back at address (row base << 16) + column, row = row base + lane.  This keeps the epilogues' thread = row mapping
+// (v1 policy forward, BPTT, fp32 weight gradients); the other kernels keep their fragments in registers.
 #define ACC_COLS 512
 __device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
   return (uint64_t)((saddr >> 4) & 0x3FFFu) | ((uint64_t)((lbo >> 4) & 0x3FFFu) << 16) |
@@ -88,8 +89,10 @@ __device__ __forceinline__ void wgmma_n16(float (&d)[8], uint64_t da, uint64_t d
                : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
                : "l"(da), "l"(db), "r"(accum), "n"(TA), "n"(TB) : "memory");
 }
-template <int TA, int TB>
-__device__ __forceinline__ void wgmma_n32(float (&d)[16], uint64_t da, uint64_t db, uint32_t accum) {
+// (a larger fragment array: its first 16 registers)
+template <int TA, int TB, int N>
+__device__ __forceinline__ void wgmma_n32(float (&d)[N], uint64_t da, uint64_t db, uint32_t accum) {
+  static_assert(N >= 16, "m64n32 accumulator needs 16 registers");
   asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
                "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, %19, %20;\n\t}"
                : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
@@ -596,92 +599,95 @@ extern "C" int tscl_policy_step(tscl_handle* h, const float* params, const void*
 }
 
 // ===================================================================================================
-// v2: the fc front end also runs on the tensor cores.
-//   A0 = observation slice tile [128 x 64] (wave32|fp16|wait16, bf16) staged in the LAST 8 K-chunks of the A tile,
-//   B0 = block-diagonal fc weights [64 x dx] staged in the FIRST chunks of the A tile (both regions are dead
-//        until the fc result is written / the h part is loaded), D0 = accumulator columns 256..256+dx;
-//   accumulator tile -> (+bias, relu, bf16) -> A tile chunks 0..dx/8, then h_prev -> last 8 chunks, then the
-//   gate MMA and the epilogue exactly as in v1.  Two MMA completions per tile on one mbarrier.
-// NT = 256: thread = (replica row, 32 hidden units); NT = 512: thread = (replica row, 16 hidden units) — twice the warps
-// per SM for the latency-bound staging / epilogue phases (one CTA per SM either way: the weight operand fills shared
-// memory), same arithmetic per element, so both variants produce identical bits.
-// A-tile region of the v2 kernel: the operand tile, or the largest copy-out staging pass (128 rows x 528 B + the parked
-// head partial sums behind the X pass), whichever is larger
-__host__ __device__ inline size_t tc2_a_bytes(int K) {
-  const size_t a = (size_t)(K / 8) * 2048;
-  return a > 69632 ? a : 69632;
+// v2: the fc front end also runs on the tensor cores, and the kernel is warp-specialised: 384 threads, three warpgroups.
+// A work item is (unit, 64 replica rows); a CTA walks a contiguous range of items, the items of one unit at a time.
+//   warpgroup 0, producer: stages the items in turn into two A tiles (item parity = tile): the unit's fc-weight block
+//     B0 [8][dx][16 B] by one bulk copy into the X chunks of the tile (it fills exactly dx / 8 chunks: a region that is
+//     dead until the fc result is written), and the observation slice A0 [64 x 64] (bf16) into the last 8 chunks (dead
+//     until h_{t-1} is written); L2 prefetch of the state rows of the item after next.
+//   warpgroups 1 and 2, consumers: consumer c takes the items of parity c, in tile c, so that one consumer's MMAs and
+//     operand loads overlap the other's epilogue:
+//       MMA0  D0[64 x dx] = A0 . B0 into registers; + bias, relu, bf16 -> X chunks of the tile (and the activation
+//             store st_x, copied out of shared memory in whole sectors); h_{t-1} -> the last 8 chunks;
+//       MMA1  gates[64 x 256] = [X | h] . [Wx;Wh] into registers, one m64n64 fragment per gate;
+//       LSTM cell, state and activation-store writes and the head dot products straight from the fragments.
+// The resident [Wx;Wh] image is copied into shared memory with its gate columns permuted: packed column 8i + 2q + e holds
+// gate i / 8, hidden unit 16q + 2(i % 8) + e (gate_col).  So lane q of each quad holds all four gates of hidden units
+// 16q .. 16q + 15 of its two fragment rows: thread = (row, 16 hidden units), the cell's natural assignment.  The MMAs
+// are the same m64nN k16 instructions in the same k order as a 128-row tile walked 64 columns at a time, and the cell,
+// store and head arithmetic is per element what it was, so the outputs do not depend on this organisation.
+#define P2_ROWS 64
+#define P2_DX_OK(dx) ((dx) == 160 || (dx) == 192 || (dx) == 224)   // keep in sync with BatchedA2C.tc_v2
+#define P2_THREADS 384
+// setmaxnreg: the producer gives registers back, the consumers (four m64n64 gate fragments = 128 per thread, plus the
+// cell state) take them.  setmaxnreg.inc only draws on what the CTA was launched with (168 per thread at 384 threads =
+// 64512; a larger request waits forever), so 128 * P2_PROD_REGS + 256 * P2_CONS_REGS must not exceed 384 * 168.
+#define P2_PROD_REGS 40
+#define P2_CONS_REGS 232
+static_assert(128 * P2_PROD_REGS + 256 * P2_CONS_REGS <= P2_THREADS * 168, "setmaxnreg split exceeds the CTA's registers");
+
+// v -> bf16 (round to nearest even) into the low (hi = 0) or high half of w
+__device__ __forceinline__ void bf16_pack(uint32_t& w, float v, int hi) {
+  const uint32_t b = __bfloat16_as_ushort(__float2bfloat16_rn(v));
+  w = hi ? (w | (b << 16)) : b;
 }
-template <int NT, bool PROF>
-__global__ void __launch_bounds__(NT, 1)
+// unpermuted gate-image column ([i | f | o | u] x 64) held by packed column n of the consumers' B operand
+__host__ __device__ inline int gate_col(int n) {
+  const int i = n >> 3, q = (n >> 1) & 3, e = n & 1;
+  return (i >> 3) * 64 + 16 * q + 2 * (i & 7) + e;
+}
+
+// DX = d.dx: the fragment sizes and the k loops are compile-time.  Instantiated for the fc widths of the shipped
+// configurations (P2_DX_OK): 224 (grid MA2C), 192 (Monaco), 160 (IA2C: no fingerprint block)
+template <int DX, bool PROF>
+__global__ void __launch_bounds__(P2_THREADS, 1)
 policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
-  constexpr int NG = NT / 128;                 // hidden-unit groups per row (2 or 4)
-  constexpr int HPT = TC_H / NG;               // hidden units per thread (32 or 16)
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int K = d.dx + TC_H, KC = K / 8, KS = K / 16, KCX = d.dx / 8;
-  unsigned char* sB = tc_smem;                                  // KC * 4096
-  unsigned char* sA = sB + (size_t)KC * 4096;                   // KC * 2048
-  float* sRed = reinterpret_cast<float*>(sA + tc2_a_bytes(K));      // [128][8]
-  float* sWo = sRed + TC_M * 8;                                 // [64][8]
-  float* sBo = sWo + TC_H * 8;                                  // [8]
-  float* sBias = sBo + 8;                                       // [256]  lstm bias
-  float* sBias0 = sBias + TC_N;                                 // [256]  fc biases
-  uint64_t* sBar = reinterpret_cast<uint64_t*>(sBias0 + TC_N);
-  const uint32_t bar = smem_u32(sBar), bar_fc = smem_u32(sBar + 1);   // MMA completion; fc-weight bulk copy landed
+  const int tid = threadIdx.x, wg = tid >> 7, lane = tid & 31;
+  constexpr int K = DX + TC_H, KC = K / 8, KS = K / 16, KCX = DX / 8, NXF = (DX + 63) / 64;
+  unsigned char* sB = tc_smem;                                               // KC * 4096, gate columns permuted
+  unsigned char* sA0 = sB + (size_t)KC * 4096;                               // two A tiles [KC][64 rows][16 B]
+  float* sWo = reinterpret_cast<float*>(sA0 + (size_t)2 * KC * 1024);        // [64][8]
+  float* sBo = sWo + TC_H * 8;                                               // [8]
+  float* sBias = sBo + 8;                                                    // [256]  lstm bias
+  float* sBias0 = sBias + TC_N;                                              // [256]  fc biases
+  uint64_t* sBar = reinterpret_cast<uint64_t*>(sBias0 + TC_N);               // full[2], empty[2]
+  const uint32_t aB = smem_u32(sB);
   if (tid == 0) {
-    mbar_init(bar, 1); mbar_init(bar_fc, 1);
+    for (int s = 0; s < 2; ++s) {
+      mbar_init(smem_u32(sBar + s), 128 + 1);        // producer threads + the fc-weight copy's expect_tx
+      mbar_init(smem_u32(sBar + 2 + s), 128);        // consumer threads: the tile is dead
+    }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
-  float* const acc = a.acc + (size_t)blockIdx.x * TC_M * ACC_COLS;
-  const int64_t n_tiles = (a.R + TC_M - 1) / TC_M;
+  const int64_t n_tiles = (a.R + P2_ROWS - 1) / P2_ROWS;
   const int64_t ld = a.ld > 0 ? a.ld : a.R;
   const int64_t n_items = n_tiles * 2 * d.A;
   const int64_t it_lo = n_items * blockIdx.x / gridDim.x, it_hi = n_items * (blockIdx.x + 1) / gridDim.x;
-  int cur_u = -1;
-  uint32_t parity = 0, par_fc = 0;
-  int nw = 0, nt = 0, nf = 0, ooff = 0, na = 0, src_a = -1, src_b = -1;
-  const uint32_t aA = smem_u32(sA), aB = smem_u32(sB);
 
-  long long pt[16] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0}, pc = 0;
-#define PROF_MARK(i) do { if (PROF && tid == 0) { const long long c_ = clock64(); pt[i] += c_ - pc; pc = c_; } } while (0)
-  if (PROF && tid == 0) pc = clock64();
-  for (int64_t it = it_lo; it < it_hi; ++it) {
-    const int u = (int)(it / n_tiles);
-    const int64_t r0 = (it - (int64_t)u * n_tiles) * TC_M;
-    const int ag = u >> 1;
-    // row of the activation store (chunk-outermost [R/rc][2A][T][rc][w]) for tile row `row`: one division per item
-    const int64_t st_c0 = (a.row0 + r0) / a.rc, st_rin0 = (a.row0 + r0) - st_c0 * a.rc;
-    auto store_row = [&](int row) -> int64_t {
-      int64_t c = st_c0, rin = st_rin0 + row;
-      while (rin >= a.rc) { rin -= a.rc; ++c; }
-      return ((c * (2 * d.A) + u) * a.T + a.t) * a.rc + rin;
-    };
-    const __nv_bfloat16* Wu = a.Wp + (int64_t)u * wp_stride(d.dx);
-    // NT = 512: no block-wide barrier here.  Warps 0-3 may still be in the previous tile's head softmax / sampling (they read
-    // sRed, sRed2 = sA + 32 KB, sBo) while warps 4-15 already fetch and stage this tile's observation slice (last 8 chunks
-    // of sA) and the fc-weight block (first 28 KB of sA); the barrier after the staging retires the previous tile.
-    if (NT != 512 || u != cur_u) __syncthreads();      // previous tile fully retired (sRed, sA, sBo, accumulator readers)
-    if (u != cur_u) {
-      cur_u = u;
-      const uint4* src = reinterpret_cast<const uint4*>(Wu);
+  // phase clocks of the producer's thread 0 and consumer 0's thread 0, added straight into the counters (no register
+  // arrays: the producer's budget is small)
+  long long pc = 0;
+  const bool prof_thread = PROF && (tid == 0 || tid == 128);
+#define PROF_MARK(i) do { if (PROF && prof_thread) { const long long c_ = clock64(); atomicAdd(a.prof + (i), (unsigned long long)(c_ - pc)); pc = c_; } } while (0)
+  if (PROF && prof_thread) pc = clock64();
+
+  // the constants of unit u, written by the 256 consumer threads between two CTA barriers that every role passes (all
+  // roles have retired the previous unit); the producer, with its small register budget, only takes the barriers
+  auto load_unit = [&](int u, bool consumer) {
+    __syncthreads();
+    if (consumer) {
+      const int t = tid - 128;
+      const uint4* src = reinterpret_cast<const uint4*>(a.Wp + (int64_t)u * wp_stride(DX));
       uint4* dst = reinterpret_cast<uint4*>(sB);
-      for (int i = tid; i < KC * TC_N; i += NT) dst[i] = src[i];
-      nw = d.n_wave[ag]; nt = d.n_wait[ag]; nf = d.ff > 0 ? d.n_fp[ag] : 0;
-      ooff = d.obs_off[ag]; na = d.n_a[ag];
-      {      // observation index of this lane's two input slots (-1: unused slot)
-        auto slot_src = [&](int c) -> int {
-          if (c < d.kw) return c < nw ? c : -1;
-          if (c < d.kw + TC_KF) return c - d.kw < nf ? nw + nt + (c - d.kw) : -1;
-          return c - d.kw - TC_KF < nt ? nw + (c - d.kw - TC_KF) : -1;
-        };
-        src_a = slot_src(2 * lane); src_b = slot_src(2 * lane + 1);
-      }
-      for (int i = tid; i < TC_H * 8; i += NT) {
+#pragma unroll 4
+      for (int i = t; i < KC * TC_N; i += 256) dst[i] = src[(i & ~(TC_N - 1)) + gate_col(i & (TC_N - 1))];
+      for (int i = t; i < TC_H * 8; i += 256) {
         const int k = i >> 3, j = i & 7;
         sWo[i] = j < d.max_na ? a.P[d.off_wo + ((int64_t)u * TC_H + k) * d.max_na + j] : 0.f;
       }
-      if (tid < 8) sBo[tid] = tid < d.max_na ? a.P[d.off_bo + (int64_t)u * d.max_na + tid] : 0.f;
-      for (int i = tid; i < TC_N; i += NT) {
+      if (t < 8) sBo[t] = t < d.max_na ? a.P[d.off_bo + (int64_t)u * d.max_na + t] : 0.f;
+      for (int i = t; i < TC_N; i += 256) {
         sBias[i] = a.P[d.off_bl + (int64_t)u * TC_N + i];
         float b0 = 0.f;
         if (i < d.fw) b0 = a.P[d.off_fcw_b[u] + i];
@@ -689,357 +695,306 @@ policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
         else if (i < d.dx) b0 = a.P[d.off_fct_b[u] + (i - d.fw - d.ff)];
         sBias0[i] = b0;
       }
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");      // the B image is read by wgmma
     }
-    PROF_MARK(0);      // item-top sync + per-unit weight / constant (re)load
-    // L2 prefetch of the NEXT work item's operands (observation slice, c, h): they are consumed ~one tile later
-    if (it + 1 < it_hi) {
-      const int un = (int)((it + 1) / n_tiles);
-      const int64_t rn = ((it + 1) - (int64_t)un * n_tiles) * TC_M + (tid / NG);
-      if (rn < a.R && (tid % NG) < 2) {
-        const int an = un >> 1;
-        const float* op = a.obs + rn * d.n_obs + d.obs_off[an] + (tid % NG) * 32;
-        asm volatile("prefetch.global.L2 [%0];" ::"l"(op));
-        const int64_t so = ((int64_t)un * ld + rn) * TC_H + (tid % NG) * 32;
-        asm volatile("prefetch.global.L2 [%0];" ::"l"(a.c_in + so));
-        asm volatile("prefetch.global.L2 [%0];" ::"l"(a.h_in + so));
-      }
-    }
-    // ---- 1a. B0 (fc weights) -> first chunks of the A tile; 1b. observation slice -> last 8 chunks ----
-    {
-      // fc weights (one contiguous 8 * dx * 16-byte block of the packed image) by ONE bulk copy (TMA unit, completion on
-      // bar_fc): it overlaps the observation staging below; only the MMA-issuing thread waits for it
-      // NT = 512: the copy for every tile but the CTA's first was issued right after the previous tile's gate MMA had
-      // completed (the whole epilogue hides it)
-      if (tid == NT - 1 && (NT != 512 || it == it_lo)) {
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // earlier generic-proxy stores to the A tile precede this async write
-        mbar_expect_tx(bar_fc, (uint32_t)(8 * d.dx * 16));
-        bulk_g2s(aA, reinterpret_cast<const unsigned char*>(Wu + (int64_t)KC * TC_N * 8), (uint32_t)(8 * d.dx * 16), bar_fc);
-      }
-      if constexpr (NT == 512) {
-        // a warp takes 8 rows; lane l owns input slots 2l, 2l + 1 of every row (their observation indices src_a / src_b were
-        // resolved when the unit changed).  The slice of a row is one contiguous <= 256 B run of the observation vector, so
-        // a warp load touches 2-3 sectors of ONE row (the former thread = (row, chunk) mapping touched 32 rows per
-        // instruction: 8 k sector requests per tile, the whole staging phase); the two values leave as one packed store.
-        // warps 4-15 share the 128 rows (11 each); warps 0-3 finish the previous tile's heads meanwhile
-        if (warp >= 4) {
-          const int rb = (warp - 4) * 11;
-          float xa[11], xb[11];
+    __syncthreads();
+  };
+
+  if (wg == 0) {
+    // ================= producer =================
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(P2_PROD_REGS));
+    const int warp = tid >> 5;
+    uint32_t ph_empty = 0;
+    for (int64_t seg = it_lo; seg < it_hi;) {
+      const int u = (int)(seg / n_tiles), ag = u >> 1;
+      const int64_t seg_hi = (int64_t)(u + 1) * n_tiles < it_hi ? (int64_t)(u + 1) * n_tiles : it_hi;
+      load_unit(u, false);
+      PROF_MARK(8);      // producer: unit constants
+      const int nw = d.n_wave[ag], nt = d.n_wait[ag], nf = d.ff > 0 ? d.n_fp[ag] : 0, ooff = d.obs_off[ag];
+      // observation index of this lane's two input slots 2 lane, 2 lane + 1 (-1: unused slot)
+      auto slot_src = [&](int c) -> int {
+        if (c < d.kw) return c < nw ? c : -1;
+        if (c < d.kw + TC_KF) return c - d.kw < nf ? nw + nt + (c - d.kw) : -1;
+        return c - d.kw - TC_KF < nt ? nw + (c - d.kw - TC_KF) : -1;
+      };
+      const int src_a = slot_src(2 * lane), src_b = slot_src(2 * lane + 1);
+      const __nv_bfloat16* Wfc = a.Wp + (int64_t)u * wp_stride(DX) + (int64_t)KC * TC_N * 8;
+      for (int64_t it = seg; it < seg_hi; ++it) {
+        const int s = (int)((it - it_lo) & 1);
+        const int64_t r0 = (it - (int64_t)u * n_tiles) * P2_ROWS;
+        unsigned char* sA = sA0 + (size_t)s * KC * 1024;
+        const uint32_t full = smem_u32(sBar + s), empty = smem_u32(sBar + 2 + s);
+        mbar_wait(empty, ((ph_empty >> s) & 1) ^ 1);       // the tile's previous item has left it (first use: passes)
+        ph_empty ^= 1u << s;
+        PROF_MARK(9);    // producer: waiting for a free tile
+        if (tid == 0) {
+          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+          mbar_expect_tx(full, (uint32_t)(8 * DX * 16));
+          bulk_g2s(smem_u32(sA), Wfc, (uint32_t)(8 * DX * 16), full);
+        }
+        if (it + 2 < it_hi) {      // L2 prefetch of the state rows and observations of the next item of this tile
+          const int un = (int)((it + 2) / n_tiles);
+          const int64_t rn = ((it + 2) - (int64_t)un * n_tiles) * P2_ROWS + (tid & 63);
+          if (rn < a.R) {
+            const int64_t so = ((int64_t)un * ld + rn) * TC_H + (tid >> 6) * 32;
+            asm volatile("prefetch.global.L2 [%0];" ::"l"(a.c_in + so));
+            asm volatile("prefetch.global.L2 [%0];" ::"l"(a.h_in + so));
+            asm volatile("prefetch.global.L2 [%0];" ::"l"(a.obs + rn * d.n_obs + d.obs_off[un >> 1] + (tid >> 6) * 32));
+          }
+        }
+        // observation slice: warp w takes rows 16 w .. 16 w + 15, lane l the input slots 2l, 2l + 1 of each (the slice of
+        // a row is one contiguous <= 256 B run of the observation vector); the two values leave as one packed store
 #pragma unroll
-          for (int rr = 0; rr < 11; ++rr) {
+        for (int h4 = 0; h4 < 4; ++h4) {
+          const int rb = warp * 16 + h4 * 4;
+          float xa[4], xb[4];
+#pragma unroll
+          for (int rr = 0; rr < 4; ++rr) {
             const int64_t r = r0 + rb + rr;
-            const bool ok = rb + rr < TC_M && r < a.R;
+            const bool ok = r < a.R;
             const float* op = a.obs + (ok ? r : 0) * d.n_obs + ooff;
             xa[rr] = (src_a >= 0 && ok) ? __ldg(op + src_a) : 0.f;
             xb[rr] = (src_b >= 0 && ok) ? __ldg(op + src_b) : 0.f;
           }
 #pragma unroll
-          for (int rr = 0; rr < 11; ++rr) {
-            const int row = rb + rr;
-            if (row < TC_M) {
-              const __nv_bfloat162 v = __floats2bfloat162_rn(xa[rr], xb[rr]);
-              *reinterpret_cast<__nv_bfloat162*>(sA + (size_t)(KC - 8 + (lane >> 2)) * 2048 + row * 16 + (lane & 3) * 4) = v;
+          for (int rr = 0; rr < 4; ++rr)
+            *reinterpret_cast<__nv_bfloat162*>(sA + (size_t)(KC - 8 + (lane >> 2)) * 1024 + (rb + rr) * 16 + (lane & 3) * 4) =
+                __floats2bfloat162_rn(xa[rr], xb[rr]);
+        }
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+        mbar_arrive(full);
+        PROF_MARK(10);   // producer: fc-weight copy issue + observation staging
+      }
+      seg = seg_hi;
+    }
+  } else {
+    // ================= consumers =================
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(P2_CONS_REGS));
+    const int c = wg - 1, ct = tid & 127, q = lane & 3;
+    const int rq = 16 * (ct >> 5) + (lane >> 2);                  // fragment rows rq, rq + 8
+    unsigned char* sA = sA0 + (size_t)c * KC * 1024;
+    const uint32_t aA = smem_u32(sA), full = smem_u32(sBar + c), empty = smem_u32(sBar + 2 + c);
+    uint32_t ph_full = 0;
+    for (int64_t seg = it_lo; seg < it_hi;) {
+      const int u = (int)(seg / n_tiles), ag = u >> 1;
+      const int64_t seg_hi = (int64_t)(u + 1) * n_tiles < it_hi ? (int64_t)(u + 1) * n_tiles : it_hi;
+      load_unit(u, true);
+      PROF_MARK(0);      // unit constants
+      const int na = d.n_a[ag];
+      for (int64_t it = seg + (((seg - it_lo) & 1) != c ? 1 : 0); it < seg_hi; it += 2) {
+        const int64_t r0 = (it - (int64_t)u * n_tiles) * P2_ROWS;
+        // row of the activation store (chunk-outermost [R/rc][2A][T][rc][w]) for tile row `row`
+        const int64_t st_c0 = (a.row0 + r0) / a.rc, st_rin0 = (a.row0 + r0) - st_c0 * a.rc;
+        auto store_row = [&](int row) -> int64_t {
+          int64_t cc = st_c0, rin = st_rin0 + row;
+          while (rin >= a.rc) { rin -= a.rc; ++cc; }
+          return ((cc * (2 * d.A) + u) * a.T + a.t) * a.rc + rin;
+        };
+        mbar_wait(full, ph_full);
+        ph_full ^= 1;
+        PROF_MARK(1);    // waiting for the staged operands
+        // ---- MMA0: D0[64 x dx] = A0[64 x 64] . B0[64 x dx], 64 columns at a time (a last 32-column piece if dx % 64) ----
+        float x[NXF][32];
+        wg_fence();
+#pragma unroll
+        for (int j = 0; j < NXF; ++j)
+#pragma unroll
+          for (int ks = 0; ks < 4; ++ks) {
+            const uint64_t da = make_desc(aA + (KC - 8 + 2 * ks) * 1024, 1024, 128);
+            const uint64_t db = desc_adv_mn(make_desc(aA + ks * 2 * (DX * 16), DX * 16, 128), 64 * j);
+            if (64 * j + 64 <= DX) wgmma_n64<0, 0>(x[j], da, db, ks > 0 ? 1u : 0u);
+            else wgmma_n32<0, 0>(x[j], da, db, ks > 0 ? 1u : 0u);
+          }
+        wg_commit();
+        wg_wait<0>();
+#pragma unroll
+        for (int j = 0; j < NXF; ++j) wg_frag_fence(x[j]);
+        PROF_MARK(2);    // MMA0 issue + wait
+        // ---- X = relu(D0 + b) as bf16 -> chunks 0 .. dx/8 (B0 is dead); h_{t-1} -> the last 8 (A0 is dead) ----
+#pragma unroll
+        for (int j = 0; j < NXF; ++j)
+#pragma unroll
+          for (int i = 0; i < 8; ++i) {
+            const int col = 64 * j + 8 * i;
+            if (col < DX) {
+              const float b0 = sBias0[col + 2 * q], b1 = sBias0[col + 2 * q + 1];
+#pragma unroll
+              for (int hr = 0; hr < 2; ++hr)
+                *reinterpret_cast<__nv_bfloat162*>(sA + (size_t)(col >> 3) * 1024 + (rq + 8 * hr) * 16 + q * 4) =
+                    __floats2bfloat162_rn(fmaxf(x[j][4 * i + 2 * hr] + b0, 0.f), fmaxf(x[j][4 * i + 2 * hr + 1] + b1, 0.f));
+            }
+          }
+        // h_{t-1} of row ct & 63, hidden units 32 (ct >> 6) .. (the producer prefetched it to L2)
+        float4 hpre[8];
+        {
+          const int64_t r = r0 + (ct & 63);
+          const bool live = r < a.R && !a.done;
+          const float4* hp = reinterpret_cast<const float4*>(a.h_in + ((int64_t)u * ld + (r < a.R ? r : 0)) * TC_H + (ct >> 6) * 32);
+#pragma unroll
+          for (int i = 0; i < 8; ++i) hpre[i] = live ? hp[i] : make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+#pragma unroll
+        for (int c8 = 0; c8 < 4; ++c8) {
+          __align__(16) __nv_bfloat16 v[8];
+          const float4 x0 = hpre[2 * c8], x1 = hpre[2 * c8 + 1];
+          v[0] = __float2bfloat16_rn(x0.x); v[1] = __float2bfloat16_rn(x0.y); v[2] = __float2bfloat16_rn(x0.z); v[3] = __float2bfloat16_rn(x0.w);
+          v[4] = __float2bfloat16_rn(x1.x); v[5] = __float2bfloat16_rn(x1.y); v[6] = __float2bfloat16_rn(x1.z); v[7] = __float2bfloat16_rn(x1.w);
+          *reinterpret_cast<uint4*>(sA + (size_t)(KCX + (ct >> 6) * 4 + c8) * 1024 + (ct & 63) * 16) = *reinterpret_cast<const uint4*>(v);
+        }
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+        if (c == 0) asm volatile("bar.sync 1, 128;" ::: "memory");     // the whole tile of this consumer is written
+        else asm volatile("bar.sync 2, 128;" ::: "memory");
+        // st_x out of the tile, 32 bytes of a row per thread (the 8 lanes of a quarter-warp read 8 rows of one chunk
+        // pair: no bank conflicts)
+        if (a.st_x) {
+          constexpr int np = DX / 16;
+#pragma unroll 2
+          for (int p = ct; p < P2_ROWS * np; p += 128) {
+            const int rest = p >> 3, pcol = rest % np, row = (rest / np) * 8 + (p & 7);
+            if (r0 + row < a.R) {
+              const uint4 lo = *reinterpret_cast<const uint4*>(sA + (size_t)(2 * pcol) * 1024 + row * 16);
+              const uint4 hi = *reinterpret_cast<const uint4*>(sA + (size_t)(2 * pcol + 1) * 1024 + row * 16);
+              uint4* o = reinterpret_cast<uint4*>(a.st_x + store_row(row) * DX + 16 * pcol);
+              o[0] = lo; o[1] = hi;
             }
           }
         }
-      } else {
-        // thread = (row, 16-byte chunk) : 128 x 8 pairs, 4 per thread
+        PROF_MARK(3);    // relu epilogue + h staging + st_x copy-out
+        // ---- MMA1: gates[64 x 256] = [X | h][64 x K] . [Wx;Wh][K x 256], one m64n64 fragment per gate ----
+        float g[4][32];
+        // descriptors = base + address offset >> 4 (no carry out of the 14-bit field: shared addresses < 256 KB); the base
+        // is made opaque here so that the 2 x 4 KS descriptors are formed at issue, not hoisted out of the item loop
+        uint64_t dA1 = make_desc(aA, 1024, 128), dB1 = make_desc(aB, 4096, 128);
+        asm volatile("" : "+l"(dA1), "+l"(dB1));
+        wg_fence();
 #pragma unroll
-        for (int p = 0; p < 1024 / NT; ++p) {
-          const int pair = p * NT + tid;
-          const int row = pair & 127, ch = pair >> 7;          // consecutive threads -> consecutive rows
+        for (int gi = 0; gi < 4; ++gi)
+#pragma unroll
+          for (int ks = 0; ks < KS; ++ks)
+            wgmma_n64<0, 0>(g[gi], dA1 + (uint64_t)((ks * 2 * 1024) >> 4), dB1 + (uint64_t)((ks * 2 * 4096 + gi * 1024) >> 4),
+                            ks > 0 ? 1u : 0u);
+        wg_commit();
+        wg_wait<0>();
+#pragma unroll
+        for (int gi = 0; gi < 4; ++gi) wg_frag_fence(g[gi]);
+        mbar_arrive(empty);      // this thread is done with the tile (its st_x reads have returned)
+        PROF_MARK(4);    // gate MMA issue + wait
+        // ---- epilogue: the two fragment rows of this thread, 16 hidden units 16 q .. each ----
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+          const int row = rq + 8 * hr;
           const int64_t r = r0 + row;
-          __align__(16) __nv_bfloat16 v[8];
+          const bool valid = r < a.R;
+          const int64_t srow = ((int64_t)u * ld + (valid ? r : 0)) * TC_H + 16 * q;
+          float cprev[16];      // c_{t-1} of (row, hidden units 16 q ..), prefetched to L2 by the producer
+          if (valid && !a.done) {
 #pragma unroll
-          for (int e = 0; e < 8; ++e) {
-            const int c = ch * 8 + e;
-            int src = -1;
-            if (c < d.kw) { if (c < nw) src = c; }
-            else if (c < d.kw + TC_KF) { if (c - d.kw < nf) src = nw + nt + (c - d.kw); }
-            else { if (c - d.kw - TC_KF < nt) src = nw + (c - d.kw - TC_KF); }
-            float x = 0.f;
-            if (src >= 0 && r < a.R) x = __ldg(a.obs + r * d.n_obs + ooff + src);
-            v[e] = __float2bfloat16_rn(x);
-          }
-          *reinterpret_cast<uint4*>(sA + (size_t)(KC - 8 + ch) * 2048 + row * 16) = *reinterpret_cast<const uint4*>(v);
-        }
-      }
-    }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    __syncthreads();
-    PROF_MARK(1);      // staging: fc weights + observation slice
-    // ---- 2. MMA0: D0[128 x dx] = A0[128 x 64] . B0[64 x dx]  (accumulator columns 256..) ----
-    if (warp < 8) {
-      mbar_wait(bar_fc, par_fc);
-      wg_mma<0, 0>(acc, 256, d.dx, 4, false, [&](int ks, uint64_t& da, uint64_t& db) {
-        da = make_desc(aA + (KC - 8 + 2 * ks) * 2048, 2048, 128);
-        db = make_desc(aA + ks * 2 * (d.dx * 16), d.dx * 16, 128);
-      });
-      wg_mma_done(bar);
-    }
-    par_fc ^= 1;
-    // h_{t-1} of this thread's (row, hidden-unit group): requested before the MMA wait, staged after the relu epilogue
-    float4 hpre[HPT / 4];
-    {
-      const int64_t r = r0 + tid / NG;
-      const bool live = r < a.R && !a.done;
-      const float4* hp = reinterpret_cast<const float4*>(a.h_in + ((int64_t)u * ld + (r < a.R ? r : 0)) * TC_H + (tid % NG) * HPT);
-#pragma unroll
-      for (int i = 0; i < HPT / 4; ++i) hpre[i] = live ? hp[i] : make_float4(0.f, 0.f, 0.f, 0.f);
-    }
-    mbar_wait(bar, parity);
-    parity ^= 1;
-    PROF_MARK(2);      // MMA0 issue + wait
-    // ---- 3. X = relu(D0 + b) as bf16 -> A tile chunks 0..dx/8 ; h_prev -> last 8 chunks ----
-    {
-      const int q = warp & 3, hw = warp >> 2;
-      const int row = q * 32 + lane;
-      const int ncol = d.dx / NG;                      // columns per group (multiple of 8: dx % 32 == 0)
-      const bool st = a.st_x && r0 + row < a.R;
-      const int64_t m = st ? store_row(row) : 0;
-      const int cend = (hw + 1) * ncol;
-      for (int c0 = hw * ncol; c0 < cend;) {
-        if (NT == 512 && (c0 & 15) == 0 && c0 + 16 <= cend) {      // 16 columns: two 128-bit stores of the activation row
-          float z[16];
-          acc_ld16(acc, ((uint32_t)(q * 32) << 16) + 256u + (uint32_t)c0, z);
-          __align__(32) __nv_bfloat16 v[16];
-#pragma unroll
-          for (int e = 0; e < 16; ++e) v[e] = __float2bfloat16_rn(fmaxf(z[e] + sBias0[c0 + e], 0.f));
-          *reinterpret_cast<uint4*>(sA + (size_t)(c0 >> 3) * 2048 + row * 16) = *reinterpret_cast<const uint4*>(v);
-          *reinterpret_cast<uint4*>(sA + (size_t)((c0 >> 3) + 1) * 2048 + row * 16) = *reinterpret_cast<const uint4*>(v + 8);
-          if (st) {
-            const uint4 x = reinterpret_cast<const uint4*>(v)[0], y = reinterpret_cast<const uint4*>(v)[1];
-            reinterpret_cast<uint4*>(a.st_x + (m * d.dx + c0))[0] = x;
-            reinterpret_cast<uint4*>(a.st_x + (m * d.dx + c0))[1] = y;
-          }
-          c0 += 16;
-        } else {
-          float z[8];
-          acc_ld8(acc, ((uint32_t)(q * 32) << 16) + 256u + (uint32_t)c0, z);
-          __align__(16) __nv_bfloat16 v[8];
-#pragma unroll
-          for (int e = 0; e < 8; ++e) v[e] = __float2bfloat16_rn(fmaxf(z[e] + sBias0[c0 + e], 0.f));
-          *reinterpret_cast<uint4*>(sA + (size_t)(c0 >> 3) * 2048 + row * 16) = *reinterpret_cast<const uint4*>(v);
-          if (st) *reinterpret_cast<uint4*>(a.st_x + (m * d.dx + c0)) = *reinterpret_cast<const uint4*>(v);
-          c0 += 8;
-        }
-      }
-    }
-    {
-      const int row = tid / NG, half = tid % NG;      // `half` = hidden-unit group of HPT units
-#pragma unroll
-      for (int c8 = 0; c8 < HPT / 8; ++c8) {
-        __align__(16) __nv_bfloat16 v[8];
-        const float4 x0 = hpre[2 * c8], x1 = hpre[2 * c8 + 1];
-        v[0] = __float2bfloat16_rn(x0.x); v[1] = __float2bfloat16_rn(x0.y); v[2] = __float2bfloat16_rn(x0.z); v[3] = __float2bfloat16_rn(x0.w);
-        v[4] = __float2bfloat16_rn(x1.x); v[5] = __float2bfloat16_rn(x1.y); v[6] = __float2bfloat16_rn(x1.z); v[7] = __float2bfloat16_rn(x1.w);
-        *reinterpret_cast<uint4*>(sA + (size_t)(KCX + half * (HPT / 8) + c8) * 2048 + row * 16) = *reinterpret_cast<const uint4*>(v);
-      }
-    }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    __syncthreads();
-    PROF_MARK(3);      // relu epilogue of the fc GEMM (+ st_x) and h staging
-    // ---- 4. MMA1: gates D1[128 x 256] = [X | h][128 x K] . [Wx;Wh][K x 256] ----
-    if (warp < 8) {
-      wg_mma<0, 0>(acc, 0, TC_N, KS, false, [&](int ks, uint64_t& da, uint64_t& db) {
-        da = make_desc(aA + ks * 2 * 2048, 2048, 128);
-        db = make_desc(aB + ks * 2 * 4096, 4096, 128);
-      });
-      wg_mma_done(bar);
-    }
-    float cpre[16];        // c_{t-1} of this thread's 16 hidden units (NT = 512): in flight while the gate MMA runs
-    if constexpr (NT == 512) {
-      const int64_t r = r0 + (warp & 3) * 32 + lane;
-      if (r < a.R && !a.done) {
-        const float* cp = a.c_in + ((int64_t)u * ld + r) * TC_H + (warp >> 2) * HPT;
-#pragma unroll
-        for (int e4 = 0; e4 < 4; ++e4) {
-          const float4 x = reinterpret_cast<const float4*>(cp)[e4];
-          cpre[4 * e4] = x.x; cpre[4 * e4 + 1] = x.y; cpre[4 * e4 + 2] = x.z; cpre[4 * e4 + 3] = x.w;
-        }
-      } else {
-#pragma unroll
-        for (int e = 0; e < 16; ++e) cpre[e] = 0.f;
-      }
-    }
-    mbar_wait(bar, parity);
-    parity ^= 1;
-    if (NT == 512 && tid == NT - 1 && it + 1 < it_hi) {
-      // the A tile is dead: fetch the NEXT tile's fc-weight block now (its unit may differ)
-      const int un = (int)((it + 1) / n_tiles);
-      const __nv_bfloat16* Wn = a.Wp + (int64_t)un * wp_stride(d.dx);
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      mbar_expect_tx(bar_fc, (uint32_t)(8 * d.dx * 16));
-      bulk_g2s(aA, reinterpret_cast<const unsigned char*>(Wn + (int64_t)KC * TC_N * 8), (uint32_t)(8 * d.dx * 16), bar_fc);
-    }
-    PROF_MARK(4);      // gate MMA issue + wait
-    // ---- 5. epilogue (identical to v1) ----
-    {
-      const int q = warp & 3, half = warp >> 2;
-      const int row = q * 32 + lane;
-      const int64_t r = r0 + row;
-      const bool valid = r < a.R;
-      const int64_t srow = ((int64_t)u * ld + (valid ? r : 0)) * TC_H + half * HPT;
-      float lg[8];
-#pragma unroll
-      for (int j = 0; j < 8; ++j) lg[j] = 0.f;
-      // partial head sums of groups 1..NG-1: group 1 in sRed, groups 2, 3 (NT = 512) in the A tile, which is dead once the
-      // gate MMA has been committed; group 0 adds them in a fixed order (deterministic bits)
-      float* sRed2 = reinterpret_cast<float*>(sA + 32768);      // behind the fc-weight block, before the observation chunks
-      auto finish_heads = [&]() {
-        if (NG == 2) {
-#pragma unroll
-          for (int j = 0; j < 8; ++j) lg[j] += sRed[row * 8 + j] + sBo[j];
-        } else {
-#pragma unroll
-          for (int j = 0; j < 8; ++j)
-            lg[j] = ((lg[j] + sRed[row * 8 + j]) + (sRed2[row * 8 + j] + sRed2[(TC_M + row) * 8 + j])) + sBo[j];
-        }
-        if ((u & 1) == 0) {
-          float mx = -1e30f;
-#pragma unroll
-          for (int j = 0; j < 8; ++j) if (j < na) mx = fmaxf(mx, lg[j]);
-          float s = 0.f;
-#pragma unroll
-          for (int j = 0; j < 8; ++j) { lg[j] = j < na ? __expf(lg[j] - mx) : 0.f; s += lg[j]; }
-          const float inv = 1.0f / s;
-          float* po = a.pi + ((int64_t)r * d.A + ag) * d.max_na;
-#pragma unroll
-          for (int j = 0; j < 8; ++j) if (j < d.max_na) po[j] = lg[j] * inv;
-          if (a.act) {
-            uint32_t hsh = pmix32(a.seed_lo ^ (a.step * 0x9E3779B1U));
-            hsh = pmix32(hsh ^ a.seed_hi ^ ((uint32_t)(a.replica0 + r) * 0x85EBCA77U));
-            hsh = pmix32(hsh ^ ((uint32_t)ag * 0xC2B2AE3DU));
-            const float uu = (float)(hsh >> 8) * (1.0f / 16777216.0f);
-            float cum = 0.f;
-            int pick = na - 1;
-            bool found = false;
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-              if (j < na) { cum += lg[j] * inv; if (!found && uu < cum) { pick = j; found = true; } }
-            a.act[(int64_t)r * d.A + ag] = pick;
-          }
-        } else {
-          a.val[(int64_t)r * d.A + ag] = lg[0];
-        }
-      };
-#pragma unroll
-      for (int jb = 0; jb < HPT / 16; ++jb) {
-        float zi[16], zf[16], zo[16], zu[16];
-        const uint32_t tbase = ((uint32_t)(q * 32) << 16) + (uint32_t)(half * HPT + jb * 16);
-        acc_ld16(acc, tbase, zi); acc_ld16(acc, tbase + 64, zf); acc_ld16(acc, tbase + 128, zo); acc_ld16(acc, tbase + 192, zu);
-        if (a.zdbg && valid) {
-          float* z = a.zdbg + ((int64_t)u * ld + r) * TC_N + half * HPT + jb * 16;
-#pragma unroll
-          for (int e = 0; e < 16; ++e) { z[e] = zi[e]; z[64 + e] = zf[e]; z[128 + e] = zo[e]; z[192 + e] = zu[e]; }
-        }
-        float cprev[16];
-        if constexpr (NT == 512) {
-#pragma unroll
-          for (int e = 0; e < 16; ++e) cprev[e] = cpre[e];
-        } else if (valid && !a.done) {
-          const float4* cp = reinterpret_cast<const float4*>(a.c_in + srow + jb * 16);
-#pragma unroll
-          for (int e4 = 0; e4 < 4; ++e4) {
-            const float4 x = cp[e4];
-            cprev[4 * e4] = x.x; cprev[4 * e4 + 1] = x.y; cprev[4 * e4 + 2] = x.z; cprev[4 * e4 + 3] = x.w;
-          }
-        } else {
-#pragma unroll
-          for (int e = 0; e < 16; ++e) cprev[e] = 0.f;
-        }
-        float cn[16], hn[16];
-        __align__(16) __nv_bfloat16 gbuf[4][16];
-#pragma unroll
-        for (int e = 0; e < 16; ++e) {
-          const int j = half * HPT + jb * 16 + e;
-          const float gi = sigm(zi[e] + sBias[j]), gf = sigm(zf[e] + sBias[64 + j]);
-          const float go = sigm(zo[e] + sBias[128 + j]), gu = tanh_fast(zu[e] + sBias[192 + j]);
-          cn[e] = gf * cprev[e] + gi * gu;
-          hn[e] = go * tanh_fast(cn[e]);
-          gbuf[0][e] = __float2bfloat16_rn(gi); gbuf[1][e] = __float2bfloat16_rn(gf);
-          gbuf[2][e] = __float2bfloat16_rn(go); gbuf[3][e] = __float2bfloat16_rn(gu);
-#pragma unroll
-          for (int jj = 0; jj < 8; ++jj) lg[jj] = fmaf(hn[e], sWo[j * 8 + jj], lg[jj]);
-        }
-        if constexpr (NT == 512) {
-          // Stores: a thread owns (row, 16 hidden units), i.e. 32-byte pieces of its row.  They leave as pairs of 128-bit stores
-          // (one full 32-byte sector per thread) straight from the registers, interleaved with the
-          // other warps' cell math.  Alternatives: a SIMT copy-out through XOR-swizzled shared memory (coalesced, but 4
-          // staging passes with 8 block-wide barriers) or the same passes handed to the copy engine row by row.
-          auto st32 = [](void* p, const void* v) {
-            const uint4 x = reinterpret_cast<const uint4*>(v)[0], y = reinterpret_cast<const uint4*>(v)[1];
-            reinterpret_cast<uint4*>(p)[0] = x; reinterpret_cast<uint4*>(p)[1] = y;
-          };
-          if (valid) {
-            if (a.st_g) {
-              const int64_t m = store_row(row);
-#pragma unroll
-              for (int g = 0; g < 4; ++g) st32(a.st_g + m * TC_N + g * 64 + half * HPT, &gbuf[g][0]);
-              __align__(32) __nv_bfloat16 cb[16], hb[16];
-#pragma unroll
-              for (int e = 0; e < 16; ++e) { cb[e] = __float2bfloat16_rn(cn[e]); hb[e] = __float2bfloat16_rn(hn[e]); }
-              st32(a.st_c + m * TC_H + half * HPT, cb);
-              st32(a.st_h + m * TC_H + half * HPT, hb);
+            for (int e4 = 0; e4 < 4; ++e4) {
+              const float4 v = reinterpret_cast<const float4*>(a.c_in + srow)[e4];
+              cprev[4 * e4] = v.x; cprev[4 * e4 + 1] = v.y; cprev[4 * e4 + 2] = v.z; cprev[4 * e4 + 3] = v.w;
             }
-            float* co = a.c_out + srow;
-            float* ho = a.h_out + srow;
-            st32(co, cn); st32(co + 8, cn + 8);
-            st32(ho, hn); st32(ho + 8, hn + 8);
-          }
-        } else {
-        if (valid && a.st_g) {
-          const int64_t m = store_row((int)(r - r0));
-          const int jo = half * HPT + jb * 16;
+          } else {
 #pragma unroll
-          for (int g = 0; g < 4; ++g) {
-            uint4* o = reinterpret_cast<uint4*>(a.st_g + m * TC_N + g * 64 + jo);
-            o[0] = *reinterpret_cast<const uint4*>(&gbuf[g][0]); o[1] = *reinterpret_cast<const uint4*>(&gbuf[g][8]);
+            for (int e = 0; e < 16; ++e) cprev[e] = 0.f;
           }
-          __align__(16) __nv_bfloat16 cb[16], hb[16];
+          // fragment entry of (this row, hidden unit 16 q + e) in a gate's fragment
+#define GF(gate, e) g[gate][4 * ((e) >> 1) + 2 * hr + ((e) & 1)]
+          if (a.zdbg && valid) {
+            float* z = a.zdbg + ((int64_t)u * ld + r) * TC_N + 16 * q;
 #pragma unroll
-          for (int e = 0; e < 16; ++e) { cb[e] = __float2bfloat16_rn(cn[e]); hb[e] = __float2bfloat16_rn(hn[e]); }
-          uint4* oc = reinterpret_cast<uint4*>(a.st_c + m * TC_H + jo);
-          uint4* oh = reinterpret_cast<uint4*>(a.st_h + m * TC_H + jo);
-          oc[0] = *reinterpret_cast<const uint4*>(cb); oc[1] = *reinterpret_cast<const uint4*>(cb + 8);
-          oh[0] = *reinterpret_cast<const uint4*>(hb); oh[1] = *reinterpret_cast<const uint4*>(hb + 8);
-        }
-        if (valid) {
-          float4* co = reinterpret_cast<float4*>(a.c_out + srow + jb * 16);
-          float4* ho = reinterpret_cast<float4*>(a.h_out + srow + jb * 16);
+            for (int e = 0; e < 16; ++e) { z[e] = GF(0, e); z[64 + e] = GF(1, e); z[128 + e] = GF(2, e); z[192 + e] = GF(3, e); }
+          }
+          float lg[8];
 #pragma unroll
-          for (int e4 = 0; e4 < 4; ++e4) {
-            co[e4] = make_float4(cn[4 * e4], cn[4 * e4 + 1], cn[4 * e4 + 2], cn[4 * e4 + 3]);
-            ho[e4] = make_float4(hn[4 * e4], hn[4 * e4 + 1], hn[4 * e4 + 2], hn[4 * e4 + 3]);
+          for (int j = 0; j < 8; ++j) lg[j] = 0.f;
+          // bf16 gates / c / h packed in pairs as they are produced; the fp32 state leaves 4 units at a time
+          uint32_t gw[4][8], cw[8], hw[8];
+          float cn[4], hn[4];
+          const bool st_row = valid && a.st_g;
+          const int64_t m = st_row ? store_row(row) : 0;
+#pragma unroll
+          for (int e = 0; e < 16; ++e) {
+            const int j = 16 * q + e;
+            const float gi = sigm(GF(0, e) + sBias[j]), gf = sigm(GF(1, e) + sBias[64 + j]);
+            const float go = sigm(GF(2, e) + sBias[128 + j]), gu = tanh_fast(GF(3, e) + sBias[192 + j]);
+            const float c1 = gf * cprev[e] + gi * gu;
+            const float h1 = go * tanh_fast(c1);
+            cn[e & 3] = c1; hn[e & 3] = h1;
+            const float gv[4] = {gi, gf, go, gu};
+#pragma unroll
+            for (int gg = 0; gg < 4; ++gg) bf16_pack(gw[gg][e >> 1], gv[gg], e & 1);
+            bf16_pack(cw[e >> 1], c1, e & 1);
+            bf16_pack(hw[e >> 1], h1, e & 1);
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) lg[jj] = fmaf(h1, sWo[j * 8 + jj], lg[jj]);
+            if ((e & 3) == 3 && valid) {
+              reinterpret_cast<float4*>(a.c_out + srow)[e >> 2] = make_float4(cn[0], cn[1], cn[2], cn[3]);
+              reinterpret_cast<float4*>(a.h_out + srow)[e >> 2] = make_float4(hn[0], hn[1], hn[2], hn[3]);
+            }
+            if ((e & 7) == 7 && st_row) {      // 16-byte halves of the 32-byte pieces
+              const int hv = e >> 3;
+#pragma unroll
+              for (int gg = 0; gg < 4; ++gg)
+                reinterpret_cast<uint4*>(a.st_g + m * TC_N + gg * 64 + 16 * q)[hv] =
+                    make_uint4(gw[gg][4 * hv], gw[gg][4 * hv + 1], gw[gg][4 * hv + 2], gw[gg][4 * hv + 3]);
+              reinterpret_cast<uint4*>(a.st_c + m * TC_H + 16 * q)[hv] = make_uint4(cw[4 * hv], cw[4 * hv + 1], cw[4 * hv + 2], cw[4 * hv + 3]);
+              reinterpret_cast<uint4*>(a.st_h + m * TC_H + 16 * q)[hv] = make_uint4(hw[4 * hv], hw[4 * hv + 1], hw[4 * hv + 2], hw[4 * hv + 3]);
+            }
+          }
+#undef GF
+          // head sums over the quad's four 16-unit groups as ((g0 + g1) + (g2 + g3)) + bo (fp32 addition commutes, so
+          // every lane ends with the same bits); lane q = hr finishes the row
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            lg[j] += __shfl_xor_sync(0xffffffffu, lg[j], 1);
+            lg[j] += __shfl_xor_sync(0xffffffffu, lg[j], 2);
+            lg[j] += sBo[j];
+          }
+          if (q == hr && valid) {
+            if ((u & 1) == 0) {
+              float mx = -1e30f;
+#pragma unroll
+              for (int j = 0; j < 8; ++j) if (j < na) mx = fmaxf(mx, lg[j]);
+              float sm = 0.f;
+#pragma unroll
+              for (int j = 0; j < 8; ++j) { lg[j] = j < na ? __expf(lg[j] - mx) : 0.f; sm += lg[j]; }
+              const float inv = 1.0f / sm;
+              float* po = a.pi + ((int64_t)r * d.A + ag) * d.max_na;
+#pragma unroll
+              for (int j = 0; j < 8; ++j) if (j < d.max_na) po[j] = lg[j] * inv;
+              if (a.act) {
+                uint32_t hsh = pmix32(a.seed_lo ^ (a.step * 0x9E3779B1U));
+                hsh = pmix32(hsh ^ a.seed_hi ^ ((uint32_t)(a.replica0 + r) * 0x85EBCA77U));
+                hsh = pmix32(hsh ^ ((uint32_t)ag * 0xC2B2AE3DU));
+                const float uu = (float)(hsh >> 8) * (1.0f / 16777216.0f);
+                float cum = 0.f;
+                int pick = na - 1;
+                bool found = false;
+#pragma unroll
+                for (int j = 0; j < 8; ++j)
+                  if (j < na) { cum += lg[j] * inv; if (!found && uu < cum) { pick = j; found = true; } }
+                a.act[(int64_t)r * d.A + ag] = pick;
+              }
+            } else {
+              a.val[(int64_t)r * d.A + ag] = lg[0];
+            }
           }
         }
-        }
+        PROF_MARK(5);    // cell + stores + heads
       }
-      if (half == 1) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) sRed[row * 8 + j] = lg[j];
-      } else if (half > 1) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) sRed2[((half - 2) * TC_M + row) * 8 + j] = lg[j];
-      }
-      __syncthreads();
-      PROF_MARK(5);    // cell + stores + head partial sums
-      if (half == 0 && valid) finish_heads();
+      seg = seg_hi;
     }
   }
-  PROF_MARK(6);        // head softmax / sampling of the last item
-  if (PROF && tid == 0)
-    for (int i = 0; i < 16; ++i) atomicAdd(a.prof + i, (unsigned long long)pt[i]);
 #undef PROF_MARK
-  __syncthreads();
 }
 
 static size_t tc2_smem_bytes(int K) {
   const int KC = K / 8;
-  return (size_t)KC * 4096 + tc2_a_bytes(K) + (TC_M * 8 + TC_H * 8 + 8 + TC_N + TC_N) * 4 + 32;
+  return (size_t)KC * 4096 + (size_t)2 * KC * 1024 + (TC_H * 8 + 8 + TC_N + TC_N) * 4 + 4 * sizeof(uint64_t);
 }
 
 static unsigned long long* g_policy_prof = nullptr;
-// tools only: device pointer to 8 uint64 counters that receive per-phase clock64 sums of the v2 kernel (NULL = off)
+// tools only: device pointer to 16 uint64 counters that receive per-phase clock64 sums of the v2 kernel (NULL = off)
 extern "C" int tscl_debug_policy_prof(void* counters_dev) { g_policy_prof = (unsigned long long*)counters_dev; return 0; }
 static unsigned long long* g_bptt_prof = nullptr;
 extern "C" int tscl_debug_bptt_prof(void* counters_dev) { g_bptt_prof = (unsigned long long*)counters_dev; return 0; }
@@ -1055,38 +1010,34 @@ extern "C" int tscl_policy_step_v2r(tscl_handle* h, const float* params, const v
   PCK(cudaSetDevice(tscl_device_of(h)));
   const DDimsTC& d = *tscl_dims_of(h);
   const int K = d.dx + TC_H;
-  if ((d.dx % 32) != 0 || d.dx > 256) return tsc_set_error("tscl_policy_step_v2r: dx must be a multiple of 32, <= 256");
+  if (!P2_DX_OK(d.dx)) return tsc_set_error("tscl_policy_step_v2r: no kernel for this dx (160, 192 or 224)");
   if (d.kw == 0) return tsc_set_error("tscl_policy_step_v2r: observation slice does not fit the 64-column input tile");
-  if (8 * d.dx * 16 > (d.dx / 8) * 2048) return tsc_set_error("tscl_policy_step_v2r: fc operand does not fit its staging region");
-  const bool wide_tile = d.dx <= 224;   // NT = 512: the A-tile region doubles as the copy-out staging (X pitch dx * 2 + 16 <= 464 B)
   const size_t smem = tc2_smem_bytes(K);
   if (smem > 232448) return tsc_set_error("tscl_policy_step_v2r: operand tiles exceed shared memory");
+  void (*kern)(const DDimsTC, const StepTC) = nullptr;
+  const bool prof = g_policy_prof != nullptr;
+#define P2_CASE(n) case n: kern = prof ? policy_step_tc2_kernel<n, true> : policy_step_tc2_kernel<n, false>; break;
+  switch (d.dx) { P2_CASE(160) P2_CASE(192) P2_CASE(224) }
+#undef P2_CASE
   static int attr_dev = -1;
-  if (attr_dev != tscl_device_of(h)) {
-    PCK(cudaFuncSetAttribute(policy_step_tc2_kernel<256, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    PCK(cudaFuncSetAttribute(policy_step_tc2_kernel<512, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    PCK(cudaFuncSetAttribute(policy_step_tc2_kernel<512, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_dev = tscl_device_of(h);
+  static void (*attr_kern)(const DDimsTC, const StepTC) = nullptr;
+  if (attr_dev != tscl_device_of(h) || attr_kern != kern) {
+    PCK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 232448));
+    attr_dev = tscl_device_of(h); attr_kern = kern;
   }
   int n_sm = 0;
   PCK(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, tscl_device_of(h)));
-  const int64_t n_items = ((R + TC_M - 1) / TC_M) * 2 * d.A;
+  const int64_t n_items = ((R + P2_ROWS - 1) / P2_ROWS) * 2 * d.A;
   const int grid = (int)(n_items < n_sm ? n_items : n_sm);
   StepTC a;
-  a.acc = acc_tiles(h, stream);
-  if (!a.acc) return tsc_set_error("accumulator tiles: cudaMalloc failed");
+  a.acc = nullptr;
   a.P = params; a.Wp = (const __nv_bfloat16*)wpack_bf16; a.obs = obs; a.c_in = c_in; a.h_in = h_in; a.c_out = c_out;
   a.h_out = h_out; a.pi = pi; a.val = val; a.act = act; a.zdbg = zdbg; a.R = R; a.done = done; a.swap_lbo_sbo = 0;
   a.seed_lo = (uint32_t)seed; a.seed_hi = (uint32_t)(seed >> 32); a.step = (uint32_t)step; a.replica0 = replica0;
   a.st_x = (__nv_bfloat16*)st_x; a.st_g = (__nv_bfloat16*)st_g; a.st_c = (__nv_bfloat16*)st_c; a.st_h = (__nv_bfloat16*)st_h;
   a.t = t; a.T = T > 0 ? T : 1; a.rc = rc > 0 ? rc : R; a.ld = ld_state; a.row0 = ld_state > 0 ? row0 : 0;
   a.prof = g_policy_prof;
-  // 512 threads (thread = row and 16 hidden units) where the copy-out staging fits the A-tile region, else 256;
-  // TSC_POLICY_THREADS=256 selects the 256-thread mapping for experiments
-  static const int pol_threads = []() { const char* e = getenv("TSC_POLICY_THREADS"); return e && atoi(e) == 256 ? 256 : 512; }();
-  if (a.prof && wide_tile) policy_step_tc2_kernel<512, true><<<grid, 512, smem, (cudaStream_t)stream>>>(d, a);
-  else if (pol_threads == 512 && wide_tile) policy_step_tc2_kernel<512, false><<<grid, 512, smem, (cudaStream_t)stream>>>(d, a);
-  else policy_step_tc2_kernel<256, false><<<grid, 256, smem, (cudaStream_t)stream>>>(d, a);
+  kern<<<grid, P2_THREADS, smem, (cudaStream_t)stream>>>(d, a);
   PCK(cudaGetLastError());
   return 0;
 }

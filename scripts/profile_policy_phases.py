@@ -13,8 +13,10 @@ from deeprl_signal_control_b200.net.large_grid import build_large_grid
 R = int(sys.argv[1]) if len(sys.argv) > 1 else 8192
 net = build_large_grid(agent="ma2c")
 lay = PolicyLayout(net.n_s_ls, net.n_a_ls, net.n_w_ls, net.n_f_ls, net.node_obs_off, net.n_obs, fw=128, ft=32, ff=64, h=64)
-names = ["item top (sync, per-unit weights)", "staging (fc weights + obs slice)", "MMA0 + wait", "relu epilogue + h staging",
-         "gate MMA + wait", "head partial sums + rest of epilogue", "head softmax (last item)"]
+# consumer 0 (items of even parity) and the producer warpgroup, thread 0 of each
+names = ["consumer: unit constants", "consumer: wait for staged operands", "consumer: MMA0 + wait",
+         "consumer: relu epilogue, h staging, st_x", "consumer: gate MMA + wait", "consumer: cell, stores, heads"]
+pnames = ["producer: unit constants", "producer: wait for a free tile", "producer: fc copy + obs staging"]
 for store in (True, False):
     m = BatchedA2C(lay, R, n_step=8, seed=1, store_acts=store)
     obs = torch.rand(R, lay.n_obs, device="cuda")
@@ -30,14 +32,11 @@ for store in (True, False):
         m.forward(obs, False)
     torch.cuda.synchronize()
     lib.tscl_debug_policy_prof(None)
-    n_cta = min(((R + 127) // 128) * 2 * lay.A, torch.cuda.get_device_properties(0).multi_processor_count)
+    n_cta = min(((R + 63) // 64) * 2 * lay.A, torch.cuda.get_device_properties(0).multi_processor_count)
     pa = prof.cpu().numpy().astype(float) / n / n_cta
-    p = pa[:7]
-    tot = pa.sum()
-    print("activation store %s: %.0f cycles per CTA per launch" % (store, tot))
-    for nm, v in zip(names, p):
-        print("   %-36s %9.0f cycles  %5.1f %%" % (nm, v, 100 * v / tot))
+    for who, nm_list, p in (("consumer 0", names, pa[:6]), ("producer", pnames, pa[8:11])):
+        tot = p.sum()
+        print("activation store %s, %s: %.0f cycles per CTA per launch" % (store, who, tot))
+        for nm, v in zip(nm_list, p):
+            print("   %-42s %9.0f cycles  %5.1f %%" % (nm, v, 100 * v / tot))
     del m
-    for nm, v in zip(["  epilogue: accumulator loads + cell math", "  epilogue: X copy-out", "  epilogue: gates copy-out",
-                      "  epilogue: c / h fp32 state copy-out", "  epilogue: c | h bf16 copy-out"], pa[8:13]):
-        print("   %-36s %9.0f cycles  %5.1f %%" % (nm, v, 100 * v / tot))
