@@ -1,0 +1,268 @@
+"""`Evaluator`: test-mode evaluation of a trained policy (or the greedy controller) on the device, every test seed at
+once — the batched counterpart of reference utils.py:Tester.perform / Evaluator.run (utils.py:195-234, 311-388).
+
+    Evaluator(env, model, output_path, demo=False, policy_type='default', seed=None).run()
+
+`env` is a scenario env (LargeGridEnv, RealNetEnv, ...) built with `n_replicas == env.test_num`: replica k plays the
+episode the one-replica env plays after `reset(test_ind=k)` (seed `test_seeds[k]`, test-mode rewards), and in record
+mode `output_data()` writes the control / traffic / trip CSVs with the rows, in the order, that the one-replica env
+writes when it runs the seeds one after another.  `model` is an IA2C / MA2C wrapper (agents/models.py; only its
+parameters `batched.P` and the packed image `batched.Wp` are read) or a greedy controller (`model.name == 'greedy'`).
+
+Per control step, with no host synchronisation inside the episode: the pi-only forward (tscl_policy_step_pi for the
+fused tensor-core widths; the v1 forward or the fc-policy kernels, then tscl_argmax_actions, otherwise) or
+tsc_greedy_actions; for MA2C the fingerprint is the pi just computed; tsc_step (tsc_step_record in record mode); the
+global reward goes into a [T][R] float32 trace.  The evaluator owns every buffer it writes, so a live learner's
+parameters, optimiser slot, recurrent states, rollout and counters are left as they were.
+"""
+from __future__ import annotations
+
+import ctypes as C
+import logging
+
+import numpy as np
+import torch
+
+from .. import _lib
+
+
+def _p(t):
+    return None if t is None else C.c_void_p(t.data_ptr())
+
+
+def replica_seeds(env):
+    """Replica k plays test episode k: the seed the one-replica env takes after reset(test_ind=k) in test mode (not the
+    `seed + r` mapping env.reset uses for n_replicas > 1)."""
+    return np.asarray(env.test_seeds, dtype=np.uint64)
+
+
+def control_frame(actions, greward, ci):
+    """Control rows of envs/env.py (the reference's `control_data`): actions [R][T][N] int, greward [R][T] float32;
+    replica k is episode k + 1."""
+    import pandas as pd
+    R, T = greward.shape
+    return pd.DataFrame({'episode': np.repeat(np.arange(1, R + 1), T),
+                         'time_sec': np.tile(np.arange(1, T + 1) * ci, R),
+                         'step': np.tile(np.arange(1, T + 1) * ci / ci, R),
+                         'action': [','.join(['%d' % a for a in row]) for row in actions.reshape(R * T, -1)],
+                         'reward': greward.reshape(-1).astype(np.float64)})
+
+
+def traffic_frame(stats):
+    """Traffic rows of envs/env.py `_record_traffic`: stats [R][S][8] float32 per simulated second (tsc_step_record
+    fields); departed / arrived are per-second differences of the cumulative counters."""
+    import pandas as pd
+    R, S, _ = stats.shape
+    dep, arr = stats[..., 1].astype(np.int64), stats[..., 2].astype(np.int64)
+    zero = np.zeros((R, 1), np.int64)
+    return pd.DataFrame({'episode': np.repeat(np.arange(1, R + 1), S), 'time_sec': np.tile(np.arange(1, S + 1), R),
+                         'number_total_car': stats[..., 0].astype(np.int64).reshape(-1),
+                         'number_departed_car': np.diff(dep, axis=1, prepend=zero).reshape(-1),
+                         'number_arrived_car': np.diff(arr, axis=1, prepend=zero).reshape(-1),
+                         'avg_wait_sec': stats[..., 3].astype(np.float64).reshape(-1),
+                         'avg_speed_mps': stats[..., 4].astype(np.float64).reshape(-1),
+                         'std_queue': stats[..., 6].astype(np.float64).reshape(-1),
+                         'avg_queue': stats[..., 5].astype(np.float64).reshape(-1)})
+
+
+def trip_frame(trips):
+    """Trip rows of envs/env.py `collect_tripinfo`: trips[k] = BatchedSim.trips(k) of episode k + 1."""
+    import pandas as pd
+    if sum(len(t) for t in trips) == 0:
+        return pd.DataFrame([])                               # what the env writes when no vehicle arrived
+    ep = np.concatenate([np.full(len(t), k + 1, np.int64) for k, t in enumerate(trips)] + [np.zeros(0, np.int64)])
+    rows = np.concatenate([np.asarray(t, np.int64).reshape(-1, 5) for t in trips] + [np.zeros((0, 5), np.int64)])
+    dep, arr, route, wsec, wcnt = rows.T
+    return pd.DataFrame({'episode': ep, 'id': ['r%d.%d' % (r, d) for r, d in zip(route, dep)],
+                         'depart_sec': dep.astype(np.float64), 'arrival_sec': arr.astype(np.float64),
+                         'duration_sec': (arr - dep).astype(np.float64), 'wait_step': wcnt,
+                         'wait_sec': wsec.astype(np.float64)})
+
+
+class Evaluator:
+    def __init__(self, env, model, output_path, demo=False, policy_type='default', seed=None):
+        if policy_type not in ('default', 'stochastic', 'deterministic'):
+            raise ValueError("policy_type must be 'default', 'stochastic' or 'deterministic' (got %r)" % (policy_type,))
+        if env.n_replicas != env.test_num:
+            raise ValueError("the evaluator plays every test seed at once: build the env with n_replicas == test_num "
+                             "(%d), got %d" % (env.test_num, env.n_replicas))
+        self.env, self.model, self.output_path, self.demo = env, model, output_path, demo
+        self.policy_type = policy_type
+        self.agent = env.agent
+        self.seed = int(env.seed if seed is None else seed)
+        self.env.train_mode = False
+        self.test_num = env.test_num
+        sim = env._ensure_sim()
+        self.sim, self.R, self.dev = sim, sim.R, sim.device
+        net = env._tables
+        self.N, self.n_obs, self.max_na = net.n_nodes, net.n_obs, net.max_na
+        self.T = int(env.T)
+        self.ci = int(env.control_interval_sec)
+        name = getattr(model, 'name', None)
+        self.greedy = name == 'greedy'
+        self.fingerprint = name == 'ma2c'
+        f32 = dict(dtype=torch.float32, device=self.dev)
+        self.obs = torch.zeros(self.R, self.n_obs, **f32)
+        self.act = torch.zeros(self.R, self.N, dtype=torch.int32, device=self.dev)
+        self.reward = torch.zeros(self.R, self.N, **f32)
+        self.done = torch.zeros(self.R, dtype=torch.uint8, device=self.dev)
+        self.trace = torch.zeros(self.T, self.R, **f32)
+        self.act_trace = None
+        self.stats = None
+        self.recorded = None          # (control, traffic, trip) frames written by the last output_data()
+        if self.greedy:
+            prog = model.greedy_program(net.node_obs_off)
+            max_cand, off, idx, act = (int(prog[0]),) + tuple(np.ascontiguousarray(a, np.int32) for a in prog[1:])
+            _lib.check(_lib.lib().tsc_set_greedy_program(
+                sim._h, C.c_int32(max_cand), off.ctypes.data_as(C.POINTER(C.c_int32)),
+                idx.ctypes.data_as(C.POINTER(C.c_int32)), act.ctypes.data_as(C.POINTER(C.c_int32))))
+            return
+        b = getattr(model, 'batched', None)
+        if b is None or name not in ('ia2c', 'ma2c'):
+            raise ValueError("Evaluator: batched evaluation covers the greedy controller and IA2C / MA2C; %r stays on the "
+                             "one-replica protocol" % (name,))
+        L = b.lay
+        if L.n_obs != self.n_obs or not np.array_equal(L.obs_off, np.asarray(net.node_obs_off[:L.A])):
+            raise ValueError("Evaluator: the model's observation layout differs from the env's (build the model with "
+                             "obs_off=env node_obs_off)")
+        self.b, self.lay = b, L
+        if not L.recurrent:
+            self.family = 'fc'
+        elif not b.use_tc:
+            raise ValueError("Evaluator: the fp32 twin forward (use_tc=False) has no batched evaluation path; evaluate the "
+                             "tensor-core model")
+        else:
+            self.family = 'v2' if b.tc_v2 else 'v1'
+        self.pi = torch.zeros(self.R, L.A, L.max_na, **f32)
+        if self.family == 'v2':            # compact pi-unit state [A][R][h]
+            self.c = torch.zeros(L.A, self.R, L.h, **f32); self.h = torch.zeros_like(self.c)
+        else:
+            self.val = torch.zeros(self.R, L.A, **f32)
+            if self.family == 'v1':
+                self.c = torch.zeros(L.U, self.R, L.h, **f32); self.h = torch.zeros_like(self.c)
+            else:
+                self.X = torch.empty(L.U, self.R, L.dx, **f32); self.H = torch.empty(L.U, self.R, L.h, **f32)
+        if self.fingerprint:
+            u = torch.zeros(self.R, self.N, self.max_na, **f32)
+            for i, na in enumerate(L.n_a):
+                u[:, i, :na] = 1.0 / int(na)                          # envs/env.py:263-269
+            self.fp0 = u
+
+    def _st(self):
+        return C.c_void_p(torch.cuda.current_stream(self.dev).cuda_stream)
+
+    # ---- one decision for all replicas -----------------------------------------------------------
+    def _actions(self, step: int):
+        lib = _lib.lib()
+        if self.greedy:
+            _lib.check(lib.tsc_greedy_actions(self.sim._h, _p(self.obs), _p(self.act), self._st()))
+            return None
+        b, R, done = self.b, self.R, 1 if step == 0 else 0
+        argmax = self.policy_type == 'deterministic'
+        seed, stp = C.c_uint64(self.seed), C.c_int64(step)
+        if self.family == 'v2':
+            _lib.check(lib.tscl_policy_step_pi(b._h, _p(b.P), _p(b.Wp), _p(self.obs), C.c_int64(R), _p(self.c), _p(self.h),
+                                               _p(self.c), _p(self.h), _p(self.pi), _p(self.act), C.c_int32(int(argmax)),
+                                               C.c_int32(done), seed, stp, C.c_int64(0), C.c_int64(0), C.c_int64(0),
+                                               self._st()))
+            return self.pi
+        act = None if argmax else _p(self.act)
+        if self.family == 'v1':
+            _lib.check(lib.tscl_policy_step(b._h, _p(b.P), _p(b.Wp), _p(self.obs), C.c_int64(R), _p(self.c), _p(self.h),
+                                            _p(self.c), _p(self.h), _p(self.pi), _p(self.val), act, C.c_int32(done), seed,
+                                            stp, C.c_int64(0), None, C.c_int32(0), self._st()))
+        else:
+            _lib.check(lib.tscl_fc_embed(b._h, _p(b.P), _p(self.obs), C.c_int64(R), C.c_int64(R), C.c_int64(0), _p(self.X),
+                                         self._st()))
+            _lib.check(lib.tscl_fc_hidden_fwd(b._h, _p(b.P), _p(self.X), C.c_int64(R), _p(self.H), self._st()))
+            _lib.check(lib.tscl_heads(b._h, _p(b.P), _p(self.H), C.c_int64(R), _p(self.pi), _p(self.val), act, seed, stp,
+                                      C.c_int64(0), self._st()))
+        if argmax:
+            _lib.check(lib.tscl_argmax_actions(b._h, _p(self.pi), C.c_int64(R), _p(self.act), self._st()))
+        return self.pi
+
+    def _episode(self):
+        """All test seeds, one episode each (Tester.perform for every test_ind at once)."""
+        env, sim, lib = self.env, self.sim, _lib.lib()
+        record = bool(env.is_record)
+        sim.reset(replica_seeds(env))
+        sim.set_train_mode(False)
+        if record:
+            sim.set_record(True)
+            self.stats = torch.zeros(self.T, self.R, self.ci, 8, dtype=torch.float32, device=self.dev)
+            self.act_trace = torch.zeros(self.T, self.R, self.N, dtype=torch.int32, device=self.dev)
+        if not self.greedy and self.family != 'fc':
+            self.c.zero_(); self.h.zero_()
+        fp = self.fp0 if self.fingerprint else None
+        sim.observe(fp, obs_out=self.obs)
+        for t in range(self.T):
+            pi = self._actions(t)
+            fp = pi if self.fingerprint else None
+            if record:
+                _lib.check(lib.tsc_step_record(sim._h, _p(self.act), _p(fp), _p(self.obs), _p(self.reward),
+                                               _p(self.trace[t]), _p(self.done), _p(self.stats[t]), self._st()))
+                self.act_trace[t].copy_(self.act)
+            else:
+                _lib.check(lib.tsc_step(sim._h, _p(self.act), _p(fp), _p(self.obs), _p(self.reward), _p(self.trace[t]),
+                                        _p(self.done), self._st()))
+        env.cur_sec = self.T * self.ci
+
+    # ---- reference interface ----------------------------------------------------------------------
+    def perform_all(self):
+        """Batched Tester.perform: (mean_reward [R], std_reward [R]) float64, np.mean / np.std of each replica's
+        per-step global rewards (utils.py:230-234)."""
+        self._episode()
+        tr = self.trace.cpu().numpy()
+        cols = [np.array(tr[:, k], dtype=np.float64) for k in range(self.R)]
+        return np.array([np.mean(c) for c in cols]), np.array([np.std(c) for c in cols])
+
+    def run(self):
+        """Evaluator.run (utils.py:376-388): every test seed, then the CSVs when the env records."""
+        env = self.env
+        env.cur_episode = 0
+        if env.is_record:
+            env.init_data(True, env.record_stats, self.output_path)
+        mean, std = self.perform_all()
+        for k in range(self.R):
+            logging.info('test %i, avg reward %.2f' % (k, mean[k]))
+        env.cur_episode = self.R
+        if env.is_record:
+            self.output_data()
+        return mean, std
+
+    def summary(self, mean, std, traffic=None, trip=None):
+        """The quantities of the reference's recorded-evaluation table (BASELINE.md §1): mean and std over episodes of the
+        per-episode mean step reward; with the recorded frames also the means of avg_queue / avg_speed_mps /
+        avg_wait_sec over all recorded seconds and the completed trips per episode."""
+        out = {'scenario': self.env.name, 'agent': self.env.agent, 'policy_type': self.policy_type,
+               'seeds': [int(s) for s in self.env.test_seeds], 'episode_length_sec': int(self.env.episode_length_sec),
+               'episode_mean_reward': [float(x) for x in mean], 'episode_std_reward': [float(x) for x in std],
+               'mean_reward': float(np.mean(mean)), 'std_reward': float(np.std(mean))}
+        if traffic is not None:
+            out.update(avg_queue=float(traffic.avg_queue.mean()), avg_speed_mps=float(traffic.avg_speed_mps.mean()),
+                       avg_wait_sec=float(traffic.avg_wait_sec.mean()))
+        if trip is not None:
+            ep = trip.episode.values.astype(np.int64) if len(trip) else np.zeros(0, np.int64)
+            n = np.bincount(ep, minlength=self.R + 1)[1:]
+            out.update(trips_per_episode=[int(x) for x in n], mean_trips=float(np.mean(n)))
+        return out
+
+    def frames(self):
+        """(control, traffic, trip) DataFrames of the last recorded episode set."""
+        R, T = self.R, self.T
+        control = control_frame(self.act_trace.permute(1, 0, 2).cpu().numpy(), self.trace.t().cpu().numpy(), self.ci)
+        traffic = traffic_frame(self.stats.permute(1, 0, 2, 3).reshape(R, T * self.ci, 8).cpu().numpy())
+        trip = trip_frame([self.sim.trips(k) for k in range(R)])
+        return control, traffic, trip
+
+    def output_data(self):
+        """The reference's three CSVs (envs/env.py output_data): <output_path><scenario>_<agent>_{control,traffic,trip}.csv"""
+        if not self.env.is_record or self.stats is None:
+            logging.error('Evaluator: no record to output!')
+            return None
+        control, traffic, trip = self.recorded = self.frames()
+        base = self.output_path + ('%s_%s_' % (self.env.name, self.env.agent))
+        control.to_csv(base + 'control.csv')
+        traffic.to_csv(base + 'traffic.csv')
+        trip.to_csv(base + 'trip.csv')
+        return control, traffic, trip

@@ -1242,3 +1242,28 @@ extern "C" int tscl_memcpy_async(tscl_handle* h, void* dst, const void* src, int
                       (cudaStream_t)stream));
   return 0;
 }
+
+// ------------------------------------------------------------------------------------------------
+// Deterministic (test-mode) action choice for the forwards that have no fused pi-only kernel (fc policy, v1 LSTM):
+// act[r][a] = the FIRST j < n_a[a] with the largest pi[r][a][j], i.e. np.argmax on the float32 policy the reference hands
+// to the host (utils.py:213,220).  One thread per (replica, agent).
+__global__ void argmax_actions_kernel(const DDims d, const float* __restrict__ pi, int64_t RA, int32_t* __restrict__ act) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= RA) return;
+  const int na = d.n_a[i % d.A];
+  const float* p = pi + i * d.max_na;
+  float best = p[0];
+  int pick = 0;
+  for (int j = 1; j < na; ++j)
+    if (p[j] > best) { best = p[j]; pick = j; }
+  act[i] = pick;
+}
+
+extern "C" int tscl_argmax_actions(tscl_handle* h, const float* pi, int64_t R, int32_t* act, void* stream) {
+  if (!h || !pi || !act || R <= 0) return tsc_set_error("tscl_argmax_actions: bad argument");
+  LCK(cudaSetDevice(h->device));
+  const int64_t RA = R * h->d.A;
+  argmax_actions_kernel<<<(unsigned)((RA + 255) / 256), 256, 0, (cudaStream_t)stream>>>(h->d, pi, RA, act);
+  LCK(cudaGetLastError());
+  return 0;
+}

@@ -300,6 +300,7 @@ struct StepTC {
   // store is indexed by the absolute replica row0 + r; every pointer is the base of the range's slice
   int64_t ld, row0;
   unsigned long long* prof;   // optional: per-phase clock64 sums of thread 0 of every CTA (tools/profile only)
+  int act_mode;               // pi-only instantiation: 0 = counter-RNG sample, 1 = first argmax of pi
 };
 
 extern __shared__ __align__(1024) unsigned char tc_smem[];
@@ -577,8 +578,8 @@ extern "C" int tscl_policy_step(tscl_handle* h, const float* params, const void*
   const size_t smem = tc_smem_bytes(K);
   if (smem > 232448) return tsc_set_error("tscl_policy_step: operand tiles exceed shared memory");
   static int attr_dev = -1;
-  if (attr_dev != tscl_device_of(h)) {
-    PCK(cudaFuncSetAttribute(policy_step_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  if (attr_dev != tscl_device_of(h)) {      // the largest opt-in, so that a later handle with a wider dx can launch too
+    PCK(cudaFuncSetAttribute(policy_step_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 232448));
     attr_dev = tscl_device_of(h);
   }
   int n_sm = 0;
@@ -639,7 +640,11 @@ __host__ __device__ inline int gate_col(int n) {
 
 // DX = d.dx: the fragment sizes and the k loops are compile-time.  Instantiated for the fc widths of the shipped
 // configurations (P2_DX_OK): 224 (grid MA2C), 192 (Monaco), 160 (IA2C: no fingerprint block)
-template <int DX, bool PROF>
+// EVAL: the pi-only forward of test-mode evaluation (tscl_policy_step_pi).  Work items are (pi unit u = 2 * agent, 64 rows),
+// n_tiles * A of them; V units are never loaded, multiplied or stored.  The recurrent state is compact, [A][ld][h] (row
+// (u >> 1) * ld + r); there is no activation store, no zdbg and no value output.  Per element the arithmetic is the
+// training instantiation's, so pi, c and h are bit-identical to its pi units.
+template <int DX, bool PROF, bool EVAL>
 __global__ void __launch_bounds__(P2_THREADS, 1)
 policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
   const int tid = threadIdx.x, wg = tid >> 7, lane = tid & 31;
@@ -662,7 +667,7 @@ policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
   __syncthreads();
   const int64_t n_tiles = (a.R + P2_ROWS - 1) / P2_ROWS;
   const int64_t ld = a.ld > 0 ? a.ld : a.R;
-  const int64_t n_items = n_tiles * 2 * d.A;
+  const int64_t n_items = n_tiles * (EVAL ? 1 : 2) * d.A;
   const int64_t it_lo = n_items * blockIdx.x / gridDim.x, it_hi = n_items * (blockIdx.x + 1) / gridDim.x;
 
   // phase clocks of the producer's thread 0 and consumer 0's thread 0, added straight into the counters (no register
@@ -706,8 +711,8 @@ policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
     const int warp = tid >> 5;
     uint32_t ph_empty = 0;
     for (int64_t seg = it_lo; seg < it_hi;) {
-      const int u = (int)(seg / n_tiles), ag = u >> 1;
-      const int64_t seg_hi = (int64_t)(u + 1) * n_tiles < it_hi ? (int64_t)(u + 1) * n_tiles : it_hi;
+      const int ui = (int)(seg / n_tiles), u = EVAL ? 2 * ui : ui, ag = u >> 1;   // ui: item block = state unit
+      const int64_t seg_hi = (int64_t)(ui + 1) * n_tiles < it_hi ? (int64_t)(ui + 1) * n_tiles : it_hi;
       load_unit(u, false);
       PROF_MARK(8);      // producer: unit constants
       const int nw = d.n_wave[ag], nt = d.n_wait[ag], nf = d.ff > 0 ? d.n_fp[ag] : 0, ooff = d.obs_off[ag];
@@ -721,7 +726,7 @@ policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
       const __nv_bfloat16* Wfc = a.Wp + (int64_t)u * wp_stride(DX) + (int64_t)KC * TC_N * 8;
       for (int64_t it = seg; it < seg_hi; ++it) {
         const int s = (int)((it - it_lo) & 1);
-        const int64_t r0 = (it - (int64_t)u * n_tiles) * P2_ROWS;
+        const int64_t r0 = (it - (int64_t)ui * n_tiles) * P2_ROWS;
         unsigned char* sA = sA0 + (size_t)s * KC * 1024;
         const uint32_t full = smem_u32(sBar + s), empty = smem_u32(sBar + 2 + s);
         mbar_wait(empty, ((ph_empty >> s) & 1) ^ 1);       // the tile's previous item has left it (first use: passes)
@@ -739,7 +744,7 @@ policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
             const int64_t so = ((int64_t)un * ld + rn) * TC_H + (tid >> 6) * 32;
             asm volatile("prefetch.global.L2 [%0];" ::"l"(a.c_in + so));
             asm volatile("prefetch.global.L2 [%0];" ::"l"(a.h_in + so));
-            asm volatile("prefetch.global.L2 [%0];" ::"l"(a.obs + rn * d.n_obs + d.obs_off[un >> 1] + (tid >> 6) * 32));
+            asm volatile("prefetch.global.L2 [%0];" ::"l"(a.obs + rn * d.n_obs + d.obs_off[EVAL ? un : un >> 1] + (tid >> 6) * 32));
           }
         }
         // observation slice: warp w takes rows 16 w .. 16 w + 15, lane l the input slots 2l, 2l + 1 of each (the slice of
@@ -776,13 +781,13 @@ policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
     const uint32_t aA = smem_u32(sA), full = smem_u32(sBar + c), empty = smem_u32(sBar + 2 + c);
     uint32_t ph_full = 0;
     for (int64_t seg = it_lo; seg < it_hi;) {
-      const int u = (int)(seg / n_tiles), ag = u >> 1;
-      const int64_t seg_hi = (int64_t)(u + 1) * n_tiles < it_hi ? (int64_t)(u + 1) * n_tiles : it_hi;
+      const int ui = (int)(seg / n_tiles), u = EVAL ? 2 * ui : ui, ag = u >> 1;   // ui: item block = state unit
+      const int64_t seg_hi = (int64_t)(ui + 1) * n_tiles < it_hi ? (int64_t)(ui + 1) * n_tiles : it_hi;
       load_unit(u, true);
       PROF_MARK(0);      // unit constants
       const int na = d.n_a[ag];
       for (int64_t it = seg + (((seg - it_lo) & 1) != c ? 1 : 0); it < seg_hi; it += 2) {
-        const int64_t r0 = (it - (int64_t)u * n_tiles) * P2_ROWS;
+        const int64_t r0 = (it - (int64_t)ui * n_tiles) * P2_ROWS;
         // row of the activation store (chunk-outermost [R/rc][2A][T][rc][w]) for tile row `row`
         const int64_t st_c0 = (a.row0 + r0) / a.rc, st_rin0 = (a.row0 + r0) - st_c0 * a.rc;
         auto store_row = [&](int row) -> int64_t {
@@ -829,7 +834,7 @@ policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
         {
           const int64_t r = r0 + (ct & 63);
           const bool live = r < a.R && !a.done;
-          const float4* hp = reinterpret_cast<const float4*>(a.h_in + ((int64_t)u * ld + (r < a.R ? r : 0)) * TC_H + (ct >> 6) * 32);
+          const float4* hp = reinterpret_cast<const float4*>(a.h_in + ((int64_t)ui * ld + (r < a.R ? r : 0)) * TC_H + (ct >> 6) * 32);
 #pragma unroll
           for (int i = 0; i < 8; ++i) hpre[i] = live ? hp[i] : make_float4(0.f, 0.f, 0.f, 0.f);
         }
@@ -846,7 +851,7 @@ policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
         else asm volatile("bar.sync 2, 128;" ::: "memory");
         // st_x out of the tile, 32 bytes of a row per thread (the 8 lanes of a quarter-warp read 8 rows of one chunk
         // pair: no bank conflicts)
-        if (a.st_x) {
+        if (!EVAL && a.st_x) {
           constexpr int np = DX / 16;
 #pragma unroll 2
           for (int p = ct; p < P2_ROWS * np; p += 128) {
@@ -885,7 +890,7 @@ policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
           const int row = rq + 8 * hr;
           const int64_t r = r0 + row;
           const bool valid = r < a.R;
-          const int64_t srow = ((int64_t)u * ld + (valid ? r : 0)) * TC_H + 16 * q;
+          const int64_t srow = ((int64_t)ui * ld + (valid ? r : 0)) * TC_H + 16 * q;
           float cprev[16];      // c_{t-1} of (row, hidden units 16 q ..), prefetched to L2 by the producer
           if (valid && !a.done) {
 #pragma unroll
@@ -899,7 +904,7 @@ policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
           }
           // fragment entry of (this row, hidden unit 16 q + e) in a gate's fragment
 #define GF(gate, e) g[gate][4 * ((e) >> 1) + 2 * hr + ((e) & 1)]
-          if (a.zdbg && valid) {
+          if (!EVAL && a.zdbg && valid) {
             float* z = a.zdbg + ((int64_t)u * ld + r) * TC_N + 16 * q;
 #pragma unroll
             for (int e = 0; e < 16; ++e) { z[e] = GF(0, e); z[64 + e] = GF(1, e); z[128 + e] = GF(2, e); z[192 + e] = GF(3, e); }
@@ -910,7 +915,7 @@ policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
           // bf16 gates / c / h packed in pairs as they are produced; the fp32 state leaves 4 units at a time
           uint32_t gw[4][8], cw[8], hw[8];
           float cn[4], hn[4];
-          const bool st_row = valid && a.st_g;
+          const bool st_row = !EVAL && valid && a.st_g;
           const int64_t m = st_row ? store_row(row) : 0;
 #pragma unroll
           for (int e = 0; e < 16; ++e) {
@@ -951,7 +956,7 @@ policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
             lg[j] += sBo[j];
           }
           if (q == hr && valid) {
-            if ((u & 1) == 0) {
+            if (EVAL || (u & 1) == 0) {
               float mx = -1e30f;
 #pragma unroll
               for (int j = 0; j < 8; ++j) if (j < na) mx = fmaxf(mx, lg[j]);
@@ -962,7 +967,14 @@ policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
               float* po = a.pi + ((int64_t)r * d.A + ag) * d.max_na;
 #pragma unroll
               for (int j = 0; j < 8; ++j) if (j < d.max_na) po[j] = lg[j] * inv;
-              if (a.act) {
+              if (EVAL && a.act && a.act_mode == 1) {      // first maximum of the pi values written above (np.argmax)
+                float best = lg[0] * inv;
+                int pick = 0;
+#pragma unroll
+                for (int j = 1; j < 8; ++j)
+                  if (j < na && lg[j] * inv > best) { best = lg[j] * inv; pick = j; }
+                a.act[(int64_t)r * d.A + ag] = pick;
+              } else if (a.act) {
                 uint32_t hsh = pmix32(a.seed_lo ^ (a.step * 0x9E3779B1U));
                 hsh = pmix32(hsh ^ a.seed_hi ^ ((uint32_t)(a.replica0 + r) * 0x85EBCA77U));
                 hsh = pmix32(hsh ^ ((uint32_t)ag * 0xC2B2AE3DU));
@@ -975,7 +987,7 @@ policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
                   if (j < na) { cum += lg[j] * inv; if (!found && uu < cum) { pick = j; found = true; } }
                 a.act[(int64_t)r * d.A + ag] = pick;
               }
-            } else {
+            } else if (!EVAL) {
               a.val[(int64_t)r * d.A + ag] = lg[0];
             }
           }
@@ -1016,7 +1028,7 @@ extern "C" int tscl_policy_step_v2r(tscl_handle* h, const float* params, const v
   if (smem > 232448) return tsc_set_error("tscl_policy_step_v2r: operand tiles exceed shared memory");
   void (*kern)(const DDimsTC, const StepTC) = nullptr;
   const bool prof = g_policy_prof != nullptr;
-#define P2_CASE(n) case n: kern = prof ? policy_step_tc2_kernel<n, true> : policy_step_tc2_kernel<n, false>; break;
+#define P2_CASE(n) case n: kern = prof ? policy_step_tc2_kernel<n, true, false> : policy_step_tc2_kernel<n, false, false>; break;
   switch (d.dx) { P2_CASE(160) P2_CASE(192) P2_CASE(224) }
 #undef P2_CASE
   static int attr_dev = -1;
@@ -1037,6 +1049,7 @@ extern "C" int tscl_policy_step_v2r(tscl_handle* h, const float* params, const v
   a.st_x = (__nv_bfloat16*)st_x; a.st_g = (__nv_bfloat16*)st_g; a.st_c = (__nv_bfloat16*)st_c; a.st_h = (__nv_bfloat16*)st_h;
   a.t = t; a.T = T > 0 ? T : 1; a.rc = rc > 0 ? rc : R; a.ld = ld_state; a.row0 = ld_state > 0 ? row0 : 0;
   a.prof = g_policy_prof;
+  a.act_mode = 0;
   kern<<<grid, P2_THREADS, smem, (cudaStream_t)stream>>>(d, a);
   PCK(cudaGetLastError());
   return 0;
@@ -1049,6 +1062,47 @@ extern "C" int tscl_policy_step_v2(tscl_handle* h, const float* params, const vo
                                    void* stream) {
   return tscl_policy_step_v2r(h, params, wpack_bf16, obs, R, c_in, h_in, c_out, h_out, pi, val, act, done, seed, step, replica0,
                               zdbg, st_x, st_g, st_c, st_h, t, T, rc, 0, 0, stream);
+}
+
+extern "C" int tscl_policy_step_pi(tscl_handle* h, const float* params, const void* wpack_bf16, const float* obs, int64_t R,
+                                   const float* c_in, const float* h_in, float* c_out, float* h_out, float* pi, int32_t* act,
+                                   int32_t act_mode, int32_t done, uint64_t seed, int64_t step, int64_t replica0,
+                                   int64_t ld_state, int64_t row0, void* stream) {
+  if (!h || !params || !wpack_bf16 || !obs || !c_in || !h_in || !c_out || !h_out || !pi || R <= 0)
+    return tsc_set_error("tscl_policy_step_pi: bad argument");
+  if (act_mode != 0 && act_mode != 1) return tsc_set_error("tscl_policy_step_pi: act_mode must be 0 (sample) or 1 (argmax)");
+  if (ld_state > 0 && (row0 < 0 || row0 + R > ld_state)) return tsc_set_error("tscl_policy_step_pi: replica range outside [0, ld_state)");
+  PCK(cudaSetDevice(tscl_device_of(h)));
+  const DDimsTC& d = *tscl_dims_of(h);
+  if (!P2_DX_OK(d.dx)) return tsc_set_error("tscl_policy_step_pi: no kernel for this dx (160, 192 or 224)");
+  if (d.kw == 0) return tsc_set_error("tscl_policy_step_pi: observation slice does not fit the 64-column input tile");
+  const size_t smem = tc2_smem_bytes(d.dx + TC_H);
+  if (smem > 232448) return tsc_set_error("tscl_policy_step_pi: operand tiles exceed shared memory");
+  void (*kern)(const DDimsTC, const StepTC) = nullptr;
+  switch (d.dx) {
+    case 160: kern = policy_step_tc2_kernel<160, false, true>; break;
+    case 192: kern = policy_step_tc2_kernel<192, false, true>; break;
+    case 224: kern = policy_step_tc2_kernel<224, false, true>; break;
+  }
+  static int attr_dev = -1;
+  static void (*attr_kern)(const DDimsTC, const StepTC) = nullptr;
+  if (attr_dev != tscl_device_of(h) || attr_kern != kern) {
+    PCK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 232448));
+    attr_dev = tscl_device_of(h); attr_kern = kern;
+  }
+  int n_sm = 0;
+  PCK(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, tscl_device_of(h)));
+  const int64_t n_items = ((R + P2_ROWS - 1) / P2_ROWS) * d.A;
+  const int grid = (int)(n_items < n_sm ? n_items : n_sm);
+  StepTC a{};
+  a.P = params; a.Wp = (const __nv_bfloat16*)wpack_bf16; a.obs = obs; a.c_in = c_in; a.h_in = h_in; a.c_out = c_out;
+  a.h_out = h_out; a.pi = pi; a.act = act; a.R = R; a.done = done;
+  a.seed_lo = (uint32_t)seed; a.seed_hi = (uint32_t)(seed >> 32); a.step = (uint32_t)step; a.replica0 = replica0;
+  a.t = 0; a.T = 1; a.rc = R; a.ld = ld_state; a.row0 = ld_state > 0 ? row0 : 0;
+  a.act_mode = act_mode;
+  kern<<<grid, P2_THREADS, smem, (cudaStream_t)stream>>>(d, a);
+  PCK(cudaGetLastError());
+  return 0;
 }
 
 // ===================================================================================================

@@ -940,6 +940,9 @@ struct tsc_handle {
   unsigned long long* d_scalar = nullptr;
   int n_nodes = 0, n_obs = 0, max_na = 0, n_det = 0;
   int meas_words = 0;
+  // greedy program (tsc_set_greedy_program): CSR over (node, candidate) of observation offsets + action per candidate
+  int gp_max_cand = 0;
+  int32_t* d_gp_off = nullptr; int32_t* d_gp_idx = nullptr; int32_t* d_gp_act = nullptr;
 };
 
 template <class T>
@@ -1084,6 +1087,7 @@ extern "C" int tsc_destroy(tsc_handle* h) {
   if (!h) return 0;
   cudaSetDevice(h->device);
   for (void* p : h->owned) cudaFree(p);
+  cudaFree(h->d_gp_off); cudaFree(h->d_gp_idx); cudaFree(h->d_gp_act);
   delete h;
   return 0;
 }
@@ -1322,6 +1326,68 @@ extern "C" int tsc_get_traffic_stats(tsc_handle* h, float* stats_dev, void* stre
   const DevNet& d = h->args.net;
   tsc_stats_kernel<<<h->R, 128, (2 * d.n_lanes + 1) * 4, (cudaStream_t)stream>>>(d, h->args.veh, h->args.lane_cnt,
                                                                                    h->args.ctl, h->args.ctl_words, stats_dev, 8);
+  CK(cudaGetLastError());
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------------------
+// Greedy controllers (reference envs/large_grid_env.py:45-60, envs/real_net_env.py:78-111, envs/small_grid_env.py:41-57):
+// per node, every candidate phase scores the sum of a fixed list of that node's observation entries, accumulated in
+// float64 in list order (the reference sums float64 copies of the observation), and the FIRST maximum wins (np.argmax).
+// One thread per (replica, node).
+__global__ void tsc_greedy_kernel(const float* __restrict__ obs, int32_t* __restrict__ action, int64_t RN, int n_nodes,
+                                  int n_obs, int max_cand, const int32_t* __restrict__ off, const int32_t* __restrict__ idx,
+                                  const int32_t* __restrict__ act) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= RN) return;
+  const int64_t r = i / n_nodes;
+  const int node = (int)(i - r * n_nodes);
+  const float* o = obs + r * n_obs;
+  double best = 0.0;
+  int pick = 0;
+  bool any = false;
+  for (int c = 0; c < max_cand; ++c) {
+    const int k = node * max_cand + c;
+    if (act[k] < 0) continue;             // padding: the node has fewer candidates
+    double s = 0.0;
+    for (int e = off[k]; e < off[k + 1]; ++e) s += (double)o[idx[e]];
+    if (!any || s > best) { best = s; pick = act[k]; any = true; }
+  }
+  action[i] = pick;
+}
+
+extern "C" int tsc_set_greedy_program(tsc_handle* h, int32_t max_cand, const int32_t* off_host, const int32_t* idx_host,
+                                      const int32_t* act_host) {
+  if (!h || max_cand <= 0 || !off_host || !act_host) return fail("tsc_set_greedy_program: bad argument");
+  const int nk = h->n_nodes * max_cand;
+  if (off_host[0] != 0) return fail("tsc_set_greedy_program: off[0] must be 0");
+  for (int k = 0; k < nk; ++k)
+    if (off_host[k + 1] < off_host[k]) return fail("tsc_set_greedy_program: offsets must not decrease");
+  const int n_idx = off_host[nk];
+  if (n_idx > 0 && !idx_host) return fail("tsc_set_greedy_program: bad argument");
+  for (int e = 0; e < n_idx; ++e)
+    if (idx_host[e] < 0 || idx_host[e] >= h->n_obs) return fail("tsc_set_greedy_program: observation offset out of range");
+  CK(cudaSetDevice(h->device));
+  cudaFree(h->d_gp_off); cudaFree(h->d_gp_idx); cudaFree(h->d_gp_act);
+  h->d_gp_off = h->d_gp_idx = h->d_gp_act = nullptr;
+  h->gp_max_cand = 0;
+  CK(cudaMalloc(&h->d_gp_off, sizeof(int32_t) * (nk + 1)));
+  CK(cudaMalloc(&h->d_gp_idx, sizeof(int32_t) * (n_idx > 0 ? n_idx : 1)));
+  CK(cudaMalloc(&h->d_gp_act, sizeof(int32_t) * nk));
+  CK(cudaMemcpy(h->d_gp_off, off_host, sizeof(int32_t) * (nk + 1), cudaMemcpyHostToDevice));
+  if (n_idx > 0) CK(cudaMemcpy(h->d_gp_idx, idx_host, sizeof(int32_t) * n_idx, cudaMemcpyHostToDevice));
+  CK(cudaMemcpy(h->d_gp_act, act_host, sizeof(int32_t) * nk, cudaMemcpyHostToDevice));
+  h->gp_max_cand = max_cand;
+  return 0;
+}
+
+extern "C" int tsc_greedy_actions(tsc_handle* h, const float* obs_dev, int32_t* action_dev, void* stream) {
+  if (!h || !obs_dev || !action_dev) return fail("tsc_greedy_actions: bad argument");
+  if (h->gp_max_cand <= 0) return fail("tsc_greedy_actions: no greedy program (call tsc_set_greedy_program)");
+  CK(cudaSetDevice(h->device));
+  const int64_t RN = (int64_t)h->R * h->n_nodes;
+  tsc_greedy_kernel<<<(unsigned)((RN + 127) / 128), 128, 0, (cudaStream_t)stream>>>(
+      obs_dev, action_dev, RN, h->n_nodes, h->n_obs, h->gp_max_cand, h->d_gp_off, h->d_gp_idx, h->d_gp_act);
   CK(cudaGetLastError());
   return 0;
 }

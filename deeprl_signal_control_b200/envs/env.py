@@ -27,6 +27,37 @@ DEFAULT_PORT = 8000
 REALNET_REWARD_NORM = 20     # envs/env.py:18
 
 
+def greedy_table(cands):
+    """CSR form of a greedy controller (tsc_set_greedy_program): cands[i] = list of (observation offsets, action) of node
+    i's candidate phases, in the controller's order.  Returns (max_cand, off, idx, act) int32 arrays; padding candidates
+    carry action -1."""
+    max_cand = max(len(c) for c in cands)
+    off, idx, act = [0], [], []
+    for node in cands:
+        for c in range(max_cand):
+            entries, a = node[c] if c < len(node) else ([], -1)
+            idx.extend(int(e) for e in entries)
+            off.append(len(idx))
+            act.append(int(a))
+    return (max_cand, np.asarray(off, np.int32), np.asarray(idx, np.int32), np.asarray(act, np.int32))
+
+
+def green_lane_entries(node, phases, green, base):
+    """[(observation offsets, action)] of a node's phases: the detector entry of every lane whose signal is in `green`,
+    each lane counted once (envs/real_net_env.py:90-111)."""
+    out = []
+    for a, phase in enumerate(phases):
+        entries, seen = [], set()
+        for i, signal in enumerate(phase):
+            if signal in green:
+                ild = node.lanes_in[i]
+                if ild not in seen:
+                    entries.append(base + node.ilds_in.index(ild))
+                    seen.add(ild)
+        out.append((entries, a))
+    return out
+
+
 class PhaseSet:              # envs/env.py:20-39
     def __init__(self, phases):
         self.num_phase = len(phases)
@@ -195,6 +226,12 @@ class TrafficSimulator:
                                       'std_queue': float(st[6]), 'avg_queue': float(st[5])})
             self._n_dep_prev, self._n_arr_prev = dep, arr
 
+    def _record_control(self, action, greward):
+        self.control_data.append({'episode': self.cur_episode, 'time_sec': self.cur_sec,
+                                  'step': self.cur_sec / self.control_interval_sec,
+                                  'action': ','.join(['%d' % a for a in action]),
+                                  'reward': float(greward)})
+
     def collect_tripinfo(self):
         """Trip rows of the episode that just finished (the reference parses SUMO's --tripinfo-output,
         envs/env.py:498-515; here: the arrival log of replica 0, `tsc_get_trips`)."""
@@ -287,10 +324,7 @@ class TrafficSimulator:
         for name, a in zip(self.node_names, act[0]):
             self.nodes[name].prev_action = int(a)
         if self.is_record:
-            self.control_data.append({'episode': self.cur_episode, 'time_sec': self.cur_sec,
-                                      'step': self.cur_sec / self.control_interval_sec,
-                                      'action': ','.join(['%d' % a for a in act[0]]),
-                                      'reward': float(greward[0])})
+            self._record_control(act[0], greward[0])
         if self.n_replicas > 1:
             return obs.copy(), reward.copy(), bool(done[0]), greward.copy()
         reward0 = reward[0].astype(np.float64)

@@ -25,6 +25,15 @@ class LargeGridController:
     def greedy(self, ob, node_name):
         return int(self.forward([ob])[0])
 
+    # the five candidate phases of forward() as pairs of wave entries, candidate index = action
+    GREEDY_PAIRS = ((0, 3), (2, 5), (1, 4), (1, 2), (4, 5))
+
+    def greedy_program(self, node_obs_off):
+        """forward() as a table for tsc_greedy_actions (envs.env.greedy_table)."""
+        from .env import greedy_table
+        return greedy_table([[((node_obs_off[i] + a, node_obs_off[i] + b), c) for c, (a, b) in enumerate(self.GREEDY_PAIRS)]
+                             for i in range(len(self.node_names))])
+
 
 from .env import PhaseMap, PhaseSet, TrafficSimulator        # noqa: E402
 from ..net import large_grid as _grid                         # noqa: E402

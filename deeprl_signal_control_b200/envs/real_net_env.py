@@ -44,6 +44,13 @@ class RealNetController:
             flows.append(wave)
         return int(np.argmax(np.array(flows)))
 
+    def greedy_program(self, node_obs_off):
+        """greedy() as a table for tsc_greedy_actions (envs.env.greedy_table): per phase, the observation entries of its
+        'G' lanes, each lane once, in the order greedy() adds them."""
+        from .env import greedy_table, green_lane_entries
+        return greedy_table([green_lane_entries(self.nodes[name], PHASES[NODES[name][0]], 'G', node_obs_off[i])
+                             for i, name in enumerate(self.node_names)])
+
 
 class RealNetEnv(TrafficSimulator):
     """Drop-in for reference envs/real_net_env.py:114-136.  The net is parsed from

@@ -38,6 +38,13 @@ class SmallGridController:
         flows = np.asarray(ob)[..., :len(phases)]
         return np.asarray(phases)[np.argmax(flows, axis=-1)]
 
+    def greedy_program(self, node_obs_off):
+        """greedy() as a table for tsc_greedy_actions (envs.env.greedy_table): candidate c = wave entry c, mapped to
+        STATE_PHASE_MAP's phase."""
+        from .env import greedy_table
+        return greedy_table([[((node_obs_off[i] + c,), a) for c, a in enumerate(STATE_PHASE_MAP[name])]
+                             for i, name in enumerate(self.node_names)])
+
 
 class SmallGridEnv(TrafficSimulator):
     """Drop-in for reference envs/small_grid_env.py:60-84: `SmallGridEnv(config['ENV_CONFIG'], port=0, output_path='',

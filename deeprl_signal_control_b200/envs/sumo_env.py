@@ -59,3 +59,9 @@ class SumoNetController:
                 flows.append(wave)
             acts.append(int(np.argmax(flows)))
         return acts
+
+    def greedy_program(self, node_obs_off):
+        """forward() as a table for tsc_greedy_actions (envs.env.greedy_table): the 'G' / 'g' lanes of each phase."""
+        from .env import greedy_table, green_lane_entries
+        return greedy_table([green_lane_entries(self.nodes[name], self.phases[name], 'Gg', node_obs_off[i])
+                             for i, name in enumerate(self.node_names)])

@@ -180,6 +180,18 @@ int tsc_step_record(tsc_handle* h, const int32_t* action_dev, const float* fp_de
                     float* greward_dev, uint8_t* done_dev, float* sub_stats_dev, void* stream);
 int tsc_get_trips(tsc_handle* h, int32_t replica, uint32_t* rows_host, int32_t max_rows, int32_t* n_rows);
 
+/* ---- greedy controllers (reference envs/large_grid_env.py:45-60, envs/real_net_env.py:78-111,
+ * envs/small_grid_env.py:41-57) as one table-driven rule ------------------------------------------------------------
+ * tsc_set_greedy_program: per node i and candidate c < max_cand (k = i * max_cand + c), the candidate scores the sum of
+ *   the observation entries idx_host[off_host[k] .. off_host[k+1]) (offsets into the [n_obs] row) and maps to action
+ *   act_host[k] (-1: no such candidate).  off_host [n_nodes * max_cand + 1].  Host arrays, copied (synchronous).
+ * tsc_greedy_actions: action_dev int32 [R][n_nodes] = per node, the action of the FIRST candidate with the largest score,
+ *   scores summed in float64 in table order (np.argmax over the reference's float64 sums, ties included).
+ *   obs_dev float [R][n_obs]. */
+int tsc_set_greedy_program(tsc_handle* h, int32_t max_cand, const int32_t* off_host, const int32_t* idx_host,
+                           const int32_t* act_host);
+int tsc_greedy_actions(tsc_handle* h, const float* obs_dev, int32_t* action_dev, void* stream);
+
 /* Integer parity taps measured at the end of the last step, per detector lane
  * (lanearea.getLastStepVehicleNumber / getLastStepHaltingNumber / head getWaitingTime,
  * envs/env.py:333-349,377-395) and per node (the phase index = action applied).

@@ -221,6 +221,19 @@ int tscl_policy_step_v2r(tscl_handle* h, const float* params, const void* wpack_
                          int32_t* act, int32_t done, uint64_t seed, int64_t step, int64_t replica0, float* zdbg,
                          void* st_x, void* st_g, void* st_c, void* st_h, int32_t t, int32_t T, int64_t rc,
                          int64_t ld_state, int64_t row0, void* stream);
+/* pi-only form of the v2 forward for test-mode evaluation (reference utils.py:Evaluator, LstmACPolicy.forward(.., 'p')):
+ * the same kernel restricted to the A pi units (V units are never touched), bit-identical pi / c / h to the pi units of
+ * tscl_policy_step_v2.  State is compact: c_in/h_in/c_out/h_out [A][ld_state or R][h] (out may alias in); pi
+ * [R][A][max_na]; act [R][A] or NULL.  act_mode 0 = the counter-RNG sample of tscl_policy_step_v2 (seed, step,
+ * replica0 + r, agent); 1 = the first maximum of the written pi (np.argmax).  ld_state / row0: replica-range form as in
+ * tscl_policy_step_v2r (pointers are the range's slices); ld_state = 0: plain call. */
+int tscl_policy_step_pi(tscl_handle* h, const float* params, const void* wpack_bf16, const float* obs, int64_t R,
+                        const float* c_in, const float* h_in, float* c_out, float* h_out, float* pi, int32_t* act,
+                        int32_t act_mode, int32_t done, uint64_t seed, int64_t step, int64_t replica0, int64_t ld_state,
+                        int64_t row0, void* stream);
+/* Deterministic action choice for the forwards without a fused pi-only kernel (fc policy, v1 LSTM forward):
+ * act[r][a] = first j < n_a[a] with the largest pi[r][a][j]; pi [R][A][max_na], act [R][A]. */
+int tscl_argmax_actions(tscl_handle* h, const float* pi, int64_t R, int32_t* act, void* stream);
 /* st_x/st_g/st_c/st_h (all or none, may be NULL): bf16 activation store [R/rc][2A][T][rc][dx | 4h | h | h]
  * (replica-chunk major; rc must divide R) written at time index t — the relu'd fc outputs, the gate activations i,f,o,u, c_t and h_t — so that the update can
  * back-propagate through the rollout's own forward pass instead of recomputing it.

@@ -6,7 +6,8 @@ same episodes (reference utils.py:296-305: mean over the 720 control steps of th
 
 --fp32         plain fp32 learner kernels (no tensor cores, no bf16 activation store): the A/B partner of the default path
 --reward-norm  override MODEL_CONFIG.reward_norm (reference: 2000 for MA2C on the grid, config/config_ma2c_large.ini)
---greedy       no learning: the reference's greedy controller (envs/large_grid_env.py:56-60) on the same seeds
+--greedy       no learning: the reference's greedy controller (envs/large_grid_env.py:56-60, envs/real_net_env.py:78-111)
+               on the same seeds, through the batched evaluator (agents/evaluator.py)
 Writes $OUT/train_curve_<tag>.json (OUT defaults to results/).
 """
 import argparse
@@ -27,6 +28,47 @@ from deeprl_signal_control_b200.net.large_grid import build_large_grid
 from deeprl_signal_control_b200.net.tables import EnvParams
 from deeprl_signal_control_b200.sim import BatchedSim
 
+
+
+GREEDY_INI = {"grid": """
+[ENV_CONFIG]
+clip_wave = 2.0
+clip_wait = 2.0
+control_interval_sec = 5
+agent = greedy
+coop_gamma = 0.9
+data_path = ./large_grid/data/
+episode_length_sec = 3600
+norm_wave = 5.0
+norm_wait = 100.0
+coef_wait = 0.2
+peak_flow1 = 1100
+peak_flow2 = 925
+init_density = 0
+objective = hybrid
+scenario = large_grid
+seed = 12
+test_seeds = %s
+yellow_interval_sec = 2
+""", "real": """
+[ENV_CONFIG]
+clip_wave = 2.0
+clip_wait = 2.0
+control_interval_sec = 5
+agent = greedy
+coop_gamma = 0.9
+data_path = ./real_net/data/
+episode_length_sec = 3600
+norm_wave = 5.0
+norm_wait = 30.0
+coef_wait = 0
+flow_rate = 325
+objective = queue
+scenario = real_net
+seed = 12
+test_seeds = %s
+yellow_interval_sec = 2
+"""}
 
 
 def out_path(tag):
@@ -68,23 +110,26 @@ sim = BatchedSim(net, par, R)
 t0 = time.time()
 
 if a.greedy:
-    assert a.scenario == "grid", "greedy baseline: grid only"
-    sim.set_train_mode(True)
-    off = torch.tensor(net.node_obs_off[:net.n_nodes], device="cuda")
-    idx = (off[:, None] + torch.arange(6, device="cuda")[None, :]).reshape(-1)
+    # the batched evaluator's greedy path (tsc_greedy_actions) on the training seeds of every episode; the greedy agent's
+    # rewards are the same in train and test mode (local rewards, envs/env.py:591-594)
+    import configparser
+    from deeprl_signal_control_b200.agents.evaluator import Evaluator
+    cp = configparser.ConfigParser()
+    cp.read_string(GREEDY_INI[a.scenario] % ",".join(["0"] * R))
+    if a.scenario == "real":
+        from deeprl_signal_control_b200.envs.real_net_env import RealNetController, RealNetEnv
+        env = RealNetEnv(cp["ENV_CONFIG"], n_replicas=R)
+        ctrl = RealNetController(env.node_names, env.nodes)
+    else:
+        from deeprl_signal_control_b200.envs.large_grid_env import LargeGridController, LargeGridEnv
+        env = LargeGridEnv(cp["ENV_CONFIG"], n_replicas=R)
+        ctrl = LargeGridController(env.node_names)
+    ev = Evaluator(env, ctrl, "", policy_type="deterministic")
     curve = []
     for ep in range(a.episodes):
-        sim.reset(episode_seeds(12, ep, 0, R, R))
-        obs = sim.observe()
-        acc = torch.zeros(R, device="cuda")
-        for t in range(720):
-            o = obs[:, idx].reshape(R, net.n_nodes, 6)
-            flows = torch.stack([o[..., 0] + o[..., 3], o[..., 2] + o[..., 5], o[..., 1] + o[..., 4],
-                                 o[..., 1] + o[..., 2], o[..., 4] + o[..., 5]], -1)
-            act = flows.argmax(-1).to(torch.int32).contiguous()
-            obs, _, g, _ = sim.step(act)
-            acc += g
-        curve.append(float((acc / 720).mean()))
+        env.init_test_seeds([int(x) for x in episode_seeds(12, ep, 0, R, R)])
+        mean, _ = ev.perform_all()
+        curve.append(float(np.mean(mean)))
         print("greedy episode %3d  mean step reward %9.2f" % (ep + 1, curve[-1]), flush=True)
     json.dump({"agent": "greedy", "scenario": a.scenario, "replicas": R, "episodes": len(curve), "mean_episode_reward": curve,
                "wall_s": time.time() - t0}, open(out_path(tag), "w"))
