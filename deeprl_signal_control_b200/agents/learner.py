@@ -109,7 +109,8 @@ class BatchedA2C:
         self.Wt = torch.zeros(U, 32, L.h, 8, dtype=torch.bfloat16, device=self.dev)    # Wh^T image for the BPTT MMA
         self.Wxt = torch.zeros(U, 32, L.dx, 8, dtype=torch.bfloat16, device=self.dev)  # Wx^T image: dX fused into the BPTT
         # fusing dX into the BPTT step lengthens its serial per-step chain, so the default keeps dX as a separate
-        # product; `dx_fused = True` selects the fused kernel (tested)
+        # product; `dx_fused = True` selects the fused kernel (tests/test_update_bench_size_gpu.py: test_fused_dx_bptt,
+        # test_whole_update_matches_chunked_reference)
         self.dx_fused = False
         self.dx_fusable = self.use_tc and L.dx % 32 == 0 and L.dx <= 256
         # stand-alone dX = dZ . Wx^T kernel (tscl_dx_tc); False falls back to the library GEMM (A/B measurements only)

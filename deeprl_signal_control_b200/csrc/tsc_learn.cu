@@ -450,17 +450,29 @@ heads_loss_kernel(const DDims d, const float* __restrict__ P, const float* __res
       const float inv = 1.0f / s;
       const int at = act[io];
       const float adv = Adv[io];
-      float lp[8], ent = 0.f;
+      // log(clip(pi, 1e-10, 1)) (agents/policies.py:47) has zero derivative where the clip is active: a taken action
+      // with pi < 1e-10 contributes no policy gradient, and a clipped pi_k drops its "+1" from the entropy gradient
+      // beta * pi_j * (lp_j + m_j + ent - sum_k pi_k m_k),  m_k = [1e-10 <= pi_k <= 1],  written with
+      // sum_k pi_k m_k = 1 - clip_mass so that nothing changes when no pi is clipped
+      float lp[8], ent = 0.f, clip_mass = 0.f;
+      bool in_at = true;
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
         lg[j] *= inv;                                             // pi_j
         lp[j] = j < na ? __logf(fminf(fmaxf(lg[j], 1e-10f), 1.0f)) : 0.f;   // agents/policies.py:47
         ent -= lg[j] * lp[j];
+        const bool clipped = j < na && !(lg[j] >= 1e-10f && lg[j] <= 1.0f);
+        if (clipped) clip_mass += lg[j];
+        if (clipped && j == at) in_at = false;
       }
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
         float g = 0.f;
-        if (j < na) g = scale * (-adv * ((j == at ? 1.f : 0.f) - lg[j]) + beta * lg[j] * (lp[j] + ent));
+        if (j < na) {
+          const bool clipped = !(lg[j] >= 1e-10f && lg[j] <= 1.0f);
+          const float pg = in_at ? -adv * ((j == at ? 1.f : 0.f) - lg[j]) : 0.f;
+          g = scale * (pg + beta * lg[j] * (lp[j] + ent + clip_mass - (clipped ? 1.f : 0.f)));
+        }
         dl[j] = g;
       }
       if (dlog) {

@@ -25,17 +25,28 @@ def nstep_returns(rs, vs, dones_post, R, gamma):
     return np.array(Rs[::-1]), np.array(Advs[::-1])
 
 
-def unit_forward(v, lay, u, obs, dones, c, h):
-    """obs [T, R, n_obs] -> (pi or value [T, R, ...], H [T, R, h], final c, h).  float64 torch."""
+def _obs_blocks(lay, u, obs):
+    """(wave, wait, fingerprint) input slices of unit u."""
     a = u // 2
     o0 = int(lay.obs_off[a]); nw, nt, nf = int(lay.n_wave[a]), int(lay.n_wait[a]), int(lay.n_fp[a])
-    wave = obs[..., o0:o0 + nw]; wait = obs[..., o0 + nw:o0 + nw + nt]; fp = obs[..., o0 + nw + nt:o0 + nw + nt + nf]
+    return obs[..., o0:o0 + nw], obs[..., o0 + nw:o0 + nw + nt], obs[..., o0 + nw + nt:o0 + nw + nt + nf]
+
+
+def fc_front(v, lay, u, obs):
+    """x = concat(fcw, fcf, fct) of unit u (agents/policies.py:191-211)."""
+    wave, wait, fp = _obs_blocks(lay, u, obs)
     parts = [torch.relu(wave @ v["fcw_w%d" % u] + v["fcw_b%d" % u])]
     if lay.ff > 0:
         parts.append(torch.relu(fp @ v["fcf_w%d" % u] + v["fcf_b%d" % u]))
     if lay.ft > 0:
         parts.append(torch.relu(wait @ v["fct_w%d" % u] + v["fct_b%d" % u]))
-    x = torch.cat(parts, -1)
+    return torch.cat(parts, -1)
+
+
+def unit_forward(v, lay, u, obs, dones, c, h):
+    """obs [T, R, n_obs] -> (pi or value [T, R, ...], H [T, R, h], final c, h).  float64 torch."""
+    a = u // 2
+    x = fc_front(v, lay, u, obs)
     H = lay.h
     if not getattr(lay, "recurrent", True):      # FcACPolicy: one more fc layer instead of the LSTM
         Hs = torch.relu(x @ v["wx"][u] + v["bl"][u])
@@ -93,3 +104,190 @@ def clip_rmsprop(P, G, MS, agent_of, max_norm, lr, alpha, eps, n_agents):
         MS[m] = alpha * MS[m] + (1 - alpha) * g * g
         P[m] = P[m] - lr * g / np.sqrt(MS[m] + eps)
     return P, MS, norms
+
+
+# ------------------------------------------------------------------------------------------------
+# The update from the bf16 activation store (BatchedA2C.backward with use_tc and store_acts), in float64.
+# Per chunk of rc replicas starting at r0 the kernels read the store [U][T][rc][w] (X, gate activations i, f, o, u, c, h),
+# obs / actions / returns / advantages, the fp32 parameters, c_bw / h_bw rows r0 .. r0 + rc and done_pre, and run
+#   heads_loss -> BPTT (dZ) -> [X | Hp | 1]^T dZ and dX = dZ . Wx^T -> fc front-end gradients.
+# These functions take exactly those inputs and return float64 results.  With round_bf16 they round to bf16 where the
+# kernels do and nowhere else: the Wh / Wx operand images, dz before the recurrent product and as the dZ operand, dX as
+# stored, obs and h0 as GEMM operands.  round_bf16=False gives the exact gradient of a2c_loss through the same store.
+
+def bf16(x):
+    """Round to the nearest bf16 (ties to even) and back to x's dtype."""
+    return x.to(torch.bfloat16).to(x.dtype)
+
+
+def store_forward(v, lay, u, obs, dones, c0, h0):
+    """Float64 forward of unit u in the activation-store layout: obs [T, rc, n_obs], c0 / h0 [rc, h] ->
+    (X [T, rc, dx], gate activations [T, rc, 4h] in the order i, f, o, u, c [T, rc, h], h [T, rc, h])."""
+    x = fc_front(v, lay, u, obs)
+    H = lay.h
+    gs, cs, hs = [], [], []
+    c, h = c0, h0
+    for t in range(obs.shape[0]):
+        keep = 1.0 - float(dones[t])
+        c = c * keep; h = h * keep
+        z = x[t] @ v["wx"][u] + h @ v["wh"][u] + v["bl"][u]
+        g = torch.cat([torch.sigmoid(z[:, :3 * H]), torch.tanh(z[:, 3 * H:])], -1)
+        c = g[:, H:2 * H] * c + g[:, :H] * g[:, 3 * H:]
+        h = g[:, 2 * H:3 * H] * torch.tanh(c)
+        gs.append(g); cs.append(c); hs.append(h)
+    return x, torch.stack(gs), torch.stack(cs), torch.stack(hs)
+
+
+def heads_ref(lay, v, a, H_pi, H_v, act, Rs, Adv, scale, v_coef, beta):
+    """Loss gradients at the heads of agent a (tscl_heads_loss) over rows [M]: H_pi / H_v [M, h], act / Rs / Adv [M].
+    Returns dH_pi / dH_v [M, h], the head gradients wo_pi [h, n_a], bo_pi [n_a], wo_v [h], bo_v [] and the loss sums
+    (policy, value, entropy) times `scale` (BatchedA2C.stats for agent 0).  TF clip semantics:
+    d log(clip(p, 1e-10, 1)) / dp = 0 outside [1e-10, 1] (agents/policies.py:47)."""
+    na = int(lay.n_a[a])
+    Wp, bp = v["wo"][2 * a][:, :na], v["bo"][2 * a][:na]
+    wv, bv = v["wo"][2 * a + 1][:, 0], v["bo"][2 * a + 1][0]
+    val = H_v @ wv + bv
+    dv = scale * v_coef * (val - Rs)
+    pi = torch.softmax(H_pi @ Wp + bp, -1)
+    m = ((pi >= 1e-10) & (pi <= 1.0)).to(pi.dtype)
+    lp = torch.log(pi.clamp(1e-10, 1.0))
+    ent = -(pi * lp).sum(-1)
+    onehot = torch.nn.functional.one_hot(act.long(), na).to(pi.dtype)
+    m_at = (m * onehot).sum(-1)
+    dl = scale * (-(Adv * m_at)[:, None] * (onehot - pi)
+                  + beta * pi * (lp + m + ent[:, None] - (pi * m).sum(-1, keepdim=True)))
+    lp_at = (lp * onehot).sum(-1)
+    stats = scale * torch.stack([-(lp_at * Adv).sum(), 0.5 * v_coef * ((Rs - val) ** 2).sum(), -beta * ent.sum()])
+    return dict(dH_pi=dl @ Wp.T, dH_v=dv[:, None] * wv[None, :], wo_pi=H_pi.T @ dl, bo_pi=dl.sum(0), wo_v=H_v.T @ dv,
+                bo_v=dv.sum(), stats=stats)
+
+
+def bptt_ref(gates, c, c0, dH, dones, wh, round_bf16=True, c_prev=None):
+    """BPTT through the LSTM from stored activations, t = T-1 .. 0 (tscl_lstm_seq_bwd_tc).  gates [..., T, rc, 4h]
+    (i, f, o, u activated), c [..., T, rc, h], c0 [..., rc, h] (c_bw rows r0 .. r0 + rc), dH [..., T, rc, h],
+    wh [..., h, 4h]; the leading dimensions are units.  c_{t-1} and the carries into step t-1 are masked by
+    1 - done[t].  Returns dZ [..., T, rc, 4h] unrounded; the recurrent product is bf16(dz) . bf16(Wh)^T with round_bf16.
+    `c_prev` [..., T, rc, h] replaces (c0, c_0 .. c_{T-2}) as the previous cell state (tests use it to plant defects)."""
+    H, T = c.shape[-1], c.shape[-3]
+    whT = (bf16(wh) if round_bf16 else wh).transpose(-1, -2)
+    dZ = torch.empty_like(gates)
+    dc = torch.zeros_like(c0)
+    dhc = torch.zeros_like(c0)
+    for t in range(T - 1, -1, -1):
+        keep = 1.0 - float(dones[t])
+        g = gates[..., t, :, :]
+        i, f, o, u = g[..., :H], g[..., H:2 * H], g[..., 2 * H:3 * H], g[..., 3 * H:]
+        if c_prev is not None:
+            cp = c_prev[..., t, :, :] * keep
+        else:
+            cp = (c[..., t - 1, :, :] if t > 0 else c0) * keep
+        dh = dH[..., t, :, :] + dhc
+        tc = torch.tanh(c[..., t, :, :])
+        dcc = dc + dh * o * (1.0 - tc * tc)
+        dz = torch.cat([dcc * u * i * (1.0 - i), dcc * cp * f * (1.0 - f), dh * tc * o * (1.0 - o),
+                        dcc * i * (1.0 - u * u)], -1)
+        dZ[..., t, :, :] = dz
+        dc = dcc * f * keep
+        dhc = ((bf16(dz) if round_bf16 else dz) @ whT) * keep
+    return dZ
+
+
+def lstm_grads_ref(X, Hs, h0, dones, dZ, wx, round_bf16=True):
+    """LSTM weight gradients [X | Hp | 1]^T dZ and dX = dZ . Wx^T (tscl_wgrad_tc, tscl_dx_tc).  X [..., T, rc, dx],
+    Hs [..., T, rc, h] (store), h0 [..., rc, h] (h_bw rows r0 .. r0 + rc), dZ [..., T, rc, 4h], wx [..., dx, 4h].
+    Hp[t] = (1 - done[t]) * (h[t-1], or h0 at t = 0).  Returns (wx, wh, bl, dX [..., T, rc, dx])."""
+    keep = (1.0 - torch.as_tensor([float(d) for d in dones], dtype=X.dtype, device=X.device))[:, None, None]
+    h0r = bf16(h0) if round_bf16 else h0
+    Hp = torch.cat([h0r.unsqueeze(-3), Hs[..., :-1, :, :]], -3) * keep
+    Z = bf16(dZ) if round_bf16 else dZ
+    flat = lambda t_: t_.reshape(*t_.shape[:-3], -1, t_.shape[-1])
+    Zf = flat(Z)
+    gwx = flat(X).transpose(-1, -2) @ Zf
+    gwh = flat(Hp).transpose(-1, -2) @ Zf
+    dX = Z @ (bf16(wx) if round_bf16 else wx).transpose(-1, -2).unsqueeze(-3)
+    return gwx, gwh, Zf.sum(-2), (bf16(dX) if round_bf16 else dX)
+
+
+def fc_grads_ref(lay, u, obs, X, dX, round_bf16=True):
+    """fc front-end gradients of unit u (tscl_fc_bwd_tc): obs [T, rc, n_obs] (the chunk's rows), X / dX [T, rc, dx].
+    relu mask from X.  Returns {view name: gradient} for the fcw / fcf / fct weights and biases of u."""
+    wave, wait, fp = _obs_blocks(lay, u, bf16(obs) if round_bf16 else obs)
+    dd = (dX * (X > 0)).reshape(-1, lay.dx)
+    out = {}
+    for name, inp, c0, w in (("fcw", wave, 0, lay.fw), ("fcf", fp, lay.fw, lay.ff), ("fct", wait, lay.fw + lay.ff, lay.ft)):
+        if w == 0:
+            continue
+        d_ = dd[:, c0:c0 + w]
+        out["%s_w%d" % (name, u)] = inp.reshape(-1, inp.shape[-1]).T @ d_
+        out["%s_b%d" % (name, u)] = d_.sum(0)
+    return out
+
+
+def update_ref(lay, P, store, obs, act, Rs, Adv, c_bw, h_bw, dones, scale, v_coef, beta, chunk, round_bf16=True,
+               agents_per_group=None):
+    """Flat gradient G (float64) of one update from the activation store, summed over the chunks r0 = 0, chunk, ...
+    P: fp32 parameters (any float tensor); store(ci) -> (st_x, st_g, st_c, st_h) of chunk ci, each [U][T][rc][w];
+    obs [T, R, n_obs], act / Rs / Adv [T, R, A], c_bw / h_bw [U, R, h], dones = done_pre [T].  Work runs on P's device,
+    `agents_per_group` agents at a time (bounds the float64 working set).  Returns (G, agent-0 stats)."""
+    f64 = dict(dtype=torch.float64, device=P.device)
+    v = lay.views(P.to(torch.float64))
+    G = torch.zeros(lay.n_params, **f64)
+    gv = lay.views(G)
+    stats = torch.zeros(3, **f64)
+    T, R, A, hd = obs.shape[0], obs.shape[1], lay.A, lay.h
+    grp = agents_per_group or A
+    for ci, r0 in enumerate(range(0, R, chunk)):
+        rc = min(chunk, R - r0)
+        st = store(ci)
+        ob = obs[:, r0:r0 + rc].to(**f64)
+        for a0 in range(0, A, grp):
+            a1 = min(A, a0 + grp)
+            us = slice(2 * a0, 2 * a1)
+            X, Gt, Cs, Hs = (s[us].to(**f64) for s in st)
+            dH = torch.empty_like(Hs)
+            for a in range(a0, a1):
+                k = 2 * (a - a0)
+                hr = heads_ref(lay, v, a, Hs[k].reshape(-1, hd), Hs[k + 1].reshape(-1, hd),
+                               act[:, r0:r0 + rc, a].reshape(-1).to(P.device), Rs[:, r0:r0 + rc, a].reshape(-1).to(**f64),
+                               Adv[:, r0:r0 + rc, a].reshape(-1).to(**f64), scale, v_coef, beta)
+                dH[k] = hr["dH_pi"].reshape(T, rc, hd)
+                dH[k + 1] = hr["dH_v"].reshape(T, rc, hd)
+                na = int(lay.n_a[a])
+                gv["wo"][2 * a][:, :na] += hr["wo_pi"]
+                gv["bo"][2 * a][:na] += hr["bo_pi"]
+                gv["wo"][2 * a + 1][:, 0] += hr["wo_v"]
+                gv["bo"][2 * a + 1][0] += hr["bo_v"]
+                if a == 0:
+                    stats += hr["stats"]
+            c0 = c_bw[us, r0:r0 + rc].to(**f64)
+            h0 = h_bw[us, r0:r0 + rc].to(**f64)
+            dZ = bptt_ref(Gt, Cs, c0, dH, dones, v["wh"][us], round_bf16)
+            del dH, Gt, Cs
+            gwx, gwh, gbl, dX = lstm_grads_ref(X, Hs, h0, dones, dZ, v["wx"][us], round_bf16)
+            del dZ
+            gv["wx"][us] += gwx
+            gv["wh"][us] += gwh
+            gv["bl"][us] += gbl
+            for k, u in enumerate(range(us.start, us.stop)):
+                for name, g in fc_grads_ref(lay, u, ob, X[k], dX[k], round_bf16).items():
+                    gv[name] += g
+            del X, Hs, dX
+    return G, stats
+
+
+def bptt_mutations(gates, c, c_state, r0, dH, dones):
+    """Arguments of bptt_ref (without wh) for the correct chunk and for six planted defects of a BPTT kernel:
+    returns ({gates, c, c0, dH, dones}, {defect name: the same with the defect}).  c_state [..., R, h] is c_bw; the chunk
+    starts at replica r0 > 0."""
+    rc, H, T = c.shape[-2], c.shape[-1], len(dones)
+    ok = dict(gates=gates, c=c, c0=c_state[..., r0:r0 + rc, :], dH=dH, dones=[float(d) for d in dones])
+    swapped = torch.cat([gates[..., H:2 * H], gates[..., :H], gates[..., 2 * H:]], -1)
+    late = lambda x: torch.cat([torch.zeros_like(x[..., :1, :, :]), x[..., :-1, :, :]], -3)
+    return ok, {
+        "c0 from row r instead of r0 + r": dict(ok, c0=c_state[..., :rc, :]),
+        "done one step late": dict(ok, dones=[0.0] + ok["dones"][:-1]),
+        "done ignored": dict(ok, dones=[0.0] * T),
+        "i and f gates swapped": dict(ok, gates=swapped),
+        "c_t in place of c_{t-1}": dict(ok, c_prev=c),
+        "dH one step late": dict(ok, dH=late(dH)),
+    }
