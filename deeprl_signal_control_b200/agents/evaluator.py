@@ -7,10 +7,13 @@ once — the batched counterpart of reference utils.py:Tester.perform / Evaluato
 episode the one-replica env plays after `reset(test_ind=k)` (seed `test_seeds[k]`, test-mode rewards), and in record
 mode `output_data()` writes the control / traffic / trip CSVs with the rows, in the order, that the one-replica env
 writes when it runs the seeds one after another.  `model` is an IA2C / MA2C wrapper (agents/models.py; only its
-parameters `batched.P` and the packed image `batched.Wp` are read) or a greedy controller (`model.name == 'greedy'`).
+parameters `batched.P` and the packed image `batched.Wp` are read), an IQL (`model.name == 'iql'`, LR or DQN; only its
+`nets` are read, packed into the evaluator's own parameter vector at the start of every perform_all()) or a greedy
+controller (`model.name == 'greedy'`).
 
 Per control step, with no host synchronisation inside the episode: the pi-only forward (tscl_policy_step_pi for the
-fused tensor-core widths; the v1 forward or the fc-policy kernels, then tscl_argmax_actions, otherwise) or
+fused tensor-core widths; the v1 forward or the fc-policy kernels, then tscl_argmax_actions, otherwise), the fp32 Q
+forward tscl_q_step (IQL: argmax of q, or the normalised-q sample of IQL.forward(stochastic=True)) or
 tsc_greedy_actions; for MA2C the fingerprint is the pi just computed; tsc_step (tsc_step_record in record mode); the
 global reward goes into a [T][R] float32 trace.  The evaluator owns every buffer it writes, so a live learner's
 parameters, optimiser slot, recurrent states, rollout and counters are left as they were.
@@ -117,10 +120,13 @@ class Evaluator:
                 sim._h, C.c_int32(max_cand), off.ctypes.data_as(C.POINTER(C.c_int32)),
                 idx.ctypes.data_as(C.POINTER(C.c_int32)), act.ctypes.data_as(C.POINTER(C.c_int32))))
             return
+        if name == 'iql':
+            self._init_q(model, net)
+            return
         b = getattr(model, 'batched', None)
         if b is None or name not in ('ia2c', 'ma2c'):
-            raise ValueError("Evaluator: batched evaluation covers the greedy controller and IA2C / MA2C; %r stays on the "
-                             "one-replica protocol" % (name,))
+            raise ValueError("Evaluator: batched evaluation covers the greedy controller, IA2C / MA2C and IQL; %r stays on "
+                             "the one-replica protocol" % (name,))
         L = b.lay
         if L.n_obs != self.n_obs or not np.array_equal(L.obs_off, np.asarray(net.node_obs_off[:L.A])):
             raise ValueError("Evaluator: the model's observation layout differs from the env's (build the model with "
@@ -148,6 +154,29 @@ class Evaluator:
                 u[:, i, :na] = 1.0 / int(na)                          # envs/env.py:263-269
             self.fp0 = u
 
+    def _init_q(self, model, net):
+        """IQL (agents/models.py): LRQPolicy / DeepQPolicy networks on tscl_q_step."""
+        from .layout import QLayout
+        off = np.asarray(net.node_obs_off)
+        n_s = [int(off[i + 1] - off[i]) for i in range(self.N)]
+        if list(model.n_s_ls) != n_s or list(model.n_a_ls) != [int(a) for a in net.n_a_ls]:
+            raise ValueError("Evaluator: the model's observation layout differs from the env's (IQL n_s %s / n_a %s, env "
+                             "observation widths %s / n_a %s)" % (list(model.n_s_ls), list(model.n_a_ls), n_s,
+                                                                  list(net.n_a_ls)))
+        self.family = 'q'
+        self.qlay = QLayout.from_iql(model, off, self.n_obs, max_na=self.max_na)
+        self._qh = C.c_void_p()
+        _lib.check(_lib.lib().tscl_q_create(C.byref(self.qlay.as_c()), C.c_int32(self.dev.index or 0), C.byref(self._qh)))
+        self.params = torch.zeros(self.qlay.n_params, dtype=torch.float32, device=self.dev)
+        self.q = torch.zeros(self.R, self.N, self.max_na, dtype=torch.float32, device=self.dev)
+        self.bad = torch.full((1,), -1, dtype=torch.int64, device=self.dev)
+
+    def __del__(self):
+        h = getattr(self, '_qh', None)
+        if h is not None and h.value:
+            _lib.lib().tscl_q_destroy(h)
+            self._qh = None
+
     def _st(self):
         return C.c_void_p(torch.cuda.current_stream(self.dev).cuda_stream)
 
@@ -156,6 +185,11 @@ class Evaluator:
         lib = _lib.lib()
         if self.greedy:
             _lib.check(lib.tsc_greedy_actions(self.sim._h, _p(self.obs), _p(self.act), self._st()))
+            return None
+        if self.family == 'q':
+            _lib.check(lib.tscl_q_step(self._qh, _p(self.params), _p(self.obs), C.c_int64(self.R), _p(self.q),
+                                       _p(self.act), C.c_int32(int(self.policy_type == 'stochastic')),
+                                       C.c_uint64(self.seed), C.c_int64(step), C.c_int64(0), _p(self.bad), self._st()))
             return None
         b, R, done = self.b, self.R, 1 if step == 0 else 0
         argmax = self.policy_type == 'deterministic'
@@ -191,7 +225,7 @@ class Evaluator:
             sim.set_record(True)
             self.stats = torch.zeros(self.T, self.R, self.ci, 8, dtype=torch.float32, device=self.dev)
             self.act_trace = torch.zeros(self.T, self.R, self.N, dtype=torch.int32, device=self.dev)
-        if not self.greedy and self.family != 'fc':
+        if not self.greedy and self.family in ('v1', 'v2'):
             self.c.zero_(); self.h.zero_()
         fp = self.fp0 if self.fingerprint else None
         sim.observe(fp, obs_out=self.obs)
@@ -210,8 +244,20 @@ class Evaluator:
     # ---- reference interface ----------------------------------------------------------------------
     def perform_all(self):
         """Batched Tester.perform: (mean_reward [R], std_reward [R]) float64, np.mean / np.std of each replica's
-        per-step global rewards (utils.py:230-234)."""
+        per-step global rewards (utils.py:230-234).  IQL: the model's current weights are packed first (the model itself
+        is not written), and with policy_type 'stochastic' a row whose normalised q is not a distribution raises the
+        ValueError np.random.choice raises in the reference."""
+        q = not self.greedy and self.family == 'q'
+        if q:
+            self.params.copy_(self.qlay.pack(self.model.nets))
+            self.bad.fill_(-1)
         self._episode()
+        if q and self.policy_type == 'stochastic':
+            key = int(self.bad.item())
+            if key != -1:
+                r, step, agent = key >> 40, (key >> 16) & 0xFFFFFF, key & 0xFFFF
+                raise ValueError('probabilities are not non-negative: q / sum(q) of agent %d at control step %d of test '
+                                 'episode %d (seed %d)' % (agent, step, r, int(self.env.test_seeds[r])))
         tr = self.trace.cpu().numpy()
         cols = [np.array(tr[:, k], dtype=np.float64) for k in range(self.R)]
         return np.array([np.mean(c) for c in cols]), np.array([np.std(c) for c in cols])

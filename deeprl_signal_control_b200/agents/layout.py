@@ -29,6 +29,17 @@ class CDims(C.Structure):
                 ("off_wo", C.c_int64), ("off_bo", C.c_int64), ("n_params", C.c_int64)]
 
 
+class CQDims(C.Structure):
+    _fields_ = [("n_agents", C.c_int32), ("n_obs", C.c_int32), ("max_na", C.c_int32), ("model", C.c_int32),
+                ("n_fc", C.c_int32), ("n_ft", C.c_int32), ("n_h", C.c_int32),
+                ("obs_off", C.POINTER(C.c_int32)), ("n_s", C.POINTER(C.c_int32)), ("n_w", C.POINTER(C.c_int32)),
+                ("n_a", C.POINTER(C.c_int32)),
+                ("off_fcw_w", C.POINTER(C.c_int64)), ("off_fcw_b", C.POINTER(C.c_int64)),
+                ("off_fct_w", C.POINTER(C.c_int64)), ("off_fct_b", C.POINTER(C.c_int64)),
+                ("off_fc0_w", C.POINTER(C.c_int64)), ("off_fc0_b", C.POINTER(C.c_int64)),
+                ("off_q_w", C.POINTER(C.c_int64)), ("off_q_b", C.POINTER(C.c_int64)), ("n_params", C.c_int64)]
+
+
 def ortho_init(rng: np.random.RandomState, shape, scale=np.sqrt(2)):
     """agents/utils.py:11-24 (lasagne-style orthogonal init via SVD)."""
     a = rng.standard_normal(shape)
@@ -149,3 +160,102 @@ class PolicyLayout:
             n_out = int(self.n_a[a]) if u % 2 == 0 else 1
             v["wo"][u][:, :n_out] = ortho_init(rng, (self.h, n_out))
         return flat
+
+
+class QLayout:
+    """Flat fp32 parameter vector of the IQL Q networks (agents/policies.py:341-389), agent after agent, each agent's
+    tensors in the order q_fcw/w, q_fcw/b, q_fct/w, q_fct/b, q_fc_0/w, q_fc_0/b, q/w, q/b (dqn; q_fct only for n_w > 0)
+    or q/w, q/b (lr), every weight row-major [in][out] as `IQL.nets` holds it.  This is the `tscl_qdims` image the
+    test-mode Q kernel reads (include/tsc_learn.h)."""
+    OFF = {"q_fcw/w": "off_fcw_w", "q_fcw/b": "off_fcw_b", "q_fct/w": "off_fct_w", "q_fct/b": "off_fct_b",
+           "q_fc_0/w": "off_fc0_w", "q_fc_0/b": "off_fc0_b", "q/w": "off_q_w", "q/b": "off_q_b"}
+
+    def __init__(self, model_type: str, n_s_ls: Sequence[int], n_a_ls: Sequence[int], n_w_ls: Sequence[int],
+                 obs_off: Sequence[int], n_obs: int, n_fc: int = 0, n_ft: int = 0, n_h: int = 0, max_na: int | None = None):
+        if model_type not in ("lr", "dqn"):
+            raise ValueError("model_type must be 'lr' or 'dqn' (got %r)" % (model_type,))
+        self.model_type = model_type
+        self.A = len(n_s_ls)
+        self.n_s = np.asarray(n_s_ls, np.int32)
+        self.n_a = np.asarray(n_a_ls, np.int32)
+        self.n_w = np.asarray(n_w_ls, np.int32) if model_type == "dqn" else np.zeros(self.A, np.int32)
+        self.obs_off = np.asarray(obs_off, np.int32)[:self.A].copy()
+        self.n_obs = int(n_obs)
+        self.max_na = int(max_na or self.n_a.max())
+        dqn = model_type == "dqn"
+        self.n_fc, self.n_h = (int(n_fc), int(n_h)) if dqn else (0, 0)
+        self.n_ft = int(n_ft) if dqn and (self.n_w > 0).any() else 0
+        self.shapes = []                      # per agent: {name: shape} in flat order
+        for n in self.OFF.values():
+            setattr(self, n, np.zeros(self.A, np.int64))
+        off = 0
+        for i in range(self.A):
+            n_s, n_a, n_w = int(self.n_s[i]), int(self.n_a[i]), int(self.n_w[i])
+            if dqn:
+                shp = {"q_fcw/w": (n_s - n_w, self.n_fc), "q_fcw/b": (self.n_fc,)}
+                if n_w > 0:
+                    shp.update({"q_fct/w": (n_w, self.n_ft), "q_fct/b": (self.n_ft,)})
+                width = self.n_fc + (self.n_ft if n_w > 0 else 0)
+                shp.update({"q_fc_0/w": (width, self.n_h), "q_fc_0/b": (self.n_h,), "q/w": (self.n_h, n_a), "q/b": (n_a,)})
+            else:
+                shp = {"q/w": (n_s, n_a), "q/b": (n_a,)}
+            self.shapes.append(shp)
+            for k, s in shp.items():
+                getattr(self, self.OFF[k])[i] = off
+                off += int(np.prod(s))
+            for k, n in self.OFF.items():     # layers the agent lacks: zero length at the end of its block
+                if k not in shp:
+                    getattr(self, n)[i] = off
+        self.n_params = off
+
+    @classmethod
+    def from_iql(cls, model, obs_off, n_obs, max_na=None) -> "QLayout":
+        """The layout of an `agents/models.py:IQL`, with the widths read from its tensors (not from the config)."""
+        nets = model.nets
+        if model.model_type == "dqn":
+            n_fc = int(nets[0]["q_fcw/w"].shape[1])
+            n_h = int(nets[0]["q_fc_0/w"].shape[1])
+            with_t = [p for p in nets if "q_fct/w" in p]
+            n_ft = int(with_t[0]["q_fct/w"].shape[1]) if with_t else 0
+        else:
+            n_fc = n_ft = n_h = 0
+        lay = cls(model.model_type, model.n_s_ls, model.n_a_ls, model.n_w_ls, obs_off, n_obs, n_fc=n_fc, n_ft=n_ft,
+                  n_h=n_h, max_na=max_na)
+        for i, p in enumerate(nets):
+            got = {k: tuple(v.shape) for k, v in p.items()}
+            if got != {k: tuple(s) for k, s in lay.shapes[i].items()}:
+                raise ValueError("IQL agent %d: tensor shapes %s differ from the layout's %s" % (i, got, lay.shapes[i]))
+        return lay
+
+    def pack(self, nets):
+        """`IQL.nets` (a list of {name: tensor}) -> the flat float32 vector: a torch tensor on the tensors' device when
+        they are torch tensors (no host round trip), else a numpy array."""
+        parts = [nets[i][k] for i in range(self.A) for k in self.shapes[i]]
+        if parts and hasattr(parts[0], "detach"):
+            import torch
+            return torch.cat([t.detach().reshape(-1).to(torch.float32) for t in parts])
+        return np.concatenate([np.asarray(t, np.float32).reshape(-1) for t in parts]).astype(np.float32)
+
+    def views(self, flat):
+        """Per agent {name: view} into a flat vector (numpy or torch), the inverse of pack()."""
+        out = []
+        for i in range(self.A):
+            v = {}
+            for k, s in self.shapes[i].items():
+                o = int(getattr(self, self.OFF[k])[i])
+                v[k] = flat[o:o + int(np.prod(s))].reshape(s)
+            out.append(v)
+        return out
+
+    def as_c(self) -> CQDims:
+        c = CQDims()
+        c.n_agents, c.n_obs, c.max_na = self.A, self.n_obs, self.max_na
+        c.model = 1 if self.model_type == "dqn" else 0
+        c.n_fc, c.n_ft, c.n_h = self.n_fc, self.n_ft, self.n_h
+        for name in ("obs_off", "n_s", "n_w", "n_a"):
+            setattr(c, name, getattr(self, name).ctypes.data_as(C.POINTER(C.c_int32)))
+        for name in self.OFF.values():
+            setattr(c, name, getattr(self, name).ctypes.data_as(C.POINTER(C.c_int64)))
+        c.n_params = self.n_params
+        c._keep = self
+        return c

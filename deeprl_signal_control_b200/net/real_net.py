@@ -425,6 +425,8 @@ def real_net_tables(agent: str = 'ma2c', net_file: str | None = None, flow_rate:
     if net_file is not None and os.path.exists(net_file):
         return build_real_net(net_file, flow_rate=flow_rate, agent=agent, coop_gamma=coop_gamma)
     path = _CACHE % agent
+    if not os.path.exists(path) and agent in ('iqll', 'iqld'):
+        path = _CACHE % 'ia2c'      # IQL agents observe what IA2C agents do (AGENT_MODES, build_obs_program)
     if not os.path.exists(path):
         raise FileNotFoundError('no Monaco net file given and no derived table cache at %s' % path)
     return load_tables(path)

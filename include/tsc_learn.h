@@ -239,6 +239,51 @@ int tscl_argmax_actions(tscl_handle* h, const float* pi, int64_t R, int32_t* act
  * back-propagate through the rollout's own forward pass instead of recomputing it.
  * bf16 elements per unit in the packed weight image: ((dx+h)/8)*4h*8 + 8*dx*8 */
 
+/* ---- IQL Q-network forward for test-mode evaluation, csrc/tsc_q.cu ------------------------------
+ * The per-agent networks of the reference's value-based agents (agents/policies.py:341-389, variable names
+ * agents/checkpoint.py), all agents and R replicas in one launch:
+ *   model 0, LRQPolicy:   q = S.W_q + b_q                               S = the agent's n_s observation floats
+ *   model 1, DeepQPolicy: h0 = relu(S[:, :n_s-n_w].W_fcw + b)           width n_fc  (num_fc)
+ *                         h1 = relu(S[:, n_s-n_w:].W_fct + b)           width n_ft  (num_fc / 4), agents with n_w > 0
+ *                         h  = relu([h0 | h1].W_fc0 + b)                width n_h   (num_h)
+ *                         q  = h.W_q + b_q
+ * Every tensor is row-major [in][out] at its per-agent offset (in floats) into one flat fp32 parameter vector; offsets of
+ * layers a model does not have may be NULL.  fp32 FMAs throughout (no tensor cores), so that argmax ties resolve as in an
+ * fp32 host forward.  Limits: max_na <= 8; dqn widths multiples of 16 with n_fc <= 128, n_ft <= 32, n_h <= 64. */
+typedef struct tscl_qdims {
+  int32_t n_agents;   /* A                                                          */
+  int32_t n_obs;      /* row stride of the observation matrix                       */
+  int32_t max_na;     /* row stride of q                                            */
+  int32_t model;      /* 0 = lr, 1 = dqn                                            */
+  int32_t n_fc, n_ft, n_h;  /* dqn layer widths (ignored for lr)                   */
+  const int32_t* obs_off;   /* [A] first observation float of agent i               */
+  const int32_t* n_s;       /* [A] observation floats of agent i (wave | wait)      */
+  const int32_t* n_w;       /* [A] trailing wait floats of agent i (dqn: q_fct input) */
+  const int32_t* n_a;       /* [A]                                                  */
+  const int64_t* off_fcw_w; /* [A] [n_s-n_w][n_fc]  */ const int64_t* off_fcw_b; /* [A] [n_fc] */
+  const int64_t* off_fct_w; /* [A] [n_w][n_ft]      */ const int64_t* off_fct_b; /* [A] [n_ft] */
+  const int64_t* off_fc0_w; /* [A] [n_fc (+n_ft)][n_h] */ const int64_t* off_fc0_b; /* [A] [n_h] */
+  const int64_t* off_q_w;   /* [A] [n_s or n_h][n_a] */ const int64_t* off_q_b;   /* [A] [n_a] */
+  int64_t n_params;
+} tscl_qdims;
+
+typedef struct tscl_qhandle tscl_qhandle;
+
+int tscl_q_create(const tscl_qdims* dims, int32_t device, tscl_qhandle** out);
+int tscl_q_destroy(tscl_qhandle* h);
+/* One decision of IQL.forward(obs, mode='act', stochastic) (agents/models.py:347-363) for R replicas:
+ *   obs [R][n_obs] -> q [R][A][max_na] (zero padded), act [R][A].
+ *   mode 0: act = the first maximum of q (np.argmax; policy types 'default' and 'deterministic', utils.py:221-225).
+ *   mode 1: qs / np.sum(qs) and np.random.choice(n_a, p=qs): s = sum of q in index order, p_j = q_j / s, both fp32; the
+ *           inverse CDF of p at the counter-hash uniform of tscl_heads keyed (seed, step, replica0 + r, agent): the first
+ *           j with u < p_0 + .. + p_j, else n_a - 1.  A row where np.random.choice would raise (some p_j negative or not
+ *           finite: mixed signs, s = 0 or non-finite) gets action 0, and bad_flag (int64, caller-initialised to -1, may
+ *           be NULL) receives, as an unsigned atomic minimum, (replica0 + r) << 40 | (step & 0xFFFFFF) << 16 | agent: the
+ *           failure the one-replica protocol, playing the replicas in order, meets first.  All-negative q is valid.
+ * Replica-range form: pass obs + r0 * n_obs, q + r0 * A * max_na, act + r0 * A, R = n and replica0 = r0. */
+int tscl_q_step(tscl_qhandle* h, const float* params, const float* obs, int64_t R, float* q, int32_t* act, int32_t mode,
+                uint64_t seed, int64_t step, int64_t replica0, int64_t* bad_flag, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -6,8 +6,9 @@
                              [--policy lstm|fc]
 
 DIR holds `data/*.ini` (the run's config, [ENV_CONFIG] + [MODEL_CONFIG]) and, unless the agent is greedy,
-`model/checkpoint-<step>.npz` as written by IA2C.save / MA2C.save.  The agent is the directory's name, as in the reference
-(ia2c, ma2c or greedy).  Writes the reference's `<scenario>_<agent>_{control,traffic,trip}.csv` and
+`model/checkpoint-<step>.npz` as written by IA2C.save / MA2C.save / IQL.save.  The agent is the directory's name, as in
+the reference (main.py:179-190): ia2c, ma2c, greedy, iqld (IQL with DeepQPolicy) or any other name, e.g. iqll (IQL with
+LRQPolicy).  Writes the reference's `<scenario>_<agent>_{control,traffic,trip}.csv` and
 `<agent>_summary.json` (mean / std over episodes of the per-episode mean step reward, mean avg_queue / avg_speed_mps /
 avg_wait_sec, completed trips per episode) into OUT (default: DIR/eva_data).
 """
@@ -63,6 +64,12 @@ def greedy_controller(env):
     return SumoNetController(env.node_names, env.nodes, {n: env.phase_map.phases[n].phases for n in env.node_names})
 
 
+def iql_model_type(agent):
+    """main.py:185-190: 'iqld' is the DeepQPolicy IQL, every other agent name that is not an A2C variant or greedy the
+    LRQPolicy one."""
+    return 'dqn' if agent == 'iqld' else 'lr'
+
+
 def main(argv=None):
     a = parse_args(argv)
     logging.basicConfig(level=logging.INFO, format="%(message)s")
@@ -89,15 +96,17 @@ def main(argv=None):
     if agent == "greedy":
         model = greedy_controller(env)
     else:
-        from deeprl_signal_control_b200.agents.models import IA2C, MA2C
+        from deeprl_signal_control_b200.agents.models import IA2C, IQL, MA2C
         mc = config["MODEL_CONFIG"]
         kw = dict(n_replicas=1, obs_off=env._tables.node_obs_off, policy=a.policy)
         if agent == "ma2c":
             model = MA2C(env.n_s_ls, env.n_a_ls, env.n_w_ls, env.n_f_ls, 0, mc, **kw)
         elif agent == "ia2c":
             model = IA2C(env.n_s_ls, env.n_a_ls, env.n_w_ls, 0, mc, **kw)
+        elif agent == "a2c":
+            raise SystemExit("batched evaluation covers greedy, ia2c, ma2c and IQL (got %r)" % agent)
         else:
-            raise SystemExit("batched evaluation covers greedy, ia2c and ma2c (got %r)" % agent)
+            model = IQL(env.n_s_ls, env.n_a_ls, env.n_w_ls, 0, mc, seed=0, model_type=iql_model_type(agent))
         if not model.load(os.path.join(agent_dir, "model") + "/"):
             raise SystemExit("no checkpoint under %s/model/" % agent_dir)
     from deeprl_signal_control_b200.agents.evaluator import Evaluator

@@ -11,6 +11,9 @@
    MA2C at R = 2048, grid greedy at R = 4096; agent-env-steps/s = R x agents x control steps / time, and episodes/hour.
 3. The one-seed-at-a-time reference protocol (utils.py:Tester.perform on the one-replica env + MA2C wrapper) on the grid:
    the user-visible "before", timed over the first S seconds of one episode and scaled to 720 control steps.
+4. IQL: the fp32 Q forward (tscl_q_step, argmax actions) alone for LR and DQN, grid R = 4096 and Monaco R = 2048, CUDA
+   events, with the FLOPs and HBM bytes of one launch computed from the shapes; and whole 3600-s episodes of grid IQL-LR
+   / IQL-DQN at R = 4096 and Monaco IQL-LR / IQL-DQN at R = 2048 (--iql-only: this part alone).
 The card and its power limit are read in the same run.
 """
 import argparse
@@ -187,15 +190,121 @@ def time_reference(budget_s):
           "%.3g agent-env-steps/s, %.0f episodes/hour" % (n, el, per_ep, 25 * 720 / per_ep, 3600 / per_ep))
 
 
+IQL_INI = """
+[MODEL_CONFIG]
+gamma = 0.99
+max_grad_norm = 40
+batch_size = 20
+reward_norm = 2000.0
+reward_clip = 2.0
+num_fc = 128
+num_h = 64
+"""
+
+
+def q_cost(lay, R):
+    """(FLOPs, HBM bytes) of one tscl_q_step launch: 2 x multiply-adds of every layer; observations read once, q, the
+    actions and the parameters moved once"""
+    mac = 0
+    for i in range(lay.A):
+        n_s, n_a, n_w = int(lay.n_s[i]), int(lay.n_a[i]), int(lay.n_w[i])
+        if lay.model_type == "lr":
+            mac += n_s * n_a
+        else:
+            ft = lay.n_ft if n_w > 0 else 0
+            mac += (n_s - n_w) * lay.n_fc + n_w * ft + (lay.n_fc + ft) * lay.n_h + lay.n_h * n_a
+    return 2 * R * mac, R * lay.n_obs * 4 + R * lay.A * (lay.max_na + 1) * 4 + lay.n_params * 4
+
+
+def make_iql(scenario, agent, R):
+    from deeprl_signal_control_b200.agents.models import IQL
+    cp = configparser.ConfigParser()
+    cp.read_string(ENV_INI[scenario] % (agent, ",".join(str(10000 + 7 * k) for k in range(R))) + IQL_INI)
+    if scenario == "large_grid":
+        from deeprl_signal_control_b200.envs.large_grid_env import LargeGridEnv as Env
+    else:
+        from deeprl_signal_control_b200.envs.real_net_env import RealNetEnv as Env
+    env = Env(cp["ENV_CONFIG"], output_path="", is_record=False, n_replicas=R)
+    model = IQL(env.n_s_ls, env.n_a_ls, env.n_w_ls, 0, cp["MODEL_CONFIG"], seed=1,
+                model_type="dqn" if agent == "iqld" else "lr", device="cuda")
+    return env, model
+
+
+def time_q_kernel(scenario, agent, R, launches, warmup):
+    from deeprl_signal_control_b200.agents.layout import QLayout
+    env, model = make_iql(scenario, agent, 1)
+    net = env._tables
+    lay = QLayout.from_iql(model, net.node_obs_off, net.n_obs, max_na=net.max_na)
+    h = C.c_void_p()
+    lib = _lib.lib()
+    _lib.check(lib.tscl_q_create(C.byref(lay.as_c()), C.c_int32(0), C.byref(h)))
+    P = lay.pack(model.nets)
+    g = torch.Generator(device="cuda").manual_seed(0)
+    obs = torch.rand(R, net.n_obs, device="cuda", generator=g) * 2
+    q = torch.zeros(R, lay.A, lay.max_na, device="cuda")
+    act = torch.zeros(R, lay.A, dtype=torch.int32, device="cuda")
+    st = C.c_void_p(torch.cuda.current_stream().cuda_stream)
+
+    def fn():
+        _lib.check(lib.tscl_q_step(h, _p(P), _p(obs), C.c_int64(R), _p(q), _p(act), C.c_int32(0), C.c_uint64(1),
+                                   C.c_int64(0), C.c_int64(0), None, st))
+    for _ in range(warmup):
+        fn()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(launches):
+        fn()
+    e1.record()
+    torch.cuda.synchronize()
+    ms = e0.elapsed_time(e1) / launches
+    flops, b = q_cost(lay, R)
+    print("  Q forward %-4s %s R = %d: %.4f ms per launch (%d launches), %.2f GFLOP, %.1f MB -> %.1f TFLOP/s, %.0f GB/s"
+          % (lay.model_type, scenario, R, ms, launches, flops / 1e9, b / 1e6, flops / (ms * 1e-3) / 1e12,
+             b / (ms * 1e-3) / 1e9))
+    lib.tscl_q_destroy(h)
+
+
+def time_iql_evaluation(name, scenario, agent, R):
+    from deeprl_signal_control_b200.agents.evaluator import Evaluator
+    env, model = make_iql(scenario, agent, R)
+    ev = Evaluator(env, model, "", policy_type="default")
+    ev.perform_all()
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    mean, _ = ev.perform_all()
+    el = time.perf_counter() - t0
+    steps = R * env._tables.n_nodes * ev.T
+    print("  %-40s R = %d: %.3f s per episode set (%d control steps), %.3g agent-env-steps/s, %.0f episodes/hour; "
+          "mean step reward %.2f" % (name, R, el, ev.T, steps / el, R / el * 3600, float(np.mean(mean))))
+    del ev, env, model
+    torch.cuda.empty_cache()
+
+
+def time_iql(launches, warmup):
+    print("IQL Q forward alone (fp32 SIMT, argmax actions):")
+    for scenario, R in (("large_grid", 4096), ("real_net", 2048)):
+        for agent in ("iqll", "iqld"):
+            time_q_kernel(scenario, agent, R, launches, warmup)
+    print("IQL evaluation, whole 3600-s episodes (untrained weights):")
+    time_iql_evaluation("grid IQL-LR", "large_grid", "iqll", 4096)
+    time_iql_evaluation("grid IQL-DQN", "large_grid", "iqld", 4096)
+    time_iql_evaluation("Monaco IQL-LR", "real_net", "iqll", 2048)
+    time_iql_evaluation("Monaco IQL-DQN", "real_net", "iqld", 2048)
+
+
 def main():
     p = argparse.ArgumentParser()
     p.add_argument("--launches", type=int, default=200)
     p.add_argument("--warmup", type=int, default=20)
     p.add_argument("--ref-seconds", type=float, default=20.0)
+    p.add_argument("--iql-only", action="store_true")
     a = p.parse_args()
     smi = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
                          capture_output=True, text=True).stdout.strip()
     print("card: %s" % smi)
+    if a.iql_only:
+        time_iql(a.launches, a.warmup)
+        return
     print("policy forward alone:")
     time_kernels("large_grid", 4096, a.launches, a.warmup)
     time_kernels("real_net", 2048, a.launches, a.warmup)
@@ -206,6 +315,7 @@ def main():
     time_evaluation("grid greedy", "large_grid", "greedy", 4096, False)
     print("before:")
     time_reference(a.ref_seconds)
+    time_iql(a.launches, a.warmup)
 
 
 if __name__ == "__main__":
