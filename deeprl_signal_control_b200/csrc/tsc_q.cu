@@ -53,6 +53,11 @@ struct tscl_qhandle {
   std::vector<void*> owned;
   size_t smem = 0;
   int ctas_per_sm = 1, n_sm = 1;
+  int64_t n_params = 0;
+  size_t td_smem = 0;            // 0: the TD kernel's layout does not fit a CTA (tscl_q_td refuses)
+  int td_ctas_per_sm = 1;
+  const int64_t* blk = nullptr;  // [A + 1] first float of every agent's block in the flat vector, then n_params
+  float* part = nullptr;         // TD partials [groups][n_params + A]
 };
 
 struct QSmem {          // float offsets of the shared-memory regions
@@ -79,6 +84,35 @@ __host__ __device__ inline QSmem q_smem_layout(const QDims& d) {
   return o;
 }
 
+// The TD kernel's shared memory: the forward's regions, except that the q_fc_0 weight lives at an odd row pitch in w2p
+// (the transposed reads of the backward are then free of bank conflicts) and the forward's unpadded w2 region holds that
+// weight's gradient.  Then the other weight-gradient accumulators, at the weights' unpadded shapes (their order in the
+// flat vector), and three per-row arrays of a tile: TD target, dL/dq of the taken action, the action.
+struct QTdSmem {
+  QSmem f;
+  int ld2, w2p, gw1, gb1, gwt, gw2, gb2, gwq, gbq, tq, dq, act, total;
+};
+
+__host__ __device__ inline QTdSmem q_td_smem_layout(const QDims& d) {
+  QTdSmem o;
+  o.f = q_smem_layout(d);
+  int p = o.f.total;
+  o.ld2 = d.n_h + 1;
+  o.gw2 = o.f.w2;
+  o.w2p = p; p += d.in2_max * o.ld2;
+  o.gw1 = p; p += d.wave_max * d.n_fc;
+  o.gb1 = p; p += d.n_fc + d.n_ft;
+  o.gwt = p; p += d.w_max * d.n_ft;
+  o.gb2 = p; p += d.n_h;
+  o.gwq = p; p += d.q_in * QT_NA;
+  o.gbq = p; p += QT_NA;
+  o.tq = p; p += QT_ROWS;
+  o.dq = p; p += QT_ROWS;
+  o.act = p; p += QT_ROWS;
+  o.total = p;
+  return o;
+}
+
 __device__ __forceinline__ uint32_t qmix32(uint32_t h) {   // the counter hash of the A2C sampling kernels
   h ^= h >> 16; h *= 0x7feb352dU; h ^= h >> 15; h *= 0x846ca68bU; h ^= h >> 16;
   return h;
@@ -86,7 +120,9 @@ __device__ __forceinline__ uint32_t qmix32(uint32_t h) {   // the counter hash o
 
 // One hidden layer on a 64-row tile: out[c][row] = relu(sum_k in[k][row] W[k][c] + b[c]) for the columns c = tx + 16 j,
 // j < ncol (ncol <= NJ), k < K.  `in` / `out` column-major with pitch QT_LD; W row-major with `ldw` columns.
-template <int NJ>
+// BWD: the same layer's input gradient, in place: out[c][row] = (sum_k in[k][row] W[c][k]) * (out[c][row] > 0), with
+// `in` the output gradient and `out` holding the layer input's relu activations (b unused).
+template <int NJ, bool BWD = false>
 __device__ __forceinline__ void q_dense_relu(const float* __restrict__ in, int K, const float* __restrict__ W, int ldw,
                                              const float* __restrict__ b, int ncol, float* __restrict__ out, int ty,
                                              int tx) {
@@ -102,7 +138,7 @@ __device__ __forceinline__ void q_dense_relu(const float* __restrict__ in, int K
 #pragma unroll
     for (int j = 0; j < NJ; ++j) {
       if (j < ncol) {
-        const float wj = w[16 * j];
+        const float wj = BWD ? W[(tx + 16 * j) * ldw + k] : w[16 * j];
         acc[0][j] = fmaf(x.x, wj, acc[0][j]); acc[1][j] = fmaf(x.y, wj, acc[1][j]);
         acc[2][j] = fmaf(x.z, wj, acc[2][j]); acc[3][j] = fmaf(x.w, wj, acc[3][j]);
       }
@@ -111,20 +147,68 @@ __device__ __forceinline__ void q_dense_relu(const float* __restrict__ in, int K
 #pragma unroll
   for (int j = 0; j < NJ; ++j) {
     if (j < ncol) {
-      const float bj = b[tx + 16 * j];
-      *reinterpret_cast<float4*>(out + (tx + 16 * j) * QT_LD + ty * 4) =
-          make_float4(fmaxf(acc[0][j] + bj, 0.f), fmaxf(acc[1][j] + bj, 0.f), fmaxf(acc[2][j] + bj, 0.f),
-                      fmaxf(acc[3][j] + bj, 0.f));
+      float4* o = reinterpret_cast<float4*>(out + (tx + 16 * j) * QT_LD + ty * 4);
+      if (BWD) {
+        const float4 h = *o;
+        *o = make_float4(h.x > 0.f ? acc[0][j] : 0.f, h.y > 0.f ? acc[1][j] : 0.f, h.z > 0.f ? acc[2][j] : 0.f,
+                         h.w > 0.f ? acc[3][j] : 0.f);
+      } else {
+        const float bj = b[tx + 16 * j];
+        *o = make_float4(fmaxf(acc[0][j] + bj, 0.f), fmaxf(acc[1][j] + bj, 0.f), fmaxf(acc[2][j] + bj, 0.f),
+                         fmaxf(acc[3][j] + bj, 0.f));
+      }
     }
   }
 }
 
-// grid (groups, A), 256 threads.  DQN = false: LRQPolicy, true: DeepQPolicy.
+// The network on one tile whose observation slice is in sS: q of the 64 rows into sQ [row][QT_NA] (hidden activations
+// left in sH1 / sH2), with q_fc_0's weight at row pitch ld2.  Ends before the barrier that publishes sQ.  The TD kernel's
+// forward; q_fwd_kernel keeps the same statements inline so that its evaluation instantiations compile as before.
 template <bool DQN>
+__device__ __forceinline__ void q_tile_forward(const QDims& d, const float* sS, const float* sW1, const float* sB1,
+                                               const float* sWt, const float* sW2, int ld2, const float* sB2,
+                                               const float* sWq, const float* sBq, float* sH1, float* sH2, float* sQ,
+                                               int n_wave, int n_w, int n_ft, int q_in, int tid, int ty, int tx) {
+  const float* qin = sS;
+  if (DQN) {
+    q_dense_relu<QT_FC_MAX / 16>(sS, n_wave, sW1, d.n_fc, sB1, d.n_fc / 16, sH1, ty, tx);
+    if (n_ft > 0)
+      q_dense_relu<QT_FT_MAX / 16>(sS + n_wave * QT_LD, n_w, sWt, n_ft, sB1 + d.n_fc, n_ft / 16,
+                                   sH1 + d.n_fc * QT_LD, ty, tx);
+    __syncthreads();
+    q_dense_relu<QT_H_MAX / 16>(sH1, d.n_fc + n_ft, sW2, ld2, sB2, d.n_h / 16, sH2, ty, tx);
+    __syncthreads();
+    qin = sH2;
+  }
+  // output layer (linear): thread = (row, two actions)
+  const int row = tid & (QT_ROWS - 1), j0 = (tid >> 6) * 2;
+  float q0 = 0.f, q1 = 0.f;
+#pragma unroll 4
+  for (int k = 0; k < q_in; ++k) {
+    const float x = qin[k * QT_LD + row];
+    q0 = fmaf(x, sWq[k * QT_NA + j0], q0);
+    q1 = fmaf(x, sWq[k * QT_NA + j0 + 1], q1);
+  }
+  sQ[row * QT_NA + j0] = q0 + sBq[j0];
+  sQ[row * QT_NA + j0 + 1] = q1 + sBq[j0 + 1];
+}
+
+// The counter hash keyed (seed, step, replica, agent) of ε-greedy exploration: the chain of mode 1 in q_fwd_kernel.
+__device__ __forceinline__ uint32_t q_row_hash(uint32_t seed_lo, uint32_t seed_hi, uint32_t step, int64_t replica, int a) {
+  uint32_t hsh = qmix32(seed_lo ^ (step * 0x9E3779B1U));
+  hsh = qmix32(hsh ^ seed_hi ^ ((uint32_t)replica * 0x85EBCA77U));
+  return qmix32(hsh ^ ((uint32_t)a * 0xC2B2AE3DU));
+}
+
+// grid (groups, A), 256 threads.  DQN = false: LRQPolicy, true: DeepQPolicy.
+// EXPLORE: IQL.forward(obs, mode='explore') — the first maximum of q, replaced by a uniform action when the row's
+// uniform is below eps; also stores act (int8) and, from the agent-0 CTAs, whole observation rows into a replay slot.
+template <bool DQN, bool EXPLORE = false>
 __global__ void __launch_bounds__(256)
 q_fwd_kernel(const QDims d, const float* __restrict__ P, const float* __restrict__ obs, int64_t R,
              float* __restrict__ q, int32_t* __restrict__ act, int mode, uint32_t seed_lo, uint32_t seed_hi,
-             uint32_t step, int64_t replica0, unsigned long long* __restrict__ bad) {
+             uint32_t step, int64_t replica0, unsigned long long* __restrict__ bad, float eps,
+             float* __restrict__ ring_s, int8_t* __restrict__ ring_a) {
   extern __shared__ __align__(16) float qsm[];
   const QSmem L = q_smem_layout(d);
   const int a = blockIdx.y, tid = threadIdx.x, ty = tid >> 4, tx = tid & 15;
@@ -159,6 +243,10 @@ q_fwd_kernel(const QDims d, const float* __restrict__ P, const float* __restrict
       const int row = i / n_s, k = i - row * n_s;
       const int64_t m = m0 + row;
       sS[k * QT_LD + row] = m < R ? __ldg(obs + m * d.n_obs + ooff + k) : 0.f;
+    }
+    if (EXPLORE && blockIdx.y == 0 && ring_s) {
+      const int64_t nr = R - m0 < QT_ROWS ? R - m0 : QT_ROWS;
+      for (int64_t i = tid; i < nr * d.n_obs; i += 256) ring_s[m0 * d.n_obs + i] = obs[m0 * d.n_obs + i];
     }
     __syncthreads();
     const float* qin = sS;
@@ -201,6 +289,12 @@ q_fwd_kernel(const QDims d, const float* __restrict__ P, const float* __restrict
 #pragma unroll
         for (int j = 1; j < QT_NA; ++j)
           if (j < n_a && qv[j] > best) { best = qv[j]; pick = j; }
+        if (EXPLORE) {                        // np.random.random() < eps: np.random.randint(n_a)
+          const uint32_t hsh = q_row_hash(seed_lo, seed_hi, step, replica0 + r, a);
+          if ((float)(hsh >> 8) * (1.0f / 16777216.0f) < eps)
+            pick = (int)(((uint64_t)qmix32(hsh ^ 0x5BD1E995U) * (uint32_t)n_a) >> 32);
+          if (ring_a) ring_a[r * d.A + a] = (int8_t)pick;
+        }
       } else {                                // qs / np.sum(qs); np.random.choice(n_a, p=qs)
         float s = 0.f;
 #pragma unroll
@@ -236,6 +330,300 @@ q_fwd_kernel(const QDims d, const float* __restrict__ P, const float* __restrict
       }
       act[r * d.A + a] = pick;
     }
+  }
+}
+
+
+// ================================================================================================
+// Training (IQL.backward, agents/models.py:305-312): minibatch sampler, fused TD forward / backward, reduction, clip + Adam.
+
+// Counter-hash key of agent a's minibatch draws in one round of one update, for global replica `replica`.
+__device__ __forceinline__ uint32_t q_sample_key(uint32_t seed_lo, uint32_t seed_hi, uint32_t update, uint32_t round,
+                                                 int64_t replica, int a) {
+  uint32_t hsh = qmix32(seed_lo ^ (update * 0x9E3779B1U));
+  hsh = qmix32(hsh ^ seed_hi ^ ((uint32_t)replica * 0x85EBCA77U));
+  return qmix32(hsh ^ ((uint32_t)a * 0xC2B2AE3DU) ^ (round * 0x27D4EB2FU));
+}
+
+// random.sample(range(size), batch) per (agent, replica): Floyd's algorithm, draw d picks t uniform in [0, j] with
+// j = size - batch + d by multiply-shift (bias <= size / 2^32) and keeps j instead when t was already taken.  One thread
+// per (agent, replica); idx [A][R][batch].
+__global__ void q_sample_kernel(int A, int64_t R, int batch, int size, uint32_t seed_lo, uint32_t seed_hi,
+                                uint32_t update, uint32_t round, int64_t replica0, int32_t* __restrict__ idx) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (int64_t)A * R) return;
+  const int a = (int)(i / R);
+  const int64_t r = i - (int64_t)a * R;
+  const uint32_t key = q_sample_key(seed_lo, seed_hi, update, round, replica0 + r, a);
+  int32_t* out = idx + i * batch;
+  for (int dd = 0; dd < batch; ++dd) {
+    const uint32_t j = (uint32_t)(size - batch + dd);
+    const uint32_t x = qmix32(key ^ ((uint32_t)(dd + 1) * 0x165667B1U));
+    const int32_t t = (int32_t)(((uint64_t)x * (j + 1u)) >> 32);
+    bool taken = false;
+    for (int e = 0; e < dd; ++e) taken |= out[e] == t;
+    out[dd] = taken ? (int32_t)j : t;
+  }
+}
+
+// G[k][c] += sum over the tile's rows of A[k][row] B[c][row] for k < K and the columns c = tx + 16 j, j < ncol (<= NJ);
+// A / B column-major tiles (pitch QT_LD), G row-major with ldg columns.  Every G element has one owner thread.
+template <int KI, int NJ>
+__device__ __forceinline__ void q_wgrad(const float* __restrict__ A, int K, const float* __restrict__ B, int ncol,
+                                        float* __restrict__ G, int ldg, int ty, int tx) {
+  for (int k0 = 0; k0 < K; k0 += 16 * KI) {
+    float acc[KI][NJ];
+#pragma unroll
+    for (int i = 0; i < KI; ++i)
+#pragma unroll
+      for (int j = 0; j < NJ; ++j) acc[i][j] = 0.f;
+    for (int r = 0; r < QT_ROWS; r += 4) {
+      float4 b[NJ];
+#pragma unroll
+      for (int j = 0; j < NJ; ++j)
+        if (j < ncol) b[j] = *reinterpret_cast<const float4*>(B + (tx + 16 * j) * QT_LD + r);
+#pragma unroll
+      for (int i = 0; i < KI; ++i) {
+        const int k = k0 + ty + 16 * i;
+        if (k < K) {
+          const float4 x = *reinterpret_cast<const float4*>(A + k * QT_LD + r);
+#pragma unroll
+          for (int j = 0; j < NJ; ++j)
+            if (j < ncol) {
+              acc[i][j] = fmaf(x.x, b[j].x, acc[i][j]); acc[i][j] = fmaf(x.y, b[j].y, acc[i][j]);
+              acc[i][j] = fmaf(x.z, b[j].z, acc[i][j]); acc[i][j] = fmaf(x.w, b[j].w, acc[i][j]);
+            }
+        }
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < KI; ++i) {
+      const int k = k0 + ty + 16 * i;
+#pragma unroll
+      for (int j = 0; j < NJ; ++j)
+        if (k < K && j < ncol) G[k * ldg + tx + 16 * j] += acc[i][j];
+    }
+  }
+}
+
+// Gb[c] += sum over the tile's rows of B[c][row], c < n
+__device__ __forceinline__ void q_bgrad(const float* __restrict__ B, int n, float* __restrict__ Gb, int tid) {
+  for (int c = tid; c < n; c += 256) {
+    float s = 0.f;
+    for (int r = 0; r < QT_ROWS; ++r) s += B[c * QT_LD + r];
+    Gb[c] += s;
+  }
+}
+
+// One round of QPolicy.backward for every agent (agents/policies.py:307-338): rows m < R * batch of agent a are the
+// ring entries (slot idx[a][r][m % batch], replica r = m / batch).  tq = done ? r : r + gamma max_j q(s1)_j (no gradient,
+// same network), e = q(s)[act] - tq, loss = sum e^2 * inv_n, dq = 2 e inv_n.  grid (groups, A), 256 threads; CTA (g, a)
+// walks tiles g, g + groups, .. with agent a's weights resident, accumulates its weight gradients in shared memory, and
+// writes them at the agent's flat offsets into partial row g (part [groups][ld], loss at column n_params + a).
+template <bool DQN>
+__global__ void __launch_bounds__(256)
+q_td_kernel(const QDims d, const float* __restrict__ P, const float* __restrict__ ring_s,
+            const float* __restrict__ ring_s1, const int8_t* __restrict__ ring_a, const float* __restrict__ ring_r,
+            const uint8_t* __restrict__ ring_done, const int32_t* __restrict__ idx, int64_t R, int batch, float gamma,
+            float inv_n, int64_t n_params, float* __restrict__ part, int64_t ld) {
+  extern __shared__ __align__(16) float qsm[];
+  const QTdSmem T = q_td_smem_layout(d);
+  const QSmem& L = T.f;
+  const int a = blockIdx.y, tid = threadIdx.x, ty = tid >> 4, tx = tid & 15;
+  const int n_s = d.n_s[a], n_a = d.n_a[a], ooff = d.obs_off[a];
+  const int n_w = DQN ? d.n_w[a] : 0, n_wave = n_s - n_w;
+  const int n_ft = n_w > 0 ? d.n_ft : 0;
+  const int q_in = DQN ? d.n_h : n_s, h1w = d.n_fc + n_ft;
+  float *sW1 = qsm + L.w1, *sB1 = qsm + L.b1, *sWt = qsm + L.wt, *sW2 = qsm + T.w2p, *sB2 = qsm + L.b2;
+  float *sWq = qsm + L.wq, *sBq = qsm + L.bq, *sS = qsm + L.s, *sH1 = qsm + L.h1, *sH2 = qsm + L.h2, *sQ = qsm + L.q;
+  float *gW1 = qsm + T.gw1, *gB1 = qsm + T.gb1, *gWt = qsm + T.gwt, *gW2 = qsm + T.gw2, *gB2 = qsm + T.gb2;
+  float *gWq = qsm + T.gwq, *gBq = qsm + T.gbq, *sTq = qsm + T.tq, *sDq = qsm + T.dq;
+  int* sAct = reinterpret_cast<int*>(qsm + T.act);
+
+  if (DQN) {
+    for (int i = tid; i < n_wave * d.n_fc; i += 256) { sW1[i] = P[d.off_fcw_w[a] + i]; gW1[i] = 0.f; }
+    for (int i = tid; i < h1w; i += 256) {
+      sB1[i] = i < d.n_fc ? P[d.off_fcw_b[a] + i] : P[d.off_fct_b[a] + i - d.n_fc];
+      gB1[i] = 0.f;
+    }
+    for (int i = tid; i < n_w * n_ft; i += 256) { sWt[i] = P[d.off_fct_w[a] + i]; gWt[i] = 0.f; }
+    for (int i = tid; i < h1w * d.n_h; i += 256) {
+      const int k = i / d.n_h, c = i - k * d.n_h;
+      sW2[k * T.ld2 + c] = P[d.off_fc0_w[a] + i];
+      gW2[i] = 0.f;
+    }
+    for (int i = tid; i < d.n_h; i += 256) { sB2[i] = P[d.off_fc0_b[a] + i]; gB2[i] = 0.f; }
+  }
+  for (int i = tid; i < q_in * QT_NA; i += 256) {
+    const int k = i / QT_NA, j = i - k * QT_NA;
+    sWq[i] = j < n_a ? P[d.off_q_w[a] + (int64_t)k * n_a + j] : 0.f;
+    gWq[i] = 0.f;
+  }
+  for (int i = tid; i < QT_NA; i += 256) { sBq[i] = i < n_a ? P[d.off_q_b[a] + i] : 0.f; gBq[i] = 0.f; }
+
+  float loss = 0.f;                                   // threads < QT_ROWS: their rows' squared TD errors
+  const int64_t rows = R * batch, n_tiles = (rows + QT_ROWS - 1) / QT_ROWS;
+  const int32_t* ia = idx + (int64_t)a * rows;
+  for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+    const int64_t m0 = tile * QT_ROWS;
+    for (int pass = 0; pass < 2; ++pass) {           // 0: s1 -> TD target, 1: s -> q and the activations kept
+      const float* src = pass ? ring_s : ring_s1;
+      __syncthreads();
+      for (int i = tid; i < QT_ROWS * n_s; i += 256) {
+        const int row = i / n_s, k = i - row * n_s;
+        const int64_t m = m0 + row;
+        float x = 0.f;
+        if (m < rows) {
+          const int64_t r = m / batch;
+          x = __ldg(src + ((int64_t)ia[m] * R + r) * d.n_obs + ooff + k);
+        }
+        sS[k * QT_LD + row] = x;
+      }
+      __syncthreads();
+      q_tile_forward<DQN>(d, sS, sW1, sB1, sWt, sW2, T.ld2, sB2, sWq, sBq, sH1, sH2, sQ, n_wave, n_w, n_ft, q_in, tid,
+                          ty, tx);
+      __syncthreads();
+      if (tid < QT_ROWS) {
+        const int64_t m = m0 + tid;
+        if (pass == 0) {                              // tq = done ? r : r + gamma * max q(s1)  (torch.where, fp32 ops)
+          float tq = 0.f;
+          int act = -1;
+          if (m < rows) {
+            const int64_t r = m / batch, e = (int64_t)ia[m] * R + r;
+            float best = sQ[tid * QT_NA];
+            for (int j = 1; j < n_a; ++j) best = fmaxf(best, sQ[tid * QT_NA + j]);
+            const float rw = ring_r[e * d.A + a];
+            tq = ring_done[e] ? rw : __fadd_rn(rw, __fmul_rn(gamma, best));
+            act = ring_a[e * d.A + a];
+          }
+          sTq[tid] = tq;
+          sAct[tid] = act;
+        } else {
+          float dq = 0.f;
+          if (m < rows) {
+            const float e = __fsub_rn(sQ[tid * QT_NA + sAct[tid]], sTq[tid]);
+            loss = fmaf(e, e, loss);
+            dq = 2.f * e * inv_n;
+          }
+          sDq[tid] = dq;
+        }
+      }
+    }
+    __syncthreads();
+    // output layer: gWq[k][j] += sum_rows in[k][row] dq[row] [act[row] == j], gBq[j] += sum_rows dq[row] [act == j]
+    const float* qin = DQN ? sH2 : sS;
+    for (int i = tid; i < q_in * QT_NA; i += 256) {
+      const int k = i / QT_NA, j = i - k * QT_NA;
+      if (j < n_a) {
+        float acc = 0.f;
+        for (int r = 0; r < QT_ROWS; ++r) acc = fmaf(qin[k * QT_LD + r], sAct[r] == j ? sDq[r] : 0.f, acc);
+        gWq[i] += acc;
+      }
+    }
+    if (tid < n_a) {
+      float acc = 0.f;
+      for (int r = 0; r < QT_ROWS; ++r) acc += sAct[r] == tid ? sDq[r] : 0.f;
+      gBq[tid] += acc;
+    }
+    if (DQN) {
+      __syncthreads();
+      // dh2 = dq Wq[:, act]^T masked by h2 > 0, in place of h2
+      for (int i = tid; i < d.n_h * QT_ROWS; i += 256) {
+        const int c = i / QT_ROWS, r = i - c * QT_ROWS;
+        const float h = sH2[c * QT_LD + r];
+        sH2[c * QT_LD + r] = (h > 0.f && sAct[r] >= 0) ? sDq[r] * sWq[c * QT_NA + sAct[r]] : 0.f;
+      }
+      __syncthreads();
+      q_wgrad<4, QT_H_MAX / 16>(sH1, h1w, sH2, d.n_h / 16, gW2, d.n_h, ty, tx);
+      q_bgrad(sH2, d.n_h, gB2, tid);
+      __syncthreads();
+      // dh1 = dh2 W2^T masked by h1 > 0, in place of h1
+      q_dense_relu<(QT_FC_MAX + QT_FT_MAX) / 16, true>(sH2, d.n_h, sW2, T.ld2, nullptr, h1w / 16, sH1, ty, tx);
+      __syncthreads();
+      q_wgrad<2, QT_FC_MAX / 16>(sS, n_wave, sH1, d.n_fc / 16, gW1, d.n_fc, ty, tx);
+      if (n_ft > 0) q_wgrad<1, QT_FT_MAX / 16>(sS + n_wave * QT_LD, n_w, sH1 + d.n_fc * QT_LD, n_ft / 16, gWt, n_ft, ty, tx);
+      q_bgrad(sH1, h1w, gB1, tid);
+    }
+  }
+  // the CTA's loss: fixed-order shuffle reduction over the 64 row threads
+  if (tid < QT_ROWS) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) loss += __shfl_down_sync(0xffffffffu, loss, o);
+    if ((tid & 31) == 0) sTq[tid >> 5] = loss;
+  }
+  __syncthreads();
+  float* out = part + (int64_t)blockIdx.x * ld;
+  if (tid == 0) out[n_params + a] = (sTq[0] + sTq[1]) * inv_n;
+  if (DQN) {
+    for (int i = tid; i < n_wave * d.n_fc; i += 256) out[d.off_fcw_w[a] + i] = gW1[i];
+    for (int i = tid; i < d.n_fc; i += 256) out[d.off_fcw_b[a] + i] = gB1[i];
+    for (int i = tid; i < n_w * n_ft; i += 256) out[d.off_fct_w[a] + i] = gWt[i];
+    for (int i = tid; i < n_ft; i += 256) out[d.off_fct_b[a] + i] = gB1[d.n_fc + i];
+    for (int i = tid; i < h1w * d.n_h; i += 256) out[d.off_fc0_w[a] + i] = gW2[i];
+    for (int i = tid; i < d.n_h; i += 256) out[d.off_fc0_b[a] + i] = gB2[i];
+  }
+  for (int i = tid; i < q_in * n_a; i += 256) {
+    const int k = i / n_a, j = i - k * n_a;
+    out[d.off_q_w[a] + i] = gWq[k * QT_NA + j];
+  }
+  for (int i = tid; i < n_a; i += 256) out[d.off_q_b[a] + i] = gBq[i];
+}
+
+// grad[i] = sum over the partial rows g = 0, 1, .. of part[g][i], in that order (no atomics: bit-reproducible)
+__global__ void q_reduce_kernel(const float* __restrict__ part, int groups, int64_t ld, float* __restrict__ grad) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= ld) return;
+  float s = 0.f;
+  for (int g = 0; g < groups; ++g) s += part[(int64_t)g * ld + i];
+  grad[i] = s;
+}
+
+// Per agent (one CTA of 512 threads): tf.clip_by_global_norm and the TF1 Adam step of IQL.td_update
+// (agents/models.py:290-302) on the agent's block [blk[a], blk[a+1]) of the flat vector, loss / norm written out.
+__global__ void __launch_bounds__(512)
+q_adam_kernel(float* __restrict__ P, const float* __restrict__ grad, float* __restrict__ m, float* __restrict__ v,
+              const int64_t* __restrict__ blk, int64_t n_params, float lr_t, float max_norm, float* __restrict__ loss_out,
+              float* __restrict__ norm_out) {
+  __shared__ float red[512];
+  const int a = blockIdx.x, tid = threadIdx.x;
+  const int64_t b0 = blk[a], b1 = blk[a + 1];
+  float ss = 0.f;
+  for (int64_t i = b0 + tid; i < b1; i += 512) ss = fmaf(grad[i], grad[i], ss);
+  red[tid] = ss;
+  __syncthreads();
+  for (int o = 256; o > 0; o >>= 1) {
+    if (tid < o) red[tid] += red[tid + o];
+    __syncthreads();
+  }
+  const float norm = sqrtf(red[0]);
+  const float scale = max_norm > 0.f ? __fdiv_rn(max_norm, fmaxf(norm, max_norm)) : 1.f;
+  const float c1 = (float)(1.0 - 0.9), c2 = (float)(1.0 - 0.999);
+  for (int64_t i = b0 + tid; i < b1; i += 512) {
+    const float g = max_norm > 0.f ? __fmul_rn(grad[i], scale) : grad[i];
+    const float mi = __fadd_rn(m[i], __fmul_rn(__fsub_rn(g, m[i]), c1));
+    const float vi = __fadd_rn(v[i], __fmul_rn(__fsub_rn(__fmul_rn(g, g), v[i]), c2));
+    m[i] = mi;
+    v[i] = vi;
+    P[i] = __fsub_rn(P[i], __fdiv_rn(__fmul_rn(lr_t, mi), __fadd_rn(__fsqrt_rn(vi), 1e-8f)));
+  }
+  if (tid == 0) { loss_out[a] = grad[n_params + a]; norm_out[a] = norm; }
+}
+
+// IQL.add_transition's reward (r / reward_norm, then clipped) and the post-step done into one replay slot, and the
+// episode's global-reward sum.
+__global__ void q_transition_kernel(const float* __restrict__ rew, int64_t RA, float reward_norm, float reward_clip,
+                                    float* __restrict__ ring_r, const float* __restrict__ grew, float* __restrict__ rew_acc,
+                                    uint8_t* __restrict__ ring_done, int64_t R, int done) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < RA) {
+    float x = rew[i];
+    if (reward_norm != 0.f) x = __fdiv_rn(x, reward_norm);
+    if (reward_clip != 0.f) x = fminf(fmaxf(x, -reward_clip), reward_clip);
+    ring_r[i] = x;
+  }
+  if (i < R) {
+    ring_done[i] = (uint8_t)done;
+    if (rew_acc) rew_acc[i] += grew[i];
   }
 }
 
@@ -296,8 +684,16 @@ extern "C" int tscl_q_create(const tscl_qdims* x, int32_t device, tscl_qhandle**
     rc |= qup(h, x->off_fc0_w, A, &d.off_fc0_w); rc |= qup(h, x->off_fc0_b, A, &d.off_fc0_b);
     if (any_w) { rc |= qup(h, x->off_fct_w, A, &d.off_fct_w); rc |= qup(h, x->off_fct_b, A, &d.off_fct_b); }
   }
+  // agent blocks of the flat vector, in agent order (QLayout): the per-agent clip + Adam ranges
+  std::vector<int64_t> blk(A + 1);
+  for (int a = 0; a < A; ++a) blk[a] = dqn ? x->off_fcw_w[a] : x->off_q_w[a];
+  blk[A] = x->n_params;
+  for (int a = 0; a < A; ++a)
+    if (blk[a] < 0 || blk[a] >= blk[a + 1]) rc = tsc_set_error("tscl_q_create: agent blocks are not in agent order");
+  if (!rc) rc |= qup(h, blk.data(), A + 1, &h->blk);
   if (rc) { tscl_q_destroy(h); return -1; }
   h->d = d;
+  h->n_params = x->n_params;
   h->smem = (size_t)q_smem_layout(d).total * sizeof(float);
   int optin = 0;
   LCK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device));
@@ -310,6 +706,16 @@ extern "C" int tscl_q_create(const tscl_qdims* x, int32_t device, tscl_qhandle**
   LCK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem));
   LCK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&h->ctas_per_sm, fn, 256, h->smem));
   if (h->ctas_per_sm < 1) h->ctas_per_sm = 1;
+  const void* ex = dqn ? (const void*)q_fwd_kernel<true, true> : (const void*)q_fwd_kernel<false, true>;
+  LCK(cudaFuncSetAttribute(ex, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem));
+  const size_t td_smem = (size_t)q_td_smem_layout(d).total * sizeof(float);
+  if (td_smem <= (size_t)optin) {
+    const void* td = dqn ? (const void*)q_td_kernel<true> : (const void*)q_td_kernel<false>;
+    LCK(cudaFuncSetAttribute(td, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)td_smem));
+    LCK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&h->td_ctas_per_sm, td, 256, td_smem));
+    if (h->td_ctas_per_sm < 1) h->td_ctas_per_sm = 1;
+    h->td_smem = td_smem;
+  }
   *out = h;
   return 0;
 }
@@ -318,6 +724,7 @@ extern "C" int tscl_q_destroy(tscl_qhandle* h) {
   if (!h) return 0;
   cudaSetDevice(h->device);
   for (void* p : h->owned) cudaFree(p);
+  if (h->part) cudaFree(h->part);
   delete h;
   return 0;
 }
@@ -336,10 +743,97 @@ extern "C" int tscl_q_step(tscl_qhandle* h, const float* params, const float* ob
   const uint32_t lo = (uint32_t)(seed & 0xFFFFFFFFu), hi = (uint32_t)(seed >> 32);
   if (h->d.model == 1)
     q_fwd_kernel<true><<<grid, 256, h->smem, (cudaStream_t)stream>>>(h->d, params, obs, R, q, act, mode, lo, hi,
-                                                                      (uint32_t)step, replica0, bad);
+                                                                      (uint32_t)step, replica0, bad, 0.f, nullptr,
+                                                                      nullptr);
   else
     q_fwd_kernel<false><<<grid, 256, h->smem, (cudaStream_t)stream>>>(h->d, params, obs, R, q, act, mode, lo, hi,
-                                                                       (uint32_t)step, replica0, bad);
+                                                                       (uint32_t)step, replica0, bad, 0.f, nullptr,
+                                                                       nullptr);
+  LCK(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int tscl_q_explore(tscl_qhandle* h, const float* params, const float* obs, int64_t R, float* q, int32_t* act,
+                              float eps, uint64_t seed, int64_t step, int64_t replica0, float* ring_s, int8_t* ring_a,
+                              void* stream) {
+  if (!h || !params || !obs || !q || !act || R <= 0 || replica0 < 0) return tsc_set_error("tscl_q_explore: bad argument");
+  LCK(cudaSetDevice(h->device));
+  const int64_t n_tiles = (R + QT_ROWS - 1) / QT_ROWS;
+  int64_t groups = ((int64_t)h->n_sm * h->ctas_per_sm + h->d.A - 1) / h->d.A;
+  if (groups > n_tiles) groups = n_tiles;
+  dim3 grid((unsigned)groups, (unsigned)h->d.A);
+  const uint32_t lo = (uint32_t)(seed & 0xFFFFFFFFu), hi = (uint32_t)(seed >> 32);
+  if (h->d.model == 1)
+    q_fwd_kernel<true, true><<<grid, 256, h->smem, (cudaStream_t)stream>>>(h->d, params, obs, R, q, act, 0, lo, hi,
+                                                                          (uint32_t)step, replica0, nullptr, eps, ring_s,
+                                                                          ring_a);
+  else
+    q_fwd_kernel<false, true><<<grid, 256, h->smem, (cudaStream_t)stream>>>(h->d, params, obs, R, q, act, 0, lo, hi,
+                                                                           (uint32_t)step, replica0, nullptr, eps, ring_s,
+                                                                           ring_a);
+  LCK(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int tscl_q_sample(tscl_qhandle* h, int64_t R, int32_t batch, int32_t size, uint64_t seed, int64_t update,
+                             int32_t round, int64_t replica0, int32_t* idx, void* stream) {
+  if (!h || !idx || R <= 0 || batch <= 0 || size < batch || replica0 < 0 || round < 0)
+    return tsc_set_error("tscl_q_sample: bad argument (the ring must hold at least batch entries)");
+  LCK(cudaSetDevice(h->device));
+  const int64_t n = (int64_t)h->d.A * R;
+  q_sample_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
+      h->d.A, R, batch, size, (uint32_t)(seed & 0xFFFFFFFFu), (uint32_t)(seed >> 32), (uint32_t)update, (uint32_t)round,
+      replica0, idx);
+  LCK(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int tscl_q_td(tscl_qhandle* h, const float* params, const float* ring_s, const float* ring_s1,
+                         const int8_t* ring_a, const float* ring_r, const uint8_t* ring_done, const int32_t* idx, int64_t R,
+                         int32_t batch, float gamma, float inv_n, float* grad, void* stream) {
+  if (!h || !params || !ring_s || !ring_s1 || !ring_a || !ring_r || !ring_done || !idx || !grad || R <= 0 || batch <= 0)
+    return tsc_set_error("tscl_q_td: bad argument");
+  if (!h->td_smem)
+    return tsc_set_error("tscl_q_td: the weights, gradients and tiles of one agent need more shared memory than a CTA has");
+  LCK(cudaSetDevice(h->device));
+  const int A = h->d.A;
+  const int64_t ld = h->n_params + A, n_tiles = (R * batch + QT_ROWS - 1) / QT_ROWS;
+  const int64_t max_groups = ((int64_t)h->n_sm * h->td_ctas_per_sm + A - 1) / A;
+  int64_t groups = max_groups < n_tiles ? max_groups : n_tiles;
+  if (!h->part) LCK(cudaMalloc(&h->part, (size_t)max_groups * ld * sizeof(float)));
+  dim3 grid((unsigned)groups, (unsigned)A);
+  if (h->d.model == 1)
+    q_td_kernel<true><<<grid, 256, h->td_smem, (cudaStream_t)stream>>>(h->d, params, ring_s, ring_s1, ring_a, ring_r,
+                                                                        ring_done, idx, R, batch, gamma, inv_n,
+                                                                        h->n_params, h->part, ld);
+  else
+    q_td_kernel<false><<<grid, 256, h->td_smem, (cudaStream_t)stream>>>(h->d, params, ring_s, ring_s1, ring_a, ring_r,
+                                                                         ring_done, idx, R, batch, gamma, inv_n,
+                                                                         h->n_params, h->part, ld);
+  LCK(cudaGetLastError());
+  q_reduce_kernel<<<(unsigned)((ld + 255) / 256), 256, 0, (cudaStream_t)stream>>>(h->part, (int)groups, ld, grad);
+  LCK(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int tscl_q_adam(tscl_qhandle* h, float* params, const float* grad, float* adam_m, float* adam_v, float lr_t,
+                           float max_grad_norm, float* loss_out, float* norm_out, void* stream) {
+  if (!h || !params || !grad || !adam_m || !adam_v || !loss_out || !norm_out) return tsc_set_error("tscl_q_adam: bad argument");
+  LCK(cudaSetDevice(h->device));
+  q_adam_kernel<<<h->d.A, 512, 0, (cudaStream_t)stream>>>(params, grad, adam_m, adam_v, h->blk, h->n_params, lr_t,
+                                                          max_grad_norm, loss_out, norm_out);
+  LCK(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int tscl_q_transition(tscl_qhandle* h, const float* rew, int64_t R, float reward_norm, float reward_clip,
+                                 float* ring_r, const float* grew, float* rew_acc, uint8_t* ring_done, int32_t done,
+                                 void* stream) {
+  if (!h || !rew || !ring_r || !ring_done || R <= 0 || (rew_acc && !grew)) return tsc_set_error("tscl_q_transition: bad argument");
+  LCK(cudaSetDevice(h->device));
+  const int64_t RA = R * h->d.A;
+  q_transition_kernel<<<(unsigned)((RA + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
+      rew, RA, reward_norm, reward_clip, ring_r, grew, rew_acc, ring_done, R, done);
   LCK(cudaGetLastError());
   return 0;
 }

@@ -284,6 +284,34 @@ int tscl_q_destroy(tscl_qhandle* h);
 int tscl_q_step(tscl_qhandle* h, const float* params, const float* obs, int64_t R, float* q, int32_t* act, int32_t mode,
                 uint64_t seed, int64_t step, int64_t replica0, int64_t* bad_flag, void* stream);
 
+/* ---- IQL training (IQL.explore / add_transition / backward, agents/models.py:305-376), same handle ----------------
+ * Replay ring of one rank's R replicas, slot-major, capacity B: s / s1 [B][R][n_obs] fp32, a [B][R][A] int8,
+ * r [B][R][A] fp32 (already normalised and clipped), done [B][R] u8.  The learner owns the write position.
+ *
+ * Explore forward: act = the first maximum of q, replaced by floor(n_a * u2) (multiply-shift) when u < eps, u and u2
+ * from the counter hash keyed (seed, step, replica0 + r, agent) (u2 from a second, salted stream).  Also writes act as
+ * int8 into ring_a [R][A] and copies the observation rows into ring_s [R][n_obs] (either may be NULL). */
+int tscl_q_explore(tscl_qhandle* h, const float* params, const float* obs, int64_t R, float* q, int32_t* act, float eps,
+                   uint64_t seed, int64_t step, int64_t replica0, float* ring_s, int8_t* ring_a, void* stream);
+/* random.sample(range(size), batch) for every (agent, replica): idx [A][R][batch] (int32), Floyd's algorithm with
+ * multiply-shift draws keyed (seed, update, round, replica0 + r, agent, draw).  size >= batch. */
+int tscl_q_sample(tscl_qhandle* h, int64_t R, int32_t batch, int32_t size, uint64_t seed, int64_t update, int32_t round,
+                  int64_t replica0, int32_t* idx, void* stream);
+/* One round of the TD loss for all agents: the rows idx[a][r][*] of the ring (pointers to slot 0), tq = done ? r :
+ * r + gamma max q(s1), loss = inv_n sum (q(s)[a] - tq)^2 over this rank's rows.  grad [n_params + A] receives the
+ * weight gradients (flat layout) followed by the per-agent loss sums; reduced in a fixed order (bit-reproducible). */
+int tscl_q_td(tscl_qhandle* h, const float* params, const float* ring_s, const float* ring_s1, const int8_t* ring_a,
+              const float* ring_r, const uint8_t* ring_done, const int32_t* idx, int64_t R, int32_t batch, float gamma,
+              float inv_n, float* grad, void* stream);
+/* Per agent: tf.clip_by_global_norm(max_grad_norm) of grad and the TF1 Adam step (b1 0.9, b2 0.999, eps 1e-8) with
+ * lr_t = lr sqrt(1 - b2^t) / (1 - b1^t); loss_out [A] = grad's loss sums, norm_out [A] = the pre-clip norms. */
+int tscl_q_adam(tscl_qhandle* h, float* params, const float* grad, float* adam_m, float* adam_v, float lr_t,
+                float max_grad_norm, float* loss_out, float* norm_out, void* stream);
+/* IQL.add_transition's reward and done into one ring slot: ring_r [R][A] = clip(rew / reward_norm), ring_done [R] = done,
+ * and rew_acc [R] += grew [R] (rew_acc may be NULL). */
+int tscl_q_transition(tscl_qhandle* h, const float* rew, int64_t R, float reward_norm, float reward_clip, float* ring_r,
+                      const float* grew, float* rew_acc, uint8_t* ring_done, int32_t done, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

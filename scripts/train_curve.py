@@ -3,7 +3,11 @@ same episodes (reference utils.py:296-305: mean over the 720 control steps of th
 
   python scripts/train_curve.py --replicas 512 --episodes 300 --agent ma2c [--scenario grid|real] [--policy lstm|fc]
                                 [--fp32] [--reward-norm X] [--lr X] [--tag NAME] [--greedy]
+  python scripts/train_curve.py --replicas 4096 --episodes 20 --agent iqll|iqld [--scenario grid|real] [--eval-seeds S,..]
 
+--agent iqll / iqld  IQL-LR / IQL-DQN on the batched IQL learner (agents/learner_iql.py) with the MODEL_CONFIG of the
+               reference's config_iql{l,d}_{large,real}.ini, then test-mode evaluation of the trained weights on
+               --eval-seeds through the batched evaluator
 --fp32         plain fp32 learner kernels (no tensor cores, no bf16 activation store): the A/B partner of the default path
 --reward-norm  override MODEL_CONFIG.reward_norm (reference: 2000 for MA2C on the grid, config/config_ma2c_large.ini)
 --greedy       no learning: the reference's greedy controller (envs/large_grid_env.py:56-60, envs/real_net_env.py:78-111)
@@ -85,13 +89,15 @@ p.add_argument("--scenario", default="grid", choices=["grid", "real"])
 p.add_argument("--policy", default="lstm", choices=["lstm", "fc"])
 p.add_argument("--fp32", action="store_true")
 p.add_argument("--reward-norm", type=float, default=None)
-p.add_argument("--lr", type=float, default=5e-4)
+p.add_argument("--lr", type=float, default=None, help="default 5e-4 (A2C), 1e-4 (IQL)")
+p.add_argument("--eval-seeds", default="10000,20000", help="IQL: test seeds of the evaluation after training")
 p.add_argument("--seed", type=int, default=1)
 p.add_argument("--tag", default=None)
 p.add_argument("--greedy", action="store_true")
 a = p.parse_args()
 R, agent = a.replicas, a.agent
-tag = a.tag or "%s_%s_%s%s" % (agent, a.scenario, a.policy, "_fp32" if a.fp32 else "")
+tag = a.tag or ("%s_%s" % (agent, a.scenario) if agent in ("iqll", "iqld") else
+                "%s_%s_%s%s" % (agent, a.scenario, a.policy, "_fp32" if a.fp32 else ""))
 
 if a.scenario == "real":
     from deeprl_signal_control_b200.net.real_net import real_net_tables
@@ -135,6 +141,49 @@ if a.greedy:
                "wall_s": time.time() - t0}, open(out_path(tag), "w"))
     sys.exit(0)
 
+if agent in ("iqll", "iqld"):
+    # reference config/config_iql{l,d}_{large,real}.ini, MODEL_CONFIG
+    import configparser
+    from deeprl_signal_control_b200.agents.evaluator import Evaluator
+    from deeprl_signal_control_b200.agents.layout import QLayout
+    from deeprl_signal_control_b200.agents.learner_iql import BatchedIQL, BatchedIQLTrainer
+    from deeprl_signal_control_b200.agents.utils import Scheduler
+    kind = "dqn" if agent == "iqld" else "lr"
+    lr = 1e-4 if a.lr is None else a.lr
+    rn = (1.0 if a.scenario == "real" else 3000.0) if a.reward_norm is None else a.reward_norm
+    cp = configparser.ConfigParser()
+    cp.read_string("[MODEL_CONFIG]\nmax_grad_norm = 40\ngamma = 0.99\nnum_fc = 128\nnum_h = 64\nbatch_size = 20\n"
+                   "buffer_size = 1000\nreward_norm = %r\nreward_clip = 2.0\n" % rn)
+    total_step = 1e6
+    off = np.asarray(net.node_obs_off)
+    qlay = QLayout(kind, [int(off[i + 1] - off[i]) for i in range(net.n_nodes)], net.n_a_ls, net.n_w_ls, off, net.n_obs,
+                   n_fc=128, n_ft=32, n_h=64, max_na=net.max_na)
+    model = BatchedIQL(qlay, R, cp["MODEL_CONFIG"], kind, seed=a.seed)
+    tr = BatchedIQLTrainer(sim, model, Scheduler(lr, decay="constant"), Scheduler(1.0, 0.01, total_step * 0.5), seed0=12)
+    curve = []
+    while len(tr.episode_rewards) < a.episodes:
+        tr.run(tr.T_episode)
+        torch.cuda.synchronize()
+        curve = list(tr.episode_rewards)
+        print("episode %3d  mean step reward %9.2f   loss[0] %.4g   grad-norm[0] %.3f   %.1fs" %
+              (len(curve), curve[-1], float(model.losses[-1, 0]), float(model.norms[-1, 0]), time.time() - t0), flush=True)
+    seeds = [int(x) for x in a.eval_seeds.split(",")]
+    ecp = configparser.ConfigParser()
+    ecp.read_string(GREEDY_INI[a.scenario].replace("agent = greedy", "agent = " + agent) % ",".join(map(str, seeds)))
+    if a.scenario == "real":
+        from deeprl_signal_control_b200.envs.real_net_env import RealNetEnv as Env
+    else:
+        from deeprl_signal_control_b200.envs.large_grid_env import LargeGridEnv as Env
+    env = Env(ecp["ENV_CONFIG"], n_replicas=len(seeds))
+    mean, std = Evaluator(env, model, "", policy_type="default").perform_all()
+    print("evaluation on seeds %s: mean step reward %s" % (seeds, np.round(mean, 2).tolist()), flush=True)
+    json.dump({"agent": agent, "scenario": a.scenario, "replicas": R, "episodes": len(curve), "lr": lr, "reward_norm": rn,
+               "mean_episode_reward": curve, "eval_seeds": seeds, "eval_mean": [float(x) for x in mean],
+               "eval_std": [float(x) for x in std], "wall_s": time.time() - t0, "env_steps": tr.n_env_steps},
+              open(out_path(tag), "w"))
+    sys.exit(0)
+
+a.lr = 5e-4 if a.lr is None else a.lr
 lay = PolicyLayout(net.n_s_ls, net.n_a_ls, net.n_w_ls, net.n_f_ls, net.node_obs_off, net.n_obs, fw=128, ft=32,
                    ff=64 if agent == "ma2c" else 0, h=64, max_na=net.max_na, recurrent=a.policy != "fc")
 kw = dict(use_tc=False, allow_tf32=False) if a.fp32 else {}
