@@ -1153,7 +1153,7 @@ struct BwdTC {
   const __nv_bfloat16* Cb;   //           ([2A][T*Rc][256] / [..][64]); when set, ZG is write-only and C is unused
   __nv_bfloat16* dZb;        // optional: dZ as bf16 [2A][T*Rc][256] (operand of the tensor-core weight-gradient kernels);
                              //           ZG may then be null (needs Gb / Cb)
-  unsigned long long* prof;  // optional: 8 phase counters of the staged kernel (tscl_debug_bptt_prof)
+  unsigned long long* prof;  // optional: phase counters of lstm_bwd_tc_regs_kernel (tscl_debug_bptt_prof)
 };
 
 // NT = 512: thread = (replica row, 16 hidden units), one CTA per SM.
@@ -1346,248 +1346,243 @@ lstm_bwd_tc_kernel(const DDimsTC d, const BwdTC a) {
 }
 
 // ---------------------------------------------------------------------------------------------------
-// BPTT, staged variant (the activation-store path of the training loop: gates / c from the bf16 store, dZ written as
-// bf16).  Same arithmetic as lstm_bwd_tc_kernel<512>; what changes is how the operands reach the threads.  There a
-// thread owns (row, 16 hidden units) and loads its 16-byte pieces straight from global memory, 128-512 B apart between
-// the lanes of a warp (32 sectors per load instruction).  Here each step's tile — gates [128 x 512 B], c_{t-1} [128 x 128 B], dH [128 x 256 B] — is fetched by
-// coalesced 16-byte cp.async (one row segment per warp instruction) into XOR-swizzled shared memory one step AHEAD
-// (issued as soon as every thread has taken step t's operands into registers, landing while step t's cell math, MMA
-// and accumulator read-back run), and the threads pick their pieces from there without bank conflicts.
-__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
+// BPTT with the recurrence in registers: the activation-store path of the training loop (gates / c from the bf16 store,
+// dZ written as bf16).  Same operands, k-step order, per-element formulas and bf16 rounding points as
+// lstm_bwd_tc_kernel<512>, hence the same bits.  A CTA takes the same (unit, 128-row tile) items; each of its two
+// warpgroups owns 64 of the rows and runs its own step loop, and the two meet only between items (they share the
+// unit's Wh^T image).
+// Why no accumulator tile is needed: with k = gate * 64 + unit, k-step 4 g + c of an RS-form wgmma m64n64k16 takes from
+// thread (warp w of the warpgroup, lane l) rows 16 w + l / 4 (+ 8) and units 16 c + 2 (l % 4) + {0, 1, 8, 9} of gate g.
+// Over c = 0..3 those are units 8 j + 2 (l % 4) + {0, 1}, j = 0..7: exactly the accumulator columns the same thread
+// holds for the same rows.  So the thread that computes dz for (row, unit, all four gates) supplies it as the A
+// operand, and receives dh_{t-1} for that (row, unit) in its own accumulator.
+// Per step and warpgroup:
+//   1. wait on the warpgroup's mbarrier for step t's operands (TMA copies, 128-byte swizzle);
+//   2. ldmatrix (gates, c_t, c_{t-1}: the fragment layout straight out of the swizzled boxes), 8-byte reads for dH;
+//   3. warpgroup barrier, then one thread issues step t-1's copies into the buffers just read;
+//   4. cell backward -> the 16 A fragments (bf16 pairs, lower column in the low half) and the dc carry;
+//   5. stmatrix of the fragments into a swizzled staging tile, 16 RS wgmmas, warpgroup barrier, TMA store of dZ;
+//   6. wait for the MMA: dh_{t-1} = accumulator * keep is the next step's carry.
+// The tensor maps are 3-D [2A * T][Rc][cols], so every copy is clipped at Rc: rows past Rc read as zero and are never
+// written, and no copy reaches another step's rows.
+#define BR_WG_BYTES (96 * 1024)   // per warpgroup: gates 4 x 8 KB | dH 2 x 8 KB | c ring 2 x 8 KB | dZ staging 4 x 8 KB
+#define BR_SMEM (BW_KC * 1024 + 2 * BR_WG_BYTES + 16)
+__device__ __forceinline__ void ldsm_x4(uint32_t (&r)[4], uint32_t addr) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr) : "memory");
 }
-// TMA = true: the per-step operand tile (gates 64 KB, dH 32 KB, c 16 KB) arrives by SEVEN cp.async.bulk.tensor copies issued
-// by one thread (hardware 128-byte swizzle = the pattern the readers use) instead of 14 cp.async per thread, whose issue
-// (7168 16-byte copies per step) blocks every warp.
-template <bool PROF, bool TMA>
-__global__ void __launch_bounds__(512, 1)
-lstm_bwd_tc_staged_kernel(const DDimsTC d, const BwdTC a, const __grid_constant__ CUtensorMap mapG,
-                          const __grid_constant__ CUtensorMap mapC, const __grid_constant__ CUtensorMap mapD) {
-  constexpr int NT = 512, HPT = 16, NSUB = 2;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  long long bp[8] = {0, 0, 0, 0, 0, 0, 0, 0}, pc = 0;
-#define BP_MARK(i) do { if (PROF && tid == 0) { const long long c_ = clock64(); bp[i] += c_ - pc; pc = c_; } } while (0)
-  unsigned char* sB = tc_smem;                       // 32 KB : Wh^T image
-  unsigned char* sA = sB + BW_KC * 1024;             // 64 KB : dz tile (A operand)
-  unsigned char* sG = sA + BW_KC * 2048;             // 64 KB : gates [128][32 chunks ^ (row & 31)]   (1024-byte aligned)
-                                                     //         TMA: 4 boxes [128 rows][8 chunks ^ (row & 7)], one per gate
-  unsigned char* sC0 = sG + 128 * 512;               // 16 KB x 2 : c ring, [128][8 chunks ^ (row & 7)]
-  unsigned char* sD = sC0 + 2 * 128 * 128;           // 32 KB : dH fp32 [128][16 chunks ^ (row & 15)]; TMA: 2 boxes of 32 floats
-  uint64_t* sBar = reinterpret_cast<uint64_t*>(sD + 128 * 256);
-  const uint32_t bar = smem_u32(sBar), ldbar = bar + 8;
-  uint32_t ldpar = 0;
-  if (tid == 0) {
-    mbar_init(bar, 1); mbar_init(ldbar, 1);
+__device__ __forceinline__ void stsm_x4(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};"
+               ::"r"(addr), "r"(r0), "r"(r1), "r"(r2), "r"(r3) : "memory");
+}
+// bf16 pair, `lo` in the low half (round to nearest even, as __float2bfloat16_rn)
+__device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
+  uint32_t r;
+  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
+  return r;
+}
+__device__ __forceinline__ float bf16_lo(uint32_t v) { return __uint_as_float(v << 16); }
+__device__ __forceinline__ float bf16_hi(uint32_t v) { return __uint_as_float(v & 0xffff0000u); }
+// m64n64k16 with A from registers (this thread's four bf16 pairs) and B K-major in shared memory
+__device__ __forceinline__ void wgmma_n64_rs(float (&d)[32], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint64_t db,
+                                             uint32_t accum) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, {%32,%33,%34,%35}, %36, p, 1, 1, 0;\n\t}"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+               : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(db), "r"(accum) : "memory");
+}
+__device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* m, int x, int y, int z, uint32_t bar) {
+  asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];"
+               ::"r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(x), "r"(y), "r"(z), "r"(bar) : "memory");
+}
+__device__ __forceinline__ void tma_store_3d(const CUtensorMap* m, int x, int y, int z, uint32_t src) {
+  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%1, %2, %3}], [%4];"
+               ::"l"(reinterpret_cast<uint64_t>(m)), "r"(x), "r"(y), "r"(z), "r"(src) : "memory");
+}
+
+// PROF: clock64 phase sums of thread 0 of every warpgroup into a.prof[0..3] (operand wait | smem -> regs + cell backward |
+// MMA issue -> wait | dZ store), a separate instantiation (tscl_debug_bptt_prof)
+template <bool PROF>
+__global__ void __launch_bounds__(256, 1)
+lstm_bwd_tc_regs_kernel(const DDimsTC d, const BwdTC a, const __grid_constant__ CUtensorMap mapG,
+                        const __grid_constant__ CUtensorMap mapC, const __grid_constant__ CUtensorMap mapD,
+                        const __grid_constant__ CUtensorMap mapZ) {
+  const int tid = threadIdx.x, wg = tid >> 7, w = (tid >> 5) & 3, lane = tid & 31, q = lane & 3;
+  const bool lead = (tid & 127) == 0;
+  long long bp[4] = {0, 0, 0, 0}, pc = 0;
+#define BR_MARK(i) do { if (PROF && lead) { const long long c_ = clock64(); bp[i] += c_ - pc; pc = c_; } } while (0)
+  unsigned char* sB = tc_smem;                                       // 32 KB: Wh^T image, shared by both warpgroups
+  unsigned char* sW = sB + BW_KC * 1024 + wg * BR_WG_BYTES;          // this warpgroup's buffers (1024-byte aligned)
+  const uint32_t aB = smem_u32(sB), aG = smem_u32(sW), aD = aG + 32768, aC = aG + 49152, aZ = aG + 65536;
+  const uint32_t ldbar = smem_u32(sB + BW_KC * 1024 + 2 * BR_WG_BYTES) + 8 * wg;
+  if (lead) {
+    mbar_init(ldbar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
-  float* const acc = a.acc + (size_t)blockIdx.x * TC_M * ACC_COLS;
-  const uint32_t aA = smem_u32(sA), aB = smem_u32(sB);
-  const uint32_t aG = smem_u32(sG), aC = smem_u32(sC0), aD = smem_u32(sD);
+  // ldmatrix / stmatrix lane address in a [64 rows][128 B] swizzled box for 16-byte chunks 2 c, 2 c + 1: lanes 0-7 / 8-15 /
+  // 16-23 / 24-31 give the rows of matrices (rows 16 w.., chunk 2 c) / (rows 16 w + 8.., 2 c) / (16 w.., 2 c + 1) /
+  // (16 w + 8.., 2 c + 1), which are this thread's fragment registers (j = 2 c, row r) (2 c, r + 8) (2 c + 1, r) (2 c + 1, r + 8)
+  const uint32_t lm_row = (uint32_t)(16 * w + (lane & 7) + ((lane >> 3) & 1) * 8) * 128, lm_sw = lane & 7, lm_hi = lane >> 4;
+  auto lm = [&](uint32_t box, int c) { return box + lm_row + (((2 * c + lm_hi) ^ lm_sw) << 4); };
+  const int rq = 16 * w + (lane >> 2);                               // the thread's rows: rq, rq + 8 of the warpgroup's 64
   const int64_t n_tiles = (a.Rc + TC_M - 1) / TC_M;
   const int64_t n_items = n_tiles * 2 * d.A;
   int cur_u = -1;
-  uint32_t parity = 0;
-  const int q = warp & 3, qt = warp >> 2;            // row quadrant of the accumulator tile, hidden-unit group (16 units)
-  const int row = q * 32 + lane, jq = qt * HPT;
-  auto bf8 = [](const uint4 v, float* o) {
-    const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-    for (int i = 0; i < 4; ++i) { o[2 * i] = __uint_as_float(w[i] << 16); o[2 * i + 1] = __uint_as_float(w[i] & 0xffff0000u); }
-  };
+  uint32_t ldpar = 0;
   for (int64_t it = blockIdx.x; it < n_items; it += gridDim.x) {
     const int u = (int)(it / n_tiles);
-    const int64_t rt0 = (it - (int64_t)u * n_tiles) * TC_M;       // first replica row of the tile
-    const int64_t r = rt0 + row;
-    const bool valid = r < a.Rc;
-    __syncthreads();
+    const int rw0 = (int)((it - (int64_t)u * n_tiles) * TC_M) + 64 * wg;   // first row of this warpgroup
+    __syncthreads();                                                 // both warpgroups are done with the previous item
     if (u != cur_u) {
       cur_u = u;
       const uint4* src = reinterpret_cast<const uint4*>(a.Wt + (int64_t)u * BW_KC * TC_H * 8);
       uint4* dst = reinterpret_cast<uint4*>(sB);
-      for (int i = tid; i < BW_KC * TC_H; i += NT) dst[i] = src[i];
+      for (int i = tid; i < BW_KC * TC_H; i += 256) dst[i] = src[i];
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic writes -> operand of the wgmmas
+      __syncthreads();
     }
-    // coalesced fetch of one step's tile: rows beyond Rc are clamped to a valid row (their results are never stored)
+    if (rw0 >= a.Rc) continue;                                       // a partial tile with no row for this warpgroup
+    const int z0 = u * a.T;                                          // plane of step 0 in the [2A * T][Rc][cols] maps
+    // step t's gates and dH, c_{t-1} into its ring slot, and c_t as well for the item's first step (lead thread)
     auto fetch = [&](int t, bool with_c_t) {
-      const int64_t mb = ((int64_t)u * a.T + t) * a.Rc;            // row index of replica 0 at step t
-      if constexpr (TMA) {
-        if (tid == 0) {       // rows past the end of the tensors are zero-filled; rows past Rc belong to other tiles and are never stored
-          auto tma2d = [&](uint32_t dst, const CUtensorMap* mp, int x, int64_t y) {
-            asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
-                         ::"r"(dst), "l"(reinterpret_cast<uint64_t>(mp)), "r"(x), "r"((int)y), "r"(ldbar) : "memory");
-          };
-          const int64_t y = mb + rt0;
-          mbar_expect_tx(ldbar, (uint32_t)(65536 + 32768 + (with_c_t ? 16384 : 0) + (t > 0 ? 16384 : 0)));
+      mbar_expect_tx(ldbar, (uint32_t)(32768 + 16384 + (with_c_t ? 8192 : 0) + (t > 0 ? 8192 : 0)));
 #pragma unroll
-          for (int g = 0; g < 4; ++g) tma2d(aG + g * 16384, &mapG, g * 64, y);
-          tma2d(aD, &mapD, 0, y); tma2d(aD + 16384, &mapD, 32, y);
-          if (with_c_t) tma2d(aC + (t & 1) * 16384, &mapC, 0, y);
-          if (t > 0) tma2d(aC + ((t - 1) & 1) * 16384, &mapC, 0, y - a.Rc);
-        }
-        return;
-      }
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {                                // gates: 128 rows x 32 chunks
-        const int id = i * NT + tid, rw = id >> 5, c = id & 31;
-        const int64_t rr = rt0 + rw < a.Rc ? rt0 + rw : a.Rc - 1;
-        cp_async16(aG + rw * 512 + ((c ^ (rw & 31)) << 4), a.Gb + (mb + rr) * TC_N + c * 8);
-      }
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {                                // dH fp32: 128 rows x 16 chunks
-        const int id = i * NT + tid, rw = id >> 4, c = id & 15;
-        const int64_t rr = rt0 + rw < a.Rc ? rt0 + rw : a.Rc - 1;
-        cp_async16(aD + rw * 256 + ((c ^ (rw & 15)) << 4), a.dH + (mb + rr) * TC_H + c * 4);
-      }
-#pragma unroll
-      for (int i = 0; i < 2; ++i) {                                // c_{t-1} (and c_t for the first step): 128 rows x 8 chunks
-        const int id = i * NT + tid, rw = id >> 3, c = id & 7;
-        const int64_t rr = rt0 + rw < a.Rc ? rt0 + rw : a.Rc - 1;
-        const uint32_t off = rw * 128 + ((c ^ (rw & 7)) << 4);
-        if (with_c_t) cp_async16(aC + (t & 1) * 16384 + off, a.Cb + (mb + rr) * TC_H + c * 8);
-        if (t > 0) cp_async16(aC + ((t - 1) & 1) * 16384 + off, a.Cb + (mb - a.Rc + rr) * TC_H + c * 8);
-      }
-      asm volatile("cp.async.commit_group;" ::: "memory");
+      for (int g = 0; g < 4; ++g) tma_load_3d(aG + g * 8192, &mapG, g * 64, rw0, z0 + t, ldbar);
+      tma_load_3d(aD, &mapD, 0, rw0, z0 + t, ldbar);
+      tma_load_3d(aD + 8192, &mapD, 32, rw0, z0 + t, ldbar);
+      if (with_c_t) tma_load_3d(aC + (t & 1) * 8192, &mapC, 0, rw0, z0 + t, ldbar);
+      if (t > 0) tma_load_3d(aC + ((t - 1) & 1) * 8192, &mapC, 0, rw0, z0 + t - 1, ldbar);
     };
-    fetch(a.T - 1, true);
-    float dc[HPT], dhc[HPT];
+    if (lead) fetch(a.T - 1, true);
+    // per-thread state, entry [j][e]: row rq + 8 (e >> 1), unit 8 j + 2 q + (e & 1) (= accumulator entry 4 j + e)
+    float dc[8][4], dhc[8][4];
 #pragma unroll
-    for (int e = 0; e < HPT; ++e) { dc[e] = 0.f; dhc[e] = 0.f; }
-    if (PROF && tid == 0) pc = clock64();
+    for (int j = 0; j < 8; ++j)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) { dc[j][e] = 0.f; dhc[j][e] = 0.f; }
+    if (PROF && lead) pc = clock64();
     for (int t = a.T - 1; t >= 0; --t) {
       const float keep = 1.0f - a.done[t];
-      const int64_t m = ((int64_t)u * a.T + t) * a.Rc + (valid ? r : 0);
-      if (!TMA && t > 1) {      // pull step t-2's operands towards L2: they are fetched into shared memory during step t-1
-        const int64_t mp = ((int64_t)u * a.T + t - 2) * a.Rc + (valid ? r : 0);
-        asm volatile("prefetch.global.L2 [%0];" ::"l"(a.Gb + mp * TC_N + qt * 64));
-        if (qt == 0) asm volatile("prefetch.global.L2 [%0];" ::"l"(a.Cb + mp * TC_H));
-        if (qt >= 2) asm volatile("prefetch.global.L2 [%0];" ::"l"(a.dH + mp * TC_H + (qt - 2) * 32));
-      }
-      if constexpr (TMA) {
-        mbar_wait(ldbar, ldpar); ldpar ^= 1;          // step t's tile has landed (complete_tx of all its copies)
-      } else {
-        asm volatile("cp.async.wait_group 0;" ::: "memory");
-        __syncthreads();                            // step t's tile is in shared memory
-      }
-      BP_MARK(0);                                   // waiting for step t's operands
-      const unsigned char* cT = sC0 + (t & 1) * 16384;
-      const unsigned char* cP = sC0 + ((t - 1) & 1) * 16384;
-      uint4 zpk[4][NSUB];
+      mbar_wait(ldbar, ldpar); ldpar ^= 1;                           // step t's operands have landed
+      BR_MARK(0);
+      // shared memory -> registers; bf16 pairs [j][h]: row rq + 8 h, units 8 j + 2 q + {0 (low half), 1}
+      uint32_t gr[4][8][2], cr[8][2], pr[8][2];
 #pragma unroll
-      for (int jb = 0; jb < NSUB; ++jb) {
-        const int jo = jq + jb * 8;
-        float gi[8], gf[8], go[8], gu[8], ct[8], cp[8], dh[8];
-        {
-          const int cg = jo >> 3, sw = row & 31;     // chunk of 8 hidden units inside each 64-wide gate block
-          if constexpr (TMA) {
-            const unsigned char* gp = sG + row * 128 + ((cg ^ (row & 7)) << 4);
-            bf8(*reinterpret_cast<const uint4*>(gp), gi);
-            bf8(*reinterpret_cast<const uint4*>(gp + 16384), gf);
-            bf8(*reinterpret_cast<const uint4*>(gp + 32768), go);
-            bf8(*reinterpret_cast<const uint4*>(gp + 49152), gu);
-          } else {
-          bf8(*reinterpret_cast<const uint4*>(sG + row * 512 + (((cg) ^ sw) << 4)), gi);
-          bf8(*reinterpret_cast<const uint4*>(sG + row * 512 + (((8 + cg) ^ sw) << 4)), gf);
-          bf8(*reinterpret_cast<const uint4*>(sG + row * 512 + (((16 + cg) ^ sw) << 4)), go);
-          bf8(*reinterpret_cast<const uint4*>(sG + row * 512 + (((24 + cg) ^ sw) << 4)), gu);
-          }
-          bf8(*reinterpret_cast<const uint4*>(cT + row * 128 + ((cg ^ (row & 7)) << 4)), ct);
-          if (t > 0) bf8(*reinterpret_cast<const uint4*>(cP + row * 128 + ((cg ^ (row & 7)) << 4)), cp);
-          else if (valid) {
-            const float4 x = reinterpret_cast<const float4*>(a.c0 + ((int64_t)u * a.ld_state + a.r0 + r) * TC_H + jo)[0];
-            const float4 y = reinterpret_cast<const float4*>(a.c0 + ((int64_t)u * a.ld_state + a.r0 + r) * TC_H + jo)[1];
-            cp[0] = x.x; cp[1] = x.y; cp[2] = x.z; cp[3] = x.w; cp[4] = y.x; cp[5] = y.y; cp[6] = y.z; cp[7] = y.w;
-          } else {
-#pragma unroll
-            for (int e = 0; e < 8; ++e) cp[e] = 0.f;
-          }
-          const int cd = jo >> 2;                    // dH: 4 floats per chunk
-          const float4 d0 = TMA ? *reinterpret_cast<const float4*>(sD + (cd >> 3) * 16384 + row * 128 + (((cd & 7) ^ (row & 7)) << 4))
-                                : *reinterpret_cast<const float4*>(sD + row * 256 + ((cd ^ (row & 15)) << 4));
-          const float4 d1 = TMA ? *reinterpret_cast<const float4*>(sD + (cd >> 3) * 16384 + row * 128 + ((((cd + 1) & 7) ^ (row & 7)) << 4))
-                                : *reinterpret_cast<const float4*>(sD + row * 256 + (((cd + 1) ^ (row & 15)) << 4));
-          dh[0] = d0.x; dh[1] = d0.y; dh[2] = d0.z; dh[3] = d0.w; dh[4] = d1.x; dh[5] = d1.y; dh[6] = d1.z; dh[7] = d1.w;
-#pragma unroll
-          for (int e = 0; e < 8; ++e) cp[e] *= keep;
-          if (!valid) {
-#pragma unroll
-            for (int e = 0; e < 8; ++e) { gi[e] = gf[e] = go[e] = gu[e] = ct[e] = cp[e] = dh[e] = 0.f; }
-          }
-        }
-        if (jb == NSUB - 1) {      // every thread holds its last operands: the staging buffers can take step t-1
-          BP_MARK(5);              // shared memory -> registers (both sub-batches) + first sub-batch's math and stores
-          __syncthreads();
-          BP_MARK(6);              // barrier: staging buffers free
-          if (t > 0) fetch(t - 1, false);
-          BP_MARK(7);              // cp.async issue of step t-1
-        }
-        float dzi[8], dzf[8], dzo[8], dzu[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) {
-          const int k = jb * 8 + e;
-          const float dht = dh[e] + dhc[k];
-          const float tc = tanh_fast(ct[e]);
-          const float dcc = dc[k] + dht * go[e] * (1.0f - tc * tc);
-          dzi[e] = dcc * gu[e] * gi[e] * (1.0f - gi[e]);
-          dzf[e] = dcc * cp[e] * gf[e] * (1.0f - gf[e]);
-          dzo[e] = dht * tc * go[e] * (1.0f - go[e]);
-          dzu[e] = dcc * gi[e] * (1.0f - gu[e] * gu[e]);
-          dc[k] = dcc * gf[e] * keep;
-        }
-        const float* srcs[4] = {dzi, dzf, dzo, dzu};
+      for (int c = 0; c < 4; ++c) {
+        uint32_t r[4];
 #pragma unroll
         for (int g = 0; g < 4; ++g) {
-          __align__(16) __nv_bfloat16 v[8];
-#pragma unroll
-          for (int e = 0; e < 8; ++e) v[e] = __float2bfloat16_rn(srcs[g][e]);
-          *reinterpret_cast<uint4*>(sA + (size_t)((g * 64 + jo) >> 3) * 2048 + row * 16) = *reinterpret_cast<const uint4*>(v);
-          zpk[g][jb] = *reinterpret_cast<const uint4*>(v);
+          ldsm_x4(r, lm(aG + g * 8192, c));
+          gr[g][2 * c][0] = r[0]; gr[g][2 * c][1] = r[1]; gr[g][2 * c + 1][0] = r[2]; gr[g][2 * c + 1][1] = r[3];
+        }
+        ldsm_x4(r, lm(aC + (t & 1) * 8192, c));
+        cr[2 * c][0] = r[0]; cr[2 * c][1] = r[1]; cr[2 * c + 1][0] = r[2]; cr[2 * c + 1][1] = r[3];
+        if (t > 0) {
+          ldsm_x4(r, lm(aC + ((t - 1) & 1) * 8192, c));
+          pr[2 * c][0] = r[0]; pr[2 * c][1] = r[1]; pr[2 * c + 1][0] = r[2]; pr[2 * c + 1][1] = r[3];
         }
       }
-      if (valid) {      // dZ of this thread's 16 hidden units: two 128-bit stores (a full sector) per gate
+      float dht[8][4];                                               // dH + dh carry
 #pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          const uint4 x = zpk[g][0], y = zpk[g][1];
-          reinterpret_cast<uint4*>(a.dZb + m * TC_N + g * 64 + jq)[0] = x;
-          reinterpret_cast<uint4*>(a.dZb + m * TC_N + g * 64 + jq)[1] = y;
+      for (int j = 0; j < 8; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = rq + 8 * h;
+          const float2 v = *reinterpret_cast<const float2*>(sW + 32768 + (j >> 2) * 8192 + row * 128 +
+                                                           (((2 * (j & 3) + (q >> 1)) ^ (row & 7)) << 4) + 8 * (q & 1));
+          dht[j][2 * h] = v.x + dhc[j][2 * h];
+          dht[j][2 * h + 1] = v.y + dhc[j][2 * h + 1];
         }
-      }
-      BP_MARK(1);                                   // second sub-batch: cell backward, dZ stores
-      if (keep != 0.f && t > 0) {
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        __syncthreads();
-        BP_MARK(2);                                 // barrier before the MMA
-        if (warp < 8) {
-          wg_mma<0, 0>(acc, 0, TC_H, 16, false, [&](int ks, uint64_t& da, uint64_t& db) {
-            da = make_desc(aA + ks * 2 * 2048, 2048, 128);
-            db = make_desc(aB + ks * 2 * 1024, 1024, 128);
-          });
-          wg_mma_done(bar);
+      if (lead) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");   // the last dZ store has left the staging tile
+      asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");    // the operand buffers are free
+      if (lead && t > 0) fetch(t - 1, false);
+      // cell backward (the formulas of lstm_bwd_tc_kernel) -> A fragments af[g][j][h]
+      uint32_t af[4][8][2];
+#pragma unroll
+      for (int j = 0; j < 8; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float cp2[2];
+          if (t > 0) {
+            cp2[0] = bf16_lo(pr[j][h]); cp2[1] = bf16_hi(pr[j][h]);
+          } else {
+            const int64_t r = rw0 + rq + 8 * h;
+            float2 v = make_float2(0.f, 0.f);
+            if (r < a.Rc) v = *reinterpret_cast<const float2*>(a.c0 + ((int64_t)u * a.ld_state + a.r0 + r) * TC_H + 8 * j + 2 * q);
+            cp2[0] = v.x; cp2[1] = v.y;
+          }
+          float z[4][2];
+#pragma unroll
+          for (int ee = 0; ee < 2; ++ee) {
+            const int e = 2 * h + ee;
+            const float gi = ee ? bf16_hi(gr[0][j][h]) : bf16_lo(gr[0][j][h]);
+            const float gf = ee ? bf16_hi(gr[1][j][h]) : bf16_lo(gr[1][j][h]);
+            const float go = ee ? bf16_hi(gr[2][j][h]) : bf16_lo(gr[2][j][h]);
+            const float gu = ee ? bf16_hi(gr[3][j][h]) : bf16_lo(gr[3][j][h]);
+            const float ct = ee ? bf16_hi(cr[j][h]) : bf16_lo(cr[j][h]);
+            const float cp = cp2[ee] * keep;
+            const float dh = dht[j][e];
+            const float tc = tanh_fast(ct);
+            const float dcc = dc[j][e] + dh * go * (1.0f - tc * tc);
+            z[0][ee] = dcc * gu * gi * (1.0f - gi);
+            z[1][ee] = dcc * cp * gf * (1.0f - gf);
+            z[2][ee] = dh * tc * go * (1.0f - go);
+            z[3][ee] = dcc * gi * (1.0f - gu * gu);
+            dc[j][e] = dcc * gf * keep;
+          }
+#pragma unroll
+          for (int g = 0; g < 4; ++g) af[g][j][h] = pack_bf16x2(z[g][0], z[g][1]);
         }
-        mbar_wait(bar, parity);
-        parity ^= 1;
-        BP_MARK(3);                                 // MMA issue + commit + wait
-        float dhp[HPT];
-        acc_ld16(acc, ((uint32_t)(q * 32) << 16) + (uint32_t)jq, dhp);
+      BR_MARK(1);
 #pragma unroll
-        for (int e = 0; e < HPT; ++e) dhc[e] = dhp[e] * keep;
-        BP_MARK(4);                                 // accumulator read-back
-      } else {
+      for (int g = 0; g < 4; ++g)
 #pragma unroll
-        for (int e = 0; e < HPT; ++e) dhc[e] = 0.f;
+        for (int c = 0; c < 4; ++c)
+          stsm_x4(lm(aZ + g * 8192, c), af[g][2 * c][0], af[g][2 * c][1], af[g][2 * c + 1][0], af[g][2 * c + 1][1]);
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // staging tile -> the TMA store
+      BR_MARK(3);
+      // The MMA is issued on every step (a branch around it makes ptxas serialise the wgmmas); its result is used only
+      // where lstm_bwd_tc_kernel runs it, keep != 0 and t > 0.
+      float acc[32];
+#pragma unroll
+      for (int i = 0; i < 32; ++i) acc[i] = 0.f;
+      wg_fence();
+#pragma unroll
+      for (int g = 0; g < 4; ++g)
+#pragma unroll
+        for (int c = 0; c < 4; ++c)                                  // k-step 4 g + c, in order
+          wgmma_n64_rs(acc, af[g][2 * c][0], af[g][2 * c][1], af[g][2 * c + 1][0], af[g][2 * c + 1][1],
+                       make_desc(aB + (4 * g + c) * 2 * 1024, 1024, 128), (g | c) != 0);
+      wg_commit();
+      BR_MARK(2);
+      asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");    // the whole staging tile is written
+      if (lead) {
+#pragma unroll
+        for (int g = 0; g < 4; ++g) tma_store_3d(&mapZ, g * 64, rw0, z0 + t, aZ + g * 8192);
+        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
       }
+      BR_MARK(3);
+      wg_wait<0>();
+      wg_frag_fence(acc);
+      const bool need_dh = keep != 0.f && t > 0;
+#pragma unroll
+      for (int j = 0; j < 8; ++j)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) dhc[j][e] = need_dh ? acc[4 * j + e] * keep : 0.f;
+      BR_MARK(2);
     }
   }
-  if (PROF && tid == 0)
-    for (int i = 0; i < 8; ++i) atomicAdd(a.prof + i, (unsigned long long)bp[i]);
-#undef BP_MARK
-  asm volatile("cp.async.wait_group 0;" ::: "memory");
-  __syncthreads();
+  if (lead) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // dZ stores complete before the CTA leaves
+  if (PROF && lead)
+    for (int i = 0; i < 4; ++i) atomicAdd(a.prof + i, (unsigned long long)bp[i]);
+#undef BR_MARK
 }
 
-// 2-D tiled tensor map (row-major [rows][cols], box = box_cols x box_rows, inner box = 128 bytes, 128-byte swizzle) through the
-// driver entry point (no link-time dependency on libcuda)
-static bool make_tmap_2d(CUtensorMap* m, CUtensorMapDataType dt, int elem_bytes, const void* base, uint64_t rows, uint64_t cols,
-                         uint32_t box_cols, uint32_t box_rows) {
+// 3-D tiled tensor map over row-major [planes][rows][cols] (box = box_cols x box_rows x 1, inner box = 128 bytes,
+// 128-byte swizzle) through the driver entry point (no link-time dependency on libcuda)
+static bool make_tmap_3d(CUtensorMap* m, CUtensorMapDataType dt, int elem_bytes, const void* base, uint64_t planes,
+                         uint64_t rows, uint64_t cols, uint32_t box_cols, uint32_t box_rows) {
   typedef CUresult (*encode_fn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                 const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                 CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -1599,12 +1594,18 @@ static bool make_tmap_2d(CUtensorMap* m, CUtensorMapDataType dt, int elem_bytes,
     return (encode_fn)p;
   }();
   if (!fn || !base) return false;
-  const cuuint64_t dims[2] = {cols, rows};
-  const cuuint64_t strides[1] = {cols * (uint64_t)elem_bytes};
-  const cuuint32_t box[2] = {box_cols, box_rows};
-  const cuuint32_t es[2] = {1, 1};
-  return fn(m, dt, 2, const_cast<void*>(base), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+  memset(m, 0, sizeof(*m));
+  const cuuint64_t dims[3] = {cols, rows, planes};
+  const cuuint64_t strides[2] = {cols * (uint64_t)elem_bytes, rows * cols * (uint64_t)elem_bytes};
+  const cuuint32_t box[3] = {box_cols, box_rows, 1};
+  const cuuint32_t es[3] = {1, 1, 1};
+  return fn(m, dt, 3, const_cast<void*>(base), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
             CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+
+// 16-byte cp.async global -> shared (the dX kernel's operand loader)
+__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
 }
 
 extern "C" int tscl_pack_wxt(tscl_handle* h, const float* params, void* wxt_bf16, void* stream) {
@@ -1667,37 +1668,32 @@ extern "C" int tscl_lstm_seq_bwd_tc_dx(tscl_handle* h, const void* wt_bf16, floa
   // default: the one-CTA-per-SM 512-thread variant; TSC_BPTT_THREADS=256 selects the two-CTA-per-SM 256-thread variant
   // for experiments (same arithmetic, same bits)
   static const int bw_threads = []() { const char* e = getenv("TSC_BPTT_THREADS"); return e && atoi(e) == 256 ? 256 : 512; }();
-  // staged variant (coalesced cp.async into swizzled shared memory one step ahead): store path without fused dX
+  // store path without fused dX: the register-recurrence kernel (TSC_BPTT_STAGED=0 selects lstm_bwd_tc_kernel, same bits)
   static const int bw_staged = []() { const char* e = getenv("TSC_BPTT_STAGED"); return e ? atoi(e) : 1; }();
   if (bw_staged && bw_threads == 512 && a.Gb && a.Cb && a.dZb && !a.ZG && !a.dXb) {
-    const size_t smem_s = BW_KC * 1024 + BW_KC * 2048 + 128 * 512 + 2 * 128 * 128 + 128 * 256 + 32;
-    static int attr_s = -1;
-    if (attr_s != tscl_device_of(h)) {
-      PCK(cudaFuncSetAttribute(lstm_bwd_tc_staged_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_s));
-      PCK(cudaFuncSetAttribute(lstm_bwd_tc_staged_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_s));
-      PCK(cudaFuncSetAttribute(lstm_bwd_tc_staged_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_s));
-      PCK(cudaFuncSetAttribute(lstm_bwd_tc_staged_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_s));
-      attr_s = tscl_device_of(h);
+    // tensor maps [2A * T][Rc][cols] over this chunk's gates / c / dH / dZ; if they cannot be encoded,
+    // lstm_bwd_tc_kernel<512> below gives the same bits
+    CUtensorMap mG, mC, mD, mZ;
+    const uint64_t planes = (uint64_t)2 * d.A * T;
+    if (make_tmap_3d(&mG, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, gates_bf16, planes, Rc, TC_N, 64, 64) &&
+        make_tmap_3d(&mC, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, c_bf16, planes, Rc, TC_H, 64, 64) &&
+        make_tmap_3d(&mD, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, dH, planes, Rc, TC_H, 32, 64) &&
+        make_tmap_3d(&mZ, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, dz_bf16, planes, Rc, TC_N, 64, 64)) {
+      static int attr_r = -1;
+      if (attr_r != tscl_device_of(h)) {
+        PCK(cudaFuncSetAttribute(lstm_bwd_tc_regs_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, BR_SMEM));
+        PCK(cudaFuncSetAttribute(lstm_bwd_tc_regs_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, BR_SMEM));
+        attr_r = tscl_device_of(h);
+      }
+      const int grid_r = (int)(n_items < n_sm ? n_items : n_sm);
+      a.prof = g_bptt_prof;
+      if (a.prof) lstm_bwd_tc_regs_kernel<true><<<grid_r, 256, BR_SMEM, (cudaStream_t)stream>>>(d, a, mG, mC, mD, mZ);
+      else lstm_bwd_tc_regs_kernel<false><<<grid_r, 256, BR_SMEM, (cudaStream_t)stream>>>(d, a, mG, mC, mD, mZ);
+      PCK(cudaGetLastError());
+      return 0;
     }
-    const int grid_s = (int)(n_items < n_sm ? n_items : n_sm);
-    a.prof = g_bptt_prof;
-    // operand tiles by TMA (tensor maps over this chunk's gate / c / dH arrays, 128-byte swizzle); TSC_BPTT_TMA=0: cp.async
-    static const int bw_tma = []() { const char* e = getenv("TSC_BPTT_TMA"); return e ? atoi(e) : 1; }();
-    CUtensorMap mG, mC, mD;
-    memset(&mG, 0, sizeof(mG)); memset(&mC, 0, sizeof(mC)); memset(&mD, 0, sizeof(mD));
-    const uint64_t rows = (uint64_t)2 * d.A * T * Rc;
-    const bool tma = bw_tma && rows < (1ull << 31) &&
-                     make_tmap_2d(&mG, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, gates_bf16, rows, TC_N, 64, 128) &&
-                     make_tmap_2d(&mC, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, c_bf16, rows, TC_H, 64, 128) &&
-                     make_tmap_2d(&mD, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, dH, rows, TC_H, 32, 128);
-    if (tma) {
-      if (a.prof) lstm_bwd_tc_staged_kernel<true, true><<<grid_s, 512, smem_s, (cudaStream_t)stream>>>(d, a, mG, mC, mD);
-      else lstm_bwd_tc_staged_kernel<false, true><<<grid_s, 512, smem_s, (cudaStream_t)stream>>>(d, a, mG, mC, mD);
-    } else {
-      if (a.prof) lstm_bwd_tc_staged_kernel<true, false><<<grid_s, 512, smem_s, (cudaStream_t)stream>>>(d, a, mG, mC, mD);
-      else lstm_bwd_tc_staged_kernel<false, false><<<grid_s, 512, smem_s, (cudaStream_t)stream>>>(d, a, mG, mC, mD);
-    }
-  } else if (bw_threads == 512) lstm_bwd_tc_kernel<512><<<grid, 512, smem, (cudaStream_t)stream>>>(d, a);
+  }
+  if (bw_threads == 512) lstm_bwd_tc_kernel<512><<<grid, 512, smem, (cudaStream_t)stream>>>(d, a);
   else lstm_bwd_tc_kernel<256><<<grid, 256, smem, (cudaStream_t)stream>>>(d, a);
   PCK(cudaGetLastError());
   return 0;

@@ -132,10 +132,11 @@ int tscl_wgrad_tc(tscl_handle* h, const float* dZ, const void* dz_bf16, const fl
 
 /* BPTT on the tensor cores (wgmma): same contract as tscl_lstm_seq_bwd, with the recurrent product dz.Wh^T as
  * a bf16 MMA (M=128, N=64, K=256) per step; wt_bf16 [2A][32][64][8] comes from tscl_pack_wht (refresh after
- * every optimizer step).  With gates_bf16 / c_bf16 / dz_bf16 and ZG == NULL (the shipping call) the per-step operand tile
- * of 128 replicas (gates, c, dH: 112 KB) is fetched one step ahead by cp.async.bulk.tensor copies through tensor maps
- * built over the caller's arrays (cuTensorMapEncodeTiled via the driver entry point; TSC_BPTT_TMA=0 selects the
- * cp.async variant); the arrays must be 16-byte aligned and hold 2A * T * Rc rows. */
+ * every optimizer step).  With gates_bf16 / c_bf16 / dz_bf16 and ZG == NULL (the shipping call) each warpgroup runs the
+ * recurrence of 64 replica rows in registers: its per-step operands (gates, c, dH: 56 KB) are fetched one step ahead by
+ * cp.async.bulk.tensor copies, and dZ leaves by a bulk tensor store, through 3-D tensor maps [2A * T][Rc][cols] built over
+ * the caller's arrays (cuTensorMapEncodeTiled via the driver entry point; if they cannot be built the call runs the
+ * row-per-thread kernel, which gives the same bits); the arrays must be 16-byte aligned and hold 2A * T * Rc rows. */
 int tscl_pack_wht(tscl_handle* h, const float* params, void* wt_bf16, void* stream);
 int tscl_lstm_seq_bwd_tc(tscl_handle* h, const void* wt_bf16, float* ZG, const float* C, const float* dH, const float* c0,
                          const float* done, int32_t T, int64_t Rc, int64_t ld_state, int64_t r0,
@@ -183,8 +184,8 @@ int tscl_unpack_store(tscl_handle* h, const void* st_x, const void* st_g, const 
 /* Tools only (scripts/profile_policy_phases.py): per-phase clock64 sums of tscl_policy_step_v2 are added to 8 uint64
  * device counters while the pointer is set (NULL = off; a separate instantiation of the kernel, the hot one is unchanged). */
 int tscl_debug_policy_prof(void* counters_dev);
-/* same for the staged BPTT kernel: 8 counters (operand wait | smem->regs + cell backward + dZ stores | barrier | MMA + wait |
- * accumulator read-back), summed over CTAs; NULL switches profiling off */
+/* same for the store-path BPTT kernel: the first 4 of 8 counters (operand wait | smem->regs + cell backward | MMA issue ->
+ * wait | dZ store), summed over the warpgroups; NULL switches profiling off */
 int tscl_debug_bptt_prof(void* counters_dev);
 
 /* Per-agent clip_by_global_norm(max_norm) + RMSProp step (TF1 semantics).  agent_of [n_params] u8.

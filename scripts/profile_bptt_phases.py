@@ -1,4 +1,5 @@
-"""Per-phase clock64 breakdown of the staged BPTT kernel (thread 0 of every CTA) during one update: python scripts/profile_bptt_phases.py [R] [chunk]"""
+"""Per-phase clock64 breakdown of the store-path BPTT kernel (lstm_bwd_tc_regs_kernel: thread 0 of every warpgroup) during
+one update: python scripts/profile_bptt_phases.py [R] [chunk]"""
 import ctypes as C
 import sys
 
@@ -30,12 +31,13 @@ torch.cuda.synchronize()
 _lib.lib().tscl_debug_bptt_prof(None)
 n_sm = torch.cuda.get_device_properties(0).multi_processor_count
 n_items = 2 * lay.A * ((chunk + 127) // 128) * ((R + chunk - 1) // chunk)
-n_cta = min(n_items, n_sm)                      # persistent grid of the staged kernel
-p = prof.cpu().numpy().astype(float) / n_cta
+n_cta = min(n_items, n_sm)                      # persistent grid, two warpgroups per CTA
+wg_steps = 2 * lay.A * ((R + chunk - 1) // chunk) * ((chunk + 63) // 64) * 120   # (64-row slab, step) pairs
+p = prof.cpu().numpy()[:4].astype(float) / (2 * n_cta)
 tot = p.sum()
-steps = n_items * 120 / n_cta
-print("BPTT: %.0f cycles per CTA per update, %.0f (tile, step) pairs per CTA = %.0f cycles each" % (tot, steps, tot / steps))
-for nm, v in zip(["wait for step t's operands", "smem -> regs, prefetch issue, cell backward, dZ stores",
-                  "fence + barrier before the MMA", "MMA + fragment store + barrier", "accumulator read-back",
-                  "  (of phase 2) smem -> regs + first sub-batch", "  (of phase 2) barrier", "  (of phase 2) operand issue (TMA / cp.async)"], p):
-    print("   %-56s %9.0f cycles  %5.1f %%   %.0f per step" % (nm, v, 100 * v / tot, v / steps))
+steps = wg_steps / (2 * n_cta)
+print("BPTT: %.0f cycles per warpgroup per update, %.0f (64-row slab, step) pairs per warpgroup = %.0f cycles each"
+      % (tot, steps, tot / steps))
+for nm, v in zip(["wait for step t's operands", "smem -> regs, operand issue, cell backward",
+                  "MMA issue -> wait", "dZ store (stmatrix, barrier, TMA store issue)"], p):
+    print("   %-48s %9.0f cycles  %5.1f %%   %.0f per step" % (nm, v, 100 * v / tot, v / steps))
