@@ -115,6 +115,9 @@ class BatchedA2C:
         self.dx_fusable = self.use_tc and L.dx % 32 == 0 and L.dx <= 256
         # stand-alone dX = dZ . Wx^T kernel (tscl_dx_tc); False falls back to the library GEMM (A/B measurements only)
         self.dx_own = self.use_tc and L.dx % 16 == 0 and L.dx <= 224 and os.environ.get("TSC_DX_LIBRARY", "0") != "1"
+        # dX fused into the fc weight-gradient kernel (tscl_dx_fc_bwd_tc: dX never reaches memory) at the fc widths of
+        # the v2 forward; False runs tscl_dx_tc + tscl_fc_bwd_tc (tests/test_dx_fc_bwd_fused_gpu.py compares the two)
+        self.dx_fc_fused = self.dx_own and self.tc_v2
         self.bwd_tc = self.use_tc
         self.fc_bwd_tc = self.use_tc and layout.fc_bwd_tc_ok     # front-end weight gradients on the tensor cores
         self.wgrad_tc = self.use_tc and L.dx % 8 == 0 and L.dx <= 240   # LSTM weight gradients on the tensor cores
@@ -302,10 +305,11 @@ class BatchedA2C:
         self.done_post[t] = 1.0 if done_post else 0.0
         self.t += 1
 
-    def _bufs(self, rc, lean=False):
+    def _bufs(self, rc, lean=False, dxb=True):
         """Work buffers of one update chunk.  `lean`: every consumer reads the bf16 activation store itself and dZ / dX
-        travel as bf16 between the tensor-core kernels, so only dH (fp32), dZb and dXb (bf16) exist; the fp32 set is
-        allocated the first time a fallback path needs it."""
+        travel as bf16 between the tensor-core kernels, so only dH (fp32), dZb and dXb (bf16) exist (dXb only with
+        `dxb`: the fused dX / fc kernel never writes dX); the fp32 set is allocated the first time a fallback path
+        needs it."""
         L, T, U = self.lay, self.T, self.lay.U
         f32 = dict(dtype=torch.float32, device=self.dev)
         if self._upd_bufs is None or self._upd_bufs["rc"] < rc:
@@ -314,8 +318,9 @@ class BatchedA2C:
         b = self._upd_bufs
         M = T * b["rc"]
         if lean and "dZb" not in b:
-            b.update(dZb=torch.empty(U, M, 4 * L.h, dtype=torch.bfloat16, device=self.dev),
-                     dXb=torch.empty(U, M, L.dx, dtype=torch.bfloat16, device=self.dev))
+            b["dZb"] = torch.empty(U, M, 4 * L.h, dtype=torch.bfloat16, device=self.dev)
+        if lean and dxb and "dXb" not in b:
+            b["dXb"] = torch.empty(U, M, L.dx, dtype=torch.bfloat16, device=self.dev)
         if not lean and "X" not in b:
             b.update(ZG=torch.empty(U, M, 4 * L.h, **f32), dX=torch.empty(U, M, L.dx, **f32),
                      X=torch.empty(U, M, L.dx, **f32), C=torch.empty(U, M, L.h, **f32), H=torch.empty(U, M, L.h, **f32),
@@ -348,19 +353,22 @@ class BatchedA2C:
             M = T * rc
             ci = r0 // self.chunk
             all_tc = use_store and self.bwd_tc and self.fc_bwd_tc and self.wgrad_tc and self.fused_heads
-            b = self._bufs(rc, lean=all_tc)
+            fuse_dx = all_tc and self.dx_fused and self.dx_fusable   # dX = dZ . Wx^T inside the BPTT kernel (second MMA per step)
+            fuse_fc = all_tc and not fuse_dx and self.dx_fc_fused    # dX inside the fc weight-gradient kernel, never stored
+            b = self._bufs(rc, lean=all_tc, dxb=not fuse_fc)
             X = Cc = H = Hp = dlog = ZG = dX = dZb = dXb = None
             bf16 = dict(dtype=torch.bfloat16, device=self.dev)
             if b["rc"] == rc:
                 dH = b["dH"]
                 if all_tc:
-                    dZb, dXb = b["dZb"], b["dXb"]
+                    dZb, dXb = b["dZb"], b.get("dXb")
                 else:
                     ZG, dX, X, Cc, H, Hp, dlog = (b[k] for k in ("ZG", "dX", "X", "C", "H", "Hp", "dlog"))
             else:               # tail chunk: dense temporaries of the right shape
                 dH = torch.empty(U, M, L.h, **f32)
                 if all_tc:
-                    dZb, dXb = torch.empty(U, M, 4 * L.h, **bf16), torch.empty(U, M, L.dx, **bf16)
+                    dZb = torch.empty(U, M, 4 * L.h, **bf16)
+                    dXb = None if fuse_fc else torch.empty(U, M, L.dx, **bf16)
                 else:
                     ZG, dX, X, Cc, H, Hp, dlog = (torch.empty(U, M, s_, **f32) for s_ in
                                                   (4 * L.h, L.dx, L.dx, L.h, L.h, L.h, L.max_na))
@@ -392,7 +400,6 @@ class BatchedA2C:
                 # head weight / bias gradients (plain batched GEMM + column sums)
                 self.gv["wo"].baddbmm_(H.transpose(1, 2), dlog)
                 self.gv["bo"].add_(dlog.sum(dim=1))
-            fuse_dx = all_tc and self.dx_fused and self.dx_fusable   # dX = dZ . Wx^T inside the BPTT kernel (second MMA per step)
             if self.bwd_tc:
                 gb = (_p(self.st_g[ci]), _p(self.st_c[ci])) if use_store else (None, None)
                 _lib.check(lib.tscl_lstm_seq_bwd_tc_dx(self._h, _p(self.Wt), _p(ZG), _p(Cc), _p(dH), _p(self.c_bw),
@@ -415,15 +422,21 @@ class BatchedA2C:
                 self.gv["wx"].baddbmm_(X.transpose(1, 2), dZ)
                 self.gv["wh"].baddbmm_(Hp.transpose(1, 2), dZ)
                 self.gv["bl"].add_(dZ.sum(dim=1))
-            # dX = dZ . Wx^T: own warp-specialised wgmma kernel on the shipping path (tscl_dx_tc); a library GEMM only on
-            # the fp32 twin path, for dx > 224 and under TSC_DX_LIBRARY=1 (A/B measurements)
-            if all_tc and not fuse_dx and self.dx_own:
+            # dX = dZ . Wx^T: fused into the fc weight gradients on the shipping path (tscl_dx_fc_bwd_tc); else its own
+            # warp-specialised wgmma kernel (tscl_dx_tc); a library GEMM only on the fp32 twin path, for dx > 224 and
+            # under TSC_DX_LIBRARY=1 (A/B measurements)
+            if fuse_fc:
+                _lib.check(lib.tscl_dx_fc_bwd_tc(self._h, _p(obs0), _p(self.st_x[ci]), _p(dZb), _p(self.Wxt), C.c_int64(M),
+                                                 C.c_int64(rc), C.c_int64(R * n_obs), _p(self.G), st()))
+            elif all_tc and not fuse_dx and self.dx_own:
                 _lib.check(lib.tscl_dx_tc(self._h, _p(dZb), _p(self.Wxt), _p(dXb), C.c_int64(M), st()))
             elif all_tc and not fuse_dx:
                 torch.bmm(dZb, self.wx_b.transpose(1, 2), out=dXb)
             elif not all_tc:
                 torch.bmm(dZ, self.pv["wx"].transpose(1, 2), out=dX)
-            if self.fc_bwd_tc:
+            if fuse_fc:
+                pass            # the fc weight gradients came out of tscl_dx_fc_bwd_tc above
+            elif self.fc_bwd_tc:
                 xb = _p(self.st_x[ci]) if use_store else None
                 _lib.check(lib.tscl_fc_bwd_tc(self._h, _p(obs0), None if all_tc else _p(X), xb, _p(dX), _p(dXb),
                                               C.c_int64(M), C.c_int64(rc), C.c_int64(R * n_obs), _p(self.G), C.c_int32(0),
@@ -431,7 +444,7 @@ class BatchedA2C:
             else:
                 _lib.check(lib.tscl_fc_bwd(self._h, _p(obs0), _p(X), _p(dX), C.c_int64(M), C.c_int64(rc),
                                            C.c_int64(R * n_obs), _p(self.G), st()))
-            self.kernel_launches += 4 if use_store else 5
+            self.kernel_launches += 3 if fuse_fc else 4 if use_store else 5
         if self.pg is not None:
             _dist.allreduce_sum_(self.G, self.pg)
         _lib.check(lib.tscl_clip_rmsprop(self._h, _p(self.P), _p(self.G), _p(self.MS), _p(self.agent_of),

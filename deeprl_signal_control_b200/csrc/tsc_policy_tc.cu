@@ -1580,9 +1580,10 @@ lstm_bwd_tc_regs_kernel(const DDimsTC d, const BwdTC a, const __grid_constant__ 
 }
 
 // 3-D tiled tensor map over row-major [planes][rows][cols] (box = box_cols x box_rows x 1, inner box = 128 bytes,
-// 128-byte swizzle) through the driver entry point (no link-time dependency on libcuda)
+// 128-byte swizzle unless `sw` says otherwise) through the driver entry point (no link-time dependency on libcuda)
 static bool make_tmap_3d(CUtensorMap* m, CUtensorMapDataType dt, int elem_bytes, const void* base, uint64_t planes,
-                         uint64_t rows, uint64_t cols, uint32_t box_cols, uint32_t box_rows) {
+                         uint64_t rows, uint64_t cols, uint32_t box_cols, uint32_t box_rows,
+                         CUtensorMapSwizzle sw = CU_TENSOR_MAP_SWIZZLE_128B) {
   typedef CUresult (*encode_fn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                 const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                 CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -1599,7 +1600,7 @@ static bool make_tmap_3d(CUtensorMap* m, CUtensorMapDataType dt, int elem_bytes,
   const cuuint64_t strides[2] = {cols * (uint64_t)elem_bytes, rows * cols * (uint64_t)elem_bytes};
   const cuuint32_t box[3] = {box_cols, box_rows, 1};
   const cuuint32_t es[3] = {1, 1, 1};
-  return fn(m, dt, 3, const_cast<void*>(base), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+  return fn(m, dt, 3, const_cast<void*>(base), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE, sw,
             CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
@@ -2589,6 +2590,353 @@ extern "C" int tscl_dx_tc(tscl_handle* h, const void* dz_bf16, const void* wxt_b
   DxTC a;
   a.dZb = (const __nv_bfloat16*)dz_bf16; a.Wxt = (const __nv_bfloat16*)wxt_bf16; a.dXb = (__nv_bfloat16*)dx_bf16; a.M = M;
   kern<<<grid, DXK_THREADS, smem, (cudaStream_t)stream>>>(d, a);
+  PCK(cudaGetLastError());
+  return 0;
+}
+
+// ===================================================================================================
+// dX fused into the fc front-end weight gradients: per (unit, 128-row tile) the kernel forms dX = dZ . Wx^T exactly as
+// dx_tc_kernel does (same operands, same 4 atoms x 4 k16 order, so the bf16-rounded dX has the same bits), masks it by
+// X > 0 (fc_bwd_tc_kernel's bf16 test) in registers, and multiplies it straight into the fc weight gradients:
+//   D[64 input slots][dx] += In^T . dXm      (wgmma, A = In and B = dXm both MN-major in shared memory, K = 128 rows)
+// dX never leaves the SM: per row the kernel reads dZ (512 B), X (2 dx B) and the observation slice, and writes nothing.
+//   warp 8, lane 0    : TMA issue: dZ one swizzle atom (128 rows x 64 K, 16 KB) per stage, 2 stages; the tile's X as
+//                       dx / 8 boxes of [128 rows][8 columns] straight into the MN-major dXm buffer
+//   warps 9-11        : the observation tile In, gathered into the 64 input slots (plus the ones slot of the bias)
+//   warps 0-7         : two warpgroups (64 rows each) run the dX MMAs into register fragments (dx / 2 per thread), then
+//                       overwrite each X word in shared memory with the masked bf16 dX of the same (row, column pair), meet
+//                       at a 256-thread barrier and multiply: warpgroup g owns dX columns [g dx / 2, (g + 1) dx / 2) of D,
+//                       dx / 4 fp32 per thread, kept over all tiles of a unit and flushed to G with atomics when the unit
+//                       changes (the column -> fcw / fcf / fct and slot -> input mapping of fc_bwd_tc_kernel)
+// Shared memory at dx = 224: 32 KB dZ stages + 112 KB Wx^T image + 56 KB dXm + 16.1 KB In = 216 KB.  setmaxnreg gives the
+// consumers 216 registers at dx = 224 (dX 112 + fc 56 fragments), the producer warps 72.
+#define DXF_THREADS 384
+#define DXF_STAGES 2
+#define DXF_SBO 2048                       // dXm chunk stride: 128 rows x 16 B (a TMA destination: 128-byte aligned)
+#define DXF_BUILDERS 96                    // warps 9-11
+// (dx = 224 needs 8 more consumer registers than the narrower widths, which leave the producer warps 80)
+#define DXF_CONS_REGS(dx) ((dx) > 192 ? 216 : 208)
+#define DXF_PROD_REGS(dx) ((dx) > 192 ? 72 : 80)
+static_assert(128 * DXF_PROD_REGS(224) + 256 * DXF_CONS_REGS(224) <= DXF_THREADS * 168 &&
+              128 * DXF_PROD_REGS(160) + 256 * DXF_CONS_REGS(160) <= DXF_THREADS * 168,
+              "setmaxnreg split exceeds the CTA's registers");
+static size_t dxf_smem(int dx) {
+  return (size_t)DXF_STAGES * DXK_STAGE_BYTES + (size_t)BW_KC * dx * 16 + (size_t)(dx / 8) * DXF_SBO + 8 * FBT_SBO + 8 * 8;
+}
+struct DxFcTC {
+  const float* obs;            // rows as tscl_fc_embed
+  const __nv_bfloat16* Wxt;    // [2A][32][dx][8]  (tscl_pack_wxt)
+  float* G;
+  int64_t M, rows_per_t, stride_t;
+};
+// 0xFFFF per 16-bit half of x where that bf16 value is > 0
+__device__ __forceinline__ uint32_t bf16x2_pos_mask(uint32_t x) {
+  const uint32_t nz = ((x & 0x7FFF7FFFu) + 0x7FFF7FFFu) & ~x & 0x80008000u;
+  return (nz >> 15) * 0xFFFFu;
+}
+// an fc fragment of unit u into G: input slot 16 (warp & 3) + lane / 4 (+ 8 for entries 4 i + 2, 4 i + 3),
+// dX column cb + 8 i + 2 (lane & 3) (+ 1 for the odd entries)
+template <int NR>
+__device__ __forceinline__ void dxf_flush(const DDimsTC& d, float* G, int u, const float (&f)[NR], int cb) {
+  const int lane = threadIdx.x & 31, w4 = (threadIdx.x >> 5) & 3, ag = u >> 1;
+  const int nw = d.n_wave[ag], nt = d.n_wait[ag], nf = d.ff > 0 ? d.n_fp[ag] : 0;
+#pragma unroll
+  for (int e = 0; e < NR; ++e) {
+    const int slot = 16 * w4 + (lane >> 2) + 8 * ((e >> 1) & 1);
+    const int c = cb + 8 * (e >> 2) + 2 * (lane & 3) + (e & 1);
+    int64_t wo, bo; int ld, cc, s0, n;
+    if (c < d.fw) { wo = d.off_fcw_w[u]; bo = d.off_fcw_b[u]; ld = d.fw; cc = c; s0 = 0; n = nw; }
+    else if (c < d.fw + d.ff) { wo = d.off_fcf_w[u]; bo = d.off_fcf_b[u]; ld = d.ff; cc = c - d.fw; s0 = d.kw; n = nf; }
+    else { wo = d.off_fct_w[u]; bo = d.off_fct_b[u]; ld = d.ft; cc = c - d.fw - d.ff; s0 = d.kw + TC_KF; n = nt; }
+    const int kin = slot - s0;
+    if (kin >= 0 && kin < n) atomicAdd(&G[wo + (int64_t)kin * ld + cc], f[e]);
+    if (slot == d.ones_slot) atomicAdd(&G[bo + cc], f[e]);
+  }
+}
+
+template <int DX>
+__global__ void __launch_bounds__(DXF_THREADS, 1)
+dx_fc_bwd_tc_kernel(const DDimsTC d, const DxFcTC a, const __grid_constant__ CUtensorMap mapZ,
+                    const __grid_constant__ CUtensorMap mapX) {
+  constexpr int N64 = DX / 64, R32 = (DX % 64) >= 32, R16 = (DX % 32) >= 16;      // dX fragments: the tile's dx columns
+  constexpr int HN = DX / 2, H32 = (HN % 64) >= 32, H16 = (HN % 32) >= 16;        // fc fragments: this warpgroup's half
+  static_assert(HN >= 64 && HN < 128 && HN % 16 == 0, "fc half width must be 64 + {0, 16, 32, 48}");
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  unsigned char* sStage = tc_smem;
+  unsigned char* sW = sStage + DXF_STAGES * DXK_STAGE_BYTES;
+  unsigned char* sA = sW + (size_t)BW_KC * DX * 16;              // X, then masked dX: [dx / 8][128 rows][8] bf16
+  unsigned char* sB = sA + (size_t)(DX / 8) * DXF_SBO;           // In: [8][128 rows][8] bf16, chunk stride FBT_SBO
+  uint64_t* sBar = reinterpret_cast<uint64_t*>(sB + 8 * FBT_SBO);
+  const uint32_t bar_full = smem_u32(sBar), bar_empty = bar_full + 16, bar_w = bar_full + 32, bar_x = bar_full + 40,
+                 bar_in = bar_full + 48, bar_free = bar_full + 56;
+  if (tid == 0) {
+    for (int s = 0; s < DXF_STAGES; ++s) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, 8); }
+    mbar_init(bar_w, 1); mbar_init(bar_x, 1); mbar_init(bar_in, DXF_BUILDERS); mbar_init(bar_free, 8);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+  // the CTA's contiguous range [j0, j1) of the (unit, tile) list, formed in each role after its setmaxnreg
+#define DXF_RANGE                                                                                   \
+  const int64_t tpu = (a.M + 127) / 128;                                                            \
+  const int64_t NT = tpu * 2 * d.A;                                                                 \
+  const int64_t j0 = NT * blockIdx.x / gridDim.x, j1 = NT * (blockIdx.x + 1) / gridDim.x;
+
+  if (warp >= 8) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(DXF_PROD_REGS(DX)));
+    DXF_RANGE
+    if (warp == 8) {
+      // ---------------- TMA issue ----------------
+      if (lane == 0) {
+        const uint32_t aS = smem_u32(sStage), aA = smem_u32(sA);
+        int64_t it = 0;
+        for (int64_t j = j0; j < j1; ++j) {
+          const int u = (int)(j / tpu), m0 = (int)((j - (int64_t)u * tpu) * 128);
+          auto atom = [&](int at) {
+            const int s = (int)(it % DXF_STAGES);
+            const int64_t n = it / DXF_STAGES;
+            if (n > 0) mbar_wait(bar_empty + 8 * s, (uint32_t)((n - 1) & 1));
+            mbar_expect_tx(bar_full + 8 * s, DXK_STAGE_BYTES);
+            tma_load_3d(aS + s * DXK_STAGE_BYTES, &mapZ, at * 64, m0, u, bar_full + 8 * s);
+            ++it;
+          };
+          atom(0); atom(1);
+          // X of this tile once both warpgroups have multiplied the previous tile's dXm
+          if (j > j0) mbar_wait(bar_free, (uint32_t)((j - j0 - 1) & 1));
+          mbar_expect_tx(bar_x, (DX / 8) * DXF_SBO);
+#pragma unroll 1
+          for (int cg = 0; cg < DX / 8; ++cg) tma_load_3d(aA + cg * DXF_SBO, &mapX, cg * 8, m0, u, bar_x);
+          atom(2); atom(3);
+        }
+      }
+    } else {
+      // ---------------- observation tile: item i = (row i / 8, input-slot chunk i % 8) ----------------
+      const int bt = tid - 288, bc = bt & 7;      // DXF_BUILDERS is a multiple of 8: every item of a thread has chunk bc
+      int cur_u = -1, ooff = 0;
+      int src[8];                                 // observation index of each of the chunk's 8 slots (-1 none, -2 one)
+      for (int64_t j = j0; j < j1; ++j) {
+        const int u = (int)(j / tpu);
+        const int64_t m0 = (j - (int64_t)u * tpu) * 128;
+        if (u != cur_u) {
+          cur_u = u;
+          const int ag = u >> 1;
+          const int nw = d.n_wave[ag], nt = d.n_wait[ag], nf = d.ff > 0 ? d.n_fp[ag] : 0;
+          ooff = d.obs_off[ag];
+#pragma unroll
+          for (int e = 0; e < 8; ++e) {
+            const int slot = bc * 8 + e;
+            int sidx = -1;
+            if (slot < d.kw) { if (slot < nw) sidx = slot; }
+            else if (slot < d.kw + TC_KF) { if (slot - d.kw < nf) sidx = nw + nt + (slot - d.kw); }
+            else { if (slot - d.kw - TC_KF < nt) sidx = nw + (slot - d.kw - TC_KF); }
+            if (slot == d.ones_slot) sidx = -2;
+            src[e] = sidx;
+          }
+        }
+        const int rows_valid = (a.M - m0) < 128 ? (int)(a.M - m0) : 128;
+        const int64_t tq = m0 / a.rows_per_t, rem0 = m0 - tq * a.rows_per_t;
+        if (j > j0) mbar_wait(bar_free, (uint32_t)((j - j0 - 1) & 1));
+#pragma unroll 1
+        for (int i = bt; i < 128 * 8; i += 2 * DXF_BUILDERS) {      // two items (rows i / 8, i / 8 + 12) per pass
+          float v[2][8];
+#pragma unroll
+          for (int p = 0; p < 2; ++p) {
+            const int row = (i + p * DXF_BUILDERS) >> 3;
+#pragma unroll
+            for (int e = 0; e < 8; ++e) v[p][e] = 0.f;
+            if (i + p * DXF_BUILDERS < 128 * 8 && row < rows_valid) {
+              int64_t tt = tq, rem = rem0 + row;
+              while (rem >= a.rows_per_t) { rem -= a.rows_per_t; ++tt; }
+              const float* op = a.obs + tt * a.stride_t + rem * d.n_obs + ooff;
+#pragma unroll
+              for (int e = 0; e < 8; ++e) v[p][e] = src[e] >= 0 ? __ldg(op + src[e]) : (src[e] == -2 ? 1.0f : 0.f);
+            }
+          }
+#pragma unroll
+          for (int p = 0; p < 2; ++p) {
+            const int ii = i + p * DXF_BUILDERS;
+            if (ii < 128 * 8) {
+              __align__(16) __nv_bfloat16 o[8];
+#pragma unroll
+              for (int e = 0; e < 8; ++e) o[e] = __float2bfloat16_rn(v[p][e]);
+              *reinterpret_cast<uint4*>(sB + (size_t)bc * FBT_SBO + (ii >> 3) * 16) = *reinterpret_cast<const uint4*>(o);
+            }
+          }
+        }
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");      // generic writes -> operand of the wgmmas
+        mbar_arrive(bar_in);
+        if (j + 1 < j1) {      // pull the next tile's observation rows towards L2 while this tile is multiplied
+          const int un = (int)((j + 1) / tpu);
+          const int ooff_n = d.obs_off[un >> 1];
+          for (int r = bt; r < 128; r += DXF_BUILDERS) {
+            const int64_t m = (j + 1 - (int64_t)un * tpu) * 128 + r;
+            if (m >= a.M) break;
+            const float* op = a.obs + (m / a.rows_per_t) * a.stride_t + (m % a.rows_per_t) * d.n_obs + ooff_n;
+            asm volatile("prefetch.global.L2 [%0];" ::"l"(op));
+            asm volatile("prefetch.global.L2 [%0];" ::"l"(op + 32));
+          }
+        }
+      }
+    }
+  } else {
+    // ---------------- dX MMA, mask, fc MMA: warps 0-7, one warpgroup per 64-row half ----------------
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(DXF_CONS_REGS(DX)));
+    DXF_RANGE
+    const int wg = warp >> 2;
+    const uint32_t aS = smem_u32(sStage), aW = smem_u32(sW), aA = smem_u32(sA), aB = smem_u32(sB);
+    const uint32_t b_lbo = (uint32_t)DX * 16;
+    float f64[N64][32], f32[R32 ? 16 : 1], f16[R16 ? 8 : 1];
+    float g64[32], g32[H32 ? 16 : 1], g16[H16 ? 8 : 1];
+    const int n0 = wg * HN;                       // this warpgroup's first dX column of D
+    int64_t it = 0;
+    int cur_u = -1, prev_s = 0;
+    uint32_t wph = 0;
+    bool first = true;
+    const int fr = wg * 64 + (warp & 3) * 16 + (lane >> 2), c0 = 2 * (lane & 3);
+    // the X word of (row r, columns col, col + 1) becomes the masked bf16 dX of the same pair
+    auto mask_put = [&](int col, float x, float y, int r) {
+      uint32_t* p = reinterpret_cast<uint32_t*>(sA + (size_t)(col >> 3) * DXF_SBO + r * 16 + (col & 7) * 2);
+      const __nv_bfloat162 v = __floats2bfloat162_rn(x, y);
+      *p = *reinterpret_cast<const uint32_t*>(&v) & bf16x2_pos_mask(*p);
+    };
+    auto flush = [&](int u) {
+      dxf_flush(d, a.G, u, g64, n0);
+      if constexpr (H32) dxf_flush(d, a.G, u, g32, n0 + 64);
+      if constexpr (H16) dxf_flush(d, a.G, u, g16, n0 + 64 + 32 * H32);
+    };
+    for (int64_t j = j0; j < j1; ++j) {
+      const int u = (int)(j / tpu);
+      const uint32_t ph = (uint32_t)((j - j0) & 1);
+      if (u != cur_u) {
+        if (cur_u >= 0) flush(cur_u);
+        cur_u = u; first = true;
+        asm volatile("bar.sync 1, 256;" ::: "memory");      // both warpgroups' MMAs of the previous unit have completed
+        if (tid == 0) {
+          const uint32_t bytes = (uint32_t)BW_KC * DX * 16;
+          mbar_expect_tx(bar_w, bytes);
+          bulk_g2s(aW, a.Wxt + (int64_t)u * BW_KC * DX * 8, bytes, bar_w);
+        }
+        mbar_wait(bar_w, wph); wph ^= 1;
+      }
+      // ---- dX = dZ . Wx^T: dx_tc_kernel's MMA sequence ----
+      for (int at = 0; at < 4; ++at, ++it) {
+        const int s = (int)(it % DXF_STAGES);
+        mbar_wait(bar_full + 8 * s, (uint32_t)((it / DXF_STAGES) & 1));
+        const uint32_t a0 = aS + s * DXK_STAGE_BYTES + wg * 8192;
+        const uint32_t b0 = aW + (uint32_t)(at * 8) * b_lbo;
+        wg_fence();
+#pragma unroll
+        for (int q = 0; q < N64; ++q)
+          wg_mma_regs<64, 0, 0>(f64[q], 4, at > 0, [&](int k, uint64_t& da, uint64_t& db) {
+            da = make_desc_sw128(a0 + k * 32);
+            db = make_desc(b0 + (uint32_t)(k * 2) * b_lbo + q * 64 * 16, b_lbo, 128);
+          });
+        if constexpr (R32)
+          wg_mma_regs<32, 0, 0>(f32, 4, at > 0, [&](int k, uint64_t& da, uint64_t& db) {
+            da = make_desc_sw128(a0 + k * 32);
+            db = make_desc(b0 + (uint32_t)(k * 2) * b_lbo + N64 * 64 * 16, b_lbo, 128);
+          });
+        if constexpr (R16)
+          wg_mma_regs<16, 0, 0>(f16, 4, at > 0, [&](int k, uint64_t& da, uint64_t& db) {
+            da = make_desc_sw128(a0 + k * 32);
+            db = make_desc(b0 + (uint32_t)(k * 2) * b_lbo + (N64 * 64 + R32 * 32) * 16, b_lbo, 128);
+          });
+        wg_commit();
+        if (at > 0) {        // the MMAs of the previous atom have completed: release its stage
+          wg_wait<1>();
+          if (lane == 0) mbar_arrive(bar_empty + 8 * prev_s);
+        }
+        prev_s = s;
+      }
+      wg_wait<0>();
+      if (lane == 0) mbar_arrive(bar_empty + 8 * prev_s);
+#pragma unroll
+      for (int q = 0; q < N64; ++q) wg_frag_fence(f64[q]);
+      if constexpr (R32) wg_frag_fence(f32);
+      if constexpr (R16) wg_frag_fence(f16);
+      // ---- mask in place: X -> dX (bf16) where X > 0, else 0 (rows past M: X is zero-filled by the TMA) ----
+      mbar_wait(bar_x, ph);
+#pragma unroll
+      for (int q = 0; q < N64; ++q)
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          mask_put(q * 64 + 8 * i + c0, f64[q][4 * i], f64[q][4 * i + 1], fr);
+          mask_put(q * 64 + 8 * i + c0, f64[q][4 * i + 2], f64[q][4 * i + 3], fr + 8);
+        }
+      if constexpr (R32)
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          mask_put(N64 * 64 + 8 * i + c0, f32[4 * i], f32[4 * i + 1], fr);
+          mask_put(N64 * 64 + 8 * i + c0, f32[4 * i + 2], f32[4 * i + 3], fr + 8);
+        }
+      if constexpr (R16)
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          mask_put(N64 * 64 + R32 * 32 + 8 * i + c0, f16[4 * i], f16[4 * i + 1], fr);
+          mask_put(N64 * 64 + R32 * 32 + 8 * i + c0, f16[4 * i + 2], f16[4 * i + 3], fr + 8);
+        }
+      mbar_wait(bar_in, ph);
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+      asm volatile("bar.sync 1, 256;" ::: "memory");      // the whole 128-row dXm tile is in place
+      // ---- D[slot][n0 ..] += In^T . dXm over the tile's 128 rows ----
+      wg_fence();
+      wg_mma_regs<64, 1, 1>(g64, 8, !first, [&](int ks, uint64_t& da, uint64_t& db) {
+        da = make_desc(aB + ks * 256, 128, FBT_SBO);
+        db = make_desc(aA + (n0 / 8) * DXF_SBO + ks * 256, 128, DXF_SBO);
+      });
+      if constexpr (H32)
+        wg_mma_regs<32, 1, 1>(g32, 8, !first, [&](int ks, uint64_t& da, uint64_t& db) {
+          da = make_desc(aB + ks * 256, 128, FBT_SBO);
+          db = make_desc(aA + ((n0 + 64) / 8) * DXF_SBO + ks * 256, 128, DXF_SBO);
+        });
+      if constexpr (H16)
+        wg_mma_regs<16, 1, 1>(g16, 8, !first, [&](int ks, uint64_t& da, uint64_t& db) {
+          da = make_desc(aB + ks * 256, 128, FBT_SBO);
+          db = make_desc(aA + ((n0 + 64 + 32 * H32) / 8) * DXF_SBO + ks * 256, 128, DXF_SBO);
+        });
+      wg_commit();
+      wg_wait<0>();
+      wg_frag_fence(g64);
+      if constexpr (H32) wg_frag_fence(g32);
+      if constexpr (H16) wg_frag_fence(g16);
+      if (lane == 0) mbar_arrive(bar_free);      // this warp is done reading dXm and In
+      first = false;
+    }
+    if (cur_u >= 0) flush(cur_u);
+  }
+#undef DXF_RANGE
+}
+
+extern "C" int tscl_dx_fc_bwd_tc(tscl_handle* h, const float* obs, const void* x_bf16, const void* dz_bf16,
+                                 const void* wxt_bf16, int64_t M, int64_t rows_per_t, int64_t stride_t, float* grads,
+                                 void* stream) {
+  if (!h || !obs || !x_bf16 || !dz_bf16 || !wxt_bf16 || !grads || M <= 0 || rows_per_t <= 0)
+    return tsc_set_error("tscl_dx_fc_bwd_tc: bad argument");
+  if (M >= ((int64_t)1 << 31) - 128) return tsc_set_error("tscl_dx_fc_bwd_tc: M must be below 2^31 - 128 rows");
+  PCK(cudaSetDevice(tscl_device_of(h)));
+  const DDimsTC& d = *tscl_dims_of(h);
+  if (!P2_DX_OK(d.dx)) return tsc_set_error("tscl_dx_fc_bwd_tc: dx must be 160, 192 or 224 (use tscl_dx_tc + tscl_fc_bwd_tc)");
+  if (d.kw == 0 || d.ones_slot < 0) return tsc_set_error("tscl_dx_fc_bwd_tc: no free input slot for the bias column");
+  CUtensorMap mZ, mX;
+  if (!make_tmap_3d(&mZ, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, dz_bf16, 2 * d.A, M, TC_N, 64, 128) ||
+      !make_tmap_3d(&mX, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, x_bf16, 2 * d.A, M, d.dx, 8, 128, CU_TENSOR_MAP_SWIZZLE_NONE))
+    return tsc_set_error("tscl_dx_fc_bwd_tc: cannot build the tensor maps (dz_bf16 / x_bf16 must be 16-byte aligned)");
+  void (*kern)(const DDimsTC, const DxFcTC, const CUtensorMap, const CUtensorMap) =
+      d.dx == 224 ? dx_fc_bwd_tc_kernel<224> : d.dx == 192 ? dx_fc_bwd_tc_kernel<192> : dx_fc_bwd_tc_kernel<160>;
+  const size_t smem = dxf_smem(d.dx);
+  static int attr_dev = -1;
+  if (attr_dev != tscl_device_of(h)) {
+    PCK(cudaFuncSetAttribute(dx_fc_bwd_tc_kernel<224>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dxf_smem(224)));
+    PCK(cudaFuncSetAttribute(dx_fc_bwd_tc_kernel<192>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dxf_smem(192)));
+    PCK(cudaFuncSetAttribute(dx_fc_bwd_tc_kernel<160>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dxf_smem(160)));
+    attr_dev = tscl_device_of(h);
+  }
+  int n_sm = 0;
+  PCK(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, tscl_device_of(h)));
+  const int64_t NT = ((M + 127) / 128) * 2 * d.A;
+  const int grid = (int)(NT < n_sm ? NT : n_sm);
+  DxFcTC a;
+  a.obs = obs; a.Wxt = (const __nv_bfloat16*)wxt_bf16; a.G = grads; a.M = M; a.rows_per_t = rows_per_t; a.stride_t = stride_t;
+  kern<<<grid, DXF_THREADS, smem, (cudaStream_t)stream>>>(d, a, mZ, mX);
   PCK(cudaGetLastError());
   return 0;
 }

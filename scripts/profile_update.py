@@ -47,6 +47,8 @@ BYTES = {   # per update
     "wgrad_tc_async_kernel": n_chunks * U * M * (4 * H * 2 + dx * 2 + H * 2),     # dZ, X, Hp (bf16)
     "dx_tc_kernel": n_chunks * U * M * (4 * H * 2 + dx * 2),                      # dZ in, dX out (bf16)
     "fc_bwd_tc_kernel": n_chunks * U * M * (dx * 2 + dx * 2),                     # dX, X (bf16)
+    # dZ, X (bf16); the observation slice (fp32, shared by an agent's two units and read through L2) is not counted
+    "dx_fc_bwd_tc_kernel": n_chunks * U * M * (4 * H * 2 + dx * 2),
     "lstm_bwd_tc_regs_kernel": n_chunks * U * M * (4 * H * 2 + H * 2 + H * 4 + 4 * H * 2),   # gates, c, dH (fp32) in, dZ out
 }
 
@@ -100,5 +102,6 @@ print("%-34s %9s %7s %6s %9s" % ("kernel", "ms", "launches", "%", "GB/s"))
 for name, (ms, n) in sorted(agg.items(), key=lambda x: -x[1][0]):
     gbs = "%9.0f" % (BYTES[name] / (ms * 1e-3) / 1e9) if name in BYTES else "        -"
     print("%-34s %9.2f %7d %6.1f %s" % (name[:34], ms, n, 100 * ms / tot, gbs))
-three = sum(agg[k][0] for k in ("wgrad_tc_async_kernel", "dx_tc_kernel", "fc_bwd_tc_kernel") if k in agg)
-print("wgrad + dx + fc_bwd: %.2f ms = %.1f %% of the update's kernel time" % (three, 100 * three / tot))
+three = sum(agg[k][0] for k in ("wgrad_tc_async_kernel", "dx_tc_kernel", "fc_bwd_tc_kernel", "dx_fc_bwd_tc_kernel")
+            if k in agg)
+print("wgrad + dx + fc_bwd (or dx_fc_bwd): %.2f ms = %.1f %% of the update's kernel time" % (three, 100 * three / tot))
