@@ -120,6 +120,13 @@ def bf16(x):
     return x.to(torch.bfloat16).to(x.dtype)
 
 
+def tf32(x):
+    """Round to the nearest TF32 value (11 significant bits, ties to even) in x's dtype: the operand rounding of a TF32
+    tensor-core product.  A model of it only: how the library rounds its TF32 operands is not specified."""
+    m, e = torch.frexp(x)
+    return torch.ldexp(torch.round(m * 2048.0) / 2048.0, e)
+
+
 def store_forward(v, lay, u, obs, dones, c0, h0):
     """Float64 forward of unit u in the activation-store layout: obs [T, rc, n_obs], c0 / h0 [rc, h] ->
     (X [T, rc, dx], gate activations [T, rc, 4h] in the order i, f, o, u, c [T, rc, h], h [T, rc, h])."""
@@ -192,19 +199,28 @@ def bptt_ref(gates, c, c0, dH, dones, wh, round_bf16=True, c_prev=None):
     return dZ
 
 
-def lstm_grads_ref(X, Hs, h0, dones, dZ, wx, round_bf16=True):
+def lstm_grads_ref(X, Hs, h0, dones, dZ, wx, round_bf16=True, round_operands=False, dx_product="bf16"):
     """LSTM weight gradients [X | Hp | 1]^T dZ and dX = dZ . Wx^T (tscl_wgrad_tc, tscl_dx_tc).  X [..., T, rc, dx],
     Hs [..., T, rc, h] (store), h0 [..., rc, h] (h_bw rows r0 .. r0 + rc), dZ [..., T, rc, 4h], wx [..., dx, 4h].
-    Hp[t] = (1 - done[t]) * (h[t-1], or h0 at t = 0).  Returns (wx, wh, bl, dX [..., T, rc, dx])."""
+    Hp[t] = (1 - done[t]) * (h[t-1], or h0 at t = 0).  Returns (wx, wh, bl, dX [..., T, rc, dx]).
+    With round_bf16 (nothing is rounded without it):
+      round_operands  X and all of Hp are rounded to bf16 as GEMM operands (the recompute path: wgrad_tc_kernel converts
+                      its fp32 X / Hp; on the store path they are bf16 already and only h0 is rounded);
+      dx_product      operands of dX: "bf16" bf16(dZ) . bf16(Wx)^T (the store path's tensor-core kernels), "fp32" the
+                      unrounded fp32 dZ . Wx^T, "tf32" both rounded to TF32 (torch.bmm with TF32 allowed);
+    dX is then rounded to bf16, where the fc weight-gradient kernel converts it."""
     keep = (1.0 - torch.as_tensor([float(d) for d in dones], dtype=X.dtype, device=X.device))[:, None, None]
     h0r = bf16(h0) if round_bf16 else h0
     Hp = torch.cat([h0r.unsqueeze(-3), Hs[..., :-1, :, :]], -3) * keep
+    if round_bf16 and round_operands:
+        X, Hp = bf16(X), bf16(Hp)
     Z = bf16(dZ) if round_bf16 else dZ
     flat = lambda t_: t_.reshape(*t_.shape[:-3], -1, t_.shape[-1])
     Zf = flat(Z)
     gwx = flat(X).transpose(-1, -2) @ Zf
     gwh = flat(Hp).transpose(-1, -2) @ Zf
-    dX = Z @ (bf16(wx) if round_bf16 else wx).transpose(-1, -2).unsqueeze(-3)
+    rnd = {"bf16": bf16, "fp32": lambda t_: t_, "tf32": tf32}[dx_product if round_bf16 else "fp32"]
+    dX = (Z if dx_product == "bf16" else rnd(dZ)) @ rnd(wx).transpose(-1, -2).unsqueeze(-3)
     return gwx, gwh, Zf.sum(-2), (bf16(dX) if round_bf16 else dX)
 
 
@@ -224,11 +240,15 @@ def fc_grads_ref(lay, u, obs, X, dX, round_bf16=True):
 
 
 def update_ref(lay, P, store, obs, act, Rs, Adv, c_bw, h_bw, dones, scale, v_coef, beta, chunk, round_bf16=True,
-               agents_per_group=None):
+               agents_per_group=None, store_units=False, round_operands=False, dx_product="bf16", agents=None):
     """Flat gradient G (float64) of one update from the activation store, summed over the chunks r0 = 0, chunk, ...
-    P: fp32 parameters (any float tensor); store(ci) -> (st_x, st_g, st_c, st_h) of chunk ci, each [U][T][rc][w];
+    P: fp32 parameters (any float tensor); store(ci) -> (st_x, st_g, st_c, st_h) of chunk ci, each [U][T][rc][w], or
+    with `store_units` store(ci, us) -> the same for the unit slice `us` only (lets a caller compute the store of one agent
+    group at a time, e.g. store_group below for the recompute path);
     obs [T, R, n_obs], act / Rs / Adv [T, R, A], c_bw / h_bw [U, R, h], dones = done_pre [T].  Work runs on P's device,
-    `agents_per_group` agents at a time (bounds the float64 working set).  Returns (G, agent-0 stats)."""
+    `agents_per_group` agents at a time (bounds the float64 working set); `agents` (a range) restricts the sum to those
+    agents.  round_operands / dx_product: see lstm_grads_ref (the defaults are the store path's rounding; the recompute
+    path is round_operands=True with dx_product "fp32" or "tf32").  Returns (G, agent-0 stats)."""
     f64 = dict(dtype=torch.float64, device=P.device)
     v = lay.views(P.to(torch.float64))
     G = torch.zeros(lay.n_params, **f64)
@@ -236,14 +256,15 @@ def update_ref(lay, P, store, obs, act, Rs, Adv, c_bw, h_bw, dones, scale, v_coe
     stats = torch.zeros(3, **f64)
     T, R, A, hd = obs.shape[0], obs.shape[1], lay.A, lay.h
     grp = agents_per_group or A
+    agents = agents if agents is not None else range(A)
     for ci, r0 in enumerate(range(0, R, chunk)):
         rc = min(chunk, R - r0)
-        st = store(ci)
+        st = None if store_units else store(ci)
         ob = obs[:, r0:r0 + rc].to(**f64)
-        for a0 in range(0, A, grp):
-            a1 = min(A, a0 + grp)
+        for a0 in range(agents.start, agents.stop, grp):
+            a1 = min(agents.stop, a0 + grp)
             us = slice(2 * a0, 2 * a1)
-            X, Gt, Cs, Hs = (s[us].to(**f64) for s in st)
+            X, Gt, Cs, Hs = (s.to(**f64) for s in store(ci, us)) if store_units else (s[us].to(**f64) for s in st)
             dH = torch.empty_like(Hs)
             for a in range(a0, a1):
                 k = 2 * (a - a0)
@@ -263,7 +284,7 @@ def update_ref(lay, P, store, obs, act, Rs, Adv, c_bw, h_bw, dones, scale, v_coe
             h0 = h_bw[us, r0:r0 + rc].to(**f64)
             dZ = bptt_ref(Gt, Cs, c0, dH, dones, v["wh"][us], round_bf16)
             del dH, Gt, Cs
-            gwx, gwh, gbl, dX = lstm_grads_ref(X, Hs, h0, dones, dZ, v["wx"][us], round_bf16)
+            gwx, gwh, gbl, dX = lstm_grads_ref(X, Hs, h0, dones, dZ, v["wx"][us], round_bf16, round_operands, dx_product)
             del dZ
             gv["wx"][us] += gwx
             gv["wh"][us] += gwh
@@ -291,3 +312,84 @@ def bptt_mutations(gates, c, c_state, r0, dH, dones):
         "c_t in place of c_{t-1}": dict(ok, c_prev=c),
         "dH one step late": dict(ok, dH=late(dH)),
     }
+
+
+# ------------------------------------------------------------------------------------------------
+# The recompute update (BatchedA2C.backward without the activation store): per chunk the forward is recomputed in fp32
+# (tscl_fc_embed, X . Wx + bl, tscl_lstm_seq_fwd from c_bw / h_bw rows r0 .. r0 + rc), then heads_loss -> BPTT with fp32
+# gates / c (dZ written fp32; the recurrent product is bf16(dz) . bf16(Wh)^T as on the store path) -> wgrad_tc_kernel,
+# which rounds its fp32 X / Hp / dZ operands to bf16 -> dX = dZ . Wx^T in fp32 or TF32 -> fc weight gradients from
+# bf16(obs) and bf16(dX * (X > 0)).  Its float64 reference is update_ref over the float64 forward (store_group) with
+# round_operands=True and dx_product "fp32" / "tf32".
+
+def store_group(v, lay, us, obs, dones, c0, h0):
+    """store_forward of the units of slice `us`, stacked: obs [T, rc, n_obs], c0 / h0 [U, rc, h] (all units, the chunk's
+    rows) -> (X, gates, c, h), each [len(us)][T][rc][w]."""
+    st = [store_forward(v, lay, u, obs, dones, c0[u], h0[u]) for u in range(us.start, us.stop)]
+    return tuple(torch.stack([s[k] for s in st]) for k in range(4))
+
+
+def recompute_mutations(obs, c_state, h_state, dones, r0, rc):
+    """Forward inputs of store_group for the chunk of rc replicas at r0, correct and with four planted defects of the
+    recompute forward: returns ({obs, dones, c0, h0}, {defect name: the same with the defect}).  obs [T + 1, R, n_obs]
+    are the rollout's observation slots (slot T is the next observation), c_state / h_state [U, R, h] are c_bw / h_bw."""
+    T = len(dones)
+    ok = dict(obs=obs[:T, r0:r0 + rc], dones=[float(d) for d in dones], c0=c_state[:, r0:r0 + rc],
+              h0=h_state[:, r0:r0 + rc])
+    return ok, {
+        "recompute from zero state": dict(ok, c0=torch.zeros_like(ok["c0"]), h0=torch.zeros_like(ok["h0"])),
+        "state from row r instead of r0 + r": dict(ok, c0=c_state[:, :rc], h0=h_state[:, :rc]),
+        "done one step late": dict(ok, dones=[0.0] + ok["dones"][:-1]),
+        "obs slot t + 1 instead of t": dict(ok, obs=obs[1:T + 1, r0:r0 + rc]),
+    }
+
+
+# ------------------------------------------------------------------------------------------------
+# The FcACPolicy update (BatchedFcA2C.backward): per chunk fc front end -> H = relu(X . wx + bl) (tscl_fc_hidden_fwd) ->
+# heads_loss -> dHm = dH * (H > 0), dX = dHm . wx^T, bl / wx gradients (tscl_fc_hidden_bwd, all fp32) -> fc weight
+# gradients from bf16(obs) and bf16(dX * (X > 0)) (tscl_fc_bwd_tc).
+
+FC_DEFECTS = ("hidden relu mask ignored", "bias gradient from unmasked dH",
+              "value unit uses the policy unit's hidden weights")
+
+
+def fc_update_ref(lay, P, obs, act, Rs, Adv, scale, v_coef, beta, chunk, round_bf16=False, agents=None, defect=None):
+    """Flat gradient G (float64) of one FcACPolicy update, summed over the chunks r0 = 0, chunk, ...: P fp32 parameters
+    of a PolicyLayout(recurrent=False), obs [T, R, n_obs], act / Rs / Adv [T, R, A].  round_bf16: obs and dX rounded to
+    bf16 where the tensor-core fc weight-gradient kernel reads them (nothing else is rounded: the other kernels are fp32).
+    `agents` (a range) restricts the sum to those agents; `defect` plants one of FC_DEFECTS.  Returns (G, agent-0 stats)."""
+    assert defect is None or defect in FC_DEFECTS, defect
+    f64 = dict(dtype=torch.float64, device=P.device)
+    v = lay.views(P.to(torch.float64))
+    G = torch.zeros(lay.n_params, **f64)
+    gv = lay.views(G)
+    stats = torch.zeros(3, **f64)
+    T, R, hd = obs.shape[0], obs.shape[1], lay.h
+    for r0 in range(0, R, chunk):
+        rc = min(chunk, R - r0)
+        ob = obs[:, r0:r0 + rc].to(**f64)
+        for a in (agents if agents is not None else range(lay.A)):
+            units = (2 * a, 2 * a + 1)
+            # hidden weights each unit's kernels read (the third defect: the value unit reads the policy unit's)
+            w_of = {u: v["wx"][2 * a if defect == FC_DEFECTS[2] else u] for u in units}
+            X = {u: fc_front(v, lay, u, ob).reshape(-1, lay.dx) for u in units}
+            H = {u: torch.relu(X[u] @ w_of[u] + v["bl"][u]) for u in units}
+            sl = lambda t_: t_[:, r0:r0 + rc, a].reshape(-1)
+            hr = heads_ref(lay, v, a, H[units[0]], H[units[1]], sl(act).to(P.device), sl(Rs).to(**f64),
+                           sl(Adv).to(**f64), scale, v_coef, beta)
+            na = int(lay.n_a[a])
+            gv["wo"][units[0]][:, :na] += hr["wo_pi"]
+            gv["bo"][units[0]][:na] += hr["bo_pi"]
+            gv["wo"][units[1]][:, 0] += hr["wo_v"]
+            gv["bo"][units[1]][0] += hr["bo_v"]
+            if a == 0:
+                stats += hr["stats"]
+            for u, dH in zip(units, (hr["dH_pi"], hr["dH_v"])):
+                dHm = dH if defect == FC_DEFECTS[0] else dH * (H[u] > 0)
+                gv["wx"][u] += X[u].T @ dHm
+                gv["bl"][u] += (dH if defect == FC_DEFECTS[1] else dHm).sum(0)
+                dX = (dHm @ w_of[u].T).reshape(T, rc, lay.dx)
+                for name, g in fc_grads_ref(lay, u, ob, X[u].reshape(T, rc, lay.dx), bf16(dX) if round_bf16 else dX,
+                                            round_bf16).items():
+                    gv[name] += g
+    return G, stats
