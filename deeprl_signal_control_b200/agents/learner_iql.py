@@ -203,14 +203,18 @@ class BatchedIQLTrainer:
     """The reference's IQL explore / backward protocol (utils.py:142-190, 236-250) for R lock-stepped replicas: per control
     step eps = eps_scheduler.get(1), ε-greedy forward, simulator step in train mode straight into the ring slot's s1,
     the slot's r / done; every n_step steps lr = lr_scheduler.get(n_step) and backward; episode ends reset every
-    replica with `dist.episode_seeds`."""
+    replica with `dist.episode_seeds`.  greward_trace: as in `BatchedTrainer` (row t of the current episode gets step t's
+    global reward of every replica; None issues no copy)."""
 
-    def __init__(self, sim, model: BatchedIQL, lr_sched, eps_sched, seed0: int = 12, replica0: int = 0):
+    def __init__(self, sim, model: BatchedIQL, lr_sched, eps_sched, seed0: int = 12, replica0: int = 0,
+                 greward_trace=None):
+        from .trainer import _check_trace
         self.sim, self.model = sim, model
         self.lr_sched, self.eps_sched = lr_sched, eps_sched
         self.seed0, self.replica0 = int(seed0), int(replica0)
         self.total_replicas = model.total_replicas
         self.T_episode = int(np.ceil(sim.params.episode_length_sec / sim.params.control_interval_sec))
+        self.greward_trace = _check_trace(greward_trace, self.T_episode, sim)
         self.episode = 0
         self.episode_rewards = []
         self.n_env_steps = 0
@@ -249,6 +253,8 @@ class BatchedIQLTrainer:
             k = m.slot
             act = m.explore(self.obs, eps, self.n_env_steps)
             _, reward, greward, _ = sim.step(act, None, obs_out=m.s1[k])
+            if self.greward_trace is not None:
+                self.greward_trace[self.step_in_episode].copy_(greward)
             self.step_in_episode += 1
             new_done = self.step_in_episode >= self.T_episode
             m.add_transition(reward, greward, self._rew_acc, new_done)

@@ -171,6 +171,21 @@ class MA2C(IA2C):
         super().__init__(n_s_ls, n_a_ls, n_w_ls, total_step, model_config, seed=seed, n_f_ls=n_f_ls, **kw)
 
 
+def iql_schedulers(model_config, total_step):
+    """(lr_scheduler, eps_scheduler) of IQL (agents/models.py:305-321): lr decays over total_step, ε over
+    total_step * epsilon_ratio, each 'constant' or 'linear'.  Shared by `IQL` and the batched training driver."""
+    lr_init = model_config.getfloat('lr_init')
+    lr_decay = model_config.get('lr_decay')
+    lr = Scheduler(lr_init, decay=lr_decay) if lr_decay == 'constant' else \
+        Scheduler(lr_init, model_config.getfloat('lr_min'), total_step, decay=lr_decay)
+    eps_init = model_config.getfloat('epsilon_init')
+    eps_decay = model_config.get('epsilon_decay')
+    eps = Scheduler(eps_init, decay=eps_decay) if eps_decay == 'constant' else \
+        Scheduler(eps_init, model_config.getfloat('epsilon_min'), total_step * model_config.getfloat('epsilon_ratio'),
+                  decay=eps_decay)
+    return lr, eps
+
+
 class IQL:
     """Independent Q-learning (agents/models.py:264-376, agents/policies.py:285-389): per-agent
     linear ('lr', LRQPolicy) or two-layer ('dqn', DeepQPolicy) Q network, epsilon-greedy exploration,
@@ -216,15 +231,7 @@ class IQL:
                 params[k + '/b'] = torch.zeros(shp[1], device=self.dev, requires_grad=True)
             self.nets.append(params)
         if total_step:
-            lr_init = model_config.getfloat('lr_init')
-            lr_decay = model_config.get('lr_decay')
-            self.lr_scheduler = Scheduler(lr_init, decay=lr_decay) if lr_decay == 'constant' else \
-                Scheduler(lr_init, model_config.getfloat('lr_min'), total_step, decay=lr_decay)
-            eps_init = model_config.getfloat('epsilon_init')
-            eps_decay = model_config.get('epsilon_decay')
-            self.eps_scheduler = Scheduler(eps_init, decay=eps_decay) if eps_decay == 'constant' else \
-                Scheduler(eps_init, model_config.getfloat('epsilon_min'),
-                          total_step * model_config.getfloat('epsilon_ratio'), decay=eps_decay)
+            self.lr_scheduler, self.eps_scheduler = iql_schedulers(model_config, total_step)
             buffer_size = model_config.getfloat('buffer_size')
             self.trans_buffer_ls = [ReplayBuffer(buffer_size, self.n_step) for _ in range(self.n_agent)]
             # TF1 AdamOptimizer state (agents/policies.py:327): first / second moments per tensor and the step count

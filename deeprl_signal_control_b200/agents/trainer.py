@@ -20,12 +20,22 @@ from ..sim import BatchedSim
 from .learner import BatchedA2C
 
 
+def _check_trace(trace, T_episode, sim):
+    if trace is not None and (tuple(trace.shape) != (T_episode, sim.R) or trace.dtype != torch.float32
+                              or trace.device != sim.device):
+        raise ValueError("greward_trace must be a float32 [%d, %d] tensor on %s (got %s %s on %s)"
+                         % (T_episode, sim.R, sim.device, tuple(trace.shape), trace.dtype, trace.device))
+    return trace
+
+
 class BatchedTrainer:
     def __init__(self, sim: BatchedSim, model: BatchedA2C, agent: str, lr, beta,
-                 seed0: int = 12, replica0: int = 0):
+                 seed0: int = 12, replica0: int = 0, greward_trace: Optional[torch.Tensor] = None):
         """lr / beta: floats (the 'constant' schedules of every shipped A2C config) or objects with the reference's
         `Scheduler.get(n_step)` (agents/utils.py:268-281, agents/models.py:175-176); a schedule advances by n_step per
-        update exactly as in the reference (its unit is control steps of ONE environment)."""
+        update exactly as in the reference (its unit is control steps of ONE environment).
+        greward_trace: optional float32 [T_episode, R] device tensor; control_step() copies step t's global reward of
+        every replica into row t of the current episode.  None: no copy is issued."""
         self.sim, self.model, self.agent = sim, model, agent
         self.lr, self.beta = lr, beta
         self.seed0, self.replica0 = int(seed0), int(replica0)
@@ -33,6 +43,7 @@ class BatchedTrainer:
         self.episode = 0
         self.T_episode = int(np.ceil(sim.params.episode_length_sec / sim.params.control_interval_sec))
         assert self.T_episode % model.T == 0                      # utils.py:121
+        self.greward_trace = _check_trace(greward_trace, self.T_episode, sim)
         self.step_in_episode = 0
         self.done = True
         self.episode_rewards = []
@@ -81,6 +92,8 @@ class BatchedTrainer:
         if self.sim_events is not None:
             e1.record()
             self.sim_events.append((e0, e1))
+        if self.greward_trace is not None:
+            self.greward_trace[self.step_in_episode].copy_(greward)
         self.step_in_episode += 1
         new_done = self.step_in_episode >= self.T_episode         # lock-step: envs/env.py:577-579
         if fused:

@@ -22,6 +22,8 @@ import sys
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
+from deeprl_signal_control_b200.envs import greedy_controller, make_env  # noqa: E402
+
 
 def parse_args(argv=None):
     p = argparse.ArgumentParser()
@@ -33,35 +35,6 @@ def parse_args(argv=None):
     p.add_argument("--output-dir", default=None)
     p.add_argument("--policy", default="lstm", choices=["lstm", "fc"])
     return p.parse_args(argv)
-
-
-def make_env(cfg, n_replicas, output_path):
-    scen = cfg.get("scenario")
-    if scen == "large_grid":
-        from deeprl_signal_control_b200.envs.large_grid_env import LargeGridEnv as Env
-    elif scen == "real_net":
-        from deeprl_signal_control_b200.envs.real_net_env import RealNetEnv as Env
-    elif scen == "small_grid":
-        from deeprl_signal_control_b200.envs.small_grid_env import SmallGridEnv as Env
-    elif cfg.get("net_file", fallback=None):
-        from deeprl_signal_control_b200.envs.sumo_env import SumoNetEnv as Env
-    else:
-        raise ValueError("unknown scenario %r" % scen)
-    return Env(cfg, output_path=output_path, is_record=True, record_stat=False, n_replicas=n_replicas)
-
-
-def greedy_controller(env):
-    from deeprl_signal_control_b200.envs.large_grid_env import LargeGridController
-    from deeprl_signal_control_b200.envs.real_net_env import RealNetController
-    from deeprl_signal_control_b200.envs.small_grid_env import SmallGridController
-    from deeprl_signal_control_b200.envs.sumo_env import SumoNetController
-    if env.name == "large_grid":
-        return LargeGridController(env.node_names)
-    if env.name == "real_net":
-        return RealNetController(env.node_names, env.nodes)
-    if env.name == "small_grid":
-        return SmallGridController(env.node_names)
-    return SumoNetController(env.node_names, env.nodes, {n: env.phase_map.phases[n].phases for n in env.node_names})
 
 
 def iql_model_type(agent):
