@@ -1,11 +1,17 @@
 """`train`: the reference's `main.py train` (main.py:82-155) with its `utils.py:Counter` / `Trainer.run`
 (utils.py:70-108, 255-308), for R lock-stepped replicas on the device.
 
-    train(config, base_dir, test_mode='no_test', n_replicas=1, policy='lstm', device=0)
+    train(config, base_dir, test_mode='no_test', n_replicas=1, policy='lstm', device=0, process_group=None)
 
 leaves the reference's agent directory: `data/` with a copy of the config and `train_reward.csv`, `model/checkpoint-<step>`
 and `log/<time>.log`; with `after_train_test` / `all_test` also `data/<scenario>_<agent>_{control,traffic,trip}.csv`.
 `scripts/evaluate.py --agent-dir base_dir` reads that directory back.
+
+With a `process_group` of W ranks, one agent trains on `n_replicas` replicas in all: rank k steps the global replicas
+[k*R/W, (k+1)*R/W) on its device, and the learner all-reduces its gradient once per update (A2C) or per round (IQL).
+Seeds, actions and replay draws are keyed by the global replica, so a run over W ranks plays the episodes of the
+one-process run with the same n_replicas; only the order in which the gradient is summed differs.  Rank 0 owns every
+file and runs every test; the other ranks write nothing under base_dir and log WARNING and above to stderr.
 
 Protocol (the reference's, applied to R replicas):
 * the global step counts control steps of the lock-step: one episode of all replicas advances it by T, so a run of
@@ -14,6 +20,7 @@ Protocol (the reference's, applied to R replicas):
   when `cur_step >= total_step`, checked only between episodes;
 * one `train_reward.csv` row per episode set (test_id -1): avg_reward = mean and std_reward = np.std of the per-step
   global reward pooled over every replica and step; one row per test seed (test_id k) with that seed's mean / std.
+  Over W > 1 ranks rank 0 gathers the [T, R] trace of all global replicas first (`training_row`).
 The training loop itself is `BatchedTrainer` / `BatchedIQLTrainer`; the tests run on the batched `Evaluator` over an
 env of its own (`ENV_CONFIG.test_seeds`, test mode, policy_type 'default'), which reads the learner's live weights on
 the device and leaves the training sim and the learner's recurrent state alone.
@@ -21,6 +28,7 @@ the device and leaves the training sim and the learner's recurrent state alone.
 from __future__ import annotations
 
 import configparser
+import hashlib
 import logging
 import os
 import shutil
@@ -28,6 +36,8 @@ import time
 import types
 
 import numpy as np
+
+from .. import dist as _dist
 
 TEST_MODES = ('no_test', 'in_train_test', 'after_train_test', 'all_test')
 
@@ -52,6 +62,15 @@ def init_log(log_dir):
         root.addHandler(h)
     root.setLevel(logging.INFO)
     return handlers
+
+
+def init_rank_log(rank):
+    """A rank other than 0 writes no log file: WARNING records and above go to stderr, prefixed with the rank."""
+    h = logging.StreamHandler()
+    h.setLevel(logging.WARNING)
+    h.setFormatter(logging.Formatter('[rank %d] %%(asctime)s [%%(levelname)s] %%(message)s' % rank))
+    logging.getLogger().addHandler(h)
+    return [h]
 
 
 def init_test_flag(test_mode):
@@ -101,29 +120,56 @@ class Counter:
         return self.cur_step >= self.total_step
 
 
+def training_row(rewards):
+    """(avg_reward, std_reward) of a training row over W > 1 ranks from the gathered [T, R_total] trace: the float64
+    mean over global replicas of each replica's episode mean, and np.std of the very array a one-process run holds.
+    avg_reward can differ in the last bits from the one-process row, which takes the trainer's float32
+    `episode_rewards[-1]`."""
+    rewards = np.asarray(rewards, np.float64)
+    return float(rewards.mean(axis=0).mean()), float(np.std(rewards))
+
+
 class Trainer:
     """utils.py:Trainer.run / Tester.run_offline over a batched trainer (`run(n)`, `T_episode`, `episode_rewards`,
-    `greward_trace` [T_episode, R]) and a batched `Evaluator` (`perform_all()`, `run()`, `env`)."""
+    `greward_trace` [T_episode, R]) and a batched `Evaluator` (`perform_all()`, `run()`, `env`).
 
-    def __init__(self, trainer, evaluator, counter: Counter, agent: str, run_test: bool, output_path: str):
+    `group`: None for one process; over W > 1 ranks a group that takes CPU tensors (gloo).  Every rank then runs the
+    same schedule; rank 0 gathers the traces, holds the rows, runs the tests (only it has an evaluator) and writes the
+    CSV, and all ranks meet at a barrier after each test."""
+
+    def __init__(self, trainer, evaluator, counter: Counter, agent: str, run_test: bool, output_path: str,
+                 group=None):
         if trainer.greward_trace is None:
             raise ValueError('the driver needs the trainer to keep a greward_trace')
         self.trainer, self.evaluator, self.counter = trainer, evaluator, counter
         self.agent, self.run_test, self.output_path = agent, run_test, output_path
+        self.group = group
+        if group is None:
+            self.rank0 = True
+        else:
+            import torch.distributed as dist
+            self.rank0 = dist.get_rank(group) == 0
         self.T = int(trainer.T_episode)
         self.data = []
         self.n_episode_sets = 0
-        if run_test:
+        if run_test and self.rank0:
             logging.info('Testing: total test num: %d' % evaluator.test_num)
 
+    def _barrier(self):
+        if self.group is not None:
+            import torch.distributed as dist
+            dist.barrier(group=self.group)
+
     def test(self):
-        step = self.counter.cur_step
-        t0 = time.time()
-        mean, std = self.evaluator.perform_all()
-        for k in range(len(mean)):
-            self.data.append({'agent': self.agent, 'step': step, 'test_id': k, 'avg_reward': float(mean[k]),
-                              'std_reward': float(std[k])})
-        logging.info('Testing: global step %d, avg R: %.2f (%.2f s)' % (step, np.mean(mean), time.time() - t0))
+        if self.rank0:
+            step = self.counter.cur_step
+            t0 = time.time()
+            mean, std = self.evaluator.perform_all()
+            for k in range(len(mean)):
+                self.data.append({'agent': self.agent, 'step': step, 'test_id': k, 'avg_reward': float(mean[k]),
+                                  'std_reward': float(std[k])})
+            logging.info('Testing: global step %d, avg R: %.2f (%.2f s)' % (step, np.mean(mean), time.time() - t0))
+        self._barrier()
 
     def run(self):
         c = self.counter
@@ -134,31 +180,47 @@ class Trainer:
             self.trainer.run(self.T)                                  # one episode of every replica
             step = c.next(self.T)
             self.n_episode_sets += 1
-            rewards = np.asarray(self.trainer.greward_trace.cpu().numpy(), np.float64)
-            mean, std = float(self.trainer.episode_rewards[-1]), float(np.std(rewards))
+            if self.group is None:
+                rewards = np.asarray(self.trainer.greward_trace.cpu().numpy(), np.float64)
+                mean, std = float(self.trainer.episode_rewards[-1]), float(np.std(rewards))
+            else:
+                rewards = _dist.gather_traces(self.trainer.greward_trace.cpu(), self.group)
+                if rewards is None:
+                    continue
+                mean, std = training_row(rewards)
             self.data.append({'agent': self.agent, 'step': step, 'test_id': -1, 'avg_reward': mean, 'std_reward': std})
             if c.should_log(prev):
                 logging.info('Training: global step %d, episode set %d, avg R: %.2f, std R: %.2f'
                              % (step, self.n_episode_sets, mean, std))
-        import pandas as pd
-        pd.DataFrame(self.data).to_csv(self.output_path + 'train_reward.csv')
+        if self.rank0:
+            import pandas as pd
+            pd.DataFrame(self.data).to_csv(self.output_path + 'train_reward.csv')
 
     def run_offline(self):
         """Tester.run_offline: every test seed in record mode, the three CSVs into output_path.  Returns the per-seed
-        (mean, std)."""
-        self.evaluator.env.init_data(True, False, self.output_path)
-        mean, std = self.evaluator.run()
-        logging.info('Offline testing: avg R: %.2f' % np.mean(mean))
-        return mean, std
+        (mean, std) on rank 0, None on the other ranks."""
+        out = None
+        if self.rank0:
+            self.evaluator.env.init_data(True, False, self.output_path)
+            mean, std = self.evaluator.run()
+            logging.info('Offline testing: avg R: %.2f' % np.mean(mean))
+            out = mean, std
+        self._barrier()
+        return out
 
 
-def build_model(agent, env, model_config, total_step, n_replicas, policy='lstm', seed=0, device=0):
-    """main.py:110-121 on the batched learners: IA2C / MA2C wrappers (seed = ENV_CONFIG.seed) or BatchedIQL (seed 0)."""
+def build_model(agent, env, model_config, total_step, n_replicas, policy='lstm', seed=0, device=0, replica0=0,
+                total_replicas=None, process_group=None):
+    """main.py:110-121 on the batched learners: IA2C / MA2C wrappers (seed = ENV_CONFIG.seed) or BatchedIQL (seed 0).
+    `n_replicas` are this rank's replicas, the global ones [replica0, replica0 + n_replicas) of `total_replicas`; the
+    learner all-reduces its gradient over `process_group` when one is given."""
     kind, model_type = model_spec(agent)
     t = env._tables
     if kind != 'iql':
         from .models import IA2C, MA2C
         kw = dict(seed=seed, n_replicas=n_replicas, obs_off=t.node_obs_off, policy=policy, device=device)
+        if process_group is not None:
+            kw.update(replica0=replica0, total_replicas=total_replicas, process_group=process_group)
         if kind == 'ma2c':
             return MA2C(env.n_s_ls, env.n_a_ls, env.n_w_ls, env.n_f_ls, total_step, model_config, **kw)
         return IA2C(env.n_s_ls, env.n_a_ls, env.n_w_ls, total_step, model_config, **kw)
@@ -169,14 +231,21 @@ def build_model(agent, env, model_config, total_step, n_replicas, policy='lstm',
     n_h = model_config.getint('num_h', fallback=0) if model_type == 'dqn' else 0
     lay = QLayout(model_type, [int(off[i + 1] - off[i]) for i in range(t.n_nodes)], t.n_a_ls, t.n_w_ls, off, t.n_obs,
                   n_fc=n_fc, n_ft=n_fc // 4, n_h=n_h, max_na=t.max_na)          # q_fct width: agents/policies.py:383
-    return BatchedIQL(lay, n_replicas, model_config, model_type, seed=0, device=device)
+    return BatchedIQL(lay, n_replicas, model_config, model_type, seed=0, device=device, replica0=replica0,
+                      total_replicas=total_replicas, pg=process_group)
 
 
-def train(config, base_dir, test_mode='no_test', n_replicas=1, policy='lstm', device=0):
+def train(config, base_dir, test_mode='no_test', n_replicas=1, policy='lstm', device=0, process_group=None):
     """main.py train.  `config`: the path of a reference config (copied into data/) or a parsed ConfigParser (written
     to data/config.ini), with [ENV_CONFIG], [MODEL_CONFIG] and [TRAIN_CONFIG].  Returns a namespace with final_step,
-    episode_sets, env_samples (= final_step * n_replicas), wall_sec, data (the train_reward.csv rows), post_test (the
-    per-seed (mean, std) of the post-training test or None), and the live model and trainer.
+    episode_sets, env_samples (= final_step * n_replicas), wall_sec, world, rank, data (the train_reward.csv rows),
+    post_test (the per-seed (mean, std) of the post-training test or None), and the live model and trainer.
+
+    `process_group`: None trains in this process alone.  A group of W > 1 ranks trains one agent on `n_replicas`
+    replicas in all, R/W on each rank (W must divide n_replicas), on `device`; every rank of the group calls train()
+    with the same arguments.  Rank 0 writes every file and runs every test; `data` and `post_test` are None on the
+    other ranks.  The host-side gathers and barriers run on the group itself when its backend is gloo, else on a gloo
+    group over the same ranks, which torch.distributed.new_group makes every process of the default group enter.
 
     The post-training test follows what the reference intends (main.py:147-150) rather than what its code does: its
     `Tester.__init__` calls `Trainer.__init__` without `run_test`, and `run_offline` is passed an argument it does not
@@ -184,18 +253,30 @@ def train(config, base_dir, test_mode='no_test', n_replicas=1, policy='lstm', de
     every test seed is played once in record mode and the three CSVs go into data/."""
     t0 = time.time()
     in_test, post_test = init_test_flag(test_mode)
-    dirs = init_dir(base_dir)
-    handlers = init_log(dirs['log'])
+    world, rank = 1, 0
+    if process_group is not None:
+        import torch.distributed as dist
+        world, rank = dist.get_world_size(process_group), dist.get_rank(process_group)
+    pg = process_group if world > 1 else None
+    _dist.replica_range(rank, world, int(n_replicas))                 # every rank rejects an uneven split alike
+    if rank == 0:
+        dirs = init_dir(base_dir)
+        handlers = init_log(dirs['log'])
+    else:
+        dirs = {k: os.path.join(base_dir, k) + os.sep for k in ('log', 'data', 'model')}
+        handlers = init_rank_log(rank)
     try:
         if isinstance(config, configparser.ConfigParser):
-            with open(os.path.join(dirs['data'], 'config.ini'), 'w') as f:
-                config.write(f)
+            if rank == 0:
+                with open(os.path.join(dirs['data'], 'config.ini'), 'w') as f:
+                    config.write(f)
         else:
-            shutil.copy(config, dirs['data'])
+            if rank == 0:
+                shutil.copy(config, dirs['data'])
             path, config = config, configparser.ConfigParser()
             if not config.read(path):
                 raise FileNotFoundError(path)
-        out = _train(config, dirs, in_test, post_test, int(n_replicas), policy, device)
+        out = _train(config, dirs, in_test, post_test, int(n_replicas), policy, device, pg)
     finally:
         for h in handlers:
             logging.getLogger().removeHandler(h)
@@ -204,46 +285,98 @@ def train(config, base_dir, test_mode='no_test', n_replicas=1, policy='lstm', de
     return out
 
 
-def _train(config, dirs, in_test, post_test, R, policy, device):
+def host_group(pg):
+    """The group of the driver's host-side gathers and barriers: `pg` itself when its backend is gloo, else a new gloo
+    group over the same ranks.  Keeps them off the learner's NCCL stream and lets CPU tensors through."""
+    import torch.distributed as dist
+    if dist.get_backend(pg) == 'gloo':
+        return pg, False
+    return dist.new_group(ranks=dist.get_process_group_ranks(pg), backend='gloo'), True
+
+
+def state_digest(model):
+    """SHA-256 of the learner state every rank must hold bit for bit: the weights and the optimiser slots (RMSProp ms,
+    or Adam m, v and step count)."""
+    if model.name == 'iql':
+        tensors, extra = (model.P, model.M, model.V), np.int64(model.t).tobytes()
+    else:
+        tensors, extra = (model.batched.P, model.batched.MS), b''
+    h = hashlib.sha256(extra)
+    for t in tensors:
+        h.update(t.detach().cpu().numpy().tobytes())
+    return h.digest()
+
+
+def check_ranks_agree(model, group):
+    """Raise on every rank unless all ranks of `group` (gloo) hold bit-identical learner state.  The ranks apply the
+    same all-reduced gradient to the same weights, so a difference means one of them drifted."""
+    import torch
+    import torch.distributed as dist
+    mine = torch.frombuffer(bytearray(state_digest(model)), dtype=torch.uint8)
+    all_ = [torch.empty_like(mine) for _ in range(dist.get_world_size(group))]
+    dist.all_gather(all_, mine, group=group)
+    differ = [k for k, d in enumerate(all_) if not torch.equal(d, all_[0])]
+    if differ:
+        raise RuntimeError('the learner state of rank(s) %s differs from rank 0\'s: the ranks no longer train one '
+                           'model' % differ)
+
+
+def _train(config, dirs, in_test, post_test, R_total, policy, device, pg):
     import torch
     from ..envs import make_env
     from .evaluator import Evaluator
     env_cfg, mc = config['ENV_CONFIG'], config['MODEL_CONFIG']
     agent = env_cfg.get('agent')
     model_spec(agent)                                                 # reject greedy / a2c before any device work
+    world, rank = 1, 0
+    if pg is not None:
+        import torch.distributed as dist
+        world, rank = dist.get_world_size(pg), dist.get_rank(pg)
+    replica0, R = _dist.replica_range(rank, world, R_total)
     env = make_env(env_cfg, R, dirs['data'], is_record=False, device=device)
     logging.info('Training: s dim: %d, s dim ls: %r, a dim ls: %r, replicas: %d'
-                 % (env.n_s, env.n_s_ls, env.n_a_ls, R))
+                 % (env.n_s, env.n_s_ls, env.n_a_ls, R_total) + (' over %d ranks' % world if world > 1 else ''))
     total_step = int(config.getfloat('TRAIN_CONFIG', 'total_step'))
     counter = Counter(total_step, int(config.getfloat('TRAIN_CONFIG', 'test_interval')),
                       int(config.getfloat('TRAIN_CONFIG', 'log_interval')))
     seed = env_cfg.getint('seed')
-    model = build_model(agent, env, mc, total_step, R, policy=policy, seed=seed, device=device)
-    sim = env._ensure_sim()
     T = int(env.T)
     if T % mc.getint('batch_size'):                                   # utils.py:121
         raise ValueError('episode length T = %d is not a multiple of batch_size = %d' % (T, mc.getint('batch_size')))
-    trace = torch.zeros(T, R, dtype=torch.float32, device=sim.device)
-    if model.name == 'iql':
-        from .learner_iql import BatchedIQLTrainer
-        from .models import iql_schedulers
-        lr_s, eps_s = iql_schedulers(mc, total_step)
-        trainer = BatchedIQLTrainer(sim, model, lr_s, eps_s, seed0=seed, greward_trace=trace)
-    else:
-        from .trainer import BatchedTrainer
-        trainer = BatchedTrainer(sim, model.batched, agent, model.lr_scheduler, model.beta_scheduler, seed0=seed,
-                                 greward_trace=trace)
-    evaluator = None
-    if in_test or post_test:
-        test_env = make_env(env_cfg, len(env.test_seeds), dirs['data'], is_record=False, device=device)
-        evaluator = Evaluator(test_env, model, dirs['data'], policy_type='default')
-    driver = Trainer(trainer, evaluator, counter, agent, in_test, dirs['data'])
-    driver.run()
-    final_step = counter.cur_step
-    logging.info('Training: save final model at step %d ...' % final_step)
-    model.save(dirs['model'], final_step)
-    post = driver.run_offline() if post_test else None
-    torch.cuda.synchronize(sim.device)
+    group, own_group = host_group(pg) if pg is not None else (None, False)
+    try:
+        model = build_model(agent, env, mc, total_step, R, policy=policy, seed=seed, device=device, replica0=replica0,
+                            total_replicas=R_total, process_group=pg)
+        sim = env._ensure_sim()
+        trace = torch.zeros(T, R, dtype=torch.float32, device=sim.device)
+        if model.name == 'iql':
+            from .learner_iql import BatchedIQLTrainer
+            from .models import iql_schedulers
+            lr_s, eps_s = iql_schedulers(mc, total_step)
+            trainer = BatchedIQLTrainer(sim, model, lr_s, eps_s, seed0=seed, replica0=replica0, greward_trace=trace)
+        else:
+            from .trainer import BatchedTrainer
+            trainer = BatchedTrainer(sim, model.batched, agent, model.lr_scheduler, model.beta_scheduler, seed0=seed,
+                                     replica0=replica0, greward_trace=trace)
+        evaluator = None
+        if (in_test or post_test) and rank == 0:
+            test_env = make_env(env_cfg, len(env.test_seeds), dirs['data'], is_record=False, device=device)
+            evaluator = Evaluator(test_env, model, dirs['data'], policy_type='default')
+        driver = Trainer(trainer, evaluator, counter, agent, in_test, dirs['data'], group=group)
+        driver.run()
+        final_step = counter.cur_step
+        if group is not None:
+            check_ranks_agree(model, group)
+        if rank == 0:
+            logging.info('Training: save final model at step %d ...' % final_step)
+            model.save(dirs['model'], final_step)
+        post = driver.run_offline() if post_test else None
+        torch.cuda.synchronize(sim.device)
+    finally:
+        if own_group:
+            import torch.distributed as dist
+            dist.destroy_process_group(group)
     return types.SimpleNamespace(final_step=final_step, episode_sets=driver.n_episode_sets,
-                                 env_samples=final_step * R, data=driver.data, post_test=post, model=model,
+                                 env_samples=final_step * R_total, world=world, rank=rank,
+                                 data=driver.data if rank == 0 else None, post_test=post, model=model,
                                  trainer=trainer)

@@ -3,10 +3,36 @@ simulation path has no collective; the learner all-reduces (SUM) its flat gradie
 after each rank scaled its local sum by 1 / (n_step * total_replicas).
 
 Used by the product path: `BatchedTrainer.start_episode` (episode_seeds), `BatchedA2C.backward` (grad_scale,
-allreduce_sum_) and bench.py (shard_replicas)."""
+allreduce_sum_), the training driver `agents/train.py` (replica_range, gather_traces) and bench.py (shard_replicas)."""
 from __future__ import annotations
 
 import numpy as np
+
+
+def replica_range(rank: int, world: int, total_replicas: int):
+    """(replica0, n_local) of `rank` when `total_replicas` global replicas are split evenly over `world` ranks: rank k
+    owns [k*R/W, (k+1)*R/W).  Raises ValueError unless world divides total_replicas, so that every rank rejects a bad
+    split alike, before any collective."""
+    rank, world, total = int(rank), int(world), int(total_replicas)
+    if world < 1 or not 0 <= rank < world:
+        raise ValueError("rank %d is not in a world of %d" % (rank, world))
+    if total % world:
+        raise ValueError("%d replicas cannot be split evenly over %d ranks" % (total, world))
+    n = total // world
+    return rank * n, n
+
+
+def gather_traces(trace, group=None, dst: int = 0):
+    """Host-side gather of every rank's [T, r] trace (the same r on every rank) to group rank `dst`, in global replica
+    order: rank k's columns land at [k*r, (k+1)*r) of the result.  `trace` is a host array or CPU tensor, so the group
+    must take CPU tensors (gloo).  Returns the float32 [T, world*r] numpy array on `dst`, None on every other rank."""
+    import torch
+    import torch.distributed as dist
+    t = torch.as_tensor(np.ascontiguousarray(trace, dtype=np.float32))
+    parts = [torch.empty_like(t) for _ in range(dist.get_world_size(group))] \
+        if dist.get_rank(group) == dst else None
+    dist.gather(t, parts, group=group, group_dst=dst)
+    return None if parts is None else torch.cat(parts, 1).numpy()
 
 
 def shard_replicas(rank: int, world: int, replicas_per_rank: int, seed0: int):

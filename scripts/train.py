@@ -3,6 +3,8 @@ device-resident learners (deeprl_signal_control_b200/agents/train.py).
 
   python scripts/train.py --base-dir DIR train --config-dir CFG.ini
                           [--test-mode no_test|in_train_test|after_train_test|all_test] [--replicas N] [--policy lstm|fc]
+  torchrun --nproc-per-node W scripts/train.py --base-dir DIR train --config-dir CFG.ini --replicas N
+                          [--backend nccl|gloo] ...
 
 The agent is `[ENV_CONFIG] agent` of the config: ia2c, ma2c, iqld (IQL with DeepQPolicy) or any other name, e.g. iqll
 (IQL with LRQPolicy).  `--replicas` lock-stepped environments train together (default 1, the reference's single
@@ -11,13 +13,23 @@ run, each on N times the data.  DIR receives data/<config>.ini, data/train_rewar
 log/<time>.log, and with after_train_test / all_test the three evaluation CSVs in data/.  Name DIR after the agent
 and `scripts/evaluate.py --agent-dir DIR` evaluates the result.  Prints one JSON line: final step, episode sets, env
 samples (steps x replicas) and wall seconds.
+
+Under torchrun with W > 1 processes, the N replicas are split over the W ranks (W must divide N), one GPU per rank
+(LOCAL_RANK), and the learner all-reduces its gradient once per update over `--backend` (default nccl).  Rank 0 writes
+the directory and prints the JSON line, with "world": W; the run plays the episodes of a one-process run with the same
+--replicas.
 """
 import argparse
+import datetime
 import json
 import os
 import sys
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+# The longest wait at a collective is the other ranks' at the barrier while rank 0 runs a test; a rank that fails ends
+# the run after this long instead of leaving the others waiting.
+TIMEOUT = datetime.timedelta(minutes=10)
 
 
 def parse_args(argv=None):
@@ -28,8 +40,10 @@ def parse_args(argv=None):
     sp.add_argument("--test-mode", default="no_test", help="test mode during training",
                     choices=["no_test", "in_train_test", "after_train_test", "all_test"])
     sp.add_argument("--config-dir", default="./config/config_test_large.ini", help="experiment config path")
-    sp.add_argument("--replicas", type=int, default=1, help="lock-stepped environments (default 1)")
+    sp.add_argument("--replicas", type=int, default=1, help="lock-stepped environments in all ranks (default 1)")
     sp.add_argument("--policy", default="lstm", choices=["lstm", "fc"])
+    sp.add_argument("--backend", default="nccl", choices=["nccl", "gloo"],
+                    help="gradient all-reduce backend under torchrun (default nccl)")
     a = p.parse_args(argv)
     if not a.option:
         p.print_help()
@@ -39,10 +53,31 @@ def parse_args(argv=None):
 
 def main(argv=None):
     a = parse_args(argv)
-    from deeprl_signal_control_b200.agents.train import train
-    out = train(a.config_dir, a.base_dir, a.test_mode, n_replicas=a.replicas, policy=a.policy)
-    print(json.dumps({"final_step": out.final_step, "episode_sets": out.episode_sets, "env_samples": out.env_samples,
-                      "replicas": a.replicas, "wall_sec": round(out.wall_sec, 3)}))
+    world = int(os.environ.get("WORLD_SIZE", "1"))
+    if world <= 1:
+        from deeprl_signal_control_b200.agents.train import train
+        out = train(a.config_dir, a.base_dir, a.test_mode, n_replicas=a.replicas, policy=a.policy)
+        print(json.dumps({"final_step": out.final_step, "episode_sets": out.episode_sets,
+                          "env_samples": out.env_samples, "replicas": a.replicas, "wall_sec": round(out.wall_sec, 3)}))
+        return out
+    local_rank = int(os.environ["LOCAL_RANK"])
+    from deeprl_signal_control_b200.dist import bind_to_gpu_numa
+    bind_to_gpu_numa(local_rank)                  # before torch allocates anything page-locked
+    import torch
+    import torch.distributed as dist
+    torch.cuda.set_device(local_rank)
+    kw = {"device_id": torch.device("cuda", local_rank)} if a.backend == "nccl" else {}
+    dist.init_process_group(a.backend, timeout=TIMEOUT, **kw)
+    try:
+        from deeprl_signal_control_b200.agents.train import train
+        out = train(a.config_dir, a.base_dir, a.test_mode, n_replicas=a.replicas, policy=a.policy, device=local_rank,
+                    process_group=dist.group.WORLD)
+    finally:
+        dist.destroy_process_group()
+    if out.rank == 0:
+        print(json.dumps({"final_step": out.final_step, "episode_sets": out.episode_sets,
+                          "env_samples": out.env_samples, "replicas": a.replicas, "world": world,
+                          "wall_sec": round(out.wall_sec, 3)}))
     return out
 
 
