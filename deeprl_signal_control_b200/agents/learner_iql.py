@@ -79,7 +79,8 @@ class BatchedIQL:
         self.q = torch.zeros(R, A, layout.max_na, **f32)
         self.act = torch.zeros(R, A, dtype=torch.int32, device=self.dev)
         self.idx = torch.zeros(A, R, self.batch_size, dtype=torch.int32, device=self.dev)
-        self.grad = torch.zeros(layout.n_params + A, **f32)
+        # flat gradient, then per agent the loss, mean q(s)[a] and mean tq of the round (tscl_q_td's tails)
+        self.grad = torch.zeros(layout.n_params + 3 * A, **f32)
         self.losses = torch.zeros(N_ROUNDS, A, **f32)
         self.norms = torch.zeros(N_ROUNDS, A, **f32)
         self.n_updates = 0                             # backwards that ran (keys the minibatch draws)
@@ -139,8 +140,10 @@ class BatchedIQL:
             C.c_int64(self.n_updates), C.c_int32(rnd), C.c_int64(self.replica0), _p(self.idx), self._st()))
         return self.idx
 
-    def td_round(self, rnd: int, lr: float, idx=None):
-        """One minibatch round for every agent on the ring entries idx [A][R][batch] (default: this round's draws)."""
+    def td_round(self, rnd: int, lr: float, idx=None, rec=None):
+        """One minibatch round for every agent on the ring entries idx [A][R][batch] (default: this round's draws).
+        `rec`: optional float32 [A, 4] device tensor that receives every agent's (loss, mean q, mean tq, pre-clip norm),
+        the reference's QPolicy summaries (agents/policies.py:331-338), written by the Adam kernel itself."""
         lib = _lib.lib()
         if idx is None:
             idx = self.sample(rnd)
@@ -153,14 +156,22 @@ class BatchedIQL:
         self.t += 1
         lr_t = lr * np.sqrt(1.0 - 0.999 ** self.t) / (1.0 - 0.9 ** self.t)
         _lib.check(lib.tscl_q_adam(self._h, _p(self.P), _p(self.grad), _p(self.M), _p(self.V), C.c_float(lr_t),
-                                   C.c_float(self.max_grad_norm), _p(self.losses[rnd]), _p(self.norms[rnd]), self._st()))
+                                   C.c_float(self.max_grad_norm), _p(self.losses[rnd]), _p(self.norms[rnd]), _p(rec),
+                                   self._st()))
 
-    def backward(self, lr: float) -> bool:
-        """IQL.backward after lr = lr_scheduler.get(n_step) (taken by the caller even when this returns False)."""
+    def backward(self, lr: float, rec=None) -> bool:
+        """IQL.backward after lr = lr_scheduler.get(n_step) (taken by the caller even when this returns False).
+        `rec`: optional float32 [N_ROUNDS, A, 4] device tensor; row k receives round k's summaries (td_round)."""
         if self.size < self.batch_size:
             return False
+        if rec is not None and (tuple(rec.shape) != (N_ROUNDS, self.n_agent, 4) or rec.dtype != torch.float32
+                                or rec.device != self.dev or not rec.is_contiguous()):
+            raise ValueError('rec must be a contiguous float32 [%d, %d, 4] tensor on %s' % (N_ROUNDS, self.n_agent, self.dev))
         for k in range(N_ROUNDS):
-            self.td_round(k, lr)
+            if rec is None:
+                self.td_round(k, lr)
+            else:
+                self.td_round(k, lr, rec=rec[k])
         self.n_updates += 1
         return True
 
@@ -204,17 +215,23 @@ class BatchedIQLTrainer:
     step eps = eps_scheduler.get(1), ε-greedy forward, simulator step in train mode straight into the ring slot's s1,
     the slot's r / done; every n_step steps lr = lr_scheduler.get(n_step) and backward; episode ends reset every
     replica with `dist.episode_seeds`.  greward_trace: as in `BatchedTrainer` (row t of the current episode gets step t's
-    global reward of every replica; None issues no copy)."""
+    global reward of every replica; None issues no copy).
+    summary_rec: optional float32 [ceil(T_episode / n_step), N_ROUNDS, A, 4] device tensor; the Adam kernel of round k
+    of the episode's update j writes every agent's (loss, mean q, mean tq, pre-clip norm) into [j, k], and
+    summary_ran[j] says whether update j ran (False while the ring holds fewer than batch_size entries)."""
 
     def __init__(self, sim, model: BatchedIQL, lr_sched, eps_sched, seed0: int = 12, replica0: int = 0,
-                 greward_trace=None):
-        from .trainer import _check_trace
+                 greward_trace=None, summary_rec=None):
+        from .trainer import _check_rec, _check_trace
         self.sim, self.model = sim, model
         self.lr_sched, self.eps_sched = lr_sched, eps_sched
         self.seed0, self.replica0 = int(seed0), int(replica0)
         self.total_replicas = model.total_replicas
         self.T_episode = int(np.ceil(sim.params.episode_length_sec / sim.params.control_interval_sec))
         self.greward_trace = _check_trace(greward_trace, self.T_episode, sim)
+        n_upd = -(-self.T_episode // model.n_step)
+        self.summary_rec = _check_rec(summary_rec, (n_upd, N_ROUNDS, model.n_agent, 4), sim.device)
+        self.summary_ran = np.zeros(n_upd, bool)
         self.episode = 0
         self.episode_rewards = []
         self.n_env_steps = 0
@@ -267,7 +284,13 @@ class BatchedIQLTrainer:
         if self._since_update == m.n_step or done:
             self._since_update = 0
             lr = self.lr_sched.get(m.n_step)
-            if self._timed(self.update_events, lambda: m.backward(lr)):
+            if self.summary_rec is None:
+                ran = self._timed(self.update_events, lambda: m.backward(lr))
+            else:
+                j = (self.step_in_episode - 1) // m.n_step
+                ran = self._timed(self.update_events, lambda: m.backward(lr, rec=self.summary_rec[j]))
+                self.summary_ran[j] = ran
+            if ran:
                 self.n_updates += 1
         if done:
             self.episode_rewards.append(float((self._rew_acc / self.T_episode).mean()))

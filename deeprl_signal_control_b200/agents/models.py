@@ -2,7 +2,8 @@
 
     IA2C(n_s_ls, n_a_ls, n_w_ls, total_step, model_config, seed=0)
     MA2C(n_s_ls, n_a_ls, n_w_ls, n_f_ls, total_step, model_config, seed=0)
-    forward(obs, done, out_type='pv'), backward(R_ls, summary_writer=None, global_step=None),
+    forward(obs, done, out_type='pv'), backward(R_ls, summary_writer=None, global_step=None) (the writer receives agent
+    0's loss terms and gradient norm, agents/policies.py:62-72),
     add_transition(obs, actions, rewards, values, done), reset(), save(dir, step), load(dir, checkpoint)
     attributes n_step, n_agent, sess (None: there is no TF session), policy_ls is not provided.
 
@@ -40,6 +41,7 @@ class IA2C:
         self.n_step = model_config.getint('batch_size')
         self.sess = None
         self.total_step = total_step
+        self.policy = policy
         if obs_off is None:
             obs_off = np.concatenate([[0], np.cumsum(self.n_s_ls)])
         n_obs = int(obs_off[self.n_agent]) if len(obs_off) > self.n_agent else int(np.sum(self.n_s_ls))
@@ -116,6 +118,14 @@ class IA2C:
         cur_beta = self.beta_scheduler.get(self.n_step)
         boot = torch.tensor(np.asarray(R_ls, np.float32).reshape(1, -1), device=self.batched.dev)
         self.batched.backward(boot, cur_lr, cur_beta)
+        if summary_writer is not None:
+            # agents/policies.py:62-72: agent 0's loss terms and pre-clip gradient norm at global_step; any writer with
+            # add_scalar(tag, value, step) (agents/summary.py:SummaryWriter, torch.utils.tensorboard) will do
+            from .summary import a2c_values, summary_name
+            b = self.batched
+            rec = torch.cat([b.stats[:3], b.norms[:1]]).cpu().numpy()
+            for tag, v in a2c_values(summary_name(self.name, self.policy), rec).items():
+                summary_writer.add_scalar(tag, float(v), global_step)
 
     def reset(self):
         self.batched.reset()
@@ -292,6 +302,7 @@ class IQL:
         with torch.no_grad():
             tq = torch.where(D, R, R + self.gamma * self._q(i, S1).max(1)[0])
         loss = ((q0 - tq) ** 2).mean()
+        self.td_means = (q0.detach().mean(), tq.mean())         # the summaries' q and tq (agents/policies.py:335-336)
         keys = list(p.keys())
         grads = torch.autograd.grad(loss, [p[k] for k in keys])
         norm = torch.sqrt(sum((g * g).sum() for g in grads))
@@ -310,13 +321,20 @@ class IQL:
         return float(loss.detach()), float(norm)
 
     def backward(self, summary_writer=None, global_step=None):
+        """With a writer (add_scalar(tag, value, step)), agent 0's loss, mean q, mean tq and pre-clip gradient norm of
+        round k go in at global_step + k (agents/policies.py:331-338, agents/models.py:337-345)."""
         cur_lr = self.lr_scheduler.get(self.n_step)
         if self.trans_buffer_ls[0].size < self.trans_buffer_ls[0].batch_size:
             return
+        name = self._prefix(0)[:-len('_q/')]
         for i in range(self.n_agent):
-            for _ in range(10):                                   # agents/models.py:337-345
+            for k in range(10):                                   # agents/models.py:337-345
                 obs, acts, next_obs, rs, dones = self.trans_buffer_ls[i].sample_transition()
-                self.td_update(i, obs, acts, next_obs, dones, rs, cur_lr)
+                loss, norm = self.td_update(i, obs, acts, next_obs, dones, rs, cur_lr)
+                if i == 0 and summary_writer is not None:
+                    q, tq = (float(x) for x in self.td_means)
+                    for tag, v in (('loss', loss), ('q', q), ('tq', tq), ('gradnorm', norm)):
+                        summary_writer.add_scalar('train/%s_%s' % (name, tag), v, global_step + k)
 
     def reset(self):
         return

@@ -1,10 +1,12 @@
 """`train`: the reference's `main.py train` (main.py:82-155) with its `utils.py:Counter` / `Trainer.run`
 (utils.py:70-108, 255-308), for R lock-stepped replicas on the device.
 
-    train(config, base_dir, test_mode='no_test', n_replicas=1, policy='lstm', device=0, process_group=None)
+    train(config, base_dir, test_mode='no_test', n_replicas=1, policy='lstm', device=0, process_group=None,
+          summaries=False)
 
 leaves the reference's agent directory: `data/` with a copy of the config and `train_reward.csv`, `model/checkpoint-<step>`
-and `log/<time>.log`; with `after_train_test` / `all_test` also `data/<scenario>_<agent>_{control,traffic,trip}.csv`.
+and `log/<time>.log`; with `after_train_test` / `all_test` also `data/<scenario>_<agent>_{control,traffic,trip}.csv`;
+with `summaries` also the TensorBoard event file `log/events.out.tfevents.<time>.<host>` (`Summaries`).
 `scripts/evaluate.py --agent-dir base_dir` reads that directory back.
 
 With a `process_group` of W ranks, one agent trains on `n_replicas` replicas in all: rank k steps the global replicas
@@ -120,6 +122,51 @@ class Counter:
         return self.cur_step >= self.total_step
 
 
+class Summaries:
+    """The reference's TensorBoard log of a training run (utils.py:129-140, 255-306; agents/policies.py:62-72, 331-338):
+    agent 0's scalars of every update (A2C: policy / value / total loss and gradient norm at the step of the backward;
+    IQL: loss, mean q, mean target and gradient norm of round k at that step + k), `train_reward` once per episode set
+    (the training row's avg_reward, at the step of its last update) and `test_reward` once per in-training test (the
+    mean over test seeds of the per-seed means, at the step of the test).
+
+    The learners keep each update's record on the device (the trainers' `summary_rec`); the driver reads it once per
+    episode set, where it reads the reward trace, and writes that set's events then (wall_time: the time of writing).
+    Over W > 1 ranks the A2C loss terms are each rank's partial sums, so rank 0 adds them over the ranks
+    (`dist.sum_partials`); the gradient norms and the IQL records are global after the gradient all-reduce.  `writer` is
+    the SummaryWriter on rank 0 and None on the other ranks, which only take part in the sums."""
+
+    def __init__(self, writer, name, kind, n_step):
+        self.writer, self.name, self.kind, self.n_step = writer, name, kind, int(n_step)
+
+    def record(self, trainer, group=None):
+        """This episode set's records on rank 0 (A2C [n_updates, 4], IQL agent 0's [n_updates, rounds, 4]), None on
+        the other ranks; every rank of `group` must call it."""
+        if self.kind == 'iql':
+            return None if self.writer is None else trainer.summary_rec[:, :, 0, :].cpu().numpy()
+        rec = trainer.summary_rec.cpu().numpy()
+        if group is not None:
+            loss = _dist.sum_partials(rec[:, :3], group)
+            if loss is None:
+                return None
+            rec = np.concatenate([loss, rec[:, 3:]], 1)
+        return rec
+
+    def episode_set(self, rec, ran, prev_step, step, train_reward):
+        from .summary import a2c_events, iql_events
+        first = prev_step + self.n_step
+        events = iql_events(self.name, rec, ran, first, self.n_step) if self.kind == 'iql' else \
+            a2c_events(self.name, rec, first, self.n_step)
+        now = time.time()
+        for st, values in events:
+            self.writer.add_scalars(values, st, now)
+        self.writer.add_scalar('train_reward', train_reward, step, now)
+        self.writer.flush()
+
+    def test_reward(self, value, step):
+        self.writer.add_scalar('test_reward', value, step)
+        self.writer.flush()
+
+
 def training_row(rewards):
     """(avg_reward, std_reward) of a training row over W > 1 ranks from the gathered [T, R_total] trace: the float64
     mean over global replicas of each replica's episode mean, and np.std of the very array a one-process run holds.
@@ -135,15 +182,16 @@ class Trainer:
 
     `group`: None for one process; over W > 1 ranks a group that takes CPU tensors (gloo).  Every rank then runs the
     same schedule; rank 0 gathers the traces, holds the rows, runs the tests (only it has an evaluator) and writes the
-    CSV, and all ranks meet at a barrier after each test."""
+    CSV, and all ranks meet at a barrier after each test.
+    `summary`: None, or the `Summaries` of the run (the trainer then keeps a `summary_rec`)."""
 
     def __init__(self, trainer, evaluator, counter: Counter, agent: str, run_test: bool, output_path: str,
-                 group=None):
+                 group=None, summary=None):
         if trainer.greward_trace is None:
             raise ValueError('the driver needs the trainer to keep a greward_trace')
         self.trainer, self.evaluator, self.counter = trainer, evaluator, counter
         self.agent, self.run_test, self.output_path = agent, run_test, output_path
-        self.group = group
+        self.group, self.summary = group, summary
         if group is None:
             self.rank0 = True
         else:
@@ -169,6 +217,8 @@ class Trainer:
                 self.data.append({'agent': self.agent, 'step': step, 'test_id': k, 'avg_reward': float(mean[k]),
                                   'std_reward': float(std[k])})
             logging.info('Testing: global step %d, avg R: %.2f (%.2f s)' % (step, np.mean(mean), time.time() - t0))
+            if self.summary is not None:
+                self.summary.test_reward(float(np.mean(mean)), step)
         self._barrier()
 
     def run(self):
@@ -180,6 +230,7 @@ class Trainer:
             self.trainer.run(self.T)                                  # one episode of every replica
             step = c.next(self.T)
             self.n_episode_sets += 1
+            rec = self.summary.record(self.trainer, self.group) if self.summary is not None else None
             if self.group is None:
                 rewards = np.asarray(self.trainer.greward_trace.cpu().numpy(), np.float64)
                 mean, std = float(self.trainer.episode_rewards[-1]), float(np.std(rewards))
@@ -189,6 +240,8 @@ class Trainer:
                     continue
                 mean, std = training_row(rewards)
             self.data.append({'agent': self.agent, 'step': step, 'test_id': -1, 'avg_reward': mean, 'std_reward': std})
+            if self.summary is not None:
+                self.summary.episode_set(rec, self.trainer.summary_ran, prev, step, mean)
             if c.should_log(prev):
                 logging.info('Training: global step %d, episode set %d, avg R: %.2f, std R: %.2f'
                              % (step, self.n_episode_sets, mean, std))
@@ -235,7 +288,8 @@ def build_model(agent, env, model_config, total_step, n_replicas, policy='lstm',
                       total_replicas=total_replicas, pg=process_group)
 
 
-def train(config, base_dir, test_mode='no_test', n_replicas=1, policy='lstm', device=0, process_group=None):
+def train(config, base_dir, test_mode='no_test', n_replicas=1, policy='lstm', device=0, process_group=None,
+          summaries=False):
     """main.py train.  `config`: the path of a reference config (copied into data/) or a parsed ConfigParser (written
     to data/config.ini), with [ENV_CONFIG], [MODEL_CONFIG] and [TRAIN_CONFIG].  Returns a namespace with final_step,
     episode_sets, env_samples (= final_step * n_replicas), wall_sec, world, rank, data (the train_reward.csv rows),
@@ -250,7 +304,10 @@ def train(config, base_dir, test_mode='no_test', n_replicas=1, policy='lstm', de
     The post-training test follows what the reference intends (main.py:147-150) rather than what its code does: its
     `Tester.__init__` calls `Trainer.__init__` without `run_test`, and `run_offline` is passed an argument it does not
     take, so both raise TypeError and the reference's after_train_test never runs.  Here the model is saved first, then
-    every test seed is played once in record mode and the three CSVs go into data/."""
+    every test seed is played once in record mode and the three CSVs go into data/.
+
+    `summaries`: also write the reference's TensorBoard event file into log/ (`Summaries`; rank 0 only).  Off by default:
+    the run then allocates, launches and writes nothing for it."""
     t0 = time.time()
     in_test, post_test = init_test_flag(test_mode)
     world, rank = 1, 0
@@ -276,7 +333,7 @@ def train(config, base_dir, test_mode='no_test', n_replicas=1, policy='lstm', de
             path, config = config, configparser.ConfigParser()
             if not config.read(path):
                 raise FileNotFoundError(path)
-        out = _train(config, dirs, in_test, post_test, int(n_replicas), policy, device, pg)
+        out = _train(config, dirs, in_test, post_test, int(n_replicas), policy, device, pg, bool(summaries))
     finally:
         for h in handlers:
             logging.getLogger().removeHandler(h)
@@ -321,7 +378,7 @@ def check_ranks_agree(model, group):
                            'model' % differ)
 
 
-def _train(config, dirs, in_test, post_test, R_total, policy, device, pg):
+def _train(config, dirs, in_test, post_test, R_total, policy, device, pg, summaries=False):
     import torch
     from ..envs import make_env
     from .evaluator import Evaluator
@@ -344,25 +401,42 @@ def _train(config, dirs, in_test, post_test, R_total, policy, device, pg):
     if T % mc.getint('batch_size'):                                   # utils.py:121
         raise ValueError('episode length T = %d is not a multiple of batch_size = %d' % (T, mc.getint('batch_size')))
     group, own_group = host_group(pg) if pg is not None else (None, False)
+    writer = None
     try:
         model = build_model(agent, env, mc, total_step, R, policy=policy, seed=seed, device=device, replica0=replica0,
                             total_replicas=R_total, process_group=pg)
         sim = env._ensure_sim()
         trace = torch.zeros(T, R, dtype=torch.float32, device=sim.device)
+        summary, srec = None, {}
+        if summaries:
+            from .summary import SummaryWriter, summary_name
+            n_step = int(model.n_step)
+            if model.name == 'iql':
+                from .learner_iql import N_ROUNDS
+                shape = (-(-T // n_step), N_ROUNDS, model.n_agent, 4)
+            else:
+                shape = (T // n_step, 4)
+            srec = dict(summary_rec=torch.zeros(shape, dtype=torch.float32, device=sim.device))
+            if rank == 0:
+                writer = SummaryWriter(dirs['log'])
+                logging.info('Summaries: TensorBoard events into %s' % writer.path)
+            summary = Summaries(writer, summary_name(agent, policy, getattr(model, 'model_type', None)),
+                                'iql' if model.name == 'iql' else 'a2c', n_step)
         if model.name == 'iql':
             from .learner_iql import BatchedIQLTrainer
             from .models import iql_schedulers
             lr_s, eps_s = iql_schedulers(mc, total_step)
-            trainer = BatchedIQLTrainer(sim, model, lr_s, eps_s, seed0=seed, replica0=replica0, greward_trace=trace)
+            trainer = BatchedIQLTrainer(sim, model, lr_s, eps_s, seed0=seed, replica0=replica0, greward_trace=trace,
+                                        **srec)
         else:
             from .trainer import BatchedTrainer
             trainer = BatchedTrainer(sim, model.batched, agent, model.lr_scheduler, model.beta_scheduler, seed0=seed,
-                                     replica0=replica0, greward_trace=trace)
+                                     replica0=replica0, greward_trace=trace, **srec)
         evaluator = None
         if (in_test or post_test) and rank == 0:
             test_env = make_env(env_cfg, len(env.test_seeds), dirs['data'], is_record=False, device=device)
             evaluator = Evaluator(test_env, model, dirs['data'], policy_type='default')
-        driver = Trainer(trainer, evaluator, counter, agent, in_test, dirs['data'], group=group)
+        driver = Trainer(trainer, evaluator, counter, agent, in_test, dirs['data'], group=group, summary=summary)
         driver.run()
         final_step = counter.cur_step
         if group is not None:
@@ -373,6 +447,8 @@ def _train(config, dirs, in_test, post_test, R_total, policy, device, pg):
         post = driver.run_offline() if post_test else None
         torch.cuda.synchronize(sim.device)
     finally:
+        if writer is not None:
+            writer.close()
         if own_group:
             import torch.distributed as dist
             dist.destroy_process_group(group)

@@ -28,14 +28,26 @@ def _check_trace(trace, T_episode, sim):
     return trace
 
 
+def _check_rec(rec, shape, dev):
+    if rec is not None and (tuple(rec.shape) != tuple(shape) or rec.dtype != torch.float32 or rec.device != dev
+                            or not rec.is_contiguous()):
+        raise ValueError("summary_rec must be a contiguous float32 %s tensor on %s (got %s %s on %s)"
+                         % (list(shape), dev, tuple(rec.shape), rec.dtype, rec.device))
+    return rec
+
+
 class BatchedTrainer:
     def __init__(self, sim: BatchedSim, model: BatchedA2C, agent: str, lr, beta,
-                 seed0: int = 12, replica0: int = 0, greward_trace: Optional[torch.Tensor] = None):
+                 seed0: int = 12, replica0: int = 0, greward_trace: Optional[torch.Tensor] = None,
+                 summary_rec: Optional[torch.Tensor] = None):
         """lr / beta: floats (the 'constant' schedules of every shipped A2C config) or objects with the reference's
         `Scheduler.get(n_step)` (agents/utils.py:268-281, agents/models.py:175-176); a schedule advances by n_step per
         update exactly as in the reference (its unit is control steps of ONE environment).
         greward_trace: optional float32 [T_episode, R] device tensor; control_step() copies step t's global reward of
-        every replica into row t of the current episode.  None: no copy is issued."""
+        every replica into row t of the current episode.  None: no copy is issued.
+        summary_rec: optional float32 [T_episode / n_step, 4] device tensor; update j of the current episode copies
+        agent 0's (policy, value, entropy) loss terms (model.stats[:3]) and pre-clip gradient norm (model.norms[0]) into
+        row j with two device copies, so that the summaries of an episode need one read.  None: nothing is copied."""
         self.sim, self.model, self.agent = sim, model, agent
         self.lr, self.beta = lr, beta
         self.seed0, self.replica0 = int(seed0), int(replica0)
@@ -44,6 +56,8 @@ class BatchedTrainer:
         self.T_episode = int(np.ceil(sim.params.episode_length_sec / sim.params.control_interval_sec))
         assert self.T_episode % model.T == 0                      # utils.py:121
         self.greward_trace = _check_trace(greward_trace, self.T_episode, sim)
+        self.summary_rec = _check_rec(summary_rec, (self.T_episode // model.T, 4), sim.device)
+        self.summary_ran = np.ones(self.T_episode // model.T, bool)       # every A2C update runs
         self.step_in_episode = 0
         self.done = True
         self.episode_rewards = []
@@ -231,6 +245,10 @@ class BatchedTrainer:
         lr = self.lr.get(m.T) if hasattr(self.lr, "get") else self.lr
         beta = self.beta.get(m.T) if hasattr(self.beta, "get") else self.beta
         m.backward(boot, lr, beta)
+        if self.summary_rec is not None:
+            j = self.step_in_episode // m.T - 1
+            self.summary_rec[j, :3].copy_(m.stats[:3])
+            self.summary_rec[j, 3:].copy_(m.norms[:1])
         self.n_updates += 1
         if self.done:
             self.episode_rewards.append(float((self._rew_acc / self.T_episode).mean()))   # utils.py:296-305

@@ -57,7 +57,7 @@ struct tscl_qhandle {
   size_t td_smem = 0;            // 0: the TD kernel's layout does not fit a CTA (tscl_q_td refuses)
   int td_ctas_per_sm = 1;
   const int64_t* blk = nullptr;  // [A + 1] first float of every agent's block in the flat vector, then n_params
-  float* part = nullptr;         // TD partials [groups][n_params + A]
+  float* part = nullptr;         // TD partials [groups][n_params + 3 A]
 };
 
 struct QSmem {          // float offsets of the shared-memory regions
@@ -419,7 +419,9 @@ __device__ __forceinline__ void q_bgrad(const float* __restrict__ B, int n, floa
 // ring entries (slot idx[a][r][m % batch], replica r = m / batch).  tq = done ? r : r + gamma max_j q(s1)_j (no gradient,
 // same network), e = q(s)[act] - tq, loss = sum e^2 * inv_n, dq = 2 e inv_n.  grid (groups, A), 256 threads; CTA (g, a)
 // walks tiles g, g + groups, .. with agent a's weights resident, accumulates its weight gradients in shared memory, and
-// writes them at the agent's flat offsets into partial row g (part [groups][ld], loss at column n_params + a).
+// writes them at the agent's flat offsets into partial row g (part [groups][ld]); the tail columns n_params + a,
+// n_params + A + a and n_params + 2 A + a get inv_n times the CTA's sums of e^2, q(s)[act] and tq (the summaries of
+// QPolicy, agents/policies.py:331-338: loss, mean q, mean tq).
 template <bool DQN>
 __global__ void __launch_bounds__(256)
 q_td_kernel(const QDims d, const float* __restrict__ P, const float* __restrict__ ring_s,
@@ -461,7 +463,7 @@ q_td_kernel(const QDims d, const float* __restrict__ P, const float* __restrict_
   }
   for (int i = tid; i < QT_NA; i += 256) { sBq[i] = i < n_a ? P[d.off_q_b[a] + i] : 0.f; gBq[i] = 0.f; }
 
-  float loss = 0.f;                                   // threads < QT_ROWS: their rows' squared TD errors
+  float loss = 0.f, qsum = 0.f, tqsum = 0.f;          // threads < QT_ROWS: their rows' e^2, q(s)[act] and tq
   const int64_t rows = R * batch, n_tiles = (rows + QT_ROWS - 1) / QT_ROWS;
   const int32_t* ia = idx + (int64_t)a * rows;
   for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
@@ -501,8 +503,11 @@ q_td_kernel(const QDims d, const float* __restrict__ P, const float* __restrict_
         } else {
           float dq = 0.f;
           if (m < rows) {
-            const float e = __fsub_rn(sQ[tid * QT_NA + sAct[tid]], sTq[tid]);
+            const float q0 = sQ[tid * QT_NA + sAct[tid]];
+            const float e = __fsub_rn(q0, sTq[tid]);
             loss = fmaf(e, e, loss);
+            qsum += q0;
+            tqsum += sTq[tid];
             dq = 2.f * e * inv_n;
           }
           sDq[tid] = dq;
@@ -545,15 +550,23 @@ q_td_kernel(const QDims d, const float* __restrict__ P, const float* __restrict_
       q_bgrad(sH1, h1w, gB1, tid);
     }
   }
-  // the CTA's loss: fixed-order shuffle reduction over the 64 row threads
+  // the CTA's loss, q and tq sums: fixed-order shuffle reductions over the 64 row threads
   if (tid < QT_ROWS) {
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) loss += __shfl_down_sync(0xffffffffu, loss, o);
-    if ((tid & 31) == 0) sTq[tid >> 5] = loss;
+    for (int o = 16; o > 0; o >>= 1) {
+      loss += __shfl_down_sync(0xffffffffu, loss, o);
+      qsum += __shfl_down_sync(0xffffffffu, qsum, o);
+      tqsum += __shfl_down_sync(0xffffffffu, tqsum, o);
+    }
+    if ((tid & 31) == 0) { sTq[tid >> 5] = loss; sTq[2 + (tid >> 5)] = qsum; sTq[4 + (tid >> 5)] = tqsum; }
   }
   __syncthreads();
   float* out = part + (int64_t)blockIdx.x * ld;
-  if (tid == 0) out[n_params + a] = (sTq[0] + sTq[1]) * inv_n;
+  if (tid == 0) {
+    out[n_params + a] = (sTq[0] + sTq[1]) * inv_n;
+    out[n_params + d.A + a] = (sTq[2] + sTq[3]) * inv_n;
+    out[n_params + 2 * d.A + a] = (sTq[4] + sTq[5]) * inv_n;
+  }
   if (DQN) {
     for (int i = tid; i < n_wave * d.n_fc; i += 256) out[d.off_fcw_w[a] + i] = gW1[i];
     for (int i = tid; i < d.n_fc; i += 256) out[d.off_fcw_b[a] + i] = gB1[i];
@@ -579,11 +592,12 @@ __global__ void q_reduce_kernel(const float* __restrict__ part, int groups, int6
 }
 
 // Per agent (one CTA of 512 threads): tf.clip_by_global_norm and the TF1 Adam step of IQL.td_update
-// (agents/models.py:290-302) on the agent's block [blk[a], blk[a+1]) of the flat vector, loss / norm written out.
+// (agents/models.py:290-302) on the agent's block [blk[a], blk[a+1]) of the flat vector, loss / norm written out, and
+// with rec_out the agent's row (loss, mean q, mean tq, norm) of the round's summaries.
 __global__ void __launch_bounds__(512)
 q_adam_kernel(float* __restrict__ P, const float* __restrict__ grad, float* __restrict__ m, float* __restrict__ v,
-              const int64_t* __restrict__ blk, int64_t n_params, float lr_t, float max_norm, float* __restrict__ loss_out,
-              float* __restrict__ norm_out) {
+              const int64_t* __restrict__ blk, int64_t n_params, int A, float lr_t, float max_norm,
+              float* __restrict__ loss_out, float* __restrict__ norm_out, float* __restrict__ rec_out) {
   __shared__ float red[512];
   const int a = blockIdx.x, tid = threadIdx.x;
   const int64_t b0 = blk[a], b1 = blk[a + 1];
@@ -606,7 +620,14 @@ q_adam_kernel(float* __restrict__ P, const float* __restrict__ grad, float* __re
     v[i] = vi;
     P[i] = __fsub_rn(P[i], __fdiv_rn(__fmul_rn(lr_t, mi), __fadd_rn(__fsqrt_rn(vi), 1e-8f)));
   }
-  if (tid == 0) { loss_out[a] = grad[n_params + a]; norm_out[a] = norm; }
+  if (tid == 0) {
+    loss_out[a] = grad[n_params + a];
+    norm_out[a] = norm;
+    if (rec_out) {
+      float* r = rec_out + 4 * a;
+      r[0] = grad[n_params + a]; r[1] = grad[n_params + A + a]; r[2] = grad[n_params + 2 * A + a]; r[3] = norm;
+    }
+  }
 }
 
 // IQL.add_transition's reward (r / reward_norm, then clipped) and the post-step done into one replay slot, and the
@@ -797,7 +818,7 @@ extern "C" int tscl_q_td(tscl_qhandle* h, const float* params, const float* ring
     return tsc_set_error("tscl_q_td: the weights, gradients and tiles of one agent need more shared memory than a CTA has");
   LCK(cudaSetDevice(h->device));
   const int A = h->d.A;
-  const int64_t ld = h->n_params + A, n_tiles = (R * batch + QT_ROWS - 1) / QT_ROWS;
+  const int64_t ld = h->n_params + 3 * A, n_tiles = (R * batch + QT_ROWS - 1) / QT_ROWS;
   const int64_t max_groups = ((int64_t)h->n_sm * h->td_ctas_per_sm + A - 1) / A;
   int64_t groups = max_groups < n_tiles ? max_groups : n_tiles;
   if (!h->part) LCK(cudaMalloc(&h->part, (size_t)max_groups * ld * sizeof(float)));
@@ -817,11 +838,11 @@ extern "C" int tscl_q_td(tscl_qhandle* h, const float* params, const float* ring
 }
 
 extern "C" int tscl_q_adam(tscl_qhandle* h, float* params, const float* grad, float* adam_m, float* adam_v, float lr_t,
-                           float max_grad_norm, float* loss_out, float* norm_out, void* stream) {
+                           float max_grad_norm, float* loss_out, float* norm_out, float* rec_out, void* stream) {
   if (!h || !params || !grad || !adam_m || !adam_v || !loss_out || !norm_out) return tsc_set_error("tscl_q_adam: bad argument");
   LCK(cudaSetDevice(h->device));
-  q_adam_kernel<<<h->d.A, 512, 0, (cudaStream_t)stream>>>(params, grad, adam_m, adam_v, h->blk, h->n_params, lr_t,
-                                                          max_grad_norm, loss_out, norm_out);
+  q_adam_kernel<<<h->d.A, 512, 0, (cudaStream_t)stream>>>(params, grad, adam_m, adam_v, h->blk, h->n_params, h->d.A,
+                                                          lr_t, max_grad_norm, loss_out, norm_out, rec_out);
   LCK(cudaGetLastError());
   return 0;
 }

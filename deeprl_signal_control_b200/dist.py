@@ -3,7 +3,7 @@ simulation path has no collective; the learner all-reduces (SUM) its flat gradie
 after each rank scaled its local sum by 1 / (n_step * total_replicas).
 
 Used by the product path: `BatchedTrainer.start_episode` (episode_seeds), `BatchedA2C.backward` (grad_scale,
-allreduce_sum_), the training driver `agents/train.py` (replica_range, gather_traces) and bench.py (shard_replicas)."""
+allreduce_sum_), the training driver `agents/train.py` (replica_range, gather_traces, sum_partials) and bench.py (shard_replicas)."""
 from __future__ import annotations
 
 import numpy as np
@@ -33,6 +33,25 @@ def gather_traces(trace, group=None, dst: int = 0):
         if dist.get_rank(group) == dst else None
     dist.gather(t, parts, group=group, group_dst=dst)
     return None if parts is None else torch.cat(parts, 1).numpy()
+
+
+def sum_partials(x, group=None, dst: int = 0):
+    """Host-side sum over the ranks of `group` (gloo) of every rank's same-shape float array, to group rank `dst`:
+    gathered as float32, added in float64 in rank order.  Returns the float64 numpy sum on `dst`, None on every other
+    rank.  The training driver adds the A2C loss terms with it, each rank's being its partial sum already scaled by
+    1 / (n_step * R_total)."""
+    import torch
+    import torch.distributed as dist
+    t = torch.as_tensor(np.ascontiguousarray(x, dtype=np.float32))
+    parts = [torch.empty_like(t) for _ in range(dist.get_world_size(group))] \
+        if dist.get_rank(group) == dst else None
+    dist.gather(t, parts, group=group, group_dst=dst)
+    if parts is None:
+        return None
+    out = np.zeros(t.shape, np.float64)
+    for p in parts:
+        out += p.numpy()
+    return out
 
 
 def shard_replicas(rank: int, world: int, replicas_per_rank: int, seed0: int):

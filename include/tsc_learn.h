@@ -306,15 +306,17 @@ int tscl_q_explore(tscl_qhandle* h, const float* params, const float* obs, int64
 int tscl_q_sample(tscl_qhandle* h, int64_t R, int32_t batch, int32_t size, uint64_t seed, int64_t update, int32_t round,
                   int64_t replica0, int32_t* idx, void* stream);
 /* One round of the TD loss for all agents: the rows idx[a][r][*] of the ring (pointers to slot 0), tq = done ? r :
- * r + gamma max q(s1), loss = inv_n sum (q(s)[a] - tq)^2 over this rank's rows.  grad [n_params + A] receives the
- * weight gradients (flat layout) followed by the per-agent loss sums; reduced in a fixed order (bit-reproducible). */
+ * r + gamma max q(s1), loss = inv_n sum (q(s)[a] - tq)^2 over this rank's rows.  grad [n_params + 3 A] receives the
+ * weight gradients (flat layout) followed by three per-agent tails: the loss sums, inv_n sum q(s)[a] and inv_n sum tq;
+ * reduced in a fixed order (bit-reproducible).  Summed over ranks, the tails are the global means. */
 int tscl_q_td(tscl_qhandle* h, const float* params, const float* ring_s, const float* ring_s1, const int8_t* ring_a,
               const float* ring_r, const uint8_t* ring_done, const int32_t* idx, int64_t R, int32_t batch, float gamma,
               float inv_n, float* grad, void* stream);
 /* Per agent: tf.clip_by_global_norm(max_grad_norm) of grad and the TF1 Adam step (b1 0.9, b2 0.999, eps 1e-8) with
- * lr_t = lr sqrt(1 - b2^t) / (1 - b1^t); loss_out [A] = grad's loss sums, norm_out [A] = the pre-clip norms. */
+ * lr_t = lr sqrt(1 - b2^t) / (1 - b1^t); loss_out [A] = grad's loss sums, norm_out [A] = the pre-clip norms.
+ * rec_out (optional) [A][4]: per agent (loss, mean q, mean tq, pre-clip norm), the round's summaries. */
 int tscl_q_adam(tscl_qhandle* h, float* params, const float* grad, float* adam_m, float* adam_v, float lr_t,
-                float max_grad_norm, float* loss_out, float* norm_out, void* stream);
+                float max_grad_norm, float* loss_out, float* norm_out, float* rec_out, void* stream);
 /* IQL.add_transition's reward and done into one ring slot: ring_r [R][A] = clip(rew / reward_norm), ring_done [R] = done,
  * and rew_acc [R] += grew [R] (rew_acc may be NULL). */
 int tscl_q_transition(tscl_qhandle* h, const float* rew, int64_t R, float reward_norm, float reward_clip, float* ring_r,

@@ -3,6 +3,7 @@ device-resident learners (deeprl_signal_control_b200/agents/train.py).
 
   python scripts/train.py --base-dir DIR train --config-dir CFG.ini
                           [--test-mode no_test|in_train_test|after_train_test|all_test] [--replicas N] [--policy lstm|fc]
+                          [--summaries]
   torchrun --nproc-per-node W scripts/train.py --base-dir DIR train --config-dir CFG.ini --replicas N
                           [--backend nccl|gloo] ...
 
@@ -12,7 +13,9 @@ environment); the step counts control steps of the lock-step, so `total_step` gi
 run, each on N times the data.  DIR receives data/<config>.ini, data/train_reward.csv, model/checkpoint-<step>.npz and
 log/<time>.log, and with after_train_test / all_test the three evaluation CSVs in data/.  Name DIR after the agent
 and `scripts/evaluate.py --agent-dir DIR` evaluates the result.  Prints one JSON line: final step, episode sets, env
-samples (steps x replicas) and wall seconds.
+samples (steps x replicas) and wall seconds.  `--summaries` also writes the reference's TensorBoard event file into
+log/ (agent 0's per-update losses and gradient norm, train_reward, test_reward): `tensorboard --logdir DIR/log`, or
+`scripts/extract_summaries.py --log-dir DIR/log --scalar-name TAG` for a CSV.
 
 Under torchrun with W > 1 processes, the N replicas are split over the W ranks (W must divide N), one GPU per rank
 (LOCAL_RANK), and the learner all-reduces its gradient once per update over `--backend` (default nccl).  Rank 0 writes
@@ -42,6 +45,8 @@ def parse_args(argv=None):
     sp.add_argument("--config-dir", default="./config/config_test_large.ini", help="experiment config path")
     sp.add_argument("--replicas", type=int, default=1, help="lock-stepped environments in all ranks (default 1)")
     sp.add_argument("--policy", default="lstm", choices=["lstm", "fc"])
+    sp.add_argument("--summaries", action="store_true",
+                    help="also write the reference's TensorBoard event file into log/")
     sp.add_argument("--backend", default="nccl", choices=["nccl", "gloo"],
                     help="gradient all-reduce backend under torchrun (default nccl)")
     a = p.parse_args(argv)
@@ -56,7 +61,8 @@ def main(argv=None):
     world = int(os.environ.get("WORLD_SIZE", "1"))
     if world <= 1:
         from deeprl_signal_control_b200.agents.train import train
-        out = train(a.config_dir, a.base_dir, a.test_mode, n_replicas=a.replicas, policy=a.policy)
+        out = train(a.config_dir, a.base_dir, a.test_mode, n_replicas=a.replicas, policy=a.policy,
+                    summaries=a.summaries)
         print(json.dumps({"final_step": out.final_step, "episode_sets": out.episode_sets,
                           "env_samples": out.env_samples, "replicas": a.replicas, "wall_sec": round(out.wall_sec, 3)}))
         return out
@@ -71,7 +77,7 @@ def main(argv=None):
     try:
         from deeprl_signal_control_b200.agents.train import train
         out = train(a.config_dir, a.base_dir, a.test_mode, n_replicas=a.replicas, policy=a.policy, device=local_rank,
-                    process_group=dist.group.WORLD)
+                    process_group=dist.group.WORLD, summaries=a.summaries)
     finally:
         dist.destroy_process_group()
     if out.rank == 0:
