@@ -11,6 +11,14 @@ Device-side counterpart of reference agents/models.py (IA2C/MA2C) + agents/polic
 Replicas share the weights: the gradient is the mean over replicas (and over ranks: one
 `all_reduce(SUM)` of the flat gradient per update, then identical updates everywhere).
 
+Population (`seeds` with K > 1 entries): K independent members of the same agent, member k with its own weights
+(initialised from seeds[k]), RMSProp slot, gradient and packed images, on n_replicas replicas each; the rows
+k*n_replicas .. (k+1)*n_replicas - 1 of every per-replica array are member k's.  One grouped forward launch
+(tscl_policy_step_v2g) serves all members and samples member k with the key of its own one-member learner (seed
+seeds[k], replica index relative to the member), so each member trains what `BatchedA2C(seed=seeds[k])` trains alone.
+The update runs the one-member kernels chunk by chunk (a chunk never straddles two members) with the member's
+pointers, then one clip + RMSProp and one repack per member.  `member(k)` is a solo-model view of member k.
+
 Shipping path (`use_tc`, the default): every kernel is hand-written — the fused wgmma forward
 (csrc/tsc_policy_tc.cu: fc front end, gate GEMM, LSTM cell, heads, sampling, bf16 activation store), the wgmma
 update (BPTT with TMA operand copies, dX = dZ.Wx^T, LSTM and fc weight gradients) and the SIMT kernels of
@@ -23,7 +31,8 @@ from __future__ import annotations
 
 import ctypes as C
 import os
-from typing import Optional
+import types
+from typing import Optional, Sequence
 
 import numpy as np
 import torch
@@ -37,16 +46,43 @@ def _p(t):
     return None if t is None else C.c_void_p(t.data_ptr())
 
 
+def check_population(seeds, seed, n_replicas, chunk, process_group):
+    """The member seeds of a learner: [seed] without `seeds`, else the list, which must hold distinct seeds; with
+    more than one member, n_replicas (per member) must be a multiple of 64 (a forward tile never straddles two
+    members), the update chunk min(chunk, n_replicas) must divide it, and there is no process group."""
+    if seeds is None:
+        return [int(seed)]
+    seeds = [int(s) for s in seeds]
+    if not seeds:
+        raise ValueError("a population needs at least one seed")
+    if len(set(seeds)) != len(seeds):
+        raise ValueError("population seeds must be distinct (got %s)" % seeds)
+    if any(s < 0 or s >= 1 << 63 for s in seeds):
+        raise ValueError("population seeds must lie in [0, 2^63) (got %s)" % seeds)
+    if len(seeds) > 1:
+        R_m, rc = int(n_replicas), min(int(chunk), int(n_replicas))
+        if R_m <= 0 or R_m % 64:
+            raise ValueError("a population needs a multiple of 64 replicas per member (got %d)" % R_m)
+        if R_m % rc:
+            raise ValueError("the update chunk (%d) must divide the replicas per member (%d)" % (rc, R_m))
+        if process_group is not None:
+            raise ValueError("a population trains in one process: it takes no process group")
+    return seeds
+
+
 class BatchedA2C:
     def __init__(self, layout: PolicyLayout, n_replicas: int, n_step: int, gamma: float = 0.99,
                  v_coef: float = 0.5, max_grad_norm: float = 40.0, alpha: float = 0.99, eps: float = 1e-5,
                  reward_norm: float = 1.0, reward_clip: float = 0.0, seed: int = 0, device: int = 0,
                  chunk: int = 1024, replica0: int = 0, total_replicas: Optional[int] = None,
                  process_group=None, allow_tf32: bool = True, use_tc: bool = True,
-                 store_acts: Optional[bool] = None):
+                 store_acts: Optional[bool] = None, seeds: Optional[Sequence[int]] = None):
+        self.seeds = check_population(seeds, seed, n_replicas, chunk, process_group)
+        seed = self.seeds[0]                  # with `seeds`, a one-member population is the solo learner of seeds[0]
+        self.K, self.R_m = len(self.seeds), int(n_replicas)
         if not torch.cuda.is_available():
             raise RuntimeError("BatchedA2C needs a CUDA device (no CPU fallback exists)")
-        self.lay, self.R, self.T = layout, int(n_replicas), int(n_step)
+        self.lay, self.R, self.T = layout, self.K * int(n_replicas), int(n_step)
         self.gamma, self.v_coef, self.max_grad_norm = gamma, v_coef, max_grad_norm
         self.alpha, self.eps = alpha, eps
         self.reward_norm, self.reward_clip = reward_norm, reward_clip
@@ -55,7 +91,7 @@ class BatchedA2C:
         self.pg = process_group
         self.allow_tf32 = allow_tf32
         self.dev = torch.device("cuda", device)
-        self.chunk = min(int(chunk), self.R)
+        self.chunk = min(int(chunk), self.R_m if self.K > 1 else self.R)
         lib = _lib.lib()
         self._cd = layout.as_c()
         h = C.c_void_p()
@@ -63,13 +99,17 @@ class BatchedA2C:
         self._h = h
         L, R, T, U, A = layout, self.R, self.T, layout.U, layout.A
         f32 = dict(dtype=torch.float32, device=self.dev)
-        self.P = torch.from_numpy(layout.init_params(seed)).to(self.dev)
+        if self.K == 1:
+            self.P = torch.from_numpy(layout.init_params(seed)).to(self.dev)
+        else:                                                  # [K][n_params], member k from its own seed
+            self.P = torch.from_numpy(np.stack([layout.init_params(s) for s in self.seeds])).to(self.dev)
         self.G = torch.zeros_like(self.P)
         self.MS = torch.ones_like(self.P)                      # TF1 RMSProp slot "rms" starts at 1
         self.agent_of = torch.from_numpy(layout.agent_of).to(self.dev)
-        self.norms = torch.zeros(A, **f32)
-        self.stats = torch.zeros(4, **f32)
-        self.pv, self.gv = layout.views(self.P), layout.views(self.G)
+        self.norms = torch.zeros(A, **f32) if self.K == 1 else torch.zeros(self.K, A, **f32)
+        self.stats = torch.zeros(4, **f32) if self.K == 1 else torch.zeros(self.K, 4, **f32)
+        # parameter views of the fp32 twin path (K = 1 only)
+        self.pv, self.gv = (layout.views(self.P), layout.views(self.G)) if self.K == 1 else (None, None)
         # recurrent state: [U][R][h] each
         self.c_fw = torch.zeros(U, R, L.h, **f32); self.h_fw = torch.zeros(U, R, L.h, **f32)
         self.c_bw = torch.zeros_like(self.c_fw); self.h_bw = torch.zeros_like(self.h_fw)
@@ -104,10 +144,15 @@ class BatchedA2C:
         # fc front end on the tensor cores too; the v2 kernel is instantiated for the shipped fc widths (grid 224,
         # Monaco 192, IA2C 160), other widths take the v1 kernel
         self.tc_v2 = self.use_tc and L.dx in (160, 192, 224)
-        self.Wp = torch.zeros(U, ((L.dx + L.h) // 8) * 4 * L.h * 8 + 8 * L.dx * 8, dtype=torch.bfloat16,
+        if self.K > 1 and not self.tc_v2:
+            raise ValueError("a population needs the fused tensor-core forward (use_tc with fc width 160, 192 or 224; got "
+                             "use_tc=%s, dx=%d)" % (bool(use_tc), L.dx))
+        mdim = () if self.K == 1 else (self.K,)                # packed images per member
+        self.Wp = torch.zeros(*mdim, U, ((L.dx + L.h) // 8) * 4 * L.h * 8 + 8 * L.dx * 8, dtype=torch.bfloat16,
                               device=self.dev)
-        self.Wt = torch.zeros(U, 32, L.h, 8, dtype=torch.bfloat16, device=self.dev)    # Wh^T image for the BPTT MMA
-        self.Wxt = torch.zeros(U, 32, L.dx, 8, dtype=torch.bfloat16, device=self.dev)  # Wx^T image: dX fused into the BPTT
+        self.Wt = torch.zeros(*mdim, U, 32, L.h, 8, dtype=torch.bfloat16, device=self.dev)    # Wh^T image for the BPTT MMA
+        self.Wxt = torch.zeros(*mdim, U, 32, L.dx, 8, dtype=torch.bfloat16, device=self.dev)  # Wx^T image: dX fused into the BPTT
+        self.seeds_dev = torch.tensor(self.seeds, dtype=torch.int64, device=self.dev) if self.K > 1 else None
         # fusing dX into the BPTT step lengthens its serial per-step chain, so the default keeps dX as a separate
         # product; `dx_fused = True` selects the fused kernel (tests/test_update_bench_size_gpu.py: test_fused_dx_bptt,
         # test_whole_update_matches_chunked_reference)
@@ -122,6 +167,8 @@ class BatchedA2C:
         self.fc_bwd_tc = self.use_tc and layout.fc_bwd_tc_ok     # front-end weight gradients on the tensor cores
         self.wgrad_tc = self.use_tc and L.dx % 8 == 0 and L.dx <= 240   # LSTM weight gradients on the tensor cores
         self.fused_heads = True                                  # head weight gradients inside tscl_heads_loss
+        if self.K > 1 and not self.dx_fc_fused:
+            raise ValueError("a population needs dX fused into the fc weight-gradient kernel (unset TSC_DX_LIBRARY)")
         self.pack_weights()
         # bf16 activation store of the rollout's own forward pass (written by the v2 kernel): the update then
         # back-propagates through it instead of recomputing fc + gate GEMM + LSTM forward.
@@ -130,6 +177,9 @@ class BatchedA2C:
             free, _ = torch.cuda.mem_get_info(self.dev)
             store_acts = self.tc_v2 and need < 0.5 * free
         self.store_acts = bool(store_acts) and self.tc_v2 and (R % self.chunk == 0)
+        if self.K > 1 and not self.store_acts:
+            raise ValueError("a population back-propagates through the activation store, which does not fit: %.2f GB "
+                             "for %d x %d replicas" % (need / 1e9, self.K, self.R_m))
         self.st_x = self.st_g = self.st_c = self.st_h = None
         if self.store_acts:       # [R/chunk][U][T][chunk][w]: every update chunk is one contiguous block
             bf = dict(dtype=torch.bfloat16, device=self.dev)
@@ -149,10 +199,27 @@ class BatchedA2C:
         except Exception:
             pass
 
+    def member(self, k: int):
+        """Member k as a solo learner reads: its parameters P, RMSProp slot MS, packed image Wp, loss terms stats and
+        gradient norms norms (views into the stacked tensors, so they follow training), with the layout and handle."""
+        if self.K == 1:
+            return self
+        return types.SimpleNamespace(lay=self.lay, _h=self._h, dev=self.dev, use_tc=self.use_tc, tc_v2=self.tc_v2,
+                                     K=1, P=self.P[k], MS=self.MS[k], Wp=self.Wp[k], stats=self.stats[k],
+                                     norms=self.norms[k], seed=self.seeds[k])
+
     def _st(self):
         return C.c_void_p(torch.cuda.current_stream(self.dev).cuda_stream)
 
     def pack_weights(self):
+        if self.K > 1:
+            lib = _lib.lib()
+            for k in range(self.K):
+                _lib.check(lib.tscl_pack_weights(self._h, _p(self.P[k]), _p(self.Wp[k]), self._st()))
+                _lib.check(lib.tscl_pack_wht(self._h, _p(self.P[k]), _p(self.Wt[k]), self._st()))
+                _lib.check(lib.tscl_pack_wxt(self._h, _p(self.P[k]), _p(self.Wxt[k]), self._st()))
+            self.kernel_launches += 3 * self.K
+            return
         if self.use_tc:
             _lib.check(_lib.lib().tscl_pack_weights(self._h, _p(self.P), _p(self.Wp), self._st()))
             _lib.check(_lib.lib().tscl_pack_wht(self._h, _p(self.P), _p(self.Wt), self._st()))
@@ -181,6 +248,23 @@ class BatchedA2C:
         want_act = sample and commit
         to_hist = to_hist and self.use_tc and self.tc_v2 and want_act and self.t < self.T
         val_o, act_o = (self.val_hist[self.t], self.act_hist[self.t]) if to_hist else (self.val, self.act)
+        if self.K > 1:
+            c1, h1 = (self.c_fw, self.h_fw) if commit else (self.c_tmp, self.h_tmp)
+            store = commit and self.t < self.T
+            st = (_p(self.st_x), _p(self.st_g), _p(self.st_c), _p(self.st_h)) if store else (None,) * 4
+            _lib.check(lib.tscl_policy_step_v2g(
+                self._h, _p(self.P), C.c_int64(self.P.shape[1]), _p(self.Wp), C.c_int64(self.Wp[0].numel()), _p(obs),
+                C.c_int32(self.K), C.c_int64(self.R_m), _p(self.c_fw), _p(self.h_fw), _p(c1), _p(h1), _p(self.pi),
+                _p(val_o), _p(act_o) if want_act else None, C.c_int32(1 if done else 0), _p(self.seeds_dev),
+                C.c_int64(self.n_forward), *st, C.c_int32(self.t if store else 0), C.c_int32(self.T),
+                C.c_int64(self.chunk), self._st()))
+            if store:
+                self._acts_ok[self.t] = True
+            self.kernel_launches += 1
+            if commit:
+                self.n_forward += 1
+            self._hist_direct = to_hist
+            return self.pi, val_o, (act_o if want_act else None)
         if self.use_tc:
             c1, h1 = (self.c_fw, self.h_fw) if commit else (self.c_tmp, self.h_tmp)
             args = (self._h, _p(self.P), _p(self.Wp), _p(obs), C.c_int64(R), _p(self.c_fw), _p(self.h_fw), _p(c1),
@@ -226,6 +310,7 @@ class BatchedA2C:
         `stream`: raw CUDA stream handle (default: torch's current stream).  `to_hist`: actions / values go straight into
         the rollout slots act_hist[t] / val_hist[t] (what add_transition would copy there) and those views are returned."""
         assert self.use_tc and self.tc_v2, "forward_range needs the fused tensor-core forward"
+        assert self.K == 1, "forward_range serves one-member learners"
         L, R, A = self.lay, self.R, self.lay.A
         store = self.store_acts and t < self.T
         st = (_p(self.st_x), _p(self.st_g), _p(self.st_c), _p(self.st_h)) if store else (None,) * 4
@@ -347,8 +432,14 @@ class BatchedA2C:
         self.stats.zero_()
         scale = _dist.grad_scale(T, 1, self.total_replicas)       # local SUM x 1/(n_step * R_total); ranks add up
         use_store = self.store_acts and all(self._acts_ok)
+        if self.K > 1 and not use_store:
+            raise RuntimeError("a population update needs every step of the rollout in the activation store")
         n_obs = L.n_obs
+        P, G, Wt, Wxt, stats = self.P, self.G, self.Wt, self.Wxt, self.stats
         for r0 in range(0, R, self.chunk):
+            if self.K > 1:        # the member of this chunk: its weights, images, gradient and loss terms
+                k = r0 // self.R_m
+                P, G, Wt, Wxt, stats = self.P[k], self.G[k], self.Wt[k], self.Wxt[k], self.stats[k]
             rc = min(self.chunk, R - r0)
             M = T * rc
             ci = r0 // self.chunk
@@ -384,40 +475,40 @@ class BatchedA2C:
                                                  _p(dpre), C.c_int32(T), C.c_int64(rc), C.c_int64(R), C.c_int64(r0),
                                                  st()))
             else:
-                _lib.check(lib.tscl_fc_embed(self._h, _p(self.P), _p(obs0), C.c_int64(M), C.c_int64(rc),
+                _lib.check(lib.tscl_fc_embed(self._h, _p(P), _p(obs0), C.c_int64(M), C.c_int64(rc),
                                              C.c_int64(R * n_obs), _p(X), st()))
                 torch.baddbmm(self.pv["bl"].unsqueeze(1), X, self.pv["wx"], out=ZG)
-                _lib.check(lib.tscl_lstm_seq_fwd(self._h, _p(self.P), _p(ZG), _p(Cc), _p(H), _p(Hp), _p(self.c_bw),
+                _lib.check(lib.tscl_lstm_seq_fwd(self._h, _p(P), _p(ZG), _p(Cc), _p(H), _p(Hp), _p(self.c_bw),
                                                  _p(self.h_bw), None, None, _p(dpre), C.c_int32(T), C.c_int64(rc),
                                                  C.c_int64(R), C.c_int64(r0), st()))
             hb = _p(self.st_h[ci]) if use_store else None
-            _lib.check(lib.tscl_heads_loss(self._h, _p(self.P), None if all_tc else _p(H), _p(self.act_hist[0, r0:]),
+            _lib.check(lib.tscl_heads_loss(self._h, _p(P), None if all_tc else _p(H), _p(self.act_hist[0, r0:]),
                                            _p(self.Rs[0, r0:]), _p(self.Adv[0, r0:]), C.c_int64(M), C.c_int64(rc),
                                            C.c_int64(R * A), C.c_float(self.v_coef), C.c_float(beta), C.c_float(scale),
-                                           None if self.fused_heads else _p(dlog), _p(dH), _p(self.stats),
-                                           hb if all_tc else None, _p(self.G) if self.fused_heads else None, st()))
+                                           None if self.fused_heads else _p(dlog), _p(dH), _p(stats),
+                                           hb if all_tc else None, _p(G) if self.fused_heads else None, st()))
             if not self.fused_heads:
                 # head weight / bias gradients (plain batched GEMM + column sums)
                 self.gv["wo"].baddbmm_(H.transpose(1, 2), dlog)
                 self.gv["bo"].add_(dlog.sum(dim=1))
             if self.bwd_tc:
                 gb = (_p(self.st_g[ci]), _p(self.st_c[ci])) if use_store else (None, None)
-                _lib.check(lib.tscl_lstm_seq_bwd_tc_dx(self._h, _p(self.Wt), _p(ZG), _p(Cc), _p(dH), _p(self.c_bw),
+                _lib.check(lib.tscl_lstm_seq_bwd_tc_dx(self._h, _p(Wt), _p(ZG), _p(Cc), _p(dH), _p(self.c_bw),
                                                        _p(dpre), C.c_int32(T), C.c_int64(rc), C.c_int64(R), C.c_int64(r0),
-                                                       *gb, _p(dZb), _p(self.Wxt) if fuse_dx else None,
+                                                       *gb, _p(dZb), _p(Wxt) if fuse_dx else None,
                                                        _p(dXb) if fuse_dx else None, st()))
             else:
-                _lib.check(lib.tscl_lstm_seq_bwd(self._h, _p(self.P), _p(ZG), _p(Cc), _p(dH), _p(self.c_bw), _p(dpre),
+                _lib.check(lib.tscl_lstm_seq_bwd(self._h, _p(P), _p(ZG), _p(Cc), _p(dH), _p(self.c_bw), _p(dpre),
                                                  C.c_int32(T), C.c_int64(rc), C.c_int64(R), C.c_int64(r0), st()))
             dZ = ZG
             if self.wgrad_tc:
                 if use_store:
                     _lib.check(lib.tscl_wgrad_tc(self._h, _p(dZ), _p(dZb), None, _p(self.st_x[ci]), None, _p(self.st_h[ci]),
                                                  _p(self.h_bw), _p(dpre), C.c_int32(T), C.c_int64(rc), C.c_int64(R),
-                                                 C.c_int64(r0), _p(self.G), C.c_int32(0), st()))
+                                                 C.c_int64(r0), _p(G), C.c_int32(0), st()))
                 else:
                     _lib.check(lib.tscl_wgrad_tc(self._h, _p(dZ), None, _p(X), None, _p(Hp), None, None, None, C.c_int32(T),
-                                                 C.c_int64(rc), C.c_int64(R), C.c_int64(r0), _p(self.G), C.c_int32(0), st()))
+                                                 C.c_int64(rc), C.c_int64(R), C.c_int64(r0), _p(G), C.c_int32(0), st()))
             else:
                 self.gv["wx"].baddbmm_(X.transpose(1, 2), dZ)
                 self.gv["wh"].baddbmm_(Hp.transpose(1, 2), dZ)
@@ -426,10 +517,10 @@ class BatchedA2C:
             # warp-specialised wgmma kernel (tscl_dx_tc); a library GEMM only on the fp32 twin path, for dx > 224 and
             # under TSC_DX_LIBRARY=1 (A/B measurements)
             if fuse_fc:
-                _lib.check(lib.tscl_dx_fc_bwd_tc(self._h, _p(obs0), _p(self.st_x[ci]), _p(dZb), _p(self.Wxt), C.c_int64(M),
-                                                 C.c_int64(rc), C.c_int64(R * n_obs), _p(self.G), st()))
+                _lib.check(lib.tscl_dx_fc_bwd_tc(self._h, _p(obs0), _p(self.st_x[ci]), _p(dZb), _p(Wxt), C.c_int64(M),
+                                                 C.c_int64(rc), C.c_int64(R * n_obs), _p(G), st()))
             elif all_tc and not fuse_dx and self.dx_own:
-                _lib.check(lib.tscl_dx_tc(self._h, _p(dZb), _p(self.Wxt), _p(dXb), C.c_int64(M), st()))
+                _lib.check(lib.tscl_dx_tc(self._h, _p(dZb), _p(Wxt), _p(dXb), C.c_int64(M), st()))
             elif all_tc and not fuse_dx:
                 torch.bmm(dZb, self.wx_b.transpose(1, 2), out=dXb)
             elif not all_tc:
@@ -439,18 +530,20 @@ class BatchedA2C:
             elif self.fc_bwd_tc:
                 xb = _p(self.st_x[ci]) if use_store else None
                 _lib.check(lib.tscl_fc_bwd_tc(self._h, _p(obs0), None if all_tc else _p(X), xb, _p(dX), _p(dXb),
-                                              C.c_int64(M), C.c_int64(rc), C.c_int64(R * n_obs), _p(self.G), C.c_int32(0),
+                                              C.c_int64(M), C.c_int64(rc), C.c_int64(R * n_obs), _p(G), C.c_int32(0),
                                               st()))
             else:
                 _lib.check(lib.tscl_fc_bwd(self._h, _p(obs0), _p(X), _p(dX), C.c_int64(M), C.c_int64(rc),
-                                           C.c_int64(R * n_obs), _p(self.G), st()))
+                                           C.c_int64(R * n_obs), _p(G), st()))
             self.kernel_launches += 3 if fuse_fc else 4 if use_store else 5
         if self.pg is not None:
             _dist.allreduce_sum_(self.G, self.pg)
-        _lib.check(lib.tscl_clip_rmsprop(self._h, _p(self.P), _p(self.G), _p(self.MS), _p(self.agent_of),
-                                         C.c_float(self.max_grad_norm), C.c_float(lr), C.c_float(self.alpha),
-                                         C.c_float(self.eps), _p(self.norms), st()))
-        self.kernel_launches += 3
+        for k in range(self.K):
+            m = (lambda t_: t_) if self.K == 1 else (lambda t_: t_[k])
+            _lib.check(lib.tscl_clip_rmsprop(self._h, _p(m(self.P)), _p(m(self.G)), _p(m(self.MS)), _p(self.agent_of),
+                                             C.c_float(self.max_grad_norm), C.c_float(lr), C.c_float(self.alpha),
+                                             C.c_float(self.eps), _p(m(self.norms)), st()))
+            self.kernel_launches += 3
         self.pack_weights()
         # states_bw <- states_fw (agents/policies.py:153); next rollout starts at slot 0
         self.c_bw.copy_(self.c_fw); self.h_bw.copy_(self.h_fw)

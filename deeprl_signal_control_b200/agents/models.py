@@ -29,9 +29,16 @@ class IA2C:
     name = 'ia2c'
 
     def __init__(self, n_s_ls, n_a_ls, n_w_ls, total_step, model_config, seed=0, n_f_ls=None,
-                 n_replicas=1, device=0, obs_off=None, policy='lstm', **learner_kw):
+                 n_replicas=1, device=0, obs_off=None, policy='lstm', seeds=None, **learner_kw):
         """policy='lstm': LstmACPolicy / FPLstmACPolicy, what the reference builds (agents/models.py:40-51);
-        policy='fc': FcACPolicy (agents/policies.py:214-256), the FC variant of BASELINE config 2."""
+        policy='fc': FcACPolicy (agents/policies.py:214-256), the FC variant of BASELINE config 2.
+        seeds: a population of len(seeds) members, n_replicas each, member k initialised from seeds[k] (`BatchedA2C`;
+        LSTM policy only); `members()` gives each as a solo model."""
+        if seeds is not None and len(seeds) > 1 and policy == 'fc':
+            raise ValueError("a population trains the LSTM policy only (got policy='fc')")
+        if seeds is not None:
+            learner_kw['seeds'] = seeds
+            seed = int(seeds[0])
         self.n_agent = len(n_s_ls)
         self._pre_done = False
         self.reward_clip = model_config.getfloat('reward_clip')
@@ -130,6 +137,14 @@ class IA2C:
     def reset(self):
         self.batched.reset()
 
+    def members(self):
+        """One solo model per population member (itself without a population): name, layout, n_step and the member's
+        learner view as `batched`, for `save`, the `Evaluator` and the summaries."""
+        b = self.batched
+        if getattr(b, 'K', 1) == 1:
+            return [self]
+        return [A2CMember(self, b.member(k)) for k in range(b.K)]
+
     # ---- checkpoints: reference file-name convention and VARIABLE NAMES (agents/models.py:83-108, checkpoint.py) ---
     def save(self, model_dir, global_step):
         """`checkpoint-<step>.npz` keyed by the reference's TF variable names (`<policy>_<i>a/pi_fcw/w`, ...); the
@@ -172,6 +187,17 @@ class IA2C:
             return True
         logging.error('Can not find old checkpoint for %s' % model_dir)
         return False
+
+
+class A2CMember:
+    """Population member k of an IA2C / MA2C as a solo model: `batched` is the learner's member view."""
+
+    def __init__(self, model, batched):
+        self.name, self.policy, self.layout, self.n_agent = model.name, model.policy, model.layout, model.n_agent
+        self.n_s_ls, self.n_a_ls, self.n_step = model.n_s_ls, model.n_a_ls, model.n_step
+        self.batched = batched
+
+    save = IA2C.save
 
 
 class MA2C(IA2C):

@@ -183,15 +183,18 @@ class Trainer:
     `group`: None for one process; over W > 1 ranks a group that takes CPU tensors (gloo).  Every rank then runs the
     same schedule; rank 0 gathers the traces, holds the rows, runs the tests (only it has an evaluator) and writes the
     CSV, and all ranks meet at a barrier after each test.
-    `summary`: None, or the `Summaries` of the run (the trainer then keeps a `summary_rec`)."""
+    `summary`: None, or the `Summaries` of the run (the trainer then keeps a `summary_rec`).
+    `log_extra`: the `extra` of its log records (a population member's tag, see `train_population`).
+    `run_schedule` runs one schedule for several drivers that share a batched trainer and counter."""
 
     def __init__(self, trainer, evaluator, counter: Counter, agent: str, run_test: bool, output_path: str,
-                 group=None, summary=None):
+                 group=None, summary=None, log_extra=None):
         if trainer.greward_trace is None:
             raise ValueError('the driver needs the trainer to keep a greward_trace')
         self.trainer, self.evaluator, self.counter = trainer, evaluator, counter
         self.agent, self.run_test, self.output_path = agent, run_test, output_path
         self.group, self.summary = group, summary
+        self.log_extra = dict(log_extra or {})
         if group is None:
             self.rank0 = True
         else:
@@ -201,7 +204,7 @@ class Trainer:
         self.data = []
         self.n_episode_sets = 0
         if run_test and self.rank0:
-            logging.info('Testing: total test num: %d' % evaluator.test_num)
+            logging.info('Testing: total test num: %d' % evaluator.test_num, extra=self.log_extra)
 
     def _barrier(self):
         if self.group is not None:
@@ -216,35 +219,36 @@ class Trainer:
             for k in range(len(mean)):
                 self.data.append({'agent': self.agent, 'step': step, 'test_id': k, 'avg_reward': float(mean[k]),
                                   'std_reward': float(std[k])})
-            logging.info('Testing: global step %d, avg R: %.2f (%.2f s)' % (step, np.mean(mean), time.time() - t0))
+            logging.info('Testing: global step %d, avg R: %.2f (%.2f s)' % (step, np.mean(mean), time.time() - t0),
+                         extra=self.log_extra)
             if self.summary is not None:
                 self.summary.test_reward(float(np.mean(mean)), step)
         self._barrier()
 
     def run(self):
+        run_schedule([self])
+
+    def episode_set(self, prev, step):
+        """The training row (and the summaries) of the episode set that took the step from prev to step."""
         c = self.counter
-        while not c.should_stop():
-            if self.run_test and c.should_test():
-                self.test()
-            prev = c.cur_step
-            self.trainer.run(self.T)                                  # one episode of every replica
-            step = c.next(self.T)
-            self.n_episode_sets += 1
-            rec = self.summary.record(self.trainer, self.group) if self.summary is not None else None
-            if self.group is None:
-                rewards = np.asarray(self.trainer.greward_trace.cpu().numpy(), np.float64)
-                mean, std = float(self.trainer.episode_rewards[-1]), float(np.std(rewards))
-            else:
-                rewards = _dist.gather_traces(self.trainer.greward_trace.cpu(), self.group)
-                if rewards is None:
-                    continue
-                mean, std = training_row(rewards)
-            self.data.append({'agent': self.agent, 'step': step, 'test_id': -1, 'avg_reward': mean, 'std_reward': std})
-            if self.summary is not None:
-                self.summary.episode_set(rec, self.trainer.summary_ran, prev, step, mean)
-            if c.should_log(prev):
-                logging.info('Training: global step %d, episode set %d, avg R: %.2f, std R: %.2f'
-                             % (step, self.n_episode_sets, mean, std))
+        self.n_episode_sets += 1
+        rec = self.summary.record(self.trainer, self.group) if self.summary is not None else None
+        if self.group is None:
+            rewards = np.asarray(self.trainer.greward_trace.cpu().numpy(), np.float64)
+            mean, std = float(self.trainer.episode_rewards[-1]), float(np.std(rewards))
+        else:
+            rewards = _dist.gather_traces(self.trainer.greward_trace.cpu(), self.group)
+            if rewards is None:
+                return
+            mean, std = training_row(rewards)
+        self.data.append({'agent': self.agent, 'step': step, 'test_id': -1, 'avg_reward': mean, 'std_reward': std})
+        if self.summary is not None:
+            self.summary.episode_set(rec, self.trainer.summary_ran, prev, step, mean)
+        if c.should_log(prev):
+            logging.info('Training: global step %d, episode set %d, avg R: %.2f, std R: %.2f'
+                         % (step, self.n_episode_sets, mean, std), extra=self.log_extra)
+
+    def write_rows(self):
         if self.rank0:
             import pandas as pd
             pd.DataFrame(self.data).to_csv(self.output_path + 'train_reward.csv')
@@ -256,17 +260,37 @@ class Trainer:
         if self.rank0:
             self.evaluator.env.init_data(True, False, self.output_path)
             mean, std = self.evaluator.run()
-            logging.info('Offline testing: avg R: %.2f' % np.mean(mean))
+            logging.info('Offline testing: avg R: %.2f' % np.mean(mean), extra=self.log_extra)
             out = mean, std
         self._barrier()
         return out
 
 
+def run_schedule(drivers):
+    """utils.py:Trainer.run for drivers that share one batched trainer and counter (drivers[0]'s): the tests before an
+    episode set, one episode of every replica, then each driver's training row; finally each driver's CSV.  One driver
+    is `Trainer.run`; a population has one driver per member, each over its member's view of the trainer."""
+    d0 = drivers[0]
+    c = d0.counter
+    while not c.should_stop():
+        if d0.run_test and c.should_test():
+            for d in drivers:
+                d.test()
+        prev = c.cur_step
+        d0.trainer.run(d0.T)                                          # one episode of every replica
+        step = c.next(d0.T)
+        for d in drivers:
+            d.episode_set(prev, step)
+    for d in drivers:
+        d.write_rows()
+
+
 def build_model(agent, env, model_config, total_step, n_replicas, policy='lstm', seed=0, device=0, replica0=0,
-                total_replicas=None, process_group=None):
+                total_replicas=None, process_group=None, seeds=None):
     """main.py:110-121 on the batched learners: IA2C / MA2C wrappers (seed = ENV_CONFIG.seed) or BatchedIQL (seed 0).
     `n_replicas` are this rank's replicas, the global ones [replica0, replica0 + n_replicas) of `total_replicas`; the
-    learner all-reduces its gradient over `process_group` when one is given."""
+    learner all-reduces its gradient over `process_group` when one is given.  `seeds`: an A2C population, one member
+    per seed on n_replicas replicas each (`BatchedA2C`)."""
     kind, model_type = model_spec(agent)
     t = env._tables
     if kind != 'iql':
@@ -274,6 +298,8 @@ def build_model(agent, env, model_config, total_step, n_replicas, policy='lstm',
         kw = dict(seed=seed, n_replicas=n_replicas, obs_off=t.node_obs_off, policy=policy, device=device)
         if process_group is not None:
             kw.update(replica0=replica0, total_replicas=total_replicas, process_group=process_group)
+        if seeds is not None:
+            kw.update(seeds=seeds)
         if kind == 'ma2c':
             return MA2C(env.n_s_ls, env.n_a_ls, env.n_w_ls, env.n_f_ls, total_step, model_config, **kw)
         return IA2C(env.n_s_ls, env.n_a_ls, env.n_w_ls, total_step, model_config, **kw)
@@ -288,8 +314,28 @@ def build_model(agent, env, model_config, total_step, n_replicas, policy='lstm',
                       total_replicas=total_replicas, pg=process_group)
 
 
+def parse_seeds(text):
+    """'12,13,14' -> [12, 13, 14]: the member seeds of a population run (distinct non-negative integers)."""
+    try:
+        seeds = [int(x) for x in str(text).split(',') if x.strip()]
+    except ValueError:
+        raise ValueError('seeds must be comma-separated integers (got %r)' % (text,))
+    if not seeds:
+        raise ValueError('no seed in %r' % (text,))
+    if len(set(seeds)) != len(seeds):
+        raise ValueError('population seeds must be distinct (got %s)' % seeds)
+    if min(seeds) < 0:
+        raise ValueError('population seeds must be non-negative (got %s)' % seeds)
+    return seeds
+
+
+def member_dir(base_dir, seed, agent):
+    """The agent directory of the population member with `seed`: <base_dir>/seed<seed>/<agent>."""
+    return os.path.join(base_dir, 'seed%d' % int(seed), agent)
+
+
 def train(config, base_dir, test_mode='no_test', n_replicas=1, policy='lstm', device=0, process_group=None,
-          summaries=False):
+          summaries=False, seeds=None):
     """main.py train.  `config`: the path of a reference config (copied into data/) or a parsed ConfigParser (written
     to data/config.ini), with [ENV_CONFIG], [MODEL_CONFIG] and [TRAIN_CONFIG].  Returns a namespace with final_step,
     episode_sets, env_samples (= final_step * n_replicas), wall_sec, world, rank, data (the train_reward.csv rows),
@@ -307,7 +353,14 @@ def train(config, base_dir, test_mode='no_test', n_replicas=1, policy='lstm', de
     every test seed is played once in record mode and the three CSVs go into data/.
 
     `summaries`: also write the reference's TensorBoard event file into log/ (`Summaries`; rank 0 only).  Off by default:
-    the run then allocates, launches and writes nothing for it."""
+    the run then allocates, launches and writes nothing for it.
+
+    `seeds`: train a population instead, one member per seed, each on `n_replicas` replicas, in one process
+    (`train_population`).  Returns its namespace."""
+    if seeds is not None:
+        if process_group is not None:
+            raise ValueError('a population trains in one process: seeds and process_group exclude each other')
+        return train_population(config, base_dir, seeds, test_mode, n_replicas, policy, device, summaries)
     t0 = time.time()
     in_test, post_test = init_test_flag(test_mode)
     world, rank = 1, 0
@@ -378,6 +431,17 @@ def check_ranks_agree(model, group):
                            'model' % differ)
 
 
+def _schedule(config, env):
+    """(total_step, Counter, episode length T) of a run; T must be a multiple of batch_size (utils.py:121)."""
+    total_step = int(config.getfloat('TRAIN_CONFIG', 'total_step'))
+    counter = Counter(total_step, int(config.getfloat('TRAIN_CONFIG', 'test_interval')),
+                      int(config.getfloat('TRAIN_CONFIG', 'log_interval')))
+    T, n_step = int(env.T), config['MODEL_CONFIG'].getint('batch_size')
+    if T % n_step:
+        raise ValueError('episode length T = %d is not a multiple of batch_size = %d' % (T, n_step))
+    return total_step, counter, T
+
+
 def _train(config, dirs, in_test, post_test, R_total, policy, device, pg, summaries=False):
     import torch
     from ..envs import make_env
@@ -393,13 +457,8 @@ def _train(config, dirs, in_test, post_test, R_total, policy, device, pg, summar
     env = make_env(env_cfg, R, dirs['data'], is_record=False, device=device)
     logging.info('Training: s dim: %d, s dim ls: %r, a dim ls: %r, replicas: %d'
                  % (env.n_s, env.n_s_ls, env.n_a_ls, R_total) + (' over %d ranks' % world if world > 1 else ''))
-    total_step = int(config.getfloat('TRAIN_CONFIG', 'total_step'))
-    counter = Counter(total_step, int(config.getfloat('TRAIN_CONFIG', 'test_interval')),
-                      int(config.getfloat('TRAIN_CONFIG', 'log_interval')))
+    total_step, counter, T = _schedule(config, env)
     seed = env_cfg.getint('seed')
-    T = int(env.T)
-    if T % mc.getint('batch_size'):                                   # utils.py:121
-        raise ValueError('episode length T = %d is not a multiple of batch_size = %d' % (T, mc.getint('batch_size')))
     group, own_group = host_group(pg) if pg is not None else (None, False)
     writer = None
     try:
@@ -456,3 +515,109 @@ def _train(config, dirs, in_test, post_test, R_total, policy, device, pg, summar
                                  env_samples=final_step * R_total, world=world, rank=rank,
                                  data=driver.data if rank == 0 else None, post_test=post, model=model,
                                  trainer=trainer)
+
+
+def _member_filter(k):
+    """Log records of member k, and those of no member in particular, go to member k's log file."""
+    return lambda rec: getattr(rec, 'member', k) == k
+
+
+def train_population(config, base_dir, seeds, test_mode='no_test', n_replicas=1, policy='lstm', device=0,
+                     summaries=False):
+    """Train K = len(seeds) members of one A2C agent (ia2c / ma2c, LSTM policy) in one process, member k with
+    `[ENV_CONFIG] seed = seeds[k]` on `n_replicas` replicas (a multiple of 64).  One simulator launch and one grouped
+    policy forward per control step cover all K * n_replicas replicas (`BatchedA2C` with seeds); the update, the
+    optimiser step, the tests and every file are per member.  Member k trains what `train(config with seed seeds[k],
+    n_replicas=n_replicas)` trains alone, and its directory `member_dir(base_dir, seeds[k], agent)` holds what that
+    run leaves: data/ (the config with the member's seed, train_reward.csv, test CSVs), model/checkpoint-<step>.npz,
+    log/<time>.log and, with `summaries`, the member's event file.  Returns a namespace like train()'s with per-member
+    lists `dirs`, `data`, `post_test` and `members`."""
+    import copy
+    import torch
+    from ..envs import make_env
+    from .evaluator import Evaluator
+    from .learner import check_population
+    from .trainer import BatchedTrainer
+    t0 = time.time()
+    in_test, post_test = init_test_flag(test_mode)
+    seeds = parse_seeds(','.join(str(int(x)) for x in seeds)) if not isinstance(seeds, str) else parse_seeds(seeds)
+    if isinstance(config, configparser.ConfigParser):
+        name = 'config.ini'
+    else:
+        path, name, config = config, os.path.basename(config), configparser.ConfigParser()
+        if not config.read(path):
+            raise FileNotFoundError(path)
+    agent = config['ENV_CONFIG'].get('agent')
+    kind, _ = model_spec(agent)
+    if kind == 'iql':
+        raise ValueError("a population trains an A2C agent (ia2c or ma2c), not %r" % agent)
+    if policy != 'lstm':
+        raise ValueError("a population trains the LSTM policy only (got policy=%r)" % policy)
+    check_population(seeds, 0, n_replicas, 1024, None)               # before any directory or device work
+    K, R_m = len(seeds), int(n_replicas)
+    cfgs, dirs, handlers = [], [], []
+    fmt = logging.Formatter('%(asctime)s [%(levelname)s] %(message)s')
+    for k, s in enumerate(seeds):
+        cfg = copy.deepcopy(config)
+        cfg['ENV_CONFIG']['seed'] = str(s)
+        d = init_dir(member_dir(base_dir, s, agent))
+        with open(os.path.join(d['data'], name), 'w') as f:
+            cfg.write(f)
+        h = logging.FileHandler(os.path.join(d['log'], '%d.log' % time.time()))
+        h.setFormatter(fmt)
+        h.addFilter(_member_filter(k))
+        cfgs.append(cfg); dirs.append(d); handlers.append(h)
+    handlers.append(logging.StreamHandler())
+    handlers[-1].setFormatter(fmt)
+    root = logging.getLogger()
+    for h in handlers:
+        root.addHandler(h)
+    root.setLevel(logging.INFO)
+    writers = []
+    try:
+        env_cfg, mc = cfgs[0]['ENV_CONFIG'], cfgs[0]['MODEL_CONFIG']
+        env = make_env(env_cfg, K * R_m, dirs[0]['data'], is_record=False, device=device)
+        logging.info('Training: s dim: %d, s dim ls: %r, a dim ls: %r, population of %d seeds %s x %d replicas'
+                     % (env.n_s, env.n_s_ls, env.n_a_ls, K, seeds, R_m))
+        total_step, counter, T = _schedule(config, env)
+        model = build_model(agent, env, mc, total_step, R_m, seeds=seeds, device=device)
+        members = model.members()
+        sim = env._ensure_sim()
+        trace = torch.zeros(T, K * R_m, dtype=torch.float32, device=sim.device)
+        srec, summ = {}, None
+        if summaries:
+            from .summary import SummaryWriter, summary_name
+            shape = (T // model.n_step,) + ((K,) if K > 1 else ()) + (4,)
+            srec = dict(summary_rec=torch.zeros(shape, dtype=torch.float32, device=sim.device))
+            writers = [SummaryWriter(d['log']) for d in dirs]
+            summ = [Summaries(w, summary_name(agent, policy), 'a2c', model.n_step) for w in writers]
+        trainer = BatchedTrainer(sim, model.batched, agent, model.lr_scheduler, model.beta_scheduler,
+                                 seed0=seeds[0], greward_trace=trace, **srec)
+        drivers = []
+        for k in range(K):                  # one driver per member, over its view of the shared trainer
+            evaluator = None
+            if in_test or post_test:
+                test_env = make_env(cfgs[k]['ENV_CONFIG'], len(env.test_seeds), dirs[k]['data'], is_record=False,
+                                    device=device)
+                evaluator = Evaluator(test_env, members[k], dirs[k]['data'], policy_type='default')
+            drivers.append(Trainer(trainer.member(k), evaluator, counter, agent, in_test, dirs[k]['data'],
+                                   summary=summ[k] if summ else None, log_extra={'member': k}))
+        run_schedule(drivers)
+        post = [None] * K
+        for k, d in enumerate(drivers):
+            logging.info('Training: save final model at step %d ...' % counter.cur_step, extra=d.log_extra)
+            members[k].save(dirs[k]['model'], counter.cur_step)
+            if post_test:
+                post[k] = d.run_offline()
+        torch.cuda.synchronize(sim.device)
+    finally:
+        for w in writers:
+            w.close()
+        for h in handlers:
+            root.removeHandler(h)
+            h.close()
+    return types.SimpleNamespace(final_step=counter.cur_step, episode_sets=drivers[0].n_episode_sets,
+                                 env_samples=counter.cur_step * K * R_m, world=1, rank=0, seeds=seeds,
+                                 dirs=[member_dir(base_dir, s, agent) for s in seeds], data=[d.data for d in drivers],
+                                 post_test=post, model=model, members=members, trainer=trainer,
+                                 wall_sec=time.time() - t0)

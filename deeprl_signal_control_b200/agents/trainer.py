@@ -36,6 +36,41 @@ def _check_rec(rec, shape, dev):
     return rec
 
 
+def member_episode_seeds(seeds, episode: int, n_replicas: int) -> np.ndarray:
+    """Reset seeds of a population's K * n_replicas replicas for its `episode`-th episode: member k's block is what its
+    solo run draws, episode_seeds(seeds[k], episode, 0, n_replicas, n_replicas).  The simulator's random stream is keyed
+    by the reset seed and the simulated second only, so member k's replicas then play the solo run's episodes."""
+    return np.concatenate([_dist.episode_seeds(s, episode, 0, n_replicas, n_replicas) for s in seeds])
+
+
+class MemberTrainer:
+    """Population member k of a `BatchedTrainer` as the training driver reads a one-member trainer: its rows of the
+    reward trace, its episode means and its summary records.  run() steps the whole population."""
+
+    def __init__(self, trainer, k):
+        self._tr, self._k = trainer, int(k)
+        R_m = trainer.model.R_m
+        self._rows = slice(self._k * R_m, (self._k + 1) * R_m)
+        self.T_episode, self.summary_ran = trainer.T_episode, trainer.summary_ran
+
+    def run(self, n_control_steps: int):
+        self._tr.run(n_control_steps)
+
+    @property
+    def greward_trace(self):
+        tr = self._tr.greward_trace
+        return None if tr is None else tr[:, self._rows].contiguous()
+
+    @property
+    def episode_rewards(self):
+        return [e[self._k] for e in self._tr.episode_rewards]
+
+    @property
+    def summary_rec(self):
+        rec = self._tr.summary_rec
+        return None if rec is None else rec[:, self._k]
+
+
 class BatchedTrainer:
     def __init__(self, sim: BatchedSim, model: BatchedA2C, agent: str, lr, beta,
                  seed0: int = 12, replica0: int = 0, greward_trace: Optional[torch.Tensor] = None,
@@ -47,16 +82,21 @@ class BatchedTrainer:
         every replica into row t of the current episode.  None: no copy is issued.
         summary_rec: optional float32 [T_episode / n_step, 4] device tensor; update j of the current episode copies
         agent 0's (policy, value, entropy) loss terms (model.stats[:3]) and pre-clip gradient norm (model.norms[0]) into
-        row j with two device copies, so that the summaries of an episode need one read.  None: nothing is copied."""
+        row j with two device copies, so that the summaries of an episode need one read.  None: nothing is copied.
+        A population learner (model.K > 1 members of model.R_m replicas) resets member k's replicas with its own seeds
+        (`member_episode_seeds`; seed0 and replica0 are not used), keeps [T_episode / n_step, K, 4] records and appends
+        the list of the K members' episode means to `episode_rewards`."""
         self.sim, self.model, self.agent = sim, model, agent
         self.lr, self.beta = lr, beta
         self.seed0, self.replica0 = int(seed0), int(replica0)
         self.total_replicas = int(getattr(model, "total_replicas", sim.R))
+        self.K = int(getattr(model, "K", 1))
         self.episode = 0
         self.T_episode = int(np.ceil(sim.params.episode_length_sec / sim.params.control_interval_sec))
         assert self.T_episode % model.T == 0                      # utils.py:121
         self.greward_trace = _check_trace(greward_trace, self.T_episode, sim)
-        self.summary_rec = _check_rec(summary_rec, (self.T_episode // model.T, 4), sim.device)
+        self.summary_rec = _check_rec(summary_rec, (self.T_episode // model.T,) + ((self.K,) if self.K > 1 else ()) + (4,),
+                                      sim.device)
         self.summary_ran = np.ones(self.T_episode // model.T, bool)       # every A2C update runs
         self.step_in_episode = 0
         self.done = True
@@ -69,10 +109,17 @@ class BatchedTrainer:
         self.update_events = None     # same around update() (bootstrap forward + backward)
         self.start_episode()
 
+    def member(self, k: int):
+        """Population member k's view of this trainer (the trainer itself without a population)."""
+        return self if self.K == 1 else MemberTrainer(self, k)
+
     def start_episode(self):
         sim, m = self.sim, self.model
         # envs/env.py:560 (seed += 1 per episode and environment): disjoint over all (rank, episode) pairs
-        seeds = _dist.episode_seeds(self.seed0, self.episode, self.replica0, sim.R, max(self.total_replicas, sim.R))
+        if self.K > 1:
+            seeds = member_episode_seeds(m.seeds, self.episode, m.R_m)
+        else:
+            seeds = _dist.episode_seeds(self.seed0, self.episode, self.replica0, sim.R, max(self.total_replicas, sim.R))
         self.episode += 1
         sim.reset(seeds)
         sim.set_train_mode(True)
@@ -247,10 +294,15 @@ class BatchedTrainer:
         m.backward(boot, lr, beta)
         if self.summary_rec is not None:
             j = self.step_in_episode // m.T - 1
-            self.summary_rec[j, :3].copy_(m.stats[:3])
-            self.summary_rec[j, 3:].copy_(m.norms[:1])
+            self.summary_rec[j, ..., :3].copy_(m.stats[..., :3])
+            self.summary_rec[j, ..., 3:].copy_(m.norms[..., :1])
         self.n_updates += 1
-        if self.done:
+        if self.done and self.K > 1:
+            R_m = m.R_m
+            self.episode_rewards.append([float((self._rew_acc[k * R_m:(k + 1) * R_m] / self.T_episode).mean())
+                                         for k in range(self.K)])
+            self.start_episode()
+        elif self.done:
             self.episode_rewards.append(float((self._rew_acc / self.T_episode).mean()))   # utils.py:296-305
             self.start_episode()
 

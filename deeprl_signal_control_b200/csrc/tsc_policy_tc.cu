@@ -301,6 +301,10 @@ struct StepTC {
   int64_t ld, row0;
   unsigned long long* prof;   // optional: per-phase clock64 sums of thread 0 of every CTA (tools/profile only)
   int act_mode;               // pi-only instantiation: 0 = counter-RNG sample, 1 = first argmax of pi
+  // grouped (population) instantiation: K members of Rm rows each; member k's parameters and bf16 image start at
+  // P + k p_stride and Wp + k wp_stride, and it samples with seeds[k] (device array) and replica index r - k Rm
+  int64_t Rm, p_stride, wp_stride;
+  const uint64_t* seeds;
 };
 
 extern __shared__ __align__(1024) unsigned char tc_smem[];
@@ -644,7 +648,11 @@ __host__ __device__ inline int gate_col(int n) {
 // n_tiles * A of them; V units are never loaded, multiplied or stored.  The recurrent state is compact, [A][ld][h] (row
 // (u >> 1) * ld + r); there is no activation store, no zdbg and no value output.  Per element the arithmetic is the
 // training instantiation's, so pi, c and h are bit-identical to its pi units.
-template <int DX, bool PROF, bool EVAL>
+// GRP: the population forward (tscl_policy_step_v2g).  Rows are K members of a.Rm (a multiple of 64) each; work items
+// are (member, unit, tile), so one member's [Wx;Wh] image stays resident over its tiles, and a block of items never
+// spans two members.  Member k reads its parameters and image at stride offsets and samples with the key
+// (seeds[k], step, replica0 + r - k Rm) of its own one-member launch; per element the arithmetic is unchanged.
+template <int DX, bool PROF, bool EVAL, bool GRP = false>
 __global__ void __launch_bounds__(P2_THREADS, 1)
 policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
   const int tid = threadIdx.x, wg = tid >> 7, lane = tid & 31;
@@ -656,6 +664,9 @@ policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
   float* sBias = sBo + 8;                                                    // [256]  lstm bias
   float* sBias0 = sBias + TC_N;                                              // [256]  fc biases
   uint64_t* sBar = reinterpret_cast<uint64_t*>(sBias0 + TC_N);               // full[2], empty[2]
+  // GRP only (16 more bytes): the block's row offset rofs (int64), the member's sampling key and the low word of its
+  // first row, kept in shared memory rather than in the consumers' full register budget
+  int64_t* sGrp = reinterpret_cast<int64_t*>(sBar + 4);
   const uint32_t aB = smem_u32(sB);
   if (tid == 0) {
     for (int s = 0; s < 2; ++s) {
@@ -679,25 +690,32 @@ policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
 
   // the constants of unit u, written by the 256 consumer threads between two CTA barriers that every role passes (all
   // roles have retired the previous unit); the producer, with its small register budget, only takes the barriers
-  auto load_unit = [&](int u, bool consumer) {
+  auto load_unit = [&](int u, int mk, int64_t rofs, bool consumer) {
     __syncthreads();
     if (consumer) {
       const int t = tid - 128;
-      const uint4* src = reinterpret_cast<const uint4*>(a.Wp + (int64_t)u * wp_stride(DX));
+      if (GRP && t == 0) {
+        const uint64_t sk = a.seeds[mk];
+        sGrp[0] = rofs;
+        reinterpret_cast<uint32_t*>(sGrp)[2] = pmix32((uint32_t)sk ^ (a.step * 0x9E3779B1U)) ^ (uint32_t)(sk >> 32);
+        reinterpret_cast<uint32_t*>(sGrp)[3] = (uint32_t)((int64_t)mk * a.Rm);
+      }
+      const float* P = GRP ? a.P + (int64_t)mk * a.p_stride : a.P;
+      const uint4* src = reinterpret_cast<const uint4*>((GRP ? a.Wp + (int64_t)mk * a.wp_stride : a.Wp) + (int64_t)u * wp_stride(DX));
       uint4* dst = reinterpret_cast<uint4*>(sB);
 #pragma unroll 4
       for (int i = t; i < KC * TC_N; i += 256) dst[i] = src[(i & ~(TC_N - 1)) + gate_col(i & (TC_N - 1))];
       for (int i = t; i < TC_H * 8; i += 256) {
         const int k = i >> 3, j = i & 7;
-        sWo[i] = j < d.max_na ? a.P[d.off_wo + ((int64_t)u * TC_H + k) * d.max_na + j] : 0.f;
+        sWo[i] = j < d.max_na ? P[d.off_wo + ((int64_t)u * TC_H + k) * d.max_na + j] : 0.f;
       }
-      if (t < 8) sBo[t] = t < d.max_na ? a.P[d.off_bo + (int64_t)u * d.max_na + t] : 0.f;
+      if (t < 8) sBo[t] = t < d.max_na ? P[d.off_bo + (int64_t)u * d.max_na + t] : 0.f;
       for (int i = t; i < TC_N; i += 256) {
-        sBias[i] = a.P[d.off_bl + (int64_t)u * TC_N + i];
+        sBias[i] = P[d.off_bl + (int64_t)u * TC_N + i];
         float b0 = 0.f;
-        if (i < d.fw) b0 = a.P[d.off_fcw_b[u] + i];
-        else if (i < d.fw + d.ff) b0 = a.P[d.off_fcf_b[u] + (i - d.fw)];
-        else if (i < d.dx) b0 = a.P[d.off_fct_b[u] + (i - d.fw - d.ff)];
+        if (i < d.fw) b0 = P[d.off_fcw_b[u] + i];
+        else if (i < d.fw + d.ff) b0 = P[d.off_fcf_b[u] + (i - d.fw)];
+        else if (i < d.dx) b0 = P[d.off_fct_b[u] + (i - d.fw - d.ff)];
         sBias0[i] = b0;
       }
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");      // the B image is read by wgmma
@@ -711,9 +729,12 @@ policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
     const int warp = tid >> 5;
     uint32_t ph_empty = 0;
     for (int64_t seg = it_lo; seg < it_hi;) {
-      const int ui = (int)(seg / n_tiles), u = EVAL ? 2 * ui : ui, ag = u >> 1;   // ui: item block = state unit
-      const int64_t seg_hi = (int64_t)(ui + 1) * n_tiles < it_hi ? (int64_t)(ui + 1) * n_tiles : it_hi;
-      load_unit(u, false);
+      // GRP: item block blk = (member mk, unit ui) of bt tiles; items (item counts < 2^31) in 32-bit arithmetic
+      const int bt = GRP ? (int)(a.Rm / P2_ROWS) : 1, blk = GRP ? (int)seg / bt : 0, mk = GRP ? blk / (2 * d.A) : 0;
+      const int ui = GRP ? blk - mk * 2 * d.A : (int)(seg / n_tiles), u = EVAL ? 2 * ui : ui, ag = u >> 1;   // ui: item block = state unit
+      const int64_t seg_hi = GRP ? ((int64_t)(blk + 1) * bt < it_hi ? (int64_t)(blk + 1) * bt : it_hi)
+                                 : ((int64_t)(ui + 1) * n_tiles < it_hi ? (int64_t)(ui + 1) * n_tiles : it_hi);
+      load_unit(u, mk, GRP ? (int64_t)mk * a.Rm - (int64_t)blk * bt * P2_ROWS : 0, false);
       PROF_MARK(8);      // producer: unit constants
       const int nw = d.n_wave[ag], nt = d.n_wait[ag], nf = d.ff > 0 ? d.n_fp[ag] : 0, ooff = d.obs_off[ag];
       // observation index of this lane's two input slots 2 lane, 2 lane + 1 (-1: unused slot)
@@ -723,10 +744,10 @@ policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
         return c - d.kw - TC_KF < nt ? nw + (c - d.kw - TC_KF) : -1;
       };
       const int src_a = slot_src(2 * lane), src_b = slot_src(2 * lane + 1);
-      const __nv_bfloat16* Wfc = a.Wp + (int64_t)u * wp_stride(DX) + (int64_t)KC * TC_N * 8;
+      const __nv_bfloat16* Wfc = (GRP ? a.Wp + (int64_t)mk * a.wp_stride : a.Wp) + (int64_t)u * wp_stride(DX) + (int64_t)KC * TC_N * 8;
       for (int64_t it = seg; it < seg_hi; ++it) {
         const int s = (int)((it - it_lo) & 1);
-        const int64_t r0 = (it - (int64_t)ui * n_tiles) * P2_ROWS;
+        const int64_t r0 = GRP ? sGrp[0] + it * P2_ROWS : (it - (int64_t)ui * n_tiles) * P2_ROWS;
         unsigned char* sA = sA0 + (size_t)s * KC * 1024;
         const uint32_t full = smem_u32(sBar + s), empty = smem_u32(sBar + 2 + s);
         mbar_wait(empty, ((ph_empty >> s) & 1) ^ 1);       // the tile's previous item has left it (first use: passes)
@@ -737,9 +758,17 @@ policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
           mbar_expect_tx(full, (uint32_t)(8 * DX * 16));
           bulk_g2s(smem_u32(sA), Wfc, (uint32_t)(8 * DX * 16), full);
         }
-        if (it + 2 < it_hi) {      // L2 prefetch of the state rows and observations of the next item of this tile
-          const int un = (int)((it + 2) / n_tiles);
-          const int64_t rn = ((it + 2) - (int64_t)un * n_tiles) * P2_ROWS + (tid & 63);
+        // L2 prefetch of the state rows and observations of the next item of this tile (GRP: within the block only)
+        if (GRP ? it + 2 < seg_hi : it + 2 < it_hi) {
+          int un;
+          int64_t rn;
+          if (GRP) {
+            un = ui;
+            rn = r0 + 2 * P2_ROWS + (tid & 63);
+          } else {
+            un = (int)((it + 2) / n_tiles);
+            rn = ((it + 2) - (int64_t)un * n_tiles) * P2_ROWS + (tid & 63);
+          }
           if (rn < a.R) {
             const int64_t so = ((int64_t)un * ld + rn) * TC_H + (tid >> 6) * 32;
             asm volatile("prefetch.global.L2 [%0];" ::"l"(a.c_in + so));
@@ -781,13 +810,15 @@ policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
     const uint32_t aA = smem_u32(sA), full = smem_u32(sBar + c), empty = smem_u32(sBar + 2 + c);
     uint32_t ph_full = 0;
     for (int64_t seg = it_lo; seg < it_hi;) {
-      const int ui = (int)(seg / n_tiles), u = EVAL ? 2 * ui : ui, ag = u >> 1;   // ui: item block = state unit
-      const int64_t seg_hi = (int64_t)(ui + 1) * n_tiles < it_hi ? (int64_t)(ui + 1) * n_tiles : it_hi;
-      load_unit(u, true);
+      const int bt = GRP ? (int)(a.Rm / P2_ROWS) : 1, blk = GRP ? (int)seg / bt : 0, mk = GRP ? blk / (2 * d.A) : 0;
+      const int ui = GRP ? blk - mk * 2 * d.A : (int)(seg / n_tiles), u = EVAL ? 2 * ui : ui, ag = u >> 1;   // ui: item block = state unit
+      const int64_t seg_hi = GRP ? ((int64_t)(blk + 1) * bt < it_hi ? (int64_t)(blk + 1) * bt : it_hi)
+                                 : ((int64_t)(ui + 1) * n_tiles < it_hi ? (int64_t)(ui + 1) * n_tiles : it_hi);
+      load_unit(u, mk, GRP ? (int64_t)mk * a.Rm - (int64_t)blk * bt * P2_ROWS : 0, true);
       PROF_MARK(0);      // unit constants
       const int na = d.n_a[ag];
       for (int64_t it = seg + (((seg - it_lo) & 1) != c ? 1 : 0); it < seg_hi; it += 2) {
-        const int64_t r0 = (it - (int64_t)ui * n_tiles) * P2_ROWS;
+        const int64_t r0 = GRP ? sGrp[0] + it * P2_ROWS : (it - (int64_t)ui * n_tiles) * P2_ROWS;
         // row of the activation store (chunk-outermost [R/rc][2A][T][rc][w]) for tile row `row`
         const int64_t st_c0 = (a.row0 + r0) / a.rc, st_rin0 = (a.row0 + r0) - st_c0 * a.rc;
         auto store_row = [&](int row) -> int64_t {
@@ -975,8 +1006,16 @@ policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
                   if (j < na && lg[j] * inv > best) { best = lg[j] * inv; pick = j; }
                 a.act[(int64_t)r * d.A + ag] = pick;
               } else if (a.act) {
-                uint32_t hsh = pmix32(a.seed_lo ^ (a.step * 0x9E3779B1U));
-                hsh = pmix32(hsh ^ a.seed_hi ^ ((uint32_t)(a.replica0 + r) * 0x85EBCA77U));
+                uint32_t hsh;
+                if (GRP) {
+                  // the member's key up to the replica term (xor is associative: the bits of the step-wise hash),
+                  // and its replica index r - k Rm, of which the uint32 key sees the low word only
+                  const uint32_t* g32 = reinterpret_cast<const uint32_t*>(sGrp);
+                  hsh = pmix32(g32[2] ^ (((uint32_t)r - g32[3]) * 0x85EBCA77U));
+                } else {
+                  hsh = pmix32(a.seed_lo ^ (a.step * 0x9E3779B1U));
+                  hsh = pmix32(hsh ^ a.seed_hi ^ ((uint32_t)(a.replica0 + r) * 0x85EBCA77U));
+                }
                 hsh = pmix32(hsh ^ ((uint32_t)ag * 0xC2B2AE3DU));
                 const float uu = (float)(hsh >> 8) * (1.0f / 16777216.0f);
                 float cum = 0.f;
@@ -1062,6 +1101,52 @@ extern "C" int tscl_policy_step_v2(tscl_handle* h, const float* params, const vo
                                    void* stream) {
   return tscl_policy_step_v2r(h, params, wpack_bf16, obs, R, c_in, h_in, c_out, h_out, pi, val, act, done, seed, step, replica0,
                               zdbg, st_x, st_g, st_c, st_h, t, T, rc, 0, 0, stream);
+}
+
+extern "C" int tscl_policy_step_v2g(tscl_handle* h, const float* params, int64_t p_stride, const void* wpack_bf16,
+                                   int64_t wp_stride_m, const float* obs, int32_t K, int64_t Rm, const float* c_in,
+                                   const float* h_in, float* c_out, float* h_out, float* pi, float* val, int32_t* act,
+                                   int32_t done, const uint64_t* seeds, int64_t step, void* st_x, void* st_g, void* st_c,
+                                   void* st_h, int32_t t, int32_t T, int64_t rc, void* stream) {
+  if (!h || !params || !wpack_bf16 || !obs || !seeds || K < 1 || Rm <= 0) return tsc_set_error("tscl_policy_step_v2g: bad argument");
+  if (Rm % P2_ROWS != 0) return tsc_set_error("tscl_policy_step_v2g: the member replica count must be a multiple of 64");
+  if (st_x && (rc <= 0 || Rm % rc != 0)) return tsc_set_error("tscl_policy_step_v2g: store chunk must divide the member replica count");
+  PCK(cudaSetDevice(tscl_device_of(h)));
+  const DDimsTC& d = *tscl_dims_of(h);
+  if (!P2_DX_OK(d.dx)) return tsc_set_error("tscl_policy_step_v2g: no kernel for this dx (160, 192 or 224)");
+  if (d.kw == 0) return tsc_set_error("tscl_policy_step_v2g: observation slice does not fit the 64-column input tile");
+  if (K > 1 && (p_stride < d.n_params || wp_stride_m < 2 * d.A * wp_stride(d.dx)))
+    return tsc_set_error("tscl_policy_step_v2g: member strides smaller than one member's parameters / image");
+  const size_t smem = tc2_smem_bytes(d.dx + TC_H) + 16;      // + the block constants (sGrp)
+  if (smem > 232448) return tsc_set_error("tscl_policy_step_v2g: operand tiles exceed shared memory");
+  void (*kern)(const DDimsTC, const StepTC) = nullptr;
+  switch (d.dx) {
+    case 160: kern = policy_step_tc2_kernel<160, false, false, true>; break;
+    case 192: kern = policy_step_tc2_kernel<192, false, false, true>; break;
+    case 224: kern = policy_step_tc2_kernel<224, false, false, true>; break;
+  }
+  static int attr_dev = -1;
+  static void (*attr_kern)(const DDimsTC, const StepTC) = nullptr;
+  if (attr_dev != tscl_device_of(h) || attr_kern != kern) {
+    PCK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 232448));
+    attr_dev = tscl_device_of(h); attr_kern = kern;
+  }
+  int n_sm = 0;
+  PCK(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, tscl_device_of(h)));
+  const int64_t R = (int64_t)K * Rm;
+  const int64_t n_items = (R / P2_ROWS) * 2 * d.A;
+  if (n_items > INT32_MAX) return tsc_set_error("tscl_policy_step_v2g: more than 2^31 work items");
+  const int grid = (int)(n_items < n_sm ? n_items : n_sm);
+  StepTC a{};
+  a.P = params; a.Wp = (const __nv_bfloat16*)wpack_bf16; a.obs = obs; a.c_in = c_in; a.h_in = h_in; a.c_out = c_out;
+  a.h_out = h_out; a.pi = pi; a.val = val; a.act = act; a.R = R; a.done = done;
+  a.step = (uint32_t)step; a.replica0 = 0;
+  a.st_x = (__nv_bfloat16*)st_x; a.st_g = (__nv_bfloat16*)st_g; a.st_c = (__nv_bfloat16*)st_c; a.st_h = (__nv_bfloat16*)st_h;
+  a.t = t; a.T = T > 0 ? T : 1; a.rc = rc > 0 ? rc : Rm; a.ld = 0; a.row0 = 0;
+  a.Rm = Rm; a.p_stride = p_stride; a.wp_stride = wp_stride_m; a.seeds = seeds;
+  kern<<<grid, P2_THREADS, smem, (cudaStream_t)stream>>>(d, a);
+  PCK(cudaGetLastError());
+  return 0;
 }
 
 extern "C" int tscl_policy_step_pi(tscl_handle* h, const float* params, const void* wpack_bf16, const float* obs, int64_t R,

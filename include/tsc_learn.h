@@ -229,6 +229,18 @@ int tscl_policy_step_v2r(tscl_handle* h, const float* params, const void* wpack_
                          int32_t* act, int32_t done, uint64_t seed, int64_t step, int64_t replica0, float* zdbg,
                          void* st_x, void* st_g, void* st_c, void* st_h, int32_t t, int32_t T, int64_t rc,
                          int64_t ld_state, int64_t row0, void* stream);
+/* Population form: one launch for K members of one agent with Rm replicas each (Rm a multiple of 64), rows
+ * k*Rm .. (k+1)*Rm - 1 of the shared obs / state / pi / val / act / store arrays belonging to member k.  Member k's
+ * parameters are params + k*p_stride (floats) and its packed image wpack + k*wp_stride (bf16 elements, 2A records each);
+ * it samples with seeds[k] (device array of K uint64, required also without act: every block reads its
+ * member's seed) and replica index r - k*Rm, so its outputs are bit-identical to
+ * tscl_policy_step_v2 on its own slice with seed seeds[k] and replica0 = 0.  State [2A][K*Rm][h]; store as in
+ * tscl_policy_step_v2 over K*Rm rows, with rc dividing Rm.  Work items are (member, unit, 64-replica tile). */
+int tscl_policy_step_v2g(tscl_handle* h, const float* params, int64_t p_stride, const void* wpack_bf16,
+                         int64_t wp_stride, const float* obs, int32_t K, int64_t Rm, const float* c_in,
+                         const float* h_in, float* c_out, float* h_out, float* pi, float* val, int32_t* act,
+                         int32_t done, const uint64_t* seeds, int64_t step, void* st_x, void* st_g, void* st_c,
+                         void* st_h, int32_t t, int32_t T, int64_t rc, void* stream);
 /* pi-only form of the v2 forward for test-mode evaluation (reference utils.py:Evaluator, LstmACPolicy.forward(.., 'p')):
  * the same kernel restricted to the A pi units (V units are never touched), bit-identical pi / c / h to the pi units of
  * tscl_policy_step_v2.  State is compact: c_in/h_in/c_out/h_out [A][ld_state or R][h] (out may alias in); pi

@@ -3,7 +3,7 @@ device-resident learners (deeprl_signal_control_b200/agents/train.py).
 
   python scripts/train.py --base-dir DIR train --config-dir CFG.ini
                           [--test-mode no_test|in_train_test|after_train_test|all_test] [--replicas N] [--policy lstm|fc]
-                          [--summaries]
+                          [--summaries] [--seeds 12,13,14,15]
   torchrun --nproc-per-node W scripts/train.py --base-dir DIR train --config-dir CFG.ini --replicas N
                           [--backend nccl|gloo] ...
 
@@ -21,6 +21,11 @@ Under torchrun with W > 1 processes, the N replicas are split over the W ranks (
 (LOCAL_RANK), and the learner all-reduces its gradient once per update over `--backend` (default nccl).  Rank 0 writes
 the directory and prints the JSON line, with "world": W; the run plays the episodes of a one-process run with the same
 --replicas.
+
+`--seeds s1,s2,...` trains a population in one process: one member of the agent per seed (its [ENV_CONFIG] seed), each
+on `--replicas` replicas (a multiple of 64), all in one lock-step.  Member s gets the complete agent directory
+DIR/seed<s>/<agent>/ of a one-seed run, so `scripts/evaluate.py --agent-dir DIR/seed<s>/<agent>` reads it.  ia2c / ma2c
+with the LSTM policy only, and not under torchrun.  The JSON line gains "seeds".
 """
 import argparse
 import datetime
@@ -49,16 +54,33 @@ def parse_args(argv=None):
                     help="also write the reference's TensorBoard event file into log/")
     sp.add_argument("--backend", default="nccl", choices=["nccl", "gloo"],
                     help="gradient all-reduce backend under torchrun (default nccl)")
+    sp.add_argument("--seeds", default=None,
+                    help="comma-separated seeds: train one population member per seed into DIR/seed<s>/<agent>/")
     a = p.parse_args(argv)
     if not a.option:
         p.print_help()
         raise SystemExit(1)
+    if a.seeds is not None:
+        from deeprl_signal_control_b200.agents.train import parse_seeds
+        try:
+            a.seeds = parse_seeds(a.seeds)
+        except ValueError as e:
+            p.error(str(e))
     return a
 
 
 def main(argv=None):
     a = parse_args(argv)
     world = int(os.environ.get("WORLD_SIZE", "1"))
+    if a.seeds is not None:
+        if world > 1:
+            raise SystemExit("--seeds trains a population in one process; it does not run under torchrun")
+        from deeprl_signal_control_b200.agents.train import train
+        out = train(a.config_dir, a.base_dir, a.test_mode, n_replicas=a.replicas, policy=a.policy,
+                    summaries=a.summaries, seeds=a.seeds)
+        print(json.dumps({"final_step": out.final_step, "episode_sets": out.episode_sets, "seeds": out.seeds,
+                          "env_samples": out.env_samples, "replicas": a.replicas, "wall_sec": round(out.wall_sec, 3)}))
+        return out
     if world <= 1:
         from deeprl_signal_control_b200.agents.train import train
         out = train(a.config_dir, a.base_dir, a.test_mode, n_replicas=a.replicas, policy=a.policy,
