@@ -138,7 +138,7 @@ class Evaluator:
             raise ValueError("Evaluator: the fp32 twin forward (use_tc=False) has no batched evaluation path; evaluate the "
                              "tensor-core model")
         else:
-            self.family = 'v2' if b.tc_v2 else 'v1'
+            self.family = b.paths.forward          # 'v2' or 'v1' (agents/learner.py:learner_paths)
         self.pi = torch.zeros(self.R, L.A, L.max_na, **f32)
         if self.family == 'v2':            # compact pi-unit state [A][R][h]
             self.c = torch.zeros(L.A, self.R, L.h, **f32); self.h = torch.zeros_like(self.c)

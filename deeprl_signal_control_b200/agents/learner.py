@@ -70,6 +70,55 @@ def check_population(seeds, seed, n_replicas, chunk, process_group):
     return seeds
 
 
+# fc widths dx of the fused v2 forward and of the fused dX / fc weight-gradient kernel (P2_DX_OK, csrc/tsc_policy_tc.cu):
+# grid MA2C 224, Monaco MA2C 192, grid IA2C 160, Monaco IA2C 128 at the reference's num_fw 128 / num_ft 32 / num_fp 64
+V2_DX = (128, 160, 192, 224)
+
+
+def learner_paths(layout: PolicyLayout, use_tc: bool = True, K: int = 1, dx_library: bool = False):
+    """The kernels `BatchedA2C(layout, use_tc=use_tc)` with K members runs, as a namespace:
+      forward   'v2' (tscl_policy_step_v2: fused fc front end, LSTM and heads on the tensor cores, activation store),
+                'v1' (tscl_policy_step: fc front end in fp32; wave blocks of at most 32 inputs) or 'fp32' (the twin kernels);
+      update    with the activation store on: 'lean' (every update kernel reads the bf16 store, dX fused into the fc weight
+                gradients), 'store' (the store unpacked to fp32, dX by a torch product, SIMT tscl_fc_bwd: the layout has no
+                spare input slot for the bias column of the tensor-core fc kernels); 'recompute' (no store: the forward is
+                recomputed in fp32 per chunk) or 'fp32' (use_tc off).  Without the store every 'lean' / 'store' layout
+                recomputes too;
+      and the flags BatchedA2C keeps: use_tc, tc_v2, dx_fusable, dx_own, dx_fc_fused, bwd_tc, fc_bwd_tc, wgrad_tc.
+    `dx_library` (TSC_DX_LIBRARY=1) replaces the stand-alone dX kernel by the library GEMM.  Raises ValueError for a
+    layout the tensor-core forward does not serve, and for a population (K > 1) without the fused forward and dX."""
+    L = layout
+    use_tc = bool(use_tc) and L.dx % 16 == 0 and L.kw > 0              # else: the fp32 kernels
+    if use_tc and L.dx > 224:
+        # the fused forwards keep [Wx;Wh] resident in shared memory: 224 + 64 input rows is the most that fits
+        raise ValueError("the tensor-core policy forward supports dx <= 224 (got %d); use use_tc=False" % L.dx)
+    tc_v2 = use_tc and L.dx in V2_DX
+    if use_tc and not tc_v2 and L.kw != 32:
+        # the v1 kernel stages a 32-wide wave block (tscl_policy_step)
+        raise ValueError("no tensor-core policy forward for fc width dx = %d with a wave block of %d inputs: the fused "
+                         "forward takes dx in %s, the v1 forward other multiples of 16 up to 224 with wave blocks of at "
+                         "most 32 inputs; change num_fw or use use_tc=False" % (L.dx, int(L.n_wave.max()), V2_DX))
+    if K > 1 and not tc_v2:
+        raise ValueError("a population needs the fused tensor-core forward (use_tc with fc width %s; got use_tc=%s, dx=%d)"
+                         % (", ".join(map(str, V2_DX)), use_tc, L.dx))
+    dx_own = use_tc and L.dx <= 224 and not dx_library          # stand-alone dX = dZ . Wx^T kernel (tscl_dx_tc)
+    p = types.SimpleNamespace(
+        use_tc=use_tc, tc_v2=tc_v2,
+        dx_fusable=use_tc and L.dx % 32 == 0 and L.dx <= 256,  # dX inside the BPTT kernel (BatchedA2C.dx_fused)
+        dx_own=dx_own,
+        # dX fused into the fc weight-gradient kernel (tscl_dx_fc_bwd_tc: dX never reaches memory) at the v2 widths
+        dx_fc_fused=dx_own and tc_v2,
+        bwd_tc=use_tc,
+        fc_bwd_tc=use_tc and L.fc_bwd_tc_ok,                    # front-end weight gradients on the tensor cores
+        wgrad_tc=use_tc and L.dx % 8 == 0 and L.dx <= 240)      # LSTM weight gradients on the tensor cores
+    if K > 1 and not p.dx_fc_fused:
+        raise ValueError("a population needs dX fused into the fc weight-gradient kernel (unset TSC_DX_LIBRARY)")
+    p.forward = "v2" if tc_v2 else "v1" if use_tc else "fp32"
+    p.update = ("fp32" if not use_tc else "recompute" if not tc_v2 else
+                "lean" if p.fc_bwd_tc and p.wgrad_tc else "store")
+    return p
+
+
 class BatchedA2C:
     def __init__(self, layout: PolicyLayout, n_replicas: int, n_step: int, gamma: float = 0.99,
                  v_coef: float = 0.5, max_grad_norm: float = 40.0, alpha: float = 0.99, eps: float = 1e-5,
@@ -80,6 +129,7 @@ class BatchedA2C:
         self.seeds = check_population(seeds, seed, n_replicas, chunk, process_group)
         seed = self.seeds[0]                  # with `seeds`, a one-member population is the solo learner of seeds[0]
         self.K, self.R_m = len(self.seeds), int(n_replicas)
+        self.paths = learner_paths(layout, use_tc, self.K, os.environ.get("TSC_DX_LIBRARY", "0") == "1")
         if not torch.cuda.is_available():
             raise RuntimeError("BatchedA2C needs a CUDA device (no CPU fallback exists)")
         self.lay, self.R, self.T = layout, self.K * int(n_replicas), int(n_step)
@@ -136,17 +186,10 @@ class BatchedA2C:
         self._one = torch.zeros(1, **f32)
         self._upd_bufs = None
         self.kernel_launches = 0
-        # fused tensor-core forward (csrc/tsc_policy_tc.cu): bf16 image of [Wx;Wh], refreshed after every update
-        self.use_tc = bool(use_tc) and (L.dx % 16 == 0) and layout.kw > 0    # else: the fp32 kernels
-        if self.use_tc and L.dx > 224:
-            # the fused forwards keep [Wx;Wh] resident in shared memory: 224 + 64 input rows is the most that fits
-            raise ValueError("the tensor-core policy forward supports dx <= 224 (got %d); use use_tc=False" % L.dx)
-        # fc front end on the tensor cores too; the v2 kernel is instantiated for the shipped fc widths (grid 224,
-        # Monaco 192, IA2C 160), other widths take the v1 kernel
-        self.tc_v2 = self.use_tc and L.dx in (160, 192, 224)
-        if self.K > 1 and not self.tc_v2:
-            raise ValueError("a population needs the fused tensor-core forward (use_tc with fc width 160, 192 or 224; got "
-                             "use_tc=%s, dx=%d)" % (bool(use_tc), L.dx))
+        # fused tensor-core forward (csrc/tsc_policy_tc.cu): bf16 image of [Wx;Wh], refreshed after every update; the fc
+        # front end on the tensor cores too at the V2_DX widths, other widths take the v1 kernel (learner_paths)
+        paths = self.paths
+        self.use_tc, self.tc_v2 = paths.use_tc, paths.tc_v2
         mdim = () if self.K == 1 else (self.K,)                # packed images per member
         self.Wp = torch.zeros(*mdim, U, ((L.dx + L.h) // 8) * 4 * L.h * 8 + 8 * L.dx * 8, dtype=torch.bfloat16,
                               device=self.dev)
@@ -157,18 +200,13 @@ class BatchedA2C:
         # product; `dx_fused = True` selects the fused kernel (tests/test_update_bench_size_gpu.py: test_fused_dx_bptt,
         # test_whole_update_matches_chunked_reference)
         self.dx_fused = False
-        self.dx_fusable = self.use_tc and L.dx % 32 == 0 and L.dx <= 256
+        self.dx_fusable = paths.dx_fusable
         # stand-alone dX = dZ . Wx^T kernel (tscl_dx_tc); False falls back to the library GEMM (A/B measurements only)
-        self.dx_own = self.use_tc and L.dx % 16 == 0 and L.dx <= 224 and os.environ.get("TSC_DX_LIBRARY", "0") != "1"
-        # dX fused into the fc weight-gradient kernel (tscl_dx_fc_bwd_tc: dX never reaches memory) at the fc widths of
-        # the v2 forward; False runs tscl_dx_tc + tscl_fc_bwd_tc (tests/test_dx_fc_bwd_fused_gpu.py compares the two)
-        self.dx_fc_fused = self.dx_own and self.tc_v2
-        self.bwd_tc = self.use_tc
-        self.fc_bwd_tc = self.use_tc and layout.fc_bwd_tc_ok     # front-end weight gradients on the tensor cores
-        self.wgrad_tc = self.use_tc and L.dx % 8 == 0 and L.dx <= 240   # LSTM weight gradients on the tensor cores
+        self.dx_own = paths.dx_own
+        # False runs tscl_dx_tc + tscl_fc_bwd_tc (tests/test_dx_fc_bwd_fused_gpu.py compares the two)
+        self.dx_fc_fused = paths.dx_fc_fused
+        self.bwd_tc, self.fc_bwd_tc, self.wgrad_tc = paths.bwd_tc, paths.fc_bwd_tc, paths.wgrad_tc
         self.fused_heads = True                                  # head weight gradients inside tscl_heads_loss
-        if self.K > 1 and not self.dx_fc_fused:
-            raise ValueError("a population needs dX fused into the fc weight-gradient kernel (unset TSC_DX_LIBRARY)")
         self.pack_weights()
         # bf16 activation store of the rollout's own forward pass (written by the v2 kernel): the update then
         # back-propagates through it instead of recomputing fc + gate GEMM + LSTM forward.
@@ -205,7 +243,7 @@ class BatchedA2C:
         if self.K == 1:
             return self
         return types.SimpleNamespace(lay=self.lay, _h=self._h, dev=self.dev, use_tc=self.use_tc, tc_v2=self.tc_v2,
-                                     K=1, P=self.P[k], MS=self.MS[k], Wp=self.Wp[k], stats=self.stats[k],
+                                     paths=self.paths, K=1, P=self.P[k], MS=self.MS[k], Wp=self.Wp[k], stats=self.stats[k],
                                      norms=self.norms[k], seed=self.seeds[k])
 
     def _st(self):
@@ -523,8 +561,8 @@ class BatchedA2C:
                 _lib.check(lib.tscl_dx_tc(self._h, _p(dZb), _p(Wxt), _p(dXb), C.c_int64(M), st()))
             elif all_tc and not fuse_dx:
                 torch.bmm(dZb, self.wx_b.transpose(1, 2), out=dXb)
-            elif not all_tc:
-                torch.bmm(dZ, self.pv["wx"].transpose(1, 2), out=dX)
+            elif not all_tc:        # Wx of this chunk's member (self.pv is the K = 1 view only)
+                torch.bmm(dZ, P[L.off_wx:L.off_wh].view(U, L.dx, 4 * L.h).transpose(1, 2), out=dX)
             if fuse_fc:
                 pass            # the fc weight gradients came out of tscl_dx_fc_bwd_tc above
             elif self.fc_bwd_tc:

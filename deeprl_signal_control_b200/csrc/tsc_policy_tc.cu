@@ -622,7 +622,7 @@ extern "C" int tscl_policy_step(tscl_handle* h, const float* params, const void*
 // are the same m64nN k16 instructions in the same k order as a 128-row tile walked 64 columns at a time, and the cell,
 // store and head arithmetic is per element what it was, so the outputs do not depend on this organisation.
 #define P2_ROWS 64
-#define P2_DX_OK(dx) ((dx) == 160 || (dx) == 192 || (dx) == 224)   // keep in sync with BatchedA2C.tc_v2
+#define P2_DX_OK(dx) ((dx) == 128 || (dx) == 160 || (dx) == 192 || (dx) == 224)   // keep in sync with learner.V2_DX
 #define P2_THREADS 384
 // setmaxnreg: the producer gives registers back, the consumers (four m64n64 gate fragments = 128 per thread, plus the
 // cell state) take them.  setmaxnreg.inc only draws on what the CTA was launched with (168 per thread at 384 threads =
@@ -643,7 +643,8 @@ __host__ __device__ inline int gate_col(int n) {
 }
 
 // DX = d.dx: the fragment sizes and the k loops are compile-time.  Instantiated for the fc widths of the shipped
-// configurations (P2_DX_OK): 224 (grid MA2C), 192 (Monaco), 160 (IA2C: no fingerprint block)
+// configurations (P2_DX_OK): 224 (grid MA2C), 192 (Monaco), 160 (grid IA2C: no fingerprint block), 128 (Monaco IA2C:
+// no fingerprint or wait block)
 // EVAL: the pi-only forward of test-mode evaluation (tscl_policy_step_pi).  Work items are (pi unit u = 2 * agent, 64 rows),
 // n_tiles * A of them; V units are never loaded, multiplied or stored.  The recurrent state is compact, [A][ld][h] (row
 // (u >> 1) * ld + r); there is no activation store, no zdbg and no value output.  Per element the arithmetic is the
@@ -1061,14 +1062,14 @@ extern "C" int tscl_policy_step_v2r(tscl_handle* h, const float* params, const v
   PCK(cudaSetDevice(tscl_device_of(h)));
   const DDimsTC& d = *tscl_dims_of(h);
   const int K = d.dx + TC_H;
-  if (!P2_DX_OK(d.dx)) return tsc_set_error("tscl_policy_step_v2r: no kernel for this dx (160, 192 or 224)");
+  if (!P2_DX_OK(d.dx)) return tsc_set_error("tscl_policy_step_v2r: no kernel for this dx (128, 160, 192 or 224)");
   if (d.kw == 0) return tsc_set_error("tscl_policy_step_v2r: observation slice does not fit the 64-column input tile");
   const size_t smem = tc2_smem_bytes(K);
   if (smem > 232448) return tsc_set_error("tscl_policy_step_v2r: operand tiles exceed shared memory");
   void (*kern)(const DDimsTC, const StepTC) = nullptr;
   const bool prof = g_policy_prof != nullptr;
 #define P2_CASE(n) case n: kern = prof ? policy_step_tc2_kernel<n, true, false> : policy_step_tc2_kernel<n, false, false>; break;
-  switch (d.dx) { P2_CASE(160) P2_CASE(192) P2_CASE(224) }
+  switch (d.dx) { P2_CASE(128) P2_CASE(160) P2_CASE(192) P2_CASE(224) }
 #undef P2_CASE
   static int attr_dev = -1;
   static void (*attr_kern)(const DDimsTC, const StepTC) = nullptr;
@@ -1113,7 +1114,7 @@ extern "C" int tscl_policy_step_v2g(tscl_handle* h, const float* params, int64_t
   if (st_x && (rc <= 0 || Rm % rc != 0)) return tsc_set_error("tscl_policy_step_v2g: store chunk must divide the member replica count");
   PCK(cudaSetDevice(tscl_device_of(h)));
   const DDimsTC& d = *tscl_dims_of(h);
-  if (!P2_DX_OK(d.dx)) return tsc_set_error("tscl_policy_step_v2g: no kernel for this dx (160, 192 or 224)");
+  if (!P2_DX_OK(d.dx)) return tsc_set_error("tscl_policy_step_v2g: no kernel for this dx (128, 160, 192 or 224)");
   if (d.kw == 0) return tsc_set_error("tscl_policy_step_v2g: observation slice does not fit the 64-column input tile");
   if (K > 1 && (p_stride < d.n_params || wp_stride_m < 2 * d.A * wp_stride(d.dx)))
     return tsc_set_error("tscl_policy_step_v2g: member strides smaller than one member's parameters / image");
@@ -1121,6 +1122,7 @@ extern "C" int tscl_policy_step_v2g(tscl_handle* h, const float* params, int64_t
   if (smem > 232448) return tsc_set_error("tscl_policy_step_v2g: operand tiles exceed shared memory");
   void (*kern)(const DDimsTC, const StepTC) = nullptr;
   switch (d.dx) {
+    case 128: kern = policy_step_tc2_kernel<128, false, false, true>; break;
     case 160: kern = policy_step_tc2_kernel<160, false, false, true>; break;
     case 192: kern = policy_step_tc2_kernel<192, false, false, true>; break;
     case 224: kern = policy_step_tc2_kernel<224, false, false, true>; break;
@@ -1159,12 +1161,13 @@ extern "C" int tscl_policy_step_pi(tscl_handle* h, const float* params, const vo
   if (ld_state > 0 && (row0 < 0 || row0 + R > ld_state)) return tsc_set_error("tscl_policy_step_pi: replica range outside [0, ld_state)");
   PCK(cudaSetDevice(tscl_device_of(h)));
   const DDimsTC& d = *tscl_dims_of(h);
-  if (!P2_DX_OK(d.dx)) return tsc_set_error("tscl_policy_step_pi: no kernel for this dx (160, 192 or 224)");
+  if (!P2_DX_OK(d.dx)) return tsc_set_error("tscl_policy_step_pi: no kernel for this dx (128, 160, 192 or 224)");
   if (d.kw == 0) return tsc_set_error("tscl_policy_step_pi: observation slice does not fit the 64-column input tile");
   const size_t smem = tc2_smem_bytes(d.dx + TC_H);
   if (smem > 232448) return tsc_set_error("tscl_policy_step_pi: operand tiles exceed shared memory");
   void (*kern)(const DDimsTC, const StepTC) = nullptr;
   switch (d.dx) {
+    case 128: kern = policy_step_tc2_kernel<128, false, true>; break;
     case 160: kern = policy_step_tc2_kernel<160, false, true>; break;
     case 192: kern = policy_step_tc2_kernel<192, false, true>; break;
     case 224: kern = policy_step_tc2_kernel<224, false, true>; break;
@@ -2999,20 +3002,22 @@ extern "C" int tscl_dx_fc_bwd_tc(tscl_handle* h, const float* obs, const void* x
   if (M >= ((int64_t)1 << 31) - 128) return tsc_set_error("tscl_dx_fc_bwd_tc: M must be below 2^31 - 128 rows");
   PCK(cudaSetDevice(tscl_device_of(h)));
   const DDimsTC& d = *tscl_dims_of(h);
-  if (!P2_DX_OK(d.dx)) return tsc_set_error("tscl_dx_fc_bwd_tc: dx must be 160, 192 or 224 (use tscl_dx_tc + tscl_fc_bwd_tc)");
+  if (!P2_DX_OK(d.dx)) return tsc_set_error("tscl_dx_fc_bwd_tc: dx must be 128, 160, 192 or 224 (use tscl_dx_tc + tscl_fc_bwd_tc)");
   if (d.kw == 0 || d.ones_slot < 0) return tsc_set_error("tscl_dx_fc_bwd_tc: no free input slot for the bias column");
   CUtensorMap mZ, mX;
   if (!make_tmap_3d(&mZ, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, dz_bf16, 2 * d.A, M, TC_N, 64, 128) ||
       !make_tmap_3d(&mX, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, x_bf16, 2 * d.A, M, d.dx, 8, 128, CU_TENSOR_MAP_SWIZZLE_NONE))
     return tsc_set_error("tscl_dx_fc_bwd_tc: cannot build the tensor maps (dz_bf16 / x_bf16 must be 16-byte aligned)");
   void (*kern)(const DDimsTC, const DxFcTC, const CUtensorMap, const CUtensorMap) =
-      d.dx == 224 ? dx_fc_bwd_tc_kernel<224> : d.dx == 192 ? dx_fc_bwd_tc_kernel<192> : dx_fc_bwd_tc_kernel<160>;
+      d.dx == 224 ? dx_fc_bwd_tc_kernel<224> : d.dx == 192 ? dx_fc_bwd_tc_kernel<192> :
+      d.dx == 160 ? dx_fc_bwd_tc_kernel<160> : dx_fc_bwd_tc_kernel<128>;
   const size_t smem = dxf_smem(d.dx);
   static int attr_dev = -1;
   if (attr_dev != tscl_device_of(h)) {
     PCK(cudaFuncSetAttribute(dx_fc_bwd_tc_kernel<224>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dxf_smem(224)));
     PCK(cudaFuncSetAttribute(dx_fc_bwd_tc_kernel<192>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dxf_smem(192)));
     PCK(cudaFuncSetAttribute(dx_fc_bwd_tc_kernel<160>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dxf_smem(160)));
+    PCK(cudaFuncSetAttribute(dx_fc_bwd_tc_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dxf_smem(128)));
     attr_dev = tscl_device_of(h);
   }
   int n_sm = 0;

@@ -170,7 +170,7 @@ int tscl_memcpy_async(tscl_handle* h, void* dst, const void* src, int64_t bytes,
  * Warp-specialised wgmma kernel (cp.async loaders -> 128B-swizzled operand stages, double-buffered accumulator tiles, bulk-copy stores).
  * dx must be a multiple of 16, <= 224 for the shared-memory budget. */
 int tscl_dx_tc(tscl_handle* h, const void* dz_bf16, const void* wxt_bf16, void* dx_bf16, int64_t M, void* stream);
-/* tscl_dx_tc followed by tscl_fc_bwd_tc in one pass, without dX in memory (the shipping path for dx = 160, 192, 224):
+/* tscl_dx_tc followed by tscl_fc_bwd_tc in one pass, without dX in memory (the shipping path for dx = 128, 160, 192, 224):
  * grads[fc blocks] += obs^T . (bf16(dz_bf16 . Wx^T) * (x_bf16 > 0)) and the bias sums, rows as tscl_fc_bwd_tc.
  * x_bf16 [2A][M][dx] (one chunk of the bf16 activation store), dz_bf16 [2A][M][256], both 16-byte aligned (read through
  * tensor maps); wxt_bf16 from tscl_pack_wxt.  The masked bf16 dX has the bits of the two-call path; only the order of

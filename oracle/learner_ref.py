@@ -199,7 +199,7 @@ def bptt_ref(gates, c, c0, dH, dones, wh, round_bf16=True, c_prev=None):
     return dZ
 
 
-def lstm_grads_ref(X, Hs, h0, dones, dZ, wx, round_bf16=True, round_operands=False, dx_product="bf16"):
+def lstm_grads_ref(X, Hs, h0, dones, dZ, wx, round_bf16=True, round_operands=False, dx_product="bf16", dx_bf16=True):
     """LSTM weight gradients [X | Hp | 1]^T dZ and dX = dZ . Wx^T (tscl_wgrad_tc, tscl_dx_tc).  X [..., T, rc, dx],
     Hs [..., T, rc, h] (store), h0 [..., rc, h] (h_bw rows r0 .. r0 + rc), dZ [..., T, rc, 4h], wx [..., dx, 4h].
     Hp[t] = (1 - done[t]) * (h[t-1], or h0 at t = 0).  Returns (wx, wh, bl, dX [..., T, rc, dx]).
@@ -208,7 +208,8 @@ def lstm_grads_ref(X, Hs, h0, dones, dZ, wx, round_bf16=True, round_operands=Fal
                       its fp32 X / Hp; on the store path they are bf16 already and only h0 is rounded);
       dx_product      operands of dX: "bf16" bf16(dZ) . bf16(Wx)^T (the store path's tensor-core kernels), "fp32" the
                       unrounded fp32 dZ . Wx^T, "tf32" both rounded to TF32 (torch.bmm with TF32 allowed);
-    dX is then rounded to bf16, where the fc weight-gradient kernel converts it."""
+    dX is then rounded to bf16, where the fc weight-gradient kernel converts it (not with dx_bf16=False: the SIMT
+    tscl_fc_bwd reads it in fp32)."""
     keep = (1.0 - torch.as_tensor([float(d) for d in dones], dtype=X.dtype, device=X.device))[:, None, None]
     h0r = bf16(h0) if round_bf16 else h0
     Hp = torch.cat([h0r.unsqueeze(-3), Hs[..., :-1, :, :]], -3) * keep
@@ -221,7 +222,7 @@ def lstm_grads_ref(X, Hs, h0, dones, dZ, wx, round_bf16=True, round_operands=Fal
     gwh = flat(Hp).transpose(-1, -2) @ Zf
     rnd = {"bf16": bf16, "fp32": lambda t_: t_, "tf32": tf32}[dx_product if round_bf16 else "fp32"]
     dX = (Z if dx_product == "bf16" else rnd(dZ)) @ rnd(wx).transpose(-1, -2).unsqueeze(-3)
-    return gwx, gwh, Zf.sum(-2), (bf16(dX) if round_bf16 else dX)
+    return gwx, gwh, Zf.sum(-2), (bf16(dX) if round_bf16 and dx_bf16 else dX)
 
 
 def fc_grads_ref(lay, u, obs, X, dX, round_bf16=True):
@@ -234,13 +235,14 @@ def fc_grads_ref(lay, u, obs, X, dX, round_bf16=True):
         if w == 0:
             continue
         d_ = dd[:, c0:c0 + w]
-        out["%s_w%d" % (name, u)] = inp.reshape(-1, inp.shape[-1]).T @ d_
+        out["%s_w%d" % (name, u)] = inp.flatten(0, -2).T @ d_           # flatten: the block may be empty
         out["%s_b%d" % (name, u)] = d_.sum(0)
     return out
 
 
 def update_ref(lay, P, store, obs, act, Rs, Adv, c_bw, h_bw, dones, scale, v_coef, beta, chunk, round_bf16=True,
-               agents_per_group=None, store_units=False, round_operands=False, dx_product="bf16", agents=None):
+               agents_per_group=None, store_units=False, round_operands=False, dx_product="bf16", agents=None,
+               fc_fp32=False):
     """Flat gradient G (float64) of one update from the activation store, summed over the chunks r0 = 0, chunk, ...
     P: fp32 parameters (any float tensor); store(ci) -> (st_x, st_g, st_c, st_h) of chunk ci, each [U][T][rc][w], or
     with `store_units` store(ci, us) -> the same for the unit slice `us` only (lets a caller compute the store of one agent
@@ -248,7 +250,9 @@ def update_ref(lay, P, store, obs, act, Rs, Adv, c_bw, h_bw, dones, scale, v_coe
     obs [T, R, n_obs], act / Rs / Adv [T, R, A], c_bw / h_bw [U, R, h], dones = done_pre [T].  Work runs on P's device,
     `agents_per_group` agents at a time (bounds the float64 working set); `agents` (a range) restricts the sum to those
     agents.  round_operands / dx_product: see lstm_grads_ref (the defaults are the store path's rounding; the recompute
-    path is round_operands=True with dx_product "fp32" or "tf32").  Returns (G, agent-0 stats)."""
+    path is round_operands=True with dx_product "fp32" or "tf32").  `fc_fp32`: the fc front-end gradients from fp32 obs and
+    dX (the store path of a layout without a spare bias slot: dX by torch.bmm, then the SIMT tscl_fc_bwd).
+    Returns (G, agent-0 stats)."""
     f64 = dict(dtype=torch.float64, device=P.device)
     v = lay.views(P.to(torch.float64))
     G = torch.zeros(lay.n_params, **f64)
@@ -284,13 +288,14 @@ def update_ref(lay, P, store, obs, act, Rs, Adv, c_bw, h_bw, dones, scale, v_coe
             h0 = h_bw[us, r0:r0 + rc].to(**f64)
             dZ = bptt_ref(Gt, Cs, c0, dH, dones, v["wh"][us], round_bf16)
             del dH, Gt, Cs
-            gwx, gwh, gbl, dX = lstm_grads_ref(X, Hs, h0, dones, dZ, v["wx"][us], round_bf16, round_operands, dx_product)
+            gwx, gwh, gbl, dX = lstm_grads_ref(X, Hs, h0, dones, dZ, v["wx"][us], round_bf16, round_operands, dx_product,
+                                               dx_bf16=not fc_fp32)
             del dZ
             gv["wx"][us] += gwx
             gv["wh"][us] += gwh
             gv["bl"][us] += gbl
             for k, u in enumerate(range(us.start, us.stop)):
-                for name, g in fc_grads_ref(lay, u, ob, X[k], dX[k], round_bf16).items():
+                for name, g in fc_grads_ref(lay, u, ob, X[k], dX[k], round_bf16 and not fc_fp32).items():
                     gv[name] += g
             del X, Hs, dX
     return G, stats
