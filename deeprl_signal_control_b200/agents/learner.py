@@ -19,6 +19,12 @@ seeds[k], replica index relative to the member), so each member trains what `Bat
 The update runs the one-member kernels chunk by chunk (a chunk never straddles two members) with the member's
 pointers, then one clip + RMSProp and one repack per member.  `member(k)` is a solo-model view of member k.
 
+Sweep (`hparams`, K dicts of SWEEP_KEYS next to `seeds`, which may then repeat): a population whose members also differ
+in gamma, v_coef, max_grad_norm, RMSProp alpha / eps and reward_norm / reward_clip, and whose `backward` takes one lr
+and one beta per member.  Each chunk's loss kernel takes its member's v_coef and beta, each member's clip + RMSProp its
+own lr, max_grad_norm, alpha and eps; the returns (tscl_returns_g) and the device reward hand-over
+(tscl_device_transition_g) read per-member device arrays when the members' values differ.
+
 Shipping path (`use_tc`, the default): every kernel is hand-written — the fused wgmma forward
 (csrc/tsc_policy_tc.cu: fc front end, gate GEMM, LSTM cell, heads, sampling, bf16 activation store), the wgmma
 update (BPTT with TMA operand copies, dX = dZ.Wx^T, LSTM and fc weight gradients) and the SIMT kernels of
@@ -57,6 +63,32 @@ def check_population(seeds, seed, n_replicas, chunk, process_group):
         raise ValueError("a population needs at least one seed")
     if len(set(seeds)) != len(seeds):
         raise ValueError("population seeds must be distinct (got %s)" % seeds)
+    return _check_members(seeds, n_replicas, chunk, process_group)
+
+
+# the learner values a sweep member sets for itself (BatchedA2C(hparams=...)); lr and beta come with each backward
+SWEEP_KEYS = ("gamma", "v_coef", "max_grad_norm", "alpha", "eps", "reward_norm", "reward_clip")
+
+
+def check_sweep(seeds, hparams, n_replicas, chunk, process_group):
+    """(seeds, hparams) of a sweep learner: one seed per member (seeds may repeat) and one dict per member holding
+    exactly SWEEP_KEYS (reward_norm / reward_clip None or 0: off), under check_population's rules for replicas, the update
+    chunk and the process group."""
+    if seeds is None:
+        raise ValueError("a sweep takes `seeds`, one per member")
+    seeds, hparams = [int(s) for s in seeds], [dict(h) for h in hparams]
+    if len(seeds) != len(hparams):
+        raise ValueError("a sweep takes one seed per member (got %d seeds for %d members)" % (len(seeds), len(hparams)))
+    for k, h in enumerate(hparams):
+        if set(h) != set(SWEEP_KEYS):
+            raise ValueError("member %d's hyperparameters must be exactly %s (got %s)" % (k, SWEEP_KEYS, sorted(h)))
+    _check_members(seeds, n_replicas, chunk, process_group)
+    return seeds, [{key: float(h[key] or 0.0) for key in SWEEP_KEYS} for h in hparams]
+
+
+def _check_members(seeds, n_replicas, chunk, process_group):
+    if not seeds:
+        raise ValueError("a population needs at least one seed")
     if any(s < 0 or s >= 1 << 63 for s in seeds):
         raise ValueError("population seeds must lie in [0, 2^63) (got %s)" % seeds)
     if len(seeds) > 1:
@@ -125,8 +157,15 @@ class BatchedA2C:
                  reward_norm: float = 1.0, reward_clip: float = 0.0, seed: int = 0, device: int = 0,
                  chunk: int = 1024, replica0: int = 0, total_replicas: Optional[int] = None,
                  process_group=None, allow_tf32: bool = True, use_tc: bool = True,
-                 store_acts: Optional[bool] = None, seeds: Optional[Sequence[int]] = None):
-        self.seeds = check_population(seeds, seed, n_replicas, chunk, process_group)
+                 store_acts: Optional[bool] = None, seeds: Optional[Sequence[int]] = None,
+                 hparams: Optional[Sequence[dict]] = None):
+        if hparams is None:
+            self.seeds = check_population(seeds, seed, n_replicas, chunk, process_group)
+            self.hp = [dict(gamma=gamma, v_coef=v_coef, max_grad_norm=max_grad_norm, alpha=alpha, eps=eps,
+                            reward_norm=reward_norm, reward_clip=reward_clip)] * len(self.seeds)
+        else:                                 # a sweep: member 0's values stand for the learner's scalars
+            self.seeds, self.hp = check_sweep(seeds, hparams, n_replicas, chunk, process_group)
+            gamma, v_coef, max_grad_norm, alpha, eps, reward_norm, reward_clip = (self.hp[0][k] for k in SWEEP_KEYS)
         seed = self.seeds[0]                  # with `seeds`, a one-member population is the solo learner of seeds[0]
         self.K, self.R_m = len(self.seeds), int(n_replicas)
         self.paths = learner_paths(layout, use_tc, self.K, os.environ.get("TSC_DX_LIBRARY", "0") == "1")
@@ -196,6 +235,12 @@ class BatchedA2C:
         self.Wt = torch.zeros(*mdim, U, 32, L.h, 8, dtype=torch.bfloat16, device=self.dev)    # Wh^T image for the BPTT MMA
         self.Wxt = torch.zeros(*mdim, U, 32, L.dx, 8, dtype=torch.bfloat16, device=self.dev)  # Wx^T image: dX fused into the BPTT
         self.seeds_dev = torch.tensor(self.seeds, dtype=torch.int64, device=self.dev) if self.K > 1 else None
+        # a sweep's per-member device values, only where the members differ (else the one-member kernels run)
+        differ = lambda *keys: any(len({h[k] for h in self.hp}) > 1 for k in keys)
+        per = lambda key: torch.tensor([h[key] for h in self.hp], **f32)
+        self.gamma_dev = per("gamma") if differ("gamma") else None
+        self.rscale_differs = differ("reward_norm", "reward_clip")
+        self.rnorm_dev, self.rclip_dev = (per("reward_norm"), per("reward_clip")) if self.rscale_differs else (None, None)
         # fusing dX into the BPTT step lengthens its serial per-step chain, so the default keeps dX as a separate
         # product; `dx_fused = True` selects the fused kernel (tests/test_update_bench_size_gpu.py: test_fused_dx_bptt,
         # test_whole_update_matches_chunked_reference)
@@ -239,12 +284,26 @@ class BatchedA2C:
 
     def member(self, k: int):
         """Member k as a solo learner reads: its parameters P, RMSProp slot MS, packed image Wp, loss terms stats and
-        gradient norms norms (views into the stacked tensors, so they follow training), with the layout and handle."""
+        gradient norms norms (views into the stacked tensors, so they follow training), with the layout and handle, and
+        its own SWEEP_KEYS values."""
         if self.K == 1:
             return self
         return types.SimpleNamespace(lay=self.lay, _h=self._h, dev=self.dev, use_tc=self.use_tc, tc_v2=self.tc_v2,
                                      paths=self.paths, K=1, P=self.P[k], MS=self.MS[k], Wp=self.Wp[k], stats=self.stats[k],
-                                     norms=self.norms[k], seed=self.seeds[k])
+                                     norms=self.norms[k], seed=self.seeds[k], **self.hp[k])
+
+    def _one_reward_scaling(self, what):
+        if self.rscale_differs:
+            raise ValueError("%s applies one reward_norm / reward_clip to every replica, but the sweep's members "
+                             "differ in them; use the device-resident loop (add_transition_device)" % what)
+
+    def _per_member(self, v, name):
+        """lr / beta of backward(): one value for every member, or a sequence of K"""
+        if isinstance(v, (list, tuple, np.ndarray)):
+            if len(v) != self.K:
+                raise ValueError("%s takes one value per member (%d, got %d)" % (name, self.K, len(v)))
+            return [float(x) for x in v]
+        return [v] * self.K
 
     def _st(self):
         return C.c_void_p(torch.cuda.current_stream(self.dev).cuda_stream)
@@ -375,6 +434,7 @@ class BatchedA2C:
     def add_transition_range(self, r0: int, n: int, reward: torch.Tensor):
         """add_transition() data movement for one replica range (reward [n, A]); finish the step with
         end_transition_ranges(done_pre, done_post)."""
+        self._one_reward_scaling("add_transition_range")
         t = self.t
         r = reward
         if self.reward_norm:
@@ -399,6 +459,7 @@ class BatchedA2C:
                        act: Optional[torch.Tensor] = None, val: Optional[torch.Tensor] = None):
         """Record step t: obs must already be in obs_slot(t) (the env writes there); actions and
         values default to the ones of the last forward().  agents/models.py:222-229."""
+        self._one_reward_scaling("add_transition")
         t = self.t
         r = reward
         if self.reward_norm:
@@ -416,11 +477,17 @@ class BatchedA2C:
                               done_post: bool):
         """add_transition() of the device-resident loop in ONE launch: normalised / clipped reward into the rollout slot
         and the episode sum of the global reward; actions / values are already in their slots when the last forward ran
-        with to_hist=True (copied otherwise).  Same arithmetic as add_transition (r * (1 / norm), clamp)."""
+        with to_hist=True (copied otherwise).  Same arithmetic as add_transition (r * (1 / norm), clamp).  A sweep whose
+        members differ in reward_norm / reward_clip scales each member's rows with its own (tscl_device_transition_g)."""
         t = self.t
-        _lib.check(_lib.lib().tscl_device_transition(
-            self._h, _p(reward), _p(self.rew_hist[t]), C.c_int64(reward.numel()), C.c_float(self.reward_norm or 0.0),
-            C.c_float(self.reward_clip or 0.0), _p(greward), _p(rew_acc), C.c_int64(greward.numel()), self._st()))
+        if self.rscale_differs:
+            _lib.check(_lib.lib().tscl_device_transition_g(
+                self._h, _p(reward), _p(self.rew_hist[t]), C.c_int64(reward.numel()), _p(self.rnorm_dev),
+                _p(self.rclip_dev), C.c_int32(self.K), _p(greward), _p(rew_acc), C.c_int64(greward.numel()), self._st()))
+        else:
+            _lib.check(_lib.lib().tscl_device_transition(
+                self._h, _p(reward), _p(self.rew_hist[t]), C.c_int64(reward.numel()), C.c_float(self.reward_norm or 0.0),
+                C.c_float(self.reward_clip or 0.0), _p(greward), _p(rew_acc), C.c_int64(greward.numel()), self._st()))
         if not getattr(self, "_hist_direct", False):
             self.act_hist[t].copy_(self.act)
             self.val_hist[t].copy_(self.val)
@@ -452,9 +519,11 @@ class BatchedA2C:
 
     def backward(self, boot: Optional[torch.Tensor], lr: float, beta: float):
         """One A2C update from the stored n_step rollout (agents/models.py:174-183).  `boot` is the
-        bootstrap value [R, A] (None / zeros when the episode ended, utils.py:186-190)."""
+        bootstrap value [R, A] (None / zeros when the episode ended, utils.py:186-190).  `lr` / `beta`: one value, or one
+        per member (a sweep's schedules)."""
         assert self.t == self.T, "rollout buffer not full"
         L, R, T, U, A, lib = self.lay, self.R, self.T, self.lay.U, self.lay.A, _lib.lib()
+        lrs, betas = self._per_member(lr, "lr"), self._per_member(beta, "beta")
         self._mm()
         st = self._st
         f32 = dict(dtype=torch.float32, device=self.dev)
@@ -464,8 +533,13 @@ class BatchedA2C:
             self.boot.zero_()
         else:
             self.boot.copy_(boot)
-        _lib.check(lib.tscl_returns(self._h, _p(self.rew_hist), _p(self.val_hist), _p(self.boot), _p(dpost),
-                                    C.c_float(self.gamma), C.c_int32(T), C.c_int64(R), _p(self.Rs), _p(self.Adv), st()))
+        if self.gamma_dev is not None:
+            _lib.check(lib.tscl_returns_g(self._h, _p(self.rew_hist), _p(self.val_hist), _p(self.boot), _p(dpost),
+                                          _p(self.gamma_dev), C.c_int32(self.K), C.c_int32(T), C.c_int64(R), _p(self.Rs),
+                                          _p(self.Adv), st()))
+        else:
+            _lib.check(lib.tscl_returns(self._h, _p(self.rew_hist), _p(self.val_hist), _p(self.boot), _p(dpost),
+                                        C.c_float(self.gamma), C.c_int32(T), C.c_int64(R), _p(self.Rs), _p(self.Adv), st()))
         self.G.zero_()
         self.stats.zero_()
         scale = _dist.grad_scale(T, 1, self.total_replicas)       # local SUM x 1/(n_step * R_total); ranks add up
@@ -474,6 +548,7 @@ class BatchedA2C:
             raise RuntimeError("a population update needs every step of the rollout in the activation store")
         n_obs = L.n_obs
         P, G, Wt, Wxt, stats = self.P, self.G, self.Wt, self.Wxt, self.stats
+        k = 0
         for r0 in range(0, R, self.chunk):
             if self.K > 1:        # the member of this chunk: its weights, images, gradient and loss terms
                 k = r0 // self.R_m
@@ -522,7 +597,8 @@ class BatchedA2C:
             hb = _p(self.st_h[ci]) if use_store else None
             _lib.check(lib.tscl_heads_loss(self._h, _p(P), None if all_tc else _p(H), _p(self.act_hist[0, r0:]),
                                            _p(self.Rs[0, r0:]), _p(self.Adv[0, r0:]), C.c_int64(M), C.c_int64(rc),
-                                           C.c_int64(R * A), C.c_float(self.v_coef), C.c_float(beta), C.c_float(scale),
+                                           C.c_int64(R * A), C.c_float(self.hp[k]["v_coef"]), C.c_float(betas[k]),
+                                           C.c_float(scale),
                                            None if self.fused_heads else _p(dlog), _p(dH), _p(stats),
                                            hb if all_tc else None, _p(G) if self.fused_heads else None, st()))
             if not self.fused_heads:
@@ -578,9 +654,10 @@ class BatchedA2C:
             _dist.allreduce_sum_(self.G, self.pg)
         for k in range(self.K):
             m = (lambda t_: t_) if self.K == 1 else (lambda t_: t_[k])
+            hk = self.hp[k]
             _lib.check(lib.tscl_clip_rmsprop(self._h, _p(m(self.P)), _p(m(self.G)), _p(m(self.MS)), _p(self.agent_of),
-                                             C.c_float(self.max_grad_norm), C.c_float(lr), C.c_float(self.alpha),
-                                             C.c_float(self.eps), _p(m(self.norms)), st()))
+                                             C.c_float(hk["max_grad_norm"]), C.c_float(lrs[k]), C.c_float(hk["alpha"]),
+                                             C.c_float(hk["eps"]), _p(m(self.norms)), st()))
             self.kernel_launches += 3
         self.pack_weights()
         # states_bw <- states_fw (agents/policies.py:153); next rollout starts at slot 0

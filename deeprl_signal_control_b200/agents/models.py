@@ -25,17 +25,51 @@ from .learner import BatchedA2C
 from .utils import Scheduler
 
 
+def a2c_schedulers(model_config, total_step):
+    """(lr_scheduler, beta_scheduler) of IA2C / MA2C (agents/models.py:53-69): lr decays over total_step, the entropy
+    coefficient over total_step * entropy_ratio, each 'constant' or 'linear'."""
+    lr_init = model_config.getfloat('lr_init')
+    lr_decay = model_config.get('lr_decay')
+    beta_init = model_config.getfloat('entropy_coef_init')
+    beta_decay = model_config.get('entropy_decay')
+    if lr_decay == 'constant':
+        lr = Scheduler(lr_init, decay=lr_decay)
+    else:
+        lr = Scheduler(lr_init, model_config.getfloat('LR_MIN'), total_step, decay=lr_decay)
+    if beta_decay == 'constant':
+        beta = Scheduler(beta_init, decay=beta_decay)
+    else:
+        beta = Scheduler(beta_init, model_config.getfloat('ENTROPY_COEF_MIN'),
+                         total_step * model_config.getfloat('ENTROPY_RATIO'), decay=beta_decay)
+    return lr, beta
+
+
+def a2c_hparams(model_config):
+    """The `BatchedA2C` values of one [MODEL_CONFIG] section, keyed by learner.SWEEP_KEYS."""
+    return dict(gamma=model_config.getfloat('gamma'), v_coef=model_config.getfloat('value_coef'),
+                max_grad_norm=model_config.getfloat('max_grad_norm'), alpha=model_config.getfloat('rmsp_alpha'),
+                eps=model_config.getfloat('rmsp_epsilon'), reward_norm=model_config.getfloat('reward_norm'),
+                reward_clip=model_config.getfloat('reward_clip'))
+
+
 class IA2C:
     name = 'ia2c'
 
     def __init__(self, n_s_ls, n_a_ls, n_w_ls, total_step, model_config, seed=0, n_f_ls=None,
-                 n_replicas=1, device=0, obs_off=None, policy='lstm', seeds=None, **learner_kw):
+                 n_replicas=1, device=0, obs_off=None, policy='lstm', seeds=None, member_configs=None, **learner_kw):
         """policy='lstm': LstmACPolicy / FPLstmACPolicy, what the reference builds (agents/models.py:40-51);
         policy='fc': FcACPolicy (agents/policies.py:214-256), the FC variant of BASELINE config 2.
         seeds: a population of len(seeds) members, n_replicas each, member k initialised from seeds[k] (`BatchedA2C`;
-        LSTM policy only); `members()` gives each as a solo model."""
+        LSTM policy only); `members()` gives each as a solo model.
+        member_configs: a sweep, one [MODEL_CONFIG] section per seed (model_config is member 0's): member k takes its
+        learner values (`a2c_hparams`) and its lr / beta schedules (`lr_schedulers[k]`, `beta_schedulers[k]`) from
+        member_configs[k]; seeds may then repeat."""
         if seeds is not None and len(seeds) > 1 and policy == 'fc':
             raise ValueError("a population trains the LSTM policy only (got policy='fc')")
+        if member_configs is not None:
+            if seeds is None or len(member_configs) != len(seeds):
+                raise ValueError("a sweep takes one seed per member config")
+            learner_kw['hparams'] = [a2c_hparams(c) for c in member_configs]
         if seeds is not None:
             learner_kw['seeds'] = seeds
             seed = int(seeds[0])
@@ -66,25 +100,12 @@ class IA2C:
             alpha=model_config.getfloat('rmsp_alpha'), eps=model_config.getfloat('rmsp_epsilon'),
             reward_norm=self.reward_norm, reward_clip=self.reward_clip, seed=seed, device=device, **learner_kw)
         if total_step:
-            self._init_scheduler(model_config)
+            self.lr_scheduler, self.beta_scheduler = a2c_schedulers(model_config, total_step)
+            if member_configs is not None:
+                self.lr_schedulers, self.beta_schedulers = (
+                    list(s) for s in zip(*(a2c_schedulers(c, total_step) for c in member_configs)))
         self._rng = np.random.RandomState(seed)
         self._obs_dev = torch.zeros(n_replicas, n_obs, device=self.batched.dev)
-
-    def _init_scheduler(self, model_config):                      # agents/models.py:53-69
-        lr_init = model_config.getfloat('lr_init')
-        lr_decay = model_config.get('lr_decay')
-        beta_init = model_config.getfloat('entropy_coef_init')
-        beta_decay = model_config.get('entropy_decay')
-        if lr_decay == 'constant':
-            self.lr_scheduler = Scheduler(lr_init, decay=lr_decay)
-        else:
-            self.lr_scheduler = Scheduler(lr_init, model_config.getfloat('LR_MIN'), self.total_step, decay=lr_decay)
-        if beta_decay == 'constant':
-            self.beta_scheduler = Scheduler(beta_init, decay=beta_decay)
-        else:
-            self.beta_scheduler = Scheduler(beta_init, model_config.getfloat('ENTROPY_COEF_MIN'),
-                                            self.total_step * model_config.getfloat('ENTROPY_RATIO'),
-                                            decay=beta_decay)
 
     # ---- reference protocol (lists in / lists out, one replica) ---------------------------------
     def _pack(self, obs: List[np.ndarray]) -> torch.Tensor:

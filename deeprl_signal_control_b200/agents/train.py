@@ -3,6 +3,7 @@
 
     train(config, base_dir, test_mode='no_test', n_replicas=1, policy='lstm', device=0, process_group=None,
           summaries=False)
+    train_sweep([a.ini, b.ini, ...], base_dir, ...)   (one member per config in one process, `train_sweep`)
 
 leaves the reference's agent directory: `data/` with a copy of the config and `train_reward.csv`, `model/checkpoint-<step>`
 and `log/<time>.log`; with `after_train_test` / `all_test` also `data/<scenario>_<agent>_{control,traffic,trip}.csv`;
@@ -286,11 +287,11 @@ def run_schedule(drivers):
 
 
 def build_model(agent, env, model_config, total_step, n_replicas, policy='lstm', seed=0, device=0, replica0=0,
-                total_replicas=None, process_group=None, seeds=None):
+                total_replicas=None, process_group=None, seeds=None, member_configs=None):
     """main.py:110-121 on the batched learners: IA2C / MA2C wrappers (seed = ENV_CONFIG.seed) or BatchedIQL (seed 0).
     `n_replicas` are this rank's replicas, the global ones [replica0, replica0 + n_replicas) of `total_replicas`; the
     learner all-reduces its gradient over `process_group` when one is given.  `seeds`: an A2C population, one member
-    per seed on n_replicas replicas each (`BatchedA2C`)."""
+    per seed on n_replicas replicas each (`BatchedA2C`); with `member_configs` (one [MODEL_CONFIG] per seed) a sweep."""
     kind, model_type = model_spec(agent)
     t = env._tables
     if kind != 'iql':
@@ -300,6 +301,8 @@ def build_model(agent, env, model_config, total_step, n_replicas, policy='lstm',
             kw.update(replica0=replica0, total_replicas=total_replicas, process_group=process_group)
         if seeds is not None:
             kw.update(seeds=seeds)
+        if member_configs is not None:
+            kw.update(member_configs=member_configs)
         if kind == 'ma2c':
             return MA2C(env.n_s_ls, env.n_a_ls, env.n_w_ls, env.n_f_ls, total_step, model_config, **kw)
         return IA2C(env.n_s_ls, env.n_a_ls, env.n_w_ls, total_step, model_config, **kw)
@@ -533,11 +536,7 @@ def train_population(config, base_dir, seeds, test_mode='no_test', n_replicas=1,
     log/<time>.log and, with `summaries`, the member's event file.  Returns a namespace like train()'s with per-member
     lists `dirs`, `data`, `post_test` and `members`."""
     import copy
-    import torch
-    from ..envs import make_env
-    from .evaluator import Evaluator
     from .learner import check_population
-    from .trainer import BatchedTrainer
     t0 = time.time()
     in_test, post_test = init_test_flag(test_mode)
     seeds = parse_seeds(','.join(str(int(x)) for x in seeds)) if not isinstance(seeds, str) else parse_seeds(seeds)
@@ -554,19 +553,37 @@ def train_population(config, base_dir, seeds, test_mode='no_test', n_replicas=1,
     if policy != 'lstm':
         raise ValueError("a population trains the LSTM policy only (got policy=%r)" % policy)
     check_population(seeds, 0, n_replicas, 1024, None)               # before any directory or device work
-    K, R_m = len(seeds), int(n_replicas)
-    cfgs, dirs, handlers = [], [], []
-    fmt = logging.Formatter('%(asctime)s [%(levelname)s] %(message)s')
-    for k, s in enumerate(seeds):
+    cfgs, dirs = [], []
+    for s in seeds:
         cfg = copy.deepcopy(config)
         cfg['ENV_CONFIG']['seed'] = str(s)
         d = init_dir(member_dir(base_dir, s, agent))
         with open(os.path.join(d['data'], name), 'w') as f:
             cfg.write(f)
+        cfgs.append(cfg); dirs.append(d)
+    out = _train_members(cfgs, dirs, agent, seeds, int(n_replicas), in_test, post_test, policy, device, summaries,
+                         'population of %d seeds %s' % (len(seeds), seeds))
+    out.dirs, out.wall_sec = [member_dir(base_dir, s, agent) for s in seeds], time.time() - t0
+    return out
+
+
+def _train_members(cfgs, dirs, agent, seeds, R_m, in_test, post_test, policy, device, summaries, what, sweep=False):
+    """The training run of a population or a sweep, member k from cfgs[k] (seed seeds[k]) into the agent directory
+    dirs[k] (init_dir's dict): member-tagged log files, one simulator and one learner for all K * R_m replicas, one
+    driver per member.  A sweep gives each member its own learner values and schedules (`IA2C(member_configs=...)`)
+    and, for ma2c, its own coop_gamma in the simulator."""
+    import torch
+    from ..envs import make_env
+    from .evaluator import Evaluator
+    from .trainer import BatchedTrainer
+    K = len(cfgs)
+    handlers = []
+    fmt = logging.Formatter('%(asctime)s [%(levelname)s] %(message)s')
+    for k, d in enumerate(dirs):
         h = logging.FileHandler(os.path.join(d['log'], '%d.log' % time.time()))
         h.setFormatter(fmt)
         h.addFilter(_member_filter(k))
-        cfgs.append(cfg); dirs.append(d); handlers.append(h)
+        handlers.append(h)
     handlers.append(logging.StreamHandler())
     handlers[-1].setFormatter(fmt)
     root = logging.getLogger()
@@ -574,13 +591,19 @@ def train_population(config, base_dir, seeds, test_mode='no_test', n_replicas=1,
         root.addHandler(h)
     root.setLevel(logging.INFO)
     writers = []
+    cg = [c['ENV_CONFIG'].getfloat('coop_gamma') for c in cfgs] if sweep and agent == 'ma2c' else None
+    if cg is not None and len(set(cg)) == 1:
+        cg = None                                                     # one coop_gamma: the simulator's own
+    # the training simulator marks the observation entries it scales only when built with a coop_gamma other than 1
+    base = next((k for k in range(K) if cg[k] != 1.0), 0) if cg is not None else 0
     try:
-        env_cfg, mc = cfgs[0]['ENV_CONFIG'], cfgs[0]['MODEL_CONFIG']
+        env_cfg, mc = cfgs[base]['ENV_CONFIG'], cfgs[0]['MODEL_CONFIG']
         env = make_env(env_cfg, K * R_m, dirs[0]['data'], is_record=False, device=device)
-        logging.info('Training: s dim: %d, s dim ls: %r, a dim ls: %r, population of %d seeds %s x %d replicas'
-                     % (env.n_s, env.n_s_ls, env.n_a_ls, K, seeds, R_m))
-        total_step, counter, T = _schedule(config, env)
-        model = build_model(agent, env, mc, total_step, R_m, seeds=seeds, device=device)
+        logging.info('Training: s dim: %d, s dim ls: %r, a dim ls: %r, %s x %d replicas'
+                     % (env.n_s, env.n_s_ls, env.n_a_ls, what, R_m))
+        total_step, counter, T = _schedule(cfgs[0], env)
+        model = build_model(agent, env, mc, total_step, R_m, seeds=seeds, device=device,
+                            member_configs=[c['MODEL_CONFIG'] for c in cfgs] if sweep else None)
         members = model.members()
         sim = env._ensure_sim()
         trace = torch.zeros(T, K * R_m, dtype=torch.float32, device=sim.device)
@@ -591,8 +614,9 @@ def train_population(config, base_dir, seeds, test_mode='no_test', n_replicas=1,
             srec = dict(summary_rec=torch.zeros(shape, dtype=torch.float32, device=sim.device))
             writers = [SummaryWriter(d['log']) for d in dirs]
             summ = [Summaries(w, summary_name(agent, policy), 'a2c', model.n_step) for w in writers]
-        trainer = BatchedTrainer(sim, model.batched, agent, model.lr_scheduler, model.beta_scheduler,
-                                 seed0=seeds[0], greward_trace=trace, **srec)
+        lr, beta = (model.lr_schedulers, model.beta_schedulers) if sweep else (model.lr_scheduler, model.beta_scheduler)
+        trainer = BatchedTrainer(sim, model.batched, agent, lr, beta, seed0=seeds[0], greward_trace=trace,
+                                 coop_gamma=cg, **srec)
         drivers = []
         for k in range(K):                  # one driver per member, over its view of the shared trainer
             evaluator = None
@@ -618,6 +642,117 @@ def train_population(config, base_dir, seeds, test_mode='no_test', n_replicas=1,
             h.close()
     return types.SimpleNamespace(final_step=counter.cur_step, episode_sets=drivers[0].n_episode_sets,
                                  env_samples=counter.cur_step * K * R_m, world=1, rank=0, seeds=seeds,
-                                 dirs=[member_dir(base_dir, s, agent) for s in seeds], data=[d.data for d in drivers],
-                                 post_test=post, model=model, members=members, trainer=trainer,
-                                 wall_sec=time.time() - t0)
+                                 data=[d.data for d in drivers], post_test=post, model=model, members=members,
+                                 trainer=trainer)
+
+
+# the config keys a sweep's members may set for themselves; every other key must be equal in all of them
+SWEEP_CONFIG_KEYS = {
+    'ENV_CONFIG': ('seed', 'coop_gamma'),
+    'MODEL_CONFIG': ('lr_init', 'lr_decay', 'lr_min', 'entropy_coef_init', 'entropy_decay', 'entropy_coef_min',
+                     'entropy_ratio', 'value_coef', 'max_grad_norm', 'rmsp_alpha', 'rmsp_epsilon', 'gamma',
+                     'reward_norm', 'reward_clip')}
+
+
+def _same(a, b):
+    """Two config values agree: equal text, or equal numbers (5e-4 and 0.0005)."""
+    if a == b:
+        return True
+    try:
+        return float(a) == float(b)
+    except (TypeError, ValueError):
+        return False
+
+
+def _value(cfg, sec, key):
+    return cfg.get(sec, key, fallback=None) if cfg.has_section(sec) else None
+
+
+def sweep_members(configs):
+    """The members of a sweep as [(name, ConfigParser, path or None)], checked.  `configs`: a list of config paths
+    (member name = file stem) or a dict name -> ConfigParser.  Refused with a ValueError: no config, repeated names, a
+    key outside SWEEP_CONFIG_KEYS that differs between two members (naming the key and both members), a coop_gamma that
+    differs under ia2c (the reference reads it only for ma2c, envs/env.py:184-188, 595-609), and two identical configs."""
+    if isinstance(configs, dict):
+        items = [(str(n), c, None) for n, c in configs.items()]
+    else:
+        items = []
+        for p in configs:
+            c = configparser.ConfigParser()
+            if not c.read(p):
+                raise FileNotFoundError(p)
+            items.append((os.path.splitext(os.path.basename(p))[0], c, p))
+    if not items:
+        raise ValueError('a sweep needs at least one config')
+    names = [n for n, _, _ in items]
+    if len(set(names)) != len(names):
+        raise ValueError('sweep member names must be distinct (got %s)' % names)
+    label = lambda i: items[i][2] or items[i][0]
+    c0 = items[0][1]
+    agent = _value(c0, 'ENV_CONFIG', 'agent')
+    for i in range(1, len(items)):
+        c = items[i][1]
+        for sec in sorted(set(c0.sections()) | set(c.sections())):
+            keys = set(c0[sec] if c0.has_section(sec) else ()) | set(c[sec] if c.has_section(sec) else ())
+            for key in sorted(keys):
+                a, b = _value(c0, sec, key), _value(c, sec, key)
+                if _same(a, b):
+                    continue
+                if key not in SWEEP_CONFIG_KEYS.get(sec, ()):
+                    raise ValueError('[%s] %s differs between %s (%s) and %s (%s): the members of a sweep may differ '
+                                     'only in %s' % (sec, key, label(0), a, label(i), b, SWEEP_CONFIG_KEYS))
+                if key == 'coop_gamma' and agent != 'ma2c':
+                    raise ValueError('[ENV_CONFIG] coop_gamma differs between %s and %s, but %s does not use it (only '
+                                     'ma2c does)' % (label(0), label(i), agent))
+        for j in range(i):
+            if all(_same(_value(items[j][1], sec, key), _value(c, sec, key))
+                   for sec, keys in SWEEP_CONFIG_KEYS.items() for key in keys):
+                raise ValueError('%s and %s are identical: a sweep trains each config once' % (label(j), label(i)))
+    return items
+
+
+def sweep_dir(base_dir, name, agent):
+    """The agent directory of the sweep member `name`: <base_dir>/<name>/<agent>."""
+    return os.path.join(base_dir, name, agent)
+
+
+def train_sweep(configs, base_dir, test_mode='no_test', n_replicas=64, device=0, summaries=False, policy='lstm',
+                process_group=None):
+    """Train a hyperparameter sweep of one A2C agent (ia2c / ma2c, LSTM policy) in one process: one member per config
+    (`sweep_members`: the configs may differ only in SWEEP_CONFIG_KEYS), each on `n_replicas` replicas (a multiple of
+    64).  One simulator launch and one grouped policy forward per control step cover all K * n_replicas replicas;
+    member k runs with its own seed, coop_gamma (ma2c), learner values and lr / entropy schedules, and trains what
+    `train(config_k, n_replicas=n_replicas)` trains alone.  Its directory `sweep_dir(base_dir, name_k, agent)` holds
+    what that run leaves: data/ (its config, train_reward.csv, test CSVs), model/checkpoint-<step>.npz, log/<time>.log
+    and, with `summaries`, its event file.  Everything is checked before any directory or device work.  Returns a
+    namespace like train_population's with `names`."""
+    from .learner import check_sweep
+    from .models import a2c_hparams
+    t0 = time.time()
+    in_test, post_test = init_test_flag(test_mode)
+    if process_group is not None:
+        raise ValueError('a sweep trains in one process: it takes no process_group')
+    items = sweep_members(configs)
+    agent = items[0][1]['ENV_CONFIG'].get('agent')
+    kind, _ = model_spec(agent)
+    if kind == 'iql':
+        raise ValueError("a sweep trains an A2C agent (ia2c or ma2c), not %r" % agent)
+    if policy != 'lstm':
+        raise ValueError("a sweep trains the LSTM policy only (got policy=%r)" % policy)
+    cfgs = [c for _, c, _ in items]
+    seeds = [c['ENV_CONFIG'].getint('seed') for c in cfgs]
+    check_sweep(seeds, [a2c_hparams(c['MODEL_CONFIG']) for c in cfgs], n_replicas, 1024, None)
+    names, dirs = [n for n, _, _ in items], []
+    for name, cfg, path in items:
+        d = init_dir(sweep_dir(base_dir, name, agent))
+        if path is not None:
+            shutil.copy(path, d['data'])                              # as train() copies its config
+        else:
+            with open(os.path.join(d['data'], 'config.ini'), 'w') as f:
+                cfg.write(f)
+        dirs.append(d)
+    out = _train_members(cfgs, dirs, agent, seeds, int(n_replicas), in_test, post_test, policy, device, summaries,
+                         'sweep of %d configs %s' % (len(cfgs), names), sweep=True)
+    out.names, out.dirs = names, [sweep_dir(base_dir, n, agent) for n in names]
+    out.wall_sec = time.time() - t0
+    return out

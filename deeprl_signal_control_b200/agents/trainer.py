@@ -71,10 +71,18 @@ class MemberTrainer:
         return None if rec is None else rec[:, self._k]
 
 
+def schedule_values(sched, n_step: int):
+    """The value(s) of a schedule for the next update: a float, an object with `get(n_step)`, or a list of either (one
+    per sweep member, each advanced by n_step as its solo run's)."""
+    if isinstance(sched, (list, tuple)):
+        return [schedule_values(s, n_step) for s in sched]
+    return sched.get(n_step) if hasattr(sched, "get") else sched
+
+
 class BatchedTrainer:
     def __init__(self, sim: BatchedSim, model: BatchedA2C, agent: str, lr, beta,
                  seed0: int = 12, replica0: int = 0, greward_trace: Optional[torch.Tensor] = None,
-                 summary_rec: Optional[torch.Tensor] = None):
+                 summary_rec: Optional[torch.Tensor] = None, coop_gamma=None):
         """lr / beta: floats (the 'constant' schedules of every shipped A2C config) or objects with the reference's
         `Scheduler.get(n_step)` (agents/utils.py:268-281, agents/models.py:175-176); a schedule advances by n_step per
         update exactly as in the reference (its unit is control steps of ONE environment).
@@ -85,7 +93,15 @@ class BatchedTrainer:
         row j with two device copies, so that the summaries of an episode need one read.  None: nothing is copied.
         A population learner (model.K > 1 members of model.R_m replicas) resets member k's replicas with its own seeds
         (`member_episode_seeds`; seed0 and replica0 are not used), keeps [T_episode / n_step, K, 4] records and appends
-        the list of the K members' episode means to `episode_rewards`."""
+        the list of the K members' episode means to `episode_rewards`.
+        A sweep (a learner with `hparams`) passes lr / beta as lists with one schedule per member (`schedule_values`),
+        and `coop_gamma`, one MA2C spatial discount per member: member k's replicas then step with its own
+        (BatchedSim.set_replica_coop_gamma)."""
+        if coop_gamma is not None:
+            K, R_m = int(getattr(model, "K", 1)), sim.R // int(getattr(model, "K", 1))
+            if len(coop_gamma) != K:
+                raise ValueError("coop_gamma takes one value per member (%d, got %d)" % (K, len(coop_gamma)))
+            sim.set_replica_coop_gamma(np.repeat(np.asarray(coop_gamma, np.float32), R_m))
         self.sim, self.model, self.agent = sim, model, agent
         self.lr, self.beta = lr, beta
         self.seed0, self.replica0 = int(seed0), int(replica0)
@@ -202,6 +218,7 @@ class BatchedTrainer:
         ranges are independent and the sampling RNG is keyed by the absolute replica.  The host still receives every
         range's observations / rewards in page-locked numpy buffers before the learner consumes them."""
         sim, m = self.sim, self.model
+        m._one_reward_scaling("the host-range pipeline")
         R, A, L = sim.R, m.lay.A, m.lay
         lib = _lib.lib()
         ma2c = self.agent == 'ma2c'
@@ -289,9 +306,7 @@ class BatchedTrainer:
         boot = None
         if not self.done:
             _, boot, _ = m.forward(m.obs_slot(m.T), False, out_type='v')    # utils.py:190
-        lr = self.lr.get(m.T) if hasattr(self.lr, "get") else self.lr
-        beta = self.beta.get(m.T) if hasattr(self.beta, "get") else self.beta
-        m.backward(boot, lr, beta)
+        m.backward(boot, schedule_values(self.lr, m.T), schedule_values(self.beta, m.T))
         if self.summary_rec is not None:
             j = self.step_in_episode // m.T - 1
             self.summary_rec[j, ..., :3].copy_(m.stats[..., :3])

@@ -327,6 +327,23 @@ __global__ void returns_kernel(const float* __restrict__ rew, const float* __res
   }
 }
 
+// returns_kernel of a sweep: element i belongs to member i / RA_m and discounts with gamma[member] (same expression,
+// so each member's rows equal returns_kernel run on them alone)
+__global__ void returns_g_kernel(const float* __restrict__ rew, const float* __restrict__ val,
+                                 const float* __restrict__ boot, const float* __restrict__ done_post,
+                                 const float* __restrict__ gammas, int64_t RA_m, int T, int64_t RA,
+                                 float* __restrict__ Rs, float* __restrict__ Adv) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= RA) return;
+  const float gamma = gammas[i / RA_m];
+  float Rv = boot[i];
+  for (int t = T - 1; t >= 0; --t) {
+    Rv = rew[(int64_t)t * RA + i] + gamma * Rv * (1.0f - done_post[t]);
+    Rs[(int64_t)t * RA + i] = Rv;
+    Adv[(int64_t)t * RA + i] = Rv - val[(int64_t)t * RA + i];
+  }
+}
+
 // ------------------------------------------------------------------------------------------------
 // Loss gradients at the heads.  grid (<= HL_GX row-tile walkers, A), 128 threads, thread = row m of a 128-row tile.
 // With `G` the head weight / bias gradients  dWo += H^T dlog,  dbo += sum dlog  are accumulated here too
@@ -1122,6 +1139,18 @@ extern "C" int tscl_returns(tscl_handle* h, const float* rew, const float* val, 
   return 0;
 }
 
+extern "C" int tscl_returns_g(tscl_handle* h, const float* rew, const float* val, const float* boot,
+                              const float* done_post, const float* gamma, int32_t K, int32_t T, int64_t R, float* Rs,
+                              float* Adv, void* stream) {
+  if (!h || !gamma || K <= 0 || R <= 0 || R % K) return tsc_set_error("tscl_returns_g: bad argument");
+  LCK(cudaSetDevice(h->device));
+  const int64_t RA = R * h->d.A;
+  returns_g_kernel<<<(unsigned)((RA + 255) / 256), 256, 0, (cudaStream_t)stream>>>(rew, val, boot, done_post, gamma,
+                                                                                    RA / K, T, RA, Rs, Adv);
+  LCK(cudaGetLastError());
+  return 0;
+}
+
 extern "C" int tscl_heads_loss(tscl_handle* h, const float* params, const float* H, const int32_t* act,
                                const float* Rs, const float* Adv, int64_t M, int64_t Rc, int64_t stride_t,
                                float v_coef, float beta, float scale, float* dlog, float* dH, float* stats,
@@ -1241,6 +1270,38 @@ extern "C" int tscl_device_transition(tscl_handle* h, const float* rew_dev, floa
   LCK(cudaSetDevice(h->device));
   host_transition_kernel<<<(unsigned)((rew_floats + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
       rew_dev, rew_hist_dev, rew_floats, reward_norm != 0.f ? 1.0f / reward_norm : 0.f, reward_clip, grew_dev, rew_acc_dev, n);
+  LCK(cudaGetLastError());
+  return 0;
+}
+
+// the device hand-over of a sweep: reward element i belongs to member i / n_rew_m and takes that member's norm / clip
+// with host_transition_kernel's arithmetic (1 / norm rounded once, 0 = off); the global rewards are only summed
+__global__ void device_transition_g_kernel(const float* __restrict__ rew_in, float* __restrict__ rew_hist, int64_t n_rew,
+                                           int64_t n_rew_m, const float* __restrict__ norms,
+                                           const float* __restrict__ clips, const float* __restrict__ grew_in,
+                                           float* __restrict__ rew_acc, int64_t n) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n_rew) {
+    const int k = (int)(i / n_rew_m);
+    const float norm = norms[k], clip = clips[k];
+    const float inv_norm = norm != 0.f ? __frcp_rn(norm) : 0.f;    // = the host's 1.0f / reward_norm
+    float r = rew_in[i];
+    if (inv_norm != 0.f) r = r * inv_norm;
+    if (clip > 0.f) r = fminf(fmaxf(r, -clip), clip);
+    rew_hist[i] = r;
+  }
+  if (i < n) rew_acc[i] += grew_in[i];
+}
+
+extern "C" int tscl_device_transition_g(tscl_handle* h, const float* rew_dev, float* rew_hist_dev, int64_t rew_floats,
+                                        const float* reward_norm, const float* reward_clip, int32_t K,
+                                        const float* grew_dev, float* rew_acc_dev, int64_t n, void* stream) {
+  if (!h || !rew_dev || !rew_hist_dev || !grew_dev || !rew_acc_dev || !reward_norm || !reward_clip || K <= 0 ||
+      rew_floats <= 0 || n <= 0 || n > rew_floats || rew_floats % K || n % K)
+    return tsc_set_error("tscl_device_transition_g: bad argument");
+  LCK(cudaSetDevice(h->device));
+  device_transition_g_kernel<<<(unsigned)((rew_floats + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
+      rew_dev, rew_hist_dev, rew_floats, rew_floats / K, reward_norm, reward_clip, grew_dev, rew_acc_dev, n);
   LCK(cudaGetLastError());
   return 0;
 }

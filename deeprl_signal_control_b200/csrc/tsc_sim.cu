@@ -98,6 +98,7 @@ struct StepArgs {
   float* reward;
   float* greward;
   uint8_t* done;
+  const float* cg;    // [R] per-replica coop_gamma (tsc_set_replica_coop_gamma) or null: cfg.coop_gamma / obs_scale_val
 };
 
 // ------------------------------------------------------------------------------------------------
@@ -776,7 +777,8 @@ tsc_step_kernel(const StepArgs A) {
         } else {
           rw = s_loc[i];
           const int q0 = __ldg(&n.node_nbr_off[i]), q1 = __ldg(&n.node_nbr_off[i + 1]);
-          for (int q = q0; q < q1; ++q) rw = rw + c.coop_gamma * s_loc[__ldg(&n.node_nbr[q])];
+          const float cg = A.cg ? __ldg(&A.cg[rep]) : c.coop_gamma;
+          for (int q = q0; q < q1; ++q) rw = rw + cg * s_loc[__ldg(&n.node_nbr[q])];
           if (c.real_net_norm) rw = rw / ((float)(1 + q1 - q0) * 20.0f);
         }
         A.reward[(size_t)rep * N + i] = rw;
@@ -791,6 +793,7 @@ tsc_step_kernel(const StepArgs A) {
     __syncthreads();
     const float* fp = A.fp ? A.fp + (size_t)rep * N * n.max_na : nullptr;
     float* o = A.obs + (size_t)rep * n.n_obs;
+    const float sv = A.cg ? __ldg(&A.cg[rep]) : n.obs_scale_val;
     for (int k = tid; k < n.n_obs; k += TSC_THREADS) {
       const uint32_t pw = __ldg(&n.obs_prog[k]);
       const int kind = (int)(pw & 3u), idx = (int)(pw >> 3);
@@ -798,7 +801,7 @@ tsc_step_kernel(const StepArgs A) {
       if (kind == 0) v = s_obsv[idx];
       else if (kind == 1) v = s_obsv[n.n_det + idx];
       else v = fp ? fp[idx] : 0.0f;
-      o[k] = ((pw & 4u) ? n.obs_scale_val : 1.0f) * v;      // same product as obs_scale[k] * v
+      o[k] = ((pw & 4u) ? sv : 1.0f) * v;      // same product as obs_scale[k] * v
     }
   }
   if (A.n_sub == 0) return;  // observe only: state untouched
@@ -938,6 +941,7 @@ struct tsc_handle {
   int32_t* d_action = nullptr; float* d_fp = nullptr; float* d_obs = nullptr; float* d_reward = nullptr;
   float* d_greward = nullptr; uint8_t* d_done = nullptr;
   unsigned long long* d_scalar = nullptr;
+  float* d_cg = nullptr;     // per-replica coop_gamma (tsc_set_replica_coop_gamma), allocated on first use
   int n_nodes = 0, n_obs = 0, max_na = 0, n_det = 0;
   int meas_words = 0;
   // greedy program (tsc_set_greedy_program): CSR over (node, candidate) of observation offsets + action per candidate
@@ -1110,6 +1114,17 @@ extern "C" int tsc_reset(tsc_handle* h, const uint64_t* seeds_host, void* stream
 extern "C" int tsc_set_train_mode(tsc_handle* h, int32_t m) {
   if (!h) return fail("tsc_set_train_mode: null handle");
   h->args.train_mode = m ? 1 : 0;
+  return 0;
+}
+
+extern "C" int tsc_set_replica_coop_gamma(tsc_handle* h, const float* cg_host) {
+  if (!h) return fail("tsc_set_replica_coop_gamma: null handle");
+  if (!cg_host) { h->args.cg = nullptr; return 0; }
+  CK(cudaSetDevice(h->device));
+  if (!h->d_cg && dalloc(h, (size_t)h->R, &h->d_cg)) return -1;
+  CK(cudaDeviceSynchronize());          // no launch in flight still reads the previous values
+  CK(cudaMemcpy(h->d_cg, cg_host, (size_t)h->R * 4, cudaMemcpyHostToDevice));
+  h->args.cg = h->d_cg;
   return 0;
 }
 

@@ -66,6 +66,22 @@ class BatchedSim:
     def set_train_mode(self, train: bool) -> None:
         _lib.check(_lib.lib().tsc_set_train_mode(self._h, C.c_int32(int(train))))
 
+    def set_replica_coop_gamma(self, values=None) -> None:
+        """MA2C spatial discount per replica (`tsc_set_replica_coop_gamma`): `values` [R] floats, replica r then steps as
+        a simulator built with coop_gamma = values[r]; None returns to the configured coop_gamma.  The scaled observation
+        entries are the ones the network was built to scale, so a network built with coop_gamma = 1 (none scaled) takes
+        only values of 1."""
+        if values is None:
+            _lib.check(_lib.lib().tsc_set_replica_coop_gamma(self._h, None))
+            return
+        cg = np.ascontiguousarray(values, dtype=np.float32)
+        if cg.shape != (self.R,):
+            raise ValueError("set_replica_coop_gamma takes %d values (got shape %s)" % (self.R, cg.shape))
+        if not (np.asarray(self.net.obs_scale) != 1.0).any() and (cg != 1.0).any() and self.params.agent == "ma2c":
+            raise ValueError("the network was built with coop_gamma = 1, so no observation entry is scaled; build it "
+                             "with a coop_gamma other than 1")
+        _lib.check(_lib.lib().tsc_set_replica_coop_gamma(self._h, _np(cg, C.c_float)))
+
     def observe(self, fp: Optional[torch.Tensor] = None, obs_out: Optional[torch.Tensor] = None) -> torch.Tensor:
         obs = self.obs if obs_out is None else obs_out
         _lib.check(_lib.lib().tsc_observe(self._h, _ptr(fp), _ptr(obs), self._stream()))

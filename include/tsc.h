@@ -133,6 +133,14 @@ int tsc_reset(tsc_handle* h, const uint64_t* seeds_host, void* stream);
  * envs/env.py:591-592). */
 int tsc_set_train_mode(tsc_handle* h, int32_t train_mode);
 
+/* Per-replica MA2C spatial discount (a hyperparameter sweep over coop_gamma in one simulator): cg_host [R] host floats,
+ * copied (synchronous).  While set, replica r uses cg_host[r] wherever the process-wide cfg->coop_gamma applies: the
+ * neighbour sum of the ma2c reward (envs/env.py:595-609) and the scale of the observation entries the network was
+ * built to scale (neighbour waves, envs/env.py:184-188); every step / observe / record / host-range call reads it.
+ * Replica r is then bit-identical to a simulator built with coop_gamma = cg_host[r] (the network must have been built
+ * with a coop_gamma != 1, else no observation entry is marked as scaled).  NULL returns to cfg->coop_gamma. */
+int tsc_set_replica_coop_gamma(tsc_handle* h, const float* cg_host);
+
 /* Replaces _get_state() without stepping (the observation reset() returns,
  * envs/env.py:561,163-205).  fp_dev: [R][n_nodes][max_na] policy probabilities installed by
  * update_fingerprint (envs/env.py:633-635) or NULL (zeros).  obs_dev: [R][n_obs]. */

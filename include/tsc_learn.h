@@ -89,6 +89,10 @@ int tscl_heads(tscl_handle* h, const float* params, const float* Hs, int64_t R, 
  *   rew,val,Rs,Adv [T][R][A]; boot [R][A]; done_post [T] float */
 int tscl_returns(tscl_handle* h, const float* rew, const float* val, const float* boot, const float* done_post,
                  float gamma, int32_t T, int64_t R, float* Rs, float* Adv, void* stream);
+/* tscl_returns for a sweep of K members of R / K replicas each (K must divide R): replica r discounts with the device
+ * float gamma[r / (R / K)].  Each member's rows of Rs / Adv equal tscl_returns run on those rows alone with its gamma. */
+int tscl_returns_g(tscl_handle* h, const float* rew, const float* val, const float* boot, const float* done_post,
+                   const float* gamma, int32_t K, int32_t T, int64_t R, float* Rs, float* Adv, void* stream);
 
 /* Loss gradients at the heads for all (t, r) of a chunk (agents/policies.py:41-52):
  *   H [2A][M][h], act/Rs/Adv rows m -> base + (m / Rc)*stride_t + (m % Rc)*A
@@ -163,6 +167,11 @@ int tscl_host_transition(tscl_handle* h, const float* obs_host, float* obs_dev, 
  * reward_norm), rew_acc_dev += grew_dev, one launch. */
 int tscl_device_transition(tscl_handle* h, const float* rew_dev, float* rew_hist_dev, int64_t rew_floats, float reward_norm,
                            float reward_clip, const float* grew_dev, float* rew_acc_dev, int64_t n, void* stream);
+/* The same for a sweep of K members (K divides rew_floats and n): reward element i is member i / (rew_floats / K)'s and
+ * is scaled with the device floats reward_norm[k] / reward_clip[k] (0 = off), with tscl_device_transition's arithmetic. */
+int tscl_device_transition_g(tscl_handle* h, const float* rew_dev, float* rew_hist_dev, int64_t rew_floats,
+                             const float* reward_norm, const float* reward_clip, int32_t K, const float* grew_dev,
+                             float* rew_acc_dev, int64_t n, void* stream);
 /* cudaMemcpyAsync on a caller-supplied stream; kind 1 = host->device, 2 = device->host, 3 = device->device */
 int tscl_memcpy_async(tscl_handle* h, void* dst, const void* src, int64_t bytes, int32_t kind, void* stream);
 /* dX = dZ . Wx^T as a stand-alone streaming product (the shipping path; reference: tf.gradients through

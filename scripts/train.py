@@ -3,7 +3,7 @@ device-resident learners (deeprl_signal_control_b200/agents/train.py).
 
   python scripts/train.py --base-dir DIR train --config-dir CFG.ini
                           [--test-mode no_test|in_train_test|after_train_test|all_test] [--replicas N] [--policy lstm|fc]
-                          [--summaries] [--seeds 12,13,14,15]
+                          [--summaries] [--seeds 12,13,14,15 | --sweep a.ini,b.ini,...]
   torchrun --nproc-per-node W scripts/train.py --base-dir DIR train --config-dir CFG.ini --replicas N
                           [--backend nccl|gloo] ...
 
@@ -26,6 +26,12 @@ the directory and prints the JSON line, with "world": W; the run plays the episo
 on `--replicas` replicas (a multiple of 64), all in one lock-step.  Member s gets the complete agent directory
 DIR/seed<s>/<agent>/ of a one-seed run, so `scripts/evaluate.py --agent-dir DIR/seed<s>/<agent>` reads it.  ia2c / ma2c
 with the LSTM policy only, and not under torchrun.  The JSON line gains "seeds".
+
+`--sweep a.ini,b.ini,...` trains a hyperparameter sweep in one process: one member per config, each on `--replicas`
+replicas (a multiple of 64), all in one lock-step.  The configs may differ only in [ENV_CONFIG] seed / coop_gamma (ma2c)
+and the [MODEL_CONFIG] learning-rate, entropy, value / gradient-norm, RMSProp, gamma and reward-scaling keys
+(agents/train.py: SWEEP_CONFIG_KEYS).  Member a.ini gets the complete agent directory DIR/a/<agent>/ of
+`train --config-dir a.ini`.  Not with --seeds, and not under torchrun.  The JSON line gains "members".
 """
 import argparse
 import datetime
@@ -56,10 +62,18 @@ def parse_args(argv=None):
                     help="gradient all-reduce backend under torchrun (default nccl)")
     sp.add_argument("--seeds", default=None,
                     help="comma-separated seeds: train one population member per seed into DIR/seed<s>/<agent>/")
+    sp.add_argument("--sweep", default=None,
+                    help="comma-separated configs: train one sweep member per config into DIR/<config stem>/<agent>/")
     a = p.parse_args(argv)
     if not a.option:
         p.print_help()
         raise SystemExit(1)
+    if a.sweep is not None:
+        if a.seeds is not None:
+            p.error("--sweep and --seeds exclude each other (a sweep takes each member's seed from its config)")
+        a.sweep = [x.strip() for x in a.sweep.split(",") if x.strip()]
+        if not a.sweep:
+            p.error("--sweep needs at least one config")
     if a.seeds is not None:
         from deeprl_signal_control_b200.agents.train import parse_seeds
         try:
@@ -72,6 +86,15 @@ def parse_args(argv=None):
 def main(argv=None):
     a = parse_args(argv)
     world = int(os.environ.get("WORLD_SIZE", "1"))
+    if a.sweep is not None:
+        if world > 1:
+            raise SystemExit("--sweep trains a sweep in one process; it does not run under torchrun")
+        from deeprl_signal_control_b200.agents.train import train_sweep
+        out = train_sweep(a.sweep, a.base_dir, a.test_mode, n_replicas=a.replicas, summaries=a.summaries,
+                          policy=a.policy)
+        print(json.dumps({"final_step": out.final_step, "episode_sets": out.episode_sets, "members": out.names,
+                          "env_samples": out.env_samples, "replicas": a.replicas, "wall_sec": round(out.wall_sec, 3)}))
+        return out
     if a.seeds is not None:
         if world > 1:
             raise SystemExit("--seeds trains a population in one process; it does not run under torchrun")
