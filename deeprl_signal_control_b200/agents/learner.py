@@ -252,6 +252,11 @@ class BatchedA2C:
         self.dx_fc_fused = paths.dx_fc_fused
         self.bwd_tc, self.fc_bwd_tc, self.wgrad_tc = paths.bwd_tc, paths.fc_bwd_tc, paths.wgrad_tc
         self.fused_heads = True                                  # head weight gradients inside tscl_heads_loss
+        # on the lean path the BPTT kernel computes the loss gradients at the heads itself (tscl_lstm_seq_bwd_tc_heads:
+        # same dZ bits, no fp32 dH round trip) and, for one member, runs once over every chunk; TSC_BPTT_HEADS=0 restores
+        # tscl_heads_loss + one tscl_lstm_seq_bwd_tc per chunk (A/B measurements)
+        self.heads_in_bptt = os.environ.get("TSC_BPTT_HEADS", "1") != "0"
+        self._dz_all = None
         self.pack_weights()
         # bf16 activation store of the rollout's own forward pass (written by the v2 kernel): the update then
         # back-propagates through it instead of recomputing fc + gate GEMM + LSTM forward.
@@ -495,19 +500,21 @@ class BatchedA2C:
         self.done_post[t] = 1.0 if done_post else 0.0
         self.t += 1
 
-    def _bufs(self, rc, lean=False, dxb=True):
+    def _bufs(self, rc, lean=False, dxb=True, dh=True, dzb=True):
         """Work buffers of one update chunk.  `lean`: every consumer reads the bf16 activation store itself and dZ / dX
         travel as bf16 between the tensor-core kernels, so only dH (fp32), dZb and dXb (bf16) exist (dXb only with
-        `dxb`: the fused dX / fc kernel never writes dX); the fp32 set is allocated the first time a fallback path
-        needs it."""
+        `dxb`: the fused dX / fc kernel never writes dX; dH only with `dh`: not when the BPTT computes it; dZb only with
+        `dzb`: not when one BPTT launch writes every chunk's dZ); the fp32 set is allocated the first time a fallback
+        path needs it."""
         L, T, U = self.lay, self.T, self.lay.U
         f32 = dict(dtype=torch.float32, device=self.dev)
         if self._upd_bufs is None or self._upd_bufs["rc"] < rc:
-            M = T * rc
-            self._upd_bufs = dict(rc=rc, dH=torch.empty(U, M, L.h, **f32))
+            self._upd_bufs = dict(rc=rc)
         b = self._upd_bufs
         M = T * b["rc"]
-        if lean and "dZb" not in b:
+        if (dh or not lean) and "dH" not in b:
+            b["dH"] = torch.empty(U, M, L.h, **f32)
+        if lean and dzb and "dZb" not in b:
             b["dZb"] = torch.empty(U, M, 4 * L.h, dtype=torch.bfloat16, device=self.dev)
         if lean and dxb and "dXb" not in b:
             b["dXb"] = torch.empty(U, M, L.dx, dtype=torch.bfloat16, device=self.dev)
@@ -516,6 +523,30 @@ class BatchedA2C:
                      X=torch.empty(U, M, L.dx, **f32), C=torch.empty(U, M, L.h, **f32), H=torch.empty(U, M, L.h, **f32),
                      Hp=torch.empty(U, M, L.h, **f32), dlog=torch.empty(U, M, L.max_na, **f32))
         return b
+
+    def _dz_all_buf(self):
+        """bf16 dZ of every chunk [R/chunk][U][T * chunk][4h] (one BPTT launch per update), or None when it does not fit
+        in half of the free device memory (the activation store's rule)."""
+        if self._dz_all is None:
+            L, nc = self.lay, self.R // self.chunk
+            need = nc * L.U * self.T * self.chunk * 4 * L.h * 2
+            free, _ = torch.cuda.mem_get_info(self.dev)
+            if need >= 0.5 * free:
+                return None
+            if self._upd_bufs is not None:          # the per-chunk dZ buffer is not needed beside it
+                self._upd_bufs.pop("dZb", None)
+            self._dz_all = torch.empty(nc, L.U, self.T * self.chunk, 4 * L.h, dtype=torch.bfloat16, device=self.dev)
+        return self._dz_all
+
+    def _bwd_heads(self, P, G, Wt, stats, r0, n_chunks, v_coef, beta, scale, dpre, dZb):
+        """tscl_lstm_seq_bwd_tc_heads over `n_chunks` chunks of the store from replica r0: loss gradients at the heads and
+        BPTT in one kernel, dZ (bf16) into dZb, head weight gradients into G, agent 0's loss sums into stats."""
+        ci, R, A = r0 // self.chunk, self.R, self.lay.A
+        _lib.check(_lib.lib().tscl_lstm_seq_bwd_tc_heads(
+            self._h, _p(Wt), _p(P), _p(self.st_g[ci]), _p(self.st_c[ci]), _p(self.st_h[ci]), _p(self.c_bw), _p(dpre),
+            _p(self.act_hist[0, r0:]), _p(self.Rs[0, r0:]), _p(self.Adv[0, r0:]), C.c_int32(self.T),
+            C.c_int64(self.chunk), C.c_int32(n_chunks), C.c_int64(R), C.c_int64(r0), C.c_int64(R * A), C.c_float(v_coef),
+            C.c_float(beta), C.c_float(scale), _p(dZb), _p(stats), _p(G), self._st()))
 
     def backward(self, boot: Optional[torch.Tensor], lr: float, beta: float):
         """One A2C update from the stored n_step rollout (agents/models.py:174-183).  `boot` is the
@@ -549,6 +580,13 @@ class BatchedA2C:
         n_obs = L.n_obs
         P, G, Wt, Wxt, stats = self.P, self.G, self.Wt, self.Wxt, self.stats
         k = 0
+        lean = use_store and self.bwd_tc and self.fc_bwd_tc and self.wgrad_tc and self.fused_heads
+        heads_bptt = lean and self.heads_in_bptt and not (self.dx_fused and self.dx_fusable)
+        # one BPTT launch over every chunk (one member, and the all-chunk dZ fits); else one per chunk, the same bits
+        dz_all = self._dz_all_buf() if heads_bptt and self.K == 1 and R > self.chunk else None
+        if dz_all is not None:
+            self._bwd_heads(P, G, Wt, stats, 0, R // self.chunk, self.hp[0]["v_coef"], betas[0], scale, dpre, dz_all)
+            self.kernel_launches += 1
         for r0 in range(0, R, self.chunk):
             if self.K > 1:        # the member of this chunk: its weights, images, gradient and loss terms
                 k = r0 // self.R_m
@@ -556,16 +594,16 @@ class BatchedA2C:
             rc = min(self.chunk, R - r0)
             M = T * rc
             ci = r0 // self.chunk
-            all_tc = use_store and self.bwd_tc and self.fc_bwd_tc and self.wgrad_tc and self.fused_heads
+            all_tc = lean
             fuse_dx = all_tc and self.dx_fused and self.dx_fusable   # dX = dZ . Wx^T inside the BPTT kernel (second MMA per step)
             fuse_fc = all_tc and not fuse_dx and self.dx_fc_fused    # dX inside the fc weight-gradient kernel, never stored
-            b = self._bufs(rc, lean=all_tc, dxb=not fuse_fc)
-            X = Cc = H = Hp = dlog = ZG = dX = dZb = dXb = None
+            b = self._bufs(rc, lean=all_tc, dxb=not fuse_fc, dh=not heads_bptt, dzb=dz_all is None)
+            X = Cc = H = Hp = dlog = ZG = dX = dZb = dXb = dH = None
             bf16 = dict(dtype=torch.bfloat16, device=self.dev)
             if b["rc"] == rc:
-                dH = b["dH"]
+                dH = b.get("dH")
                 if all_tc:
-                    dZb, dXb = b["dZb"], b.get("dXb")
+                    dZb, dXb = (b["dZb"] if dz_all is None else dz_all[ci]), b.get("dXb")
                 else:
                     ZG, dX, X, Cc, H, Hp, dlog = (b[k] for k in ("ZG", "dX", "X", "C", "H", "Hp", "dlog"))
             else:               # tail chunk: dense temporaries of the right shape
@@ -595,17 +633,25 @@ class BatchedA2C:
                                                  _p(self.h_bw), None, None, _p(dpre), C.c_int32(T), C.c_int64(rc),
                                                  C.c_int64(R), C.c_int64(r0), st()))
             hb = _p(self.st_h[ci]) if use_store else None
-            _lib.check(lib.tscl_heads_loss(self._h, _p(P), None if all_tc else _p(H), _p(self.act_hist[0, r0:]),
-                                           _p(self.Rs[0, r0:]), _p(self.Adv[0, r0:]), C.c_int64(M), C.c_int64(rc),
-                                           C.c_int64(R * A), C.c_float(self.hp[k]["v_coef"]), C.c_float(betas[k]),
-                                           C.c_float(scale),
-                                           None if self.fused_heads else _p(dlog), _p(dH), _p(stats),
-                                           hb if all_tc else None, _p(G) if self.fused_heads else None, st()))
+            if heads_bptt:      # heads + BPTT in one kernel (already run for every chunk when dz_all is set)
+                if dz_all is None:
+                    self._bwd_heads(P, G, Wt, stats, r0, 1, self.hp[k]["v_coef"], betas[k], scale, dpre, dZb)
+                    self.kernel_launches += 1
+            else:
+                _lib.check(lib.tscl_heads_loss(self._h, _p(P), None if all_tc else _p(H), _p(self.act_hist[0, r0:]),
+                                               _p(self.Rs[0, r0:]), _p(self.Adv[0, r0:]), C.c_int64(M), C.c_int64(rc),
+                                               C.c_int64(R * A), C.c_float(self.hp[k]["v_coef"]), C.c_float(betas[k]),
+                                               C.c_float(scale),
+                                               None if self.fused_heads else _p(dlog), _p(dH), _p(stats),
+                                               hb if all_tc else None, _p(G) if self.fused_heads else None, st()))
+                self.kernel_launches += 2
             if not self.fused_heads:
                 # head weight / bias gradients (plain batched GEMM + column sums)
                 self.gv["wo"].baddbmm_(H.transpose(1, 2), dlog)
                 self.gv["bo"].add_(dlog.sum(dim=1))
-            if self.bwd_tc:
+            if heads_bptt:
+                pass
+            elif self.bwd_tc:
                 gb = (_p(self.st_g[ci]), _p(self.st_c[ci])) if use_store else (None, None)
                 _lib.check(lib.tscl_lstm_seq_bwd_tc_dx(self._h, _p(Wt), _p(ZG), _p(Cc), _p(dH), _p(self.c_bw),
                                                        _p(dpre), C.c_int32(T), C.c_int64(rc), C.c_int64(R), C.c_int64(r0),
@@ -649,7 +695,7 @@ class BatchedA2C:
             else:
                 _lib.check(lib.tscl_fc_bwd(self._h, _p(obs0), _p(X), _p(dX), C.c_int64(M), C.c_int64(rc),
                                            C.c_int64(R * n_obs), _p(G), st()))
-            self.kernel_launches += 3 if fuse_fc else 4 if use_store else 5
+            self.kernel_launches += 1 if fuse_fc else 2 if use_store else 3     # heads / BPTT counted above
         if self.pg is not None:
             _dist.allreduce_sum_(self.G, self.pg)
         for k in range(self.K):

@@ -1242,6 +1242,16 @@ struct BwdTC {
   __nv_bfloat16* dZb;        // optional: dZ as bf16 [2A][T*Rc][256] (operand of the tensor-core weight-gradient kernels);
                              //           ZG may then be null (needs Gb / Cb)
   unsigned long long* prof;  // optional: phase counters of lstm_bwd_tc_regs_kernel (tscl_debug_bptt_prof)
+  // lstm_bwd_tc_regs_kernel<., true> (tscl_lstm_seq_bwd_tc_heads): dH from h_t and the heads instead of a dH tensor
+  const float* P;            // parameters (head weights / biases at off_wo / off_bo)
+  const int32_t* act;        // [T][..][A] at the first chunk's first replica, row (t, r, a) at t * stride_t + r * A + a
+  const float* Rs;
+  const float* Adv;
+  int64_t stride_t;
+  float v_coef, beta, scale;
+  float* stats;              // optional: agent 0's loss sums (policy, value, entropy) x scale
+  float* G;                  // head weight / bias gradients are added here
+  int n_chunks;              // consecutive chunks of Rc replicas ([n_chunks][2A][T][Rc][w] store blocks)
 };
 
 // NT = 512: thread = (replica row, 16 hidden units), one CTA per SM.
@@ -1488,9 +1498,162 @@ __device__ __forceinline__ void tma_store_3d(const CUtensorMap* m, int x, int y,
                ::"l"(reinterpret_cast<uint64_t>(m)), "r"(x), "r"(y), "r"(z), "r"(src) : "memory");
 }
 
+// Loss gradients at the heads for one step of a warpgroup of lstm_bwd_tc_regs_kernel<., true>: the thread's rows
+// rr0, rr0 + 8 of the chunk (rg0, rg0 + 8 of the update), h_t in the swizzled tile sH.  Writes dht = dH + dhc for the
+// thread's 16 units (the register layout of the kernel), the rows' dlog into sDl (value unit: dv in slot 0) and adds
+// agent 0's loss terms.  The per-row arithmetic is heads_loss_kernel's (tsc_learn.cu), expression for expression.
+__device__ __forceinline__ void heads_step(const DDimsTC& d, const BwdTC& a, const unsigned char* sH, const float* sHW,
+                                           float* sDl, bool pol, int ag, int na, int rq, int rr0, int lane, int q,
+                                           int64_t rg0, int t, const float (&dhc)[8][4], float (&dht)[8][4], float& pl,
+                                           float& vl, float& el) {
+  constexpr int HB_DL = 12;
+  const float* sWp = sHW;                  // [64][8]
+  const float* sWv = sHW + 512;            // [64]
+  const float* sBo = sHW + 576;            // [8]
+  bool valid[2];
+  int64_t io[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    valid[h] = rr0 + 8 * h < a.Rc;
+    io[h] = valid[h] ? (int64_t)t * a.stride_t + (rg0 + 8 * h) * d.A + ag : 0;
+  }
+  auto row8 = [&](int h, int c, float* x) {   // h[row rq + 8 h][8 c .. 8 c + 7] as fp32
+    const uint4 v = *reinterpret_cast<const uint4*>(sH + (rq + 8 * h) * 128 + ((c ^ (rq & 7)) << 4));
+    const uint32_t wv[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+    for (int i = 0; i < 4; ++i) { x[2 * i] = __uint_as_float(wv[i] << 16); x[2 * i + 1] = __uint_as_float(wv[i] & 0xffff0000u); }
+  };
+  if (pol) {
+    // logits 2 q, 2 q + 1 of both rows: each its own sequential chain over k
+    float l[2][2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) { l[h][0] = sBo[2 * q]; l[h][1] = sBo[2 * q + 1]; }
+#pragma unroll
+    for (int c = 0; c < 8; ++c) {
+      float x[2][8];
+      row8(0, c, x[0]); row8(1, c, x[1]);
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        const float2 wv = *reinterpret_cast<const float2*>(sWp + (8 * c + e) * 8 + 2 * q);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) { l[h][0] = fmaf(x[h][e], wv.x, l[h][0]); l[h][1] = fmaf(x[h][e], wv.y, l[h][1]); }
+      }
+    }
+    float dl[2][8];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float lg[8];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) lg[j] = __shfl_sync(0xffffffffu, l[h][j & 1], (lane & ~3) | (j >> 1));
+#pragma unroll
+      for (int j = 0; j < 8; ++j) dl[h][j] = 0.f;
+      if (valid[h]) {
+        float mx = -1e30f;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) if (j < na) mx = fmaxf(mx, lg[j]);
+        float s = 0.f;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) { lg[j] = j < na ? __expf(lg[j] - mx) : 0.f; s += lg[j]; }
+        const float inv = 1.0f / s;
+        const int at = a.act[io[h]];
+        const float adv = a.Adv[io[h]];
+        // log(clip(pi, 1e-10, 1)) and its gradient: see heads_loss_kernel
+        float lp[8], ent = 0.f, clip_mass = 0.f;
+        bool in_at = true;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          lg[j] *= inv;                                             // pi_j
+          lp[j] = j < na ? __logf(fminf(fmaxf(lg[j], 1e-10f), 1.0f)) : 0.f;
+          ent -= lg[j] * lp[j];
+          const bool clipped = j < na && !(lg[j] >= 1e-10f && lg[j] <= 1.0f);
+          if (clipped) clip_mass += lg[j];
+          if (clipped && j == at) in_at = false;
+        }
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          float g = 0.f;
+          if (j < na) {
+            const bool clipped = !(lg[j] >= 1e-10f && lg[j] <= 1.0f);
+            const float pg = in_at ? -adv * ((j == at ? 1.f : 0.f) - lg[j]) : 0.f;
+            g = a.scale * (pg + a.beta * lg[j] * (lp[j] + ent + clip_mass - (clipped ? 1.f : 0.f)));
+          }
+          dl[h][j] = g;
+        }
+        if (ag == 0 && q == 0) {
+#pragma unroll
+          for (int j = 0; j < 8; ++j) if (j == at) pl += -lp[j] * adv;
+          el += -a.beta * ent;
+        }
+      }
+      float s0 = 0.f, s1 = 0.f;              // this thread's share of the staging row: dlog 2 q, 2 q + 1
+#pragma unroll
+      for (int j = 0; j < 8; j += 2) if ((j >> 1) == q) { s0 = dl[h][j]; s1 = dl[h][j + 1]; }
+      *reinterpret_cast<float2*>(sDl + (rq + 8 * h) * HB_DL + 2 * q) = make_float2(s0, s1);
+    }
+    // dH[k] = sum_j dlog_j Wp[k][j] in heads_loss_kernel's order, for the thread's units k = 8 j + 2 q + e
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int k = 8 * j + 2 * q + e;
+        const float4 w0 = *reinterpret_cast<const float4*>(sWp + k * 8), w1 = *reinterpret_cast<const float4*>(sWp + k * 8 + 4);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float tt = 0.f;
+          tt = fmaf(dl[h][0], w0.x, tt); tt = fmaf(dl[h][1], w0.y, tt); tt = fmaf(dl[h][2], w0.z, tt); tt = fmaf(dl[h][3], w0.w, tt);
+          tt = fmaf(dl[h][4], w1.x, tt); tt = fmaf(dl[h][5], w1.y, tt); tt = fmaf(dl[h][6], w1.z, tt); tt = fmaf(dl[h][7], w1.w, tt);
+          dht[j][2 * h + e] = (valid[h] ? tt : 0.f) + dhc[j][2 * h + e];
+        }
+      }
+  } else {
+    float v[2] = {sBo[0], sBo[0]};
+#pragma unroll
+    for (int c = 0; c < 8; ++c) {
+      float x[2][8];
+      row8(0, c, x[0]); row8(1, c, x[1]);
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        const float wv = sWv[8 * c + e];
+        v[0] = fmaf(x[0][e], wv, v[0]); v[1] = fmaf(x[1][e], wv, v[1]);
+      }
+    }
+    float dv[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      dv[h] = 0.f;
+      if (valid[h]) {
+        const float ret = a.Rs[io[h]];
+        dv[h] = a.scale * a.v_coef * (v[h] - ret);
+        if (ag == 0 && q == 0) vl += 0.5f * a.v_coef * (ret - v[h]) * (ret - v[h]);
+      }
+      *reinterpret_cast<float2*>(sDl + (rq + 8 * h) * HB_DL + 2 * q) = make_float2(q == 0 ? dv[h] : 0.f, 0.f);
+    }
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const float wv = sWv[8 * j + 2 * q + e];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) dht[j][2 * h + e] = (valid[h] ? __fmul_rn(dv[h], wv) : 0.f) + dhc[j][2 * h + e];
+      }
+  }
+}
+
 // PROF: clock64 phase sums of thread 0 of every warpgroup into a.prof[0..3] (operand wait | smem -> regs + cell backward |
 // MMA issue -> wait | dZ store), a separate instantiation (tscl_debug_bptt_prof)
-template <bool PROF>
+//
+// HEADS: the loss gradients at the heads are computed here instead of read from a dH tensor (tscl_lstm_seq_bwd_tc_heads).
+// mapD is then the bf16 h store ([.][T][Rc][64]); the warpgroup's 8 KB h_t tile takes the first half of the dH space,
+// on its own mbarrier, and is refilled with h_{t-1} once the step's readers are past the staging barrier.  Per step:
+//   after the operand wait, the quad of threads that share rows rq, rq + 8 computes each row's logits (policy unit:
+//   thread q the logits 2 q, 2 q + 1, the sequential fmaf chain over k = 0..63 of heads_loss_kernel; value unit: every
+//   thread the whole v chain), gathers them by shuffles (no arithmetic), and repeats heads_loss_kernel's per-row loss
+//   arithmetic and its 8-term dH chains for the thread's own 16 units.  dH is therefore the bits tscl_heads_loss
+//   writes, and dZ the bits of the tscl_heads_loss -> tscl_lstm_seq_bwd_tc pair.  The rows' dlog go to a small
+//   staging tile; while the step's MMA runs, thread (k, logits 4 hh..4 hh + 3) adds h[row][k] * dlog[row][j] over the
+//   warpgroup's 64 rows into registers, flushed to G with one atomic per output at every unit change.
+// Items run over n_chunks consecutive chunks (chunk-outermost, the activation store's order).
+template <bool PROF, bool HEADS = false>
 __global__ void __launch_bounds__(256, 1)
 lstm_bwd_tc_regs_kernel(const DDimsTC d, const BwdTC a, const __grid_constant__ CUtensorMap mapG,
                         const __grid_constant__ CUtensorMap mapC, const __grid_constant__ CUtensorMap mapD,
@@ -1503,8 +1666,16 @@ lstm_bwd_tc_regs_kernel(const DDimsTC d, const BwdTC a, const __grid_constant__ 
   unsigned char* sW = sB + BW_KC * 1024 + wg * BR_WG_BYTES;          // this warpgroup's buffers (1024-byte aligned)
   const uint32_t aB = smem_u32(sB), aG = smem_u32(sW), aD = aG + 32768, aC = aG + 49152, aZ = aG + 65536;
   const uint32_t ldbar = smem_u32(sB + BW_KC * 1024 + 2 * BR_WG_BYTES) + 8 * wg;
+  // HEADS: in the dH space of each warpgroup, h_t tile [64][128 B] | dlog staging [64][HB_DL] fp32 | (warpgroup 0 only)
+  // the unit's head weights [64][8] (padded to 8 logits), Wv [64], biases [8] | h mbarrier
+  constexpr int HB_DL = 12;
+  const unsigned char* sH = sW + 32768;
+  float* sDl = reinterpret_cast<float*>(sW + 40960);
+  float* sHW = reinterpret_cast<float*>(sB + BW_KC * 1024 + 40960 + 64 * HB_DL * 4);
+  const uint32_t hbar = aG + 47104;
   if (lead) {
     mbar_init(ldbar, 1);
+    if (HEADS) mbar_init(hbar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -1515,34 +1686,71 @@ lstm_bwd_tc_regs_kernel(const DDimsTC d, const BwdTC a, const __grid_constant__ 
   auto lm = [&](uint32_t box, int c) { return box + lm_row + (((2 * c + lm_hi) ^ lm_sw) << 4); };
   const int rq = 16 * w + (lane >> 2);                               // the thread's rows: rq, rq + 8 of the warpgroup's 64
   const int64_t n_tiles = (a.Rc + TC_M - 1) / TC_M;
-  const int64_t n_items = n_tiles * 2 * d.A;
+  const int64_t per_chunk = n_tiles * 2 * d.A;
+  const int64_t n_items = per_chunk * (HEADS ? a.n_chunks : 1);
   int cur_u = -1;
-  uint32_t ldpar = 0;
+  uint32_t ldpar = 0, hpar = 0;
+  // HEADS: head weight / bias gradient sums of the current unit, thread = (hidden unit hk, logits 4 hh .. 4 hh + 3)
+  const int hk = tid & 63, hh = (tid >> 6) & 1;
+  float gw[4] = {0.f, 0.f, 0.f, 0.f}, gb = 0.f, pl = 0.f, vl = 0.f, el = 0.f;
+  auto flush = [&](int uu) {
+    const int nl = (uu & 1) ? 1 : d.max_na;                          // value units have one output
+#pragma unroll
+    for (int jj = 0; jj < 4; ++jj) {
+      if (hh * 4 + jj < nl) atomicAdd(&a.G[d.off_wo + ((int64_t)uu * TC_H + hk) * d.max_na + hh * 4 + jj], gw[jj]);
+      gw[jj] = 0.f;
+    }
+    if ((tid & 127) < nl) atomicAdd(&a.G[d.off_bo + (int64_t)uu * d.max_na + (tid & 127)], gb);
+    gb = 0.f;
+  };
   for (int64_t it = blockIdx.x; it < n_items; it += gridDim.x) {
-    const int u = (int)(it / n_tiles);
-    const int rw0 = (int)((it - (int64_t)u * n_tiles) * TC_M) + 64 * wg;   // first row of this warpgroup
+    const int ci = HEADS ? (int)(it / per_chunk) : 0;                // chunk of the item
+    const int64_t ic = it - (int64_t)ci * per_chunk;
+    const int u = (int)(ic / n_tiles);
+    const int rw0 = (int)((ic - (int64_t)u * n_tiles) * TC_M) + 64 * wg;   // first row of this warpgroup
     __syncthreads();                                                 // both warpgroups are done with the previous item
     if (u != cur_u) {
+      if (HEADS && cur_u >= 0) flush(cur_u);
       cur_u = u;
       const uint4* src = reinterpret_cast<const uint4*>(a.Wt + (int64_t)u * BW_KC * TC_H * 8);
       uint4* dst = reinterpret_cast<uint4*>(sB);
       for (int i = tid; i < BW_KC * TC_H; i += 256) dst[i] = src[i];
+      if (HEADS) {       // the unit's head weights and biases, padded to 8 logits as heads_loss_kernel pads them
+        const int mna = d.max_na;
+        const float* wo = a.P + d.off_wo + (int64_t)u * TC_H * mna;
+        for (int i = tid; i < TC_H * 8; i += 256) { const int k = i >> 3, j = i & 7; sHW[i] = j < mna ? wo[k * mna + j] : 0.f; }
+        if (tid < TC_H) sHW[512 + tid] = wo[tid * mna];
+        if (tid < 8) sHW[576 + tid] = tid < mna ? a.P[d.off_bo + (int64_t)u * mna + tid] : 0.f;
+      }
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic writes -> operand of the wgmmas
       __syncthreads();
     }
     if (rw0 >= a.Rc) continue;                                       // a partial tile with no row for this warpgroup
-    const int z0 = u * a.T;                                          // plane of step 0 in the [2A * T][Rc][cols] maps
+    const int z0 = (ci * 2 * d.A + u) * a.T;                         // plane of step 0 in the [2A * T][Rc][cols] maps
     // step t's gates and dH, c_{t-1} into its ring slot, and c_t as well for the item's first step (lead thread)
     auto fetch = [&](int t, bool with_c_t) {
-      mbar_expect_tx(ldbar, (uint32_t)(32768 + 16384 + (with_c_t ? 8192 : 0) + (t > 0 ? 8192 : 0)));
+      mbar_expect_tx(ldbar, (uint32_t)(32768 + (HEADS ? 0 : 16384) + (with_c_t ? 8192 : 0) + (t > 0 ? 8192 : 0)));
 #pragma unroll
       for (int g = 0; g < 4; ++g) tma_load_3d(aG + g * 8192, &mapG, g * 64, rw0, z0 + t, ldbar);
-      tma_load_3d(aD, &mapD, 0, rw0, z0 + t, ldbar);
-      tma_load_3d(aD + 8192, &mapD, 32, rw0, z0 + t, ldbar);
+      if (!HEADS) {
+        tma_load_3d(aD, &mapD, 0, rw0, z0 + t, ldbar);
+        tma_load_3d(aD + 8192, &mapD, 32, rw0, z0 + t, ldbar);
+      }
       if (with_c_t) tma_load_3d(aC + (t & 1) * 8192, &mapC, 0, rw0, z0 + t, ldbar);
       if (t > 0) tma_load_3d(aC + ((t - 1) & 1) * 8192, &mapC, 0, rw0, z0 + t - 1, ldbar);
     };
-    if (lead) fetch(a.T - 1, true);
+    auto fetch_h = [&](int t) {                                      // HEADS: h_t of this warpgroup's rows
+      mbar_expect_tx(hbar, 8192u);
+      tma_load_3d(aD, &mapD, 0, rw0, z0 + t, hbar);
+    };
+    if (lead) {
+      fetch(a.T - 1, true);
+      if (HEADS) fetch_h(a.T - 1);
+    }
+    // HEADS: the item's agent, and this thread's rows as rows of the whole update (act / Rs / Adv index)
+    const int ag = u >> 1, na = HEADS ? d.n_a[ag] : 0;
+    const bool pol = (u & 1) == 0;
+    const int64_t rg0 = (int64_t)ci * a.Rc + rw0 + rq;
     // per-thread state, entry [j][e]: row rq + 8 (e >> 1), unit 8 j + 2 q + (e & 1) (= accumulator entry 4 j + e)
     float dc[8][4], dhc[8][4];
 #pragma unroll
@@ -1553,7 +1761,10 @@ lstm_bwd_tc_regs_kernel(const DDimsTC d, const BwdTC a, const __grid_constant__ 
     for (int t = a.T - 1; t >= 0; --t) {
       const float keep = 1.0f - a.done[t];
       mbar_wait(ldbar, ldpar); ldpar ^= 1;                           // step t's operands have landed
+      if (HEADS) { mbar_wait(hbar, hpar); hpar ^= 1; }               // and h_t
       BR_MARK(0);
+      float dht[8][4];                                               // dH + dh carry
+      if constexpr (HEADS) heads_step(d, a, sH, sHW, sDl, pol, ag, na, rq, rw0 + rq, lane, q, rg0, t, dhc, dht, pl, vl, el);
       // shared memory -> registers; bf16 pairs [j][h]: row rq + 8 h, units 8 j + 2 q + {0 (low half), 1}
       uint32_t gr[4][8][2], cr[8][2], pr[8][2];
 #pragma unroll
@@ -1571,17 +1782,18 @@ lstm_bwd_tc_regs_kernel(const DDimsTC d, const BwdTC a, const __grid_constant__ 
           pr[2 * c][0] = r[0]; pr[2 * c][1] = r[1]; pr[2 * c + 1][0] = r[2]; pr[2 * c + 1][1] = r[3];
         }
       }
-      float dht[8][4];                                               // dH + dh carry
+      if constexpr (!HEADS) {
 #pragma unroll
-      for (int j = 0; j < 8; ++j)
+        for (int j = 0; j < 8; ++j)
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int row = rq + 8 * h;
-          const float2 v = *reinterpret_cast<const float2*>(sW + 32768 + (j >> 2) * 8192 + row * 128 +
-                                                           (((2 * (j & 3) + (q >> 1)) ^ (row & 7)) << 4) + 8 * (q & 1));
-          dht[j][2 * h] = v.x + dhc[j][2 * h];
-          dht[j][2 * h + 1] = v.y + dhc[j][2 * h + 1];
-        }
+          for (int h = 0; h < 2; ++h) {
+            const int row = rq + 8 * h;
+            const float2 v = *reinterpret_cast<const float2*>(sW + 32768 + (j >> 2) * 8192 + row * 128 +
+                                                             (((2 * (j & 3) + (q >> 1)) ^ (row & 7)) << 4) + 8 * (q & 1));
+            dht[j][2 * h] = v.x + dhc[j][2 * h];
+            dht[j][2 * h + 1] = v.y + dhc[j][2 * h + 1];
+          }
+      }
       if (lead) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");   // the last dZ store has left the staging tile
       asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");    // the operand buffers are free
       if (lead && t > 0) fetch(t - 1, false);
@@ -1597,7 +1809,9 @@ lstm_bwd_tc_regs_kernel(const DDimsTC d, const BwdTC a, const __grid_constant__ 
           } else {
             const int64_t r = rw0 + rq + 8 * h;
             float2 v = make_float2(0.f, 0.f);
-            if (r < a.Rc) v = *reinterpret_cast<const float2*>(a.c0 + ((int64_t)u * a.ld_state + a.r0 + r) * TC_H + 8 * j + 2 * q);
+            if (r < a.Rc)
+              v = *reinterpret_cast<const float2*>(a.c0 + ((int64_t)u * a.ld_state + a.r0 + (int64_t)ci * a.Rc + r) * TC_H +
+                                                   8 * j + 2 * q);
             cp2[0] = v.x; cp2[1] = v.y;
           }
           float z[4][2];
@@ -1644,11 +1858,24 @@ lstm_bwd_tc_regs_kernel(const DDimsTC d, const BwdTC a, const __grid_constant__ 
                        make_desc(aB + (4 * g + c) * 2 * 1024, 1024, 128), (g | c) != 0);
       wg_commit();
       BR_MARK(2);
+      if constexpr (HEADS) {     // head weight / bias gradients of step t while the MMA runs (dlog staged before bar 1)
+#pragma unroll 8
+        for (int row = 0; row < 64; ++row) {
+          const uint16_t hb = *reinterpret_cast<const uint16_t*>(sH + row * 128 + (((hk >> 3) ^ (row & 7)) << 4) + (hk & 7) * 2);
+          const float x = __uint_as_float((uint32_t)hb << 16);
+          const float4 g4 = *reinterpret_cast<const float4*>(sDl + row * HB_DL + hh * 4);
+          gw[0] = fmaf(x, g4.x, gw[0]); gw[1] = fmaf(x, g4.y, gw[1]);
+          gw[2] = fmaf(x, g4.z, gw[2]); gw[3] = fmaf(x, g4.w, gw[3]);
+        }
+        if ((tid & 127) < 8)
+          for (int row = 0; row < 64; ++row) gb += sDl[row * HB_DL + (tid & 127)];
+      }
       asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");    // the whole staging tile is written
       if (lead) {
 #pragma unroll
         for (int g = 0; g < 4; ++g) tma_store_3d(&mapZ, g * 64, rw0, z0 + t, aZ + g * 8192);
         asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+        if (HEADS && t > 0) fetch_h(t - 1);                          // every reader of h_t / dlog is past the barrier
       }
       BR_MARK(3);
       wg_wait<0>();
@@ -1662,6 +1889,20 @@ lstm_bwd_tc_regs_kernel(const DDimsTC d, const BwdTC a, const __grid_constant__ 
     }
   }
   if (lead) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // dZ stores complete before the CTA leaves
+  if (HEADS) {
+    if (cur_u >= 0) flush(cur_u);
+    if (a.stats) {
+#pragma unroll
+      for (int o = 16; o; o >>= 1) {
+        pl += __shfl_down_sync(0xffffffffu, pl, o);
+        vl += __shfl_down_sync(0xffffffffu, vl, o);
+        el += __shfl_down_sync(0xffffffffu, el, o);
+      }
+      if (lane == 0 && (pl != 0.f || vl != 0.f || el != 0.f)) {
+        atomicAdd(&a.stats[0], pl * a.scale); atomicAdd(&a.stats[1], vl * a.scale); atomicAdd(&a.stats[2], el * a.scale);
+      }
+    }
+  }
   if (PROF && lead)
     for (int i = 0; i < 4; ++i) atomicAdd(a.prof + i, (unsigned long long)bp[i]);
 #undef BR_MARK
@@ -1784,6 +2025,47 @@ extern "C" int tscl_lstm_seq_bwd_tc_dx(tscl_handle* h, const void* wt_bf16, floa
   }
   if (bw_threads == 512) lstm_bwd_tc_kernel<512><<<grid, 512, smem, (cudaStream_t)stream>>>(d, a);
   else lstm_bwd_tc_kernel<256><<<grid, 256, smem, (cudaStream_t)stream>>>(d, a);
+  PCK(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int tscl_lstm_seq_bwd_tc_heads(tscl_handle* h, const void* wt_bf16, const float* params, const void* gates_bf16,
+                                          const void* c_bf16, const void* h_bf16, const float* c0, const float* done,
+                                          const int32_t* act, const float* Rs, const float* Adv, int32_t T, int64_t Rc,
+                                          int32_t n_chunks, int64_t ld_state, int64_t r0, int64_t stride_t, float v_coef,
+                                          float beta, float scale, void* dz_bf16, float* stats, float* grads, void* stream) {
+  if (!h || !wt_bf16 || !params || !gates_bf16 || !c_bf16 || !h_bf16 || !c0 || !done || !act || !Rs || !Adv || !dz_bf16 ||
+      !grads || T <= 0 || Rc <= 0 || n_chunks <= 0)
+    return tsc_set_error("tscl_lstm_seq_bwd_tc_heads: bad argument");
+  PCK(cudaSetDevice(tscl_device_of(h)));
+  const DDimsTC& d = *tscl_dims_of(h);
+  if (d.max_na > 8) return tsc_set_error("tscl_lstm_seq_bwd_tc_heads: more than 8 actions");
+  if ((uint64_t)n_chunks * 2 * d.A * T > 0x7fffffffu) return tsc_set_error("tscl_lstm_seq_bwd_tc_heads: too many planes");
+  CUtensorMap mG, mC, mH, mZ;
+  const uint64_t planes = (uint64_t)n_chunks * 2 * d.A * T;
+  if (!(make_tmap_3d(&mG, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, gates_bf16, planes, Rc, TC_N, 64, 64) &&
+        make_tmap_3d(&mC, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, c_bf16, planes, Rc, TC_H, 64, 64) &&
+        make_tmap_3d(&mH, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, h_bf16, planes, Rc, TC_H, 64, 64) &&
+        make_tmap_3d(&mZ, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, dz_bf16, planes, Rc, TC_N, 64, 64)))
+    return tsc_set_error("tscl_lstm_seq_bwd_tc_heads: cannot encode the tensor maps (cuTensorMapEncodeTiled)");
+  static int attr_r = -1;
+  if (attr_r != tscl_device_of(h)) {
+    PCK(cudaFuncSetAttribute(lstm_bwd_tc_regs_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, BR_SMEM));
+    PCK(cudaFuncSetAttribute(lstm_bwd_tc_regs_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, BR_SMEM));
+    attr_r = tscl_device_of(h);
+  }
+  int n_sm = 0;
+  PCK(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, tscl_device_of(h)));
+  const int64_t n_items = (int64_t)n_chunks * ((Rc + TC_M - 1) / TC_M) * 2 * d.A;
+  const int grid = (int)(n_items < n_sm ? n_items : n_sm);
+  BwdTC a = {};
+  a.Wt = (const __nv_bfloat16*)wt_bf16; a.c0 = c0; a.done = done; a.T = T; a.Rc = Rc; a.ld_state = ld_state; a.r0 = r0;
+  a.Gb = (const __nv_bfloat16*)gates_bf16; a.Cb = (const __nv_bfloat16*)c_bf16; a.dZb = (__nv_bfloat16*)dz_bf16;
+  a.P = params; a.act = act; a.Rs = Rs; a.Adv = Adv; a.stride_t = stride_t; a.v_coef = v_coef; a.beta = beta;
+  a.scale = scale; a.stats = stats; a.G = grads; a.n_chunks = n_chunks;
+  a.prof = g_bptt_prof;
+  if (a.prof) lstm_bwd_tc_regs_kernel<true, true><<<grid, 256, BR_SMEM, (cudaStream_t)stream>>>(d, a, mG, mC, mH, mZ);
+  else lstm_bwd_tc_regs_kernel<false, true><<<grid, 256, BR_SMEM, (cudaStream_t)stream>>>(d, a, mG, mC, mH, mZ);
   PCK(cudaGetLastError());
   return 0;
 }

@@ -155,6 +155,18 @@ int tscl_lstm_seq_bwd_tc_dx(tscl_handle* h, const void* wt_bf16, float* ZG, cons
                             const float* done, int32_t T, int64_t Rc, int64_t ld_state, int64_t r0,
                             const void* gates_bf16, const void* c_bf16, void* dz_bf16, const void* wxt_bf16, void* dx_bf16,
                             void* stream);
+/* tscl_heads_loss followed by the store-path tscl_lstm_seq_bwd_tc in one kernel: each BPTT step computes its dH from h_t
+ * of the bf16 store `h_bf16` and the head weights in `params` with tscl_heads_loss's arithmetic, so dz_bf16 is bit-identical
+ * to that pair's; the head weight / bias gradients are added to `grads` and agent 0's loss sums to `stats` (optional) as
+ * tscl_heads_loss adds them (up to summation order).  Runs over `n_chunks` consecutive chunks of Rc replicas: gates_bf16 /
+ * c_bf16 / h_bf16 / dz_bf16 are [n_chunks][2A][T][Rc][w] (the activation store's layout), chunk i's replicas are
+ * r0 + i * Rc .. of c0 ([2A][ld_state][64]), and act / Rs / Adv point at the first chunk's first replica, row (t, r, a) at
+ * t * stride_t + r * A + a with r counted over all chunks.  Needs cuTensorMapEncodeTiled and max_na <= 8. */
+int tscl_lstm_seq_bwd_tc_heads(tscl_handle* h, const void* wt_bf16, const float* params, const void* gates_bf16,
+                               const void* c_bf16, const void* h_bf16, const float* c0, const float* done,
+                               const int32_t* act, const float* Rs, const float* Adv, int32_t T, int64_t Rc,
+                               int32_t n_chunks, int64_t ld_state, int64_t r0, int64_t stride_t, float v_coef, float beta,
+                               float scale, void* dz_bf16, float* stats, float* grads, void* stream);
 /* Host-buffer loop, one call per replica range and control step (replaces the reference's per-step numpy hand-over of
  * ob / reward into `model.add_transition`, agents/models.py:222-229, main.py / utils.py:272-286): observations
  * host -> obs_dev (the rollout slot), rewards host -> rew_hist_dev = clip(reward / reward_norm) (0 = off for either),

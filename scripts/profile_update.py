@@ -49,8 +49,11 @@ BYTES = {   # per update
     "fc_bwd_tc_kernel": n_chunks * U * M * (dx * 2 + dx * 2),                     # dX, X (bf16)
     # dZ, X (bf16); the observation slice (fp32, shared by an agent's two units and read through L2) is not counted
     "dx_fc_bwd_tc_kernel": n_chunks * U * M * (4 * H * 2 + dx * 2),
-    "lstm_bwd_tc_regs_kernel": n_chunks * U * M * (4 * H * 2 + H * 2 + H * 4 + 4 * H * 2),   # gates, c, dH (fp32) in, dZ out
+    # gates, c, then h_t (bf16) when the kernel computes dH itself (heads_in_bptt) or dH (fp32) in; dZ out
+    "lstm_bwd_tc_regs_kernel": n_chunks * U * M * (4 * H * 2 + H * 2 + (H * 2 if m.heads_in_bptt else H * 4) + 4 * H * 2),
+    "heads_loss_kernel": n_chunks * U * M * (H * 2 + H * 4),                      # h (bf16) in, dH (fp32) out
 }
+print("heads in the BPTT kernel: %s (TSC_BPTT_HEADS=0 runs heads_loss_kernel + the BPTT per chunk)" % m.heads_in_bptt)
 
 assert m.store_acts, "the bf16 activation store does not fit: the update would take the fp32 path"
 tr.run(T)                              # one rollout + one update: warms up every shape of the update
