@@ -305,6 +305,10 @@ struct StepTC {
   // P + k p_stride and Wp + k wp_stride, and it samples with seeds[k] (device array) and replica index r - k Rm
   int64_t Rm, p_stride, wp_stride;
   const uint64_t* seeds;
+  // grouped pi-only instantiation (EVAL && GRP): ragged members, member k owns rows rows[k] .. rows[k+1] - 1 (device
+  // array of K + 1 ascending boundaries); Rm is unused
+  const int64_t* rows;
+  int K;
 };
 
 extern __shared__ __align__(1024) unsigned char tc_smem[];
@@ -642,6 +646,27 @@ __host__ __device__ inline int gate_col(int n) {
   return (i >> 3) * 64 + 16 * q + 2 * (i & 7) + e;
 }
 
+// EVAL && GRP: the item block (member mk, pi unit ui) holding item `seg`.  Member k's items are its A units times its
+// ceil(S_k / 64) tiles, in member order; the item count the launcher sizes the grid with is an upper bound, so an item
+// past the last member returns false.  rofs: the block's first row minus 64 times its first item.
+__device__ __forceinline__ bool grp_block(const DDimsTC& d, const StepTC& a, int64_t seg, int64_t it_hi, int& mk, int& ui,
+                                          int64_t& seg_hi, int64_t& rofs) {
+  int64_t t0 = 0;
+  for (int k = 0; k < a.K; ++k) {
+    const int64_t r0 = a.rows[k], nt = (a.rows[k + 1] - r0 + P2_ROWS - 1) / P2_ROWS, ni = nt * d.A;
+    if (seg < t0 + ni) {
+      mk = k;
+      ui = (int)((seg - t0) / nt);
+      const int64_t b0 = t0 + (int64_t)ui * nt;
+      seg_hi = b0 + nt < it_hi ? b0 + nt : it_hi;
+      rofs = r0 - b0 * P2_ROWS;
+      return true;
+    }
+    t0 += ni;
+  }
+  return false;
+}
+
 // DX = d.dx: the fragment sizes and the k loops are compile-time.  Instantiated for the fc widths of the shipped
 // configurations (P2_DX_OK): 224 (grid MA2C), 192 (Monaco), 160 (grid IA2C: no fingerprint block), 128 (Monaco IA2C:
 // no fingerprint or wait block)
@@ -653,6 +678,9 @@ __host__ __device__ inline int gate_col(int n) {
 // are (member, unit, tile), so one member's [Wx;Wh] image stays resident over its tiles, and a block of items never
 // spans two members.  Member k reads its parameters and image at stride offsets and samples with the key
 // (seeds[k], step, replica0 + r - k Rm) of its own one-member launch; per element the arithmetic is unchanged.
+// EVAL && GRP: the grouped pi-only forward (tscl_policy_step_pi_g).  Members are ragged (grp_block): items are (member,
+// pi unit, tile of the member), a member's last tile is partial and its rows past the member's end are neither loaded
+// nor stored; member k samples with (seeds[k], step, r - rows[k]).
 template <int DX, bool PROF, bool EVAL, bool GRP = false>
 __global__ void __launch_bounds__(P2_THREADS, 1)
 policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
@@ -666,7 +694,8 @@ policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
   float* sBias0 = sBias + TC_N;                                              // [256]  fc biases
   uint64_t* sBar = reinterpret_cast<uint64_t*>(sBias0 + TC_N);               // full[2], empty[2]
   // GRP only (16 more bytes): the block's row offset rofs (int64), the member's sampling key and the low word of its
-  // first row, kept in shared memory rather than in the consumers' full register budget
+  // first row, kept in shared memory rather than in the consumers' full register budget; EVAL && GRP (8 more): the
+  // member's end row
   int64_t* sGrp = reinterpret_cast<int64_t*>(sBar + 4);
   const uint32_t aB = smem_u32(sB);
   if (tid == 0) {
@@ -679,7 +708,7 @@ policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
   __syncthreads();
   const int64_t n_tiles = (a.R + P2_ROWS - 1) / P2_ROWS;
   const int64_t ld = a.ld > 0 ? a.ld : a.R;
-  const int64_t n_items = n_tiles * (EVAL ? 1 : 2) * d.A;
+  const int64_t n_items = (EVAL && GRP ? n_tiles + a.K - 1 : n_tiles) * (EVAL ? 1 : 2) * d.A;   // EVAL && GRP: bound
   const int64_t it_lo = n_items * blockIdx.x / gridDim.x, it_hi = n_items * (blockIdx.x + 1) / gridDim.x;
 
   // phase clocks of the producer's thread 0 and consumer 0's thread 0, added straight into the counters (no register
@@ -699,7 +728,12 @@ policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
         const uint64_t sk = a.seeds[mk];
         sGrp[0] = rofs;
         reinterpret_cast<uint32_t*>(sGrp)[2] = pmix32((uint32_t)sk ^ (a.step * 0x9E3779B1U)) ^ (uint32_t)(sk >> 32);
-        reinterpret_cast<uint32_t*>(sGrp)[3] = (uint32_t)((int64_t)mk * a.Rm);
+        if constexpr (EVAL) {
+          reinterpret_cast<uint32_t*>(sGrp)[3] = (uint32_t)a.rows[mk];
+          sGrp[2] = a.rows[mk + 1];
+        } else {
+          reinterpret_cast<uint32_t*>(sGrp)[3] = (uint32_t)((int64_t)mk * a.Rm);
+        }
       }
       const float* P = GRP ? a.P + (int64_t)mk * a.p_stride : a.P;
       const uint4* src = reinterpret_cast<const uint4*>((GRP ? a.Wp + (int64_t)mk * a.wp_stride : a.Wp) + (int64_t)u * wp_stride(DX));
@@ -730,12 +764,21 @@ policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
     const int warp = tid >> 5;
     uint32_t ph_empty = 0;
     for (int64_t seg = it_lo; seg < it_hi;) {
-      // GRP: item block blk = (member mk, unit ui) of bt tiles; items (item counts < 2^31) in 32-bit arithmetic
-      const int bt = GRP ? (int)(a.Rm / P2_ROWS) : 1, blk = GRP ? (int)seg / bt : 0, mk = GRP ? blk / (2 * d.A) : 0;
-      const int ui = GRP ? blk - mk * 2 * d.A : (int)(seg / n_tiles), u = EVAL ? 2 * ui : ui, ag = u >> 1;   // ui: item block = state unit
-      const int64_t seg_hi = GRP ? ((int64_t)(blk + 1) * bt < it_hi ? (int64_t)(blk + 1) * bt : it_hi)
-                                 : ((int64_t)(ui + 1) * n_tiles < it_hi ? (int64_t)(ui + 1) * n_tiles : it_hi);
-      load_unit(u, mk, GRP ? (int64_t)mk * a.Rm - (int64_t)blk * bt * P2_ROWS : 0, false);
+      int mk, ui;                 // ui: item block = state unit
+      int64_t seg_hi, rofs;
+      if constexpr (EVAL && GRP) {
+        if (!grp_block(d, a, seg, it_hi, mk, ui, seg_hi, rofs)) break;
+      } else {
+        // GRP: item block blk = (member mk, unit ui) of bt tiles; items (item counts < 2^31) in 32-bit arithmetic
+        const int bt = GRP ? (int)(a.Rm / P2_ROWS) : 1, blk = GRP ? (int)seg / bt : 0;
+        mk = GRP ? blk / (2 * d.A) : 0;
+        ui = GRP ? blk - mk * 2 * d.A : (int)(seg / n_tiles);
+        seg_hi = GRP ? ((int64_t)(blk + 1) * bt < it_hi ? (int64_t)(blk + 1) * bt : it_hi)
+                     : ((int64_t)(ui + 1) * n_tiles < it_hi ? (int64_t)(ui + 1) * n_tiles : it_hi);
+        rofs = GRP ? (int64_t)mk * a.Rm - (int64_t)blk * bt * P2_ROWS : 0;
+      }
+      const int u = EVAL ? 2 * ui : ui, ag = u >> 1;
+      load_unit(u, mk, rofs, false);
       PROF_MARK(8);      // producer: unit constants
       const int nw = d.n_wave[ag], nt = d.n_wait[ag], nf = d.ff > 0 ? d.n_fp[ag] : 0, ooff = d.obs_off[ag];
       // observation index of this lane's two input slots 2 lane, 2 lane + 1 (-1: unused slot)
@@ -749,6 +792,7 @@ policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
       for (int64_t it = seg; it < seg_hi; ++it) {
         const int s = (int)((it - it_lo) & 1);
         const int64_t r0 = GRP ? sGrp[0] + it * P2_ROWS : (it - (int64_t)ui * n_tiles) * P2_ROWS;
+        const int64_t rlim = EVAL && GRP ? sGrp[2] : a.R;      // end of the rows this item may touch
         unsigned char* sA = sA0 + (size_t)s * KC * 1024;
         const uint32_t full = smem_u32(sBar + s), empty = smem_u32(sBar + 2 + s);
         mbar_wait(empty, ((ph_empty >> s) & 1) ^ 1);       // the tile's previous item has left it (first use: passes)
@@ -770,7 +814,7 @@ policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
             un = (int)((it + 2) / n_tiles);
             rn = ((it + 2) - (int64_t)un * n_tiles) * P2_ROWS + (tid & 63);
           }
-          if (rn < a.R) {
+          if (rn < rlim) {
             const int64_t so = ((int64_t)un * ld + rn) * TC_H + (tid >> 6) * 32;
             asm volatile("prefetch.global.L2 [%0];" ::"l"(a.c_in + so));
             asm volatile("prefetch.global.L2 [%0];" ::"l"(a.h_in + so));
@@ -786,7 +830,7 @@ policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
 #pragma unroll
           for (int rr = 0; rr < 4; ++rr) {
             const int64_t r = r0 + rb + rr;
-            const bool ok = r < a.R;
+            const bool ok = r < rlim;
             const float* op = a.obs + (ok ? r : 0) * d.n_obs + ooff;
             xa[rr] = (src_a >= 0 && ok) ? __ldg(op + src_a) : 0.f;
             xb[rr] = (src_b >= 0 && ok) ? __ldg(op + src_b) : 0.f;
@@ -811,15 +855,25 @@ policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
     const uint32_t aA = smem_u32(sA), full = smem_u32(sBar + c), empty = smem_u32(sBar + 2 + c);
     uint32_t ph_full = 0;
     for (int64_t seg = it_lo; seg < it_hi;) {
-      const int bt = GRP ? (int)(a.Rm / P2_ROWS) : 1, blk = GRP ? (int)seg / bt : 0, mk = GRP ? blk / (2 * d.A) : 0;
-      const int ui = GRP ? blk - mk * 2 * d.A : (int)(seg / n_tiles), u = EVAL ? 2 * ui : ui, ag = u >> 1;   // ui: item block = state unit
-      const int64_t seg_hi = GRP ? ((int64_t)(blk + 1) * bt < it_hi ? (int64_t)(blk + 1) * bt : it_hi)
-                                 : ((int64_t)(ui + 1) * n_tiles < it_hi ? (int64_t)(ui + 1) * n_tiles : it_hi);
-      load_unit(u, mk, GRP ? (int64_t)mk * a.Rm - (int64_t)blk * bt * P2_ROWS : 0, true);
+      int mk, ui;
+      int64_t seg_hi, rofs;
+      if constexpr (EVAL && GRP) {
+        if (!grp_block(d, a, seg, it_hi, mk, ui, seg_hi, rofs)) break;
+      } else {
+        const int bt = GRP ? (int)(a.Rm / P2_ROWS) : 1, blk = GRP ? (int)seg / bt : 0;
+        mk = GRP ? blk / (2 * d.A) : 0;
+        ui = GRP ? blk - mk * 2 * d.A : (int)(seg / n_tiles);
+        seg_hi = GRP ? ((int64_t)(blk + 1) * bt < it_hi ? (int64_t)(blk + 1) * bt : it_hi)
+                     : ((int64_t)(ui + 1) * n_tiles < it_hi ? (int64_t)(ui + 1) * n_tiles : it_hi);
+        rofs = GRP ? (int64_t)mk * a.Rm - (int64_t)blk * bt * P2_ROWS : 0;
+      }
+      const int u = EVAL ? 2 * ui : ui, ag = u >> 1;
+      load_unit(u, mk, rofs, true);
       PROF_MARK(0);      // unit constants
       const int na = d.n_a[ag];
       for (int64_t it = seg + (((seg - it_lo) & 1) != c ? 1 : 0); it < seg_hi; it += 2) {
         const int64_t r0 = GRP ? sGrp[0] + it * P2_ROWS : (it - (int64_t)ui * n_tiles) * P2_ROWS;
+        const int64_t rlim = EVAL && GRP ? sGrp[2] : a.R;
         // row of the activation store (chunk-outermost [R/rc][2A][T][rc][w]) for tile row `row`
         const int64_t st_c0 = (a.row0 + r0) / a.rc, st_rin0 = (a.row0 + r0) - st_c0 * a.rc;
         auto store_row = [&](int row) -> int64_t {
@@ -865,8 +919,8 @@ policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
         float4 hpre[8];
         {
           const int64_t r = r0 + (ct & 63);
-          const bool live = r < a.R && !a.done;
-          const float4* hp = reinterpret_cast<const float4*>(a.h_in + ((int64_t)ui * ld + (r < a.R ? r : 0)) * TC_H + (ct >> 6) * 32);
+          const bool live = r < rlim && !a.done;
+          const float4* hp = reinterpret_cast<const float4*>(a.h_in + ((int64_t)ui * ld + (r < rlim ? r : 0)) * TC_H + (ct >> 6) * 32);
 #pragma unroll
           for (int i = 0; i < 8; ++i) hpre[i] = live ? hp[i] : make_float4(0.f, 0.f, 0.f, 0.f);
         }
@@ -921,7 +975,7 @@ policy_step_tc2_kernel(const DDimsTC d, const StepTC a) {
         for (int hr = 0; hr < 2; ++hr) {
           const int row = rq + 8 * hr;
           const int64_t r = r0 + row;
-          const bool valid = r < a.R;
+          const bool valid = r < rlim;
           const int64_t srow = ((int64_t)ui * ld + (valid ? r : 0)) * TC_H + 16 * q;
           float cprev[16];      // c_{t-1} of (row, hidden units 16 q ..), prefetched to L2 by the producer
           if (valid && !a.done) {
@@ -1188,6 +1242,54 @@ extern "C" int tscl_policy_step_pi(tscl_handle* h, const float* params, const vo
   a.seed_lo = (uint32_t)seed; a.seed_hi = (uint32_t)(seed >> 32); a.step = (uint32_t)step; a.replica0 = replica0;
   a.t = 0; a.T = 1; a.rc = R; a.ld = ld_state; a.row0 = ld_state > 0 ? row0 : 0;
   a.act_mode = act_mode;
+  kern<<<grid, P2_THREADS, smem, (cudaStream_t)stream>>>(d, a);
+  PCK(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int tscl_policy_step_pi_g(tscl_handle* h, const float* params, int64_t p_stride, const void* wpack_bf16,
+                                     int64_t wp_stride_m, const float* obs, int32_t K, const int64_t* rows, int64_t R,
+                                     const float* c_in, const float* h_in, float* c_out, float* h_out, float* pi,
+                                     int32_t* act, int32_t act_mode, int32_t done, const uint64_t* seeds, int64_t step,
+                                     void* stream) {
+  if (!h || !params || !wpack_bf16 || !obs || !rows || !seeds || !c_in || !h_in || !c_out || !h_out || !pi || K < 1 || R < K)
+    return tsc_set_error("tscl_policy_step_pi_g: bad argument");
+  if (act_mode != 0 && act_mode != 1) return tsc_set_error("tscl_policy_step_pi_g: act_mode must be 0 (sample) or 1 (argmax)");
+  PCK(cudaSetDevice(tscl_device_of(h)));
+  const DDimsTC& d = *tscl_dims_of(h);
+  if (!P2_DX_OK(d.dx)) return tsc_set_error("tscl_policy_step_pi_g: no kernel for this dx (128, 160, 192 or 224)");
+  if (d.kw == 0) return tsc_set_error("tscl_policy_step_pi_g: observation slice does not fit the 64-column input tile");
+  if (K > 1 && (p_stride < d.n_params || wp_stride_m < 2 * d.A * wp_stride(d.dx)))
+    return tsc_set_error("tscl_policy_step_pi_g: member strides smaller than one member's parameters / image");
+  const size_t smem = tc2_smem_bytes(d.dx + TC_H) + 32;      // + the block constants (sGrp with the member's end row)
+  if (smem > 232448) return tsc_set_error("tscl_policy_step_pi_g: operand tiles exceed shared memory");
+  void (*kern)(const DDimsTC, const StepTC) = nullptr;
+  switch (d.dx) {
+    case 128: kern = policy_step_tc2_kernel<128, false, true, true>; break;
+    case 160: kern = policy_step_tc2_kernel<160, false, true, true>; break;
+    case 192: kern = policy_step_tc2_kernel<192, false, true, true>; break;
+    case 224: kern = policy_step_tc2_kernel<224, false, true, true>; break;
+  }
+  static int attr_dev = -1;
+  static void (*attr_kern)(const DDimsTC, const StepTC) = nullptr;
+  if (attr_dev != tscl_device_of(h) || attr_kern != kern) {
+    PCK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 232448));
+    attr_dev = tscl_device_of(h); attr_kern = kern;
+  }
+  int n_sm = 0;
+  PCK(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, tscl_device_of(h)));
+  // the members' tiles sum to at most ceil(R / 64) + K - 1 (one partial tile per member); items past the last member's
+  // are empty (grp_block), so the row boundaries stay on the device
+  const int64_t n_items = ((R + P2_ROWS - 1) / P2_ROWS + K - 1) * d.A;
+  if (n_items > INT32_MAX) return tsc_set_error("tscl_policy_step_pi_g: more than 2^31 work items");
+  const int grid = (int)(n_items < n_sm ? n_items : n_sm);
+  StepTC a{};
+  a.P = params; a.Wp = (const __nv_bfloat16*)wpack_bf16; a.obs = obs; a.c_in = c_in; a.h_in = h_in; a.c_out = c_out;
+  a.h_out = h_out; a.pi = pi; a.act = act; a.R = R; a.done = done;
+  a.step = (uint32_t)step; a.replica0 = 0;
+  a.t = 0; a.T = 1; a.rc = R; a.ld = R; a.row0 = 0;
+  a.act_mode = act_mode;
+  a.p_stride = p_stride; a.wp_stride = wp_stride_m; a.seeds = seeds; a.rows = rows; a.K = K;
   kern<<<grid, P2_THREADS, smem, (cudaStream_t)stream>>>(d, a);
   PCK(cudaGetLastError());
   return 0;

@@ -333,6 +333,108 @@ q_fwd_kernel(const QDims d, const float* __restrict__ P, const float* __restrict
   }
 }
 
+// Grouped form (tscl_q_step_g): grid (groups, A, K); CTA (g, a, k) walks tiles g, g + groups, .. of member k, whose rows
+// are rows[k] .. rows[k+1] - 1 (ragged: a member's last tile is partial), with member k's weights of agent a (P + k
+// p_stride) resident.  Per row the statements of q_fwd_kernel's evaluation path (the network through q_tile_forward at
+// q_fc_0's own pitch, the same chain of fp32 operations), keyed with seeds[k] and the member-local replica index, and
+// a failed sample reported into bad[k]: member k's outputs are those of its own tscl_q_step launch.
+template <bool DQN>
+__global__ void __launch_bounds__(256)
+q_fwd_g_kernel(const QDims d, const float* __restrict__ P0, int64_t p_stride, const float* __restrict__ obs,
+               const int64_t* __restrict__ rows, float* __restrict__ q, int32_t* __restrict__ act, int mode,
+               const uint64_t* __restrict__ seeds, uint32_t step, unsigned long long* __restrict__ bad) {
+  extern __shared__ __align__(16) float qsm[];
+  const int k = blockIdx.z;
+  const int64_t row0 = rows[k], S = rows[k + 1] - row0;
+  const int64_t n_tiles = (S + QT_ROWS - 1) / QT_ROWS;
+  if (blockIdx.x >= n_tiles) return;                 // the whole CTA: no barrier is pending
+  const QSmem L = q_smem_layout(d);
+  const float* P = P0 + (int64_t)k * p_stride;
+  const int a = blockIdx.y, tid = threadIdx.x, ty = tid >> 4, tx = tid & 15;
+  const int n_s = d.n_s[a], n_a = d.n_a[a], ooff = d.obs_off[a];
+  const int n_w = DQN ? d.n_w[a] : 0, n_wave = n_s - n_w;
+  const int n_ft = n_w > 0 ? d.n_ft : 0;
+  const int q_in = DQN ? d.n_h : n_s;
+  float *sW1 = qsm + L.w1, *sB1 = qsm + L.b1, *sWt = qsm + L.wt, *sW2 = qsm + L.w2, *sB2 = qsm + L.b2;
+  float *sWq = qsm + L.wq, *sBq = qsm + L.bq, *sS = qsm + L.s, *sH1 = qsm + L.h1, *sH2 = qsm + L.h2, *sQ = qsm + L.q;
+  if (DQN) {
+    for (int i = tid; i < n_wave * d.n_fc; i += 256) sW1[i] = P[d.off_fcw_w[a] + i];
+    for (int i = tid; i < d.n_fc; i += 256) sB1[i] = P[d.off_fcw_b[a] + i];
+    for (int i = tid; i < n_w * n_ft; i += 256) sWt[i] = P[d.off_fct_w[a] + i];
+    for (int i = tid; i < n_ft; i += 256) sB1[d.n_fc + i] = P[d.off_fct_b[a] + i];
+    for (int i = tid; i < (d.n_fc + n_ft) * d.n_h; i += 256) sW2[i] = P[d.off_fc0_w[a] + i];
+    for (int i = tid; i < d.n_h; i += 256) sB2[i] = P[d.off_fc0_b[a] + i];
+  }
+  for (int i = tid; i < q_in * QT_NA; i += 256) {
+    const int kk = i / QT_NA, j = i - kk * QT_NA;
+    sWq[i] = j < n_a ? P[d.off_q_w[a] + (int64_t)kk * n_a + j] : 0.f;
+  }
+  for (int i = tid; i < QT_NA; i += 256) sBq[i] = i < n_a ? P[d.off_q_b[a] + i] : 0.f;
+  const uint64_t sk = seeds[k];
+  const uint32_t seed_lo = (uint32_t)(sk & 0xFFFFFFFFu), seed_hi = (uint32_t)(sk >> 32);
+
+  for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+    const int64_t m0 = tile * QT_ROWS;               // member-local
+    __syncthreads();
+    for (int i = tid; i < QT_ROWS * n_s; i += 256) {
+      const int row = i / n_s, kk = i - row * n_s;
+      const int64_t m = m0 + row;
+      sS[kk * QT_LD + row] = m < S ? __ldg(obs + (row0 + m) * d.n_obs + ooff + kk) : 0.f;
+    }
+    __syncthreads();
+    q_tile_forward<DQN>(d, sS, sW1, sB1, sWt, sW2, d.n_h, sB2, sWq, sBq, sH1, sH2, sQ, n_wave, n_w, n_ft, q_in, tid, ty,
+                        tx);
+    __syncthreads();
+    if (tid < QT_ROWS && m0 + tid < S) {
+      const int64_t r = m0 + tid, g = row0 + r;
+      float qv[QT_NA];
+#pragma unroll
+      for (int j = 0; j < QT_NA; ++j) qv[j] = sQ[tid * QT_NA + j];
+      float* qo = q + (g * d.A + a) * d.max_na;
+#pragma unroll
+      for (int j = 0; j < QT_NA; ++j)
+        if (j < d.max_na) qo[j] = j < n_a ? qv[j] : 0.f;
+      int pick = 0;
+      if (mode == 0) {
+        float best = qv[0];
+#pragma unroll
+        for (int j = 1; j < QT_NA; ++j)
+          if (j < n_a && qv[j] > best) { best = qv[j]; pick = j; }
+      } else {
+        float s = 0.f;
+#pragma unroll
+        for (int j = 0; j < QT_NA; ++j)
+          if (j < n_a) s = __fadd_rn(s, qv[j]);
+        bool ok = isfinite(s) && s != 0.f;
+        float p[QT_NA];
+#pragma unroll
+        for (int j = 0; j < QT_NA; ++j) {
+          p[j] = j < n_a ? __fdiv_rn(qv[j], s) : 0.f;
+          ok = ok && (j >= n_a || (p[j] >= 0.f && isfinite(p[j])));
+        }
+        if (ok) {
+          const float uu = (float)(q_row_hash(seed_lo, seed_hi, step, r, a) >> 8) * (1.0f / 16777216.0f);
+          float cum = 0.f;
+          bool found = false;
+          pick = n_a - 1;
+#pragma unroll
+          for (int j = 0; j < QT_NA; ++j) {
+            if (j < n_a) {
+              cum = __fadd_rn(cum, p[j]);
+              if (!found && uu < cum) { pick = j; found = true; }
+            }
+          }
+        } else if (bad) {
+          const unsigned long long key = ((unsigned long long)r << 40) | ((unsigned long long)(step & 0xFFFFFFu) << 16) |
+                                         (unsigned long long)a;
+          atomicMin(bad + k, key);
+        }
+      }
+      act[g * d.A + a] = pick;
+    }
+  }
+}
+
 
 // ================================================================================================
 // Training (IQL.backward, agents/models.py:305-312): minibatch sampler, fused TD forward / backward, reduction, clip + Adam.
@@ -729,6 +831,8 @@ extern "C" int tscl_q_create(const tscl_qdims* x, int32_t device, tscl_qhandle**
   if (h->ctas_per_sm < 1) h->ctas_per_sm = 1;
   const void* ex = dqn ? (const void*)q_fwd_kernel<true, true> : (const void*)q_fwd_kernel<false, true>;
   LCK(cudaFuncSetAttribute(ex, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem));
+  const void* fg = dqn ? (const void*)q_fwd_g_kernel<true> : (const void*)q_fwd_g_kernel<false>;
+  LCK(cudaFuncSetAttribute(fg, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem));
   const size_t td_smem = (size_t)q_td_smem_layout(d).total * sizeof(float);
   if (td_smem <= (size_t)optin) {
     const void* td = dqn ? (const void*)q_td_kernel<true> : (const void*)q_td_kernel<false>;
@@ -770,6 +874,29 @@ extern "C" int tscl_q_step(tscl_qhandle* h, const float* params, const float* ob
     q_fwd_kernel<false><<<grid, 256, h->smem, (cudaStream_t)stream>>>(h->d, params, obs, R, q, act, mode, lo, hi,
                                                                        (uint32_t)step, replica0, bad, 0.f, nullptr,
                                                                        nullptr);
+  LCK(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int tscl_q_step_g(tscl_qhandle* h, const float* params, int64_t p_stride, const float* obs, int32_t K,
+                             const int64_t* rows, int64_t R, float* q, int32_t* act, int32_t mode, const uint64_t* seeds,
+                             int64_t step, int64_t* bad_flags, void* stream) {
+  if (!h || !params || !obs || !rows || !seeds || !q || !act || K < 1 || K > 65535 || R < K || (mode != 0 && mode != 1) ||
+      (K > 1 && p_stride < h->n_params))
+    return tsc_set_error("tscl_q_step_g: bad argument");
+  LCK(cudaSetDevice(h->device));
+  // a member has at most ceil(R / 64) tiles; CTAs past a member's tiles return at once
+  const int64_t max_tiles = (R + QT_ROWS - 1) / QT_ROWS;
+  int64_t groups = ((int64_t)h->n_sm * h->ctas_per_sm + (int64_t)h->d.A * K - 1) / ((int64_t)h->d.A * K);
+  if (groups > max_tiles) groups = max_tiles;
+  dim3 grid((unsigned)groups, (unsigned)h->d.A, (unsigned)K);
+  unsigned long long* bad = reinterpret_cast<unsigned long long*>(bad_flags);
+  if (h->d.model == 1)
+    q_fwd_g_kernel<true><<<grid, 256, h->smem, (cudaStream_t)stream>>>(h->d, params, p_stride, obs, rows, q, act, mode,
+                                                                        seeds, (uint32_t)step, bad);
+  else
+    q_fwd_g_kernel<false><<<grid, 256, h->smem, (cudaStream_t)stream>>>(h->d, params, p_stride, obs, rows, q, act, mode,
+                                                                         seeds, (uint32_t)step, bad);
   LCK(cudaGetLastError());
   return 0;
 }

@@ -272,6 +272,17 @@ int tscl_policy_step_pi(tscl_handle* h, const float* params, const void* wpack_b
                         const float* c_in, const float* h_in, float* c_out, float* h_out, float* pi, int32_t* act,
                         int32_t act_mode, int32_t done, uint64_t seed, int64_t step, int64_t replica0, int64_t ld_state,
                         int64_t row0, void* stream);
+/* Grouped pi-only form: one launch for K members of one layout (the handle's), for evaluating several trained agents on
+ * one simulator.  rows: device array of K + 1 ascending row boundaries, rows[0] = 0, rows[K] = R; member k owns rows
+ * rows[k] .. rows[k+1] - 1 (any count >= 1: ragged, no padding) of obs [R][n_obs], pi [R][A][max_na], act [R][A] and the
+ * compact state [A][R][h] (out may alias in).  Member k reads params + k*p_stride and wpack + k*wp_stride and samples
+ * (act_mode 0) with seeds[k] (device array of K uint64) and its member-local replica r - rows[k]; act_mode 1 = first
+ * argmax.  Member k's pi, c, h and act are bit-identical to tscl_policy_step_pi on its own slice with seed seeds[k] and
+ * replica0 = 0.  Work items are (member, pi unit, 64-row tile of the member). */
+int tscl_policy_step_pi_g(tscl_handle* h, const float* params, int64_t p_stride, const void* wpack_bf16, int64_t wp_stride,
+                          const float* obs, int32_t K, const int64_t* rows, int64_t R, const float* c_in, const float* h_in,
+                          float* c_out, float* h_out, float* pi, int32_t* act, int32_t act_mode, int32_t done,
+                          const uint64_t* seeds, int64_t step, void* stream);
 /* Deterministic action choice for the forwards without a fused pi-only kernel (fc policy, v1 LSTM forward):
  * act[r][a] = first j < n_a[a] with the largest pi[r][a][j]; pi [R][A][max_na], act [R][A]. */
 int tscl_argmax_actions(tscl_handle* h, const float* pi, int64_t R, int32_t* act, void* stream);
@@ -324,6 +335,16 @@ int tscl_q_destroy(tscl_qhandle* h);
  * Replica-range form: pass obs + r0 * n_obs, q + r0 * A * max_na, act + r0 * A, R = n and replica0 = r0. */
 int tscl_q_step(tscl_qhandle* h, const float* params, const float* obs, int64_t R, float* q, int32_t* act, int32_t mode,
                 uint64_t seed, int64_t step, int64_t replica0, int64_t* bad_flag, void* stream);
+/* Grouped form: one launch for K members of one Q layout (the handle's).  rows: device array of K + 1 ascending row
+ * boundaries, rows[0] = 0, rows[K] = R; member k owns rows rows[k] .. rows[k+1] - 1 (ragged, any count >= 1) of obs, q
+ * and act, reads params + k*p_stride and keys its mode-1 draws with seeds[k] (device, K uint64) and its member-local
+ * replica r - rows[k].  bad_flags: NULL or a device array of K int64 (caller-initialised to -1); member k's failed
+ * samples go into bad_flags[k] with its own key, member-local replica << 40 | (step & 0xFFFFFF) << 16 | agent, so the
+ * member is the array index.  Member k's q, act and bad_flags[k] are bit-identical to tscl_q_step on its own slice with
+ * seed seeds[k] and replica0 = 0.  CTAs cover (tile group, agent, member). */
+int tscl_q_step_g(tscl_qhandle* h, const float* params, int64_t p_stride, const float* obs, int32_t K, const int64_t* rows,
+                  int64_t R, float* q, int32_t* act, int32_t mode, const uint64_t* seeds, int64_t step,
+                  int64_t* bad_flags, void* stream);
 
 /* ---- IQL training (IQL.explore / add_transition / backward, agents/models.py:305-376), same handle ----------------
  * Replay ring of one rank's R replicas, slot-major, capacity B: s / s1 [B][R][n_obs] fp32, a [B][R][A] int8,
