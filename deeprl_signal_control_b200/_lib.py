@@ -23,7 +23,7 @@ SYMBOLS = ["tsc_last_error", "tsc_create", "tsc_destroy", "tsc_reset", "tsc_set_
            "tscl_heads_loss", "tscl_lstm_seq_bwd", "tscl_fc_bwd", "tscl_fc_bwd_tc", "tscl_wgrad_tc", "tscl_clip_rmsprop",
            "tscl_pack_weights", "tscl_policy_step", "tscl_policy_step_v2", "tscl_policy_step_v2r", "tscl_policy_step_v2g", "tscl_unpack_store", "tscl_pack_wht", "tscl_lstm_seq_bwd_tc", "tscl_pack_wxt", "tscl_lstm_seq_bwd_tc_dx", "tscl_lstm_seq_bwd_tc_heads", "tscl_dx_tc", "tscl_dx_fc_bwd_tc", "tscl_host_transition", "tscl_device_transition", "tscl_device_transition_g","tscl_memcpy_async", "tscl_fc_hidden_fwd", "tscl_fc_hidden_bwd", "tscl_debug_policy_prof", "tscl_debug_bptt_prof",
            "tscl_policy_step_pi", "tscl_policy_step_pi_g", "tscl_argmax_actions", "tscl_q_create", "tscl_q_destroy",
-           "tscl_q_step", "tscl_q_step_g", "tscl_q_explore", "tscl_q_sample", "tscl_q_td", "tscl_q_adam", "tscl_q_transition"]
+           "tscl_q_info", "tscl_q_step", "tscl_q_step_g", "tscl_q_explore", "tscl_q_sample", "tscl_q_td", "tscl_q_adam", "tscl_q_transition"]
 
 
 def build_native(force: bool = False, verbose: bool = False) -> str:

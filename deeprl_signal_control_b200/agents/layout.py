@@ -247,6 +247,23 @@ class QLayout:
             out.append(v)
         return out
 
+    def smem_bytes(self):
+        """(forward, TD kernel) dynamic shared memory per CTA of the Q kernels for this layout: q_smem_layout and
+        q_td_smem_layout of csrc/tsc_q.cu restated, whether or not it fits (tscl_q_info reports the handle's figures,
+        0 for a TD kernel that does not fit)."""
+        rows, ld, na = 64, 68, 8                       # QT_ROWS, QT_LD, QT_NA
+        s_max = int(self.n_s.max())
+        dqn = self.model_type == "dqn"
+        wave_max = int((self.n_s - self.n_w).max()) if dqn else 0
+        w_max = int(self.n_w.max()) if dqn else 0
+        h1w = self.n_fc + self.n_ft
+        q_in = self.n_h if dqn else s_max
+        p = wave_max * self.n_fc + h1w + w_max * self.n_ft + h1w * self.n_h + self.n_h + q_in * na + na
+        p = (p + 3) & ~3
+        fwd = p + s_max * ld + h1w * ld + self.n_h * ld + rows * na
+        td = fwd + h1w * (self.n_h + 1) + wave_max * self.n_fc + h1w + w_max * self.n_ft + self.n_h + q_in * na + na + 3 * rows
+        return 4 * fwd, 4 * td
+
     def as_c(self) -> CQDims:
         c = CQDims()
         c.n_agents, c.n_obs, c.max_na = self.A, self.n_obs, self.max_na

@@ -64,6 +64,22 @@ class BatchedIQL:
         if need > free:
             raise MemoryError("BatchedIQL: the replay rings need %.2f GB (R=%d x buffer_size=%d x (8 n_obs + 5 A + 1) "
                               "bytes) but the device has %.2f GB free" % (need / 1e9, self.R, self.B, free / 1e9))
+        self._h = C.c_void_p()
+        _lib.check(_lib.lib().tscl_q_create(C.byref(layout.as_c()), C.c_int32(self.dev.index or 0), C.byref(self._h)))
+        fwd_smem, td_smem = C.c_int64(), C.c_int64()
+        _lib.check(_lib.lib().tscl_q_info(self._h, C.byref(fwd_smem), C.byref(td_smem)))
+        if td_smem.value == 0:
+            # the forward fits but the TD kernel does not: refuse here rather than at the first td_round
+            _lib.lib().tscl_q_destroy(self._h)
+            self._h = None
+            n_wave = layout.n_s - layout.n_w
+            i = int(np.argmax(n_wave))
+            raise ValueError(
+                "BatchedIQL: the TD kernel holds one agent's weights, their gradients and a 64-row tile in shared memory; "
+                "with the widest wave block (agent %d: %d wave + %d wait inputs, widths num_fc %d / %d / num_h %d) that "
+                "needs %d bytes per CTA but the device has %d.  Evaluation (Evaluator, tscl_q_step) accepts this layout."
+                % (i, int(n_wave[i]), int(layout.n_w[i]), layout.n_fc, layout.n_ft, layout.n_h, layout.smem_bytes()[1],
+                   torch.cuda.get_device_properties(self.dev).shared_memory_per_block_optin))
         f32 = dict(dtype=torch.float32, device=self.dev)
         self.P = torch.from_numpy(self.initial_params(layout, model_config, model_type, seed)).to(self.dev)
         self.nets = layout.views(self.P)
@@ -84,8 +100,6 @@ class BatchedIQL:
         self.losses = torch.zeros(N_ROUNDS, A, **f32)
         self.norms = torch.zeros(N_ROUNDS, A, **f32)
         self.n_updates = 0                             # backwards that ran (keys the minibatch draws)
-        self._h = C.c_void_p()
-        _lib.check(_lib.lib().tscl_q_create(C.byref(layout.as_c()), C.c_int32(self.dev.index or 0), C.byref(self._h)))
 
     @staticmethod
     def initial_params(layout: QLayout, model_config, model_type: str, seed: int) -> np.ndarray:

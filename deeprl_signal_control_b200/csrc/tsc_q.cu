@@ -854,6 +854,13 @@ extern "C" int tscl_q_destroy(tscl_qhandle* h) {
   return 0;
 }
 
+extern "C" int tscl_q_info(tscl_qhandle* h, int64_t* fwd_smem_bytes, int64_t* td_smem_bytes) {
+  if (!h || !fwd_smem_bytes || !td_smem_bytes) return tsc_set_error("tscl_q_info: bad argument");
+  *fwd_smem_bytes = (int64_t)h->smem;
+  *td_smem_bytes = (int64_t)h->td_smem;
+  return 0;
+}
+
 extern "C" int tscl_q_step(tscl_qhandle* h, const float* params, const float* obs, int64_t R, float* q, int32_t* act,
                            int32_t mode, uint64_t seed, int64_t step, int64_t replica0, int64_t* bad_flag, void* stream) {
   if (!h || !params || !obs || !q || !act || R <= 0 || replica0 < 0 || (mode != 0 && mode != 1))

@@ -323,6 +323,10 @@ typedef struct tscl_qhandle tscl_qhandle;
 
 int tscl_q_create(const tscl_qdims* dims, int32_t device, tscl_qhandle** out);
 int tscl_q_destroy(tscl_qhandle* h);
+/* Dynamic shared memory per CTA of the handle's kernels: the forward (tscl_q_step, _step_g, _explore) and the TD kernel
+ * (tscl_q_td).  tscl_q_create refuses a layout whose forward does not fit a CTA; one whose TD kernel does not fit is
+ * accepted for evaluation and reports td_smem_bytes = 0 (tscl_q_td then refuses it). */
+int tscl_q_info(tscl_qhandle* h, int64_t* fwd_smem_bytes, int64_t* td_smem_bytes);
 /* One decision of IQL.forward(obs, mode='act', stochastic) (agents/models.py:347-363) for R replicas:
  *   obs [R][n_obs] -> q [R][A][max_na] (zero padded), act [R][A].
  *   mode 0: act = the first maximum of q (np.argmax; policy types 'default' and 'deterministic', utils.py:221-225).

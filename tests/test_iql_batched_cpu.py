@@ -49,17 +49,24 @@ def q_td_ref(w, kind, n_w, S, A, S1, Rw, D, gamma, n_total=None, max_norm=40.0, 
     norm = float(torch.sqrt(sum((x * x).sum() for x in g.values())))
     out = dict(q=q.detach().numpy(), err=err.detach().numpy(), loss=float(loss.detach()), grads={k: v.numpy() for k, v in g.items()}, norm=norm)
     if adam is not None:
-        scale = max_norm / max(norm, max_norm) if max_norm > 0 else 1.0
-        t = adam["t"] + 1
-        lr_t = lr * np.sqrt(1 - 0.999 ** t) / (1 - 0.9 ** t)
-        new_w, m, v = {}, {}, {}
-        for k in keys:
-            gk = g[k].numpy() * scale
-            m[k] = adam["m"][k] + (gk - adam["m"][k]) * 0.1
-            v[k] = adam["v"][k] + (gk * gk - adam["v"][k]) * 0.001
-            new_w[k] = w[k].detach().numpy() - lr_t * m[k] / (np.sqrt(v[k]) + 1e-8)
-        out.update(w=new_w, adam=dict(t=t, m=m, v=v))
+        new_w, new_adam = adam_ref({k: v.detach().numpy() for k, v in w.items()}, out["grads"], norm, adam, lr, max_norm)
+        out.update(w=new_w, adam=new_adam)
     return out
+
+
+def adam_ref(w, grads, norm, adam, lr, max_norm):
+    """tf.clip_by_global_norm of grads (global norm `norm`) and one TF1 Adam step from adam = {'t', 'm', 'v'}, float64:
+    (new weights, new adam state)"""
+    scale = max_norm / max(norm, max_norm) if max_norm > 0 else 1.0
+    t = adam["t"] + 1
+    lr_t = lr * np.sqrt(1 - 0.999 ** t) / (1 - 0.9 ** t)
+    new_w, m, v = {}, {}, {}
+    for k in w:
+        gk = np.asarray(grads[k], np.float64) * scale
+        m[k] = adam["m"][k] + (gk - adam["m"][k]) * 0.1
+        v[k] = adam["v"][k] + (gk * gk - adam["v"][k]) * 0.001
+        new_w[k] = np.asarray(w[k], np.float64) - lr_t * m[k] / (np.sqrt(v[k]) + 1e-8)
+    return new_w, dict(t=t, m=m, v=v)
 
 
 def golden_batches(z, kind, k, i):
