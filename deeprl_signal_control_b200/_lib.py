@@ -1,29 +1,62 @@
-"""Loader of the native library (csrc/libtsc.so, C ABI of include/tsc.h).
+"""Loader of the native library (csrc/libtsc.so, C ABI of include/tsc.h and include/tsc_learn.h).
 
 There is deliberately NO fallback: if the CUDA library is missing or does not load, importing
 the simulator fails loudly (the product path never routes through a CPU implementation).
+
+The headers are the one statement of the ABI: every function they declare gets its ctypes `argtypes` / `restype` from
+its prototype when the library loads, so callers pass plain values (Python ints / floats / bools, `ptr(t)`, None,
+`ctypes.byref(...)`) and a call with too few arguments or a value of the wrong kind raises in Python before any launch.
 """
 from __future__ import annotations
 
 import ctypes as C
 import os
+import re
 import subprocess
+
+import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(_HERE, "csrc")
+INCLUDE = os.path.join(os.path.dirname(_HERE), "include")
+HEADERS = ("tsc.h", "tsc_learn.h")
 LIB_PATH = os.environ.get("TSC_LIB", os.path.join(CSRC, "libtsc.so"))   # TSC_LIB: tuning variants only
 _lib = None
 
-# every symbol include/tsc.h declares
-SYMBOLS = ["tsc_last_error", "tsc_create", "tsc_destroy", "tsc_reset", "tsc_set_train_mode",
-           "tsc_set_replica_coop_gamma", "tsc_observe", "tsc_step", "tsc_step_host", "tsc_step_host_range", "tsc_step_host_range_async", "tsc_set_record", "tsc_step_record", "tsc_get_trips", "tsc_get_counts", "tsc_get_traffic_stats",
-           "tsc_dump_state", "tsc_info", "tsc_mean_live", "tsc_set_greedy_program", "tsc_greedy_actions",
-           # include/tsc_learn.h
-           "tscl_create", "tscl_destroy", "tscl_fc_embed", "tscl_lstm_seq_fwd", "tscl_heads", "tscl_returns", "tscl_returns_g",
-           "tscl_heads_loss", "tscl_lstm_seq_bwd", "tscl_fc_bwd", "tscl_fc_bwd_tc", "tscl_wgrad_tc", "tscl_clip_rmsprop",
-           "tscl_pack_weights", "tscl_policy_step", "tscl_policy_step_v2", "tscl_policy_step_v2r", "tscl_policy_step_v2g", "tscl_unpack_store", "tscl_pack_wht", "tscl_lstm_seq_bwd_tc", "tscl_pack_wxt", "tscl_lstm_seq_bwd_tc_dx", "tscl_lstm_seq_bwd_tc_heads", "tscl_dx_tc", "tscl_dx_fc_bwd_tc", "tscl_host_transition", "tscl_device_transition", "tscl_device_transition_g","tscl_memcpy_async", "tscl_fc_hidden_fwd", "tscl_fc_hidden_bwd", "tscl_debug_policy_prof", "tscl_debug_bptt_prof",
-           "tscl_policy_step_pi", "tscl_policy_step_pi_g", "tscl_argmax_actions", "tscl_q_create", "tscl_q_destroy",
-           "tscl_q_info", "tscl_q_step", "tscl_q_step_g", "tscl_q_explore", "tscl_q_sample", "tscl_q_td", "tscl_q_adam", "tscl_q_transition"]
+# C parameter types of the headers; every pointer (T*, const T*, T**, handles, structs) is a c_void_p
+SCALAR_TYPES = {"int32_t": C.c_int32, "int64_t": C.c_int64, "uint64_t": C.c_uint64, "float": C.c_float}
+RESULT_TYPES = {"int": C.c_int, "const char*": C.c_char_p}
+
+
+def _param_type(fn: str, decl: str):
+    if "*" in decl:
+        return C.c_void_p
+    words = decl.split()
+    if words[0] == "const":
+        words = words[1:]
+    if len(words) != 2 or words[0] not in SCALAR_TYPES:
+        raise ImportError("%s: no ctypes mapping for parameter `%s` (add its type to _lib.SCALAR_TYPES)" % (fn, decl))
+    return SCALAR_TYPES[words[0]]
+
+
+def _prototypes() -> dict:
+    """{name: (restype, [argtypes])} of every function the headers declare, in declaration order."""
+    protos = {}
+    for header in HEADERS:
+        path = os.path.join(INCLUDE, header)
+        if not os.path.exists(path):
+            raise ImportError("C header %s is missing: the loader takes the library's prototypes from it" % path)
+        src = re.sub(r"/\*.*?\*/", "", open(path).read(), flags=re.S)
+        for ret, fn, params in re.findall(r"^\s*(int|const char\*)\s+(tscl?_[a-z0-9_]+)\s*\(([^)]*)\)\s*;", src,
+                                          flags=re.M):
+            params = " ".join(params.split())
+            protos[fn] = (RESULT_TYPES[ret],
+                          [] if params in ("", "void") else [_param_type(fn, p.strip()) for p in params.split(",")])
+    return protos
+
+
+PROTOTYPES = _prototypes()
+SYMBOLS = list(PROTOTYPES)
 
 
 def build_native(force: bool = False, verbose: bool = False) -> str:
@@ -44,11 +77,22 @@ def lib() -> C.CDLL:
             raise ImportError(
                 "native library %s is missing: run `python -c 'import __graft_entry__ as g; g.build()'` "
                 "(there is no CPU fallback)" % LIB_PATH)
-        _lib = C.CDLL(LIB_PATH)
-        _lib.tsc_last_error.restype = C.c_char_p
-        for s in SYMBOLS:
-            getattr(_lib, s)  # AttributeError here = ABI drift
+        so = C.CDLL(LIB_PATH)
+        for name, (restype, argtypes) in PROTOTYPES.items():
+            fn = getattr(so, name)  # AttributeError here = ABI drift
+            fn.restype, fn.argtypes = restype, argtypes
+        _lib = so
     return _lib
+
+
+def ptr(t):
+    """Address of tensor `t` as a pointer argument (None: NULL)."""
+    return None if t is None else t.data_ptr()
+
+
+def stream(device=None):
+    """Handle of torch's current CUDA stream on `device`, the `void* stream` argument of the entry points."""
+    return torch.cuda.current_stream(device).cuda_stream
 
 
 def check(rc: int):

@@ -33,8 +33,7 @@ import torch
 from .. import _lib
 
 
-def _p(t):
-    return None if t is None else C.c_void_p(t.data_ptr())
+_p = _lib.ptr
 
 
 def replica_seeds(env):
@@ -137,8 +136,7 @@ class Evaluator:
             prog = model.greedy_program(net.node_obs_off)
             max_cand, off, idx, act = (int(prog[0]),) + tuple(np.ascontiguousarray(a, np.int32) for a in prog[1:])
             _lib.check(_lib.lib().tsc_set_greedy_program(
-                sim._h, C.c_int32(max_cand), off.ctypes.data_as(C.POINTER(C.c_int32)),
-                idx.ctypes.data_as(C.POINTER(C.c_int32)), act.ctypes.data_as(C.POINTER(C.c_int32))))
+                sim._h, max_cand, off.ctypes.data, idx.ctypes.data, act.ctypes.data))
             return
         if name == 'iql':
             self._init_q(model, net)
@@ -186,7 +184,7 @@ class Evaluator:
         self.family = 'q'
         self.qlay = QLayout.from_iql(model, off, self.n_obs, max_na=self.max_na)
         self._qh = C.c_void_p()
-        _lib.check(_lib.lib().tscl_q_create(C.byref(self.qlay.as_c()), C.c_int32(self.dev.index or 0), C.byref(self._qh)))
+        _lib.check(_lib.lib().tscl_q_create(C.byref(self.qlay.as_c()), self.dev.index or 0, C.byref(self._qh)))
         self.params = torch.zeros(self.qlay.n_params, dtype=torch.float32, device=self.dev)
         self.q = torch.zeros(self.R, self.N, self.max_na, dtype=torch.float32, device=self.dev)
         self.bad = torch.full((1,), -1, dtype=torch.int64, device=self.dev)
@@ -198,7 +196,7 @@ class Evaluator:
             self._qh = None
 
     def _st(self):
-        return C.c_void_p(torch.cuda.current_stream(self.dev).cuda_stream)
+        return _lib.stream(self.dev)
 
     # ---- one decision for all replicas -----------------------------------------------------------
     def _actions(self, step: int):
@@ -207,32 +205,30 @@ class Evaluator:
             _lib.check(lib.tsc_greedy_actions(self.sim._h, _p(self.obs), _p(self.act), self._st()))
             return None
         if self.family == 'q':
-            _lib.check(lib.tscl_q_step(self._qh, _p(self.params), _p(self.obs), C.c_int64(self.R), _p(self.q),
-                                       _p(self.act), C.c_int32(int(self.policy_type == 'stochastic')),
-                                       C.c_uint64(self.seed), C.c_int64(step), C.c_int64(0), _p(self.bad), self._st()))
+            _lib.check(lib.tscl_q_step(self._qh, _p(self.params), _p(self.obs), self.R, _p(self.q), _p(self.act),
+                                       int(self.policy_type == 'stochastic'), self.seed, step, 0, _p(self.bad),
+                                       self._st()))
             return None
         b, R, done = self.b, self.R, 1 if step == 0 else 0
         argmax = self.policy_type == 'deterministic'
-        seed, stp = C.c_uint64(self.seed), C.c_int64(step)
+        seed, stp = self.seed, step
         if self.family == 'v2':
-            _lib.check(lib.tscl_policy_step_pi(b._h, _p(b.P), _p(b.Wp), _p(self.obs), C.c_int64(R), _p(self.c), _p(self.h),
-                                               _p(self.c), _p(self.h), _p(self.pi), _p(self.act), C.c_int32(int(argmax)),
-                                               C.c_int32(done), seed, stp, C.c_int64(0), C.c_int64(0), C.c_int64(0),
-                                               self._st()))
+            _lib.check(lib.tscl_policy_step_pi(b._h, _p(b.P), _p(b.Wp), _p(self.obs), R, _p(self.c), _p(self.h),
+                                               _p(self.c), _p(self.h), _p(self.pi), _p(self.act), int(argmax), done,
+                                               seed, stp, 0, 0, 0, self._st()))
             return self.pi
         act = None if argmax else _p(self.act)
         if self.family == 'v1':
-            _lib.check(lib.tscl_policy_step(b._h, _p(b.P), _p(b.Wp), _p(self.obs), C.c_int64(R), _p(self.c), _p(self.h),
-                                            _p(self.c), _p(self.h), _p(self.pi), _p(self.val), act, C.c_int32(done), seed,
-                                            stp, C.c_int64(0), None, C.c_int32(0), self._st()))
+            _lib.check(lib.tscl_policy_step(b._h, _p(b.P), _p(b.Wp), _p(self.obs), R, _p(self.c), _p(self.h),
+                                            _p(self.c), _p(self.h), _p(self.pi), _p(self.val), act, done, seed, stp, 0,
+                                            None, 0, self._st()))
         else:
-            _lib.check(lib.tscl_fc_embed(b._h, _p(b.P), _p(self.obs), C.c_int64(R), C.c_int64(R), C.c_int64(0), _p(self.X),
-                                         self._st()))
-            _lib.check(lib.tscl_fc_hidden_fwd(b._h, _p(b.P), _p(self.X), C.c_int64(R), _p(self.H), self._st()))
-            _lib.check(lib.tscl_heads(b._h, _p(b.P), _p(self.H), C.c_int64(R), _p(self.pi), _p(self.val), act, seed, stp,
-                                      C.c_int64(0), self._st()))
+            _lib.check(lib.tscl_fc_embed(b._h, _p(b.P), _p(self.obs), R, R, 0, _p(self.X), self._st()))
+            _lib.check(lib.tscl_fc_hidden_fwd(b._h, _p(b.P), _p(self.X), R, _p(self.H), self._st()))
+            _lib.check(lib.tscl_heads(b._h, _p(b.P), _p(self.H), R, _p(self.pi), _p(self.val), act, seed, stp, 0,
+                                      self._st()))
         if argmax:
-            _lib.check(lib.tscl_argmax_actions(b._h, _p(self.pi), C.c_int64(R), _p(self.act), self._st()))
+            _lib.check(lib.tscl_argmax_actions(b._h, _p(self.pi), R, _p(self.act), self._st()))
         return self.pi
 
     def _episode(self):
@@ -573,13 +569,12 @@ class _Group:
             prog = self.models[i].greedy_program(self.entries[i].env._tables.node_obs_off)
             max_cand, off, idx, act = (int(prog[0]),) + tuple(np.ascontiguousarray(a, np.int32) for a in prog[1:])
             _lib.check(lib.tsc_set_greedy_program(
-                self.sim._h, C.c_int32(max_cand), off.ctypes.data_as(C.POINTER(C.c_int32)),
-                idx.ctypes.data_as(C.POINTER(C.c_int32)), act.ctypes.data_as(C.POINTER(C.c_int32))))
+                self.sim._h, max_cand, off.ctypes.data, idx.ctypes.data, act.ctypes.data))
         elif kind == 'q':
             m0, net = self.models[i], self.entries[i].env._tables
             qlay = QLayout.from_iql(m0, np.asarray(net.node_obs_off), self.n_obs, max_na=self.max_na)
             h = C.c_void_p()
-            _lib.check(lib.tscl_q_create(C.byref(qlay.as_c()), C.c_int32(self.dev.index or 0), C.byref(h)))
+            _lib.check(lib.tscl_q_create(C.byref(qlay.as_c()), self.dev.index or 0, C.byref(h)))
             st.update(h=h, qlay=qlay, rows=self._rows(i, j), seeds=self._seeds(i, j),
                       params=torch.stack([qlay.pack(self.models[k].nets).to(self.dev) for k in range(i, j)]).contiguous(),
                       q=torch.zeros(n, self.N, self.max_na, **f32),
@@ -606,43 +601,40 @@ class _Group:
                 st['h'] = C.c_void_p()
 
     def _st(self):
-        return C.c_void_p(torch.cuda.current_stream(self.dev).cuda_stream)
+        return _lib.stream(self.dev)
 
     def _actions(self, t):
-        lib, done, stp = _lib.lib(), 1 if t == 0 else 0, C.c_int64(t)
+        lib, done, stp = _lib.lib(), 1 if t == 0 else 0, t
         for kind, st in self.fwd:
             r0, n = st['i'] * self.S, st['n']
             obs, pi, act = self.obs[r0:r0 + n], self.pi[r0:r0 + n], self.act[r0:r0 + n]
             if kind == 'greedy':
                 _lib.check(lib.tsc_greedy_actions(self.sim._h, _p(self.obs), _p(self.act), self._st()))
             elif kind == 'q':
-                _lib.check(lib.tscl_q_step_g(st['h'], _p(st['params']), C.c_int64(st['qlay'].n_params), _p(obs),
-                                             C.c_int32(st['j'] - st['i']), _p(st['rows']), C.c_int64(n), _p(st['q']),
-                                             _p(act), C.c_int32(int(self.ge.policy_type == 'stochastic')),
-                                             _p(st['seeds']), stp, _p(st['bad']), self._st()))
+                _lib.check(lib.tscl_q_step_g(st['h'], _p(st['params']), st['qlay'].n_params, _p(obs), st['j'] - st['i'],
+                                             _p(st['rows']), n, _p(st['q']), _p(act),
+                                             int(self.ge.policy_type == 'stochastic'), _p(st['seeds']), stp,
+                                             _p(st['bad']), self._st()))
             elif kind == 'v2':
                 b = st['b']
                 _lib.check(lib.tscl_policy_step_pi_g(
-                    b._h, _p(st['P']), C.c_int64(st['P'].shape[1]), _p(st['Wp']), C.c_int64(st['Wp'][0].numel()), _p(obs),
-                    C.c_int32(st['j'] - st['i']), _p(st['rows']), C.c_int64(n), _p(st['c']), _p(st['h']), _p(st['c']),
-                    _p(st['h']), _p(pi), _p(act), C.c_int32(int(self.argmax)), C.c_int32(done), _p(st['seeds']), stp,
-                    self._st()))
+                    b._h, _p(st['P']), st['P'].shape[1], _p(st['Wp']), st['Wp'][0].numel(), _p(obs), st['j'] - st['i'],
+                    _p(st['rows']), n, _p(st['c']), _p(st['h']), _p(st['c']), _p(st['h']), _p(pi), _p(act),
+                    int(self.argmax), done, _p(st['seeds']), stp, self._st()))
             else:
-                b, seed = st['b'], C.c_uint64(self.entries[st['i']].seed)
+                b, seed = st['b'], self.entries[st['i']].seed
                 a = None if self.argmax else _p(act)
                 if kind == 'v1':
-                    _lib.check(lib.tscl_policy_step(b._h, _p(b.P), _p(b.Wp), _p(obs), C.c_int64(n), _p(st['c']),
-                                                    _p(st['h']), _p(st['c']), _p(st['h']), _p(pi), _p(st['val']), a,
-                                                    C.c_int32(done), seed, stp, C.c_int64(0), None, C.c_int32(0),
-                                                    self._st()))
+                    _lib.check(lib.tscl_policy_step(b._h, _p(b.P), _p(b.Wp), _p(obs), n, _p(st['c']), _p(st['h']),
+                                                    _p(st['c']), _p(st['h']), _p(pi), _p(st['val']), a, done, seed, stp,
+                                                    0, None, 0, self._st()))
                 else:
-                    _lib.check(lib.tscl_fc_embed(b._h, _p(b.P), _p(obs), C.c_int64(n), C.c_int64(n), C.c_int64(0),
-                                                 _p(st['X']), self._st()))
-                    _lib.check(lib.tscl_fc_hidden_fwd(b._h, _p(b.P), _p(st['X']), C.c_int64(n), _p(st['H']), self._st()))
-                    _lib.check(lib.tscl_heads(b._h, _p(b.P), _p(st['H']), C.c_int64(n), _p(pi), _p(st['val']), a, seed,
-                                              stp, C.c_int64(0), self._st()))
+                    _lib.check(lib.tscl_fc_embed(b._h, _p(b.P), _p(obs), n, n, 0, _p(st['X']), self._st()))
+                    _lib.check(lib.tscl_fc_hidden_fwd(b._h, _p(b.P), _p(st['X']), n, _p(st['H']), self._st()))
+                    _lib.check(lib.tscl_heads(b._h, _p(b.P), _p(st['H']), n, _p(pi), _p(st['val']), a, seed, stp, 0,
+                                              self._st()))
                 if self.argmax:
-                    _lib.check(lib.tscl_argmax_actions(b._h, _p(pi), C.c_int64(n), _p(act), self._st()))
+                    _lib.check(lib.tscl_argmax_actions(b._h, _p(pi), n, _p(act), self._st()))
 
     def _episode(self, record):
         sim, lib = self.sim, _lib.lib()

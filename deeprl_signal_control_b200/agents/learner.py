@@ -48,8 +48,7 @@ from .. import dist as _dist
 from .layout import PolicyLayout
 
 
-def _p(t):
-    return None if t is None else C.c_void_p(t.data_ptr())
+_p = _lib.ptr
 
 
 def check_population(seeds, seed, n_replicas, chunk, process_group):
@@ -184,7 +183,7 @@ class BatchedA2C:
         lib = _lib.lib()
         self._cd = layout.as_c()
         h = C.c_void_p()
-        _lib.check(lib.tscl_create(C.byref(self._cd), C.c_int32(device), C.byref(h)))
+        _lib.check(lib.tscl_create(C.byref(self._cd), device, C.byref(h)))
         self._h = h
         L, R, T, U, A = layout, self.R, self.T, layout.U, layout.A
         f32 = dict(dtype=torch.float32, device=self.dev)
@@ -311,7 +310,7 @@ class BatchedA2C:
         return [v] * self.K
 
     def _st(self):
-        return C.c_void_p(torch.cuda.current_stream(self.dev).cuda_stream)
+        return _lib.stream(self.dev)
 
     def pack_weights(self):
         if self.K > 1:
@@ -355,11 +354,10 @@ class BatchedA2C:
             store = commit and self.t < self.T
             st = (_p(self.st_x), _p(self.st_g), _p(self.st_c), _p(self.st_h)) if store else (None,) * 4
             _lib.check(lib.tscl_policy_step_v2g(
-                self._h, _p(self.P), C.c_int64(self.P.shape[1]), _p(self.Wp), C.c_int64(self.Wp[0].numel()), _p(obs),
-                C.c_int32(self.K), C.c_int64(self.R_m), _p(self.c_fw), _p(self.h_fw), _p(c1), _p(h1), _p(self.pi),
-                _p(val_o), _p(act_o) if want_act else None, C.c_int32(1 if done else 0), _p(self.seeds_dev),
-                C.c_int64(self.n_forward), *st, C.c_int32(self.t if store else 0), C.c_int32(self.T),
-                C.c_int64(self.chunk), self._st()))
+                self._h, _p(self.P), self.P.shape[1], _p(self.Wp), self.Wp[0].numel(), _p(obs), self.K, self.R_m,
+                _p(self.c_fw), _p(self.h_fw), _p(c1), _p(h1), _p(self.pi), _p(val_o), _p(act_o) if want_act else None,
+                1 if done else 0, _p(self.seeds_dev), self.n_forward, *st, self.t if store else 0, self.T, self.chunk,
+                self._st()))
             if store:
                 self._acts_ok[self.t] = True
             self.kernel_launches += 1
@@ -369,19 +367,17 @@ class BatchedA2C:
             return self.pi, val_o, (act_o if want_act else None)
         if self.use_tc:
             c1, h1 = (self.c_fw, self.h_fw) if commit else (self.c_tmp, self.h_tmp)
-            args = (self._h, _p(self.P), _p(self.Wp), _p(obs), C.c_int64(R), _p(self.c_fw), _p(self.h_fw), _p(c1),
+            args = (self._h, _p(self.P), _p(self.Wp), _p(obs), R, _p(self.c_fw), _p(self.h_fw), _p(c1),
                     _p(h1), _p(self.pi), _p(val_o), _p(act_o) if want_act else None,
-                    C.c_int32(1 if done else 0), C.c_uint64(self.seed), C.c_int64(self.n_forward),
-                    C.c_int64(self.replica0), None)
+                    1 if done else 0, self.seed, self.n_forward, self.replica0, None)
             if self.tc_v2:
                 store = self.store_acts and commit and self.t < self.T
                 st = (_p(self.st_x), _p(self.st_g), _p(self.st_c), _p(self.st_h)) if store else (None,) * 4
-                _lib.check(lib.tscl_policy_step_v2(*args, *st, C.c_int32(self.t if store else 0), C.c_int32(self.T),
-                                                   C.c_int64(self.chunk), self._st()))
+                _lib.check(lib.tscl_policy_step_v2(*args, *st, self.t if store else 0, self.T, self.chunk, self._st()))
                 if commit and self.t < self.T:
                     self._acts_ok[self.t] = store
             else:
-                _lib.check(lib.tscl_policy_step(*args, C.c_int32(0), self._st()))
+                _lib.check(lib.tscl_policy_step(*args, 0, self._st()))
             self.kernel_launches += 1
             if commit:
                 self.n_forward += 1
@@ -389,16 +385,14 @@ class BatchedA2C:
             return self.pi, val_o, (act_o if want_act else None)
         self._mm()
         dflag = self._one.fill_(1.0 if done else 0.0)
-        _lib.check(lib.tscl_fc_embed(self._h, _p(self.P), _p(obs), C.c_int64(R), C.c_int64(R), C.c_int64(0),
-                                     _p(self.X1), self._st()))
+        _lib.check(lib.tscl_fc_embed(self._h, _p(self.P), _p(obs), R, R, 0, _p(self.X1), self._st()))
         torch.baddbmm(self.pv["bl"].unsqueeze(1), self.X1, self.pv["wx"], out=self.Z1)
         c1, h1 = (self.c_fw, self.h_fw) if commit else (self.c_tmp, self.h_tmp)
         _lib.check(lib.tscl_lstm_seq_fwd(self._h, _p(self.P), _p(self.Z1), None, _p(self.H1), None, _p(self.c_fw),
-                                         _p(self.h_fw), _p(c1), _p(h1), _p(dflag), C.c_int32(1), C.c_int64(R),
-                                         C.c_int64(R), C.c_int64(0), self._st()))
-        _lib.check(lib.tscl_heads(self._h, _p(self.P), _p(self.H1), C.c_int64(R), _p(self.pi), _p(self.val),
-                                  _p(self.act) if want_act else None, C.c_uint64(self.seed),
-                                  C.c_int64(self.n_forward), C.c_int64(self.replica0), self._st()))
+                                         _p(self.h_fw), _p(c1), _p(h1), _p(dflag), 1, R, R, 0, self._st()))
+        _lib.check(lib.tscl_heads(self._h, _p(self.P), _p(self.H1), R, _p(self.pi), _p(self.val),
+                                  _p(self.act) if want_act else None, self.seed, self.n_forward, self.replica0,
+                                  self._st()))
         self.kernel_launches += 3
         if commit:
             self.n_forward += 1
@@ -416,15 +410,13 @@ class BatchedA2C:
         L, R, A = self.lay, self.R, self.lay.A
         store = self.store_acts and t < self.T
         st = (_p(self.st_x), _p(self.st_g), _p(self.st_c), _p(self.st_h)) if store else (None,) * 4
-        off = lambda t_, per_row: C.c_void_p(t_.data_ptr() + r0 * per_row * t_.element_size())
+        off = lambda t_, per_row: t_.data_ptr() + r0 * per_row * t_.element_size()
         _lib.check(_lib.lib().tscl_policy_step_v2r(
-            self._h, _p(self.P), _p(self.Wp), off(self.obs_hist[t], L.n_obs), C.c_int64(n),
-            off(self.c_fw, L.h), off(self.h_fw, L.h), off(self.c_fw, L.h), off(self.h_fw, L.h),
-            off(self.pi, A * L.max_na), off(self.val_hist[t] if to_hist else self.val, A),
-            off(self.act_hist[t] if to_hist else self.act, A), C.c_int32(1 if done else 0),
-            C.c_uint64(self.seed), C.c_int64(n_forward), C.c_int64(self.replica0 + r0), None, *st,
-            C.c_int32(t if store else 0), C.c_int32(self.T), C.c_int64(self.chunk), C.c_int64(R), C.c_int64(r0),
-            self._st() if stream is None else stream))
+            self._h, _p(self.P), _p(self.Wp), off(self.obs_hist[t], L.n_obs), n, off(self.c_fw, L.h),
+            off(self.h_fw, L.h), off(self.c_fw, L.h), off(self.h_fw, L.h), off(self.pi, A * L.max_na),
+            off(self.val_hist[t] if to_hist else self.val, A), off(self.act_hist[t] if to_hist else self.act, A),
+            1 if done else 0, self.seed, n_forward, self.replica0 + r0, None, *st, t if store else 0, self.T,
+            self.chunk, R, r0, self._st() if stream is None else stream))
         self.kernel_launches += 1
         if t < self.T:
             self._acts_ok[t] = store
@@ -487,12 +479,12 @@ class BatchedA2C:
         t = self.t
         if self.rscale_differs:
             _lib.check(_lib.lib().tscl_device_transition_g(
-                self._h, _p(reward), _p(self.rew_hist[t]), C.c_int64(reward.numel()), _p(self.rnorm_dev),
-                _p(self.rclip_dev), C.c_int32(self.K), _p(greward), _p(rew_acc), C.c_int64(greward.numel()), self._st()))
+                self._h, _p(reward), _p(self.rew_hist[t]), reward.numel(), _p(self.rnorm_dev), _p(self.rclip_dev),
+                self.K, _p(greward), _p(rew_acc), greward.numel(), self._st()))
         else:
             _lib.check(_lib.lib().tscl_device_transition(
-                self._h, _p(reward), _p(self.rew_hist[t]), C.c_int64(reward.numel()), C.c_float(self.reward_norm or 0.0),
-                C.c_float(self.reward_clip or 0.0), _p(greward), _p(rew_acc), C.c_int64(greward.numel()), self._st()))
+                self._h, _p(reward), _p(self.rew_hist[t]), reward.numel(), self.reward_norm or 0.0,
+                self.reward_clip or 0.0, _p(greward), _p(rew_acc), greward.numel(), self._st()))
         if not getattr(self, "_hist_direct", False):
             self.act_hist[t].copy_(self.act)
             self.val_hist[t].copy_(self.val)
@@ -544,9 +536,8 @@ class BatchedA2C:
         ci, R, A = r0 // self.chunk, self.R, self.lay.A
         _lib.check(_lib.lib().tscl_lstm_seq_bwd_tc_heads(
             self._h, _p(Wt), _p(P), _p(self.st_g[ci]), _p(self.st_c[ci]), _p(self.st_h[ci]), _p(self.c_bw), _p(dpre),
-            _p(self.act_hist[0, r0:]), _p(self.Rs[0, r0:]), _p(self.Adv[0, r0:]), C.c_int32(self.T),
-            C.c_int64(self.chunk), C.c_int32(n_chunks), C.c_int64(R), C.c_int64(r0), C.c_int64(R * A), C.c_float(v_coef),
-            C.c_float(beta), C.c_float(scale), _p(dZb), _p(stats), _p(G), self._st()))
+            _p(self.act_hist[0, r0:]), _p(self.Rs[0, r0:]), _p(self.Adv[0, r0:]), self.T, self.chunk, n_chunks, R, r0,
+            R * A, v_coef, beta, scale, _p(dZb), _p(stats), _p(G), self._st()))
 
     def backward(self, boot: Optional[torch.Tensor], lr: float, beta: float):
         """One A2C update from the stored n_step rollout (agents/models.py:174-183).  `boot` is the
@@ -566,11 +557,10 @@ class BatchedA2C:
             self.boot.copy_(boot)
         if self.gamma_dev is not None:
             _lib.check(lib.tscl_returns_g(self._h, _p(self.rew_hist), _p(self.val_hist), _p(self.boot), _p(dpost),
-                                          _p(self.gamma_dev), C.c_int32(self.K), C.c_int32(T), C.c_int64(R), _p(self.Rs),
-                                          _p(self.Adv), st()))
+                                          _p(self.gamma_dev), self.K, T, R, _p(self.Rs), _p(self.Adv), st()))
         else:
             _lib.check(lib.tscl_returns(self._h, _p(self.rew_hist), _p(self.val_hist), _p(self.boot), _p(dpost),
-                                        C.c_float(self.gamma), C.c_int32(T), C.c_int64(R), _p(self.Rs), _p(self.Adv), st()))
+                                        self.gamma, T, R, _p(self.Rs), _p(self.Adv), st()))
         self.G.zero_()
         self.stats.zero_()
         scale = _dist.grad_scale(T, 1, self.total_replicas)       # local SUM x 1/(n_step * R_total); ranks add up
@@ -622,16 +612,13 @@ class BatchedA2C:
                 direct = self.bwd_tc        # the tensor-core BPTT kernel reads gates / c from the store itself
                 _lib.check(lib.tscl_unpack_store(self._h, _p(self.st_x[ci]), _p(self.st_g[ci]), _p(self.st_c[ci]),
                                                  _p(self.st_h[ci]), _p(X), None if direct else _p(ZG),
-                                                 None if direct else _p(Cc), _p(H), _p(Hp), _p(self.h_bw),
-                                                 _p(dpre), C.c_int32(T), C.c_int64(rc), C.c_int64(R), C.c_int64(r0),
-                                                 st()))
+                                                 None if direct else _p(Cc), _p(H), _p(Hp), _p(self.h_bw), _p(dpre), T,
+                                                 rc, R, r0, st()))
             else:
-                _lib.check(lib.tscl_fc_embed(self._h, _p(P), _p(obs0), C.c_int64(M), C.c_int64(rc),
-                                             C.c_int64(R * n_obs), _p(X), st()))
+                _lib.check(lib.tscl_fc_embed(self._h, _p(P), _p(obs0), M, rc, R * n_obs, _p(X), st()))
                 torch.baddbmm(self.pv["bl"].unsqueeze(1), X, self.pv["wx"], out=ZG)
                 _lib.check(lib.tscl_lstm_seq_fwd(self._h, _p(P), _p(ZG), _p(Cc), _p(H), _p(Hp), _p(self.c_bw),
-                                                 _p(self.h_bw), None, None, _p(dpre), C.c_int32(T), C.c_int64(rc),
-                                                 C.c_int64(R), C.c_int64(r0), st()))
+                                                 _p(self.h_bw), None, None, _p(dpre), T, rc, R, r0, st()))
             hb = _p(self.st_h[ci]) if use_store else None
             if heads_bptt:      # heads + BPTT in one kernel (already run for every chunk when dz_all is set)
                 if dz_all is None:
@@ -639,9 +626,8 @@ class BatchedA2C:
                     self.kernel_launches += 1
             else:
                 _lib.check(lib.tscl_heads_loss(self._h, _p(P), None if all_tc else _p(H), _p(self.act_hist[0, r0:]),
-                                               _p(self.Rs[0, r0:]), _p(self.Adv[0, r0:]), C.c_int64(M), C.c_int64(rc),
-                                               C.c_int64(R * A), C.c_float(self.hp[k]["v_coef"]), C.c_float(betas[k]),
-                                               C.c_float(scale),
+                                               _p(self.Rs[0, r0:]), _p(self.Adv[0, r0:]), M, rc, R * A,
+                                               self.hp[k]["v_coef"], betas[k], scale,
                                                None if self.fused_heads else _p(dlog), _p(dH), _p(stats),
                                                hb if all_tc else None, _p(G) if self.fused_heads else None, st()))
                 self.kernel_launches += 2
@@ -653,22 +639,21 @@ class BatchedA2C:
                 pass
             elif self.bwd_tc:
                 gb = (_p(self.st_g[ci]), _p(self.st_c[ci])) if use_store else (None, None)
-                _lib.check(lib.tscl_lstm_seq_bwd_tc_dx(self._h, _p(Wt), _p(ZG), _p(Cc), _p(dH), _p(self.c_bw),
-                                                       _p(dpre), C.c_int32(T), C.c_int64(rc), C.c_int64(R), C.c_int64(r0),
-                                                       *gb, _p(dZb), _p(Wxt) if fuse_dx else None,
+                _lib.check(lib.tscl_lstm_seq_bwd_tc_dx(self._h, _p(Wt), _p(ZG), _p(Cc), _p(dH), _p(self.c_bw), _p(dpre),
+                                                       T, rc, R, r0, *gb, _p(dZb), _p(Wxt) if fuse_dx else None,
                                                        _p(dXb) if fuse_dx else None, st()))
             else:
-                _lib.check(lib.tscl_lstm_seq_bwd(self._h, _p(P), _p(ZG), _p(Cc), _p(dH), _p(self.c_bw), _p(dpre),
-                                                 C.c_int32(T), C.c_int64(rc), C.c_int64(R), C.c_int64(r0), st()))
+                _lib.check(lib.tscl_lstm_seq_bwd(self._h, _p(P), _p(ZG), _p(Cc), _p(dH), _p(self.c_bw), _p(dpre), T, rc,
+                                                 R, r0, st()))
             dZ = ZG
             if self.wgrad_tc:
                 if use_store:
-                    _lib.check(lib.tscl_wgrad_tc(self._h, _p(dZ), _p(dZb), None, _p(self.st_x[ci]), None, _p(self.st_h[ci]),
-                                                 _p(self.h_bw), _p(dpre), C.c_int32(T), C.c_int64(rc), C.c_int64(R),
-                                                 C.c_int64(r0), _p(G), C.c_int32(0), st()))
+                    _lib.check(lib.tscl_wgrad_tc(self._h, _p(dZ), _p(dZb), None, _p(self.st_x[ci]), None,
+                                                 _p(self.st_h[ci]), _p(self.h_bw), _p(dpre), T, rc, R, r0, _p(G), 0,
+                                                 st()))
                 else:
-                    _lib.check(lib.tscl_wgrad_tc(self._h, _p(dZ), None, _p(X), None, _p(Hp), None, None, None, C.c_int32(T),
-                                                 C.c_int64(rc), C.c_int64(R), C.c_int64(r0), _p(G), C.c_int32(0), st()))
+                    _lib.check(lib.tscl_wgrad_tc(self._h, _p(dZ), None, _p(X), None, _p(Hp), None, None, None, T, rc, R,
+                                                 r0, _p(G), 0, st()))
             else:
                 self.gv["wx"].baddbmm_(X.transpose(1, 2), dZ)
                 self.gv["wh"].baddbmm_(Hp.transpose(1, 2), dZ)
@@ -677,10 +662,10 @@ class BatchedA2C:
             # warp-specialised wgmma kernel (tscl_dx_tc); a library GEMM only on the fp32 twin path, for dx > 224 and
             # under TSC_DX_LIBRARY=1 (A/B measurements)
             if fuse_fc:
-                _lib.check(lib.tscl_dx_fc_bwd_tc(self._h, _p(obs0), _p(self.st_x[ci]), _p(dZb), _p(Wxt), C.c_int64(M),
-                                                 C.c_int64(rc), C.c_int64(R * n_obs), _p(G), st()))
+                _lib.check(lib.tscl_dx_fc_bwd_tc(self._h, _p(obs0), _p(self.st_x[ci]), _p(dZb), _p(Wxt), M, rc,
+                                                 R * n_obs, _p(G), st()))
             elif all_tc and not fuse_dx and self.dx_own:
-                _lib.check(lib.tscl_dx_tc(self._h, _p(dZb), _p(Wxt), _p(dXb), C.c_int64(M), st()))
+                _lib.check(lib.tscl_dx_tc(self._h, _p(dZb), _p(Wxt), _p(dXb), M, st()))
             elif all_tc and not fuse_dx:
                 torch.bmm(dZb, self.wx_b.transpose(1, 2), out=dXb)
             elif not all_tc:        # Wx of this chunk's member (self.pv is the K = 1 view only)
@@ -689,12 +674,10 @@ class BatchedA2C:
                 pass            # the fc weight gradients came out of tscl_dx_fc_bwd_tc above
             elif self.fc_bwd_tc:
                 xb = _p(self.st_x[ci]) if use_store else None
-                _lib.check(lib.tscl_fc_bwd_tc(self._h, _p(obs0), None if all_tc else _p(X), xb, _p(dX), _p(dXb),
-                                              C.c_int64(M), C.c_int64(rc), C.c_int64(R * n_obs), _p(G), C.c_int32(0),
-                                              st()))
+                _lib.check(lib.tscl_fc_bwd_tc(self._h, _p(obs0), None if all_tc else _p(X), xb, _p(dX), _p(dXb), M, rc,
+                                              R * n_obs, _p(G), 0, st()))
             else:
-                _lib.check(lib.tscl_fc_bwd(self._h, _p(obs0), _p(X), _p(dX), C.c_int64(M), C.c_int64(rc),
-                                           C.c_int64(R * n_obs), _p(G), st()))
+                _lib.check(lib.tscl_fc_bwd(self._h, _p(obs0), _p(X), _p(dX), M, rc, R * n_obs, _p(G), st()))
             self.kernel_launches += 1 if fuse_fc else 2 if use_store else 3     # heads / BPTT counted above
         if self.pg is not None:
             _dist.allreduce_sum_(self.G, self.pg)
@@ -702,8 +685,8 @@ class BatchedA2C:
             m = (lambda t_: t_) if self.K == 1 else (lambda t_: t_[k])
             hk = self.hp[k]
             _lib.check(lib.tscl_clip_rmsprop(self._h, _p(m(self.P)), _p(m(self.G)), _p(m(self.MS)), _p(self.agent_of),
-                                             C.c_float(hk["max_grad_norm"]), C.c_float(lrs[k]), C.c_float(hk["alpha"]),
-                                             C.c_float(hk["eps"]), _p(m(self.norms)), st()))
+                                             hk["max_grad_norm"], lrs[k], hk["alpha"], hk["eps"], _p(m(self.norms)),
+                                             st()))
             self.kernel_launches += 3
         self.pack_weights()
         # states_bw <- states_fw (agents/policies.py:153); next rollout starts at slot 0

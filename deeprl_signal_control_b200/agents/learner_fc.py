@@ -11,7 +11,6 @@ register-tiled fp32 kernels tscl_fc_hidden_fwd / tscl_fc_hidden_bwd (no library 
 """
 from __future__ import annotations
 
-import ctypes as C
 from typing import Optional
 
 import torch
@@ -36,12 +35,11 @@ class BatchedFcA2C(BatchedA2C):
         commit = "p" in out_type
         want_act = sample and commit
         self._mm()
-        _lib.check(lib.tscl_fc_embed(self._h, _p(self.P), _p(obs), C.c_int64(R), C.c_int64(R), C.c_int64(0),
-                                     _p(self.X1), self._st()))
-        _lib.check(lib.tscl_fc_hidden_fwd(self._h, _p(self.P), _p(self.X1), C.c_int64(R), _p(self.H1), self._st()))
-        _lib.check(lib.tscl_heads(self._h, _p(self.P), _p(self.H1), C.c_int64(R), _p(self.pi), _p(self.val),
-                                  _p(self.act) if want_act else None, C.c_uint64(self.seed),
-                                  C.c_int64(self.n_forward), C.c_int64(self.replica0), self._st()))
+        _lib.check(lib.tscl_fc_embed(self._h, _p(self.P), _p(obs), R, R, 0, _p(self.X1), self._st()))
+        _lib.check(lib.tscl_fc_hidden_fwd(self._h, _p(self.P), _p(self.X1), R, _p(self.H1), self._st()))
+        _lib.check(lib.tscl_heads(self._h, _p(self.P), _p(self.H1), R, _p(self.pi), _p(self.val),
+                                  _p(self.act) if want_act else None, self.seed, self.n_forward, self.replica0,
+                                  self._st()))
         self.kernel_launches += 3
         if commit:
             self.n_forward += 1
@@ -59,8 +57,8 @@ class BatchedFcA2C(BatchedA2C):
             self.boot.zero_()
         else:
             self.boot.copy_(boot)
-        _lib.check(lib.tscl_returns(self._h, _p(self.rew_hist), _p(self.val_hist), _p(self.boot), _p(dpost),
-                                    C.c_float(self.gamma), C.c_int32(T), C.c_int64(R), _p(self.Rs), _p(self.Adv), st()))
+        _lib.check(lib.tscl_returns(self._h, _p(self.rew_hist), _p(self.val_hist), _p(self.boot), _p(dpost), self.gamma,
+                                    T, R, _p(self.Rs), _p(self.Adv), st()))
         self.G.zero_()
         self.stats.zero_()
         scale = _dist.grad_scale(T, 1, self.total_replicas)
@@ -72,29 +70,24 @@ class BatchedFcA2C(BatchedA2C):
             H = torch.empty(U, M, L.h, **f32)
             dH = torch.empty(U, M, L.h, **f32)
             obs0 = self.obs_hist[0, r0:]
-            _lib.check(lib.tscl_fc_embed(self._h, _p(self.P), _p(obs0), C.c_int64(M), C.c_int64(rc),
-                                         C.c_int64(R * n_obs), _p(X), st()))
-            _lib.check(lib.tscl_fc_hidden_fwd(self._h, _p(self.P), _p(X), C.c_int64(M), _p(H), st()))
+            _lib.check(lib.tscl_fc_embed(self._h, _p(self.P), _p(obs0), M, rc, R * n_obs, _p(X), st()))
+            _lib.check(lib.tscl_fc_hidden_fwd(self._h, _p(self.P), _p(X), M, _p(H), st()))
             _lib.check(lib.tscl_heads_loss(self._h, _p(self.P), _p(H), _p(self.act_hist[0, r0:]), _p(self.Rs[0, r0:]),
-                                           _p(self.Adv[0, r0:]), C.c_int64(M), C.c_int64(rc), C.c_int64(R * A),
-                                           C.c_float(self.v_coef), C.c_float(beta), C.c_float(scale), None, _p(dH),
+                                           _p(self.Adv[0, r0:]), M, rc, R * A, self.v_coef, beta, scale, None, _p(dH),
                                            _p(self.stats), None, _p(self.G), st()))
             dX = torch.empty(U, M, L.dx, **f32)
             # relu', dX = dH . W^T, dW += X^T dH, db += 1^T dH: own kernels (no library GEMM on this path)
-            _lib.check(lib.tscl_fc_hidden_bwd(self._h, _p(self.P), _p(X), _p(H), _p(dH), C.c_int64(M), _p(dX), _p(self.G),
-                                              st()))
+            _lib.check(lib.tscl_fc_hidden_bwd(self._h, _p(self.P), _p(X), _p(H), _p(dH), M, _p(dX), _p(self.G), st()))
             if self.fc_bwd_tc:
-                _lib.check(lib.tscl_fc_bwd_tc(self._h, _p(obs0), _p(X), None, _p(dX), None, C.c_int64(M), C.c_int64(rc),
-                                              C.c_int64(R * n_obs), _p(self.G), C.c_int32(0), st()))
+                _lib.check(lib.tscl_fc_bwd_tc(self._h, _p(obs0), _p(X), None, _p(dX), None, M, rc, R * n_obs,
+                                              _p(self.G), 0, st()))
             else:
-                _lib.check(lib.tscl_fc_bwd(self._h, _p(obs0), _p(X), _p(dX), C.c_int64(M), C.c_int64(rc),
-                                           C.c_int64(R * n_obs), _p(self.G), st()))
+                _lib.check(lib.tscl_fc_bwd(self._h, _p(obs0), _p(X), _p(dX), M, rc, R * n_obs, _p(self.G), st()))
             self.kernel_launches += 6
         if self.pg is not None:
             _dist.allreduce_sum_(self.G, self.pg)
         _lib.check(lib.tscl_clip_rmsprop(self._h, _p(self.P), _p(self.G), _p(self.MS), _p(self.agent_of),
-                                         C.c_float(self.max_grad_norm), C.c_float(lr), C.c_float(self.alpha),
-                                         C.c_float(self.eps), _p(self.norms), st()))
+                                         self.max_grad_norm, lr, self.alpha, self.eps, _p(self.norms), st()))
         self.kernel_launches += 3
         self.obs_hist[0].copy_(self.obs_hist[T])
         self.last_done = bool(self.done_post[-1])

@@ -28,8 +28,7 @@ from .models import IQL
 N_ROUNDS = 10                     # minibatches per agent per backward (agents/models.py:337-345)
 
 
-def _p(t):
-    return None if t is None else C.c_void_p(t.data_ptr())
+_p = _lib.ptr
 
 
 def ring_bytes(n_replicas: int, buffer_size: int, n_obs: int, n_agents: int) -> int:
@@ -65,7 +64,7 @@ class BatchedIQL:
             raise MemoryError("BatchedIQL: the replay rings need %.2f GB (R=%d x buffer_size=%d x (8 n_obs + 5 A + 1) "
                               "bytes) but the device has %.2f GB free" % (need / 1e9, self.R, self.B, free / 1e9))
         self._h = C.c_void_p()
-        _lib.check(_lib.lib().tscl_q_create(C.byref(layout.as_c()), C.c_int32(self.dev.index or 0), C.byref(self._h)))
+        _lib.check(_lib.lib().tscl_q_create(C.byref(layout.as_c()), self.dev.index or 0, C.byref(self._h)))
         fwd_smem, td_smem = C.c_int64(), C.c_int64()
         _lib.check(_lib.lib().tscl_q_info(self._h, C.byref(fwd_smem), C.byref(td_smem)))
         if td_smem.value == 0:
@@ -118,7 +117,7 @@ class BatchedIQL:
             self._h = None
 
     def _st(self):
-        return C.c_void_p(torch.cuda.current_stream(self.dev).cuda_stream)
+        return _lib.stream(self.dev)
 
     @property
     def size(self):
@@ -135,23 +134,23 @@ class BatchedIQL:
         ring slot's s / a.  `step` is the global control step that keys the exploration draws."""
         k = self.slot
         _lib.check(_lib.lib().tscl_q_explore(
-            self._h, _p(self.P), _p(obs), C.c_int64(self.R), _p(self.q), _p(self.act), C.c_float(eps),
-            C.c_uint64(self.seed), C.c_int64(step), C.c_int64(self.replica0), _p(self.s[k]), _p(self.a[k]), self._st()))
+            self._h, _p(self.P), _p(obs), self.R, _p(self.q), _p(self.act), eps, self.seed, step, self.replica0,
+            _p(self.s[k]), _p(self.a[k]), self._st()))
         return self.act
 
     def add_transition(self, reward, greward, rew_acc, done: bool):
         """IQL.add_transition: the slot's r (normalised, clipped) and post-step done; s1 was written by the simulator."""
         k = self.slot
         _lib.check(_lib.lib().tscl_q_transition(
-            self._h, _p(reward), C.c_int64(self.R), C.c_float(self.reward_norm or 0.0), C.c_float(self.reward_clip or 0.0),
-            _p(self.r[k]), _p(greward), _p(rew_acc), _p(self.done[k]), C.c_int32(int(done)), self._st()))
+            self._h, _p(reward), self.R, self.reward_norm or 0.0, self.reward_clip or 0.0, _p(self.r[k]), _p(greward),
+            _p(rew_acc), _p(self.done[k]), int(done), self._st()))
         self.cum_size += 1
 
     # ---- update -----------------------------------------------------------------------------------
     def sample(self, rnd: int):
         _lib.check(_lib.lib().tscl_q_sample(
-            self._h, C.c_int64(self.R), C.c_int32(self.batch_size), C.c_int32(self.size), C.c_uint64(self.seed),
-            C.c_int64(self.n_updates), C.c_int32(rnd), C.c_int64(self.replica0), _p(self.idx), self._st()))
+            self._h, self.R, self.batch_size, self.size, self.seed, self.n_updates, rnd, self.replica0, _p(self.idx),
+            self._st()))
         return self.idx
 
     def td_round(self, rnd: int, lr: float, idx=None, rec=None):
@@ -163,15 +162,13 @@ class BatchedIQL:
             idx = self.sample(rnd)
         inv_n = 1.0 / (self.batch_size * self.total_replicas)
         _lib.check(lib.tscl_q_td(self._h, _p(self.P), _p(self.s), _p(self.s1), _p(self.a), _p(self.r), _p(self.done),
-                                 _p(idx), C.c_int64(self.R), C.c_int32(self.batch_size), C.c_float(self.gamma),
-                                 C.c_float(inv_n), _p(self.grad), self._st()))
+                                 _p(idx), self.R, self.batch_size, self.gamma, inv_n, _p(self.grad), self._st()))
         if self.pg is not None:
             _dist.allreduce_sum_(self.grad, group=self.pg)
         self.t += 1
         lr_t = lr * np.sqrt(1.0 - 0.999 ** self.t) / (1.0 - 0.9 ** self.t)
-        _lib.check(lib.tscl_q_adam(self._h, _p(self.P), _p(self.grad), _p(self.M), _p(self.V), C.c_float(lr_t),
-                                   C.c_float(self.max_grad_norm), _p(self.losses[rnd]), _p(self.norms[rnd]), _p(rec),
-                                   self._st()))
+        _lib.check(lib.tscl_q_adam(self._h, _p(self.P), _p(self.grad), _p(self.M), _p(self.V), lr_t, self.max_grad_norm,
+                                   _p(self.losses[rnd]), _p(self.norms[rnd]), _p(rec), self._st()))
 
     def backward(self, lr: float, rec=None) -> bool:
         """IQL.backward after lr = lr_scheduler.get(n_step) (taken by the caller even when this returns False).

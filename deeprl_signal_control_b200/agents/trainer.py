@@ -8,7 +8,6 @@ learner's rollout slot and reads actions / fingerprints from the learner's buffe
 """
 from __future__ import annotations
 
-import ctypes as C
 from typing import Optional
 
 import numpy as np
@@ -229,12 +228,12 @@ class BatchedTrainer:
             pp = dict(primed=False, act=pin(R, A, dtype=torch.int32), pi=pin(R, A, L.max_na), obs=pin(R, sim.net.n_obs),
                       rew=pin(R, A), grew=pin(R), done=pin(R, dtype=torch.uint8),
                       rew_stage=torch.zeros(R, A, device=m.dev), grew_stage=torch.zeros(R, device=m.dev), parts=[])
-            at = lambda x, r0, per_row: C.c_void_p(x.data_ptr() + r0 * per_row * x.element_size())
+            at = lambda x, r0, per_row: x.data_ptr() + r0 * per_row * x.element_size()
             for k in range(n_parts):        # raw pointers of every range's slices: the per-step loop is host-issue-bound
                 r0, n = bounds[k], bounds[k + 1] - bounds[k]
                 st = torch.cuda.Stream(device=sim.device)
                 pp['parts'].append(dict(
-                    r0=r0, n=n, stream=st, sth=C.c_void_p(st.cuda_stream), ev=torch.cuda.Event(),
+                    r0=r0, n=n, stream=st, sth=st.cuda_stream, ev=torch.cuda.Event(),
                     act_h=at(pp['act'], r0, A), pi_h=at(pp['pi'], r0, A * L.max_na) if ma2c else None,
                     obs_h=at(pp['obs'], r0, sim.net.n_obs), rew_h=at(pp['rew'], r0, A), grew_h=at(pp['grew'], r0, 1),
                     done_h=at(pp['done'], r0, 1), rew_stage=at(pp['rew_stage'], r0, A),
@@ -244,11 +243,10 @@ class BatchedTrainer:
 
         def issue_forward(p, t, nf, done):
             pi, val, act = m.forward_range(p['r0'], p['n'], done, t, nf, stream=p['sth'], to_hist=True)
-            _lib.check(lib.tscl_memcpy_async(m._h, p['act_h'], C.c_void_p(act.data_ptr()), C.c_int64(p['n'] * A * 4),
-                                             C.c_int32(2), p['sth']))
+            _lib.check(lib.tscl_memcpy_async(m._h, p['act_h'], act.data_ptr(), p['n'] * A * 4, 2, p['sth']))
             if ma2c:
-                _lib.check(lib.tscl_memcpy_async(m._h, p['pi_h'], C.c_void_p(pi.data_ptr()),
-                                                 C.c_int64(p['n'] * A * L.max_na * 4), C.c_int32(2), p['sth']))
+                _lib.check(lib.tscl_memcpy_async(m._h, p['pi_h'], pi.data_ptr(), p['n'] * A * L.max_na * 4, 2,
+                                                 p['sth']))
             p['ev'].record(p['stream'])
 
         if not pp['primed']:
@@ -265,18 +263,17 @@ class BatchedTrainer:
         n_obs = sim.net.n_obs
         for p in pp['parts']:                           # every range's env step is enqueued as soon as its actions are here
             p['ev'].synchronize()                       # the host holds this range's actions / fingerprints
-            _lib.check(lib.tsc_step_host_range_async(sim._h, C.c_int32(p['r0']), C.c_int32(p['n']), p['act_h'], p['pi_h'],
-                                                     p['obs_h'], p['rew_h'], p['grew_h'], p['done_h'], p['sth']))
+            _lib.check(lib.tsc_step_host_range_async(sim._h, p['r0'], p['n'], p['act_h'], p['pi_h'], p['obs_h'],
+                                                     p['rew_h'], p['grew_h'], p['done_h'], p['sth']))
         obs_next, rew_t = m.obs_hist[t + 1], m.rew_hist[t]
         for p in pp['parts']:
             r0, n = p['r0'], p['n']
             p['stream'].synchronize()                   # the host holds this range's observations / rewards ...
             # ... and hands them to the learner: obs -> rollout slot t+1, reward -> normalised / clipped slot t, episode sum
             _lib.check(lib.tscl_host_transition(
-                m._h, p['obs_h'], C.c_void_p(obs_next.data_ptr() + r0 * n_obs * 4), C.c_int64(n * n_obs), p['rew_h'],
-                p['rew_stage'], C.c_void_p(rew_t.data_ptr() + r0 * A * 4), C.c_int64(n * A),
-                C.c_float(m.reward_norm or 0.0), C.c_float(m.reward_clip or 0.0), p['grew_h'], p['grew_stage'],
-                p['rew_acc'], C.c_int64(n), p['sth']))
+                m._h, p['obs_h'], obs_next.data_ptr() + r0 * n_obs * 4, n * n_obs, p['rew_h'], p['rew_stage'],
+                rew_t.data_ptr() + r0 * A * 4, n * A, m.reward_norm or 0.0, m.reward_clip or 0.0, p['grew_h'],
+                p['grew_stage'], p['rew_acc'], n, p['sth']))
             if not boundary:
                 issue_forward(p, t + 1, m.n_forward, False)
         m.end_transition_ranges(self.done, new_done)

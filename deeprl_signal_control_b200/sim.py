@@ -14,15 +14,8 @@ import numpy as np
 import torch
 
 from . import _lib
+from ._lib import ptr
 from .net.tables import EnvParams, NetTables
-
-
-def _ptr(t: Optional[torch.Tensor]):
-    return None if t is None else C.c_void_p(t.data_ptr())
-
-
-def _np(a, ct):
-    return None if a is None else a.ctypes.data_as(C.POINTER(ct))
 
 
 class BatchedSim:
@@ -33,8 +26,7 @@ class BatchedSim:
         self.device = torch.device("cuda", device)
         self._cnet, self._ccfg = net.as_c(), params.as_c()
         h = C.c_void_p()
-        _lib.check(_lib.lib().tsc_create(C.byref(self._cnet), C.byref(self._ccfg), C.c_int32(self.R),
-                                         C.c_int32(device), C.byref(h)))
+        _lib.check(_lib.lib().tsc_create(C.byref(self._cnet), C.byref(self._ccfg), self.R, device, C.byref(h)))
         self._h = h
         N = net.n_nodes
         with torch.cuda.device(self.device):
@@ -55,16 +47,16 @@ class BatchedSim:
             pass
 
     def _stream(self):
-        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+        return _lib.stream(self.device)
 
     # ---- control -------------------------------------------------------------------------
     def reset(self, seeds) -> None:
         seeds = np.ascontiguousarray(seeds, dtype=np.uint64)
         assert seeds.shape == (self.R,)
-        _lib.check(_lib.lib().tsc_reset(self._h, _np(seeds, C.c_uint64), self._stream()))
+        _lib.check(_lib.lib().tsc_reset(self._h, seeds.ctypes.data, self._stream()))
 
     def set_train_mode(self, train: bool) -> None:
-        _lib.check(_lib.lib().tsc_set_train_mode(self._h, C.c_int32(int(train))))
+        _lib.check(_lib.lib().tsc_set_train_mode(self._h, int(train)))
 
     def set_replica_coop_gamma(self, values=None) -> None:
         """MA2C spatial discount per replica (`tsc_set_replica_coop_gamma`): `values` [R] floats, replica r then steps as
@@ -80,11 +72,11 @@ class BatchedSim:
         if not (np.asarray(self.net.obs_scale) != 1.0).any() and (cg != 1.0).any() and self.params.agent == "ma2c":
             raise ValueError("the network was built with coop_gamma = 1, so no observation entry is scaled; build it "
                              "with a coop_gamma other than 1")
-        _lib.check(_lib.lib().tsc_set_replica_coop_gamma(self._h, _np(cg, C.c_float)))
+        _lib.check(_lib.lib().tsc_set_replica_coop_gamma(self._h, cg.ctypes.data))
 
     def observe(self, fp: Optional[torch.Tensor] = None, obs_out: Optional[torch.Tensor] = None) -> torch.Tensor:
         obs = self.obs if obs_out is None else obs_out
-        _lib.check(_lib.lib().tsc_observe(self._h, _ptr(fp), _ptr(obs), self._stream()))
+        _lib.check(_lib.lib().tsc_observe(self._h, ptr(fp), ptr(obs), self._stream()))
         return obs
 
     def step(self, action: torch.Tensor, fp: Optional[torch.Tensor] = None,
@@ -100,8 +92,8 @@ class BatchedSim:
             assert fp.numel() == self.R * self.net.n_nodes * self.net.max_na
         obs = self.obs if obs_out is None else obs_out
         assert obs.is_contiguous() and obs.numel() == self.R * self.net.n_obs
-        _lib.check(_lib.lib().tsc_step(self._h, _ptr(action), _ptr(fp), _ptr(obs), _ptr(self.reward),
-                                       _ptr(self.greward), _ptr(self.done), self._stream()))
+        _lib.check(_lib.lib().tsc_step(self._h, ptr(action), ptr(fp), ptr(obs), ptr(self.reward), ptr(self.greward),
+                                       ptr(self.done), self._stream()))
         return obs, self.reward, self.greward, self.done
 
     def step_host(self, action: np.ndarray, fp: Optional[np.ndarray] = None):
@@ -116,9 +108,9 @@ class BatchedSim:
                              torch.zeros(self.R, dtype=torch.uint8).pin_memory())
             self._h_out = tuple(t.numpy() for t in self._h_out_t)
         obs, reward, greward, done = self._h_out
-        _lib.check(_lib.lib().tsc_step_host(self._h, _np(action, C.c_int32), _np(fp, C.c_float),
-                                            _np(obs, C.c_float), _np(reward, C.c_float),
-                                            _np(greward, C.c_float), _np(done, C.c_uint8), self._stream()))
+        _lib.check(_lib.lib().tsc_step_host(self._h, action.ctypes.data, None if fp is None else fp.ctypes.data,
+                                            obs.ctypes.data, reward.ctypes.data, greward.ctypes.data, done.ctypes.data,
+                                            self._stream()))
         return obs, reward, greward, done
 
     def step_host_range(self, r0: int, n: int, action: np.ndarray, fp: Optional[np.ndarray], obs: np.ndarray,
@@ -127,14 +119,13 @@ class BatchedSim:
         the slices of that range (page-locked for full PCIe speed).  Blocks until the slice's results are on the host;
         with sync=False (`tsc_step_host_range_async`) the work is only enqueued and the caller synchronises the stream."""
         fn = _lib.lib().tsc_step_host_range if sync else _lib.lib().tsc_step_host_range_async
-        _lib.check(fn(self._h, C.c_int32(r0), C.c_int32(n), _np(action, C.c_int32),
-                      _np(fp, C.c_float), _np(obs, C.c_float), _np(reward, C.c_float),
-                      _np(greward, C.c_float), _np(done, C.c_uint8), self._stream()))
+        _lib.check(fn(self._h, r0, n, action.ctypes.data, None if fp is None else fp.ctypes.data, obs.ctypes.data,
+                      reward.ctypes.data, greward.ctypes.data, done.ctypes.data, self._stream()))
 
     # ---- evaluation / recording path (envs/env.py:409-437, 498-542) ------------------------
     def set_record(self, on: bool = True) -> None:
         """Record mode: per-vehicle trip words + arrival log (call right after reset())."""
-        _lib.check(_lib.lib().tsc_set_record(self._h, C.c_int32(1 if on else 0)))
+        _lib.check(_lib.lib().tsc_set_record(self._h, 1 if on else 0))
         self.record = bool(on)
 
     def step_record(self, action: torch.Tensor, fp: Optional[torch.Tensor] = None):
@@ -147,16 +138,15 @@ class BatchedSim:
         greward = torch.empty(self.R, dtype=torch.float32, device=self.device)
         done = torch.empty(self.R, dtype=torch.uint8, device=self.device)
         stats = torch.zeros(self.R, self.params.control_interval_sec, 8, dtype=torch.float32, device=self.device)
-        _lib.check(_lib.lib().tsc_step_record(self._h, _ptr(action), _ptr(fp), _ptr(obs), _ptr(reward), _ptr(greward),
-                                              _ptr(done), _ptr(stats), self._stream()))
+        _lib.check(_lib.lib().tsc_step_record(self._h, ptr(action), ptr(fp), ptr(obs), ptr(reward), ptr(greward),
+                                              ptr(done), ptr(stats), self._stream()))
         return obs, reward, greward, done, stats
 
     def trips(self, replica: int = 0) -> np.ndarray:
         """tripinfo rows of one replica: int array [n, 5] = depart_sec, arrival_sec, route, wait_sec, wait_count."""
         rows = np.zeros((8192, 2), np.uint32)
         nr = C.c_int32(0)
-        _lib.check(_lib.lib().tsc_get_trips(self._h, C.c_int32(replica), _np(rows, C.c_uint32), C.c_int32(len(rows)),
-                                            C.byref(nr)))
+        _lib.check(_lib.lib().tsc_get_trips(self._h, replica, rows.ctypes.data, len(rows), C.byref(nr)))
         w0, w1 = rows[:nr.value, 0].astype(np.int64), rows[:nr.value, 1].astype(np.int64)
         return np.stack([w0 & 4095, (w0 >> 12) & 4095, w0 >> 24, w1 & 65535, w1 >> 16], axis=1)
 
@@ -166,8 +156,7 @@ class BatchedSim:
         veh = torch.zeros(self.R, n.n_det, dtype=torch.int32, device=self.device)
         halt, wait = torch.zeros_like(veh), torch.zeros_like(veh)
         phase = torch.zeros(self.R, n.n_nodes, dtype=torch.int32, device=self.device)
-        _lib.check(_lib.lib().tsc_get_counts(self._h, _ptr(veh), _ptr(halt), _ptr(wait), _ptr(phase),
-                                             self._stream()))
+        _lib.check(_lib.lib().tsc_get_counts(self._h, ptr(veh), ptr(halt), ptr(wait), ptr(phase), self._stream()))
         return veh, halt, wait, phase
 
     def dump_state(self, replica: int = 0):
@@ -175,15 +164,14 @@ class BatchedSim:
         cnt = np.zeros(n.n_lanes, np.int32)
         veh = np.zeros((n.n_slots, 3), np.uint32)
         nv = C.c_int32(0)
-        _lib.check(_lib.lib().tsc_dump_state(self._h, C.c_int32(replica), _np(cnt, C.c_int32),
-                                             _np(veh, C.c_uint32), C.byref(nv)))
+        _lib.check(_lib.lib().tsc_dump_state(self._h, replica, cnt.ctypes.data, veh.ctypes.data, C.byref(nv)))
         return cnt, veh[:nv.value].copy()
 
     def traffic_stats(self) -> torch.Tensor:
         """[R, 8] = n_live, departed, arrived, avg_wait, avg_speed, avg_queue, std_queue, backlog
         (the fields of reference _measure_traffic_step, envs/env.py:409-437)."""
         out = torch.zeros(self.R, 8, dtype=torch.float32, device=self.device)
-        _lib.check(_lib.lib().tsc_get_traffic_stats(self._h, _ptr(out), self._stream()))
+        _lib.check(_lib.lib().tsc_get_traffic_stats(self._h, ptr(out), self._stream()))
         return out
 
     def mean_live(self) -> float:

@@ -1,6 +1,5 @@
 """Per-phase clock64 breakdown of the store-path BPTT kernel (lstm_bwd_tc_regs_kernel: thread 0 of every warpgroup) during
 one update: python scripts/profile_bptt_phases.py [R] [chunk]"""
-import ctypes as C
 import sys
 
 import torch
@@ -25,7 +24,7 @@ tr.run(120)                       # one rollout + one update (warm-up)
 tr.run(119)
 torch.cuda.synchronize()
 prof = torch.zeros(8, dtype=torch.int64, device="cuda")
-_lib.lib().tscl_debug_bptt_prof(C.c_void_p(prof.data_ptr()))
+_lib.lib().tscl_debug_bptt_prof(prof.data_ptr())
 tr.run(1)                         # the 120th step triggers the update
 torch.cuda.synchronize()
 _lib.lib().tscl_debug_bptt_prof(None)

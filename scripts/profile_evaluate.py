@@ -110,15 +110,13 @@ def time_kernels(scenario, R, launches, warmup):
     lib = _lib.lib()
 
     def full():
-        _lib.check(lib.tscl_policy_step_v2(m._h, _p(m.P), _p(m.Wp), _p(obs), C.c_int64(R), _p(m.c_fw), _p(m.h_fw),
-                                           _p(m.c_fw), _p(m.h_fw), _p(m.pi), _p(m.val), _p(m.act), C.c_int32(0),
-                                           C.c_uint64(1), C.c_int64(0), C.c_int64(0), None, None, None, None, None,
-                                           C.c_int32(0), C.c_int32(1), C.c_int64(R), m._st()))
+        _lib.check(lib.tscl_policy_step_v2(m._h, _p(m.P), _p(m.Wp), _p(obs), R, _p(m.c_fw), _p(m.h_fw), _p(m.c_fw),
+                                           _p(m.h_fw), _p(m.pi), _p(m.val), _p(m.act), 0, 1, 0, 0, None, None, None,
+                                           None, None, 0, 1, R, m._st()))
 
     def pi_only():
-        _lib.check(lib.tscl_policy_step_pi(m._h, _p(m.P), _p(m.Wp), _p(obs), C.c_int64(R), _p(c), _p(h), _p(c), _p(h),
-                                           _p(pi), _p(act), C.c_int32(1), C.c_int32(0), C.c_uint64(1), C.c_int64(0),
-                                           C.c_int64(0), C.c_int64(0), C.c_int64(0), m._st()))
+        _lib.check(lib.tscl_policy_step_pi(m._h, _p(m.P), _p(m.Wp), _p(obs), R, _p(c), _p(h), _p(c), _p(h), _p(pi),
+                                           _p(act), 1, 0, 1, 0, 0, 0, 0, m._st()))
 
     res = {}
     for rep in range(2):                       # alternate the two kernels; report the second round
@@ -237,17 +235,16 @@ def time_q_kernel(scenario, agent, R, launches, warmup):
     lay = QLayout.from_iql(model, net.node_obs_off, net.n_obs, max_na=net.max_na)
     h = C.c_void_p()
     lib = _lib.lib()
-    _lib.check(lib.tscl_q_create(C.byref(lay.as_c()), C.c_int32(0), C.byref(h)))
+    _lib.check(lib.tscl_q_create(C.byref(lay.as_c()), 0, C.byref(h)))
     P = lay.pack(model.nets)
     g = torch.Generator(device="cuda").manual_seed(0)
     obs = torch.rand(R, net.n_obs, device="cuda", generator=g) * 2
     q = torch.zeros(R, lay.A, lay.max_na, device="cuda")
     act = torch.zeros(R, lay.A, dtype=torch.int32, device="cuda")
-    st = C.c_void_p(torch.cuda.current_stream().cuda_stream)
+    st = _lib.stream()
 
     def fn():
-        _lib.check(lib.tscl_q_step(h, _p(P), _p(obs), C.c_int64(R), _p(q), _p(act), C.c_int32(0), C.c_uint64(1),
-                                   C.c_int64(0), C.c_int64(0), None, st))
+        _lib.check(lib.tscl_q_step(h, _p(P), _p(obs), R, _p(q), _p(act), 0, 1, 0, 0, None, st))
     for _ in range(warmup):
         fn()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)

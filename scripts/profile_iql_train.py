@@ -92,16 +92,14 @@ def main():
             # TD kernel (tscl_q_td: TD kernel + fixed-order reduction) alone over many launches
             m.sample(0)
             torch.cuda.synchronize()
-            import ctypes as C
             from deeprl_signal_control_b200 import _lib
-            p = lambda t: C.c_void_p(t.data_ptr())
+            p = _lib.ptr
             lib = _lib.lib()
             t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             t0.record()
             for _ in range(args.td_reps):
-                _lib.check(lib.tscl_q_td(m._h, p(m.P), p(m.s), p(m.s1), p(m.a), p(m.r), p(m.done), p(m.idx),
-                                         C.c_int64(R), C.c_int32(20), C.c_float(0.99), C.c_float(1.0 / (20 * R)),
-                                         p(m.grad), m._st()))
+                _lib.check(lib.tscl_q_td(m._h, p(m.P), p(m.s), p(m.s1), p(m.a), p(m.r), p(m.done), p(m.idx), R, 20,
+                                         0.99, 1.0 / (20 * R), p(m.grad), m._st()))
             t1.record(); torch.cuda.synchronize()
             td_ms = t0.elapsed_time(t1) / args.td_reps
             fl = td_flops(lay, R, 20)

@@ -1,5 +1,4 @@
 """Per-phase clock64 breakdown of the fused policy kernel (thread 0 of every CTA): python scripts/profile_policy_phases.py [R]"""
-import ctypes as C
 import sys
 
 import torch
@@ -25,7 +24,7 @@ for store in (True, False):
         m.forward(obs, False)
     prof = torch.zeros(16, dtype=torch.int64, device="cuda")
     lib = _lib.lib()
-    lib.tscl_debug_policy_prof(C.c_void_p(prof.data_ptr()))
+    lib.tscl_debug_policy_prof(prof.data_ptr())
     n = 4
     for i in range(n):
         m.t = i

@@ -1,5 +1,4 @@
 """Times tscl_dx_tc against the library product on one update chunk (grid MA2C: 50 units x 122 880 rows): python scripts/time_dx_kernel.py"""
-import ctypes as C
 import sys
 
 import torch
@@ -17,9 +16,8 @@ U, dx, M = lay.U, lay.dx, 1024 * 120
 dZ = (torch.randn(U, M, 256, device="cuda") * 0.1).to(torch.bfloat16)
 dX = torch.empty(U, M, dx, device="cuda", dtype=torch.bfloat16)
 wxb = m.pv["wx"].to(torch.bfloat16)
-st = C.c_void_p(torch.cuda.current_stream().cuda_stream)
-own = lambda: _lib.check(_lib.lib().tscl_dx_tc(m._h, C.c_void_p(dZ.data_ptr()), C.c_void_p(m.Wxt.data_ptr()),
-                                               C.c_void_p(dX.data_ptr()), C.c_int64(M), st))
+st = _lib.stream()
+own = lambda: _lib.check(_lib.lib().tscl_dx_tc(m._h, dZ.data_ptr(), m.Wxt.data_ptr(), dX.data_ptr(), M, st))
 libf = lambda: torch.bmm(dZ, wxb.transpose(1, 2), out=dX)
 nbytes = U * M * (256 + dx) * 2
 for name, f in (("tscl_dx_tc", own), ("torch.bmm", libf)):

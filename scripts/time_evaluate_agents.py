@@ -144,8 +144,7 @@ def time_kernels(K, S, iters):
     from deeprl_signal_control_b200.agents.layout import QLayout
     from deeprl_signal_control_b200.agents.learner import BatchedA2C
     from deeprl_signal_control_b200.agents.models import IQL
-    lib, st = _lib.lib(), C.c_void_p(torch.cuda.current_stream().cuda_stream)
-    p = lambda t: C.c_void_p(t.data_ptr())
+    lib, st, p = _lib.lib(), _lib.stream(), _lib.ptr
     R = K * S
 
     class A:
@@ -162,14 +161,13 @@ def time_kernels(K, S, iters):
     act = torch.zeros(R, lay.A, dtype=torch.int32, device="cuda")
     cm, hm = torch.zeros(lay.A, S, lay.h, device="cuda"), torch.zeros(lay.A, S, lay.h, device="cuda")
     grouped = lambda: _lib.check(lib.tscl_policy_step_pi_g(
-        ms[0]._h, p(P), C.c_int64(P.shape[1]), p(Wp), C.c_int64(Wp[0].numel()), p(obs), C.c_int32(K), p(rows), C.c_int64(R),
-        p(c), p(h), p(c), p(h), p(pi), p(act), C.c_int32(0), C.c_int32(0), p(seeds), C.c_int64(1), st))
+        ms[0]._h, p(P), P.shape[1], p(Wp), Wp[0].numel(), p(obs), K, p(rows), R, p(c), p(h), p(c), p(h), p(pi), p(act),
+        0, 0, p(seeds), 1, st))
 
     def members():
         for k, m in enumerate(ms):
-            _lib.check(lib.tscl_policy_step_pi(m._h, p(m.P), p(m.Wp), p(obs[k * S:(k + 1) * S]), C.c_int64(S), p(cm), p(hm),
-                                               p(cm), p(hm), p(pi[k * S:]), p(act[k * S:]), C.c_int32(0), C.c_int32(0),
-                                               C.c_uint64(k), C.c_int64(1), C.c_int64(0), C.c_int64(0), C.c_int64(0), st))
+            _lib.check(lib.tscl_policy_step_pi(m._h, p(m.P), p(m.Wp), p(obs[k * S:(k + 1) * S]), S, p(cm), p(hm), p(cm),
+                                               p(hm), p(pi[k * S:]), p(act[k * S:]), 0, 0, k, 1, 0, 0, 0, st))
     out = {"pi_g_us": _events(grouped, iters), "pi_members_us": _events(members, iters)}
     from deeprl_signal_control_b200.net.large_grid import build_large_grid
     qnet = build_large_grid(agent="iqll")
@@ -179,18 +177,18 @@ def time_kernels(K, S, iters):
     qm = IQL(qnet.n_s_ls, qnet.n_a_ls, qnet.n_w_ls, 0, cp["M"], seed=0, model_type="lr", device="cuda")
     ql = QLayout.from_iql(qm, np.asarray(qnet.node_obs_off), qnet.n_obs, max_na=qnet.max_na)
     hq = C.c_void_p()
-    _lib.check(lib.tscl_q_create(C.byref(ql.as_c()), C.c_int32(0), C.byref(hq)))
+    _lib.check(lib.tscl_q_create(C.byref(ql.as_c()), 0, C.byref(hq)))
     QP = ql.pack(qm.nets).cuda().repeat(K, 1).contiguous()
     qobs = torch.rand(R, qnet.n_obs, device="cuda")
     q = torch.zeros(R, ql.A, ql.max_na, device="cuda")
     qact = torch.zeros(R, ql.A, dtype=torch.int32, device="cuda")
-    qg = lambda: _lib.check(lib.tscl_q_step_g(hq, p(QP), C.c_int64(ql.n_params), p(qobs), C.c_int32(K), p(rows),
-                                              C.c_int64(R), p(q), p(qact), C.c_int32(0), p(seeds), C.c_int64(1), None, st))
+    qg = lambda: _lib.check(lib.tscl_q_step_g(hq, p(QP), ql.n_params, p(qobs), K, p(rows), R, p(q), p(qact), 0,
+                                              p(seeds), 1, None, st))
 
     def qmembers():
         for k in range(K):
-            _lib.check(lib.tscl_q_step(hq, p(QP[k]), p(qobs[k * S:]), C.c_int64(S), p(q[k * S:]), p(qact[k * S:]),
-                                       C.c_int32(0), C.c_uint64(k), C.c_int64(1), C.c_int64(0), None, st))
+            _lib.check(lib.tscl_q_step(hq, p(QP[k]), p(qobs[k * S:]), S, p(q[k * S:]), p(qact[k * S:]), 0, k, 1, 0,
+                                       None, st))
     out.update(q_g_us=_events(qg, iters), q_members_us=_events(qmembers, iters))
     lib.tscl_q_destroy(hq)
     return out

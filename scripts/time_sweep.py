@@ -15,7 +15,6 @@ A sweep whose activation store does not fit the card is reported as such.  Print
 the card's name and power limit, and writes them to $OUT/time_sweep.json (OUT defaults to results/).
 """
 import argparse
-import ctypes as C
 import dataclasses
 import json
 import os
@@ -92,27 +91,23 @@ def main():
 
     def kernel_ms(m, K, Rm):
         """(grouped, per-member) ms of the returns and of the reward hand-over on the sweep learner's buffers"""
-        lib, st = _lib.lib(), C.c_void_p(torch.cuda.current_stream().cuda_stream)
-        ptr = lambda t: C.c_void_p(t.data_ptr())
+        lib, st, ptr = _lib.lib(), _lib.stream(), _lib.ptr
         T, R, A_ = m.T, m.R, m.lay.A
         dpost = torch.zeros(T, device=m.dev)
         rew, grew, acc = torch.randn(R, A_, device=m.dev), torch.randn(R, device=m.dev), torch.zeros(R, device=m.dev)
         Rm_rows = lambda t, k: ptr(t[k * Rm:])          # member k's rows of a [R, ...] buffer
         calls = {
             "returns_g": lambda: lib.tscl_returns_g(m._h, ptr(m.rew_hist), ptr(m.val_hist), ptr(m.boot), ptr(dpost),
-                                                    ptr(m.gamma_dev), C.c_int32(K), C.c_int32(T), C.c_int64(R), ptr(m.Rs),
-                                                    ptr(m.Adv), st),
+                                                    ptr(m.gamma_dev), K, T, R, ptr(m.Rs), ptr(m.Adv), st),
             # K one-member launches on R_m-replica buffers (the layout of K solo learners)
-            "returns_solo": lambda: [lib.tscl_returns(m._h, ptr(sr[k]), ptr(sv[k]), ptr(sb[k]), ptr(dpost),
-                                                      C.c_float(0.99), C.c_int32(T), C.c_int64(Rm), ptr(sR[k]), ptr(sA[k]),
-                                                      st) for k in range(K)],
-            "transition_g": lambda: lib.tscl_device_transition_g(m._h, ptr(rew), ptr(m.rew_hist[0]), C.c_int64(R * A_),
-                                                                 ptr(m.rnorm_dev), ptr(m.rclip_dev), C.c_int32(K),
-                                                                 ptr(grew), ptr(acc), C.c_int64(R), st),
+            "returns_solo": lambda: [lib.tscl_returns(m._h, ptr(sr[k]), ptr(sv[k]), ptr(sb[k]), ptr(dpost), 0.99, T, Rm,
+                                                      ptr(sR[k]), ptr(sA[k]), st) for k in range(K)],
+            "transition_g": lambda: lib.tscl_device_transition_g(m._h, ptr(rew), ptr(m.rew_hist[0]), R * A_,
+                                                                 ptr(m.rnorm_dev), ptr(m.rclip_dev), K, ptr(grew),
+                                                                 ptr(acc), R, st),
             "transition_solo": lambda: [lib.tscl_device_transition(m._h, Rm_rows(rew, k), Rm_rows(m.rew_hist[0], k),
-                                                                   C.c_int64(Rm * A_), C.c_float(reward_norm),
-                                                                   C.c_float(2.0), Rm_rows(grew, k), Rm_rows(acc, k),
-                                                                   C.c_int64(Rm), st) for k in range(K)],
+                                                                   Rm * A_, reward_norm, 2.0, Rm_rows(grew, k),
+                                                                   Rm_rows(acc, k), Rm, st) for k in range(K)],
         }
         sr, sv, sR, sA = ([torch.randn(T, Rm, A_, device=m.dev) for _ in range(K)] for _ in range(4))
         sb = [torch.randn(Rm, A_, device=m.dev) for _ in range(K)]
