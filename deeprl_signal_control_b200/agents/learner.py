@@ -150,6 +150,24 @@ def learner_paths(layout: PolicyLayout, use_tc: bool = True, K: int = 1, dx_libr
     return p
 
 
+def deterministic_refusal(paths, store_acts: bool) -> Optional[str]:
+    """Why `BatchedA2C(deterministic=True)` with kernel paths `paths` (learner_paths) and activation store `store_acts`
+    cannot run its update in a fixed summation order, or None: only the lean update (the BPTT with the heads inside,
+    the all-bf16 LSTM weight gradients, dX fused into the fc weight gradients) has deterministic kernels."""
+    if not paths.use_tc:
+        return "use_tc=False selects the fp32 twin kernels, which add their gradients with atomics"
+    if paths.update != "lean":
+        return ("this layout's update is %r, not the lean tensor-core update (the only one with deterministic kernels)"
+                % paths.update)
+    if not paths.dx_fc_fused:
+        return "TSC_DX_LIBRARY=1 replaces the fused dX / fc weight-gradient kernel, which has the deterministic form"
+    if os.environ.get("TSC_BPTT_HEADS", "1") == "0":
+        return "TSC_BPTT_HEADS=0 selects tscl_heads_loss, which has no deterministic form"
+    if not store_acts:
+        return "the update must back-propagate through the activation store (store_acts off or it does not fit)"
+    return None
+
+
 class BatchedA2C:
     def __init__(self, layout: PolicyLayout, n_replicas: int, n_step: int, gamma: float = 0.99,
                  v_coef: float = 0.5, max_grad_norm: float = 40.0, alpha: float = 0.99, eps: float = 1e-5,
@@ -157,7 +175,13 @@ class BatchedA2C:
                  chunk: int = 1024, replica0: int = 0, total_replicas: Optional[int] = None,
                  process_group=None, allow_tf32: bool = True, use_tc: bool = True,
                  store_acts: Optional[bool] = None, seeds: Optional[Sequence[int]] = None,
-                 hparams: Optional[Sequence[dict]] = None):
+                 hparams: Optional[Sequence[dict]] = None, deterministic: bool = False):
+        if deterministic:       # the layout / switch refusals, before any device work
+            why = deterministic_refusal(learner_paths(layout, use_tc, 1 if seeds is None else len(seeds),
+                                                      os.environ.get("TSC_DX_LIBRARY", "0") == "1"),
+                                        store_acts is not False)
+            if why:
+                raise ValueError("deterministic=True needs the lean update: " + why)
         if hparams is None:
             self.seeds = check_population(seeds, seed, n_replicas, chunk, process_group)
             self.hp = [dict(gamma=gamma, v_coef=v_coef, max_grad_norm=max_grad_norm, alpha=alpha, eps=eps,
@@ -185,6 +209,10 @@ class BatchedA2C:
         h = C.c_void_p()
         _lib.check(lib.tscl_create(C.byref(self._cd), device, C.byref(h)))
         self._h = h
+        # deterministic: the update kernels add in a fixed order (tscl_set_deterministic; same bits run to run)
+        self.deterministic = bool(deterministic)
+        if self.deterministic:
+            _lib.check(lib.tscl_set_deterministic(h, 1, 0))
         L, R, T, U, A = layout, self.R, self.T, layout.U, layout.A
         f32 = dict(dtype=torch.float32, device=self.dev)
         if self.K == 1:
@@ -274,6 +302,9 @@ class BatchedA2C:
             self.st_x = torch.zeros(nc, U, T, rc_, L.dx, **bf); self.st_g = torch.zeros(nc, U, T, rc_, 4 * L.h, **bf)
             self.st_c = torch.zeros(nc, U, T, rc_, L.h, **bf); self.st_h = torch.zeros(nc, U, T, rc_, L.h, **bf)
         self._acts_ok = [False] * T      # step t of the current rollout was produced by a storing forward()
+        if self.deterministic and not self.store_acts:
+            raise ValueError("deterministic=True needs the lean update: the update must back-propagate through the "
+                             "activation store, which does not fit (%.2f GB)" % (need / 1e9))
 
     def close(self):
         if getattr(self, "_h", None) is not None:
@@ -567,6 +598,13 @@ class BatchedA2C:
         use_store = self.store_acts and all(self._acts_ok)
         if self.K > 1 and not use_store:
             raise RuntimeError("a population update needs every step of the rollout in the activation store")
+        if self.deterministic:
+            if not use_store:
+                raise RuntimeError("a deterministic update needs every step of the rollout in the activation store "
+                                   "(a step was not produced by a storing forward)")
+            if self.dx_fused:
+                raise ValueError("deterministic=True needs the lean update: dx_fused = True selects the BPTT kernel "
+                                 "with dX inside, which has no deterministic form")
         n_obs = L.n_obs
         P, G, Wt, Wxt, stats = self.P, self.G, self.Wt, self.Wxt, self.stats
         k = 0

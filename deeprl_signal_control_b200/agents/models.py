@@ -56,16 +56,23 @@ class IA2C:
     name = 'ia2c'
 
     def __init__(self, n_s_ls, n_a_ls, n_w_ls, total_step, model_config, seed=0, n_f_ls=None,
-                 n_replicas=1, device=0, obs_off=None, policy='lstm', seeds=None, member_configs=None, **learner_kw):
+                 n_replicas=1, device=0, obs_off=None, policy='lstm', seeds=None, member_configs=None,
+                 deterministic=False, **learner_kw):
         """policy='lstm': LstmACPolicy / FPLstmACPolicy, what the reference builds (agents/models.py:40-51);
         policy='fc': FcACPolicy (agents/policies.py:214-256), the FC variant of BASELINE config 2.
         seeds: a population of len(seeds) members, n_replicas each, member k initialised from seeds[k] (`BatchedA2C`;
         LSTM policy only); `members()` gives each as a solo model.
         member_configs: a sweep, one [MODEL_CONFIG] section per seed (model_config is member 0's): member k takes its
         learner values (`a2c_hparams`) and its lr / beta schedules (`lr_schedulers[k]`, `beta_schedulers[k]`) from
-        member_configs[k]; seeds may then repeat."""
+        member_configs[k]; seeds may then repeat.
+        deterministic: the update adds its gradients in a fixed order, so equal runs give equal bits
+        (`BatchedA2C(deterministic=True)`; LSTM policy only)."""
         if seeds is not None and len(seeds) > 1 and policy == 'fc':
             raise ValueError("a population trains the LSTM policy only (got policy='fc')")
+        if deterministic:
+            if policy == 'fc':
+                raise ValueError("deterministic=True needs the LSTM policy's lean update (got policy='fc')")
+            learner_kw['deterministic'] = True
         if member_configs is not None:
             if seeds is None or len(member_configs) != len(seeds):
                 raise ValueError("a sweep takes one seed per member config")

@@ -287,11 +287,13 @@ def run_schedule(drivers):
 
 
 def build_model(agent, env, model_config, total_step, n_replicas, policy='lstm', seed=0, device=0, replica0=0,
-                total_replicas=None, process_group=None, seeds=None, member_configs=None):
+                total_replicas=None, process_group=None, seeds=None, member_configs=None, deterministic=False):
     """main.py:110-121 on the batched learners: IA2C / MA2C wrappers (seed = ENV_CONFIG.seed) or BatchedIQL (seed 0).
     `n_replicas` are this rank's replicas, the global ones [replica0, replica0 + n_replicas) of `total_replicas`; the
     learner all-reduces its gradient over `process_group` when one is given.  `seeds`: an A2C population, one member
-    per seed on n_replicas replicas each (`BatchedA2C`); with `member_configs` (one [MODEL_CONFIG] per seed) a sweep."""
+    per seed on n_replicas replicas each (`BatchedA2C`); with `member_configs` (one [MODEL_CONFIG] per seed) a sweep.
+    `deterministic`: the A2C update adds in a fixed order (`BatchedA2C(deterministic=True)`); IQL's TD kernel already
+    reduces in a fixed order, so for iqll / iqld it changes nothing."""
     kind, model_type = model_spec(agent)
     t = env._tables
     if kind != 'iql':
@@ -303,6 +305,8 @@ def build_model(agent, env, model_config, total_step, n_replicas, policy='lstm',
             kw.update(seeds=seeds)
         if member_configs is not None:
             kw.update(member_configs=member_configs)
+        if deterministic:
+            kw.update(deterministic=True)
         if kind == 'ma2c':
             return MA2C(env.n_s_ls, env.n_a_ls, env.n_w_ls, env.n_f_ls, total_step, model_config, **kw)
         return IA2C(env.n_s_ls, env.n_a_ls, env.n_w_ls, total_step, model_config, **kw)
@@ -338,7 +342,7 @@ def member_dir(base_dir, seed, agent):
 
 
 def train(config, base_dir, test_mode='no_test', n_replicas=1, policy='lstm', device=0, process_group=None,
-          summaries=False, seeds=None):
+          summaries=False, seeds=None, deterministic=False):
     """main.py train.  `config`: the path of a reference config (copied into data/) or a parsed ConfigParser (written
     to data/config.ini), with [ENV_CONFIG], [MODEL_CONFIG] and [TRAIN_CONFIG].  Returns a namespace with final_step,
     episode_sets, env_samples (= final_step * n_replicas), wall_sec, world, rank, data (the train_reward.csv rows),
@@ -359,11 +363,19 @@ def train(config, base_dir, test_mode='no_test', n_replicas=1, policy='lstm', de
     the run then allocates, launches and writes nothing for it.
 
     `seeds`: train a population instead, one member per seed, each on `n_replicas` replicas, in one process
-    (`train_population`).  Returns its namespace."""
+    (`train_population`).  Returns its namespace.
+
+    `deterministic`: the A2C update adds its gradients, loss sums and clip norms in a fixed order
+    (`BatchedA2C(deterministic=True)`), so two runs with the same config, seeds, replicas, world size, build and GPU
+    model leave the same bits: checkpoint, CSVs and summaries.  The LSTM policy only (refused for policy='fc' before any
+    directory is made); a no-op for IQL, whose update is already reproducible."""
+    if deterministic and policy != 'lstm':
+        raise ValueError("deterministic=True needs the LSTM policy's lean update (got policy=%r)" % (policy,))
     if seeds is not None:
         if process_group is not None:
             raise ValueError('a population trains in one process: seeds and process_group exclude each other')
-        return train_population(config, base_dir, seeds, test_mode, n_replicas, policy, device, summaries)
+        return train_population(config, base_dir, seeds, test_mode, n_replicas, policy, device, summaries,
+                                deterministic=deterministic)
     t0 = time.time()
     in_test, post_test = init_test_flag(test_mode)
     world, rank = 1, 0
@@ -389,7 +401,8 @@ def train(config, base_dir, test_mode='no_test', n_replicas=1, policy='lstm', de
             path, config = config, configparser.ConfigParser()
             if not config.read(path):
                 raise FileNotFoundError(path)
-        out = _train(config, dirs, in_test, post_test, int(n_replicas), policy, device, pg, bool(summaries))
+        out = _train(config, dirs, in_test, post_test, int(n_replicas), policy, device, pg, bool(summaries),
+                     bool(deterministic))
     finally:
         for h in handlers:
             logging.getLogger().removeHandler(h)
@@ -445,7 +458,7 @@ def _schedule(config, env):
     return total_step, counter, T
 
 
-def _train(config, dirs, in_test, post_test, R_total, policy, device, pg, summaries=False):
+def _train(config, dirs, in_test, post_test, R_total, policy, device, pg, summaries=False, deterministic=False):
     import torch
     from ..envs import make_env
     from .evaluator import Evaluator
@@ -466,7 +479,7 @@ def _train(config, dirs, in_test, post_test, R_total, policy, device, pg, summar
     writer = None
     try:
         model = build_model(agent, env, mc, total_step, R, policy=policy, seed=seed, device=device, replica0=replica0,
-                            total_replicas=R_total, process_group=pg)
+                            total_replicas=R_total, process_group=pg, deterministic=deterministic)
         sim = env._ensure_sim()
         trace = torch.zeros(T, R, dtype=torch.float32, device=sim.device)
         summary, srec = None, {}
@@ -526,7 +539,7 @@ def _member_filter(k):
 
 
 def train_population(config, base_dir, seeds, test_mode='no_test', n_replicas=1, policy='lstm', device=0,
-                     summaries=False):
+                     summaries=False, deterministic=False):
     """Train K = len(seeds) members of one A2C agent (ia2c / ma2c, LSTM policy) in one process, member k with
     `[ENV_CONFIG] seed = seeds[k]` on `n_replicas` replicas (a multiple of 64).  One simulator launch and one grouped
     policy forward per control step cover all K * n_replicas replicas (`BatchedA2C` with seeds); the update, the
@@ -534,7 +547,8 @@ def train_population(config, base_dir, seeds, test_mode='no_test', n_replicas=1,
     n_replicas=n_replicas)` trains alone, and its directory `member_dir(base_dir, seeds[k], agent)` holds what that
     run leaves: data/ (the config with the member's seed, train_reward.csv, test CSVs), model/checkpoint-<step>.npz,
     log/<time>.log and, with `summaries`, the member's event file.  Returns a namespace like train()'s with per-member
-    lists `dirs`, `data`, `post_test` and `members`."""
+    lists `dirs`, `data`, `post_test` and `members`.  `deterministic`: as in train(); member k then equals its solo
+    deterministic run bit for bit."""
     import copy
     from .learner import check_population
     t0 = time.time()
@@ -562,12 +576,13 @@ def train_population(config, base_dir, seeds, test_mode='no_test', n_replicas=1,
             cfg.write(f)
         cfgs.append(cfg); dirs.append(d)
     out = _train_members(cfgs, dirs, agent, seeds, int(n_replicas), in_test, post_test, policy, device, summaries,
-                         'population of %d seeds %s' % (len(seeds), seeds))
+                         'population of %d seeds %s' % (len(seeds), seeds), deterministic=deterministic)
     out.dirs, out.wall_sec = [member_dir(base_dir, s, agent) for s in seeds], time.time() - t0
     return out
 
 
-def _train_members(cfgs, dirs, agent, seeds, R_m, in_test, post_test, policy, device, summaries, what, sweep=False):
+def _train_members(cfgs, dirs, agent, seeds, R_m, in_test, post_test, policy, device, summaries, what, sweep=False,
+                   deterministic=False):
     """The training run of a population or a sweep, member k from cfgs[k] (seed seeds[k]) into the agent directory
     dirs[k] (init_dir's dict): member-tagged log files, one simulator and one learner for all K * R_m replicas, one
     driver per member.  A sweep gives each member its own learner values and schedules (`IA2C(member_configs=...)`)
@@ -603,7 +618,8 @@ def _train_members(cfgs, dirs, agent, seeds, R_m, in_test, post_test, policy, de
                      % (env.n_s, env.n_s_ls, env.n_a_ls, what, R_m))
         total_step, counter, T = _schedule(cfgs[0], env)
         model = build_model(agent, env, mc, total_step, R_m, seeds=seeds, device=device,
-                            member_configs=[c['MODEL_CONFIG'] for c in cfgs] if sweep else None)
+                            member_configs=[c['MODEL_CONFIG'] for c in cfgs] if sweep else None,
+                            deterministic=deterministic)
         members = model.members()
         sim = env._ensure_sim()
         trace = torch.zeros(T, K * R_m, dtype=torch.float32, device=sim.device)
@@ -717,7 +733,7 @@ def sweep_dir(base_dir, name, agent):
 
 
 def train_sweep(configs, base_dir, test_mode='no_test', n_replicas=64, device=0, summaries=False, policy='lstm',
-                process_group=None):
+                process_group=None, deterministic=False):
     """Train a hyperparameter sweep of one A2C agent (ia2c / ma2c, LSTM policy) in one process: one member per config
     (`sweep_members`: the configs may differ only in SWEEP_CONFIG_KEYS), each on `n_replicas` replicas (a multiple of
     64).  One simulator launch and one grouped policy forward per control step cover all K * n_replicas replicas;
@@ -725,7 +741,7 @@ def train_sweep(configs, base_dir, test_mode='no_test', n_replicas=64, device=0,
     `train(config_k, n_replicas=n_replicas)` trains alone.  Its directory `sweep_dir(base_dir, name_k, agent)` holds
     what that run leaves: data/ (its config, train_reward.csv, test CSVs), model/checkpoint-<step>.npz, log/<time>.log
     and, with `summaries`, its event file.  Everything is checked before any directory or device work.  Returns a
-    namespace like train_population's with `names`."""
+    namespace like train_population's with `names`.  `deterministic`: as in train()."""
     from .learner import check_sweep
     from .models import a2c_hparams
     t0 = time.time()
@@ -752,7 +768,7 @@ def train_sweep(configs, base_dir, test_mode='no_test', n_replicas=64, device=0,
                 cfg.write(f)
         dirs.append(d)
     out = _train_members(cfgs, dirs, agent, seeds, int(n_replicas), in_test, post_test, policy, device, summaries,
-                         'sweep of %d configs %s' % (len(cfgs), names), sweep=True)
+                         'sweep of %d configs %s' % (len(cfgs), names), sweep=True, deterministic=deterministic)
     out.names, out.dirs = names, [sweep_dir(base_dir, n, agent) for n in names]
     out.wall_sec = time.time() - t0
     return out

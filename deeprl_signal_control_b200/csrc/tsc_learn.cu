@@ -50,6 +50,11 @@ struct tscl_handle {
   int max_fcw = 0;     // max fc weight floats of a unit (incl. biases)
   std::map<void*, float*> acc_tiles;   // accumulator tiles of the tensor-core kernels, per stream (tscl_acc_tiles)
   std::mutex acc_mu;
+  // deterministic mode (tscl_set_deterministic): -1 off, else the CTA cap (0 = none); partial slabs of the DET kernels
+  // (0 BPTT heads, 1 LSTM weight gradients, 2 fc weight gradients, 3 clip norms), allocated on first use
+  int det_ctas = -1;
+  float* det_slab[4] = {nullptr, nullptr, nullptr, nullptr};
+  size_t det_bytes[4] = {0, 0, 0, 0};
 };
 
 __device__ __forceinline__ float sigmoidf_(float x) { return 1.0f / (1.0f + __expf(-x)); }
@@ -778,6 +783,51 @@ __global__ void norm2_kernel(const float* __restrict__ g, const uint8_t* __restr
     atomicAdd(&norm2[a], v);
   }
 }
+// Deterministic form of norm2_kernel: block b sums the squares of elements [b NORM_DET_EL, (b + 1) NORM_DET_EL) per agent
+// in a fixed order (each warp walks its 32-element groups in order: a shuffle tree where the group is one agent's, else
+// lane 0 adds the 32 values one by one), writes part [b][A] (zeros for absent agents), and norm2_det_sum_kernel adds the
+// blocks' rows in block order.  Nothing depends on the grid.  Dynamic smem: 8 warps x A floats.
+#define NORM_DET_EL 8192
+__global__ void __launch_bounds__(256)
+norm2_det_kernel(const float* __restrict__ g, const uint8_t* __restrict__ agent_of, int64_t n, int A, float* __restrict__ part) {
+  extern __shared__ float sw[];                  // [8 warps][A]
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  for (int i = threadIdx.x; i < 8 * A; i += 256) sw[i] = 0.f;
+  __syncthreads();
+  float* acc = sw + warp * A;
+  const int64_t b0 = (int64_t)blockIdx.x * NORM_DET_EL;
+  for (int64_t i0 = b0 + warp * 32; i0 < b0 + NORM_DET_EL && i0 < n; i0 += 256) {
+    const int64_t i = i0 + lane;
+    float v = 0.f;
+    int a = -1;
+    if (i < n) { v = g[i]; v *= v; a = agent_of[i]; }
+    const int a0 = __shfl_sync(0xffffffffu, a, 0);
+    if (__all_sync(0xffffffffu, a == a0)) {
+      for (int o = 16; o; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
+      if (lane == 0) acc[a0] += v;
+    } else {
+      for (int l = 0; l < 32; ++l) {
+        const float vl = __shfl_sync(0xffffffffu, v, l);
+        const int al = __shfl_sync(0xffffffffu, a, l);
+        if (lane == 0 && al >= 0) acc[al] += vl;
+      }
+    }
+    __syncwarp();
+  }
+  __syncthreads();
+  for (int a = threadIdx.x; a < A; a += 256) {
+    float s = 0.f;
+    for (int w = 0; w < 8; ++w) s += sw[w * A + a];
+    part[(int64_t)blockIdx.x * A + a] = s;
+  }
+}
+__global__ void norm2_det_sum_kernel(const float* __restrict__ part, int64_t nb, int A, float* __restrict__ norm2) {
+  const int a = blockIdx.x * blockDim.x + threadIdx.x;
+  if (a >= A) return;
+  float s = 0.f;
+  for (int64_t b = 0; b < nb; ++b) s += part[b * A + a];
+  norm2[a] = s;
+}
 __global__ void rmsprop_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ ms,
                                const uint8_t* __restrict__ agent_of, int64_t n, const float* __restrict__ norm2,
                                float max_norm, float lr, float alpha, float eps, float* __restrict__ norms) {
@@ -971,6 +1021,29 @@ const DDimsTC* tscl_dims_of(tscl_handle* h) { return reinterpret_cast<const DDim
 int tscl_device_of(tscl_handle* h) { return h->device; }
 // `bytes` of device memory for the accumulator tiles of kernels launched on `stream`; allocated on first use, freed with
 // the handle (every caller asks for the same size)
+int tscl_det_ctas(tscl_handle* h) { return h->det_ctas; }
+// slab `kind` of at least `bytes` (grown after the stream's earlier users of the old one have finished)
+float* tscl_det_slab(tscl_handle* h, int kind, size_t bytes, void* stream) {
+  if (h->det_bytes[kind] >= bytes) return h->det_slab[kind];
+  if (h->det_slab[kind]) {
+    if (cudaStreamSynchronize((cudaStream_t)stream) != cudaSuccess) return nullptr;
+    cudaFree(h->det_slab[kind]);
+  }
+  h->det_slab[kind] = nullptr; h->det_bytes[kind] = 0;
+  if (cudaMalloc(&h->det_slab[kind], bytes) != cudaSuccess) { h->det_slab[kind] = nullptr; return nullptr; }
+  h->det_bytes[kind] = bytes;
+  return h->det_slab[kind];
+}
+// refusal of an update entry point that has no deterministic form while the handle is in deterministic mode
+#define NO_DET(name) \
+  if (h && h->det_ctas >= 0) return tsc_set_error(name ": no deterministic form (the handle is in deterministic mode)")
+
+extern "C" int tscl_set_deterministic(tscl_handle* h, int32_t on, int32_t n_ctas) {
+  if (!h || n_ctas < 0) return tsc_set_error("tscl_set_deterministic: bad argument");
+  h->det_ctas = on ? n_ctas : -1;
+  return 0;
+}
+
 float* tscl_acc_tiles(tscl_handle* h, void* stream, size_t bytes) {
   std::lock_guard<std::mutex> lock(h->acc_mu);
   float*& p = h->acc_tiles[stream];
@@ -1039,6 +1112,7 @@ extern "C" int tscl_destroy(tscl_handle* h) {
   cudaSetDevice(h->device);
   for (void* p : h->owned) cudaFree(p);
   for (auto& e : h->acc_tiles) cudaFree(e.second);
+  for (float* p : h->det_slab) if (p) cudaFree(p);
   delete h;
   return 0;
 }
@@ -1077,6 +1151,7 @@ extern "C" int tscl_fc_hidden_fwd(tscl_handle* h, const float* params, const flo
 extern "C" int tscl_fc_hidden_bwd(tscl_handle* h, const float* params, const float* X, const float* H, float* dH, int64_t M,
                                   float* dX, float* grads, void* stream) {
   if (!h || !params || !X || !H || !dH || !dX || !grads || M <= 0) return tsc_set_error("tscl_fc_hidden_bwd: bad argument");
+  NO_DET("tscl_fc_hidden_bwd");
   if (h->d.dx > 256) return tsc_set_error("tscl_fc_hidden_bwd: dx > 256");
   LCK(cudaSetDevice(h->device));
   static int attr_dev = -1;
@@ -1156,6 +1231,7 @@ extern "C" int tscl_heads_loss(tscl_handle* h, const float* params, const float*
                                float v_coef, float beta, float scale, float* dlog, float* dH, float* stats,
                                const void* h_bf16, float* grads, void* stream) {
   if (!h || M <= 0 || (!H && !h_bf16) || !dH) return tsc_set_error("tscl_heads_loss: bad argument");
+  NO_DET("tscl_heads_loss");
   if (h->d.max_na > 8) return tsc_set_error("tscl_heads_loss: more than 8 actions");
   LCK(cudaSetDevice(h->device));
   const int64_t n_tiles = (M + 127) / 128;
@@ -1171,6 +1247,7 @@ extern "C" int tscl_lstm_seq_bwd(tscl_handle* h, const float* params, float* ZG,
                                  const float* c0, const float* done, int32_t T, int64_t Rc, int64_t ld_state,
                                  int64_t r0, void* stream) {
   if (!h || T <= 0 || Rc <= 0) return tsc_set_error("tscl_lstm_seq_bwd: bad argument");
+  NO_DET("tscl_lstm_seq_bwd");
   LCK(cudaSetDevice(h->device));
   dim3 grid((unsigned)((Rc + LS_ROWS - 1) / LS_ROWS), 2 * h->d.A);
   lstm_seq_bwd_kernel<<<grid, 256, (G4 * H64 + LS_ROWS * G4) * 4, (cudaStream_t)stream>>>(h->d, params, ZG, C, dH, c0,
@@ -1182,6 +1259,7 @@ extern "C" int tscl_lstm_seq_bwd(tscl_handle* h, const float* params, float* ZG,
 extern "C" int tscl_fc_bwd(tscl_handle* h, const float* obs, const float* X, const float* dX, int64_t M,
                            int64_t rows_per_t, int64_t stride_t, float* grads, void* stream) {
   if (!h || M <= 0) return tsc_set_error("tscl_fc_bwd: bad argument");
+  NO_DET("tscl_fc_bwd");
   LCK(cudaSetDevice(h->device));
   int64_t ng = (M + FB_ROWS - 1) / FB_ROWS;
   if (ng > 24) ng = 24;
@@ -1215,7 +1293,15 @@ extern "C" int tscl_clip_rmsprop(tscl_handle* h, float* params, float* grads, fl
   LCK(cudaMallocAsync(&norm2, sizeof(float) * h->d.A, st));
   LCK(cudaMemsetAsync(norm2, 0, sizeof(float) * h->d.A, st));
   const int64_t n = h->d.n_params;
-  norm2_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(grads, agent_of, n, norm2);
+  if (h->det_ctas >= 0) {
+    const int64_t nb = (n + NORM_DET_EL - 1) / NORM_DET_EL;
+    float* part = tscl_det_slab(h, 3, (size_t)nb * h->d.A * sizeof(float), stream);
+    if (!part) return tsc_set_error("tscl_clip_rmsprop: cudaMalloc of the deterministic slab failed");
+    norm2_det_kernel<<<(unsigned)nb, 256, 8 * h->d.A * sizeof(float), st>>>(grads, agent_of, n, h->d.A, part);
+    norm2_det_sum_kernel<<<(h->d.A + 63) / 64, 64, 0, st>>>(part, nb, h->d.A, norm2);
+  } else {
+    norm2_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(grads, agent_of, n, norm2);
+  }
   rmsprop_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(params, grads, ms, agent_of, n, norm2, max_norm, lr, alpha,
                                                               eps, norms);
   LCK(cudaGetLastError());

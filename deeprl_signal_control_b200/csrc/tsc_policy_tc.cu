@@ -42,6 +42,10 @@ struct DDimsTC {   // mirror of DDims in tsc_learn.cu (kept in sync by tscl_hand
 const DDimsTC* tscl_dims_of(tscl_handle* h);   // defined in tsc_learn.cu
 int tscl_device_of(tscl_handle* h);
 float* tscl_acc_tiles(tscl_handle* h, void* stream, size_t bytes);   // defined in tsc_learn.cu
+// deterministic mode of the handle (tscl_set_deterministic): -1 off, else the CTA cap (0: none); and its partial slab
+// `kind` of at least `bytes`, allocated on first use and grown on demand (defined in tsc_learn.cu)
+int tscl_det_ctas(tscl_handle* h);
+float* tscl_det_slab(tscl_handle* h, int kind, size_t bytes, void* stream);
 
 #define TC_M 128
 #define TC_N 256
@@ -1356,6 +1360,18 @@ struct BwdTC {
   int n_chunks;              // consecutive chunks of Rc replicas ([n_chunks][2A][T][Rc][w] store blocks)
 };
 
+// Deterministic mode (tscl_set_deterministic): the DET instantiations of the update kernels store each accumulator
+// fragment into a partial slab instead of adding it to G with atomics, and a reduce kernel adds the slabs into G in a
+// fixed order.  A slab row belongs to one work item (BPTT: one (chunk, unit, 128-row tile) item) or to one segment of
+// seg_tiles consecutive tiles of one unit (weight-gradient kernels; n_seg segments per unit, both from the shapes), never
+// to a CTA, so the sums depend on the shapes only, not on the grid.  Passed as the last kernel argument, unused by the
+// atomic instantiations.
+struct DetTC {
+  float* part;               // [slab rows][floats per row]
+  float* part_st;            // BPTT: agent 0's loss sums per (item, warp) [items][8][3]
+  int64_t seg_tiles, n_seg;
+};
+
 // NT = 512: thread = (replica row, 16 hidden units), one CTA per SM.
 // NT = 256: thread = (replica row, 32 hidden units) processed 8 at a time, TWO CTAs per SM (<= 128 registers): while one
 //           tile waits for its per-step MMA / barrier the other one has its loads in flight.
@@ -1755,11 +1771,13 @@ __device__ __forceinline__ void heads_step(const DDimsTC& d, const BwdTC& a, con
 //   staging tile; while the step's MMA runs, thread (k, logits 4 hh..4 hh + 3) adds h[row][k] * dlog[row][j] over the
 //   warpgroup's 64 rows into registers, flushed to G with one atomic per output at every unit change.
 // Items run over n_chunks consecutive chunks (chunk-outermost, the activation store's order).
-template <bool PROF, bool HEADS = false>
+// DET (with HEADS): at the end of every item each thread stores its head sums into det.part [item][256 threads][5] and
+// each warp of a unit of agent 0 its loss sums into det.part_st [item][8 warps][3]; det_heads_reduce_kernel adds them.
+template <bool PROF, bool HEADS = false, bool DET = false>
 __global__ void __launch_bounds__(256, 1)
 lstm_bwd_tc_regs_kernel(const DDimsTC d, const BwdTC a, const __grid_constant__ CUtensorMap mapG,
                         const __grid_constant__ CUtensorMap mapC, const __grid_constant__ CUtensorMap mapD,
-                        const __grid_constant__ CUtensorMap mapZ) {
+                        const __grid_constant__ CUtensorMap mapZ, const DetTC det) {
   const int tid = threadIdx.x, wg = tid >> 7, w = (tid >> 5) & 3, lane = tid & 31, q = lane & 3;
   const bool lead = (tid & 127) == 0;
   long long bp[4] = {0, 0, 0, 0}, pc = 0;
@@ -1812,7 +1830,7 @@ lstm_bwd_tc_regs_kernel(const DDimsTC d, const BwdTC a, const __grid_constant__ 
     const int rw0 = (int)((ic - (int64_t)u * n_tiles) * TC_M) + 64 * wg;   // first row of this warpgroup
     __syncthreads();                                                 // both warpgroups are done with the previous item
     if (u != cur_u) {
-      if (HEADS && cur_u >= 0) flush(cur_u);
+      if (HEADS && !DET && cur_u >= 0) flush(cur_u);
       cur_u = u;
       const uint4* src = reinterpret_cast<const uint4*>(a.Wt + (int64_t)u * BW_KC * TC_H * 8);
       uint4* dst = reinterpret_cast<uint4*>(sB);
@@ -1989,9 +2007,27 @@ lstm_bwd_tc_regs_kernel(const DDimsTC d, const BwdTC a, const __grid_constant__ 
         for (int e = 0; e < 4; ++e) dhc[j][e] = need_dh ? acc[4 * j + e] * keep : 0.f;
       BR_MARK(2);
     }
+    if constexpr (HEADS && DET) {      // this item's sums into its slab row (a warpgroup without rows stores nothing)
+      float* pf = det.part + (it * 256 + tid) * 5;
+      pf[0] = gw[0]; pf[1] = gw[1]; pf[2] = gw[2]; pf[3] = gw[3]; pf[4] = gb;
+      gw[0] = gw[1] = gw[2] = gw[3] = 0.f; gb = 0.f;
+      if (a.stats && u < 2) {
+#pragma unroll
+        for (int o = 16; o; o >>= 1) {
+          pl += __shfl_down_sync(0xffffffffu, pl, o);
+          vl += __shfl_down_sync(0xffffffffu, vl, o);
+          el += __shfl_down_sync(0xffffffffu, el, o);
+        }
+        if (lane == 0) {
+          float* ps = det.part_st + (it * 8 + (tid >> 5)) * 3;
+          ps[0] = pl; ps[1] = vl; ps[2] = el;
+        }
+        pl = vl = el = 0.f;
+      }
+    }
   }
   if (lead) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // dZ stores complete before the CTA leaves
-  if (HEADS) {
+  if (HEADS && !DET) {
     if (cur_u >= 0) flush(cur_u);
     if (a.stats) {
 #pragma unroll
@@ -2069,6 +2105,7 @@ extern "C" int tscl_lstm_seq_bwd_tc_dx(tscl_handle* h, const void* wt_bf16, floa
                                        const float* c0, const float* done, int32_t T, int64_t Rc, int64_t ld_state,
                                        int64_t r0, const void* gates_bf16, const void* c_bf16, void* dz_bf16,
                                        const void* wxt_bf16, void* dx_bf16, void* stream) {
+  if (h && tscl_det_ctas(h) >= 0) return tsc_set_error("tscl_lstm_seq_bwd_tc_dx: no deterministic form (the handle is in deterministic mode)");
   if (!h || !wt_bf16 || T <= 0 || Rc <= 0) return tsc_set_error("tscl_lstm_seq_bwd_tc: bad argument");
   if ((wxt_bf16 == nullptr) != (dx_bf16 == nullptr)) return tsc_set_error("tscl_lstm_seq_bwd_tc_dx: wxt_bf16 and dx_bf16 go together");
   if (!ZG && !(gates_bf16 && c_bf16 && dz_bf16)) return tsc_set_error("tscl_lstm_seq_bwd_tc: ZG may be null only with gates_bf16, c_bf16 and dz_bf16");
@@ -2119,8 +2156,8 @@ extern "C" int tscl_lstm_seq_bwd_tc_dx(tscl_handle* h, const void* wt_bf16, floa
       }
       const int grid_r = (int)(n_items < n_sm ? n_items : n_sm);
       a.prof = g_bptt_prof;
-      if (a.prof) lstm_bwd_tc_regs_kernel<true><<<grid_r, 256, BR_SMEM, (cudaStream_t)stream>>>(d, a, mG, mC, mD, mZ);
-      else lstm_bwd_tc_regs_kernel<false><<<grid_r, 256, BR_SMEM, (cudaStream_t)stream>>>(d, a, mG, mC, mD, mZ);
+      if (a.prof) lstm_bwd_tc_regs_kernel<true><<<grid_r, 256, BR_SMEM, (cudaStream_t)stream>>>(d, a, mG, mC, mD, mZ, DetTC{});
+      else lstm_bwd_tc_regs_kernel<false><<<grid_r, 256, BR_SMEM, (cudaStream_t)stream>>>(d, a, mG, mC, mD, mZ, DetTC{});
       PCK(cudaGetLastError());
       return 0;
     }
@@ -2129,6 +2166,52 @@ extern "C" int tscl_lstm_seq_bwd_tc_dx(tscl_handle* h, const void* wt_bf16, floa
   else lstm_bwd_tc_kernel<256><<<grid, 256, smem, (cudaStream_t)stream>>>(d, a);
   PCK(cudaGetLastError());
   return 0;
+}
+
+// Deterministic mode of tscl_lstm_seq_bwd_tc_heads: block u < 2A adds unit u's head weight / bias sums chunk by chunk,
+// each chunk's sum over its tiles and warpgroups in that order (thread k = (hidden unit k & 63, logits 4 (k >> 6) ..));
+// block 2A adds agent 0's loss sums chunk by chunk: lane l takes the chunk's (unit, tile, warp) entries l, l + 32, .. in
+// order, then a fixed shuffle tree.  Adding per chunk makes one launch over n chunks give the bits of n one-chunk
+// launches.  A warpgroup whose first row is past Rc stored nothing and is skipped.
+__global__ void __launch_bounds__(128)
+det_heads_reduce_kernel(const DDimsTC d, const DetTC det, float* __restrict__ G, float* __restrict__ stats, float scale,
+                        int n_chunks, int64_t n_tiles, int64_t Rc) {
+  const int u = blockIdx.x, k = threadIdx.x;
+  if (u < 2 * d.A) {
+    const int nl = (u & 1) ? 1 : d.max_na, hk = k & 63, hh = k >> 6;
+    for (int ci = 0; ci < n_chunks; ++ci) {
+      float s[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
+      for (int64_t tl = 0; tl < n_tiles; ++tl)
+        for (int wg = 0; wg < 2; ++wg) {
+          if (tl * TC_M + 64 * wg >= Rc) continue;
+          const float* p = det.part + (((ci * 2 * d.A + u) * n_tiles + tl) * 256 + wg * 128 + k) * 5;
+#pragma unroll
+          for (int e = 0; e < 5; ++e) s[e] += p[e];
+        }
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj)
+        if (hh * 4 + jj < nl) G[d.off_wo + ((int64_t)u * TC_H + hk) * d.max_na + hh * 4 + jj] += s[jj];
+      if (k < nl) G[d.off_bo + (int64_t)u * d.max_na + k] += s[4];
+    }
+    return;
+  }
+  if (!stats || k >= 32) return;
+  const int64_t n = 2 * n_tiles * 8;                          // (unit 0 / 1, tile, warp) of one chunk
+  for (int ci = 0; ci < n_chunks; ++ci) {
+    float s[3] = {0.f, 0.f, 0.f};
+    for (int64_t e = k; e < n; e += 32) {
+      const int w8 = (int)(e & 7);
+      const int64_t tl = (e >> 3) % n_tiles, uu = (e >> 3) / n_tiles;
+      if (tl * TC_M + 64 * (w8 >> 2) >= Rc) continue;
+      const float* p = det.part_st + (((ci * 2 * d.A + uu) * n_tiles + tl) * 8 + w8) * 3;
+      s[0] += p[0]; s[1] += p[1]; s[2] += p[2];
+    }
+#pragma unroll
+    for (int o = 16; o; o >>= 1)
+#pragma unroll
+      for (int i = 0; i < 3; ++i) s[i] += __shfl_down_sync(0xffffffffu, s[i], o);
+    if (k == 0) { stats[0] += s[0] * scale; stats[1] += s[1] * scale; stats[2] += s[2] * scale; }
+  }
 }
 
 extern "C" int tscl_lstm_seq_bwd_tc_heads(tscl_handle* h, const void* wt_bf16, const float* params, const void* gates_bf16,
@@ -2154,20 +2237,34 @@ extern "C" int tscl_lstm_seq_bwd_tc_heads(tscl_handle* h, const void* wt_bf16, c
   if (attr_r != tscl_device_of(h)) {
     PCK(cudaFuncSetAttribute(lstm_bwd_tc_regs_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, BR_SMEM));
     PCK(cudaFuncSetAttribute(lstm_bwd_tc_regs_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, BR_SMEM));
+    PCK(cudaFuncSetAttribute(lstm_bwd_tc_regs_kernel<false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, BR_SMEM));
     attr_r = tscl_device_of(h);
   }
   int n_sm = 0;
   PCK(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, tscl_device_of(h)));
-  const int64_t n_items = (int64_t)n_chunks * ((Rc + TC_M - 1) / TC_M) * 2 * d.A;
-  const int grid = (int)(n_items < n_sm ? n_items : n_sm);
+  const int64_t n_tiles = (Rc + TC_M - 1) / TC_M, n_items = (int64_t)n_chunks * n_tiles * 2 * d.A;
+  const int det_ctas = tscl_det_ctas(h);
+  const int cap = det_ctas > 0 && det_ctas < n_sm ? det_ctas : n_sm;
+  const int grid = (int)(n_items < cap ? n_items : cap);
   BwdTC a = {};
   a.Wt = (const __nv_bfloat16*)wt_bf16; a.c0 = c0; a.done = done; a.T = T; a.Rc = Rc; a.ld_state = ld_state; a.r0 = r0;
   a.Gb = (const __nv_bfloat16*)gates_bf16; a.Cb = (const __nv_bfloat16*)c_bf16; a.dZb = (__nv_bfloat16*)dz_bf16;
   a.P = params; a.act = act; a.Rs = Rs; a.Adv = Adv; a.stride_t = stride_t; a.v_coef = v_coef; a.beta = beta;
   a.scale = scale; a.stats = stats; a.G = grads; a.n_chunks = n_chunks;
   a.prof = g_bptt_prof;
-  if (a.prof) lstm_bwd_tc_regs_kernel<true, true><<<grid, 256, BR_SMEM, (cudaStream_t)stream>>>(d, a, mG, mC, mH, mZ);
-  else lstm_bwd_tc_regs_kernel<false, true><<<grid, 256, BR_SMEM, (cudaStream_t)stream>>>(d, a, mG, mC, mH, mZ);
+  if (det_ctas >= 0) {
+    DetTC det = {};
+    det.part = tscl_det_slab(h, 0, (size_t)n_items * (256 * 5 + 8 * 3) * sizeof(float), stream);
+    if (!det.part) return tsc_set_error("tscl_lstm_seq_bwd_tc_heads: cudaMalloc of the deterministic slab failed");
+    det.part_st = det.part + n_items * 256 * 5;
+    lstm_bwd_tc_regs_kernel<false, true, true><<<grid, 256, BR_SMEM, (cudaStream_t)stream>>>(d, a, mG, mC, mH, mZ, det);
+    PCK(cudaGetLastError());
+    det_heads_reduce_kernel<<<2 * d.A + 1, 128, 0, (cudaStream_t)stream>>>(d, det, grads, stats, scale, n_chunks, n_tiles, Rc);
+  } else if (a.prof) {
+    lstm_bwd_tc_regs_kernel<true, true><<<grid, 256, BR_SMEM, (cudaStream_t)stream>>>(d, a, mG, mC, mH, mZ, DetTC{});
+  } else {
+    lstm_bwd_tc_regs_kernel<false, true><<<grid, 256, BR_SMEM, (cudaStream_t)stream>>>(d, a, mG, mC, mH, mZ, DetTC{});
+  }
   PCK(cudaGetLastError());
   return 0;
 }
@@ -2438,6 +2535,7 @@ fc_bwd_tc_kernel(const DDimsTC d, const FcBwdTC a) {
 extern "C" int tscl_fc_bwd_tc(tscl_handle* h, const float* obs, const float* X, const void* x_bf16, const float* dX,
                               const void* dx_bf16, int64_t M, int64_t rows_per_t, int64_t stride_t, float* grads,
                               int32_t variant, void* stream) {
+  if (h && tscl_det_ctas(h) >= 0) return tsc_set_error("tscl_fc_bwd_tc: no deterministic form (the handle is in deterministic mode)");
   if (!h || !obs || (!X && !x_bf16) || (!dX && !dx_bf16) || !grads || M <= 0) return tsc_set_error("tscl_fc_bwd_tc: bad argument");
   PCK(cudaSetDevice(tscl_device_of(h)));
   const DDimsTC& d = *tscl_dims_of(h);
@@ -2688,8 +2786,16 @@ wgrad_tc_kernel(const DDimsTC d, const WGradTC a) {
 #define WGA_STAGES 2
 #define WGA_MAXT 256
 __host__ __device__ inline int wga_slabs(int dx) { return (dx + TC_H + 1 + 63) >> 6; }
+// first tile of segment s of a (unit, tile) list with tpu tiles per unit and det.n_seg segments of det.seg_tiles per unit
+__device__ __forceinline__ int64_t det_seg_start(const DetTC& det, int64_t tpu, int64_t s) {
+  const int64_t u = s / det.n_seg, k = (s - u * det.n_seg) * det.seg_tiles;
+  return u * tpu + (k < tpu ? k : tpu);
+}
+// DET: group p takes the contiguous segment range [NS p / ngrp, NS (p + 1) / ngrp) of the NS = 2A n_seg segments, and
+// each CTA stores its fragment into det.part [segment][nsl][512 threads][32] at every segment change
+template <bool DET>
 __global__ void __launch_bounds__(FBT_THREADS, 1)
-wgrad_tc_async_kernel(const DDimsTC d, const WGradTC a) {
+wgrad_tc_async_kernel(const DDimsTC d, const WGradTC a, const DetTC det) {
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wq = warp >> 2;
   float* sDone = reinterpret_cast<float*>(tc_smem + WGA_STAGES * WGA_STAGE);
   for (int i = tid; i < a.T; i += FBT_THREADS) sDone[i] = a.done[i];
@@ -2700,16 +2806,23 @@ wgrad_tc_async_kernel(const DDimsTC d, const WGradTC a) {
   const int64_t tpu = (a.M + WGA_ROWS - 1) / WGA_ROWS;
   const int64_t NT = tpu * 2 * d.A;
   const int ngrp = gridDim.x / nsl, pb = blockIdx.x / nsl, sl = blockIdx.x - pb * nsl;
-  const int64_t j0 = NT * pb / ngrp, j1 = NT * (pb + 1) / ngrp;
+  const int64_t NS = DET ? det.n_seg * 2 * d.A : 0;
+  const int64_t j0 = DET ? det_seg_start(det, tpu, NS * pb / ngrp) : NT * pb / ngrp;
+  const int64_t j1 = DET ? det_seg_start(det, tpu, NS * (pb + 1) / ngrp) : NT * (pb + 1) / ngrp;
   // this thread's A piece: 8 columns (chunk cg of [X | Hp | 1 | 0]) of one row
   const int arow = tid >> 3, cg = sl * 8 + (tid & 7);
   float f[32];
   bool first = true;
   int cur_u = -1;
   // the fragment into G: A column sl * 64 + 16 (warp & 3) + lane / 4 (+ 8), gate column 64 wq + 8 i + 2 (lane & 3) (+ 1)
-  auto flush = [&](int u) {
+  auto flush = [&](int u) {      // DET: u is the segment
     wg_wait<0>();
     wg_frag_fence(f);
+    if constexpr (DET) {
+      float4* p = reinterpret_cast<float4*>(det.part + (((int64_t)u * nsl + sl) * FBT_THREADS + tid) * 32);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) p[i] = make_float4(f[4 * i], f[4 * i + 1], f[4 * i + 2], f[4 * i + 3]);
+    } else {
 #pragma unroll
     for (int hh = 0; hh < 2; ++hh) {
       const int ci = sl * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * hh;
@@ -2722,6 +2835,7 @@ wgrad_tc_async_kernel(const DDimsTC d, const WGradTC a) {
 #pragma unroll
         for (int i = 0; i < 8; ++i) { atomicAdd(dst + 8 * i, f[4 * i + 2 * hh]); atomicAdd(dst + 8 * i + 1, f[4 * i + 2 * hh + 1]); }
       }
+    }
     }
   };
 
@@ -2784,7 +2898,7 @@ wgrad_tc_async_kernel(const DDimsTC d, const WGradTC a) {
   if (j0 < j1) { load_tile(); store_tile(0); }
   if (j0 + 1 < j1) load_tile();
   for (int64_t j = j0; j < j1; ++j) {
-    const int u = (int)(j / tpu);
+    const int u = DET ? (int)((j / tpu) * det.n_seg + (j % tpu) / det.seg_tiles) : (int)(j / tpu);
     const int s = (int)((j - j0) & 1);
     if (u != cur_u) {
       if (cur_u >= 0) flush(cur_u);
@@ -2810,6 +2924,63 @@ wgrad_tc_async_kernel(const DDimsTC d, const WGradTC a) {
   if (cur_u >= 0) flush(cur_u);
 }
 
+// Deterministic mode: segment sizes and the reduce of the weight-gradient slabs.
+#define WGA_DET_TILES 256          // wgrad_tc_async_kernel: at most 256 tiles of 64 rows per segment
+#define DXF_DET_TILES 32           // dx_fc_bwd_tc_kernel: at most 32 tiles of 128 rows per segment
+// n_seg = ceil(tpu / max_tiles) segments per unit of (nearly) equal size seg_tiles; every segment holds at least one tile
+static void det_segments(int64_t tpu, int64_t max_tiles, DetTC* det) {
+  const int64_t n = (tpu + max_tiles - 1) / max_tiles;
+  det->seg_tiles = (tpu + n - 1) / n;
+  det->n_seg = (tpu + det->seg_tiles - 1) / det->seg_tiles;
+}
+// G index of entry k of a unit's slab row (-1: none).  KIND 0: wgrad_tc_async_kernel's [nsl][512 threads][32] fragments
+// (its flush mapping); KIND 1: dx_fc_bwd_tc_kernel's [256 threads][g64 | g32 | g16] fragments (dxf_flush's mapping).
+template <int KIND>
+__device__ __forceinline__ int64_t det_target(const DDimsTC& d, int u, int64_t k) {
+  if (KIND == 0) {
+    const int e = (int)(k & 31), tid = (int)((k >> 5) % FBT_THREADS), sl = (int)(k / (32 * FBT_THREADS));
+    const int warp = tid >> 5, lane = tid & 31;
+    const int ci = sl * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * ((e >> 1) & 1);
+    const int col = (warp >> 2) * 64 + 8 * (e >> 2) + 2 * (lane & 3) + (e & 1);
+    if (ci < d.dx) return d.off_wx + ((int64_t)u * d.dx + ci) * TC_N + col;
+    if (ci < d.dx + TC_H) return d.off_wh + ((int64_t)u * TC_H + (ci - d.dx)) * TC_N + col;
+    if (ci == d.dx + TC_H) return d.off_bl + (int64_t)u * TC_N + col;
+    return -1;
+  } else {
+    const int hn = d.dx / 2, h32 = (hn % 64) >= 32, h16 = (hn % 32) >= 16, npt = 32 + 16 * h32 + 8 * h16;
+    const int tid = (int)(k / npt), ep = (int)(k - (int64_t)tid * npt);
+    int e = ep, cb = (tid >> 7) * hn;
+    if (ep >= 32 + 16 * h32) { e = ep - 32 - 16 * h32; cb += 64 + 32 * h32; }
+    else if (ep >= 32) { e = ep - 32; cb += 64; }
+    const int lane = tid & 31, w4 = (tid >> 5) & 3, ag = u >> 1;
+    const int slot = 16 * w4 + (lane >> 2) + 8 * ((e >> 1) & 1);
+    const int c = cb + 8 * (e >> 2) + 2 * (lane & 3) + (e & 1);
+    const int nw = d.n_wave[ag], nt = d.n_wait[ag], nf = d.ff > 0 ? d.n_fp[ag] : 0;
+    int64_t wo, bo; int ld, cc, s0, n;
+    if (c < d.fw) { wo = d.off_fcw_w[u]; bo = d.off_fcw_b[u]; ld = d.fw; cc = c; s0 = 0; n = nw; }
+    else if (c < d.fw + d.ff) { wo = d.off_fcf_w[u]; bo = d.off_fcf_b[u]; ld = d.ff; cc = c - d.fw; s0 = d.kw; n = nf; }
+    else { wo = d.off_fct_w[u]; bo = d.off_fct_b[u]; ld = d.ft; cc = c - d.fw - d.ff; s0 = d.kw + TC_KF; n = nt; }
+    const int kin = slot - s0;
+    if (kin >= 0 && kin < n) return wo + (int64_t)kin * ld + cc;
+    if (slot == d.ones_slot) return bo + cc;
+    return -1;
+  }
+}
+// G[target(u, k)] += the sum of entry k over unit u's segments, in segment order; grid (per / 256, 2A)
+template <int KIND>
+__global__ void __launch_bounds__(256)
+det_reduce_kernel(const DDimsTC d, const DetTC det, float* __restrict__ G, int64_t per) {
+  const int u = blockIdx.y;
+  const int64_t k = (int64_t)blockIdx.x * 256 + threadIdx.x;
+  if (k >= per) return;
+  const int64_t g = det_target<KIND>(d, u, k);
+  if (g < 0) return;
+  const float* p = det.part + (int64_t)u * det.n_seg * per + k;
+  float s = 0.f;
+  for (int64_t i = 0; i < det.n_seg; ++i) s += p[i * per];
+  G[g] += s;
+}
+
 extern "C" int tscl_wgrad_tc(tscl_handle* h, const float* dZ, const void* dz_bf16, const float* X, const void* x_bf16,
                              const float* Hp, const void* h_bf16, const float* h0, const float* done, int32_t T, int64_t rc,
                              int64_t ld_state, int64_t r0, float* grads, int32_t variant, void* stream) {
@@ -2819,12 +2990,14 @@ extern "C" int tscl_wgrad_tc(tscl_handle* h, const float* dZ, const void* dz_bf1
   PCK(cudaSetDevice(tscl_device_of(h)));
   const DDimsTC& d = *tscl_dims_of(h);
   if ((d.dx % 8) != 0 || d.dx / 8 + 9 > WG_A_CHUNKS) return tsc_set_error("tscl_wgrad_tc: dx must be a multiple of 8, <= 240");
+  const int det_ctas = tscl_det_ctas(h);
   const size_t smem = 2 * (size_t)WG_STAGE + 32;
   const size_t smem_async = (size_t)WGA_STAGES * WGA_STAGE + 4 * WGA_MAXT;
   static int attr_dev = -1;
   if (attr_dev != tscl_device_of(h)) {
     PCK(cudaFuncSetAttribute(wgrad_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    PCK(cudaFuncSetAttribute(wgrad_tc_async_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_async));
+    PCK(cudaFuncSetAttribute(wgrad_tc_async_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_async));
+    PCK(cudaFuncSetAttribute(wgrad_tc_async_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_async));
     attr_dev = tscl_device_of(h);
   }
   int n_sm = 0;
@@ -2840,9 +3013,24 @@ extern "C" int tscl_wgrad_tc(tscl_handle* h, const float* dZ, const void* dz_bf1
     const int64_t nt2 = ((M + WGA_ROWS - 1) / WGA_ROWS) * 2 * d.A;
     const int nsl = wga_slabs(d.dx);
     const int g2 = (int)(nt2 < n_sm / nsl ? nt2 : n_sm / nsl) * nsl;      // groups of nsl CTAs, one per A slab
-    wgrad_tc_async_kernel<<<g2, FBT_THREADS, smem_async, (cudaStream_t)stream>>>(d, a);
+    if (det_ctas >= 0) {
+      DetTC det = {};
+      det_segments(nt2 / (2 * d.A), WGA_DET_TILES, &det);
+      const int64_t ns = det.n_seg * 2 * d.A, per = (int64_t)nsl * FBT_THREADS * 32;
+      det.part = tscl_det_slab(h, 1, (size_t)ns * per * sizeof(float), stream);
+      if (!det.part) return tsc_set_error("tscl_wgrad_tc: cudaMalloc of the deterministic slab failed");
+      int cap = det_ctas > 0 && det_ctas < n_sm ? det_ctas : n_sm;
+      cap = cap < nsl ? 1 : cap / nsl;
+      const int g3 = (int)(ns < cap ? ns : cap) * nsl;
+      wgrad_tc_async_kernel<true><<<g3, FBT_THREADS, smem_async, (cudaStream_t)stream>>>(d, a, det);
+      PCK(cudaGetLastError());
+      det_reduce_kernel<0><<<dim3((unsigned)((per + 255) / 256), 2 * d.A), 256, 0, (cudaStream_t)stream>>>(d, det, grads, per);
+    } else {
+      wgrad_tc_async_kernel<false><<<g2, FBT_THREADS, smem_async, (cudaStream_t)stream>>>(d, a, DetTC{});
+    }
   }
   else {
+    if (det_ctas >= 0) return tsc_set_error("tscl_wgrad_tc: only the all-bf16 store form (dz_bf16, x_bf16, h_bf16, T <= 256) has a deterministic form");
     a.acc = acc_tiles(h, stream);
     if (!a.acc) return tsc_set_error("accumulator tiles: cudaMalloc failed");
     wgrad_tc_kernel<<<grid, FBT_THREADS, smem, (cudaStream_t)stream>>>(d, a);
@@ -3036,6 +3224,7 @@ dx_tc_kernel(const DDimsTC d, const DxTC a) {
 }
 
 extern "C" int tscl_dx_tc(tscl_handle* h, const void* dz_bf16, const void* wxt_bf16, void* dx_bf16, int64_t M, void* stream) {
+  if (h && tscl_det_ctas(h) >= 0) return tsc_set_error("tscl_dx_tc: no deterministic form (the handle is in deterministic mode)");
   if (!h || !dz_bf16 || !wxt_bf16 || !dx_bf16 || M <= 0) return tsc_set_error("tscl_dx_tc: bad argument");
   PCK(cudaSetDevice(tscl_device_of(h)));
   const DDimsTC& d = *tscl_dims_of(h);
@@ -3126,10 +3315,12 @@ __device__ __forceinline__ void dxf_flush(const DDimsTC& d, float* G, int u, con
   }
 }
 
-template <int DX>
+// DET: the CTA takes the contiguous segment range [NS b / grid, NS (b + 1) / grid) of the NS = 2A n_seg segments, and
+// the consumers store their fc fragments into det.part [segment][256 threads][g64 | g32 | g16] at every segment change
+template <int DX, bool DET = false>
 __global__ void __launch_bounds__(DXF_THREADS, 1)
 dx_fc_bwd_tc_kernel(const DDimsTC d, const DxFcTC a, const __grid_constant__ CUtensorMap mapZ,
-                    const __grid_constant__ CUtensorMap mapX) {
+                    const __grid_constant__ CUtensorMap mapX, const DetTC det) {
   constexpr int N64 = DX / 64, R32 = (DX % 64) >= 32, R16 = (DX % 32) >= 16;      // dX fragments: the tile's dx columns
   constexpr int HN = DX / 2, H32 = (HN % 64) >= 32, H16 = (HN % 32) >= 16;        // fc fragments: this warpgroup's half
   static_assert(HN >= 64 && HN < 128 && HN % 16 == 0, "fc half width must be 64 + {0, 16, 32, 48}");
@@ -3150,8 +3341,9 @@ dx_fc_bwd_tc_kernel(const DDimsTC d, const DxFcTC a, const __grid_constant__ CUt
   // the CTA's contiguous range [j0, j1) of the (unit, tile) list, formed in each role after its setmaxnreg
 #define DXF_RANGE                                                                                   \
   const int64_t tpu = (a.M + 127) / 128;                                                            \
-  const int64_t NT = tpu * 2 * d.A;                                                                 \
-  const int64_t j0 = NT * blockIdx.x / gridDim.x, j1 = NT * (blockIdx.x + 1) / gridDim.x;
+  const int64_t NT = tpu * 2 * d.A, NS = DET ? det.n_seg * 2 * d.A : 0;                             \
+  const int64_t j0 = DET ? det_seg_start(det, tpu, NS * blockIdx.x / gridDim.x) : NT * blockIdx.x / gridDim.x; \
+  const int64_t j1 = DET ? det_seg_start(det, tpu, NS * (blockIdx.x + 1) / gridDim.x) : NT * (blockIdx.x + 1) / gridDim.x;
 
   if (warp >= 8) {
     asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(DXF_PROD_REGS(DX)));
@@ -3275,12 +3467,34 @@ dx_fc_bwd_tc_kernel(const DDimsTC d, const DxFcTC a, const __grid_constant__ CUt
       if constexpr (H32) dxf_flush(d, a.G, u, g32, n0 + 64);
       if constexpr (H16) dxf_flush(d, a.G, u, g16, n0 + 64 + 32 * H32);
     };
+    // DET: the fragments of segment sg into its slab row
+    constexpr int NPT = 32 + 16 * H32 + 8 * H16;
+    auto store = [&](int64_t sg) {
+      float4* p = reinterpret_cast<float4*>(det.part + (sg * 256 + tid) * NPT);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) p[i] = make_float4(g64[4 * i], g64[4 * i + 1], g64[4 * i + 2], g64[4 * i + 3]);
+      if constexpr (H32)
+#pragma unroll
+        for (int i = 0; i < 4; ++i) p[8 + i] = make_float4(g32[4 * i], g32[4 * i + 1], g32[4 * i + 2], g32[4 * i + 3]);
+      if constexpr (H16)
+#pragma unroll
+        for (int i = 0; i < 2; ++i) p[8 + 4 * H32 + i] = make_float4(g16[4 * i], g16[4 * i + 1], g16[4 * i + 2], g16[4 * i + 3]);
+    };
+    int64_t cur_sg = -1;
     for (int64_t j = j0; j < j1; ++j) {
       const int u = (int)(j / tpu);
       const uint32_t ph = (uint32_t)((j - j0) & 1);
+      if constexpr (DET) {
+        const int64_t sg = (int64_t)u * det.n_seg + (j - (int64_t)u * tpu) / det.seg_tiles;
+        if (sg != cur_sg) {
+          if (cur_sg >= 0) store(cur_sg);
+          cur_sg = sg; first = true;
+        }
+      }
       if (u != cur_u) {
-        if (cur_u >= 0) flush(cur_u);
-        cur_u = u; first = true;
+        if (!DET && cur_u >= 0) flush(cur_u);
+        cur_u = u;
+        if (!DET) first = true;
         asm volatile("bar.sync 1, 256;" ::: "memory");      // both warpgroups' MMAs of the previous unit have completed
         if (tid == 0) {
           const uint32_t bytes = (uint32_t)BW_KC * DX * 16;
@@ -3373,7 +3587,8 @@ dx_fc_bwd_tc_kernel(const DDimsTC d, const DxFcTC a, const __grid_constant__ CUt
       if (lane == 0) mbar_arrive(bar_free);      // this warp is done reading dXm and In
       first = false;
     }
-    if (cur_u >= 0) flush(cur_u);
+    if constexpr (DET) { if (cur_sg >= 0) store(cur_sg); }
+    else if (cur_u >= 0) flush(cur_u);
   }
 #undef DXF_RANGE
 }
@@ -3392,9 +3607,13 @@ extern "C" int tscl_dx_fc_bwd_tc(tscl_handle* h, const float* obs, const void* x
   if (!make_tmap_3d(&mZ, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, dz_bf16, 2 * d.A, M, TC_N, 64, 128) ||
       !make_tmap_3d(&mX, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, x_bf16, 2 * d.A, M, d.dx, 8, 128, CU_TENSOR_MAP_SWIZZLE_NONE))
     return tsc_set_error("tscl_dx_fc_bwd_tc: cannot build the tensor maps (dz_bf16 / x_bf16 must be 16-byte aligned)");
-  void (*kern)(const DDimsTC, const DxFcTC, const CUtensorMap, const CUtensorMap) =
-      d.dx == 224 ? dx_fc_bwd_tc_kernel<224> : d.dx == 192 ? dx_fc_bwd_tc_kernel<192> :
-      d.dx == 160 ? dx_fc_bwd_tc_kernel<160> : dx_fc_bwd_tc_kernel<128>;
+  const int det_ctas = tscl_det_ctas(h);
+  void (*kern)(const DDimsTC, const DxFcTC, const CUtensorMap, const CUtensorMap, const DetTC) =
+      det_ctas >= 0 ?
+      (d.dx == 224 ? dx_fc_bwd_tc_kernel<224, true> : d.dx == 192 ? dx_fc_bwd_tc_kernel<192, true> :
+       d.dx == 160 ? dx_fc_bwd_tc_kernel<160, true> : dx_fc_bwd_tc_kernel<128, true>) :
+      (d.dx == 224 ? dx_fc_bwd_tc_kernel<224, false> : d.dx == 192 ? dx_fc_bwd_tc_kernel<192, false> :
+       d.dx == 160 ? dx_fc_bwd_tc_kernel<160, false> : dx_fc_bwd_tc_kernel<128, false>);
   const size_t smem = dxf_smem(d.dx);
   static int attr_dev = -1;
   if (attr_dev != tscl_device_of(h)) {
@@ -3402,15 +3621,32 @@ extern "C" int tscl_dx_fc_bwd_tc(tscl_handle* h, const float* obs, const void* x
     PCK(cudaFuncSetAttribute(dx_fc_bwd_tc_kernel<192>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dxf_smem(192)));
     PCK(cudaFuncSetAttribute(dx_fc_bwd_tc_kernel<160>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dxf_smem(160)));
     PCK(cudaFuncSetAttribute(dx_fc_bwd_tc_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dxf_smem(128)));
+    PCK(cudaFuncSetAttribute(dx_fc_bwd_tc_kernel<224, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dxf_smem(224)));
+    PCK(cudaFuncSetAttribute(dx_fc_bwd_tc_kernel<192, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dxf_smem(192)));
+    PCK(cudaFuncSetAttribute(dx_fc_bwd_tc_kernel<160, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dxf_smem(160)));
+    PCK(cudaFuncSetAttribute(dx_fc_bwd_tc_kernel<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dxf_smem(128)));
     attr_dev = tscl_device_of(h);
   }
   int n_sm = 0;
   PCK(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, tscl_device_of(h)));
   const int64_t NT = ((M + 127) / 128) * 2 * d.A;
-  const int grid = (int)(NT < n_sm ? NT : n_sm);
   DxFcTC a;
   a.obs = obs; a.Wxt = (const __nv_bfloat16*)wxt_bf16; a.G = grads; a.M = M; a.rows_per_t = rows_per_t; a.stride_t = stride_t;
-  kern<<<grid, DXF_THREADS, smem, (cudaStream_t)stream>>>(d, a, mZ, mX);
+  if (det_ctas >= 0) {
+    DetTC det = {};
+    det_segments((M + 127) / 128, DXF_DET_TILES, &det);
+    const int hn = d.dx / 2;
+    const int64_t ns = det.n_seg * 2 * d.A, per = (int64_t)256 * (32 + 16 * ((hn % 64) >= 32) + 8 * ((hn % 32) >= 16));
+    det.part = tscl_det_slab(h, 2, (size_t)ns * per * sizeof(float), stream);
+    if (!det.part) return tsc_set_error("tscl_dx_fc_bwd_tc: cudaMalloc of the deterministic slab failed");
+    const int cap = det_ctas > 0 && det_ctas < n_sm ? det_ctas : n_sm;
+    kern<<<(int)(ns < cap ? ns : cap), DXF_THREADS, smem, (cudaStream_t)stream>>>(d, a, mZ, mX, det);
+    PCK(cudaGetLastError());
+    det_reduce_kernel<1><<<dim3((unsigned)((per + 255) / 256), 2 * d.A), 256, 0, (cudaStream_t)stream>>>(d, det, grads, per);
+  } else {
+    const int grid = (int)(NT < n_sm ? NT : n_sm);
+    kern<<<grid, DXF_THREADS, smem, (cudaStream_t)stream>>>(d, a, mZ, mX, DetTC{});
+  }
   PCK(cudaGetLastError());
   return 0;
 }

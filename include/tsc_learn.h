@@ -221,6 +221,19 @@ int tscl_debug_bptt_prof(void* counters_dev);
 int tscl_clip_rmsprop(tscl_handle* h, float* params, float* grads, float* ms, const uint8_t* agent_of,
                       float max_norm, float lr, float alpha, float eps, float* norms, void* stream);
 
+/* Deterministic mode of the lean A2C update (on != 0): later calls of tscl_lstm_seq_bwd_tc_heads, tscl_wgrad_tc (the
+ * all-bf16 store form), tscl_dx_fc_bwd_tc and tscl_clip_rmsprop on this handle add their gradients, loss sums and clip
+ * norms in a fixed order instead of with atomics, so that equal inputs give equal bits from run to run and on any
+ * H100.  Each kernel stores its accumulator fragments into a partial slab row per work item (BPTT: chunk, unit,
+ * 128-row tile) or per segment of a unit's tiles (weight gradients: at most 256 / 32 tiles, sized from the shapes), and
+ * a reduce kernel adds the rows into grads in item order; the clip norm is summed per 8192-element block, then over
+ * blocks in order.  The sums therefore depend on the shapes only, not on the grid: n_ctas = 0 keeps each kernel's
+ * device-sized grid, n_ctas > 0 caps it (the same bits).  The slabs are owned by the handle, allocated on first use.
+ * While the mode is on, the update entry points without a deterministic form (tscl_heads_loss,
+ * tscl_lstm_seq_bwd_tc[_dx], tscl_fc_bwd_tc, tscl_dx_tc, the other tscl_wgrad_tc forms, tscl_lstm_seq_bwd, tscl_fc_bwd,
+ * tscl_fc_hidden_bwd) return an error naming themselves.  on = 0 restores the atomic kernels. */
+int tscl_set_deterministic(tscl_handle* h, int32_t on, int32_t n_ctas);
+
 /* ---- fused tensor-core policy forward (wgmma), csrc/tsc_policy_tc.cu -------------------------
  * tscl_pack_weights: per unit, [Wx;Wh] -> bf16 UMMA operand image [(dx+h)/8][4h][8] followed by the
  *   block-diagonal fc image [8][dx][8]; wpack holds 2A such records (call after every optimizer step).

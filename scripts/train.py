@@ -3,7 +3,7 @@ device-resident learners (deeprl_signal_control_b200/agents/train.py).
 
   python scripts/train.py --base-dir DIR train --config-dir CFG.ini
                           [--test-mode no_test|in_train_test|after_train_test|all_test] [--replicas N] [--policy lstm|fc]
-                          [--summaries] [--seeds 12,13,14,15 | --sweep a.ini,b.ini,...]
+                          [--summaries] [--deterministic] [--seeds 12,13,14,15 | --sweep a.ini,b.ini,...]
   torchrun --nproc-per-node W scripts/train.py --base-dir DIR train --config-dir CFG.ini --replicas N
                           [--backend nccl|gloo] ...
 
@@ -32,6 +32,10 @@ replicas (a multiple of 64), all in one lock-step.  The configs may differ only 
 and the [MODEL_CONFIG] learning-rate, entropy, value / gradient-norm, RMSProp, gamma and reward-scaling keys
 (agents/train.py: SWEEP_CONFIG_KEYS).  Member a.ini gets the complete agent directory DIR/a/<agent>/ of
 `train --config-dir a.ini`.  Not with --seeds, and not under torchrun.  The JSON line gains "members".
+
+`--deterministic` makes the A2C update add its gradients in a fixed order instead of with atomics, so two runs with the
+same config, seeds, replicas, world size, build and GPU model write the same bytes (checkpoint, CSVs, summaries).  It
+combines with every option above; the LSTM policy only, and a no-op for IQL (its update is already reproducible).
 """
 import argparse
 import datetime
@@ -64,6 +68,8 @@ def parse_args(argv=None):
                     help="comma-separated seeds: train one population member per seed into DIR/seed<s>/<agent>/")
     sp.add_argument("--sweep", default=None,
                     help="comma-separated configs: train one sweep member per config into DIR/<config stem>/<agent>/")
+    sp.add_argument("--deterministic", action="store_true",
+                    help="reproducible A2C training: fixed-order gradient sums in the update")
     a = p.parse_args(argv)
     if not a.option:
         p.print_help()
@@ -91,7 +97,7 @@ def main(argv=None):
             raise SystemExit("--sweep trains a sweep in one process; it does not run under torchrun")
         from deeprl_signal_control_b200.agents.train import train_sweep
         out = train_sweep(a.sweep, a.base_dir, a.test_mode, n_replicas=a.replicas, summaries=a.summaries,
-                          policy=a.policy)
+                          policy=a.policy, deterministic=a.deterministic)
         print(json.dumps({"final_step": out.final_step, "episode_sets": out.episode_sets, "members": out.names,
                           "env_samples": out.env_samples, "replicas": a.replicas, "wall_sec": round(out.wall_sec, 3)}))
         return out
@@ -100,14 +106,14 @@ def main(argv=None):
             raise SystemExit("--seeds trains a population in one process; it does not run under torchrun")
         from deeprl_signal_control_b200.agents.train import train
         out = train(a.config_dir, a.base_dir, a.test_mode, n_replicas=a.replicas, policy=a.policy,
-                    summaries=a.summaries, seeds=a.seeds)
+                    summaries=a.summaries, seeds=a.seeds, deterministic=a.deterministic)
         print(json.dumps({"final_step": out.final_step, "episode_sets": out.episode_sets, "seeds": out.seeds,
                           "env_samples": out.env_samples, "replicas": a.replicas, "wall_sec": round(out.wall_sec, 3)}))
         return out
     if world <= 1:
         from deeprl_signal_control_b200.agents.train import train
         out = train(a.config_dir, a.base_dir, a.test_mode, n_replicas=a.replicas, policy=a.policy,
-                    summaries=a.summaries)
+                    summaries=a.summaries, deterministic=a.deterministic)
         print(json.dumps({"final_step": out.final_step, "episode_sets": out.episode_sets,
                           "env_samples": out.env_samples, "replicas": a.replicas, "wall_sec": round(out.wall_sec, 3)}))
         return out
@@ -122,7 +128,7 @@ def main(argv=None):
     try:
         from deeprl_signal_control_b200.agents.train import train
         out = train(a.config_dir, a.base_dir, a.test_mode, n_replicas=a.replicas, policy=a.policy, device=local_rank,
-                    process_group=dist.group.WORLD, summaries=a.summaries)
+                    process_group=dist.group.WORLD, summaries=a.summaries, deterministic=a.deterministic)
     finally:
         dist.destroy_process_group()
     if out.rank == 0:
