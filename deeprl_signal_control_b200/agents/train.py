@@ -4,6 +4,8 @@
     train(config, base_dir, test_mode='no_test', n_replicas=1, policy='lstm', device=0, process_group=None,
           summaries=False)
     train_sweep([a.ini, b.ini, ...], base_dir, ...)   (one member per config in one process, `train_sweep`)
+    train_iql_population(config, base_dir, seeds, ...) / train_iql_sweep([a.ini, ...], base_dir, ...)   (the same for
+                                                        iqll / iqld)
 
 leaves the reference's agent directory: `data/` with a copy of the config and `train_reward.csv`, `model/checkpoint-<step>`
 and `log/<time>.log`; with `after_train_test` / `all_test` also `data/<scenario>_<agent>_{control,traffic,trip}.csv`;
@@ -293,7 +295,8 @@ def build_model(agent, env, model_config, total_step, n_replicas, policy='lstm',
     learner all-reduces its gradient over `process_group` when one is given.  `seeds`: an A2C population, one member
     per seed on n_replicas replicas each (`BatchedA2C`); with `member_configs` (one [MODEL_CONFIG] per seed) a sweep.
     `deterministic`: the A2C update adds in a fixed order (`BatchedA2C(deterministic=True)`); IQL's TD kernel already
-    reduces in a fixed order, so for iqll / iqld it changes nothing."""
+    reduces in a fixed order, so for iqll / iqld it changes nothing.  For iqll / iqld, `seeds` and `member_configs`
+    give a `BatchedIQL` with members (each with learner seed 0, as the solo run)."""
     kind, model_type = model_spec(agent)
     t = env._tables
     if kind != 'iql':
@@ -318,7 +321,7 @@ def build_model(agent, env, model_config, total_step, n_replicas, policy='lstm',
     lay = QLayout(model_type, [int(off[i + 1] - off[i]) for i in range(t.n_nodes)], t.n_a_ls, t.n_w_ls, off, t.n_obs,
                   n_fc=n_fc, n_ft=n_fc // 4, n_h=n_h, max_na=t.max_na)          # q_fct width: agents/policies.py:383
     return BatchedIQL(lay, n_replicas, model_config, model_type, seed=0, device=device, replica0=replica0,
-                      total_replicas=total_replicas, pg=process_group)
+                      total_replicas=total_replicas, pg=process_group, seeds=seeds, member_configs=member_configs)
 
 
 def parse_seeds(text):
@@ -538,6 +541,24 @@ def _member_filter(k):
     return lambda rec: getattr(rec, 'member', k) == k
 
 
+def _member_logs(dirs):
+    """One log file per member directory (`_member_filter`) and stderr, added to the root logger and returned."""
+    handlers = []
+    fmt = logging.Formatter('%(asctime)s [%(levelname)s] %(message)s')
+    for k, d in enumerate(dirs):
+        h = logging.FileHandler(os.path.join(d['log'], '%d.log' % time.time()))
+        h.setFormatter(fmt)
+        h.addFilter(_member_filter(k))
+        handlers.append(h)
+    handlers.append(logging.StreamHandler())
+    handlers[-1].setFormatter(fmt)
+    root = logging.getLogger()
+    for h in handlers:
+        root.addHandler(h)
+    root.setLevel(logging.INFO)
+    return handlers
+
+
 def train_population(config, base_dir, seeds, test_mode='no_test', n_replicas=1, policy='lstm', device=0,
                      summaries=False, deterministic=False):
     """Train K = len(seeds) members of one A2C agent (ia2c / ma2c, LSTM policy) in one process, member k with
@@ -563,7 +584,8 @@ def train_population(config, base_dir, seeds, test_mode='no_test', n_replicas=1,
     agent = config['ENV_CONFIG'].get('agent')
     kind, _ = model_spec(agent)
     if kind == 'iql':
-        raise ValueError("a population trains an A2C agent (ia2c or ma2c), not %r" % agent)
+        raise ValueError("a population trains an A2C agent (ia2c or ma2c), not %r; train_iql_population trains IQL "
+                         "members" % agent)
     if policy != 'lstm':
         raise ValueError("a population trains the LSTM policy only (got policy=%r)" % policy)
     check_population(seeds, 0, n_replicas, 1024, None)               # before any directory or device work
@@ -592,19 +614,7 @@ def _train_members(cfgs, dirs, agent, seeds, R_m, in_test, post_test, policy, de
     from .evaluator import Evaluator
     from .trainer import BatchedTrainer
     K = len(cfgs)
-    handlers = []
-    fmt = logging.Formatter('%(asctime)s [%(levelname)s] %(message)s')
-    for k, d in enumerate(dirs):
-        h = logging.FileHandler(os.path.join(d['log'], '%d.log' % time.time()))
-        h.setFormatter(fmt)
-        h.addFilter(_member_filter(k))
-        handlers.append(h)
-    handlers.append(logging.StreamHandler())
-    handlers[-1].setFormatter(fmt)
-    root = logging.getLogger()
-    for h in handlers:
-        root.addHandler(h)
-    root.setLevel(logging.INFO)
+    root, handlers = logging.getLogger(), _member_logs(dirs)
     writers = []
     cg = [c['ENV_CONFIG'].getfloat('coop_gamma') for c in cfgs] if sweep and agent == 'ma2c' else None
     if cg is not None and len(set(cg)) == 1:
@@ -668,6 +678,11 @@ SWEEP_CONFIG_KEYS = {
     'MODEL_CONFIG': ('lr_init', 'lr_decay', 'lr_min', 'entropy_coef_init', 'entropy_decay', 'entropy_coef_min',
                      'entropy_ratio', 'value_coef', 'max_grad_norm', 'rmsp_alpha', 'rmsp_epsilon', 'gamma',
                      'reward_norm', 'reward_clip')}
+# the same for an IQL sweep (`train_iql_sweep`): IQL reads no coop_gamma, and its ring and networks are shared
+IQL_SWEEP_CONFIG_KEYS = {
+    'ENV_CONFIG': ('seed',),
+    'MODEL_CONFIG': ('lr_init', 'lr_decay', 'lr_min', 'epsilon_init', 'epsilon_min', 'epsilon_decay', 'epsilon_ratio',
+                     'gamma', 'max_grad_norm', 'reward_norm', 'reward_clip')}
 
 
 def _same(a, b):
@@ -684,11 +699,13 @@ def _value(cfg, sec, key):
     return cfg.get(sec, key, fallback=None) if cfg.has_section(sec) else None
 
 
-def sweep_members(configs):
+def sweep_members(configs, keys=None):
     """The members of a sweep as [(name, ConfigParser, path or None)], checked.  `configs`: a list of config paths
     (member name = file stem) or a dict name -> ConfigParser.  Refused with a ValueError: no config, repeated names, a
-    key outside SWEEP_CONFIG_KEYS that differs between two members (naming the key and both members), a coop_gamma that
-    differs under ia2c (the reference reads it only for ma2c, envs/env.py:184-188, 595-609), and two identical configs."""
+    key outside `keys` (default SWEEP_CONFIG_KEYS) that differs between two members (naming the key and both members), a
+    coop_gamma that differs under ia2c (the reference reads it only for ma2c, envs/env.py:184-188, 595-609), and two
+    identical configs."""
+    allowed = SWEEP_CONFIG_KEYS if keys is None else keys
     if isinstance(configs, dict):
         items = [(str(n), c, None) for n, c in configs.items()]
     else:
@@ -714,15 +731,15 @@ def sweep_members(configs):
                 a, b = _value(c0, sec, key), _value(c, sec, key)
                 if _same(a, b):
                     continue
-                if key not in SWEEP_CONFIG_KEYS.get(sec, ()):
+                if key not in allowed.get(sec, ()):
                     raise ValueError('[%s] %s differs between %s (%s) and %s (%s): the members of a sweep may differ '
-                                     'only in %s' % (sec, key, label(0), a, label(i), b, SWEEP_CONFIG_KEYS))
+                                     'only in %s' % (sec, key, label(0), a, label(i), b, allowed))
                 if key == 'coop_gamma' and agent != 'ma2c':
                     raise ValueError('[ENV_CONFIG] coop_gamma differs between %s and %s, but %s does not use it (only '
                                      'ma2c does)' % (label(0), label(i), agent))
         for j in range(i):
             if all(_same(_value(items[j][1], sec, key), _value(c, sec, key))
-                   for sec, keys in SWEEP_CONFIG_KEYS.items() for key in keys):
+                   for sec, ks in allowed.items() for key in ks):
                 raise ValueError('%s and %s are identical: a sweep trains each config once' % (label(j), label(i)))
     return items
 
@@ -752,7 +769,7 @@ def train_sweep(configs, base_dir, test_mode='no_test', n_replicas=64, device=0,
     agent = items[0][1]['ENV_CONFIG'].get('agent')
     kind, _ = model_spec(agent)
     if kind == 'iql':
-        raise ValueError("a sweep trains an A2C agent (ia2c or ma2c), not %r" % agent)
+        raise ValueError("a sweep trains an A2C agent (ia2c or ma2c), not %r; train_iql_sweep trains IQL members" % agent)
     if policy != 'lstm':
         raise ValueError("a sweep trains the LSTM policy only (got policy=%r)" % policy)
     cfgs = [c for _, c, _ in items]
@@ -772,3 +789,154 @@ def train_sweep(configs, base_dir, test_mode='no_test', n_replicas=64, device=0,
     out.names, out.dirs = names, [sweep_dir(base_dir, n, agent) for n in names]
     out.wall_sec = time.time() - t0
     return out
+
+
+def _read_config(config):
+    """(ConfigParser, name of its copy in data/) of a config path or a parsed ConfigParser."""
+    if isinstance(config, configparser.ConfigParser):
+        return config, 'config.ini'
+    c = configparser.ConfigParser()
+    if not c.read(config):
+        raise FileNotFoundError(config)
+    return c, os.path.basename(config)
+
+
+def _iql_agent(config, what):
+    agent = config['ENV_CONFIG'].get('agent')
+    if model_spec(agent)[0] != 'iql':
+        raise ValueError("%s trains an IQL agent (iqll or iqld), not %r; train(seeds=) and train_sweep train A2C "
+                         "members" % (what, agent))
+    return agent
+
+
+def train_iql_population(config, base_dir, seeds, test_mode='no_test', n_replicas=1, device=0, summaries=False):
+    """Train K = len(seeds) members of one IQL agent (iqll / iqld) in one process, member k with `[ENV_CONFIG] seed =
+    seeds[k]` on `n_replicas` replicas.  One simulator launch, one grouped ε-greedy forward per control step and one
+    grouped TD / Adam update per round cover all K * n_replicas replicas (`BatchedIQL` with seeds); the schedules, the
+    tests and every file are per member.  Member k's directory `member_dir(base_dir, seeds[k], agent)` is, bit for bit,
+    what `train(config with seed seeds[k], n_replicas=n_replicas)` leaves (the log's times aside).  Everything is
+    checked before any directory is made.  Returns a namespace like train_population's."""
+    import copy
+    t0 = time.time()
+    in_test, post_test = init_test_flag(test_mode)
+    seeds = parse_seeds(seeds if isinstance(seeds, str) else ','.join(str(int(x)) for x in seeds))
+    config, name = _read_config(config)
+    agent = _iql_agent(config, 'train_iql_population')
+    cfgs = []
+    for s in seeds:
+        cfg = copy.deepcopy(config)
+        cfg['ENV_CONFIG']['seed'] = str(s)
+        cfgs.append(cfg)
+    paths = [member_dir(base_dir, s, agent) for s in seeds]
+
+    def write(k, d):
+        with open(os.path.join(d['data'], name), 'w') as f:
+            cfgs[k].write(f)
+    out = _train_iql_members(cfgs, paths, write, agent, seeds, int(n_replicas), in_test, post_test, device, summaries,
+                             'population of %d seeds %s' % (len(seeds), seeds), sweep=False)
+    out.dirs, out.wall_sec = paths, time.time() - t0
+    return out
+
+
+def train_iql_sweep(configs, base_dir, test_mode='no_test', n_replicas=1, device=0, summaries=False):
+    """Train a hyperparameter sweep of one IQL agent (iqll / iqld) in one process: one member per config
+    (`sweep_members` with IQL_SWEEP_CONFIG_KEYS: the seed, the lr and ε schedules, gamma, max_grad_norm and the reward
+    scaling), each on `n_replicas` replicas, sharing the simulator, the replay ring and the grouped kernels.  Member k's
+    directory `sweep_dir(base_dir, name_k, agent)` is what `train(config_k, n_replicas=n_replicas)` leaves.  Everything
+    is checked before any directory is made.  Returns a namespace like train_sweep's."""
+    t0 = time.time()
+    in_test, post_test = init_test_flag(test_mode)
+    items = sweep_members(configs, IQL_SWEEP_CONFIG_KEYS)
+    agent = _iql_agent(items[0][1], 'train_iql_sweep')
+    cfgs = [c for _, c, _ in items]
+    seeds = [c['ENV_CONFIG'].getint('seed') for c in cfgs]
+    names = [n for n, _, _ in items]
+    paths = [sweep_dir(base_dir, n, agent) for n in names]
+
+    def write(k, d):
+        if items[k][2] is not None:
+            shutil.copy(items[k][2], d['data'])                       # as train() copies its config
+        else:
+            with open(os.path.join(d['data'], 'config.ini'), 'w') as f:
+                cfgs[k].write(f)
+    out = _train_iql_members(cfgs, paths, write, agent, seeds, int(n_replicas), in_test, post_test, device, summaries,
+                             'sweep of %d configs %s' % (len(cfgs), names), sweep=True)
+    out.names, out.dirs, out.wall_sec = names, paths, time.time() - t0
+    return out
+
+
+def member_schedulers(model_configs, total_step):
+    """(lr, ε) schedulers of IQL members, one `iql_schedulers` pair per member's [MODEL_CONFIG] (a population's are
+    equal): two lists, or one pair for one member.  The trainer calls each as the member's solo run calls its own."""
+    from .models import iql_schedulers
+    pairs = [iql_schedulers(c, total_step) for c in model_configs]
+    if len(pairs) == 1:
+        return pairs[0]
+    return [p[0] for p in pairs], [p[1] for p in pairs]
+
+
+def _train_iql_members(cfgs, paths, write_config, agent, seeds, R_m, in_test, post_test, device, summaries, what,
+                       sweep):
+    """The training run of IQL members: member k from cfgs[k] into the agent directory paths[k].  The environment and
+    the learner (which refuses what it cannot train) are built before any directory is made; then the directories, their
+    configs (write_config(k, dirs)), member-tagged log files, one simulator and one learner for all K * R_m replicas, and
+    one driver per member."""
+    import torch
+    from ..envs import make_env
+    from .evaluator import Evaluator
+    from .learner_iql import N_ROUNDS, BatchedIQLTrainer
+    K = len(cfgs)
+    mc = cfgs[0]['MODEL_CONFIG']
+    data0 = os.path.join(paths[0], 'data') + os.sep
+    env = make_env(cfgs[0]['ENV_CONFIG'], K * R_m, data0, is_record=False, device=device)
+    total_step, counter, T = _schedule(cfgs[0], env)
+    model = build_model(agent, env, mc, total_step, R_m, seeds=seeds, device=device,
+                        member_configs=[c['MODEL_CONFIG'] for c in cfgs] if sweep else None)
+    dirs = [init_dir(p) for p in paths]
+    for k, d in enumerate(dirs):
+        write_config(k, d)
+    root, handlers = logging.getLogger(), _member_logs(dirs)
+    writers = []
+    try:
+        logging.info('Training: s dim: %d, s dim ls: %r, a dim ls: %r, %s x %d replicas'
+                     % (env.n_s, env.n_s_ls, env.n_a_ls, what, R_m))
+        members = [model.member(k) for k in range(K)]
+        sim = env._ensure_sim()
+        trace = torch.zeros(T, K * R_m, dtype=torch.float32, device=sim.device)
+        srec, summ = {}, None
+        if summaries:
+            from .summary import SummaryWriter, summary_name
+            shape = (-(-T // model.n_step),) + ((K,) if K > 1 else ()) + (N_ROUNDS, model.n_agent, 4)
+            srec = dict(summary_rec=torch.zeros(shape, dtype=torch.float32, device=sim.device))
+            writers = [SummaryWriter(d['log']) for d in dirs]
+            summ = [Summaries(w, summary_name(agent, 'lstm', model.model_type), 'iql', model.n_step) for w in writers]
+        lr_s, eps_s = member_schedulers([c['MODEL_CONFIG'] for c in cfgs], total_step)
+        trainer = BatchedIQLTrainer(sim, model, lr_s, eps_s, seed0=seeds[0], greward_trace=trace, **srec)
+        drivers = []
+        for k in range(K):                  # one driver per member, over its view of the shared trainer
+            evaluator = None
+            if in_test or post_test:
+                test_env = make_env(cfgs[k]['ENV_CONFIG'], len(env.test_seeds), dirs[k]['data'], is_record=False,
+                                    device=device)
+                evaluator = Evaluator(test_env, members[k], dirs[k]['data'], policy_type='default')
+            drivers.append(Trainer(trainer.member(k), evaluator, counter, agent, in_test, dirs[k]['data'],
+                                   summary=summ[k] if summ else None, log_extra={'member': k}))
+        run_schedule(drivers)
+        post = [None] * K
+        for k, d in enumerate(drivers):
+            logging.info('Training: save final model at step %d ...' % counter.cur_step, extra=d.log_extra)
+            members[k].save(dirs[k]['model'], counter.cur_step)
+            if post_test:
+                post[k] = d.run_offline()
+        torch.cuda.synchronize(sim.device)
+    finally:
+        for w in writers:
+            w.close()
+        for h in handlers:
+            root.removeHandler(h)
+            h.close()
+    return types.SimpleNamespace(final_step=counter.cur_step, episode_sets=drivers[0].n_episode_sets,
+                                 env_samples=counter.cur_step * K * R_m, world=1, rank=0, seeds=seeds,
+                                 data=[d.data for d in drivers], post_test=post, model=model, members=members,
+                                 trainer=trainer)
+

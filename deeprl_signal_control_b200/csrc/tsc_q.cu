@@ -47,6 +47,20 @@ struct QDims {
   int q_in;      // rows of the resident q weight: n_h (dqn) or s_max (lr)
 };
 
+#define QG_MAX 64                // members of one grouped launch (their per-member scalars travel by value)
+
+// Per-member scalars of a grouped launch (ε, γ, lr_t, max_grad_norm, reward scaling), copied from a host array into the
+// kernel's parameters: no upload and no host sync per call.
+struct QMemberF {
+  float v[QG_MAX];
+};
+
+static QMemberF q_member_f(const float* host, int K) {
+  QMemberF o{};
+  for (int k = 0; k < K; ++k) o.v[k] = host[k];
+  return o;
+}
+
 struct tscl_qhandle {
   int device = 0;
   QDims d{};
@@ -58,6 +72,8 @@ struct tscl_qhandle {
   int td_ctas_per_sm = 1;
   const int64_t* blk = nullptr;  // [A + 1] first float of every agent's block in the flat vector, then n_params
   float* part = nullptr;         // TD partials [groups][n_params + 3 A]
+  float* part_g = nullptr;       // grouped TD partials [K][groups][n_params + 3 A] (tscl_q_td_g)
+  int part_g_k = 0;              // members part_g holds
 };
 
 struct QSmem {          // float offsets of the shared-memory regions
@@ -338,11 +354,15 @@ q_fwd_kernel(const QDims d, const float* __restrict__ P, const float* __restrict
 // p_stride) resident.  Per row the statements of q_fwd_kernel's evaluation path (the network through q_tile_forward at
 // q_fc_0's own pitch, the same chain of fp32 operations), keyed with seeds[k] and the member-local replica index, and
 // a failed sample reported into bad[k]: member k's outputs are those of its own tscl_q_step launch.
-template <bool DQN>
+// EXPLORE (tscl_q_explore_g): q_fwd_kernel's explore path per member, with ε eps.v[k] and the draws keyed by `seed`
+// and the member-local replica; the ring slot's rows ring_s / ring_a are the lock-step's (row0 + r): member k's outputs
+// are those of its own tscl_q_explore launch with replica0 = 0.
+template <bool DQN, bool EXPLORE = false>
 __global__ void __launch_bounds__(256)
 q_fwd_g_kernel(const QDims d, const float* __restrict__ P0, int64_t p_stride, const float* __restrict__ obs,
                const int64_t* __restrict__ rows, float* __restrict__ q, int32_t* __restrict__ act, int mode,
-               const uint64_t* __restrict__ seeds, uint32_t step, unsigned long long* __restrict__ bad) {
+               const uint64_t* __restrict__ seeds, uint32_t step, unsigned long long* __restrict__ bad,
+               const QMemberF eps, uint64_t seed, float* __restrict__ ring_s, int8_t* __restrict__ ring_a) {
   extern __shared__ __align__(16) float qsm[];
   const int k = blockIdx.z;
   const int64_t row0 = rows[k], S = rows[k + 1] - row0;
@@ -370,7 +390,7 @@ q_fwd_g_kernel(const QDims d, const float* __restrict__ P0, int64_t p_stride, co
     sWq[i] = j < n_a ? P[d.off_q_w[a] + (int64_t)kk * n_a + j] : 0.f;
   }
   for (int i = tid; i < QT_NA; i += 256) sBq[i] = i < n_a ? P[d.off_q_b[a] + i] : 0.f;
-  const uint64_t sk = seeds[k];
+  const uint64_t sk = EXPLORE ? seed : seeds[k];
   const uint32_t seed_lo = (uint32_t)(sk & 0xFFFFFFFFu), seed_hi = (uint32_t)(sk >> 32);
 
   for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
@@ -380,6 +400,10 @@ q_fwd_g_kernel(const QDims d, const float* __restrict__ P0, int64_t p_stride, co
       const int row = i / n_s, kk = i - row * n_s;
       const int64_t m = m0 + row;
       sS[kk * QT_LD + row] = m < S ? __ldg(obs + (row0 + m) * d.n_obs + ooff + kk) : 0.f;
+    }
+    if (EXPLORE && blockIdx.y == 0 && ring_s) {
+      const int64_t nr = S - m0 < QT_ROWS ? S - m0 : QT_ROWS, o = (row0 + m0) * d.n_obs;
+      for (int64_t i = tid; i < nr * d.n_obs; i += 256) ring_s[o + i] = obs[o + i];
     }
     __syncthreads();
     q_tile_forward<DQN>(d, sS, sW1, sB1, sWt, sW2, d.n_h, sB2, sWq, sBq, sH1, sH2, sQ, n_wave, n_w, n_ft, q_in, tid, ty,
@@ -400,6 +424,12 @@ q_fwd_g_kernel(const QDims d, const float* __restrict__ P0, int64_t p_stride, co
 #pragma unroll
         for (int j = 1; j < QT_NA; ++j)
           if (j < n_a && qv[j] > best) { best = qv[j]; pick = j; }
+        if (EXPLORE) {
+          const uint32_t hsh = q_row_hash(seed_lo, seed_hi, step, r, a);
+          if ((float)(hsh >> 8) * (1.0f / 16777216.0f) < eps.v[k])
+            pick = (int)(((uint64_t)qmix32(hsh ^ 0x5BD1E995U) * (uint32_t)n_a) >> 32);
+          if (ring_a) ring_a[g * d.A + a] = (int8_t)pick;
+        }
       } else {
         float s = 0.f;
 #pragma unroll
@@ -524,13 +554,21 @@ __device__ __forceinline__ void q_bgrad(const float* __restrict__ B, int n, floa
 // writes them at the agent's flat offsets into partial row g (part [groups][ld]); the tail columns n_params + a,
 // n_params + A + a and n_params + 2 A + a get inv_n times the CTA's sums of e^2, q(s)[act] and tq (the summaries of
 // QPolicy, agents/policies.py:331-338: loss, mean q, mean tq).
-template <bool DQN>
+// GROUPED (tscl_q_td_g): grid (groups, A, K); member k = blockIdx.z owns the ring's replica columns k R .. k R + R - 1 of
+// R_ring, reads P + k p_stride, uses gam.v[k] and writes partial row k groups + g: CTA (g, a, k) does exactly what CTA
+// (g, a) of member k's own launch does.
+template <bool DQN, bool GROUPED = false>
 __global__ void __launch_bounds__(256)
-q_td_kernel(const QDims d, const float* __restrict__ P, const float* __restrict__ ring_s,
+q_td_kernel(const QDims d, const float* __restrict__ P0, const float* __restrict__ ring_s,
             const float* __restrict__ ring_s1, const int8_t* __restrict__ ring_a, const float* __restrict__ ring_r,
-            const uint8_t* __restrict__ ring_done, const int32_t* __restrict__ idx, int64_t R, int batch, float gamma,
-            float inv_n, int64_t n_params, float* __restrict__ part, int64_t ld) {
+            const uint8_t* __restrict__ ring_done, const int32_t* __restrict__ idx, int64_t R, int batch, float gamma0,
+            float inv_n, int64_t n_params, float* __restrict__ part, int64_t ld, int64_t R_ring, int64_t p_stride,
+            const QMemberF gam) {
   extern __shared__ __align__(16) float qsm[];
+  const int mk = GROUPED ? (int)blockIdx.z : 0;
+  const float* __restrict__ P = GROUPED ? P0 + mk * p_stride : P0;
+  const float gamma = GROUPED ? gam.v[mk] : gamma0;
+  const int64_t Rr = GROUPED ? R_ring : R, rc0 = GROUPED ? (int64_t)mk * R : 0;
   const QTdSmem T = q_td_smem_layout(d);
   const QSmem& L = T.f;
   const int a = blockIdx.y, tid = threadIdx.x, ty = tid >> 4, tx = tid & 15;
@@ -579,7 +617,7 @@ q_td_kernel(const QDims d, const float* __restrict__ P, const float* __restrict_
         float x = 0.f;
         if (m < rows) {
           const int64_t r = m / batch;
-          x = __ldg(src + ((int64_t)ia[m] * R + r) * d.n_obs + ooff + k);
+          x = __ldg(src + ((int64_t)ia[m] * Rr + rc0 + r) * d.n_obs + ooff + k);
         }
         sS[k * QT_LD + row] = x;
       }
@@ -593,7 +631,7 @@ q_td_kernel(const QDims d, const float* __restrict__ P, const float* __restrict_
           float tq = 0.f;
           int act = -1;
           if (m < rows) {
-            const int64_t r = m / batch, e = (int64_t)ia[m] * R + r;
+            const int64_t r = m / batch, e = (int64_t)ia[m] * Rr + rc0 + r;
             float best = sQ[tid * QT_NA];
             for (int j = 1; j < n_a; ++j) best = fmaxf(best, sQ[tid * QT_NA + j]);
             const float rw = ring_r[e * d.A + a];
@@ -663,7 +701,7 @@ q_td_kernel(const QDims d, const float* __restrict__ P, const float* __restrict_
     if ((tid & 31) == 0) { sTq[tid >> 5] = loss; sTq[2 + (tid >> 5)] = qsum; sTq[4 + (tid >> 5)] = tqsum; }
   }
   __syncthreads();
-  float* out = part + (int64_t)blockIdx.x * ld;
+  float* out = part + ((GROUPED ? (int64_t)mk * gridDim.x : 0) + blockIdx.x) * ld;
   if (tid == 0) {
     out[n_params + a] = (sTq[0] + sTq[1]) * inv_n;
     out[n_params + d.A + a] = (sTq[2] + sTq[3]) * inv_n;
@@ -693,15 +731,37 @@ __global__ void q_reduce_kernel(const float* __restrict__ part, int groups, int6
   grad[i] = s;
 }
 
+// Grouped form: grid (x, K); grad[k][i] = sum over member k's partial rows part[k][g][i], g = 0, 1, .. in that order
+__global__ void q_reduce_g_kernel(const float* __restrict__ part, int groups, int64_t ld, float* __restrict__ grad) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= ld) return;
+  const float* p = part + (int64_t)blockIdx.y * groups * ld;
+  float s = 0.f;
+  for (int g = 0; g < groups; ++g) s += p[(int64_t)g * ld + i];
+  grad[(int64_t)blockIdx.y * ld + i] = s;
+}
+
 // Per agent (one CTA of 512 threads): tf.clip_by_global_norm and the TF1 Adam step of IQL.td_update
 // (agents/models.py:290-302) on the agent's block [blk[a], blk[a+1]) of the flat vector, loss / norm written out, and
 // with rec_out the agent's row (loss, mean q, mean tq, norm) of the round's summaries.
+// GROUPED (tscl_q_adam_g): grid (A, K); member k = blockIdx.y steps P / m / v + k p_stride with grad + k (n_params + 3 A),
+// lr.v[k] and clip.v[k], and writes loss / norm at + k out_stride and its rec row at + k rec_stride.
+template <bool GROUPED = false>
 __global__ void __launch_bounds__(512)
-q_adam_kernel(float* __restrict__ P, const float* __restrict__ grad, float* __restrict__ m, float* __restrict__ v,
-              const int64_t* __restrict__ blk, int64_t n_params, int A, float lr_t, float max_norm,
-              float* __restrict__ loss_out, float* __restrict__ norm_out, float* __restrict__ rec_out) {
+q_adam_kernel(float* __restrict__ P0, const float* __restrict__ grad0, float* __restrict__ m0, float* __restrict__ v0,
+              const int64_t* __restrict__ blk, int64_t n_params, int A, float lr_t0, float max_norm0,
+              float* __restrict__ loss_out0, float* __restrict__ norm_out0, float* __restrict__ rec_out0,
+              int64_t p_stride, int64_t out_stride, int64_t rec_stride, const QMemberF lr, const QMemberF clip) {
   __shared__ float red[512];
-  const int a = blockIdx.x, tid = threadIdx.x;
+  const int a = blockIdx.x, tid = threadIdx.x, mk = GROUPED ? (int)blockIdx.y : 0;
+  float* __restrict__ P = GROUPED ? P0 + mk * p_stride : P0;
+  float* __restrict__ m = GROUPED ? m0 + mk * p_stride : m0;
+  float* __restrict__ v = GROUPED ? v0 + mk * p_stride : v0;
+  const float* __restrict__ grad = GROUPED ? grad0 + mk * (n_params + 3 * A) : grad0;
+  float* __restrict__ loss_out = GROUPED ? loss_out0 + mk * out_stride : loss_out0;
+  float* __restrict__ norm_out = GROUPED ? norm_out0 + mk * out_stride : norm_out0;
+  float* __restrict__ rec_out = GROUPED && rec_out0 ? rec_out0 + mk * rec_stride : rec_out0;
+  const float lr_t = GROUPED ? lr.v[mk] : lr_t0, max_norm = GROUPED ? clip.v[mk] : max_norm0;
   const int64_t b0 = blk[a], b1 = blk[a + 1];
   float ss = 0.f;
   for (int64_t i = b0 + tid; i < b1; i += 512) ss = fmaf(grad[i], grad[i], ss);
@@ -733,12 +793,17 @@ q_adam_kernel(float* __restrict__ P, const float* __restrict__ grad, float* __re
 }
 
 // IQL.add_transition's reward (r / reward_norm, then clipped) and the post-step done into one replay slot, and the
-// episode's global-reward sum.
-__global__ void q_transition_kernel(const float* __restrict__ rew, int64_t RA, float reward_norm, float reward_clip,
+// episode's global-reward sum.  GROUPED (tscl_q_transition_g): row r belongs to member r / R_m and takes its
+// reward_norm / reward_clip from norms / clips.
+template <bool GROUPED = false>
+__global__ void q_transition_kernel(const float* __restrict__ rew, int64_t RA, float reward_norm0, float reward_clip0,
                                     float* __restrict__ ring_r, const float* __restrict__ grew, float* __restrict__ rew_acc,
-                                    uint8_t* __restrict__ ring_done, int64_t R, int done) {
+                                    uint8_t* __restrict__ ring_done, int64_t R, int done, int64_t R_m,
+                                    const QMemberF norms, const QMemberF clips) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < RA) {
+    const int mk = GROUPED ? (int)(i / (RA / R) / R_m) : 0;
+    const float reward_norm = GROUPED ? norms.v[mk] : reward_norm0, reward_clip = GROUPED ? clips.v[mk] : reward_clip0;
     float x = rew[i];
     if (reward_norm != 0.f) x = __fdiv_rn(x, reward_norm);
     if (reward_clip != 0.f) x = fminf(fmaxf(x, -reward_clip), reward_clip);
@@ -833,11 +898,15 @@ extern "C" int tscl_q_create(const tscl_qdims* x, int32_t device, tscl_qhandle**
   LCK(cudaFuncSetAttribute(ex, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem));
   const void* fg = dqn ? (const void*)q_fwd_g_kernel<true> : (const void*)q_fwd_g_kernel<false>;
   LCK(cudaFuncSetAttribute(fg, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem));
+  const void* eg = dqn ? (const void*)q_fwd_g_kernel<true, true> : (const void*)q_fwd_g_kernel<false, true>;
+  LCK(cudaFuncSetAttribute(eg, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem));
   const size_t td_smem = (size_t)q_td_smem_layout(d).total * sizeof(float);
   if (td_smem <= (size_t)optin) {
     const void* td = dqn ? (const void*)q_td_kernel<true> : (const void*)q_td_kernel<false>;
     LCK(cudaFuncSetAttribute(td, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)td_smem));
     LCK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&h->td_ctas_per_sm, td, 256, td_smem));
+    const void* tg = dqn ? (const void*)q_td_kernel<true, true> : (const void*)q_td_kernel<false, true>;
+    LCK(cudaFuncSetAttribute(tg, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)td_smem));
     if (h->td_ctas_per_sm < 1) h->td_ctas_per_sm = 1;
     h->td_smem = td_smem;
   }
@@ -850,6 +919,7 @@ extern "C" int tscl_q_destroy(tscl_qhandle* h) {
   cudaSetDevice(h->device);
   for (void* p : h->owned) cudaFree(p);
   if (h->part) cudaFree(h->part);
+  if (h->part_g) cudaFree(h->part_g);
   delete h;
   return 0;
 }
@@ -900,10 +970,12 @@ extern "C" int tscl_q_step_g(tscl_qhandle* h, const float* params, int64_t p_str
   unsigned long long* bad = reinterpret_cast<unsigned long long*>(bad_flags);
   if (h->d.model == 1)
     q_fwd_g_kernel<true><<<grid, 256, h->smem, (cudaStream_t)stream>>>(h->d, params, p_stride, obs, rows, q, act, mode,
-                                                                        seeds, (uint32_t)step, bad);
+                                                                        seeds, (uint32_t)step, bad, QMemberF{}, 0,
+                                                                        nullptr, nullptr);
   else
     q_fwd_g_kernel<false><<<grid, 256, h->smem, (cudaStream_t)stream>>>(h->d, params, p_stride, obs, rows, q, act, mode,
-                                                                         seeds, (uint32_t)step, bad);
+                                                                         seeds, (uint32_t)step, bad, QMemberF{}, 0,
+                                                                         nullptr, nullptr);
   LCK(cudaGetLastError());
   return 0;
 }
@@ -960,11 +1032,11 @@ extern "C" int tscl_q_td(tscl_qhandle* h, const float* params, const float* ring
   if (h->d.model == 1)
     q_td_kernel<true><<<grid, 256, h->td_smem, (cudaStream_t)stream>>>(h->d, params, ring_s, ring_s1, ring_a, ring_r,
                                                                         ring_done, idx, R, batch, gamma, inv_n,
-                                                                        h->n_params, h->part, ld);
+                                                                        h->n_params, h->part, ld, 0, 0, QMemberF{});
   else
     q_td_kernel<false><<<grid, 256, h->td_smem, (cudaStream_t)stream>>>(h->d, params, ring_s, ring_s1, ring_a, ring_r,
                                                                          ring_done, idx, R, batch, gamma, inv_n,
-                                                                         h->n_params, h->part, ld);
+                                                                         h->n_params, h->part, ld, 0, 0, QMemberF{});
   LCK(cudaGetLastError());
   q_reduce_kernel<<<(unsigned)((ld + 255) / 256), 256, 0, (cudaStream_t)stream>>>(h->part, (int)groups, ld, grad);
   LCK(cudaGetLastError());
@@ -976,7 +1048,8 @@ extern "C" int tscl_q_adam(tscl_qhandle* h, float* params, const float* grad, fl
   if (!h || !params || !grad || !adam_m || !adam_v || !loss_out || !norm_out) return tsc_set_error("tscl_q_adam: bad argument");
   LCK(cudaSetDevice(h->device));
   q_adam_kernel<<<h->d.A, 512, 0, (cudaStream_t)stream>>>(params, grad, adam_m, adam_v, h->blk, h->n_params, h->d.A,
-                                                          lr_t, max_grad_norm, loss_out, norm_out, rec_out);
+                                                          lr_t, max_grad_norm, loss_out, norm_out, rec_out, 0, 0, 0,
+                                                          QMemberF{}, QMemberF{});
   LCK(cudaGetLastError());
   return 0;
 }
@@ -988,7 +1061,101 @@ extern "C" int tscl_q_transition(tscl_qhandle* h, const float* rew, int64_t R, f
   LCK(cudaSetDevice(h->device));
   const int64_t RA = R * h->d.A;
   q_transition_kernel<<<(unsigned)((RA + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
-      rew, RA, reward_norm, reward_clip, ring_r, grew, rew_acc, ring_done, R, done);
+      rew, RA, reward_norm, reward_clip, ring_r, grew, rew_acc, ring_done, R, done, 0, QMemberF{}, QMemberF{});
+  LCK(cudaGetLastError());
+  return 0;
+}
+
+// ================================================================================================
+// Grouped training (a population or sweep of K members, R_m replicas each, in one lock-step of K R_m replicas)
+
+extern "C" int tscl_q_explore_g(tscl_qhandle* h, const float* params, int64_t p_stride, const float* obs, int32_t K,
+                                const int64_t* rows, int64_t R, float* q, int32_t* act, const float* eps, uint64_t seed,
+                                int64_t step, float* ring_s, int8_t* ring_a, void* stream) {
+  if (!h || !params || !obs || !rows || !q || !act || !eps || K < 1 || K > QG_MAX || R < K ||
+      (K > 1 && p_stride < h->n_params))
+    return tsc_set_error("tscl_q_explore_g: bad argument (1 <= K <= 64 members)");
+  LCK(cudaSetDevice(h->device));
+  const int64_t max_tiles = (R + QT_ROWS - 1) / QT_ROWS;
+  int64_t groups = ((int64_t)h->n_sm * h->ctas_per_sm + (int64_t)h->d.A * K - 1) / ((int64_t)h->d.A * K);
+  if (groups > max_tiles) groups = max_tiles;
+  dim3 grid((unsigned)groups, (unsigned)h->d.A, (unsigned)K);
+  const QMemberF e = q_member_f(eps, K);
+  if (h->d.model == 1)
+    q_fwd_g_kernel<true, true><<<grid, 256, h->smem, (cudaStream_t)stream>>>(
+        h->d, params, p_stride, obs, rows, q, act, 0, nullptr, (uint32_t)step, nullptr, e, seed, ring_s, ring_a);
+  else
+    q_fwd_g_kernel<false, true><<<grid, 256, h->smem, (cudaStream_t)stream>>>(
+        h->d, params, p_stride, obs, rows, q, act, 0, nullptr, (uint32_t)step, nullptr, e, seed, ring_s, ring_a);
+  LCK(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int tscl_q_td_g(tscl_qhandle* h, const float* params, int64_t p_stride, int32_t K, const float* ring_s,
+                           const float* ring_s1, const int8_t* ring_a, const float* ring_r, const uint8_t* ring_done,
+                           const int32_t* idx, int64_t R_m, int32_t batch, const float* gamma, float inv_n, float* grad,
+                           void* stream) {
+  if (!h || !params || !ring_s || !ring_s1 || !ring_a || !ring_r || !ring_done || !idx || !gamma || !grad || R_m <= 0 ||
+      batch <= 0 || K < 1 || K > QG_MAX || (K > 1 && p_stride < h->n_params))
+    return tsc_set_error("tscl_q_td_g: bad argument (1 <= K <= 64 members)");
+  if (!h->td_smem)
+    return tsc_set_error("tscl_q_td_g: the weights, gradients and tiles of one agent need more shared memory than a CTA "
+                         "has");
+  LCK(cudaSetDevice(h->device));
+  const int A = h->d.A;
+  // member k's partial rows are cut as its own tscl_q_td launch on R_m replicas cuts them
+  const int64_t ld = h->n_params + 3 * A, n_tiles = (R_m * batch + QT_ROWS - 1) / QT_ROWS;
+  const int64_t max_groups = ((int64_t)h->n_sm * h->td_ctas_per_sm + A - 1) / A;
+  const int64_t groups = max_groups < n_tiles ? max_groups : n_tiles;
+  if (h->part_g_k < K) {
+    if (h->part_g) LCK(cudaFree(h->part_g));
+    h->part_g = nullptr;
+    h->part_g_k = 0;
+    LCK(cudaMalloc(&h->part_g, (size_t)K * max_groups * ld * sizeof(float)));
+    h->part_g_k = K;
+  }
+  dim3 grid((unsigned)groups, (unsigned)A, (unsigned)K);
+  const QMemberF g = q_member_f(gamma, K);
+  if (h->d.model == 1)
+    q_td_kernel<true, true><<<grid, 256, h->td_smem, (cudaStream_t)stream>>>(
+        h->d, params, ring_s, ring_s1, ring_a, ring_r, ring_done, idx, R_m, batch, 0.f, inv_n, h->n_params, h->part_g,
+        ld, (int64_t)K * R_m, p_stride, g);
+  else
+    q_td_kernel<false, true><<<grid, 256, h->td_smem, (cudaStream_t)stream>>>(
+        h->d, params, ring_s, ring_s1, ring_a, ring_r, ring_done, idx, R_m, batch, 0.f, inv_n, h->n_params, h->part_g,
+        ld, (int64_t)K * R_m, p_stride, g);
+  LCK(cudaGetLastError());
+  q_reduce_g_kernel<<<dim3((unsigned)((ld + 255) / 256), (unsigned)K), 256, 0, (cudaStream_t)stream>>>(
+      h->part_g, (int)groups, ld, grad);
+  LCK(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int tscl_q_adam_g(tscl_qhandle* h, int32_t K, float* params, int64_t p_stride, const float* grad,
+                             float* adam_m, float* adam_v, const float* lr_t, const float* max_grad_norm, float* loss_out,
+                             float* norm_out, int64_t out_stride, float* rec_out, int64_t rec_stride, void* stream) {
+  if (!h || !params || !grad || !adam_m || !adam_v || !lr_t || !max_grad_norm || !loss_out || !norm_out || K < 1 ||
+      K > QG_MAX || (K > 1 && (p_stride < h->n_params || out_stride < h->d.A || (rec_out && rec_stride < 4 * h->d.A))))
+    return tsc_set_error("tscl_q_adam_g: bad argument (1 <= K <= 64 members)");
+  LCK(cudaSetDevice(h->device));
+  q_adam_kernel<true><<<dim3((unsigned)h->d.A, (unsigned)K), 512, 0, (cudaStream_t)stream>>>(
+      params, grad, adam_m, adam_v, h->blk, h->n_params, h->d.A, 0.f, 0.f, loss_out, norm_out, rec_out, p_stride,
+      out_stride, rec_stride, q_member_f(lr_t, K), q_member_f(max_grad_norm, K));
+  LCK(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int tscl_q_transition_g(tscl_qhandle* h, const float* rew, int32_t K, int64_t R_m, const float* reward_norm,
+                                   const float* reward_clip, float* ring_r, const float* grew, float* rew_acc,
+                                   uint8_t* ring_done, int32_t done, void* stream) {
+  if (!h || !rew || !ring_r || !ring_done || !reward_norm || !reward_clip || R_m <= 0 || K < 1 || K > QG_MAX ||
+      (rew_acc && !grew))
+    return tsc_set_error("tscl_q_transition_g: bad argument (1 <= K <= 64 members)");
+  LCK(cudaSetDevice(h->device));
+  const int64_t R = (int64_t)K * R_m, RA = R * h->d.A;
+  q_transition_kernel<true><<<(unsigned)((RA + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
+      rew, RA, 0.f, 0.f, ring_r, grew, rew_acc, ring_done, R, done, R_m, q_member_f(reward_norm, K),
+      q_member_f(reward_clip, K));
   LCK(cudaGetLastError());
   return 0;
 }

@@ -393,6 +393,36 @@ int tscl_q_adam(tscl_qhandle* h, float* params, const float* grad, float* adam_m
 int tscl_q_transition(tscl_qhandle* h, const float* rew, int64_t R, float reward_norm, float reward_clip, float* ring_r,
                       const float* grew, float* rew_acc, uint8_t* ring_done, int32_t done, void* stream);
 
+/* Grouped training: K members (1 <= K <= 64) of the handle's Q layout trained in one lock-step of K * R_m replicas, member
+ * k on rows k * R_m .. (k+1) * R_m - 1 with its weights, Adam slots and gradient at params / adam_m / adam_v + k * p_stride
+ * and grad + k * (n_params + 3 A).  The replay ring is one ring [B][K * R_m][...]: member k's entry (slot i, member-local
+ * replica r) is ring row i * K * R_m + k * R_m + r.  Per-member scalars (eps, gamma, lr_t, max_grad_norm, reward_norm,
+ * reward_clip) are HOST arrays of K floats, read during the call and passed to the kernel by value.  Member k's outputs
+ * are bit-identical to the solo entry point's on its own rows (replica0 = 0) with its own scalars.
+ *
+ * Minibatch indices: the draws of tscl_q_sample depend only on (seed, update, round, replica0 + r, agent), so one
+ * tscl_q_sample launch at R = R_m, replica0 = 0 gives every member the indices its solo run draws; tscl_q_td_g reads
+ * that one idx [A][R_m][batch] for all members (members share the learner seed, as every IQL run does). */
+/* tscl_q_explore for K members: rows as in tscl_q_step_g (device, K + 1 boundaries over R rows), eps host [K], draws
+ * keyed (seed, step, member-local replica, agent); ring_s [R][n_obs] / ring_a [R][A] of the slot (either may be NULL). */
+int tscl_q_explore_g(tscl_qhandle* h, const float* params, int64_t p_stride, const float* obs, int32_t K, const int64_t* rows,
+                     int64_t R, float* q, int32_t* act, const float* eps, uint64_t seed, int64_t step, float* ring_s,
+                     int8_t* ring_a, void* stream);
+/* tscl_q_td for K members of R_m replicas: gamma host [K], inv_n = 1 / (batch R_m) for every member, grad [K][n_params +
+ * 3 A].  Member k's partial rows are cut exactly as its solo launch on R_m replicas cuts them, then added in order. */
+int tscl_q_td_g(tscl_qhandle* h, const float* params, int64_t p_stride, int32_t K, const float* ring_s, const float* ring_s1,
+                const int8_t* ring_a, const float* ring_r, const uint8_t* ring_done, const int32_t* idx, int64_t R_m,
+                int32_t batch, const float* gamma, float inv_n, float* grad, void* stream);
+/* tscl_q_adam for K members: lr_t and max_grad_norm host [K]; member k's loss and norm rows at loss_out / norm_out +
+ * k * out_stride, its rec rows (rec_out may be NULL) at rec_out + k * rec_stride. */
+int tscl_q_adam_g(tscl_qhandle* h, int32_t K, float* params, int64_t p_stride, const float* grad, float* adam_m,
+                  float* adam_v, const float* lr_t, const float* max_grad_norm, float* loss_out, float* norm_out,
+                  int64_t out_stride, float* rec_out, int64_t rec_stride, void* stream);
+/* tscl_q_transition with member k's reward_norm / reward_clip (host [K]) on its R_m rows; ring_done and rew_acc as there. */
+int tscl_q_transition_g(tscl_qhandle* h, const float* rew, int32_t K, int64_t R_m, const float* reward_norm,
+                        const float* reward_clip, float* ring_r, const float* grew, float* rew_acc, uint8_t* ring_done,
+                        int32_t done, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
