@@ -350,34 +350,37 @@ def _frozen(v):
     return v
 
 
-def sim_key(env):
+def sim_key(env, demand=False):
     """Equal for two envs whose simulators are built identically: the scenario, the simulator parameters and every net
     table, compared on the built objects.  MA2C leaves out coop_gamma (parameter and observation scale): members that
     differ only there share a simulator through per-replica coop_gamma.  The env seed is not part of the simulator (it
-    keys only the policies' sampling)."""
+    keys only the policies' sampling).  `demand` leaves out the demand tables (net.tables.DEMAND_FIELDS) as well:
+    members that differ only there share a simulator through per-replica demand (tsc_set_replica_demand)."""
     import dataclasses
+    from ..net.tables import DEMAND_FIELDS
     net, par = env._tables, env._params
     ma2c = par.agent == 'ma2c'
     c = par.as_c()
     cfg = tuple((n, getattr(c, n)) for n, _ in type(c)._fields_ if not (ma2c and n == 'coop_gamma'))
     tables = tuple((f.name, _frozen(getattr(net, f.name))) for f in dataclasses.fields(net)
-                   if not (ma2c and f.name == 'obs_scale'))
+                   if not (ma2c and f.name == 'obs_scale') and not (demand and f.name in DEMAND_FIELDS))
     return env.name, cfg, tables
 
 
 class GroupEntry:
     """One agent directory of a GroupEvaluator: `label` (its name on the command line), `agent` (the directory's name),
     `model` (entry_model), `output_path`; after the checks `env` (its own one-seed-set env, no simulator), `config`,
-    `seed` ([ENV_CONFIG] seed), and `error` when it was skipped.  After run(): mean / std per episode, the three frames
-    and `summary`."""
+    `seed` ([ENV_CONFIG] seed), and `error` when it was skipped; `demand`, the {key: value} demand level it runs at
+    (None: its config's own).  After run(): mean / std per episode, the three frames and `summary`."""
 
-    def __init__(self, agent_dir, model, output_path):
+    def __init__(self, agent_dir, model, output_path, demand=None):
         import os
         self.agent_dir = agent_dir.rstrip('/')
         self.agent = os.path.basename(self.agent_dir)
         self.label = self.agent_dir
         self.model, self.output_path = model, output_path
         self.env = self.config = self.error = None
+        self.demand = demand
         self.mean = self.std = self.recorded = self.summary = None
 
 
@@ -396,20 +399,40 @@ class GroupEvaluator:
     tsc_greedy_actions, the v1 / fc A2C members' own forwards on their row slices, and one tsc_step (tsc_step_record).
     Each entry's reward trace, frames and summary are those `Evaluator` gives for its directory alone: member k samples
     with its own [ENV_CONFIG] seed and member-local replica index, ma2c members their own coop_gamma
-    (tsc_set_replica_coop_gamma)."""
+    (tsc_set_replica_coop_gamma).
 
-    def __init__(self, entries, seeds, policy_type='default', policy='lstm', device=0, max_replicas=MAX_GROUP_REPLICAS):
+    `share_demand`: entries whose simulators differ only in their demand tables (sim_key(demand=True)) share one
+    simulator too, each still at its own config's demand (tsc_set_replica_demand).  `demand_levels`: a list of
+    {[ENV_CONFIG] key: value} demand overrides (keys of the entry scenario's envs.DEMAND_KEYS; a key a level does not
+    name keeps the entry's value); implies share_demand.  Every entry is then evaluated at every level, as one member
+    per (entry, level) pair, and the output path of an entry is a list with one path per level.  `entries` (and
+    `groups`) then hold one GroupEntry per pair, with `demand` set to its level."""
+
+    def __init__(self, entries, seeds, policy_type='default', policy='lstm', device=0, max_replicas=MAX_GROUP_REPLICAS,
+                 share_demand=False, demand_levels=None):
         import configparser
         import glob
         import os
-        from ..envs import make_env
+        from ..envs import check_demand_tables, demand_keys, make_env
         if policy_type not in ('default', 'stochastic', 'deterministic'):
             raise ValueError("policy_type must be 'default', 'stochastic' or 'deterministic' (got %r)" % (policy_type,))
         self.seeds = [int(s) for s in seeds]
         if not self.seeds:
             raise ValueError('GroupEvaluator: no evaluation seeds')
         self.policy_type, self.policy, self.device = policy_type, policy, device
-        self.entries = [GroupEntry(d, m, o) for d, m, o in entries]
+        levels = None if demand_levels is None else [dict((str(k), str(v)) for k, v in lv.items()) for lv in demand_levels]
+        if levels is not None and not levels:
+            raise ValueError('GroupEvaluator: demand_levels is an empty list')
+        self.share_demand = bool(share_demand) or levels is not None
+        if levels is None:
+            self.entries = [GroupEntry(d, m, o) for d, m, o in entries]
+        else:
+            self.entries = []
+            for d, m, o in entries:
+                if isinstance(o, str) or len(o) != len(levels):
+                    raise ValueError('%s: with %d demand levels, the output path is a list of %d paths'
+                                     % (d, len(levels), len(levels)))
+                self.entries += [GroupEntry(d, m, oj, demand=lv) for oj, lv in zip(o, levels)]
         for e in self.entries:
             if e.model == 'a2c':
                 raise ValueError("%s: batched evaluation covers greedy, ia2c, ma2c and IQL (got agent 'a2c')" % e.label)
@@ -432,13 +455,25 @@ class GroupEvaluator:
             cfg['test_seeds'] = ','.join(str(s) for s in self.seeds)
             cfg['agent'] = e.agent
             e.seed = cfg.getint('seed')
+            if e.demand is not None:
+                allowed = demand_keys(cfg)
+                for key in e.demand:
+                    if key not in allowed:
+                        raise ValueError('%s: %r is not a demand key of its scenario %r (demand keys: %s)'
+                                         % (e.label, key, cfg.get('scenario'), ', '.join(allowed) or 'none'))
+                own = make_env(cfg, len(self.seeds), e.output_path, device=device)._tables
+                for key, v in e.demand.items():
+                    cfg[key] = v
+                e.env = make_env(cfg, len(self.seeds), e.output_path, device=device)
+                check_demand_tables(own, e.env._tables, e.label, ignore=())
+                continue
             e.env = make_env(cfg, len(self.seeds), e.output_path, device=device)
         self.groups = []                                 # [[entry, ...]] per shared simulator, in entry order
         keys = []
         for e in self.entries:
             if e.error:
                 continue
-            k = sim_key(e.env)
+            k = sim_key(e.env, demand=self.share_demand)
             if k in keys:
                 self.groups[keys.index(k)].append(e)
             else:
@@ -526,6 +561,12 @@ class _Group:
         self.sim = sim = BatchedSim(env._tables, env._params, R, device=ge.device)
         if cg is not None:
             sim.set_replica_coop_gamma(np.repeat(np.asarray(cg, np.float32), S))
+        if ge.share_demand:
+            # members that differ in their demand tables: each member's replicas take its own (identical ones once)
+            from ..net.tables import DEMAND_FIELDS
+            nets = [e.env._tables for e in self.entries]
+            if any(not np.array_equal(getattr(t, f), getattr(env._tables, f)) for t in nets for f in DEMAND_FIELDS):
+                sim.set_replica_demand(nets, np.repeat(np.arange(K), S))
         self.dev = sim.device
         net = env._tables
         self.N, self.n_obs, self.max_na = net.n_nodes, net.n_obs, net.max_na

@@ -604,11 +604,12 @@ def train_population(config, base_dir, seeds, test_mode='no_test', n_replicas=1,
 
 
 def _train_members(cfgs, dirs, agent, seeds, R_m, in_test, post_test, policy, device, summaries, what, sweep=False,
-                   deterministic=False):
+                   deterministic=False, demand=None):
     """The training run of a population or a sweep, member k from cfgs[k] (seed seeds[k]) into the agent directory
     dirs[k] (init_dir's dict): member-tagged log files, one simulator and one learner for all K * R_m replicas, one
     driver per member.  A sweep gives each member its own learner values and schedules (`IA2C(member_configs=...)`)
-    and, for ma2c, its own coop_gamma in the simulator."""
+    and, for ma2c, its own coop_gamma in the simulator; `demand` (member_demand) gives member k the demand of
+    demand[k]."""
     import torch
     from ..envs import make_env
     from .evaluator import Evaluator
@@ -642,7 +643,7 @@ def _train_members(cfgs, dirs, agent, seeds, R_m, in_test, post_test, policy, de
             summ = [Summaries(w, summary_name(agent, policy), 'a2c', model.n_step) for w in writers]
         lr, beta = (model.lr_schedulers, model.beta_schedulers) if sweep else (model.lr_scheduler, model.beta_scheduler)
         trainer = BatchedTrainer(sim, model.batched, agent, lr, beta, seed0=seeds[0], greward_trace=trace,
-                                 coop_gamma=cg, **srec)
+                                 coop_gamma=cg, demand=demand, **srec)
         drivers = []
         for k in range(K):                  # one driver per member, over its view of the shared trainer
             evaluator = None
@@ -699,12 +700,14 @@ def _value(cfg, sec, key):
     return cfg.get(sec, key, fallback=None) if cfg.has_section(sec) else None
 
 
-def sweep_members(configs, keys=None):
+def sweep_members(configs, keys=None, demand=False):
     """The members of a sweep as [(name, ConfigParser, path or None)], checked.  `configs`: a list of config paths
     (member name = file stem) or a dict name -> ConfigParser.  Refused with a ValueError: no config, repeated names, a
     key outside `keys` (default SWEEP_CONFIG_KEYS) that differs between two members (naming the key and both members), a
     coop_gamma that differs under ia2c (the reference reads it only for ma2c, envs/env.py:184-188, 595-609), and two
-    identical configs."""
+    identical configs.  `demand`: the members may also differ in their scenario's demand keys (envs.DEMAND_KEYS); their
+    nets, built on the host, must then differ only in their demand tables (refused naming the member and the field)."""
+    from ..envs import demand_keys
     allowed = SWEEP_CONFIG_KEYS if keys is None else keys
     if isinstance(configs, dict):
         items = [(str(n), c, None) for n, c in configs.items()]
@@ -723,6 +726,9 @@ def sweep_members(configs, keys=None):
     label = lambda i: items[i][2] or items[i][0]
     c0 = items[0][1]
     agent = _value(c0, 'ENV_CONFIG', 'agent')
+    if demand and c0.has_section('ENV_CONFIG'):
+        allowed = dict(allowed)
+        allowed['ENV_CONFIG'] = tuple(allowed.get('ENV_CONFIG', ())) + tuple(demand_keys(c0['ENV_CONFIG']))
     for i in range(1, len(items)):
         c = items[i][1]
         for sec in sorted(set(c0.sections()) | set(c.sections())):
@@ -741,7 +747,23 @@ def sweep_members(configs, keys=None):
             if all(_same(_value(items[j][1], sec, key), _value(c, sec, key))
                    for sec, ks in allowed.items() for key in ks):
                 raise ValueError('%s and %s are identical: a sweep trains each config once' % (label(j), label(i)))
+    if demand:
+        member_demand([c for _, c, _ in items], [label(i) for i in range(len(items))])
     return items
+
+
+def member_demand(cfgs, labels=None):
+    """The nets of a demand sweep's members (one NetTables per config, built on the host), or None when their demand
+    tables are all equal.  Refuses (naming the member and the field) a member whose net differs from the first member's
+    in more than its demand tables; ma2c members may differ in coop_gamma as well."""
+    from ..envs import check_demand_tables, make_env
+    from ..net.tables import DEMAND_FIELDS
+    nets = [make_env(c['ENV_CONFIG'], 1, '', is_record=False)._tables for c in cfgs]
+    ignore = ('obs_scale',) if cfgs[0]['ENV_CONFIG'].get('agent') == 'ma2c' else ()
+    for k in range(1, len(nets)):
+        check_demand_tables(nets[0], nets[k], labels[k] if labels else 'member %d' % k, ignore=ignore)
+    same = all(np.array_equal(getattr(t, f), getattr(nets[0], f)) for t in nets for f in DEMAND_FIELDS)
+    return None if same else nets
 
 
 def sweep_dir(base_dir, name, agent):
@@ -750,7 +772,7 @@ def sweep_dir(base_dir, name, agent):
 
 
 def train_sweep(configs, base_dir, test_mode='no_test', n_replicas=64, device=0, summaries=False, policy='lstm',
-                process_group=None, deterministic=False):
+                process_group=None, deterministic=False, vary_demand=False):
     """Train a hyperparameter sweep of one A2C agent (ia2c / ma2c, LSTM policy) in one process: one member per config
     (`sweep_members`: the configs may differ only in SWEEP_CONFIG_KEYS), each on `n_replicas` replicas (a multiple of
     64).  One simulator launch and one grouped policy forward per control step cover all K * n_replicas replicas;
@@ -758,14 +780,16 @@ def train_sweep(configs, base_dir, test_mode='no_test', n_replicas=64, device=0,
     `train(config_k, n_replicas=n_replicas)` trains alone.  Its directory `sweep_dir(base_dir, name_k, agent)` holds
     what that run leaves: data/ (its config, train_reward.csv, test CSVs), model/checkpoint-<step>.npz, log/<time>.log
     and, with `summaries`, its event file.  Everything is checked before any directory or device work.  Returns a
-    namespace like train_population's with `names`.  `deterministic`: as in train()."""
+    namespace like train_population's with `names`.  `deterministic`: as in train().  `vary_demand`: the members may
+    also differ in their scenario's demand keys (envs.DEMAND_KEYS, `sweep_members(demand=True)`); member k's replicas
+    then run at its own demand in the shared simulator."""
     from .learner import check_sweep
     from .models import a2c_hparams
     t0 = time.time()
     in_test, post_test = init_test_flag(test_mode)
     if process_group is not None:
         raise ValueError('a sweep trains in one process: it takes no process_group')
-    items = sweep_members(configs)
+    items = sweep_members(configs, demand=vary_demand)
     agent = items[0][1]['ENV_CONFIG'].get('agent')
     kind, _ = model_spec(agent)
     if kind == 'iql':
@@ -775,6 +799,7 @@ def train_sweep(configs, base_dir, test_mode='no_test', n_replicas=64, device=0,
     cfgs = [c for _, c, _ in items]
     seeds = [c['ENV_CONFIG'].getint('seed') for c in cfgs]
     check_sweep(seeds, [a2c_hparams(c['MODEL_CONFIG']) for c in cfgs], n_replicas, 1024, None)
+    demand = member_demand(cfgs) if vary_demand else None
     names, dirs = [n for n, _, _ in items], []
     for name, cfg, path in items:
         d = init_dir(sweep_dir(base_dir, name, agent))
@@ -785,7 +810,8 @@ def train_sweep(configs, base_dir, test_mode='no_test', n_replicas=64, device=0,
                 cfg.write(f)
         dirs.append(d)
     out = _train_members(cfgs, dirs, agent, seeds, int(n_replicas), in_test, post_test, policy, device, summaries,
-                         'sweep of %d configs %s' % (len(cfgs), names), sweep=True, deterministic=deterministic)
+                         'sweep of %d configs %s' % (len(cfgs), names), sweep=True, deterministic=deterministic,
+                         demand=demand)
     out.names, out.dirs = names, [sweep_dir(base_dir, n, agent) for n in names]
     out.wall_sec = time.time() - t0
     return out
@@ -838,20 +864,22 @@ def train_iql_population(config, base_dir, seeds, test_mode='no_test', n_replica
     return out
 
 
-def train_iql_sweep(configs, base_dir, test_mode='no_test', n_replicas=1, device=0, summaries=False):
+def train_iql_sweep(configs, base_dir, test_mode='no_test', n_replicas=1, device=0, summaries=False, vary_demand=False):
     """Train a hyperparameter sweep of one IQL agent (iqll / iqld) in one process: one member per config
     (`sweep_members` with IQL_SWEEP_CONFIG_KEYS: the seed, the lr and ε schedules, gamma, max_grad_norm and the reward
     scaling), each on `n_replicas` replicas, sharing the simulator, the replay ring and the grouped kernels.  Member k's
     directory `sweep_dir(base_dir, name_k, agent)` is what `train(config_k, n_replicas=n_replicas)` leaves.  Everything
-    is checked before any directory is made.  Returns a namespace like train_sweep's."""
+    is checked before any directory is made.  Returns a namespace like train_sweep's.  `vary_demand`: as in
+    train_sweep."""
     t0 = time.time()
     in_test, post_test = init_test_flag(test_mode)
-    items = sweep_members(configs, IQL_SWEEP_CONFIG_KEYS)
+    items = sweep_members(configs, IQL_SWEEP_CONFIG_KEYS, demand=vary_demand)
     agent = _iql_agent(items[0][1], 'train_iql_sweep')
     cfgs = [c for _, c, _ in items]
     seeds = [c['ENV_CONFIG'].getint('seed') for c in cfgs]
     names = [n for n, _, _ in items]
     paths = [sweep_dir(base_dir, n, agent) for n in names]
+    demand = member_demand(cfgs) if vary_demand else None
 
     def write(k, d):
         if items[k][2] is not None:
@@ -860,7 +888,7 @@ def train_iql_sweep(configs, base_dir, test_mode='no_test', n_replicas=1, device
             with open(os.path.join(d['data'], 'config.ini'), 'w') as f:
                 cfgs[k].write(f)
     out = _train_iql_members(cfgs, paths, write, agent, seeds, int(n_replicas), in_test, post_test, device, summaries,
-                             'sweep of %d configs %s' % (len(cfgs), names), sweep=True)
+                             'sweep of %d configs %s' % (len(cfgs), names), sweep=True, demand=demand)
     out.names, out.dirs, out.wall_sec = names, paths, time.time() - t0
     return out
 
@@ -876,7 +904,7 @@ def member_schedulers(model_configs, total_step):
 
 
 def _train_iql_members(cfgs, paths, write_config, agent, seeds, R_m, in_test, post_test, device, summaries, what,
-                       sweep):
+                       sweep, demand=None):
     """The training run of IQL members: member k from cfgs[k] into the agent directory paths[k].  The environment and
     the learner (which refuses what it cannot train) are built before any directory is made; then the directories, their
     configs (write_config(k, dirs)), member-tagged log files, one simulator and one learner for all K * R_m replicas, and
@@ -911,7 +939,7 @@ def _train_iql_members(cfgs, paths, write_config, agent, seeds, R_m, in_test, po
             writers = [SummaryWriter(d['log']) for d in dirs]
             summ = [Summaries(w, summary_name(agent, 'lstm', model.model_type), 'iql', model.n_step) for w in writers]
         lr_s, eps_s = member_schedulers([c['MODEL_CONFIG'] for c in cfgs], total_step)
-        trainer = BatchedIQLTrainer(sim, model, lr_s, eps_s, seed0=seeds[0], greward_trace=trace, **srec)
+        trainer = BatchedIQLTrainer(sim, model, lr_s, eps_s, seed0=seeds[0], greward_trace=trace, demand=demand, **srec)
         drivers = []
         for k in range(K):                  # one driver per member, over its view of the shared trainer
             evaluator = None

@@ -78,10 +78,20 @@ def schedule_values(sched, n_step: int):
     return sched.get(n_step) if hasattr(sched, "get") else sched
 
 
+def set_member_demand(sim, demand, K):
+    """Member k's replicas (the k-th block of sim.R / K) take their demand from demand[k] (a list of K NetTables);
+    None leaves the simulator's built demand."""
+    if demand is None:
+        return
+    if len(demand) != K:
+        raise ValueError("demand takes one net per member (%d, got %d)" % (K, len(demand)))
+    sim.set_replica_demand(list(demand), np.repeat(np.arange(K), sim.R // K))
+
+
 class BatchedTrainer:
     def __init__(self, sim: BatchedSim, model: BatchedA2C, agent: str, lr, beta,
                  seed0: int = 12, replica0: int = 0, greward_trace: Optional[torch.Tensor] = None,
-                 summary_rec: Optional[torch.Tensor] = None, coop_gamma=None):
+                 summary_rec: Optional[torch.Tensor] = None, coop_gamma=None, demand=None):
         """lr / beta: floats (the 'constant' schedules of every shipped A2C config) or objects with the reference's
         `Scheduler.get(n_step)` (agents/utils.py:268-281, agents/models.py:175-176); a schedule advances by n_step per
         update exactly as in the reference (its unit is control steps of ONE environment).
@@ -95,7 +105,9 @@ class BatchedTrainer:
         the list of the K members' episode means to `episode_rewards`.
         A sweep (a learner with `hparams`) passes lr / beta as lists with one schedule per member (`schedule_values`),
         and `coop_gamma`, one MA2C spatial discount per member: member k's replicas then step with its own
-        (BatchedSim.set_replica_coop_gamma)."""
+        (BatchedSim.set_replica_coop_gamma), and `demand`, one NetTables per member: member k's replicas then take
+        their traffic demand from demand[k] (BatchedSim.set_replica_demand)."""
+        set_member_demand(sim, demand, int(getattr(model, "K", 1)))
         if coop_gamma is not None:
             K, R_m = int(getattr(model, "K", 1)), sim.R // int(getattr(model, "K", 1))
             if len(coop_gamma) != K:

@@ -99,6 +99,8 @@ struct StepArgs {
   float* greward;
   uint8_t* done;
   const float* cg;    // [R] per-replica coop_gamma (tsc_set_replica_coop_gamma) or null: cfg.coop_gamma / obs_scale_val
+  const int32_t* dlevel;  // [R] demand level of each replica (tsc_set_replica_demand) or null.  When set, launch() points
+                          // net.src_due / src_plo / src_phi at the level stack [n_levels][..] and the CTA offsets them
 };
 
 // ------------------------------------------------------------------------------------------------
@@ -329,6 +331,10 @@ tsc_step_kernel(const StepArgs A) {
   const int tid = threadIdx.x;
   const int rep = blockIdx.x + A.rep0;
   const int L = n.n_lanes, N = n.n_nodes;
+  // demand tables of this replica's level (0 and the built tables when no levels are set)
+  const int dlv = A.dlevel ? __ldg(&A.dlevel[rep]) : 0;
+  const uint8_t* __restrict__ src_due = n.src_due + dlv * n.horizon * n.n_src;
+  const int p_off = dlv * n.n_pint * n.n_src;
 
   // ---- shared-memory carve-up ----
   Ring ring;
@@ -663,13 +669,14 @@ tsc_step_kernel(const StepArgs A) {
           // turn ratios when the entry lane saturates (a fixed order would starve the later siblings)
           int best = 0;
           for (int q2 = q; q2 >= 0; q2 = __ldg(&n.src_next[q2])) {
-            int due = in_h ? (int)__ldg(&n.src_due[t_abs * n.n_src + q2]) : 0;
+            int due = in_h ? (int)__ldg(&src_due[t_abs * n.n_src + q2]) : 0;
             const int gq = __ldg(&n.src_group[q2]);
             if (gq >= 0 && due > 0) {
               const float ug = u01(rng_draw(key, 0x20000u + (uint32_t)gq, 7u));
               int iv = (int)t_abs / n.pint_sec;
               if (iv >= n.n_pint) iv = n.n_pint - 1;
-              if (!(ug >= __ldg(&n.src_plo[iv * n.n_src + q2]) && ug < __ldg(&n.src_phi[iv * n.n_src + q2]))) due = 0;
+              const int pi = p_off + iv * n.n_src + q2;
+              if (!(ug >= __ldg(&n.src_plo[pi]) && ug < __ldg(&n.src_phi[pi]))) due = 0;
             }
             int b2 = s_backlog[q2] + due;
             if (b2 > 65535) b2 = 65535;
@@ -678,7 +685,7 @@ tsc_step_kernel(const StepArgs A) {
           }
         }
         for (; q >= 0; q = __ldg(&n.src_next[q])) {
-          int b_new = n.src_group ? s_backlog[q] : s_backlog[q] + (in_h ? (int)__ldg(&n.src_due[t_abs * n.n_src + q]) : 0);
+          int b_new = n.src_group ? s_backlog[q] : s_backlog[q] + (in_h ? (int)__ldg(&src_due[t_abs * n.n_src + q]) : 0);
           if (b_new > 65535) b_new = 65535;
           if (n.src_group ? (q == pick) : (b_new > 0 && lane_free)) {
             lane_free = false;
@@ -942,6 +949,8 @@ struct tsc_handle {
   float* d_greward = nullptr; uint8_t* d_done = nullptr;
   unsigned long long* d_scalar = nullptr;
   float* d_cg = nullptr;     // per-replica coop_gamma (tsc_set_replica_coop_gamma), allocated on first use
+  // per-replica demand (tsc_set_replica_demand): level of each replica and the level stacks of the three demand tables
+  int32_t* d_level = nullptr; uint8_t* d_lv_due = nullptr; float* d_lv_plo = nullptr; float* d_lv_phi = nullptr;
   int n_nodes = 0, n_obs = 0, max_na = 0, n_det = 0;
   int meas_words = 0;
   // greedy program (tsc_set_greedy_program): CSR over (node, candidate) of observation offsets + action per candidate
@@ -1092,6 +1101,7 @@ extern "C" int tsc_destroy(tsc_handle* h) {
   cudaSetDevice(h->device);
   for (void* p : h->owned) cudaFree(p);
   cudaFree(h->d_gp_off); cudaFree(h->d_gp_idx); cudaFree(h->d_gp_act);
+  cudaFree(h->d_level); cudaFree(h->d_lv_due); cudaFree(h->d_lv_plo); cudaFree(h->d_lv_phi);
   delete h;
   return 0;
 }
@@ -1128,9 +1138,53 @@ extern "C" int tsc_set_replica_coop_gamma(tsc_handle* h, const float* cg_host) {
   return 0;
 }
 
+extern "C" int tsc_set_replica_demand(tsc_handle* h, int32_t n_levels, const uint8_t* due_host, const float* plo_host,
+                                      const float* phi_host, const int32_t* level_host) {
+  if (!h) return fail("tsc_set_replica_demand: null handle");
+  const DevNet& d = h->args.net;
+  const bool stoch = d.src_group != nullptr;
+  const size_t n_due = (size_t)d.horizon * d.n_src, n_p = (size_t)d.n_pint * d.n_src;
+  if (level_host) {             // every check before the current setting is touched
+    if (n_levels <= 0 || !due_host) return fail("tsc_set_replica_demand: bad argument");
+    if (stoch != (plo_host != nullptr) || stoch != (phi_host != nullptr))
+      return fail(stoch ? "tsc_set_replica_demand: the net has stochastic demand (src_group): plo and phi are required"
+                        : "tsc_set_replica_demand: the net has no stochastic demand: plo and phi must be NULL");
+    for (int r = 0; r < h->R; ++r)
+      if (level_host[r] < 0 || level_host[r] >= n_levels)
+        return fail("tsc_set_replica_demand: replica " + std::to_string(r) + " has level " + std::to_string(level_host[r]) +
+                    ", outside [0, " + std::to_string(n_levels) + ")");
+    if ((size_t)n_levels * (n_due > n_p ? n_due : n_p) > (size_t)INT32_MAX)
+      return fail("tsc_set_replica_demand: level tables too large");
+  }
+  CK(cudaSetDevice(h->device));
+  CK(cudaDeviceSynchronize());          // no launch in flight still reads the previous tables
+  cudaFree(h->d_level); cudaFree(h->d_lv_due); cudaFree(h->d_lv_plo); cudaFree(h->d_lv_phi);
+  h->d_level = nullptr; h->d_lv_due = nullptr; h->d_lv_plo = h->d_lv_phi = nullptr;
+  if (!level_host) return 0;
+  int32_t* lv = nullptr; uint8_t* due = nullptr; float* plo = nullptr; float* phi = nullptr;
+  cudaError_t e = cudaMalloc(&lv, (size_t)h->R * 4);
+  if (e == cudaSuccess) e = cudaMalloc(&due, n_levels * n_due + 16);
+  if (e == cudaSuccess && stoch) e = cudaMalloc(&plo, n_levels * n_p * 4 + 16);
+  if (e == cudaSuccess && stoch) e = cudaMalloc(&phi, n_levels * n_p * 4 + 16);
+  if (e == cudaSuccess) e = cudaMemcpy(lv, level_host, (size_t)h->R * 4, cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaMemcpy(due, due_host, n_levels * n_due, cudaMemcpyHostToDevice);
+  if (e == cudaSuccess && stoch) e = cudaMemcpy(plo, plo_host, n_levels * n_p * 4, cudaMemcpyHostToDevice);
+  if (e == cudaSuccess && stoch) e = cudaMemcpy(phi, phi_host, n_levels * n_p * 4, cudaMemcpyHostToDevice);
+  if (e != cudaSuccess) {       // the setting stays cleared
+    cudaFree(lv); cudaFree(due); cudaFree(plo); cudaFree(phi);
+    return fail(std::string("tsc_set_replica_demand: ") + cudaGetErrorString(e));
+  }
+  h->d_level = lv; h->d_lv_due = due; h->d_lv_plo = plo; h->d_lv_phi = phi;
+  return 0;
+}
+
 static int launch(tsc_handle* h, int n_sub, const int32_t* action, const float* fp, float* obs, float* reward,
                   float* greward, uint8_t* done, cudaStream_t st, int rep0 = 0, int count = -1, int sub0 = 0) {
   StepArgs a = h->args;
+  if (h->d_level) {             // per-replica demand: the kernel offsets these stacks by its replica's level
+    a.dlevel = h->d_level; a.net.src_due = h->d_lv_due;
+    if (h->d_lv_plo) { a.net.src_plo = h->d_lv_plo; a.net.src_phi = h->d_lv_phi; }
+  }
   a.n_sub = n_sub; a.action = action; a.fp = fp; a.obs = obs; a.reward = reward; a.greward = greward; a.done = done;
   a.rep0 = rep0;
   if (h->record) {

@@ -3,6 +3,34 @@ scripts/evaluate.py): `make_env` picks the env class from `[ENV_CONFIG]` as main
 the scenario's greedy policy."""
 
 
+# the [ENV_CONFIG] keys that set each scenario's traffic demand and nothing else: two configs that differ only in these
+# build nets that differ only in net.tables.DEMAND_FIELDS, which one simulator takes per replica
+# (BatchedSim.set_replica_demand).  SUMO-file scenarios (any other scenario name with a `net_file`) take `route_file`,
+# accepted only where the other route file keeps every route and source (`check_demand_tables`).
+DEMAND_KEYS = {
+    'large_grid': ('peak_flow1', 'peak_flow2'),
+    'real_net': ('flow_rate',),
+    'small_grid': ('num_extra_car_per_hour',),
+}
+SUMO_FILE_DEMAND_KEYS = ('route_file',)
+
+
+def demand_keys(cfg):
+    """The demand keys (DEMAND_KEYS) of an `[ENV_CONFIG]` section's scenario; () for an unknown scenario."""
+    scen = cfg.get('scenario')
+    if scen in DEMAND_KEYS:
+        return DEMAND_KEYS[scen]
+    return SUMO_FILE_DEMAND_KEYS if cfg.get('net_file', fallback=None) else ()
+
+
+def check_demand_tables(base, other, what, ignore=()):
+    """Refuse (ValueError naming `what` and the field) two nets that differ in more than their demand tables."""
+    from ..net.tables import DEMAND_FIELDS, demand_mismatch
+    f = demand_mismatch(base, other, ignore=ignore)
+    if f is not None:
+        raise ValueError('%s: the net differs in %r, not only in its demand (%s)' % (what, f, ', '.join(DEMAND_FIELDS)))
+
+
 def make_env(cfg, n_replicas, output_path, is_record=True, device=0):
     """The scenario env of an `[ENV_CONFIG]` section (large_grid, real_net, small_grid, or a SUMO-file scenario through
     `net_file`) with `n_replicas` lock-stepped replicas."""

@@ -421,7 +421,8 @@ def load_tables(path: str) -> NetTables:
 def real_net_tables(agent: str = 'ma2c', net_file: str | None = None, flow_rate: int = 325,
                     coop_gamma: float = 0.9) -> NetTables:
     """Tables for the Monaco scenario: parsed from `net_file` when given (a reference checkout),
-    else from the derived table cache shipped with the package (generated by the same code)."""
+    else from the derived table cache shipped with the package (generated by the same code), with the demand table
+    rebuilt at `flow_rate`."""
     if net_file is not None and os.path.exists(net_file):
         return build_real_net(net_file, flow_rate=flow_rate, agent=agent, coop_gamma=coop_gamma)
     path = _CACHE % agent
@@ -429,4 +430,7 @@ def real_net_tables(agent: str = 'ma2c', net_file: str | None = None, flow_rate:
         path = _CACHE % 'ia2c'      # IQL agents observe what IA2C agents do (AGENT_MODES, build_obs_program)
     if not os.path.exists(path):
         raise FileNotFoundError('no Monaco net file given and no derived table cache at %s' % path)
-    return load_tables(path)
+    net = load_tables(path)
+    # the cache holds the reference's 325 veh/h; demand is the only table the flow rate changes (build_real_net)
+    net.src_due = flow_due_table(monaco_flow_list(flow_rate), net.horizon, net.n_src)
+    return net

@@ -233,6 +233,30 @@ class NetTables:
         return c
 
 
+# the tables that carry a scenario's traffic demand: two nets that differ only in these are one simulator with
+# per-replica demand levels (tsc_set_replica_demand, BatchedSim.set_replica_demand)
+DEMAND_FIELDS = ('src_due', 'src_plo', 'src_phi')
+
+
+def _same_value(a, b) -> bool:
+    if isinstance(a, np.ndarray) or isinstance(b, np.ndarray):
+        a, b = np.asarray(a), np.asarray(b)
+        return a.dtype == b.dtype and a.shape == b.shape and np.array_equal(a, b)
+    return a == b
+
+
+def demand_mismatch(a: NetTables, b: NetTables, ignore=()):
+    """The name of the first NetTables field, other than DEMAND_FIELDS and `ignore`, in which `a` and `b` differ, or
+    None when they differ at most in their demand."""
+    import dataclasses
+    for f in dataclasses.fields(NetTables):
+        if f.name in DEMAND_FIELDS or f.name in ignore:
+            continue
+        if not _same_value(getattr(a, f.name), getattr(b, f.name)):
+            return f.name
+    return None
+
+
 # --------------------------------------------------------------------------------------
 # builders shared by all scenarios
 # --------------------------------------------------------------------------------------

@@ -74,6 +74,42 @@ class BatchedSim:
                              "with a coop_gamma other than 1")
         _lib.check(_lib.lib().tsc_set_replica_coop_gamma(self._h, cg.ctypes.data))
 
+    def set_replica_demand(self, levels=None, level_of=None) -> None:
+        """Traffic demand per replica (`tsc_set_replica_demand`): `levels` a list of NetTables that differ from the
+        built net at most in their demand tables (net.tables.DEMAND_FIELDS; anything else is refused, naming the
+        field; under ma2c the observation scale too, which set_replica_coop_gamma sets per replica), `level_of` [R]
+        ints, the level of each replica.  Replica r then steps as a simulator built with levels[level_of[r]].
+        Identical levels are uploaded once.  None returns to the built tables."""
+        from .net.tables import DEMAND_FIELDS, demand_mismatch
+        lib = _lib.lib()
+        if levels is None:
+            _lib.check(lib.tsc_set_replica_demand(self._h, 0, None, None, None, None))
+            return
+        level_of = np.ascontiguousarray(level_of, dtype=np.int64)
+        if level_of.shape != (self.R,):
+            raise ValueError("set_replica_demand takes %d levels of replicas (got shape %s)" % (self.R, level_of.shape))
+        if len(levels) == 0 or level_of.min() < 0 or level_of.max() >= len(levels):
+            raise ValueError("set_replica_demand: every replica's level must index the %d levels" % len(levels))
+        n, stoch = self.net, self.net.n_pint > 0
+        uniq, index = [], []
+        for k, t in enumerate(levels):
+            f = demand_mismatch(n, t, ignore=("obs_scale",) if self.params.agent == "ma2c" else ())
+            if f is not None:
+                raise ValueError("demand level %d differs from the built net in %r, not only in its demand" % (k, f))
+            key = tuple(np.asarray(getattr(t, name)).tobytes() for name in DEMAND_FIELDS)
+            if key not in [u[0] for u in uniq]:
+                uniq.append((key, t))
+            index.append([u[0] for u in uniq].index(key))
+        due = np.ascontiguousarray(np.stack([np.asarray(t.src_due, np.uint8).reshape(n.horizon, n.n_src)
+                                             for _, t in uniq]))
+        plo = phi = None
+        if stoch:
+            plo = np.ascontiguousarray(np.stack([np.asarray(t.src_plo, np.float32) for _, t in uniq]))
+            phi = np.ascontiguousarray(np.stack([np.asarray(t.src_phi, np.float32) for _, t in uniq]))
+        lv = np.ascontiguousarray(np.asarray(index, np.int32)[level_of])
+        _lib.check(lib.tsc_set_replica_demand(self._h, len(uniq), due.ctypes.data, None if plo is None else plo.ctypes.data,
+                                              None if phi is None else phi.ctypes.data, lv.ctypes.data))
+
     def observe(self, fp: Optional[torch.Tensor] = None, obs_out: Optional[torch.Tensor] = None) -> torch.Tensor:
         obs = self.obs if obs_out is None else obs_out
         _lib.check(_lib.lib().tsc_observe(self._h, ptr(fp), ptr(obs), self._stream()))

@@ -141,6 +141,18 @@ int tsc_set_train_mode(tsc_handle* h, int32_t train_mode);
  * with a coop_gamma != 1, else no observation entry is marked as scaled).  NULL returns to cfg->coop_gamma. */
 int tsc_set_replica_coop_gamma(tsc_handle* h, const float* cg_host);
 
+/* Demand per replica (synchronous: synchronises the device, then replaces the previous setting).  n_levels demand
+ * levels of the built net, each given by its three demand tables:
+ *   due_host    uint8 [n_levels][horizon][n_src]        (tsc_net.src_due of that level)
+ *   plo_host    float [n_levels][n_pint][n_src] or NULL (tsc_net.src_plo), phi_host likewise (tsc_net.src_phi):
+ *               given exactly when the net has stochastic demand (src_group)
+ *   level_host  int32 [R] level of each replica, each in [0, n_levels)
+ * Every step / observe / record / host-range call then takes replica r's demand from level level_host[r], so replica
+ * r is bit-identical to a simulator built with that level's tables (all other tables equal).  level_host NULL
+ * returns to the built tables.  */
+int tsc_set_replica_demand(tsc_handle* h, int32_t n_levels, const uint8_t* due_host, const float* plo_host,
+                           const float* phi_host, const int32_t* level_host);
+
 /* Replaces _get_state() without stepping (the observation reset() returns,
  * envs/env.py:561,163-205).  fp_dev: [R][n_nodes][max_na] policy probabilities installed by
  * update_fingerprint (envs/env.py:633-635) or NULL (zeros).  obs_dev: [R][n_obs]. */

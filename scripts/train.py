@@ -32,6 +32,9 @@ replicas (a multiple of 64), all in one lock-step.  The configs may differ only 
 and the [MODEL_CONFIG] learning-rate, entropy, value / gradient-norm, RMSProp, gamma and reward-scaling keys
 (agents/train.py: SWEEP_CONFIG_KEYS).  Member a.ini gets the complete agent directory DIR/a/<agent>/ of
 `train --config-dir a.ini`.  Not with --seeds, and not under torchrun.  The JSON line gains "members".
+With `--vary-demand` the configs may also differ in their scenario's demand keys (peak_flow1 / peak_flow2 for
+large_grid, flow_rate for real_net, num_extra_car_per_hour for small_grid, route_file for SUMO-file scenarios;
+envs.DEMAND_KEYS): each member then trains at its own demand in the shared simulator.
 
 `--deterministic` makes the A2C update add its gradients in a fixed order instead of with atomics, so two runs with the
 same config, seeds, replicas, world size, build and GPU model write the same bytes (checkpoint, CSVs, summaries).  It
@@ -68,6 +71,8 @@ def parse_args(argv=None):
                     help="comma-separated seeds: train one population member per seed into DIR/seed<s>/<agent>/")
     sp.add_argument("--sweep", default=None,
                     help="comma-separated configs: train one sweep member per config into DIR/<config stem>/<agent>/")
+    sp.add_argument("--vary-demand", action="store_true",
+                    help="with --sweep: the configs may also differ in their scenario's traffic demand keys")
     sp.add_argument("--deterministic", action="store_true",
                     help="reproducible A2C training: fixed-order gradient sums in the update")
     a = p.parse_args(argv)
@@ -80,6 +85,8 @@ def parse_args(argv=None):
         a.sweep = [x.strip() for x in a.sweep.split(",") if x.strip()]
         if not a.sweep:
             p.error("--sweep needs at least one config")
+    elif a.vary_demand:
+        p.error("--vary-demand applies to a --sweep")
     if a.seeds is not None:
         from deeprl_signal_control_b200.agents.train import parse_seeds
         try:
@@ -97,7 +104,7 @@ def main(argv=None):
             raise SystemExit("--sweep trains a sweep in one process; it does not run under torchrun")
         from deeprl_signal_control_b200.agents.train import train_sweep
         out = train_sweep(a.sweep, a.base_dir, a.test_mode, n_replicas=a.replicas, summaries=a.summaries,
-                          policy=a.policy, deterministic=a.deterministic)
+                          policy=a.policy, deterministic=a.deterministic, vary_demand=a.vary_demand)
         print(json.dumps({"final_step": out.final_step, "episode_sets": out.episode_sets, "members": out.names,
                           "env_samples": out.env_samples, "replicas": a.replicas, "wall_sec": round(out.wall_sec, 3)}))
         return out

@@ -3,7 +3,7 @@ train.py: train_iql_population, train_iql_sweep).
 
   python scripts/train_iql_members.py --base-dir DIR (--config-dir CFG.ini --seeds 12,13,... | --sweep a.ini,b.ini,...)
                                       --replicas R_m [--test-mode no_test|in_train_test|after_train_test|all_test]
-                                      [--summaries]
+                                      [--summaries] [--vary-demand]
 
 `--seeds` trains a population: one member per seed (its [ENV_CONFIG] seed) into DIR/seed<s>/<agent>/.  `--sweep` trains
 one member per config into DIR/<config stem>/<agent>/; the configs may differ only in [ENV_CONFIG] seed and the
@@ -11,7 +11,8 @@ one member per config into DIR/<config stem>/<agent>/; the configs may differ on
 Every member trains on `--replicas` replicas; all members share one simulator, one replay ring and one grouped
 ε-greedy forward and TD / Adam update, and each member's directory is the one `scripts/train.py train` leaves for it
 alone, bit for bit.  At most 64 members; not under torchrun.  Prints one JSON line as scripts/train.py does, with
-"seeds" or "members".
+"seeds" or "members".  `--vary-demand` (with --sweep) lets the configs also differ in their scenario's demand keys
+(envs.DEMAND_KEYS, as `scripts/train.py train --sweep ... --vary-demand`).
 """
 import argparse
 import json
@@ -34,6 +35,8 @@ def parse_args(argv=None):
                    choices=["no_test", "in_train_test", "after_train_test", "all_test"])
     p.add_argument("--summaries", action="store_true",
                    help="also write the reference's TensorBoard event file into each member's log/")
+    p.add_argument("--vary-demand", action="store_true",
+                   help="with --sweep: the configs may also differ in their scenario's traffic demand keys")
     a = p.parse_args(argv)
     if (a.seeds is None) == (a.sweep is None):
         p.error("give exactly one of --seeds (with --config-dir) and --sweep")
@@ -46,6 +49,8 @@ def parse_args(argv=None):
     else:
         if a.config_dir is None:
             p.error("--seeds needs --config-dir")
+        if a.vary_demand:
+            p.error("--vary-demand applies to a --sweep")
         from deeprl_signal_control_b200.agents.train import parse_seeds
         try:
             a.seeds = parse_seeds(a.seeds)
@@ -60,7 +65,8 @@ def main(argv=None):
         raise SystemExit("train_iql_members.py trains its members in one process; it does not run under torchrun")
     from deeprl_signal_control_b200.agents.train import train_iql_population, train_iql_sweep
     if a.sweep is not None:
-        out = train_iql_sweep(a.sweep, a.base_dir, a.test_mode, n_replicas=a.replicas, summaries=a.summaries)
+        out = train_iql_sweep(a.sweep, a.base_dir, a.test_mode, n_replicas=a.replicas, summaries=a.summaries,
+                              vary_demand=a.vary_demand)
         key, val = "members", out.names
     else:
         out = train_iql_population(a.config_dir, a.base_dir, a.seeds, a.test_mode, n_replicas=a.replicas,
