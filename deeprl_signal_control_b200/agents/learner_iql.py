@@ -366,13 +366,15 @@ class BatchedIQLTrainer:
     run calls it; it resets member k's replicas with its solo run's seeds (`member_episode_seeds`; seed0 and replica0 are
     not used), keeps summary_rec [ceil(T_episode / n_step), K, N_ROUNDS, A, 4] and appends the list of the K members'
     episode means to `episode_rewards`; `member(k)` is member k's view for the training driver.  `demand`: as in
-    `BatchedTrainer`, one NetTables per member whose demand member k's replicas take."""
+    `BatchedTrainer`, one NetTables per member whose demand member k's replicas take.  `demand_mix`: as in
+    `BatchedTrainer`, the L levels of a mixture, global replica g at level g mod L."""
 
     def __init__(self, sim, model: BatchedIQL, lr_sched, eps_sched, seed0: int = 12, replica0: int = 0,
-                 greward_trace=None, summary_rec=None, demand=None):
-        from .trainer import _check_rec, _check_trace, set_member_demand
+                 greward_trace=None, summary_rec=None, demand=None, demand_mix=None):
+        from .trainer import _check_rec, _check_trace, set_member_demand, set_mix_demand
         self.K = model.K
         set_member_demand(sim, demand, self.K)
+        set_mix_demand(sim, demand_mix, replica0)
         if self.K > 1 and (len(lr_sched) != self.K or len(eps_sched) != self.K):
             raise ValueError('a learner with %d members takes one lr and one ε schedule per member' % self.K)
         self.sim, self.model = sim, model

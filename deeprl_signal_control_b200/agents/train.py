@@ -34,6 +34,7 @@ from __future__ import annotations
 
 import configparser
 import hashlib
+import json
 import logging
 import os
 import shutil
@@ -179,6 +180,10 @@ def training_row(rewards):
     return float(rewards.mean(axis=0).mean()), float(np.std(rewards))
 
 
+# data/train_reward_demand.csv of a run on a mixture of demand levels: train_reward.csv's columns and the level's label
+DEMAND_ROW_COLUMNS = ('agent', 'step', 'test_id', 'demand', 'avg_reward', 'std_reward')
+
+
 class Trainer:
     """utils.py:Trainer.run / Tester.run_offline over a batched trainer (`run(n)`, `T_episode`, `episode_rewards`,
     `greward_trace` [T_episode, R]) and a batched `Evaluator` (`perform_all()`, `run()`, `env`).
@@ -188,15 +193,21 @@ class Trainer:
     CSV, and all ranks meet at a barrier after each test.
     `summary`: None, or the `Summaries` of the run (the trainer then keeps a `summary_rec`).
     `log_extra`: the `extra` of its log records (a population member's tag, see `train_population`).
+    `levels`: a run on a mixture of L demand levels (`demand_mix_levels`), a list of (label, evaluator at that level or
+    None); global replica g runs at level g mod L.  The driver then also keeps `level_data`, the rows of
+    `train_reward_demand.csv`: per episode set one training row per level (`training_row` over that level's columns of
+    the [T, R_total] trace), per test one row per level and seed, and the post-training test writes each level's CSVs
+    into <output_path>/<label>/.
     `run_schedule` runs one schedule for several drivers that share a batched trainer and counter."""
 
     def __init__(self, trainer, evaluator, counter: Counter, agent: str, run_test: bool, output_path: str,
-                 group=None, summary=None, log_extra=None):
+                 group=None, summary=None, log_extra=None, levels=None):
         if trainer.greward_trace is None:
             raise ValueError('the driver needs the trainer to keep a greward_trace')
         self.trainer, self.evaluator, self.counter = trainer, evaluator, counter
         self.agent, self.run_test, self.output_path = agent, run_test, output_path
         self.group, self.summary = group, summary
+        self.levels, self.level_data, self.level_post = levels, [], None
         self.log_extra = dict(log_extra or {})
         if group is None:
             self.rank0 = True
@@ -226,6 +237,14 @@ class Trainer:
                          extra=self.log_extra)
             if self.summary is not None:
                 self.summary.test_reward(float(np.mean(mean)), step)
+            for label, ev in self.levels or ():
+                t0 = time.time()
+                mean, std = ev.perform_all()
+                for k in range(len(mean)):
+                    self.level_data.append({'agent': self.agent, 'step': step, 'test_id': k, 'demand': label,
+                                            'avg_reward': float(mean[k]), 'std_reward': float(std[k])})
+                logging.info('Testing: global step %d, demand %s, avg R: %.2f (%.2f s)'
+                             % (step, label, np.mean(mean), time.time() - t0), extra=self.log_extra)
         self._barrier()
 
     def run(self):
@@ -245,6 +264,14 @@ class Trainer:
                 return
             mean, std = training_row(rewards)
         self.data.append({'agent': self.agent, 'step': step, 'test_id': -1, 'avg_reward': mean, 'std_reward': std})
+        if self.levels is not None:
+            from .trainer import mix_level_of
+            L = len(self.levels)
+            level_of = mix_level_of(0, rewards.shape[1], L)
+            for j, (label, _) in enumerate(self.levels):
+                m, s = training_row(rewards[:, level_of == j])
+                self.level_data.append({'agent': self.agent, 'step': step, 'test_id': -1, 'demand': label,
+                                        'avg_reward': m, 'std_reward': s})
         if self.summary is not None:
             self.summary.episode_set(rec, self.trainer.summary_ran, prev, step, mean)
         if c.should_log(prev):
@@ -255,16 +282,29 @@ class Trainer:
         if self.rank0:
             import pandas as pd
             pd.DataFrame(self.data).to_csv(self.output_path + 'train_reward.csv')
+            if self.levels is not None:
+                pd.DataFrame(self.level_data, columns=DEMAND_ROW_COLUMNS).to_csv(
+                    self.output_path + 'train_reward_demand.csv')
 
     def run_offline(self):
-        """Tester.run_offline: every test seed in record mode, the three CSVs into output_path.  Returns the per-seed
-        (mean, std) on rank 0, None on the other ranks."""
+        """Tester.run_offline: every test seed in record mode, the three CSVs into output_path (and, on a mixture of
+        demand levels, each level's into output_path/<label>/, its (mean, std) into `level_post`).  Returns the
+        per-seed (mean, std) on rank 0, None on the other ranks."""
         out = None
         if self.rank0:
             self.evaluator.env.init_data(True, False, self.output_path)
             mean, std = self.evaluator.run()
             logging.info('Offline testing: avg R: %.2f' % np.mean(mean), extra=self.log_extra)
             out = mean, std
+            if self.levels is not None:
+                self.level_post = []
+                for label, ev in self.levels:
+                    path = os.path.join(self.output_path, label) + os.sep
+                    os.makedirs(path, exist_ok=True)
+                    ev.env.init_data(True, False, path)
+                    self.level_post.append(ev.run())
+                    logging.info('Offline testing: demand %s, avg R: %.2f' % (label, np.mean(self.level_post[-1][0])),
+                                 extra=self.log_extra)
         self._barrier()
         return out
 
@@ -344,8 +384,55 @@ def member_dir(base_dir, seed, agent):
     return os.path.join(base_dir, 'seed%d' % int(seed), agent)
 
 
+def demand_mix_levels(config, demand_mix, n_replicas):
+    """The L levels of a run on a mixture of demand levels, checked before any directory or device work: a namespace
+    with `levels` (the {[ENV_CONFIG] key: value} dicts, in order), `labels` (envs.demand_label), `configs` (`config`
+    edited to each level; a key a level leaves out keeps the config's value) and `nets` (each level's NetTables, built
+    on the host).  Refused with a ValueError naming the level, key or count: no level, a scenario without demand keys,
+    a key outside the scenario's envs.DEMAND_KEYS, a level that repeats another (same values of every demand key), a
+    level whose net differs from the config's in more than its demand tables (`check_demand_tables`), and a replica
+    count that is not a multiple of L (each level weighs the same in every gradient)."""
+    import copy
+    from ..envs import check_demand_tables, demand_keys, demand_label, make_env
+    levels = [dict((str(k), str(v)) for k, v in dict(lv).items()) for lv in demand_mix]
+    if not levels:
+        raise ValueError('demand_mix: a mixture needs at least one demand level')
+    env_cfg = config['ENV_CONFIG']
+    keys = demand_keys(env_cfg)
+    if not keys:
+        raise ValueError('demand_mix: the scenario %r has no demand keys, so it has no demand levels to mix'
+                         % env_cfg.get('scenario'))
+    labels = [demand_label(lv) for lv in levels]
+    cfgs, values = [], []
+    for j, lv in enumerate(levels):
+        for key in lv:
+            if key not in keys:
+                raise ValueError('demand level %s: %r is not a demand key of the scenario %r (demand keys: %s)'
+                                 % (labels[j], key, env_cfg.get('scenario'), ', '.join(keys)))
+        c = copy.deepcopy(config)
+        for key, v in lv.items():
+            c['ENV_CONFIG'][key] = v
+        vals = [c['ENV_CONFIG'].get(key, fallback=None) for key in keys]
+        for i, prev in enumerate(values):
+            if all(_same(a, b) for a, b in zip(prev, vals)):
+                raise ValueError('demand level %s repeats level %s: a mixture takes each level once'
+                                 % (labels[j], labels[i]))
+        cfgs.append(c)
+        values.append(vals)
+    L = len(levels)
+    if int(n_replicas) % L:
+        raise ValueError('%d replicas do not split evenly over %d demand levels: n_replicas must be a multiple of %d'
+                         % (int(n_replicas), L, L))
+    base = make_env(env_cfg, 1, '', is_record=False)._tables
+    nets = []
+    for c, label in zip(cfgs, labels):
+        nets.append(make_env(c['ENV_CONFIG'], 1, '', is_record=False)._tables)
+        check_demand_tables(base, nets[-1], 'demand level %s' % label)
+    return types.SimpleNamespace(levels=levels, labels=labels, configs=cfgs, nets=nets)
+
+
 def train(config, base_dir, test_mode='no_test', n_replicas=1, policy='lstm', device=0, process_group=None,
-          summaries=False, seeds=None, deterministic=False):
+          summaries=False, seeds=None, deterministic=False, demand_mix=None):
     """main.py train.  `config`: the path of a reference config (copied into data/) or a parsed ConfigParser (written
     to data/config.ini), with [ENV_CONFIG], [MODEL_CONFIG] and [TRAIN_CONFIG].  Returns a namespace with final_step,
     episode_sets, env_samples (= final_step * n_replicas), wall_sec, world, rank, data (the train_reward.csv rows),
@@ -371,9 +458,24 @@ def train(config, base_dir, test_mode='no_test', n_replicas=1, policy='lstm', de
     `deterministic`: the A2C update adds its gradients, loss sums and clip norms in a fixed order
     (`BatchedA2C(deterministic=True)`), so two runs with the same config, seeds, replicas, world size, build and GPU
     model leave the same bits: checkpoint, CSVs and summaries.  The LSTM policy only (refused for policy='fc' before any
-    directory is made); a no-op for IQL, whose update is already reproducible."""
+    directory is made); a no-op for IQL, whose update is already reproducible.
+
+    `demand_mix`: train the one agent on a mixture of traffic demand levels, a list of L {[ENV_CONFIG] demand key:
+    value} dicts (`demand_mix_levels` checks them, on every rank, before any directory or device work).  Global replica
+    g runs at level g mod L (the config edited to that level; a key a level leaves out keeps the config's value), so
+    n_replicas must be a multiple of L.  The directory holds what it holds without a mixture, with the same meaning:
+    the config (at its own demand), train_reward.csv (training rows pooled over every replica, test rows at the
+    config's demand), the checkpoint and the post-training CSVs.  Added: data/demand_mix.json (the levels and their
+    labels), data/train_reward_demand.csv (`DEMAND_ROW_COLUMNS`: one training row per level and episode set, one row
+    per level and seed per in-training test) and, with a post-training test, each level's three CSVs in
+    data/<label>/.  Not with `seeds`."""
     if deterministic and policy != 'lstm':
         raise ValueError("deterministic=True needs the LSTM policy's lean update (got policy=%r)" % (policy,))
+    mix = None
+    if demand_mix is not None:
+        if seeds is not None:
+            raise ValueError('demand_mix trains one agent: it does not combine with seeds (a population)')
+        mix = demand_mix_levels(_read_config(config)[0], demand_mix, n_replicas)
     if seeds is not None:
         if process_group is not None:
             raise ValueError('a population trains in one process: seeds and process_group exclude each other')
@@ -404,8 +506,11 @@ def train(config, base_dir, test_mode='no_test', n_replicas=1, policy='lstm', de
             path, config = config, configparser.ConfigParser()
             if not config.read(path):
                 raise FileNotFoundError(path)
+        if mix is not None and rank == 0:
+            with open(os.path.join(dirs['data'], 'demand_mix.json'), 'w') as f:
+                json.dump({'levels': mix.levels, 'labels': mix.labels}, f, indent=1)
         out = _train(config, dirs, in_test, post_test, int(n_replicas), policy, device, pg, bool(summaries),
-                     bool(deterministic))
+                     bool(deterministic), mix)
     finally:
         for h in handlers:
             logging.getLogger().removeHandler(h)
@@ -461,7 +566,8 @@ def _schedule(config, env):
     return total_step, counter, T
 
 
-def _train(config, dirs, in_test, post_test, R_total, policy, device, pg, summaries=False, deterministic=False):
+def _train(config, dirs, in_test, post_test, R_total, policy, device, pg, summaries=False, deterministic=False,
+           mix=None):
     import torch
     from ..envs import make_env
     from .evaluator import Evaluator
@@ -476,6 +582,10 @@ def _train(config, dirs, in_test, post_test, R_total, policy, device, pg, summar
     env = make_env(env_cfg, R, dirs['data'], is_record=False, device=device)
     logging.info('Training: s dim: %d, s dim ls: %r, a dim ls: %r, replicas: %d'
                  % (env.n_s, env.n_s_ls, env.n_a_ls, R_total) + (' over %d ranks' % world if world > 1 else ''))
+    if mix is not None:
+        logging.info('Training: %d demand levels %s, replica g at level g mod %d'
+                     % (len(mix.labels), mix.labels, len(mix.labels)))
+    mix_nets = None if mix is None else mix.nets
     total_step, counter, T = _schedule(config, env)
     seed = env_cfg.getint('seed')
     group, own_group = host_group(pg) if pg is not None else (None, False)
@@ -505,16 +615,24 @@ def _train(config, dirs, in_test, post_test, R_total, policy, device, pg, summar
             from .models import iql_schedulers
             lr_s, eps_s = iql_schedulers(mc, total_step)
             trainer = BatchedIQLTrainer(sim, model, lr_s, eps_s, seed0=seed, replica0=replica0, greward_trace=trace,
-                                        **srec)
+                                        demand_mix=mix_nets, **srec)
         else:
             from .trainer import BatchedTrainer
             trainer = BatchedTrainer(sim, model.batched, agent, model.lr_scheduler, model.beta_scheduler, seed0=seed,
-                                     replica0=replica0, greward_trace=trace, **srec)
+                                     replica0=replica0, greward_trace=trace, demand_mix=mix_nets, **srec)
         evaluator = None
+        levels = None if mix is None else [(label, None) for label in mix.labels]
         if (in_test or post_test) and rank == 0:
             test_env = make_env(env_cfg, len(env.test_seeds), dirs['data'], is_record=False, device=device)
             evaluator = Evaluator(test_env, model, dirs['data'], policy_type='default')
-        driver = Trainer(trainer, evaluator, counter, agent, in_test, dirs['data'], group=group, summary=summary)
+            if mix is not None:                     # one evaluator per level, on the config edited to that level
+                levels = []
+                for label, c in zip(mix.labels, mix.configs):
+                    path = os.path.join(dirs['data'], label) + os.sep
+                    lv_env = make_env(c['ENV_CONFIG'], len(env.test_seeds), path, is_record=False, device=device)
+                    levels.append((label, Evaluator(lv_env, model, path, policy_type='default')))
+        driver = Trainer(trainer, evaluator, counter, agent, in_test, dirs['data'], group=group, summary=summary,
+                         levels=levels)
         driver.run()
         final_step = counter.cur_step
         if group is not None:
@@ -533,7 +651,8 @@ def _train(config, dirs, in_test, post_test, R_total, policy, device, pg, summar
     return types.SimpleNamespace(final_step=final_step, episode_sets=driver.n_episode_sets,
                                  env_samples=final_step * R_total, world=world, rank=rank,
                                  data=driver.data if rank == 0 else None, post_test=post, model=model,
-                                 trainer=trainer)
+                                 trainer=trainer, demand_data=driver.level_data if mix is not None and rank == 0 else None,
+                                 demand_post_test=driver.level_post)
 
 
 def _member_filter(k):

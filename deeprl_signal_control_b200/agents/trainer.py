@@ -88,10 +88,25 @@ def set_member_demand(sim, demand, K):
     sim.set_replica_demand(list(demand), np.repeat(np.arange(K), sim.R // K))
 
 
+def mix_level_of(replica0, R, L):
+    """The demand level of replicas [replica0, replica0 + R) of a run on a mixture of L levels: global replica g runs at
+    level g mod L, so that every rank and every 64-replica tile holds every level."""
+    return (int(replica0) + np.arange(int(R))) % int(L)
+
+
+def set_mix_demand(sim, demand_mix, replica0=0):
+    """One agent on a mixture of demand levels (a list of L NetTables): this simulator's replica r, global replica
+    replica0 + r, takes its demand from demand_mix[(replica0 + r) mod L] (`mix_level_of`); None leaves the simulator's
+    built demand."""
+    if demand_mix is None:
+        return
+    sim.set_replica_demand(list(demand_mix), mix_level_of(replica0, sim.R, len(demand_mix)))
+
+
 class BatchedTrainer:
     def __init__(self, sim: BatchedSim, model: BatchedA2C, agent: str, lr, beta,
                  seed0: int = 12, replica0: int = 0, greward_trace: Optional[torch.Tensor] = None,
-                 summary_rec: Optional[torch.Tensor] = None, coop_gamma=None, demand=None):
+                 summary_rec: Optional[torch.Tensor] = None, coop_gamma=None, demand=None, demand_mix=None):
         """lr / beta: floats (the 'constant' schedules of every shipped A2C config) or objects with the reference's
         `Scheduler.get(n_step)` (agents/utils.py:268-281, agents/models.py:175-176); a schedule advances by n_step per
         update exactly as in the reference (its unit is control steps of ONE environment).
@@ -106,8 +121,11 @@ class BatchedTrainer:
         A sweep (a learner with `hparams`) passes lr / beta as lists with one schedule per member (`schedule_values`),
         and `coop_gamma`, one MA2C spatial discount per member: member k's replicas then step with its own
         (BatchedSim.set_replica_coop_gamma), and `demand`, one NetTables per member: member k's replicas then take
-        their traffic demand from demand[k] (BatchedSim.set_replica_demand)."""
+        their traffic demand from demand[k] (BatchedSim.set_replica_demand).
+        demand_mix: one agent trained on a mixture of demand levels, a list of L NetTables; global replica g (this
+        simulator's replica g - replica0) runs at level g mod L (`set_mix_demand`)."""
         set_member_demand(sim, demand, int(getattr(model, "K", 1)))
+        set_mix_demand(sim, demand_mix, replica0)
         if coop_gamma is not None:
             K, R_m = int(getattr(model, "K", 1)), sim.R // int(getattr(model, "K", 1))
             if len(coop_gamma) != K:

@@ -23,6 +23,32 @@ def demand_keys(cfg):
     return SUMO_FILE_DEMAND_KEYS if cfg.get('net_file', fallback=None) else ()
 
 
+def parse_demand(text, option='--demand'):
+    """'k=v,k=v' -> {k: v} (in the given order), the value of the command-line `option` that names one demand level.
+    Refuses an empty level, a pair without '=' and a repeated key."""
+    out = {}
+    for pair in text.split(","):
+        pair = pair.strip()
+        if not pair:
+            continue
+        key, sep, val = pair.partition("=")
+        key, val = key.strip(), val.strip()
+        if not sep or not key or not val:
+            raise ValueError("%s takes KEY=VALUE pairs separated by ',' (got %r)" % (option, text))
+        if key in out:
+            raise ValueError("%s %r names %s twice" % (option, text, key))
+        out[key] = val
+    if not out:
+        raise ValueError("%s %r names no key" % (option, text))
+    return out
+
+
+def demand_label(level):
+    """The directory name of a demand level: its key-value pairs joined by '_' (peak_flow1-1400_peak_flow2-1180)."""
+    import os
+    return "_".join("%s-%s" % (k, os.path.basename(v) if k == "route_file" else v) for k, v in level.items())
+
+
 def check_demand_tables(base, other, what, ignore=()):
     """Refuse (ValueError naming `what` and the field) two nets that differ in more than their demand tables."""
     from ..net.tables import DEMAND_FIELDS, demand_mismatch

@@ -36,6 +36,8 @@ import time
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
+from deeprl_signal_control_b200.envs import demand_label, parse_demand  # noqa: E402,F401
+
 # main.py:40-41: the reference's default evaluation seeds
 DEFAULT_SEEDS = ",".join(str(s) for s in range(10000, 100001, 10000))
 SUMMARY_COLUMNS = ("mean_reward", "std_reward", "avg_queue", "avg_speed_mps", "avg_wait_sec", "mean_trips")
@@ -62,30 +64,6 @@ def parse_args(argv=None):
         if len(set(labels)) != len(labels):
             p.error("repeated --demand levels: %s" % labels)
     return a
-
-
-def parse_demand(text):
-    """'k=v,k=v' -> {k: v} (in the given order).  Refuses an empty level, a pair without '=' and a repeated key."""
-    out = {}
-    for pair in text.split(","):
-        pair = pair.strip()
-        if not pair:
-            continue
-        key, sep, val = pair.partition("=")
-        key, val = key.strip(), val.strip()
-        if not sep or not key or not val:
-            raise ValueError("--demand takes KEY=VALUE pairs separated by ',' (got %r)" % text)
-        if key in out:
-            raise ValueError("--demand %r names %s twice" % (text, key))
-        out[key] = val
-    if not out:
-        raise ValueError("--demand %r names no key" % text)
-    return out
-
-
-def demand_label(level):
-    """The output directory name of a demand level: its key-value pairs joined by '_' (peak_flow1-1400_peak_flow2-1180)."""
-    return "_".join("%s-%s" % (k, os.path.basename(v) if k == "route_file" else v) for k, v in level.items())
 
 
 def entries(base_dir, agents, levels=None):

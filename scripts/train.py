@@ -39,6 +39,15 @@ envs.DEMAND_KEYS): each member then trains at its own demand in the shared simul
 `--deterministic` makes the A2C update add its gradients in a fixed order instead of with atomics, so two runs with the
 same config, seeds, replicas, world size, build and GPU model write the same bytes (checkpoint, CSVs, summaries).  It
 combines with every option above; the LSTM policy only, and a no-op for IQL (its update is already reproducible).
+
+`--train-demand peak_flow1=660,peak_flow2=555` (repeatable, once per level) trains the one agent on a mixture of
+traffic demand levels: of the --replicas replicas (a multiple of the number of levels L), replica g runs at level
+g mod L, on one process or under torchrun.  Levels are written as for `scripts/evaluate_agents.py --demand`: the keys of
+the scenario's envs.DEMAND_KEYS; a key a level leaves out keeps the config's value.  The directory is the usual one
+(test rows and post-training CSVs at the config's own demand) plus data/demand_mix.json, data/train_reward_demand.csv
+(per-level training and test rows) and, with a post-training test, each level's CSVs in data/<label>/, label as in
+evaluate_agents.py (peak_flow1-660_peak_flow2-555).  Not with --seeds, --sweep or --vary-demand.  The JSON line gains
+"demand", the labels.
 """
 import argparse
 import datetime
@@ -47,6 +56,8 @@ import os
 import sys
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+from deeprl_signal_control_b200.envs import demand_label, parse_demand  # noqa: E402
 
 # The longest wait at a collective is the other ranks' at the barrier while rank 0 runs a test; a rank that fails ends
 # the run after this long instead of leaving the others waiting.
@@ -75,10 +86,24 @@ def parse_args(argv=None):
                     help="with --sweep: the configs may also differ in their scenario's traffic demand keys")
     sp.add_argument("--deterministic", action="store_true",
                     help="reproducible A2C training: fixed-order gradient sums in the update")
+    sp.add_argument("--train-demand", action="append", default=None, metavar="KEY=VALUE[,KEY=VALUE...]",
+                    help="a demand level (repeatable): train the one agent on a mixture of the levels given")
     a = p.parse_args(argv)
     if not a.option:
         p.print_help()
         raise SystemExit(1)
+    if a.train_demand is not None:
+        for opt, given in (("--seeds", a.seeds is not None), ("--sweep", a.sweep is not None),
+                           ("--vary-demand", a.vary_demand)):
+            if given:
+                p.error("--train-demand and %s exclude each other (a mixture trains one agent)" % opt)
+        try:
+            a.train_demand = [parse_demand(t, "--train-demand") for t in a.train_demand]
+        except ValueError as e:
+            p.error(str(e))
+        labels = [demand_label(lv) for lv in a.train_demand]
+        if len(set(labels)) != len(labels):
+            p.error("repeated --train-demand levels: %s" % labels)
     if a.sweep is not None:
         if a.seeds is not None:
             p.error("--sweep and --seeds exclude each other (a sweep takes each member's seed from its config)")
@@ -117,12 +142,14 @@ def main(argv=None):
         print(json.dumps({"final_step": out.final_step, "episode_sets": out.episode_sets, "seeds": out.seeds,
                           "env_samples": out.env_samples, "replicas": a.replicas, "wall_sec": round(out.wall_sec, 3)}))
         return out
+    mix = {} if a.train_demand is None else {"demand": [demand_label(lv) for lv in a.train_demand]}
     if world <= 1:
         from deeprl_signal_control_b200.agents.train import train
         out = train(a.config_dir, a.base_dir, a.test_mode, n_replicas=a.replicas, policy=a.policy,
-                    summaries=a.summaries, deterministic=a.deterministic)
-        print(json.dumps({"final_step": out.final_step, "episode_sets": out.episode_sets,
-                          "env_samples": out.env_samples, "replicas": a.replicas, "wall_sec": round(out.wall_sec, 3)}))
+                    summaries=a.summaries, deterministic=a.deterministic, demand_mix=a.train_demand)
+        print(json.dumps(dict({"final_step": out.final_step, "episode_sets": out.episode_sets,
+                               "env_samples": out.env_samples, "replicas": a.replicas,
+                               "wall_sec": round(out.wall_sec, 3)}, **mix)))
         return out
     local_rank = int(os.environ["LOCAL_RANK"])
     from deeprl_signal_control_b200.dist import bind_to_gpu_numa
@@ -135,13 +162,14 @@ def main(argv=None):
     try:
         from deeprl_signal_control_b200.agents.train import train
         out = train(a.config_dir, a.base_dir, a.test_mode, n_replicas=a.replicas, policy=a.policy, device=local_rank,
-                    process_group=dist.group.WORLD, summaries=a.summaries, deterministic=a.deterministic)
+                    process_group=dist.group.WORLD, summaries=a.summaries, deterministic=a.deterministic,
+                    demand_mix=a.train_demand)
     finally:
         dist.destroy_process_group()
     if out.rank == 0:
-        print(json.dumps({"final_step": out.final_step, "episode_sets": out.episode_sets,
-                          "env_samples": out.env_samples, "replicas": a.replicas, "world": world,
-                          "wall_sec": round(out.wall_sec, 3)}))
+        print(json.dumps(dict({"final_step": out.final_step, "episode_sets": out.episode_sets,
+                               "env_samples": out.env_samples, "replicas": a.replicas, "world": world,
+                               "wall_sec": round(out.wall_sec, 3)}, **mix)))
     return out
 
 
