@@ -8,14 +8,15 @@ episode the one-replica env plays after `reset(test_ind=k)` (seed `test_seeds[k]
 mode `output_data()` writes the control / traffic / trip CSVs with the rows, in the order, that the one-replica env
 writes when it runs the seeds one after another.  `model` is an IA2C / MA2C wrapper (agents/models.py; only its
 parameters `batched.P` and the packed image `batched.Wp` are read), an IQL (`model.name == 'iql'`, LR or DQN; only its
-`nets` are read, packed into the evaluator's own parameter vector at the start of every perform_all()) or a greedy
-controller (`model.name == 'greedy'`).
+`nets` are read, packed into the evaluator's own parameter vector at the start of every perform_all()), a greedy
+controller (`model.name == 'greedy'`) or the max-pressure controller (`model.name == 'maxpressure'`,
+envs.maxpressure_controller; nothing of it is read).
 
 Per control step, with no host synchronisation inside the episode: the pi-only forward (tscl_policy_step_pi for the
 fused tensor-core widths; the v1 forward or the fc-policy kernels, then tscl_argmax_actions, otherwise), the fp32 Q
-forward tscl_q_step (IQL: argmax of q, or the normalised-q sample of IQL.forward(stochastic=True)) or
-tsc_greedy_actions; for MA2C the fingerprint is the pi just computed; tsc_step (tsc_step_record in record mode); the
-global reward goes into a [T][R] float32 trace.  The evaluator owns every buffer it writes, so a live learner's
+forward tscl_q_step (IQL: argmax of q, or the normalised-q sample of IQL.forward(stochastic=True)),
+tsc_greedy_actions or tsc_pressure_actions; for MA2C the fingerprint is the pi just computed; tsc_step
+(tsc_step_record in record mode); the global reward goes into a [T][R] float32 trace.  The evaluator owns every buffer it writes, so a live learner's
 parameters, optimiser slot, recurrent states, rollout and counters are left as they were.
 
 `GroupEvaluator` evaluates several agent directories on the same seeds in one process (the reference's `main.py evaluate
@@ -138,12 +139,16 @@ class Evaluator:
             _lib.check(_lib.lib().tsc_set_greedy_program(
                 sim._h, max_cand, off.ctypes.data, idx.ctypes.data, act.ctypes.data))
             return
+        if name == 'maxpressure':
+            self.family = 'maxpressure'
+            return
         if name == 'iql':
             self._init_q(model, net)
             return
         b = getattr(model, 'batched', None)
         if b is None or name not in ('ia2c', 'ma2c'):
-            raise ValueError("Evaluator: batched evaluation covers the greedy controller, IA2C / MA2C and IQL; %r stays on "
+            raise ValueError("Evaluator: batched evaluation covers the greedy and max-pressure controllers, IA2C / MA2C and "
+                             "IQL; %r stays on "
                              "the one-replica protocol" % (name,))
         L = b.lay
         if L.n_obs != self.n_obs or not np.array_equal(L.obs_off, np.asarray(net.node_obs_off[:L.A])):
@@ -203,6 +208,9 @@ class Evaluator:
         lib = _lib.lib()
         if self.greedy:
             _lib.check(lib.tsc_greedy_actions(self.sim._h, _p(self.obs), _p(self.act), self._st()))
+            return None
+        if self.family == 'maxpressure':
+            _lib.check(lib.tsc_pressure_actions(self.sim._h, _p(self.act), self._st()))
             return None
         if self.family == 'q':
             _lib.check(lib.tscl_q_step(self._qh, _p(self.params), _p(self.obs), self.R, _p(self.q), _p(self.act),
@@ -326,9 +334,9 @@ MAX_GROUP_REPLICAS = 1 << 16
 
 
 def entry_model(agent):
-    """The model an agent directory's name selects (main.py:179-190, scripts/evaluate.py): 'greedy', 'ia2c', 'ma2c',
-    'a2c', 'iqld' -> IQL 'dqn', any other name -> IQL 'lr'."""
-    if agent in ('greedy', 'ia2c', 'ma2c', 'a2c'):
+    """The model an agent directory's name selects (main.py:179-190, scripts/evaluate.py): 'greedy', 'maxpressure',
+    'ia2c', 'ma2c', 'a2c', 'iqld' -> IQL 'dqn', any other name -> IQL 'lr'."""
+    if agent in ('greedy', 'maxpressure', 'ia2c', 'ma2c', 'a2c'):
         return agent
     return 'dqn' if agent == 'iqld' else 'lr'
 
@@ -391,12 +399,14 @@ class GroupEvaluator:
         GroupEvaluator(entries, seeds, policy_type='default', policy='lstm').run()
 
     `entries`: (agent directory, model, output path) triples, model as entry_model gives it.  The constructor only
-    checks and groups, on the host: an entry whose directory, config or checkpoint is missing is logged as an error and
-    skipped (`skipped`); an `a2c` entry, or a simulator whose combined replicas exceed MAX_GROUP_REPLICAS, is refused
+    checks and groups, on the host: an entry whose directory, config or checkpoint (none for greedy and maxpressure) is
+    missing is logged as an error and skipped (`skipped`); an `a2c` entry, or a simulator whose combined replicas exceed MAX_GROUP_REPLICAS, is refused
     with a ValueError naming the entry.  Entries whose simulators would be built identically (sim_key) share one
     simulator, len(seeds) consecutive replicas per entry.  Per control step of a shared simulator: one
     tscl_policy_step_pi_g for the v2-family A2C members of one layout, one tscl_q_step_g per IQL layout (LR / DQN),
-    tsc_greedy_actions, the v1 / fc A2C members' own forwards on their row slices, and one tsc_step (tsc_step_record).
+    tsc_greedy_actions, tsc_pressure_actions, the v1 / fc A2C members' own forwards on their row slices, and one tsc_step
+    (tsc_step_record).  The two controller launches write every row of their simulator, so greedy and maxpressure
+    entries, which would otherwise share one, get a simulator each.
     Each entry's reward trace, frames and summary are those `Evaluator` gives for its directory alone: member k samples
     with its own [ENV_CONFIG] seed and member-local replica index, ma2c members their own coop_gamma
     (tsc_set_replica_coop_gamma).
@@ -435,7 +445,8 @@ class GroupEvaluator:
                 self.entries += [GroupEntry(d, m, oj, demand=lv) for oj, lv in zip(o, levels)]
         for e in self.entries:
             if e.model == 'a2c':
-                raise ValueError("%s: batched evaluation covers greedy, ia2c, ma2c and IQL (got agent 'a2c')" % e.label)
+                raise ValueError("%s: batched evaluation covers greedy, maxpressure, ia2c, ma2c and IQL (got agent 'a2c')"
+                                 % e.label)
         self.skipped = []
         for e in self.entries:
             inis = sorted(glob.glob(os.path.join(e.agent_dir, 'data', '*.ini')))
@@ -443,7 +454,7 @@ class GroupEvaluator:
                 e.error = 'no agent directory %s' % e.agent_dir
             elif not inis:
                 e.error = 'no config under %s/data/' % e.agent_dir
-            elif e.model != 'greedy' and not find_checkpoint(os.path.join(e.agent_dir, 'model')):
+            elif e.model not in ('greedy', 'maxpressure') and not find_checkpoint(os.path.join(e.agent_dir, 'model')):
                 e.error = 'no checkpoint under %s/model/' % e.agent_dir
             if e.error:
                 logging.error('%s: %s, skipped' % (e.label, e.error))
@@ -473,7 +484,7 @@ class GroupEvaluator:
         for e in self.entries:
             if e.error:
                 continue
-            k = sim_key(e.env, demand=self.share_demand)
+            k = (sim_key(e.env, demand=self.share_demand), e.model == 'maxpressure')
             if k in keys:
                 self.groups[keys.index(k)].append(e)
             else:
@@ -487,11 +498,13 @@ class GroupEvaluator:
     # ---- device work ----------------------------------------------------------------------------------------------
     def _build_model(self, e):
         import os
-        from ..envs import greedy_controller
+        from ..envs import greedy_controller, maxpressure_controller
         from .models import IA2C, IQL, MA2C
         env = e.env
         if e.model == 'greedy':
             return greedy_controller(env)
+        if e.model == 'maxpressure':
+            return maxpressure_controller(env)
         mc = e.config['MODEL_CONFIG']
         kw = dict(n_replicas=1, obs_off=env._tables.node_obs_off, policy=self.policy, device=self.device)
         if e.model == 'ma2c':
@@ -529,8 +542,8 @@ class _Group:
         # members ordered by forward family so that each grouped launch covers consecutive rows
         fam = []
         for e, m in zip(entries, models):
-            if e.model == 'greedy':
-                fam.append(('greedy',))
+            if e.model in ('greedy', 'maxpressure'):
+                fam.append((e.model,))
             elif e.model in ('lr', 'dqn'):
                 fam.append(('q', e.model))
             else:
@@ -611,6 +624,8 @@ class _Group:
             max_cand, off, idx, act = (int(prog[0]),) + tuple(np.ascontiguousarray(a, np.int32) for a in prog[1:])
             _lib.check(lib.tsc_set_greedy_program(
                 self.sim._h, max_cand, off.ctypes.data, idx.ctypes.data, act.ctypes.data))
+        elif kind == 'maxpressure':
+            pass                                        # reads only the simulator's own tables
         elif kind == 'q':
             m0, net = self.models[i], self.entries[i].env._tables
             qlay = QLayout.from_iql(m0, np.asarray(net.node_obs_off), self.n_obs, max_na=self.max_na)
@@ -651,6 +666,8 @@ class _Group:
             obs, pi, act = self.obs[r0:r0 + n], self.pi[r0:r0 + n], self.act[r0:r0 + n]
             if kind == 'greedy':
                 _lib.check(lib.tsc_greedy_actions(self.sim._h, _p(self.obs), _p(self.act), self._st()))
+            elif kind == 'maxpressure':
+                _lib.check(lib.tsc_pressure_actions(self.sim._h, _p(self.act), self._st()))
             elif kind == 'q':
                 _lib.check(lib.tscl_q_step_g(st['h'], _p(st['params']), st['qlay'].n_params, _p(obs), st['j'] - st['i'],
                                              _p(st['rows']), n, _p(st['q']), _p(act),

@@ -956,6 +956,12 @@ struct tsc_handle {
   // greedy program (tsc_set_greedy_program): CSR over (node, candidate) of observation offsets + action per candidate
   int gp_max_cand = 0;
   int32_t* d_gp_off = nullptr; int32_t* d_gp_idx = nullptr; int32_t* d_gp_act = nullptr;
+  // max-pressure controller (tsc_pressure_actions): host copies of the net tables it reads, taken by tsc_create (the
+  // caller may free its tables); the per-node link list is built from them and uploaded on the first call
+  std::vector<int32_t> mp_from, mp_to, mp_node, mp_tlidx, mp_nph;
+  std::vector<uint32_t> mp_green;
+  int mp_max_phases = 0;
+  int32_t* d_mp_off = nullptr; uint32_t* d_mp_link = nullptr; int32_t* d_mp_nph = nullptr; uint32_t* d_mp_green = nullptr;
 };
 
 template <class T>
@@ -1064,6 +1070,13 @@ extern "C" int tsc_create(const tsc_net* net, const tsc_cfg* cfg, int32_t R, int
   h->args.ctl_words = (CTL_FIXED + N + net->n_src + 3) & ~3;
   h->meas_words = 3 * net->n_det + N;
   h->n_nodes = N; h->n_obs = net->n_obs; h->max_na = net->max_na; h->n_det = net->n_det;
+  h->mp_from.assign(net->link_from, net->link_from + net->n_links);
+  h->mp_to.assign(net->link_to, net->link_to + net->n_links);
+  h->mp_node.assign(net->link_node, net->link_node + net->n_links);
+  h->mp_tlidx.assign(net->link_tlidx, net->link_tlidx + net->n_links);
+  h->mp_nph.assign(net->node_n_phases, net->node_n_phases + N);
+  h->mp_green.assign(net->node_green, net->node_green + (size_t)N * net->max_phases);
+  h->mp_max_phases = net->max_phases;
   rc |= dalloc(h, (size_t)R * 2 * net->n_slots, &h->args.veh);
   rc |= dalloc(h, (size_t)R * d.lpad, &h->args.lane_cnt);
   rc |= dalloc(h, (size_t)R * h->args.ctl_words, &h->args.ctl);
@@ -1102,6 +1115,7 @@ extern "C" int tsc_destroy(tsc_handle* h) {
   for (void* p : h->owned) cudaFree(p);
   cudaFree(h->d_gp_off); cudaFree(h->d_gp_idx); cudaFree(h->d_gp_act);
   cudaFree(h->d_level); cudaFree(h->d_lv_due); cudaFree(h->d_lv_plo); cudaFree(h->d_lv_phi);
+  cudaFree(h->d_mp_off); cudaFree(h->d_mp_link); cudaFree(h->d_mp_nph); cudaFree(h->d_mp_green);
   delete h;
   return 0;
 }
@@ -1457,6 +1471,94 @@ extern "C" int tsc_greedy_actions(tsc_handle* h, const float* obs_dev, int32_t* 
   const int64_t RN = (int64_t)h->R * h->n_nodes;
   tsc_greedy_kernel<<<(unsigned)((RN + 127) / 128), 128, 0, (cudaStream_t)stream>>>(
       obs_dev, action_dev, RN, h->n_nodes, h->n_obs, h->gp_max_cand, h->d_gp_off, h->d_gp_idx, h->d_gp_act);
+  CK(cudaGetLastError());
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------------------
+// Max-pressure controller (Varaiya 2013) on the vehicles per lane the last step / observe left in HBM: per node i and
+// phase p < n_phases[i], P = sum over the node's controlled links whose signal is green ('G' or 'g') in p of
+// lane_cnt[from] - lane_cnt[to], in int32; the FIRST phase with the largest P wins (np.argmax).  One CTA per `per_cta`
+// consecutive replicas: their lane_cnt rows (lpad bytes each, a multiple of 16) are staged in shared memory with 16-byte
+// loads, then one thread per (replica, node) scores its node's phases from the node's link list.
+#define TSC_PRESSURE_THREADS 256
+#define TSC_PRESSURE_SMEM (48 * 1024)
+
+__global__ void __launch_bounds__(TSC_PRESSURE_THREADS)
+tsc_pressure_kernel(const uint8_t* __restrict__ lane_cnt, int lpad, int R, int n_nodes, int per_cta, int max_phases,
+                    const int32_t* __restrict__ node_off, const uint32_t* __restrict__ link,
+                    const int32_t* __restrict__ n_phases, const uint32_t* __restrict__ green,
+                    int32_t* __restrict__ action) {
+  extern __shared__ uint4 s_cnt4[];
+  const int r0 = blockIdx.x * per_cta;
+  const int nr = min(per_cta, R - r0);
+  const uint4* src = reinterpret_cast<const uint4*>(lane_cnt + (size_t)r0 * lpad);
+  for (int k = threadIdx.x; k < nr * (lpad >> 4); k += blockDim.x) s_cnt4[k] = src[k];
+  __syncthreads();
+  const int t = threadIdx.x;
+  if (t >= nr * n_nodes) return;
+  const int rr = t / n_nodes, node = t - rr * n_nodes;
+  const uint8_t* cnt = reinterpret_cast<const uint8_t*>(s_cnt4) + rr * lpad;
+  const int e0 = __ldg(&node_off[node]), e1 = __ldg(&node_off[node + 1]), np_ = __ldg(&n_phases[node]);
+  int best = 0, pick = 0;
+  for (int p = 0; p < np_; ++p) {
+    const uint32_t g = __ldg(&green[node * max_phases + p]);
+    int s = 0;
+    for (int e = e0; e < e1; ++e) {
+      const uint32_t w = __ldg(&link[e]);   // from:10 | to:10 | tlidx:5
+      if ((g >> (w >> 20)) & 1u) s += (int)cnt[w & 1023u] - (int)cnt[(w >> 10) & 1023u];
+    }
+    if (p == 0 || s > best) { best = s; pick = p; }
+  }
+  action[(size_t)(r0 + rr) * n_nodes + node] = pick;
+}
+
+// the per-node list of controlled links: CSR offsets [n_nodes + 1] and one word per link, links in index order.  A link
+// into a lane the net does not hold (link_to = -1, e.g. Monaco's connections to non-passenger lanes) carries no vehicle
+// and is left out.
+static int pressure_tables(tsc_handle* h) {
+  const int N = h->n_nodes, nl = (int)h->mp_from.size(), L = h->args.net.n_lanes;
+  std::vector<int32_t> off(N + 1, 0);
+  std::vector<uint32_t> words;
+  for (int i = 0; i < N; ++i) {
+    for (int l = 0; l < nl; ++l) {
+      if (h->mp_node[l] != i || h->mp_from[l] < 0 || h->mp_to[l] < 0) continue;
+      const int tl = h->mp_tlidx[l];
+      if (tl < 0 || tl >= TSC_MAX_NODE_LINKS) return fail("tsc_pressure_actions: link position outside the phase string");
+      if (h->mp_from[l] >= L || h->mp_to[l] >= L) return fail("tsc_pressure_actions: link lane out of range");
+      words.push_back((uint32_t)h->mp_from[l] | ((uint32_t)h->mp_to[l] << 10) | ((uint32_t)tl << 20));
+    }
+    off[i + 1] = (int32_t)words.size();
+  }
+  const size_t ng = h->mp_green.size();
+  CK(cudaMalloc(&h->d_mp_off, sizeof(int32_t) * (N + 1)));
+  CK(cudaMalloc(&h->d_mp_link, sizeof(uint32_t) * (words.empty() ? 1 : words.size())));
+  CK(cudaMalloc(&h->d_mp_nph, sizeof(int32_t) * (N > 0 ? N : 1)));
+  CK(cudaMalloc(&h->d_mp_green, sizeof(uint32_t) * (ng > 0 ? ng : 1)));
+  CK(cudaMemcpy(h->d_mp_off, off.data(), sizeof(int32_t) * (N + 1), cudaMemcpyHostToDevice));
+  if (!words.empty())
+    CK(cudaMemcpy(h->d_mp_link, words.data(), sizeof(uint32_t) * words.size(), cudaMemcpyHostToDevice));
+  if (N > 0) CK(cudaMemcpy(h->d_mp_nph, h->mp_nph.data(), sizeof(int32_t) * N, cudaMemcpyHostToDevice));
+  if (ng > 0) CK(cudaMemcpy(h->d_mp_green, h->mp_green.data(), sizeof(uint32_t) * ng, cudaMemcpyHostToDevice));
+  return 0;
+}
+
+extern "C" int tsc_pressure_actions(tsc_handle* h, int32_t* action_dev, void* stream) {
+  if (!h || !action_dev) return fail("tsc_pressure_actions: bad argument");
+  CK(cudaSetDevice(h->device));
+  if (!h->d_mp_green && pressure_tables(h) != 0) {
+    cudaFree(h->d_mp_off); cudaFree(h->d_mp_link); cudaFree(h->d_mp_nph); cudaFree(h->d_mp_green);
+    h->d_mp_off = nullptr; h->d_mp_link = nullptr; h->d_mp_nph = nullptr; h->d_mp_green = nullptr;
+    return -1;
+  }
+  const int N = h->n_nodes, lpad = h->args.net.lpad;
+  if (N <= 0) return 0;
+  int per_cta = TSC_PRESSURE_THREADS / N;   // >= 1: tsc_create caps the nodes at TSC_THREADS - 1
+  if (lpad > 0 && per_cta * lpad > TSC_PRESSURE_SMEM) per_cta = TSC_PRESSURE_SMEM / lpad;
+  const unsigned grid = (unsigned)((h->R + per_cta - 1) / per_cta);
+  tsc_pressure_kernel<<<grid, TSC_PRESSURE_THREADS, (size_t)per_cta * lpad, (cudaStream_t)stream>>>(
+      h->args.lane_cnt, lpad, h->R, N, per_cta, h->mp_max_phases, h->d_mp_off, h->d_mp_link, h->d_mp_nph,
+      h->d_mp_green, action_dev);
   CK(cudaGetLastError());
   return 0;
 }

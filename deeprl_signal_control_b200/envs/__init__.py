@@ -1,6 +1,6 @@
 """Scenario envs with the reference's names, and the two constructors the entry points share (scripts/train.py,
 scripts/evaluate.py): `make_env` picks the env class from `[ENV_CONFIG]` as main.py:init_env does, `greedy_controller`
-the scenario's greedy policy."""
+the scenario's greedy policy, `maxpressure_controller` the max-pressure one."""
 
 
 # the [ENV_CONFIG] keys that set each scenario's traffic demand and nothing else: two configs that differ only in these
@@ -87,3 +87,9 @@ def greedy_controller(env):
     if env.name == "small_grid":
         return SmallGridController(env.node_names)
     return SumoNetController(env.node_names, env.nodes, {n: env.phase_map.phases[n].phases for n in env.node_names})
+
+
+def maxpressure_controller(env):
+    """The max-pressure controller (envs.maxpressure) of any scenario env: `name = 'maxpressure'`."""
+    from .maxpressure import MaxPressureController
+    return MaxPressureController(env)

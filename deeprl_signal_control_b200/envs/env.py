@@ -328,6 +328,6 @@ class TrafficSimulator:
         if self.n_replicas > 1:
             return obs.copy(), reward.copy(), bool(done[0]), greward.copy()
         reward0 = reward[0].astype(np.float64)
-        if self.train_mode and self.agent in ('a2c', 'greedy'):
+        if self.train_mode and self.agent in ('a2c', 'greedy', 'maxpressure'):
             reward0 = float(greward[0])                              # envs/env.py:593-594
         return self._split_obs(obs[0]), reward0, bool(done[0]), float(greward[0])

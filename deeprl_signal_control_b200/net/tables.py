@@ -73,7 +73,8 @@ _CT = {np.dtype(np.float32): C.c_float, np.dtype(np.int32): C.c_int32,
 
 OBJECTIVES = {"queue": 0, "wait": 1, "hybrid": 2}
 # reward shaping families of reference envs/env.py:591-631
-AGENT_MODES = {"greedy": 0, "a2c": 0, "ia2c": 1, "iqll": 1, "iqld": 1, "ma2c": 2}
+# maxpressure (envs.maxpressure_controller) is a non-learning controller like greedy and observes what greedy does
+AGENT_MODES = {"greedy": 0, "maxpressure": 0, "a2c": 0, "ia2c": 1, "iqll": 1, "iqld": 1, "ma2c": 2}
 
 
 @dataclass
@@ -305,13 +306,14 @@ def build_obs_program(net: NetTables, agent: str, coop_gamma: float, use_wait: b
     """Observation layout of reference envs/env.py:163-205 and dims of :303-323.
 
     per agent: [own wave | neighbour waves (x coop_gamma iff ma2c) | own wait | neighbour
-    fingerprints (ma2c)]; greedy: own wave only."""
+    fingerprints (ma2c)]; greedy and maxpressure: own wave only."""
     names = net.node_names
     idx = {n: i for i, n in enumerate(names)}
     det_off = net.node_det_off
     kinds, idxs, scales, obs_off = [], [], [], [0]
     n_s_ls, n_w_ls, n_f_ls = [], [], []
-    marl = agent not in ("a2c", "greedy")
+    own_only = agent in ("greedy", "maxpressure")
+    marl = agent != "a2c" and not own_only
     for i, name in enumerate(names):
         own = list(range(det_off[i], det_off[i + 1]))
         k0 = len(kinds)
@@ -324,7 +326,7 @@ def build_obs_program(net: NetTables, agent: str, coop_gamma: float, use_wait: b
                 for d in range(det_off[j], det_off[j + 1]):
                     kinds.append(0); idxs.append(d); scales.append(sc)
         n_w = 0
-        if use_wait and agent != "greedy":
+        if use_wait and not own_only:
             for d in own:
                 kinds.append(1); idxs.append(d); scales.append(1.0)
             n_w = len(own)

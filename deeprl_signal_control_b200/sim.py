@@ -186,6 +186,14 @@ class BatchedSim:
         w0, w1 = rows[:nr.value, 0].astype(np.int64), rows[:nr.value, 1].astype(np.int64)
         return np.stack([w0 & 4095, (w0 >> 12) & 4095, w0 >> 24, w1 & 65535, w1 >> 16], axis=1)
 
+    def pressure_actions(self, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Max-pressure phases of every replica (`tsc_pressure_actions`) from the state the last step / observe left:
+        int32 [R, n_nodes] on the device, into `out` when given."""
+        act = torch.empty(self.R, self.net.n_nodes, dtype=torch.int32, device=self.device) if out is None else out
+        assert act.dtype == torch.int32 and act.is_contiguous() and act.numel() == self.R * self.net.n_nodes
+        _lib.check(_lib.lib().tsc_pressure_actions(self._h, ptr(act), self._stream()))
+        return act
+
     # ---- parity taps ---------------------------------------------------------------------
     def counts(self):
         n = self.net

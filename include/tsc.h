@@ -212,6 +212,17 @@ int tsc_set_greedy_program(tsc_handle* h, int32_t max_cand, const int32_t* off_h
                            const int32_t* act_host);
 int tsc_greedy_actions(tsc_handle* h, const float* obs_dev, int32_t* action_dev, void* stream);
 
+/* ---- max-pressure controller (Varaiya 2013) ---------------------------------------------------------------------------
+ * tsc_pressure_actions: action_dev int32 [R][n_nodes] = per replica r and node i, the FIRST phase p < node_n_phases[i]
+ *   with the largest pressure
+ *     P(r, i, p) = sum over links l with link_node[l] == i and bit link_tlidx[l] set in node_green[i][p]
+ *                  of lane_cnt[r][link_from[l]] - lane_cnt[r][link_to[l]]
+ *   (integer; lane_cnt = whole-lane vehicle counts, as tsc_dump_state returns them), read from the state the last
+ *   tsc_step / tsc_step_record / tsc_observe left, the instant that call's observation describes.  Uncontrolled links
+ *   (link_node = -1) and links into a lane outside the net (link_to = -1: no vehicle takes them) do not count.  The per-node link list is built from the net given to tsc_create on the first call
+ *   (synchronous then); later calls are one stream-ordered launch. */
+int tsc_pressure_actions(tsc_handle* h, int32_t* action_dev, void* stream);
+
 /* Integer parity taps measured at the end of the last step, per detector lane
  * (lanearea.getLastStepVehicleNumber / getLastStepHaltingNumber / head getWaitingTime,
  * envs/env.py:333-349,377-395) and per node (the phase index = action applied).
