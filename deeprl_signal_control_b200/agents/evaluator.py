@@ -9,8 +9,10 @@ mode `output_data()` writes the control / traffic / trip CSVs with the rows, in 
 writes when it runs the seeds one after another.  `model` is an IA2C / MA2C wrapper (agents/models.py; only its
 parameters `batched.P` and the packed image `batched.Wp` are read), an IQL (`model.name == 'iql'`, LR or DQN; only its
 `nets` are read, packed into the evaluator's own parameter vector at the start of every perform_all()), a greedy
-controller (`model.name == 'greedy'`) or the max-pressure controller (`model.name == 'maxpressure'`,
-envs.maxpressure_controller; nothing of it is read).
+controller (`model.name == 'greedy'`), the max-pressure controller (`model.name == 'maxpressure'`,
+envs.maxpressure_controller; nothing of it is read) or the fixed-time controller (`model.name == 'fixedtime'`,
+envs.fixedtime_controller; its `program` is set on the simulator, which then runs it with no action launch and
+action = NULL, the recorded actions being the program phases of each interval's first second).
 
 Per control step, with no host synchronisation inside the episode: the pi-only forward (tscl_policy_step_pi for the
 fused tensor-core widths; the v1 forward or the fc-policy kernels, then tscl_argmax_actions, otherwise), the fp32 Q
@@ -142,14 +144,18 @@ class Evaluator:
         if name == 'maxpressure':
             self.family = 'maxpressure'
             return
+        if name == 'fixedtime':
+            self.family = 'fixedtime'
+            sim.set_signal_program(model.program)
+            self.fixed_act = fixed_actions(model.program, self.T, self.ci, self.R, self.dev)
+            return
         if name == 'iql':
             self._init_q(model, net)
             return
         b = getattr(model, 'batched', None)
         if b is None or name not in ('ia2c', 'ma2c'):
-            raise ValueError("Evaluator: batched evaluation covers the greedy and max-pressure controllers, IA2C / MA2C and "
-                             "IQL; %r stays on "
-                             "the one-replica protocol" % (name,))
+            raise ValueError("Evaluator: batched evaluation covers the greedy, max-pressure and fixed-time controllers, "
+                             "IA2C / MA2C and IQL; %r stays on the one-replica protocol" % (name,))
         L = b.lay
         if L.n_obs != self.n_obs or not np.array_equal(L.obs_off, np.asarray(net.node_obs_off[:L.A])):
             raise ValueError("Evaluator: the model's observation layout differs from the env's (build the model with "
@@ -212,6 +218,8 @@ class Evaluator:
         if self.family == 'maxpressure':
             _lib.check(lib.tsc_pressure_actions(self.sim._h, _p(self.act), self._st()))
             return None
+        if self.family == 'fixedtime':          # the simulator runs the program
+            return None
         if self.family == 'q':
             _lib.check(lib.tscl_q_step(self._qh, _p(self.params), _p(self.obs), self.R, _p(self.q), _p(self.act),
                                        int(self.policy_type == 'stochastic'), self.seed, step, 0, _p(self.bad),
@@ -253,15 +261,17 @@ class Evaluator:
             self.c.zero_(); self.h.zero_()
         fp = self.fp0 if self.fingerprint else None
         sim.observe(fp, obs_out=self.obs)
+        fixed = not self.greedy and self.family == 'fixedtime'
+        act = None if fixed else self.act
         for t in range(self.T):
             pi = self._actions(t)
             fp = pi if self.fingerprint else None
             if record:
-                _lib.check(lib.tsc_step_record(sim._h, _p(self.act), _p(fp), _p(self.obs), _p(self.reward),
+                _lib.check(lib.tsc_step_record(sim._h, _p(act), _p(fp), _p(self.obs), _p(self.reward),
                                                _p(self.trace[t]), _p(self.done), _p(self.stats[t]), self._st()))
-                self.act_trace[t].copy_(self.act)
+                self.act_trace[t].copy_(self.fixed_act[t] if fixed else self.act)
             else:
-                _lib.check(lib.tsc_step(sim._h, _p(self.act), _p(fp), _p(self.obs), _p(self.reward), _p(self.trace[t]),
+                _lib.check(lib.tsc_step(sim._h, _p(act), _p(fp), _p(self.obs), _p(self.reward), _p(self.trace[t]),
                                         _p(self.done), self._st()))
         env.cur_sec = self.T * self.ci
 
@@ -333,10 +343,20 @@ class Evaluator:
 MAX_GROUP_REPLICAS = 1 << 16
 
 
+def fixed_actions(program, T, ci, R, device):
+    """int32 [T][R][N] on `device`: the phases a fixed-time run records, those of each interval's first second."""
+    from ..envs.fixedtime import phase_at
+    rows = np.stack([phase_at(program, t * ci) for t in range(T)])
+    return torch.from_numpy(np.ascontiguousarray(np.repeat(rows[:, None], R, axis=1))).to(device)
+
+
+CONTROLLERS = ('greedy', 'maxpressure', 'fixedtime')       # agent directories without a checkpoint
+
+
 def entry_model(agent):
     """The model an agent directory's name selects (main.py:179-190, scripts/evaluate.py): 'greedy', 'maxpressure',
-    'ia2c', 'ma2c', 'a2c', 'iqld' -> IQL 'dqn', any other name -> IQL 'lr'."""
-    if agent in ('greedy', 'maxpressure', 'ia2c', 'ma2c', 'a2c'):
+    'fixedtime', 'ia2c', 'ma2c', 'a2c', 'iqld' -> IQL 'dqn', any other name -> IQL 'lr'."""
+    if agent in CONTROLLERS + ('ia2c', 'ma2c', 'a2c'):
         return agent
     return 'dqn' if agent == 'iqld' else 'lr'
 
@@ -399,14 +419,16 @@ class GroupEvaluator:
         GroupEvaluator(entries, seeds, policy_type='default', policy='lstm').run()
 
     `entries`: (agent directory, model, output path) triples, model as entry_model gives it.  The constructor only
-    checks and groups, on the host: an entry whose directory, config or checkpoint (none for greedy and maxpressure) is
+    checks and groups, on the host: an entry whose directory, config or checkpoint (none for greedy, maxpressure and
+    fixedtime) is
     missing is logged as an error and skipped (`skipped`); an `a2c` entry, or a simulator whose combined replicas exceed MAX_GROUP_REPLICAS, is refused
     with a ValueError naming the entry.  Entries whose simulators would be built identically (sim_key) share one
     simulator, len(seeds) consecutive replicas per entry.  Per control step of a shared simulator: one
     tscl_policy_step_pi_g for the v2-family A2C members of one layout, one tscl_q_step_g per IQL layout (LR / DQN),
     tsc_greedy_actions, tsc_pressure_actions, the v1 / fc A2C members' own forwards on their row slices, and one tsc_step
-    (tsc_step_record).  The two controller launches write every row of their simulator, so greedy and maxpressure
-    entries, which would otherwise share one, get a simulator each.
+    (tsc_step_record).  The two controller launches write every row of their simulator, and a fixed-time program governs
+    every replica of its simulator, so greedy, maxpressure and fixedtime entries, which would otherwise share one, get a
+    simulator each (fixedtime entries of one program share one, stepped with action = NULL).
     Each entry's reward trace, frames and summary are those `Evaluator` gives for its directory alone: member k samples
     with its own [ENV_CONFIG] seed and member-local replica index, ma2c members their own coop_gamma
     (tsc_set_replica_coop_gamma).
@@ -445,8 +467,8 @@ class GroupEvaluator:
                 self.entries += [GroupEntry(d, m, oj, demand=lv) for oj, lv in zip(o, levels)]
         for e in self.entries:
             if e.model == 'a2c':
-                raise ValueError("%s: batched evaluation covers greedy, maxpressure, ia2c, ma2c and IQL (got agent 'a2c')"
-                                 % e.label)
+                raise ValueError("%s: batched evaluation covers greedy, maxpressure, fixedtime, ia2c, ma2c and IQL (got "
+                                 "agent 'a2c')" % e.label)
         self.skipped = []
         for e in self.entries:
             inis = sorted(glob.glob(os.path.join(e.agent_dir, 'data', '*.ini')))
@@ -454,7 +476,7 @@ class GroupEvaluator:
                 e.error = 'no agent directory %s' % e.agent_dir
             elif not inis:
                 e.error = 'no config under %s/data/' % e.agent_dir
-            elif e.model not in ('greedy', 'maxpressure') and not find_checkpoint(os.path.join(e.agent_dir, 'model')):
+            elif e.model not in CONTROLLERS and not find_checkpoint(os.path.join(e.agent_dir, 'model')):
                 e.error = 'no checkpoint under %s/model/' % e.agent_dir
             if e.error:
                 logging.error('%s: %s, skipped' % (e.label, e.error))
@@ -484,7 +506,8 @@ class GroupEvaluator:
         for e in self.entries:
             if e.error:
                 continue
-            k = (sim_key(e.env, demand=self.share_demand), e.model == 'maxpressure')
+            k = (sim_key(e.env, demand=self.share_demand), e.model if e.model in ('maxpressure', 'fixedtime') else '',
+                 _program_key(e.env) if e.model == 'fixedtime' else None)
             if k in keys:
                 self.groups[keys.index(k)].append(e)
             else:
@@ -499,12 +522,15 @@ class GroupEvaluator:
     def _build_model(self, e):
         import os
         from ..envs import greedy_controller, maxpressure_controller
+        from ..envs.fixedtime import FixedTimeController
         from .models import IA2C, IQL, MA2C
         env = e.env
         if e.model == 'greedy':
             return greedy_controller(env)
         if e.model == 'maxpressure':
             return maxpressure_controller(env)
+        if e.model == 'fixedtime':
+            return FixedTimeController(env)         # the group's simulator runs its program (_Group._add_forward)
         mc = e.config['MODEL_CONFIG']
         kw = dict(n_replicas=1, obs_off=env._tables.node_obs_off, policy=self.policy, device=self.device)
         if e.model == 'ma2c':
@@ -532,6 +558,13 @@ def _layout_key(lay):
                  if isinstance(v, (int, float, bool, str, list, tuple, np.ndarray)))
 
 
+def _program_key(env):
+    """Fixed-time entries share a simulator only when they run the same program."""
+    from ..envs.fixedtime import env_program
+    p = env_program(env)
+    return tuple(np.asarray(getattr(p, f)).tobytes() for f in ('n_phases', 'dur', 'open', 'major', 'yellow', 'offset'))
+
+
 class _Group:
     """One shared simulator of a GroupEvaluator and its members' forwards."""
 
@@ -542,7 +575,7 @@ class _Group:
         # members ordered by forward family so that each grouped launch covers consecutive rows
         fam = []
         for e, m in zip(entries, models):
-            if e.model in ('greedy', 'maxpressure'):
+            if e.model in CONTROLLERS:
                 fam.append((e.model,))
             elif e.model in ('lr', 'dqn'):
                 fam.append(('q', e.model))
@@ -626,6 +659,9 @@ class _Group:
                 self.sim._h, max_cand, off.ctypes.data, idx.ctypes.data, act.ctypes.data))
         elif kind == 'maxpressure':
             pass                                        # reads only the simulator's own tables
+        elif kind == 'fixedtime':                       # every member runs the one program of the group
+            self.sim.set_signal_program(self.models[i].program)
+            self.fixed_act = fixed_actions(self.models[i].program, self.T, self.ci, self.R, self.dev)
         elif kind == 'q':
             m0, net = self.models[i], self.entries[i].env._tables
             qlay = QLayout.from_iql(m0, np.asarray(net.node_obs_off), self.n_obs, max_na=self.max_na)
@@ -668,6 +704,8 @@ class _Group:
                 _lib.check(lib.tsc_greedy_actions(self.sim._h, _p(self.obs), _p(self.act), self._st()))
             elif kind == 'maxpressure':
                 _lib.check(lib.tsc_pressure_actions(self.sim._h, _p(self.act), self._st()))
+            elif kind == 'fixedtime':
+                pass                                    # the simulator runs the program
             elif kind == 'q':
                 _lib.check(lib.tscl_q_step_g(st['h'], _p(st['params']), st['qlay'].n_params, _p(obs), st['j'] - st['i'],
                                              _p(st['rows']), n, _p(st['q']), _p(act),
@@ -709,15 +747,17 @@ class _Group:
                 st['bad'].fill_(-1)
         fp = self.fp0 if self.ma2c else None
         sim.observe(fp, obs_out=self.obs)
+        fixed = self.fwd[0][0] == 'fixedtime'
+        act = None if fixed else self.act
         for t in range(self.T):
             self._actions(t)
             fp = self.pi if self.ma2c else None
             if record:
-                _lib.check(lib.tsc_step_record(sim._h, _p(self.act), _p(fp), _p(self.obs), _p(self.reward),
+                _lib.check(lib.tsc_step_record(sim._h, _p(act), _p(fp), _p(self.obs), _p(self.reward),
                                                _p(self.trace[t]), _p(self.done), _p(self.stats[t]), self._st()))
-                self.act_trace[t].copy_(self.act)
+                self.act_trace[t].copy_(self.fixed_act[t] if fixed else self.act)
             else:
-                _lib.check(lib.tsc_step(sim._h, _p(self.act), _p(fp), _p(self.obs), _p(self.reward), _p(self.trace[t]),
+                _lib.check(lib.tsc_step(sim._h, _p(act), _p(fp), _p(self.obs), _p(self.reward), _p(self.trace[t]),
                                         _p(self.done), self._st()))
 
     def _failed_samples(self):

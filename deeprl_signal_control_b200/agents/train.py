@@ -88,10 +88,10 @@ def init_test_flag(test_mode):
 
 def model_spec(agent):
     """main.py:110-121: ('ia2c' | 'ma2c', None) for the A2C agents, ('iql', 'dqn') for iqld and ('iql', 'lr') for every
-    other name.  greedy has nothing to train; the centralised a2c (a joint action space of prod(n_a) actions) has no
-    batched learner."""
-    if agent == 'greedy':
-        raise ValueError("agent 'greedy' has no model to train")
+    other name.  greedy and fixedtime have nothing to train; the centralised a2c (a joint action space of prod(n_a)
+    actions) has no batched learner."""
+    if agent in ('greedy', 'fixedtime'):
+        raise ValueError("agent %r has no model to train" % agent)
     if agent == 'a2c':
         raise ValueError("agent 'a2c' (the centralised A2C) has no batched learner; train ia2c, ma2c or an IQL agent")
     if agent in ('ia2c', 'ma2c'):

@@ -101,6 +101,11 @@ struct StepArgs {
   const float* cg;    // [R] per-replica coop_gamma (tsc_set_replica_coop_gamma) or null: cfg.coop_gamma / obs_scale_val
   const int32_t* dlevel;  // [R] demand level of each replica (tsc_set_replica_demand) or null.  When set, launch() points
                           // net.src_due / src_plo / src_phi at the level stack [n_levels][..] and the CTA offsets them
+  // fixed-time signal program (tsc_set_signal_program), read only by the FIXED instantiations.  Appended last so that
+  // the parameter offsets of every field above stay those of the action-driven kernels.
+  const int4* fx_node;    // [n_nodes] {n_phases, cycle, offset, 0}
+  const uint4* fx_phase;  // [n_nodes][fx_max_phases] {duration, open, major, yellow}
+  int32_t fx_max_phases;
 };
 
 // ------------------------------------------------------------------------------------------------
@@ -319,11 +324,35 @@ __device__ __forceinline__ void node_signal(const DevNet& n, int i, int a, int p
   open[i] = o; major[i] = m; ymask[i] = y;
 }
 
+// fixed-time program: the phase of node i in force during simulated second `sec`, the k whose window
+// [start_k, start_k + d_k) holds (sec - offset) mod cycle (envs/fixedtime.py:phase_at)
+__device__ __forceinline__ int program_phase(const StepArgs& A, int i, int sec) {
+  const int4 nd = __ldg(&A.fx_node[i]);
+  int t = (sec - nd.z) % nd.y;
+  if (t < 0) t += nd.y;
+  const uint4* ph = A.fx_phase + (size_t)i * A.fx_max_phases;
+  int k = 0;
+  for (; k < nd.x - 1; ++k) {
+    const int d = (int)__ldg(&ph[k].x);
+    if (t < d) break;
+    t -= d;
+  }
+  return k;
+}
+// ... and its signal state: the program's link masks replace node_signal's action / yellow derivation
+__device__ __forceinline__ void program_signal(const StepArgs& A, int i, int sec, uint32_t* open, uint32_t* major,
+                                               uint32_t* ymask) {
+  const uint4 p = __ldg(&A.fx_phase[(size_t)i * A.fx_max_phases + program_phase(A, i, sec)]);
+  open[i] = p.y; major[i] = p.z; ymask[i] = p.w;
+}
+
 // ------------------------------------------------------------------------------------------------
 extern __shared__ __align__(16) unsigned char smem_raw[];
 
 // REC = record mode: a fourth ring word per vehicle (trip word) and the arrival log; compiled out of the hot variant.
-template <bool REC>
+// FIXED = fixed-time mode: every node runs its signal program second by second (tsc_set_signal_program); no action is
+// read, prev_action is left as it is, and the phase tap holds the program phase of the interval's first second.
+template <bool REC, bool FIXED>
 __global__ void __launch_bounds__(TSC_THREADS, TSC_MIN_BLOCKS)
 tsc_step_kernel(const StepArgs A) {
   const DevNet& n = A.net;
@@ -381,7 +410,8 @@ tsc_step_kernel(const StepArgs A) {
   if (tid < CTL_FIXED) s_misc[tid] = g_ctl[tid];
   for (int i = tid; i < N; i += TSC_THREADS) {
     s_prev[i] = g_ctl[CTL_FIXED + i];
-    s_act[i] = A.n_sub > 0 ? A.action[(size_t)rep * N + i] : s_prev[i];
+    if constexpr (FIXED) s_act[i] = program_phase(A, i, g_ctl[0] - A.sub0);
+    else s_act[i] = A.n_sub > 0 ? A.action[(size_t)rep * N + i] : s_prev[i];
     s_appr[i] = 0;
   }
   for (int q = tid; q < n.n_src; q += TSC_THREADS) s_backlog[q] = g_ctl[CTL_FIXED + N + q];
@@ -402,8 +432,10 @@ tsc_step_kernel(const StepArgs A) {
       }
     }
   }
-  for (int i = tid; i < N; i += TSC_THREADS)
-    node_signal(n, i, s_act[i], s_prev[i], A.sub0 < c.yellow_interval_sec, s_opn, s_maj, s_yel);
+  for (int i = tid; i < N; i += TSC_THREADS) {
+    if constexpr (FIXED) program_signal(A, i, s_misc[0], s_opn, s_maj, s_yel);
+    else node_signal(n, i, s_act[i], s_prev[i], A.sub0 < c.yellow_interval_sec, s_opn, s_maj, s_yel);
+  }
   __syncthreads();
 
   const uint32_t seed_lo = (uint32_t)s_misc[1], seed_hi = (uint32_t)s_misc[2];
@@ -618,8 +650,9 @@ tsc_step_kernel(const StepArgs A) {
     }
     for (int i = tid; i < N; i += TSC_THREADS) {
       s_appr[i] = 0;
-      // green part starts after the yellow sub-steps (envs/env.py:571-573)
-      if (sub + 1 == c.yellow_interval_sec) node_signal(n, i, s_act[i], s_prev[i], false, s_opn, s_maj, s_yel);
+      // green part starts after the yellow sub-steps (envs/env.py:571-573); a program sets the next second's signal
+      if constexpr (FIXED) program_signal(A, i, cur_sec + 1, s_opn, s_maj, s_yel);
+      else if (sub + 1 == c.yellow_interval_sec) node_signal(n, i, s_act[i], s_prev[i], false, s_opn, s_maj, s_yel);
     }
     __syncthreads();
     // D + E (own lanes only, so no barrier in between and none before the next A1):
@@ -839,7 +872,7 @@ tsc_step_kernel(const StepArgs A) {
     g_ctl[0] = cur_sec; g_ctl[3] = s_misc[3]; g_ctl[4] = s_misc[4];
     if constexpr (REC) { g_ctl[5] = s_misc[5]; A.trip_cnt[rep] = s_misc[5] < A.trip_cap ? s_misc[5] : A.trip_cap; }
   }
-  if (A.sub0 + A.n_sub >= c.control_interval_sec)      // the interval is complete: prev_action = action
+  if (!FIXED && A.sub0 + A.n_sub >= c.control_interval_sec)      // the interval is complete: prev_action = action
     for (int i = tid; i < N; i += TSC_THREADS) g_ctl[CTL_FIXED + i] = s_act[i];
   for (int q = tid; q < n.n_src; q += TSC_THREADS) g_ctl[CTL_FIXED + N + q] = s_backlog[q];
   if (A.meas) {
@@ -962,6 +995,8 @@ struct tsc_handle {
   std::vector<uint32_t> mp_green;
   int mp_max_phases = 0;
   int32_t* d_mp_off = nullptr; uint32_t* d_mp_link = nullptr; int32_t* d_mp_nph = nullptr; uint32_t* d_mp_green = nullptr;
+  // fixed-time signal program (tsc_set_signal_program): while set, every step launch is a FIXED instantiation
+  int4* d_fx_node = nullptr; uint4* d_fx_phase = nullptr; int fx_max_phases = 0;
 };
 
 template <class T>
@@ -1100,10 +1135,13 @@ extern "C" int tsc_create(const tsc_net* net, const tsc_cfg* cfg, int32_t R, int
   sm += (size_t)L * sizeof(LaneC) + (size_t)net->n_routes * net->max_hops * 2 * 2;
   h->smem = (int)sm + 16;
   if (sm > 227 * 1024) { tsc_destroy(h); return fail("tsc_create: replica state exceeds 227 KB of shared memory"); }
-  CK(cudaFuncSetAttribute(tsc_step_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem));
+  CK(cudaFuncSetAttribute(tsc_step_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem));
+  CK(cudaFuncSetAttribute(tsc_step_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem));
   h->smem_rec = h->smem + (int)net->n_slots * 4 + 16;   // + slack: the 16-byte alignment of the table block can shift
-  if (h->smem_rec <= 232448)
-    CK(cudaFuncSetAttribute(tsc_step_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem_rec));
+  if (h->smem_rec <= 232448) {
+    CK(cudaFuncSetAttribute(tsc_step_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem_rec));
+    CK(cudaFuncSetAttribute(tsc_step_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem_rec));
+  }
   std::vector<uint64_t> seeds(R, 0);
   *out = h;
   return tsc_reset(h, seeds.data(), nullptr);
@@ -1116,6 +1154,7 @@ extern "C" int tsc_destroy(tsc_handle* h) {
   cudaFree(h->d_gp_off); cudaFree(h->d_gp_idx); cudaFree(h->d_gp_act);
   cudaFree(h->d_level); cudaFree(h->d_lv_due); cudaFree(h->d_lv_plo); cudaFree(h->d_lv_phi);
   cudaFree(h->d_mp_off); cudaFree(h->d_mp_link); cudaFree(h->d_mp_nph); cudaFree(h->d_mp_green);
+  cudaFree(h->d_fx_node); cudaFree(h->d_fx_phase);
   delete h;
   return 0;
 }
@@ -1192,6 +1231,53 @@ extern "C" int tsc_set_replica_demand(tsc_handle* h, int32_t n_levels, const uin
   return 0;
 }
 
+extern "C" int tsc_set_signal_program(tsc_handle* h, int32_t max_phases, const int32_t* n_phases_host,
+                                      const int32_t* dur_host, const uint32_t* open_host, const uint32_t* major_host,
+                                      const uint32_t* yellow_host, const int32_t* offset_host) {
+  if (!h) return fail("tsc_set_signal_program: null handle");
+  const int N = h->n_nodes;
+  std::vector<int4> node(N > 0 ? N : 1);
+  std::vector<uint4> phase;
+  if (n_phases_host) {          // every check before the current program is touched
+    if (max_phases <= 0 || !dur_host || !open_host || !major_host || !yellow_host || !offset_host)
+      return fail("tsc_set_signal_program: bad argument");
+    phase.resize((size_t)(N > 0 ? N : 1) * max_phases);
+    for (int i = 0; i < N; ++i) {
+      const int np_ = n_phases_host[i];
+      const std::string who = "tsc_set_signal_program: node " + std::to_string(i);
+      if (np_ < 1 || np_ > max_phases) return fail(who + " has " + std::to_string(np_) + " phases, outside [1, max_phases]");
+      if (offset_host[i] < -(1 << 30) || offset_host[i] > (1 << 30)) return fail(who + ": offset out of range");
+      int64_t cycle = 0;
+      for (int k = 0; k < np_; ++k) {
+        const size_t e = (size_t)i * max_phases + k;
+        if (dur_host[e] < 1) return fail(who + ": phase " + std::to_string(k) + " lasts less than 1 s");
+        if (yellow_host[e] & open_host[e]) return fail(who + ": phase " + std::to_string(k) + " has a link open and yellow");
+        if (major_host[e] & ~open_host[e]) return fail(who + ": phase " + std::to_string(k) + " has a major link not open");
+        cycle += dur_host[e];
+        phase[e] = make_uint4((uint32_t)dur_host[e], open_host[e], major_host[e], yellow_host[e]);
+      }
+      if (cycle > (1 << 30)) return fail(who + ": cycle longer than 2^30 s");
+      node[i] = make_int4(np_, (int)cycle, offset_host[i], 0);
+    }
+  }
+  CK(cudaSetDevice(h->device));
+  CK(cudaDeviceSynchronize());          // no launch in flight still reads the previous program
+  cudaFree(h->d_fx_node); cudaFree(h->d_fx_phase);
+  h->d_fx_node = nullptr; h->d_fx_phase = nullptr; h->fx_max_phases = 0;
+  if (!n_phases_host) return 0;
+  int4* dn = nullptr; uint4* dp = nullptr;
+  cudaError_t e = cudaMalloc(&dn, node.size() * sizeof(int4));
+  if (e == cudaSuccess) e = cudaMalloc(&dp, phase.size() * sizeof(uint4));
+  if (e == cudaSuccess) e = cudaMemcpy(dn, node.data(), node.size() * sizeof(int4), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaMemcpy(dp, phase.data(), phase.size() * sizeof(uint4), cudaMemcpyHostToDevice);
+  if (e != cudaSuccess) {       // the program stays off
+    cudaFree(dn); cudaFree(dp);
+    return fail(std::string("tsc_set_signal_program: ") + cudaGetErrorString(e));
+  }
+  h->d_fx_node = dn; h->d_fx_phase = dp; h->fx_max_phases = max_phases;
+  return 0;
+}
+
 static int launch(tsc_handle* h, int n_sub, const int32_t* action, const float* fp, float* obs, float* reward,
                   float* greward, uint8_t* done, cudaStream_t st, int rep0 = 0, int count = -1, int sub0 = 0) {
   StepArgs a = h->args;
@@ -1201,13 +1287,18 @@ static int launch(tsc_handle* h, int n_sub, const int32_t* action, const float* 
   }
   a.n_sub = n_sub; a.action = action; a.fp = fp; a.obs = obs; a.reward = reward; a.greward = greward; a.done = done;
   a.rep0 = rep0;
+  const bool fixed = h->d_fx_node != nullptr;
+  if (fixed) { a.fx_node = h->d_fx_node; a.fx_phase = h->d_fx_phase; a.fx_max_phases = h->fx_max_phases; }
+  const unsigned grid = count < 0 ? h->R : count;
   if (h->record) {
     a.trip = h->d_trip; a.trip_log = h->d_trip_log; a.trip_cnt = h->d_trip_cnt; a.trip_cap = h->trip_cap;
     a.sub0 = sub0;
-    tsc_step_kernel<true><<<count < 0 ? h->R : count, TSC_THREADS, h->smem_rec, st>>>(a);
+    if (fixed) tsc_step_kernel<true, true><<<grid, TSC_THREADS, h->smem_rec, st>>>(a);
+    else tsc_step_kernel<true, false><<<grid, TSC_THREADS, h->smem_rec, st>>>(a);
   } else {
     a.sub0 = sub0;
-    tsc_step_kernel<false><<<count < 0 ? h->R : count, TSC_THREADS, h->smem, st>>>(a);
+    if (fixed) tsc_step_kernel<false, true><<<grid, TSC_THREADS, h->smem, st>>>(a);
+    else tsc_step_kernel<false, false><<<grid, TSC_THREADS, h->smem, st>>>(a);
   }
   CK(cudaGetLastError());
   return 0;
@@ -1221,7 +1312,7 @@ extern "C" int tsc_observe(tsc_handle* h, const float* fp_dev, float* obs_dev, v
 
 extern "C" int tsc_step(tsc_handle* h, const int32_t* action_dev, const float* fp_dev, float* obs_dev,
                         float* reward_dev, float* greward_dev, uint8_t* done_dev, void* stream) {
-  if (!h || !action_dev) return fail("tsc_step: bad argument");
+  if (!h || (!action_dev && !h->d_fx_node)) return fail("tsc_step: bad argument");
   CK(cudaSetDevice(h->device));
   return launch(h, h->args.cfg.control_interval_sec, action_dev, fp_dev, obs_dev, reward_dev, greward_dev, done_dev,
                 (cudaStream_t)stream);
@@ -1229,11 +1320,11 @@ extern "C" int tsc_step(tsc_handle* h, const int32_t* action_dev, const float* f
 
 extern "C" int tsc_step_host(tsc_handle* h, const int32_t* action_host, const float* fp_host, float* obs_host,
                              float* reward_host, float* greward_host, uint8_t* done_host, void* stream) {
-  if (!h || !action_host) return fail("tsc_step_host: bad argument");
+  if (!h || (!action_host && !h->d_fx_node)) return fail("tsc_step_host: bad argument");
   CK(cudaSetDevice(h->device));
   cudaStream_t st = (cudaStream_t)stream;
   const size_t R = h->R, N = h->n_nodes;
-  CK(cudaMemcpyAsync(h->d_action, action_host, R * N * 4, cudaMemcpyHostToDevice, st));
+  if (action_host) CK(cudaMemcpyAsync(h->d_action, action_host, R * N * 4, cudaMemcpyHostToDevice, st));
   if (fp_host) CK(cudaMemcpyAsync(h->d_fp, fp_host, R * N * h->max_na * 4, cudaMemcpyHostToDevice, st));
   if (launch(h, h->args.cfg.control_interval_sec, h->d_action, fp_host ? h->d_fp : nullptr, obs_host ? h->d_obs : nullptr,
              reward_host ? h->d_reward : nullptr, greward_host ? h->d_greward : nullptr,
@@ -1250,12 +1341,13 @@ extern "C" int tsc_step_host(tsc_handle* h, const int32_t* action_host, const fl
 static int step_host_range(tsc_handle* h, int32_t rep0, int32_t count, const int32_t* action_host,
                            const float* fp_host, float* obs_host, float* reward_host, float* greward_host,
                            uint8_t* done_host, void* stream, bool sync) {
-  if (!h || !action_host || rep0 < 0 || count <= 0 || rep0 + count > h->R) return fail("tsc_step_host_range: bad argument");
+  if (!h || (!action_host && !h->d_fx_node) || rep0 < 0 || count <= 0 || rep0 + count > h->R)
+    return fail("tsc_step_host_range: bad argument");
   CK(cudaSetDevice(h->device));
   cudaStream_t st = (cudaStream_t)stream;
   const size_t N = h->n_nodes, r0 = (size_t)rep0, n = (size_t)count;
   // the kernel indexes its io arrays by absolute replica: device scratch is used at offset rep0, host pointers are slice bases
-  CK(cudaMemcpyAsync(h->d_action + r0 * N, action_host, n * N * 4, cudaMemcpyHostToDevice, st));
+  if (action_host) CK(cudaMemcpyAsync(h->d_action + r0 * N, action_host, n * N * 4, cudaMemcpyHostToDevice, st));
   if (fp_host) CK(cudaMemcpyAsync(h->d_fp + r0 * N * h->max_na, fp_host, n * N * h->max_na * 4, cudaMemcpyHostToDevice, st));
   if (launch(h, h->args.cfg.control_interval_sec, h->d_action, fp_host ? h->d_fp : nullptr, obs_host ? h->d_obs : nullptr,
              reward_host ? h->d_reward : nullptr, greward_host ? h->d_greward : nullptr,
@@ -1304,7 +1396,7 @@ extern "C" int tsc_set_record(tsc_handle* h, int32_t on) {
 extern "C" int tsc_step_record(tsc_handle* h, const int32_t* action_dev, const float* fp_dev, float* obs_dev,
                                float* reward_dev, float* greward_dev, uint8_t* done_dev, float* sub_stats_dev,
                                void* stream) {
-  if (!h || !action_dev) return fail("tsc_step_record: bad argument");
+  if (!h || (!action_dev && !h->d_fx_node)) return fail("tsc_step_record: bad argument");
   if (!h->record) return fail("tsc_step_record: record mode is off (tsc_set_record)");
   CK(cudaSetDevice(h->device));
   const int ci = h->args.cfg.control_interval_sec;

@@ -1,6 +1,7 @@
 """Scenario envs with the reference's names, and the two constructors the entry points share (scripts/train.py,
 scripts/evaluate.py): `make_env` picks the env class from `[ENV_CONFIG]` as main.py:init_env does, `greedy_controller`
-the scenario's greedy policy, `maxpressure_controller` the max-pressure one."""
+the scenario's greedy policy, `maxpressure_controller` the max-pressure one, `fixedtime_controller` the fixed-time
+one."""
 
 
 # the [ENV_CONFIG] keys that set each scenario's traffic demand and nothing else: two configs that differ only in these
@@ -93,3 +94,12 @@ def maxpressure_controller(env):
     """The max-pressure controller (envs.maxpressure) of any scenario env: `name = 'maxpressure'`."""
     from .maxpressure import MaxPressureController
     return MaxPressureController(env)
+
+
+def fixedtime_controller(env):
+    """The fixed-time controller (envs.fixedtime) of any scenario env, `name = 'fixedtime'`; puts the env's simulator
+    into fixed mode, every replica running the env's signal programs."""
+    from .fixedtime import FixedTimeController
+    ctrl = FixedTimeController(env)
+    env._ensure_sim().set_signal_program(ctrl.program)
+    return ctrl

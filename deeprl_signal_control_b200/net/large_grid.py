@@ -21,6 +21,10 @@ L0_END = 75.0
 N = 5
 # envs/large_grid_env.py:40-41
 PHASES = ['GGgrrrGGgrrr', 'rrrGrGrrrGrG', 'rrrGGrrrrGGr', 'rrrGGGrrrrrr', 'rrrrrrrrrGGG']
+# the fixed-time program the reference generator writes for every node (large_grid/data/build_file.py:output_tls,
+# exp.tll.xml): three greens of 30 s, each followed by a 3-s yellow, offset 0 (envs.fixedtime runs it)
+TLS_PROGRAM = [(30, 'GGgrrrGGgrrr'), (3, 'yyyrrryyyrrr'), (30, 'rrrGrGrrrGrG'), (3, 'rrrGryrrrGry'),
+               (30, 'rrrGGrrrrGGr'), (3, 'rrryyrrrryyr')]
 # turning-speed limits of the junction-internal lanes (netconvert computes them from the
 # turning radius with --junctions.limit-turn-speed 5.5: v = sqrt(5.5 r); r ~ 5 m / 12 m)
 TURN_VMAX = {"r": 5.2, "s": 1.0e9, "l": 8.1}
@@ -421,3 +425,10 @@ def build_large_grid(peak_flow1: int = 1100, peak_flow2: int = 925, agent: str =
     net.edges = edges
     build_obs_program(net, agent, coop_gamma, use_wait)
     return net.finalize()
+
+
+def tls_programs():
+    """{tlLogic id: program} of the grid (TLS_PROGRAM on nodes nt1..nt25), in the form of
+    net.sumo_ingest.read_signal_programs."""
+    return {_nt(i): {'type': 'static', 'offset': 0, 'phases': [[d, st] for d, st in TLS_PROGRAM]}
+            for i in range(1, N * N + 1)}

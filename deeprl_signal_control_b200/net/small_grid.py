@@ -31,6 +31,11 @@ SMALL_GRID_NEIGHBOR_MAP = {'nt1': ['npc', 'nt2', 'nt6'], 'nt2': ['nt1', 'nt3'], 
 # envs/small_grid_env.py:34-38
 TWO_PHASE = ['GGrr', 'rrGG']
 THREE_PHASE = ['GGGrrrrrr', 'rrrGGGrrr', 'rrrrrrGGG']
+# the fixed-time programs the reference generator writes (small_grid/data/build_file.py:output_tls, exp.tll.xml): 30-s
+# greens, each followed by a 3-s yellow, offset 0; three greens at nt1, two at every other node
+TLS_THREE_PHASE = [(30, 'GGGrrrrrr'), (3, 'yyyrrrrrr'), (30, 'rrrGGGrrr'), (3, 'rrryyyrrr'), (30, 'rrrrrrGGG'),
+                   (3, 'rrrrrryyy')]
+TLS_TWO_PHASE = [(30, 'GGrr'), (3, 'yyrr'), (30, 'rrGG'), (3, 'rryy')]
 
 
 def node_xy() -> Dict[str, Tuple[float, float]]:
@@ -287,3 +292,11 @@ def build_small_grid(num_car_hourly: int = 1000, agent: str = "greedy", coop_gam
     net.flow_list, net.edges = flow_list, edges
     build_obs_program(net, agent, coop_gamma, use_wait)
     return net.finalize()
+
+
+def tls_programs():
+    """{tlLogic id: program} of the small grid (TLS_THREE_PHASE at nt1, TLS_TWO_PHASE at nt2..nt6), in the form of
+    net.sumo_ingest.read_signal_programs."""
+    return {'nt%d' % i: {'type': 'static', 'offset': 0,
+                         'phases': [[d, st] for d, st in (TLS_THREE_PHASE if i == 1 else TLS_TWO_PHASE)]}
+            for i in range(1, 7)}

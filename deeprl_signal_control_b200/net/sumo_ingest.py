@@ -43,6 +43,23 @@ def read_tls_programs(*files: str) -> Dict[str, List[str]]:
     return out
 
 
+def read_signal_programs(*files: str) -> Dict[str, dict]:
+    """{tlLogic id: {'type', 'offset', 'phases': [[duration, state], ...]}} of the whole static programs in net /
+    additional files (later files override; a '.gz' file is read through gzip), the attribute values as the file writes
+    them.  envs.fixedtime checks and runs them."""
+    import gzip
+    out: Dict[str, dict] = {}
+    for f in files:
+        if not f:
+            continue
+        with (gzip.open(f) if f.endswith('.gz') else open(f, 'rb')) as fh:
+            root = ET.parse(fh).getroot()
+        for tl in root.iter('tlLogic'):
+            out[tl.get('id')] = {'type': tl.get('type', 'static'), 'offset': tl.get('offset', '0'),
+                                 'phases': [[ph.get('duration'), ph.get('state')] for ph in tl.findall('phase')]}
+    return out
+
+
 def derive_neighbor_map(net_file: str, tls_ids, max_neighbors: int = 5) -> Dict[str, List[str]]:
     """Signalised junction -> neighbouring signalised junctions (by driving distance along normal edges, not passing
     through another signalised junction).  A tlLogic id is matched to the junctions whose connections carry `tl=id`."""

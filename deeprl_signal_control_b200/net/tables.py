@@ -73,8 +73,9 @@ _CT = {np.dtype(np.float32): C.c_float, np.dtype(np.int32): C.c_int32,
 
 OBJECTIVES = {"queue": 0, "wait": 1, "hybrid": 2}
 # reward shaping families of reference envs/env.py:591-631
-# maxpressure (envs.maxpressure_controller) is a non-learning controller like greedy and observes what greedy does
-AGENT_MODES = {"greedy": 0, "maxpressure": 0, "a2c": 0, "ia2c": 1, "iqll": 1, "iqld": 1, "ma2c": 2}
+# maxpressure (envs.maxpressure_controller) and fixedtime (envs.fixedtime_controller) are non-learning controllers like
+# greedy and observe what greedy does
+AGENT_MODES = {"greedy": 0, "maxpressure": 0, "fixedtime": 0, "a2c": 0, "ia2c": 1, "iqll": 1, "iqld": 1, "ma2c": 2}
 
 
 @dataclass
@@ -306,13 +307,13 @@ def build_obs_program(net: NetTables, agent: str, coop_gamma: float, use_wait: b
     """Observation layout of reference envs/env.py:163-205 and dims of :303-323.
 
     per agent: [own wave | neighbour waves (x coop_gamma iff ma2c) | own wait | neighbour
-    fingerprints (ma2c)]; greedy and maxpressure: own wave only."""
+    fingerprints (ma2c)]; greedy, maxpressure and fixedtime: own wave only."""
     names = net.node_names
     idx = {n: i for i, n in enumerate(names)}
     det_off = net.node_det_off
     kinds, idxs, scales, obs_off = [], [], [], [0]
     n_s_ls, n_w_ls, n_f_ls = [], [], []
-    own_only = agent in ("greedy", "maxpressure")
+    own_only = agent in ("greedy", "maxpressure", "fixedtime")
     marl = agent != "a2c" and not own_only
     for i, name in enumerate(names):
         own = list(range(det_off[i], det_off[i + 1]))

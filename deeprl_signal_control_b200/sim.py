@@ -152,10 +152,11 @@ class BatchedSim:
     def step_host_range(self, r0: int, n: int, action: np.ndarray, fp: Optional[np.ndarray], obs: np.ndarray,
                         reward: np.ndarray, greward: np.ndarray, done: np.ndarray, sync: bool = True):
         """`tsc_step_host_range`: the host-buffer step for replicas [r0, r0 + n) on the current stream; all arrays are
-        the slices of that range (page-locked for full PCIe speed).  Blocks until the slice's results are on the host;
+        the slices of that range (page-locked for full PCIe speed); `action` may be None while a signal program is set.  Blocks until the slice's results are on the host;
         with sync=False (`tsc_step_host_range_async`) the work is only enqueued and the caller synchronises the stream."""
         fn = _lib.lib().tsc_step_host_range if sync else _lib.lib().tsc_step_host_range_async
-        _lib.check(fn(self._h, r0, n, action.ctypes.data, None if fp is None else fp.ctypes.data, obs.ctypes.data,
+        _lib.check(fn(self._h, r0, n, None if action is None else action.ctypes.data,
+                      None if fp is None else fp.ctypes.data, obs.ctypes.data,
                       reward.ctypes.data, greward.ctypes.data, done.ctypes.data, self._stream()))
 
     # ---- evaluation / recording path (envs/env.py:409-437, 498-542) ------------------------
@@ -193,6 +194,21 @@ class BatchedSim:
         assert act.dtype == torch.int32 and act.is_contiguous() and act.numel() == self.R * self.net.n_nodes
         _lib.check(_lib.lib().tsc_pressure_actions(self._h, ptr(act), self._stream()))
         return act
+
+    def set_signal_program(self, program=None) -> None:
+        """Fixed-time control (`tsc_set_signal_program`): every replica runs `program` (an envs.fixedtime.SignalProgram
+        in the net's node order) second by second, and step / step_record / the host steps read no action; their
+        phase tap holds the program phase of each interval's first second.  None returns to action-driven stepping."""
+        lib = _lib.lib()
+        if program is None:
+            _lib.check(lib.tsc_set_signal_program(self._h, 0, None, None, None, None, None, None))
+            return
+        if len(program.n_phases) != self.net.n_nodes:
+            raise ValueError("set_signal_program: %d node programs for %d nodes" % (len(program.n_phases), self.net.n_nodes))
+        a = [np.ascontiguousarray(x, t) for x, t in ((program.n_phases, np.int32), (program.dur, np.int32),
+                                                    (program.open, np.uint32), (program.major, np.uint32),
+                                                    (program.yellow, np.uint32), (program.offset, np.int32))]
+        _lib.check(lib.tsc_set_signal_program(self._h, program.max_phases, *(x.ctypes.data for x in a)))
 
     # ---- parity taps ---------------------------------------------------------------------
     def counts(self):

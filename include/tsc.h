@@ -153,6 +153,20 @@ int tsc_set_replica_coop_gamma(tsc_handle* h, const float* cg_host);
 int tsc_set_replica_demand(tsc_handle* h, int32_t n_levels, const uint8_t* due_host, const float* plo_host,
                            const float* phi_host, const int32_t* level_host);
 
+/* Fixed-time signal control (synchronous: synchronises the device, then replaces the previous program; call right
+ * after tsc_reset, like tsc_set_record).  Node i runs a static program of n_phases_host[i] phases (1 <= n <= max_phases);
+ * phase k (entry [i][k] of the [n_nodes][max_phases] host arrays) lasts dur_host[i][k] >= 1 seconds and shows the link
+ * masks open_host ('G' or 'g'), major_host ('G') and yellow_host ('y'), bit j = link j of the node's phase string.
+ * The cycle is C_i = sum of the durations; the simulated second s -> s + 1 runs with the phase k whose window
+ * [start_k, start_k + d_k) holds (s - offset_host[i]) mod C_i.
+ * While a program is set, tsc_step, tsc_step_record, tsc_step_host and both host-range calls run every replica on it:
+ * they read no action (action_dev / action_host may be NULL), leave prev_action as it is, and the phase tap of
+ * tsc_get_counts holds the program phase in force during the first second of the interval.  n_phases_host NULL
+ * returns to action-driven stepping. */
+int tsc_set_signal_program(tsc_handle* h, int32_t max_phases, const int32_t* n_phases_host, const int32_t* dur_host,
+                           const uint32_t* open_host, const uint32_t* major_host, const uint32_t* yellow_host,
+                           const int32_t* offset_host);
+
 /* Replaces _get_state() without stepping (the observation reset() returns,
  * envs/env.py:561,163-205).  fp_dev: [R][n_nodes][max_na] policy probabilities installed by
  * update_fingerprint (envs/env.py:633-635) or NULL (zeros).  obs_dev: [R][n_obs]. */
