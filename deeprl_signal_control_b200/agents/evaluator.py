@@ -10,9 +10,11 @@ writes when it runs the seeds one after another.  `model` is an IA2C / MA2C wrap
 parameters `batched.P` and the packed image `batched.Wp` are read), an IQL (`model.name == 'iql'`, LR or DQN; only its
 `nets` are read, packed into the evaluator's own parameter vector at the start of every perform_all()), a greedy
 controller (`model.name == 'greedy'`), the max-pressure controller (`model.name == 'maxpressure'`,
-envs.maxpressure_controller; nothing of it is read) or the fixed-time controller (`model.name == 'fixedtime'`,
+envs.maxpressure_controller; nothing of it is read), the fixed-time controller (`model.name == 'fixedtime'`,
 envs.fixedtime_controller; its `program` is set on the simulator, which then runs it with no action launch and
-action = NULL, the recorded actions being the program phases of each interval's first second).
+action = NULL, the recorded actions being the program phases of each interval's first second) or the vehicle-actuated
+controller (`model.name == 'actuated'`, envs.actuated_controller; run the same way, the recorded actions copied from
+the simulator's phase tap after each step).
 
 Per control step, with no host synchronisation inside the episode: the pi-only forward (tscl_policy_step_pi for the
 fused tensor-core widths; the v1 forward or the fc-policy kernels, then tscl_argmax_actions, otherwise), the fp32 Q
@@ -149,13 +151,17 @@ class Evaluator:
             sim.set_signal_program(model.program)
             self.fixed_act = fixed_actions(model.program, self.T, self.ci, self.R, self.dev)
             return
+        if name == 'actuated':
+            self.family = 'actuated'
+            sim.set_actuated_program(model.program)
+            return
         if name == 'iql':
             self._init_q(model, net)
             return
         b = getattr(model, 'batched', None)
         if b is None or name not in ('ia2c', 'ma2c'):
-            raise ValueError("Evaluator: batched evaluation covers the greedy, max-pressure and fixed-time controllers, "
-                             "IA2C / MA2C and IQL; %r stays on the one-replica protocol" % (name,))
+            raise ValueError("Evaluator: batched evaluation covers the greedy, max-pressure, fixed-time and actuated "
+                             "controllers, IA2C / MA2C and IQL; %r stays on the one-replica protocol" % (name,))
         L = b.lay
         if L.n_obs != self.n_obs or not np.array_equal(L.obs_off, np.asarray(net.node_obs_off[:L.A])):
             raise ValueError("Evaluator: the model's observation layout differs from the env's (build the model with "
@@ -218,7 +224,7 @@ class Evaluator:
         if self.family == 'maxpressure':
             _lib.check(lib.tsc_pressure_actions(self.sim._h, _p(self.act), self._st()))
             return None
-        if self.family == 'fixedtime':          # the simulator runs the program
+        if self.family in ('fixedtime', 'actuated'):       # the simulator runs the program
             return None
         if self.family == 'q':
             _lib.check(lib.tscl_q_step(self._qh, _p(self.params), _p(self.obs), self.R, _p(self.q), _p(self.act),
@@ -261,15 +267,16 @@ class Evaluator:
             self.c.zero_(); self.h.zero_()
         fp = self.fp0 if self.fingerprint else None
         sim.observe(fp, obs_out=self.obs)
-        fixed = not self.greedy and self.family == 'fixedtime'
-        act = None if fixed else self.act
+        program = None if self.greedy or self.family not in ('fixedtime', 'actuated') else self.family
+        act = None if program else self.act
         for t in range(self.T):
             pi = self._actions(t)
             fp = pi if self.fingerprint else None
             if record:
                 _lib.check(lib.tsc_step_record(sim._h, _p(act), _p(fp), _p(self.obs), _p(self.reward),
                                                _p(self.trace[t]), _p(self.done), _p(self.stats[t]), self._st()))
-                self.act_trace[t].copy_(self.fixed_act[t] if fixed else self.act)
+                _record_actions(sim, self.act_trace[t], program, self.fixed_act[t] if program == 'fixedtime' else self.act,
+                                self._st())
             else:
                 _lib.check(lib.tsc_step(sim._h, _p(act), _p(fp), _p(self.obs), _p(self.reward), _p(self.trace[t]),
                                         _p(self.done), self._st()))
@@ -350,12 +357,21 @@ def fixed_actions(program, T, ci, R, device):
     return torch.from_numpy(np.ascontiguousarray(np.repeat(rows[:, None], R, axis=1))).to(device)
 
 
-CONTROLLERS = ('greedy', 'maxpressure', 'fixedtime')       # agent directories without a checkpoint
+def _record_actions(sim, out, program, act, st):
+    """The recorded actions of one control step into `out`: under an actuated program the phase tap the step left
+    (tsc_get_counts; the phase of the interval's first second), otherwise `act`."""
+    if program == 'actuated':
+        _lib.check(_lib.lib().tsc_get_counts(sim._h, None, None, None, _p(out), st))
+    else:
+        out.copy_(act)
+
+
+CONTROLLERS = ('greedy', 'maxpressure', 'fixedtime', 'actuated')       # agent directories without a checkpoint
 
 
 def entry_model(agent):
     """The model an agent directory's name selects (main.py:179-190, scripts/evaluate.py): 'greedy', 'maxpressure',
-    'fixedtime', 'ia2c', 'ma2c', 'a2c', 'iqld' -> IQL 'dqn', any other name -> IQL 'lr'."""
+    'fixedtime', 'actuated', 'ia2c', 'ma2c', 'a2c', 'iqld' -> IQL 'dqn', any other name -> IQL 'lr'."""
     if agent in CONTROLLERS + ('ia2c', 'ma2c', 'a2c'):
         return agent
     return 'dqn' if agent == 'iqld' else 'lr'
@@ -419,16 +435,17 @@ class GroupEvaluator:
         GroupEvaluator(entries, seeds, policy_type='default', policy='lstm').run()
 
     `entries`: (agent directory, model, output path) triples, model as entry_model gives it.  The constructor only
-    checks and groups, on the host: an entry whose directory, config or checkpoint (none for greedy, maxpressure and
-    fixedtime) is
+    checks and groups, on the host: an entry whose directory, config or checkpoint (none for greedy, maxpressure,
+    fixedtime and actuated) is
     missing is logged as an error and skipped (`skipped`); an `a2c` entry, or a simulator whose combined replicas exceed MAX_GROUP_REPLICAS, is refused
     with a ValueError naming the entry.  Entries whose simulators would be built identically (sim_key) share one
     simulator, len(seeds) consecutive replicas per entry.  Per control step of a shared simulator: one
     tscl_policy_step_pi_g for the v2-family A2C members of one layout, one tscl_q_step_g per IQL layout (LR / DQN),
     tsc_greedy_actions, tsc_pressure_actions, the v1 / fc A2C members' own forwards on their row slices, and one tsc_step
     (tsc_step_record).  The two controller launches write every row of their simulator, and a fixed-time program governs
-    every replica of its simulator, so greedy, maxpressure and fixedtime entries, which would otherwise share one, get a
-    simulator each (fixedtime entries of one program share one, stepped with action = NULL).
+    every replica of its simulator, so greedy, maxpressure, fixedtime and actuated entries, which would otherwise share
+    one, get a simulator each (fixedtime or actuated entries of one program share one, stepped with action = NULL; for
+    actuated entries the program includes the loop tables).
     Each entry's reward trace, frames and summary are those `Evaluator` gives for its directory alone: member k samples
     with its own [ENV_CONFIG] seed and member-local replica index, ma2c members their own coop_gamma
     (tsc_set_replica_coop_gamma).
@@ -467,8 +484,8 @@ class GroupEvaluator:
                 self.entries += [GroupEntry(d, m, oj, demand=lv) for oj, lv in zip(o, levels)]
         for e in self.entries:
             if e.model == 'a2c':
-                raise ValueError("%s: batched evaluation covers greedy, maxpressure, fixedtime, ia2c, ma2c and IQL (got "
-                                 "agent 'a2c')" % e.label)
+                raise ValueError("%s: batched evaluation covers greedy, maxpressure, fixedtime, actuated, ia2c, ma2c and "
+                                 "IQL (got agent 'a2c')" % e.label)
         self.skipped = []
         for e in self.entries:
             inis = sorted(glob.glob(os.path.join(e.agent_dir, 'data', '*.ini')))
@@ -506,8 +523,8 @@ class GroupEvaluator:
         for e in self.entries:
             if e.error:
                 continue
-            k = (sim_key(e.env, demand=self.share_demand), e.model if e.model in ('maxpressure', 'fixedtime') else '',
-                 _program_key(e.env) if e.model == 'fixedtime' else None)
+            k = (sim_key(e.env, demand=self.share_demand),
+                 e.model if e.model in ('maxpressure', 'fixedtime', 'actuated') else '', _program_key(e.env, e.model))
             if k in keys:
                 self.groups[keys.index(k)].append(e)
             else:
@@ -531,6 +548,9 @@ class GroupEvaluator:
             return maxpressure_controller(env)
         if e.model == 'fixedtime':
             return FixedTimeController(env)         # the group's simulator runs its program (_Group._add_forward)
+        if e.model == 'actuated':
+            from ..envs.actuated import ActuatedController
+            return ActuatedController(env)          # likewise
         mc = e.config['MODEL_CONFIG']
         kw = dict(n_replicas=1, obs_off=env._tables.node_obs_off, policy=self.policy, device=self.device)
         if e.model == 'ma2c':
@@ -558,8 +578,14 @@ def _layout_key(lay):
                  if isinstance(v, (int, float, bool, str, list, tuple, np.ndarray)))
 
 
-def _program_key(env):
-    """Fixed-time entries share a simulator only when they run the same program."""
+def _program_key(env, model):
+    """Fixed-time and actuated entries share a simulator only when they run the same program (None for the other
+    models)."""
+    if model == 'actuated':
+        from ..envs.actuated import env_program as actuated_program
+        return actuated_program(env).key()
+    if model != 'fixedtime':
+        return None
     from ..envs.fixedtime import env_program
     p = env_program(env)
     return tuple(np.asarray(getattr(p, f)).tobytes() for f in ('n_phases', 'dur', 'open', 'major', 'yellow', 'offset'))
@@ -662,6 +688,8 @@ class _Group:
         elif kind == 'fixedtime':                       # every member runs the one program of the group
             self.sim.set_signal_program(self.models[i].program)
             self.fixed_act = fixed_actions(self.models[i].program, self.T, self.ci, self.R, self.dev)
+        elif kind == 'actuated':
+            self.sim.set_actuated_program(self.models[i].program)
         elif kind == 'q':
             m0, net = self.models[i], self.entries[i].env._tables
             qlay = QLayout.from_iql(m0, np.asarray(net.node_obs_off), self.n_obs, max_na=self.max_na)
@@ -704,7 +732,7 @@ class _Group:
                 _lib.check(lib.tsc_greedy_actions(self.sim._h, _p(self.obs), _p(self.act), self._st()))
             elif kind == 'maxpressure':
                 _lib.check(lib.tsc_pressure_actions(self.sim._h, _p(self.act), self._st()))
-            elif kind == 'fixedtime':
+            elif kind in ('fixedtime', 'actuated'):
                 pass                                    # the simulator runs the program
             elif kind == 'q':
                 _lib.check(lib.tscl_q_step_g(st['h'], _p(st['params']), st['qlay'].n_params, _p(obs), st['j'] - st['i'],
@@ -747,15 +775,16 @@ class _Group:
                 st['bad'].fill_(-1)
         fp = self.fp0 if self.ma2c else None
         sim.observe(fp, obs_out=self.obs)
-        fixed = self.fwd[0][0] == 'fixedtime'
-        act = None if fixed else self.act
+        program = self.fwd[0][0] if self.fwd[0][0] in ('fixedtime', 'actuated') else None
+        act = None if program else self.act
         for t in range(self.T):
             self._actions(t)
             fp = self.pi if self.ma2c else None
             if record:
                 _lib.check(lib.tsc_step_record(sim._h, _p(act), _p(fp), _p(self.obs), _p(self.reward),
                                                _p(self.trace[t]), _p(self.done), _p(self.stats[t]), self._st()))
-                self.act_trace[t].copy_(self.fixed_act[t] if fixed else self.act)
+                _record_actions(sim, self.act_trace[t], program, self.fixed_act[t] if program == 'fixedtime' else self.act,
+                                self._st())
             else:
                 _lib.check(lib.tsc_step(sim._h, _p(act), _p(fp), _p(self.obs), _p(self.reward), _p(self.trace[t]),
                                         _p(self.done), self._st()))

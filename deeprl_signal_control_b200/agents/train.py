@@ -88,9 +88,9 @@ def init_test_flag(test_mode):
 
 def model_spec(agent):
     """main.py:110-121: ('ia2c' | 'ma2c', None) for the A2C agents, ('iql', 'dqn') for iqld and ('iql', 'lr') for every
-    other name.  greedy and fixedtime have nothing to train; the centralised a2c (a joint action space of prod(n_a)
-    actions) has no batched learner."""
-    if agent in ('greedy', 'fixedtime'):
+    other name.  greedy, fixedtime and actuated have nothing to train; the centralised a2c (a joint action space of
+    prod(n_a) actions) has no batched learner."""
+    if agent in ('greedy', 'fixedtime', 'actuated'):
         raise ValueError("agent %r has no model to train" % agent)
     if agent == 'a2c':
         raise ValueError("agent 'a2c' (the centralised A2C) has no batched learner; train ia2c, ma2c or an IQL agent")

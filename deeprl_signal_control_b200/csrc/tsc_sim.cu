@@ -106,6 +106,15 @@ struct StepArgs {
   const int4* fx_node;    // [n_nodes] {n_phases, cycle, offset, 0}
   const uint4* fx_phase;  // [n_nodes][fx_max_phases] {duration, open, major, yellow}
   int32_t fx_max_phases;
+  // actuated signal program (tsc_set_actuated_program), read only by the ACTUATED instantiations; appended last too
+  const int4* ac_node;      // [n_nodes] {n_phases, max_gap, first, end} of the node's loop-link list ac_link
+  const uint4* ac_phase;    // [n_nodes][ac_max_phases] {min_dur, max_dur, open, major}
+  const uint32_t* ac_yel;   // [n_nodes][ac_max_phases] yellow mask
+  const uint32_t* ac_link;  // per node, its controlled links: from-lane:10 | tlidx:5 << 10
+  const int32_t* ac_loop;   // [n_lanes] loop position in 1/64 m from the lane start, -1 = no loop
+  int2* ac_state;           // [R][n_nodes] {phase, seconds the phase has run before the next simulated second}
+  uint8_t* ac_gap;          // [R][lpad] seconds since the lane's loop was last covered, saturating at 255
+  int32_t ac_max_phases;
 };
 
 // ------------------------------------------------------------------------------------------------
@@ -346,15 +355,34 @@ __device__ __forceinline__ void program_signal(const StepArgs& A, int i, int sec
   open[i] = p.y; major[i] = p.z; ymask[i] = p.w;
 }
 
+// actuated program (envs/actuated.py): the link masks of phase k of node i
+__device__ __forceinline__ void actuated_signal(const StepArgs& A, int i, int k, uint32_t* open, uint32_t* major,
+                                                uint32_t* ymask) {
+  const size_t e = (size_t)i * A.ac_max_phases + k;
+  const uint4 p = __ldg(&A.ac_phase[e]);
+  open[i] = p.z; major[i] = p.w; ymask[i] = __ldg(&A.ac_yel[e]);
+}
+// a lane's loop gap after a second in which its loop was (cov != 0) or was not covered
+__device__ __forceinline__ int gap_next(int gap, int cov) { return cov ? 0 : (gap < 255 ? gap + 1 : 255); }
+
+enum : int { CTL_ACTION = 0, CTL_FIXED_TIME = 1, CTL_ACTUATED = 2 };   // signal control modes of tsc_step_kernel
+
 // ------------------------------------------------------------------------------------------------
 extern __shared__ __align__(16) unsigned char smem_raw[];
 
 // REC = record mode: a fourth ring word per vehicle (trip word) and the arrival log; compiled out of the hot variant.
-// FIXED = fixed-time mode: every node runs its signal program second by second (tsc_set_signal_program); no action is
-// read, prev_action is left as it is, and the phase tap holds the program phase of the interval's first second.
-template <bool REC, bool FIXED>
+// MODE = how signals are set:
+//   CTL_ACTION: from the action and the previous action through the net's phase tables (node_signal);
+//   CTL_FIXED_TIME: every node runs its static program second by second (tsc_set_signal_program);
+//   CTL_ACTUATED: every node runs its actuated program (tsc_set_actuated_program): loop coverage is taken in B, and at
+//     the switch point after C one thread per node decides whether its phase ends, from the phase's elapsed time and
+//     the gaps of the loops on the from-lanes of the phase's open links.  Phase state and gaps persist in HBM.
+// In both program modes no action is read, prev_action is left as it is, and the phase tap holds the phase in force
+// during the interval's first second.
+template <bool REC, int MODE>
 __global__ void __launch_bounds__(TSC_THREADS, TSC_MIN_BLOCKS)
 tsc_step_kernel(const StepArgs A) {
+  constexpr bool FIXED = MODE == CTL_FIXED_TIME, ACT = MODE == CTL_ACTUATED;
   const DevNet& n = A.net;
   const tsc_cfg& c = A.cfg;
   const int tid = threadIdx.x;
@@ -397,13 +425,22 @@ tsc_step_kernel(const StepArgs A) {
   LaneC* s_lane = reinterpret_cast<LaneC*>(smem_raw + ((reinterpret_cast<unsigned char*>(s_obsv + 2 * n.n_det) - smem_raw + 15) & ~15));
   int16_t* s_rlane = reinterpret_cast<int16_t*>(s_lane + L);
   int16_t* s_rlink = s_rlane + n.n_routes * n.max_hops;
+  // actuated mode only (the other modes are launched with the shared memory above): per node phase and elapsed time,
+  // per lane loop gap and this second's coverage flag
+  int32_t* s_aph = reinterpret_cast<int32_t*>(smem_raw + ((reinterpret_cast<unsigned char*>(s_rlink + n.n_routes * n.max_hops) - smem_raw + 3) & ~3));
+  int32_t* s_ael = s_aph + N;
+  uint8_t* s_gap = reinterpret_cast<uint8_t*>(s_ael + N);
+  uint8_t* s_cov = s_gap + L;
 
   // ---- load replica state -------------------------------------------------------------------
   const uint8_t* g_cnt = A.lane_cnt + (size_t)rep * n.lpad;
   int32_t* g_ctl = A.ctl + (size_t)rep * A.ctl_words;
   uint32_t* g_x = A.veh + (size_t)rep * 2 * n.n_slots;
   uint32_t* g_m = g_x + n.n_slots;
-  for (int l = tid; l < L; l += TSC_THREADS) { s_cnt[l] = g_cnt[l]; s_head[l] = 0; s_lane[l] = n.lane[l]; }
+  for (int l = tid; l < L; l += TSC_THREADS) {
+    s_cnt[l] = g_cnt[l]; s_head[l] = 0; s_lane[l] = n.lane[l];
+    if constexpr (ACT) s_gap[l] = A.ac_gap[(size_t)rep * n.lpad + l];
+  }
   for (int i = tid; i < n.n_routes * n.max_hops; i += TSC_THREADS) {
     s_rlane[i] = __ldg(&n.route_lane[i]); s_rlink[i] = __ldg(&n.route_link[i]);
   }
@@ -411,6 +448,12 @@ tsc_step_kernel(const StepArgs A) {
   for (int i = tid; i < N; i += TSC_THREADS) {
     s_prev[i] = g_ctl[CTL_FIXED + i];
     if constexpr (FIXED) s_act[i] = program_phase(A, i, g_ctl[0] - A.sub0);
+    else if constexpr (ACT) {
+      const int2 st = A.ac_state[(size_t)rep * N + i];
+      s_aph[i] = st.x; s_ael[i] = st.y;
+      // a launch that starts mid-interval (record mode) carries the interval's phase over from the tap
+      s_act[i] = A.sub0 == 0 ? st.x : A.meas[(size_t)rep * (3 * n.n_det + N) + 3 * n.n_det + i];
+    }
     else s_act[i] = A.n_sub > 0 ? A.action[(size_t)rep * N + i] : s_prev[i];
     s_appr[i] = 0;
   }
@@ -434,6 +477,7 @@ tsc_step_kernel(const StepArgs A) {
   }
   for (int i = tid; i < N; i += TSC_THREADS) {
     if constexpr (FIXED) program_signal(A, i, s_misc[0], s_opn, s_maj, s_yel);
+    else if constexpr (ACT) actuated_signal(A, i, s_aph[i], s_opn, s_maj, s_yel);
     else node_signal(n, i, s_act[i], s_prev[i], A.sub0 < c.yellow_interval_sec, s_opn, s_maj, s_yel);
   }
   __syncthreads();
@@ -455,6 +499,10 @@ tsc_step_kernel(const StepArgs A) {
     // A1: approach masks + reset of per-lane scratch (own lanes)
     for (int l = l_lo; l < l_hi; ++l) {
       s_hflag[l] = 0; s_acc[l] = 0; s_cntadd[l] = 0;
+      if constexpr (ACT) {      // fold the previous second's coverage into the gap (the first one was folded at store)
+        if (sub != A.sub0) s_gap[l] = (uint8_t)gap_next(s_gap[l], s_cov[l]);
+        s_cov[l] = 0;
+      }
       if (s_cnt[l] > 0) {
         const LaneC lc = s_lane[l];
         const uint2 h = ld2(ring, lc.slot0 + s_head[l]);
@@ -596,6 +644,12 @@ tsc_step_kernel(const StepArgs A) {
           }
           me.x = pack_xv(xn, vn);       // waiting was decided on the computed speed; the record stores it rounded
           me.y = (me.y & ~1023u) | w;
+          if constexpr (ACT) {          // the vehicle covers the lane's loop X iff xq - Lq <= X <= xnq (1/64 m), a
+                                        // crossing or arriving head vehicle with xnq = +inf; x unpacks xq exactly
+            const int X = __ldg(&A.ac_loop[lane]);
+            if (X >= 0 && (int)(x * 64.0f) - (int)(c.veh_len * 64.0f) <= X && (f != 0 || X <= (int)(me.x & 0xffffu)))
+              s_cov[lane] = 1;
+          }
         }
         __syncthreads();
         if (act) {
@@ -652,6 +706,25 @@ tsc_step_kernel(const StepArgs A) {
       s_appr[i] = 0;
       // green part starts after the yellow sub-steps (envs/env.py:571-573); a program sets the next second's signal
       if constexpr (FIXED) program_signal(A, i, cur_sec + 1, s_opn, s_maj, s_yel);
+      else if constexpr (ACT) {
+        // phase k has run e seconds including this one: it ends at max_dur, or from min_dur on once every loop on the
+        // from-lane of an open link has a gap of at least max_gap
+        const int4 nd = __ldg(&A.ac_node[i]);
+        int k = s_aph[i], e = s_ael[i] + 1;
+        const uint4 ph = __ldg(&A.ac_phase[(size_t)i * A.ac_max_phases + k]);
+        bool end = e >= (int)ph.y;
+        if (!end && e >= (int)ph.x) {
+          end = true;
+          for (int q = nd.z; q < nd.w && end; ++q) {
+            const uint32_t w = __ldg(&A.ac_link[q]);
+            const int l = (int)(w & 1023u);
+            if (((ph.z >> (w >> 10)) & 1u) && gap_next(s_gap[l], s_cov[l]) < nd.y) end = false;
+          }
+        }
+        if (end) { k = k + 1 < nd.x ? k + 1 : 0; e = 0; }
+        s_aph[i] = k; s_ael[i] = e;
+        actuated_signal(A, i, k, s_opn, s_maj, s_yel);
+      }
       else if (sub + 1 == c.yellow_interval_sec) node_signal(n, i, s_act[i], s_prev[i], false, s_opn, s_maj, s_yel);
     }
     __syncthreads();
@@ -868,11 +941,15 @@ tsc_step_kernel(const StepArgs A) {
   }
   uint8_t* g_cnt_w = A.lane_cnt + (size_t)rep * n.lpad;
   for (int l = tid; l < L; l += TSC_THREADS) g_cnt_w[l] = (uint8_t)s_cnt[l];
+  if constexpr (ACT) {
+    for (int l = tid; l < L; l += TSC_THREADS) A.ac_gap[(size_t)rep * n.lpad + l] = (uint8_t)gap_next(s_gap[l], s_cov[l]);
+    for (int i = tid; i < N; i += TSC_THREADS) A.ac_state[(size_t)rep * N + i] = make_int2(s_aph[i], s_ael[i]);
+  }
   if (tid == 0) {
     g_ctl[0] = cur_sec; g_ctl[3] = s_misc[3]; g_ctl[4] = s_misc[4];
     if constexpr (REC) { g_ctl[5] = s_misc[5]; A.trip_cnt[rep] = s_misc[5] < A.trip_cap ? s_misc[5] : A.trip_cap; }
   }
-  if (!FIXED && A.sub0 + A.n_sub >= c.control_interval_sec)      // the interval is complete: prev_action = action
+  if (MODE == CTL_ACTION && A.sub0 + A.n_sub >= c.control_interval_sec)      // the interval is complete: prev_action = action
     for (int i = tid; i < N; i += TSC_THREADS) g_ctl[CTL_FIXED + i] = s_act[i];
   for (int q = tid; q < n.n_src; q += TSC_THREADS) g_ctl[CTL_FIXED + N + q] = s_backlog[q];
   if (A.meas) {
@@ -895,6 +972,24 @@ __global__ void tsc_reset_kernel(uint8_t* lane_cnt, int32_t* ctl, int32_t* meas,
     ctl[(size_t)rep * ctl_words + w] = v;
   }
   for (int w = threadIdx.x; w < meas_words; w += blockDim.x) meas[(size_t)rep * meas_words + w] = 0;
+}
+
+// actuated control: every replica's nodes take their initial (phase, elapsed), every lane's loop gap is 255
+__global__ void tsc_actuated_init_kernel(int2* state, uint8_t* gap, const int2* __restrict__ init, int n_nodes, int lpad,
+                                         int R) {
+  const int rep = blockIdx.x;
+  if (rep >= R) return;
+  for (int i = threadIdx.x; i < n_nodes; i += blockDim.x) state[(size_t)rep * n_nodes + i] = init[i];
+  for (int l = threadIdx.x; l < lpad; l += blockDim.x) gap[(size_t)rep * lpad + l] = 255;
+}
+
+// tsc_get_program_phase: the phase of every (replica, node) for the next simulated second, one thread each
+__global__ void tsc_program_phase_kernel(const StepArgs A, int64_t RN, int32_t* __restrict__ phase) {
+  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= RN) return;
+  const int N = A.net.n_nodes;
+  const int64_t r = t / N;
+  phase[t] = A.ac_state ? A.ac_state[t].x : program_phase(A, (int)(t - r * N), A.ctl[r * A.ctl_words]);
 }
 
 // _measure_traffic_step (envs/env.py:409-437) for every replica: one CTA per replica over the compact state.
@@ -997,7 +1092,22 @@ struct tsc_handle {
   int32_t* d_mp_off = nullptr; uint32_t* d_mp_link = nullptr; int32_t* d_mp_nph = nullptr; uint32_t* d_mp_green = nullptr;
   // fixed-time signal program (tsc_set_signal_program): while set, every step launch is a FIXED instantiation
   int4* d_fx_node = nullptr; uint4* d_fx_phase = nullptr; int fx_max_phases = 0;
+  // actuated signal program (tsc_set_actuated_program): while set, every step launch is an ACTUATED instantiation with
+  // smem_act / smem_rec_act bytes of shared memory.  Tables, each node's initial state, and the per-replica state.
+  int4* d_ac_node = nullptr; uint4* d_ac_phase = nullptr; uint32_t* d_ac_yel = nullptr; uint32_t* d_ac_link = nullptr;
+  int32_t* d_ac_loop = nullptr; int2* d_ac_init = nullptr; int2* d_ac_state = nullptr; uint8_t* d_ac_gap = nullptr;
+  int ac_max_phases = 0, smem_act = 0, smem_rec_act = 0;
 };
+
+static bool has_program(const tsc_handle* h) { return h->d_fx_node != nullptr || h->d_ac_state != nullptr; }
+
+static void free_actuated(tsc_handle* h) {
+  cudaFree(h->d_ac_node); cudaFree(h->d_ac_phase); cudaFree(h->d_ac_yel); cudaFree(h->d_ac_link);
+  cudaFree(h->d_ac_loop); cudaFree(h->d_ac_init); cudaFree(h->d_ac_state); cudaFree(h->d_ac_gap);
+  h->d_ac_node = nullptr; h->d_ac_phase = nullptr; h->d_ac_yel = nullptr; h->d_ac_link = nullptr;
+  h->d_ac_loop = nullptr; h->d_ac_init = nullptr; h->d_ac_state = nullptr; h->d_ac_gap = nullptr;
+  h->ac_max_phases = 0;
+}
 
 template <class T>
 static int upload(tsc_handle* h, const T* src, size_t count, const T** dst) {
@@ -1135,13 +1245,17 @@ extern "C" int tsc_create(const tsc_net* net, const tsc_cfg* cfg, int32_t R, int
   sm += (size_t)L * sizeof(LaneC) + (size_t)net->n_routes * net->max_hops * 2 * 2;
   h->smem = (int)sm + 16;
   if (sm > 227 * 1024) { tsc_destroy(h); return fail("tsc_create: replica state exceeds 227 KB of shared memory"); }
-  CK(cudaFuncSetAttribute(tsc_step_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem));
-  CK(cudaFuncSetAttribute(tsc_step_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem));
+  CK(cudaFuncSetAttribute(tsc_step_kernel<false, CTL_ACTION>, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem));
+  CK(cudaFuncSetAttribute(tsc_step_kernel<false, CTL_FIXED_TIME>, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem));
   h->smem_rec = h->smem + (int)net->n_slots * 4 + 16;   // + slack: the 16-byte alignment of the table block can shift
   if (h->smem_rec <= 232448) {
-    CK(cudaFuncSetAttribute(tsc_step_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem_rec));
-    CK(cudaFuncSetAttribute(tsc_step_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem_rec));
+    CK(cudaFuncSetAttribute(tsc_step_kernel<true, CTL_ACTION>, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem_rec));
+    CK(cudaFuncSetAttribute(tsc_step_kernel<true, CTL_FIXED_TIME>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                            h->smem_rec));
   }
+  // the actuated carve-up appends s_aph, s_ael [N] int32 and s_gap, s_cov [L] bytes (+ 4-byte alignment)
+  const int ac_extra = N * 8 + L * 2 + 4;
+  h->smem_act = h->smem + ac_extra; h->smem_rec_act = h->smem_rec + ac_extra;
   std::vector<uint64_t> seeds(R, 0);
   *out = h;
   return tsc_reset(h, seeds.data(), nullptr);
@@ -1155,6 +1269,7 @@ extern "C" int tsc_destroy(tsc_handle* h) {
   cudaFree(h->d_level); cudaFree(h->d_lv_due); cudaFree(h->d_lv_plo); cudaFree(h->d_lv_phi);
   cudaFree(h->d_mp_off); cudaFree(h->d_mp_link); cudaFree(h->d_mp_nph); cudaFree(h->d_mp_green);
   cudaFree(h->d_fx_node); cudaFree(h->d_fx_phase);
+  free_actuated(h);
   delete h;
   return 0;
 }
@@ -1169,6 +1284,11 @@ extern "C" int tsc_reset(tsc_handle* h, const uint64_t* seeds_host, void* stream
   tsc_reset_kernel<<<h->R, 64, 0, st>>>(h->args.lane_cnt, h->args.ctl, h->args.meas, d_seeds, h->args.net.lpad,
                                         h->args.ctl_words, h->meas_words, h->R);
   CK(cudaGetLastError());
+  if (h->d_ac_state) {
+    tsc_actuated_init_kernel<<<h->R, 64, 0, st>>>(h->d_ac_state, h->d_ac_gap, h->d_ac_init, h->n_nodes,
+                                                  h->args.net.lpad, h->R);
+    CK(cudaGetLastError());
+  }
   CK(cudaStreamSynchronize(st));
   CK(cudaFree(d_seeds));
   return 0;
@@ -1265,6 +1385,7 @@ extern "C" int tsc_set_signal_program(tsc_handle* h, int32_t max_phases, const i
   cudaFree(h->d_fx_node); cudaFree(h->d_fx_phase);
   h->d_fx_node = nullptr; h->d_fx_phase = nullptr; h->fx_max_phases = 0;
   if (!n_phases_host) return 0;
+  free_actuated(h);             // one signal program at a time
   int4* dn = nullptr; uint4* dp = nullptr;
   cudaError_t e = cudaMalloc(&dn, node.size() * sizeof(int4));
   if (e == cudaSuccess) e = cudaMalloc(&dp, phase.size() * sizeof(uint4));
@@ -1278,6 +1399,119 @@ extern "C" int tsc_set_signal_program(tsc_handle* h, int32_t max_phases, const i
   return 0;
 }
 
+extern "C" int tsc_set_actuated_program(tsc_handle* h, int32_t max_phases, const int32_t* n_phases_host,
+                                        const int32_t* min_dur_host, const int32_t* max_dur_host,
+                                        const uint32_t* open_host, const uint32_t* major_host,
+                                        const uint32_t* yellow_host, const int32_t* init_host,
+                                        const int32_t* max_gap_host, const int32_t* loop_pos_host) {
+  if (!h) return fail("tsc_set_actuated_program: null handle");
+  const int N = h->n_nodes, L = h->args.net.n_lanes, R = h->R;
+  const size_t NP = (size_t)(N > 0 ? N : 1) * (max_phases > 0 ? max_phases : 1);
+  std::vector<int4> node(N > 0 ? N : 1);
+  std::vector<uint4> phase;
+  std::vector<uint32_t> yel, links;
+  std::vector<int2> init(N > 0 ? N : 1);
+  std::vector<int32_t> loop(L > 0 ? L : 1, -1);
+  if (n_phases_host) {          // every check before the current program is touched
+    if (max_phases <= 0 || !min_dur_host || !max_dur_host || !open_host || !major_host || !yellow_host || !init_host ||
+        !max_gap_host || !loop_pos_host)
+      return fail("tsc_set_actuated_program: bad argument");
+    if (h->smem_act > 232448) return fail("tsc_set_actuated_program: the actuated state does not fit in shared memory");
+    if (h->record && h->smem_rec_act > 232448)
+      return fail("tsc_set_actuated_program: record mode is on and its actuated state does not fit in shared memory");
+    phase.resize(NP); yel.resize(NP);
+    for (int l = 0; l < L; ++l) {
+      if (loop_pos_host[l] < -1 || loop_pos_host[l] > 65535)
+        return fail("tsc_set_actuated_program: lane " + std::to_string(l) + ": loop position outside [-1, 65535]");
+      loop[l] = loop_pos_host[l];
+    }
+    for (int i = 0; i < N; ++i) {
+      const int np_ = n_phases_host[i];
+      const std::string who = "tsc_set_actuated_program: node " + std::to_string(i);
+      if (np_ < 1 || np_ > max_phases) return fail(who + " has " + std::to_string(np_) + " phases, outside [1, max_phases]");
+      if (max_gap_host[i] < 0) return fail(who + ": max_gap below 0");
+      for (int k = 0; k < np_; ++k) {
+        const size_t e = (size_t)i * max_phases + k;
+        const std::string ph = who + ": phase " + std::to_string(k);
+        if (min_dur_host[e] < 1 || max_dur_host[e] < min_dur_host[e])
+          return fail(ph + " needs 1 <= min_dur <= max_dur");
+        if (max_dur_host[e] > (1 << 30)) return fail(ph + ": max_dur above 2^30 s");
+        if (yellow_host[e] & open_host[e]) return fail(ph + " has a link open and yellow");
+        if (major_host[e] & ~open_host[e]) return fail(ph + " has a major link not open");
+        phase[e] = make_uint4((uint32_t)min_dur_host[e], (uint32_t)max_dur_host[e], open_host[e], major_host[e]);
+        yel[e] = yellow_host[e];
+      }
+      const int k0 = init_host[2 * i], e0 = init_host[2 * i + 1];
+      if (k0 < 0 || k0 >= np_ || e0 < 0 || e0 > (1 << 30))
+        return fail(who + ": initial state outside [0, n_phases) x [0, 2^30]");
+      init[i] = make_int2(k0, e0);
+      const int first = (int)links.size();
+      for (size_t j = 0; j < h->mp_node.size(); ++j) {      // the node's controlled links, in link order
+        if (h->mp_node[j] != i || h->mp_from[j] < 0) continue;
+        const int tl = h->mp_tlidx[j], from = h->mp_from[j];
+        if (tl < 0 || tl >= TSC_MAX_NODE_LINKS || from >= L) return fail(who + ": link out of range");
+        if (loop[from] < 0) return fail(who + ": lane " + std::to_string(from) + " is the from-lane of a controlled link "
+                                               "and has no loop");
+        links.push_back((uint32_t)from | ((uint32_t)tl << 10));
+      }
+      node[i] = make_int4(np_, max_gap_host[i], first, (int)links.size());
+    }
+  }
+  CK(cudaSetDevice(h->device));
+  CK(cudaDeviceSynchronize());          // no launch in flight still reads the previous program
+  free_actuated(h);
+  if (!n_phases_host) return 0;
+  cudaFree(h->d_fx_node); cudaFree(h->d_fx_phase);     // one signal program at a time
+  h->d_fx_node = nullptr; h->d_fx_phase = nullptr; h->fx_max_phases = 0;
+  CK(cudaFuncSetAttribute(tsc_step_kernel<false, CTL_ACTUATED>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                          h->smem_act));
+  if (h->smem_rec_act <= 232448)      // else record mode is refused while this program is set
+    CK(cudaFuncSetAttribute(tsc_step_kernel<true, CTL_ACTUATED>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                            h->smem_rec_act));
+  if (links.empty()) links.push_back(0);
+  const size_t lpad = h->args.net.lpad;
+  cudaError_t e = cudaMalloc(&h->d_ac_node, node.size() * sizeof(int4));
+  if (e == cudaSuccess) e = cudaMalloc(&h->d_ac_phase, NP * sizeof(uint4));
+  if (e == cudaSuccess) e = cudaMalloc(&h->d_ac_yel, NP * sizeof(uint32_t));
+  if (e == cudaSuccess) e = cudaMalloc(&h->d_ac_link, links.size() * sizeof(uint32_t));
+  if (e == cudaSuccess) e = cudaMalloc(&h->d_ac_loop, loop.size() * sizeof(int32_t));
+  if (e == cudaSuccess) e = cudaMalloc(&h->d_ac_init, init.size() * sizeof(int2));
+  if (e == cudaSuccess) e = cudaMalloc(&h->d_ac_state, (size_t)R * init.size() * sizeof(int2));
+  if (e == cudaSuccess) e = cudaMalloc(&h->d_ac_gap, (size_t)R * lpad + 16);
+  if (e == cudaSuccess) e = cudaMemcpy(h->d_ac_node, node.data(), node.size() * sizeof(int4), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaMemcpy(h->d_ac_phase, phase.data(), NP * sizeof(uint4), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaMemcpy(h->d_ac_yel, yel.data(), NP * sizeof(uint32_t), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess)
+    e = cudaMemcpy(h->d_ac_link, links.data(), links.size() * sizeof(uint32_t), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaMemcpy(h->d_ac_loop, loop.data(), loop.size() * sizeof(int32_t), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaMemcpy(h->d_ac_init, init.data(), init.size() * sizeof(int2), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) {
+    tsc_actuated_init_kernel<<<R, 64>>>(h->d_ac_state, h->d_ac_gap, h->d_ac_init, N, (int)lpad, R);
+    e = cudaGetLastError();
+  }
+  if (e == cudaSuccess) e = cudaDeviceSynchronize();
+  if (e != cudaSuccess) {       // the program stays off
+    free_actuated(h);
+    return fail(std::string("tsc_set_actuated_program: ") + cudaGetErrorString(e));
+  }
+  h->ac_max_phases = max_phases;
+  return 0;
+}
+
+extern "C" int tsc_get_program_phase(tsc_handle* h, int32_t* phase_dev, void* stream) {
+  if (!h || !phase_dev) return fail("tsc_get_program_phase: bad argument");
+  if (!has_program(h)) return fail("tsc_get_program_phase: no signal program is set");
+  CK(cudaSetDevice(h->device));
+  StepArgs a = h->args;
+  a.fx_node = h->d_fx_node; a.fx_phase = h->d_fx_phase; a.fx_max_phases = h->fx_max_phases;
+  a.ac_state = h->d_ac_state;
+  const int64_t RN = (int64_t)h->R * h->n_nodes;
+  if (RN == 0) return 0;
+  tsc_program_phase_kernel<<<(unsigned)((RN + 127) / 128), 128, 0, (cudaStream_t)stream>>>(a, RN, phase_dev);
+  CK(cudaGetLastError());
+  return 0;
+}
+
 static int launch(tsc_handle* h, int n_sub, const int32_t* action, const float* fp, float* obs, float* reward,
                   float* greward, uint8_t* done, cudaStream_t st, int rep0 = 0, int count = -1, int sub0 = 0) {
   StepArgs a = h->args;
@@ -1287,18 +1521,24 @@ static int launch(tsc_handle* h, int n_sub, const int32_t* action, const float* 
   }
   a.n_sub = n_sub; a.action = action; a.fp = fp; a.obs = obs; a.reward = reward; a.greward = greward; a.done = done;
   a.rep0 = rep0;
-  const bool fixed = h->d_fx_node != nullptr;
+  const bool fixed = h->d_fx_node != nullptr, act = h->d_ac_state != nullptr;
   if (fixed) { a.fx_node = h->d_fx_node; a.fx_phase = h->d_fx_phase; a.fx_max_phases = h->fx_max_phases; }
+  if (act) {
+    a.ac_node = h->d_ac_node; a.ac_phase = h->d_ac_phase; a.ac_yel = h->d_ac_yel; a.ac_link = h->d_ac_link;
+    a.ac_loop = h->d_ac_loop; a.ac_state = h->d_ac_state; a.ac_gap = h->d_ac_gap; a.ac_max_phases = h->ac_max_phases;
+  }
   const unsigned grid = count < 0 ? h->R : count;
   if (h->record) {
     a.trip = h->d_trip; a.trip_log = h->d_trip_log; a.trip_cnt = h->d_trip_cnt; a.trip_cap = h->trip_cap;
     a.sub0 = sub0;
-    if (fixed) tsc_step_kernel<true, true><<<grid, TSC_THREADS, h->smem_rec, st>>>(a);
-    else tsc_step_kernel<true, false><<<grid, TSC_THREADS, h->smem_rec, st>>>(a);
+    if (act) tsc_step_kernel<true, CTL_ACTUATED><<<grid, TSC_THREADS, h->smem_rec_act, st>>>(a);
+    else if (fixed) tsc_step_kernel<true, CTL_FIXED_TIME><<<grid, TSC_THREADS, h->smem_rec, st>>>(a);
+    else tsc_step_kernel<true, CTL_ACTION><<<grid, TSC_THREADS, h->smem_rec, st>>>(a);
   } else {
     a.sub0 = sub0;
-    if (fixed) tsc_step_kernel<false, true><<<grid, TSC_THREADS, h->smem, st>>>(a);
-    else tsc_step_kernel<false, false><<<grid, TSC_THREADS, h->smem, st>>>(a);
+    if (act) tsc_step_kernel<false, CTL_ACTUATED><<<grid, TSC_THREADS, h->smem_act, st>>>(a);
+    else if (fixed) tsc_step_kernel<false, CTL_FIXED_TIME><<<grid, TSC_THREADS, h->smem, st>>>(a);
+    else tsc_step_kernel<false, CTL_ACTION><<<grid, TSC_THREADS, h->smem, st>>>(a);
   }
   CK(cudaGetLastError());
   return 0;
@@ -1312,7 +1552,7 @@ extern "C" int tsc_observe(tsc_handle* h, const float* fp_dev, float* obs_dev, v
 
 extern "C" int tsc_step(tsc_handle* h, const int32_t* action_dev, const float* fp_dev, float* obs_dev,
                         float* reward_dev, float* greward_dev, uint8_t* done_dev, void* stream) {
-  if (!h || (!action_dev && !h->d_fx_node)) return fail("tsc_step: bad argument");
+  if (!h || (!action_dev && !has_program(h))) return fail("tsc_step: bad argument");
   CK(cudaSetDevice(h->device));
   return launch(h, h->args.cfg.control_interval_sec, action_dev, fp_dev, obs_dev, reward_dev, greward_dev, done_dev,
                 (cudaStream_t)stream);
@@ -1320,7 +1560,7 @@ extern "C" int tsc_step(tsc_handle* h, const int32_t* action_dev, const float* f
 
 extern "C" int tsc_step_host(tsc_handle* h, const int32_t* action_host, const float* fp_host, float* obs_host,
                              float* reward_host, float* greward_host, uint8_t* done_host, void* stream) {
-  if (!h || (!action_host && !h->d_fx_node)) return fail("tsc_step_host: bad argument");
+  if (!h || (!action_host && !has_program(h))) return fail("tsc_step_host: bad argument");
   CK(cudaSetDevice(h->device));
   cudaStream_t st = (cudaStream_t)stream;
   const size_t R = h->R, N = h->n_nodes;
@@ -1341,7 +1581,7 @@ extern "C" int tsc_step_host(tsc_handle* h, const int32_t* action_host, const fl
 static int step_host_range(tsc_handle* h, int32_t rep0, int32_t count, const int32_t* action_host,
                            const float* fp_host, float* obs_host, float* reward_host, float* greward_host,
                            uint8_t* done_host, void* stream, bool sync) {
-  if (!h || (!action_host && !h->d_fx_node) || rep0 < 0 || count <= 0 || rep0 + count > h->R)
+  if (!h || (!action_host && !has_program(h)) || rep0 < 0 || count <= 0 || rep0 + count > h->R)
     return fail("tsc_step_host_range: bad argument");
   CK(cudaSetDevice(h->device));
   cudaStream_t st = (cudaStream_t)stream;
@@ -1378,6 +1618,8 @@ extern "C" int tsc_set_record(tsc_handle* h, int32_t on) {
   if (!h) return fail("tsc_set_record: null handle");
   CK(cudaSetDevice(h->device));
   CK(cudaDeviceSynchronize());
+  if (on && h->d_ac_state && h->smem_rec_act > 232448)
+    return fail("tsc_set_record: an actuated program is set and its record-mode state does not fit in shared memory");
   if (on && !h->d_trip) {
     if (h->smem_rec > 232448) return fail("tsc_set_record: the record-mode ring image does not fit in shared memory");
     h->trip_cap = 8192;
@@ -1396,7 +1638,7 @@ extern "C" int tsc_set_record(tsc_handle* h, int32_t on) {
 extern "C" int tsc_step_record(tsc_handle* h, const int32_t* action_dev, const float* fp_dev, float* obs_dev,
                                float* reward_dev, float* greward_dev, uint8_t* done_dev, float* sub_stats_dev,
                                void* stream) {
-  if (!h || (!action_dev && !h->d_fx_node)) return fail("tsc_step_record: bad argument");
+  if (!h || (!action_dev && !has_program(h))) return fail("tsc_step_record: bad argument");
   if (!h->record) return fail("tsc_step_record: record mode is off (tsc_set_record)");
   CK(cudaSetDevice(h->device));
   const int ci = h->args.cfg.control_interval_sec;

@@ -1,7 +1,7 @@
 """Scenario envs with the reference's names, and the two constructors the entry points share (scripts/train.py,
 scripts/evaluate.py): `make_env` picks the env class from `[ENV_CONFIG]` as main.py:init_env does, `greedy_controller`
 the scenario's greedy policy, `maxpressure_controller` the max-pressure one, `fixedtime_controller` the fixed-time
-one."""
+one, `actuated_controller` the vehicle-actuated one."""
 
 
 # the [ENV_CONFIG] keys that set each scenario's traffic demand and nothing else: two configs that differ only in these
@@ -102,4 +102,13 @@ def fixedtime_controller(env):
     from .fixedtime import FixedTimeController
     ctrl = FixedTimeController(env)
     env._ensure_sim().set_signal_program(ctrl.program)
+    return ctrl
+
+
+def actuated_controller(env):
+    """The vehicle-actuated controller (envs.actuated) of any scenario env, `name = 'actuated'`; puts the env's
+    simulator into actuated mode, every replica running the env's actuated programs."""
+    from .actuated import ActuatedController
+    ctrl = ActuatedController(env)
+    env._ensure_sim().set_actuated_program(ctrl.program)
     return ctrl

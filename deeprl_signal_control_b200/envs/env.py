@@ -121,6 +121,10 @@ class TrafficSimulator:
         test_seeds = [int(s) for s in config.get('test_seeds').split(',')]
         # optional key: a SUMO additional file whose <tlLogic> programs replace the net's in fixed-time control
         self.tll_file = config.get('tll_file', fallback=None)
+        # optional keys of actuated control (envs.actuated), read only by an 'actuated' env
+        if self.agent == 'actuated':
+            from .actuated import config_overrides
+            self.actuated_cfg = config_overrides(config)
         self.n_replicas = int(n_replicas)
         self.device = device
         self._init_map()
@@ -330,6 +334,6 @@ class TrafficSimulator:
         if self.n_replicas > 1:
             return obs.copy(), reward.copy(), bool(done[0]), greward.copy()
         reward0 = reward[0].astype(np.float64)
-        if self.train_mode and self.agent in ('a2c', 'greedy', 'maxpressure', 'fixedtime'):
+        if self.train_mode and self.agent in ('a2c', 'greedy', 'maxpressure', 'fixedtime', 'actuated'):
             reward0 = float(greward[0])                              # envs/env.py:593-594
         return self._split_obs(obs[0]), reward0, bool(done[0]), float(greward[0])

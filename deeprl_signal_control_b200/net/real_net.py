@@ -428,8 +428,8 @@ def real_net_tables(agent: str = 'ma2c', net_file: str | None = None, flow_rate:
     path = _CACHE % agent
     if not os.path.exists(path) and agent in ('iqll', 'iqld'):
         path = _CACHE % 'ia2c'      # IQL agents observe what IA2C agents do (AGENT_MODES, build_obs_program)
-    if not os.path.exists(path) and agent in ('maxpressure', 'fixedtime'):
-        path = _CACHE % 'greedy'    # and the max-pressure and fixed-time controllers what the greedy one does
+    if not os.path.exists(path) and agent in ('maxpressure', 'fixedtime', 'actuated'):
+        path = _CACHE % 'greedy'    # and the max-pressure, fixed-time and actuated controllers what the greedy one does
     if not os.path.exists(path):
         raise FileNotFoundError('no Monaco net file given and no derived table cache at %s' % path)
     net = load_tables(path)

@@ -46,7 +46,9 @@ def read_tls_programs(*files: str) -> Dict[str, List[str]]:
 def read_signal_programs(*files: str) -> Dict[str, dict]:
     """{tlLogic id: {'type', 'offset', 'phases': [[duration, state], ...]}} of the whole static programs in net /
     additional files (later files override; a '.gz' file is read through gzip), the attribute values as the file writes
-    them.  envs.fixedtime checks and runs them."""
+    them.  envs.fixedtime checks and runs them.  Two keys appear only where the file has them: 'phase_attrs', one
+    {attribute: value} per phase of its attributes other than duration and state (minDur, maxDur, next, ...), and
+    'params', {key: value} of the tlLogic's <param>s; envs.actuated reads them."""
     import gzip
     out: Dict[str, dict] = {}
     for f in files:
@@ -55,8 +57,16 @@ def read_signal_programs(*files: str) -> Dict[str, dict]:
         with (gzip.open(f) if f.endswith('.gz') else open(f, 'rb')) as fh:
             root = ET.parse(fh).getroot()
         for tl in root.iter('tlLogic'):
-            out[tl.get('id')] = {'type': tl.get('type', 'static'), 'offset': tl.get('offset', '0'),
-                                 'phases': [[ph.get('duration'), ph.get('state')] for ph in tl.findall('phase')]}
+            phases = tl.findall('phase')
+            prog = {'type': tl.get('type', 'static'), 'offset': tl.get('offset', '0'),
+                    'phases': [[ph.get('duration'), ph.get('state')] for ph in phases]}
+            attrs = [{k: v for k, v in ph.attrib.items() if k not in ('duration', 'state')} for ph in phases]
+            if any(attrs):
+                prog['phase_attrs'] = attrs
+            params = {p.get('key'): p.get('value') for p in tl.findall('param')}
+            if params:
+                prog['params'] = params
+            out[tl.get('id')] = prog
     return out
 
 

@@ -73,9 +73,10 @@ _CT = {np.dtype(np.float32): C.c_float, np.dtype(np.int32): C.c_int32,
 
 OBJECTIVES = {"queue": 0, "wait": 1, "hybrid": 2}
 # reward shaping families of reference envs/env.py:591-631
-# maxpressure (envs.maxpressure_controller) and fixedtime (envs.fixedtime_controller) are non-learning controllers like
-# greedy and observe what greedy does
-AGENT_MODES = {"greedy": 0, "maxpressure": 0, "fixedtime": 0, "a2c": 0, "ia2c": 1, "iqll": 1, "iqld": 1, "ma2c": 2}
+# maxpressure (envs.maxpressure_controller), fixedtime (envs.fixedtime_controller) and actuated
+# (envs.actuated_controller) are non-learning controllers like greedy and observe what greedy does
+AGENT_MODES = {"greedy": 0, "maxpressure": 0, "fixedtime": 0, "actuated": 0, "a2c": 0, "ia2c": 1, "iqll": 1, "iqld": 1,
+               "ma2c": 2}
 
 
 @dataclass
@@ -307,13 +308,13 @@ def build_obs_program(net: NetTables, agent: str, coop_gamma: float, use_wait: b
     """Observation layout of reference envs/env.py:163-205 and dims of :303-323.
 
     per agent: [own wave | neighbour waves (x coop_gamma iff ma2c) | own wait | neighbour
-    fingerprints (ma2c)]; greedy, maxpressure and fixedtime: own wave only."""
+    fingerprints (ma2c)]; greedy, maxpressure, fixedtime and actuated: own wave only."""
     names = net.node_names
     idx = {n: i for i, n in enumerate(names)}
     det_off = net.node_det_off
     kinds, idxs, scales, obs_off = [], [], [], [0]
     n_s_ls, n_w_ls, n_f_ls = [], [], []
-    own_only = agent in ("greedy", "maxpressure", "fixedtime")
+    own_only = agent in ("greedy", "maxpressure", "fixedtime", "actuated")
     marl = agent != "a2c" and not own_only
     for i, name in enumerate(names):
         own = list(range(det_off[i], det_off[i + 1]))

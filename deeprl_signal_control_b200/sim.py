@@ -210,6 +210,33 @@ class BatchedSim:
                                                     (program.yellow, np.uint32), (program.offset, np.int32))]
         _lib.check(lib.tsc_set_signal_program(self._h, program.max_phases, *(x.ctypes.data for x in a)))
 
+    def set_actuated_program(self, program=None, max_gap=None) -> None:
+        """Actuated control (`tsc_set_actuated_program`): every replica runs `program` (an envs.actuated.ActuatedProgram
+        in the net's node order) second by second from its initial state, which reset() restores; the steps read no
+        action, as under set_signal_program.  `max_gap` (int32 [n_nodes], whole seconds) replaces the program's.
+        None returns to action-driven stepping."""
+        lib = _lib.lib()
+        if program is None:
+            _lib.check(lib.tsc_set_actuated_program(self._h, 0, *([None] * 9)))
+            return
+        if len(program.n_phases) != self.net.n_nodes or len(program.loop_pos) != self.net.n_lanes:
+            raise ValueError("set_actuated_program: %d node programs and %d loop positions for %d nodes and %d lanes"
+                             % (len(program.n_phases), len(program.loop_pos), self.net.n_nodes, self.net.n_lanes))
+        mg = program.max_gap if max_gap is None else max_gap
+        a = [np.ascontiguousarray(x, t) for x, t in (
+            (program.n_phases, np.int32), (program.min_dur, np.int32), (program.max_dur, np.int32),
+            (program.open, np.uint32), (program.major, np.uint32), (program.yellow, np.uint32), (program.init, np.int32),
+            (mg, np.int32), (program.loop_pos, np.int32))]
+        _lib.check(lib.tsc_set_actuated_program(self._h, program.max_phases, *(x.ctypes.data for x in a)))
+
+    def program_phase(self, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """`tsc_get_program_phase`: int32 [R, n_nodes] on the device, the phase every node's signal program shows in
+        the next simulated second (into `out` when given)."""
+        ph = torch.empty(self.R, self.net.n_nodes, dtype=torch.int32, device=self.device) if out is None else out
+        assert ph.dtype == torch.int32 and ph.is_contiguous() and ph.numel() == self.R * self.net.n_nodes
+        _lib.check(_lib.lib().tsc_get_program_phase(self._h, ptr(ph), self._stream()))
+        return ph
+
     # ---- parity taps ---------------------------------------------------------------------
     def counts(self):
         n = self.net

@@ -167,6 +167,34 @@ int tsc_set_signal_program(tsc_handle* h, int32_t max_phases, const int32_t* n_p
                            const uint32_t* open_host, const uint32_t* major_host, const uint32_t* yellow_host,
                            const int32_t* offset_host);
 
+/* Vehicle-actuated signal control (synchronous, like tsc_set_signal_program; validates every table before it replaces
+ * anything).  Node i runs n_phases_host[i] phases in order (1 <= n <= max_phases); phase k (entry [i][k] of the
+ * [n_nodes][max_phases] host arrays) shows the link masks open_host, major_host and yellow_host as in
+ * tsc_set_signal_program and lasts between min_dur_host[i][k] and max_dur_host[i][k] seconds
+ * (1 <= min_dur <= max_dur <= 2^30).  loop_pos_host[n_lanes]: the induction loop of each lane, in 1/64 m from the
+ * lane start (0..65535), or -1 for none; every from-lane of a controlled link needs one.  Each lane keeps a gap g, the
+ * seconds since its loop was last covered (saturating at 255, 255 after a reset): a vehicle covers it in a second iff
+ * xq - Lq <= X <= xnq, xq / xnq its stored front position before / after the second's move (1/64 m; a head vehicle
+ * that crosses or arrives has xnq = +inf), Lq = veh_len in 1/64 m.  At the end of every simulated second a node whose
+ * phase k has run e seconds (this one included) advances to k + 1 mod n when e >= max_dur, or when e >= min_dur and
+ * every loop on the from-lane of a link open in k has g >= max_gap_host[i] (>= 0; 0 ends every phase at min_dur, 256
+ * or more runs it to max_dur); the new phase shows from the next second on.  init_host [n_nodes][2] = {phase,
+ * elapsed seconds} of every node at simulated second 0 (0 <= elapsed <= 2^30).
+ * Allocates the per-replica state ([R][n_nodes] phases, [R][lanes] gaps) and initialises every replica; tsc_reset
+ * re-initialises it.  When the record-mode actuated state does not fit in shared memory, this call refuses while
+ * record mode is on and tsc_set_record refuses while a program is set.  While set, the step calls behave as under tsc_set_signal_program (no action read, prev_action
+ * kept, the phase tap holding the phase in force during the interval's first second).  Setting it turns a
+ * tsc_set_signal_program program off, and setting that turns this one off; n_phases_host NULL turns it off and frees
+ * the state. */
+int tsc_set_actuated_program(tsc_handle* h, int32_t max_phases, const int32_t* n_phases_host,
+                             const int32_t* min_dur_host, const int32_t* max_dur_host, const uint32_t* open_host,
+                             const uint32_t* major_host, const uint32_t* yellow_host, const int32_t* init_host,
+                             const int32_t* max_gap_host, const int32_t* loop_pos_host);
+
+/* phase_dev [R][n_nodes] int32: the phase of every node's signal program (tsc_set_signal_program or
+ * tsc_set_actuated_program) in force during the next simulated second.  Fails when no program is set. */
+int tsc_get_program_phase(tsc_handle* h, int32_t* phase_dev, void* stream);
+
 /* Replaces _get_state() without stepping (the observation reset() returns,
  * envs/env.py:561,163-205).  fp_dev: [R][n_nodes][max_na] policy probabilities installed by
  * update_fingerprint (envs/env.py:633-635) or NULL (zeros).  obs_dev: [R][n_obs]. */

@@ -7,8 +7,9 @@
 
 DIR holds `data/*.ini` (the run's config, [ENV_CONFIG] + [MODEL_CONFIG]) and, unless the agent is a controller,
 `model/checkpoint-<step>.npz` as written by IA2C.save / MA2C.save / IQL.save.  The agent is the directory's name, as in
-the reference (main.py:179-190): ia2c, ma2c, the controllers greedy, maxpressure (envs.maxpressure) and fixedtime (the
-net's fixed-time signal programs, envs.fixedtime), iqld
+the reference (main.py:179-190): ia2c, ma2c, the controllers greedy, maxpressure (envs.maxpressure), fixedtime (the
+net's fixed-time signal programs, envs.fixedtime) and actuated (vehicle-actuated control on the net's programs,
+envs.actuated), iqld
 (IQL with DeepQPolicy) or any other name, e.g. iqll (IQL with LRQPolicy).  The controllers ignore
 --evaluation-policy-type and --policy.  Writes the reference's `<scenario>_<agent>_{control,traffic,trip}.csv` and
 `<agent>_summary.json` (mean / std over episodes of the per-episode mean step reward, mean avg_queue / avg_speed_mps /
@@ -24,8 +25,8 @@ import sys
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
-from deeprl_signal_control_b200.envs import (fixedtime_controller, greedy_controller, make_env,  # noqa: E402
-                                             maxpressure_controller)
+from deeprl_signal_control_b200.envs import (actuated_controller, fixedtime_controller,  # noqa: E402
+                                             greedy_controller, make_env, maxpressure_controller)
 
 
 def parse_args(argv=None):
@@ -42,7 +43,7 @@ def parse_args(argv=None):
 
 def iql_model_type(agent):
     """main.py:185-190: 'iqld' is the DeepQPolicy IQL, every other agent name that is not an A2C variant or a controller
-    (greedy, maxpressure, fixedtime) the LRQPolicy one."""
+    (greedy, maxpressure, fixedtime, actuated) the LRQPolicy one."""
     return 'dqn' if agent == 'iqld' else 'lr'
 
 
@@ -75,6 +76,8 @@ def main(argv=None):
         model = maxpressure_controller(env)
     elif agent == "fixedtime":
         model = fixedtime_controller(env)
+    elif agent == "actuated":
+        model = actuated_controller(env)
     else:
         from deeprl_signal_control_b200.agents.models import IA2C, IQL, MA2C
         mc = config["MODEL_CONFIG"]
@@ -84,8 +87,8 @@ def main(argv=None):
         elif agent == "ia2c":
             model = IA2C(env.n_s_ls, env.n_a_ls, env.n_w_ls, 0, mc, **kw)
         elif agent == "a2c":
-            raise SystemExit("batched evaluation covers greedy, maxpressure, fixedtime, ia2c, ma2c and IQL (got %r)"
-                             % agent)
+            raise SystemExit("batched evaluation covers greedy, maxpressure, fixedtime, actuated, ia2c, ma2c and IQL "
+                             "(got %r)" % agent)
         else:
             model = IQL(env.n_s_ls, env.n_a_ls, env.n_w_ls, 0, mc, seed=0, model_type=iql_model_type(agent))
         if not model.load(os.path.join(agent_dir, "model") + "/"):

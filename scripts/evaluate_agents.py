@@ -2,14 +2,15 @@
 `main.py --base-dir B evaluate --agents ...` (main.py:35-43, 158-222) on the grouped device evaluator
 (deeprl_signal_control_b200/agents/evaluator.py:GroupEvaluator).
 
-  python scripts/evaluate_agents.py --base-dir B --agents greedy,maxpressure,fixedtime,ia2c,ma2c,seed12/ma2c
+  python scripts/evaluate_agents.py --base-dir B --agents greedy,maxpressure,fixedtime,actuated,ia2c,ma2c,seed12/ma2c
                                     [--evaluation-policy-type default|stochastic|deterministic]
                                     [--evaluation-seeds 10000,20000,...,100000] [--policy lstm|fc]
                                     [--demand k=v[,k=v...] ...] [--share-demand]
 
-Each entry is an agent directory under B holding `data/*.ini` and, unless the agent is greedy, maxpressure or fixedtime,
-`model/checkpoint-*`.  The agent is the entry's last path component (ia2c, ma2c, greedy, maxpressure = the max-pressure
-controller, fixedtime = the net's fixed-time signal programs, iqld = IQL with DeepQPolicy, any other name = IQL with
+Each entry is an agent directory under B holding `data/*.ini` and, unless the agent is greedy, maxpressure, fixedtime or
+actuated, `model/checkpoint-*`.  The agent is the entry's last path component (ia2c, ma2c, greedy, maxpressure = the max-pressure
+controller, fixedtime = the net's fixed-time signal programs, actuated = vehicle-actuated control on the net's
+programs, iqld = IQL with DeepQPolicy, any other name = IQL with
 LRQPolicy; a2c is refused).  An entry without a `/` writes the reference's
 `<scenario>_<agent>_{control,traffic,trip}.csv` into B/eva_data/, an entry p/<agent> into B/eva_data/p/, each next to
 `<agent>_summary.json` (as scripts/evaluate.py writes it).  B/eva_data/summary.csv compares the entries (one row each:
