@@ -890,23 +890,25 @@ extern "C" int tscl_q_create(const tscl_qdims* x, int32_t device, tscl_qhandle**
     tscl_q_destroy(h);
     return tsc_set_error("tscl_q_create: the weights and tiles of one agent need more shared memory than a CTA has");
   }
+  // the shared-memory limit belongs to the kernel, not the handle: the opt-in maximum, so that a handle created later
+  // for a smaller layout does not lower it below what a live handle's launches need
   const void* fn = dqn ? (const void*)q_fwd_kernel<true> : (const void*)q_fwd_kernel<false>;
-  LCK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem));
+  LCK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, optin));
   LCK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&h->ctas_per_sm, fn, 256, h->smem));
   if (h->ctas_per_sm < 1) h->ctas_per_sm = 1;
   const void* ex = dqn ? (const void*)q_fwd_kernel<true, true> : (const void*)q_fwd_kernel<false, true>;
-  LCK(cudaFuncSetAttribute(ex, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem));
+  LCK(cudaFuncSetAttribute(ex, cudaFuncAttributeMaxDynamicSharedMemorySize, optin));
   const void* fg = dqn ? (const void*)q_fwd_g_kernel<true> : (const void*)q_fwd_g_kernel<false>;
-  LCK(cudaFuncSetAttribute(fg, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem));
+  LCK(cudaFuncSetAttribute(fg, cudaFuncAttributeMaxDynamicSharedMemorySize, optin));
   const void* eg = dqn ? (const void*)q_fwd_g_kernel<true, true> : (const void*)q_fwd_g_kernel<false, true>;
-  LCK(cudaFuncSetAttribute(eg, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem));
+  LCK(cudaFuncSetAttribute(eg, cudaFuncAttributeMaxDynamicSharedMemorySize, optin));
   const size_t td_smem = (size_t)q_td_smem_layout(d).total * sizeof(float);
   if (td_smem <= (size_t)optin) {
     const void* td = dqn ? (const void*)q_td_kernel<true> : (const void*)q_td_kernel<false>;
-    LCK(cudaFuncSetAttribute(td, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)td_smem));
+    LCK(cudaFuncSetAttribute(td, cudaFuncAttributeMaxDynamicSharedMemorySize, optin));
     LCK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&h->td_ctas_per_sm, td, 256, td_smem));
     const void* tg = dqn ? (const void*)q_td_kernel<true, true> : (const void*)q_td_kernel<false, true>;
-    LCK(cudaFuncSetAttribute(tg, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)td_smem));
+    LCK(cudaFuncSetAttribute(tg, cudaFuncAttributeMaxDynamicSharedMemorySize, optin));
     if (h->td_ctas_per_sm < 1) h->td_ctas_per_sm = 1;
     h->td_smem = td_smem;
   }

@@ -7,7 +7,7 @@
 
 DIR holds `data/*.ini` (the run's config, [ENV_CONFIG] + [MODEL_CONFIG]) and, unless the agent is a controller,
 `model/checkpoint-<step>.npz` as written by IA2C.save / MA2C.save / IQL.save.  The agent is the directory's name, as in
-the reference (main.py:179-190): ia2c, ma2c, the controllers greedy, maxpressure (envs.maxpressure), fixedtime (the
+the reference (main.py:179-190; agents/evaluator.py:entry_model and build_model): ia2c, ma2c, the controllers greedy, maxpressure (envs.maxpressure), fixedtime (the
 net's fixed-time signal programs, envs.fixedtime) and actuated (vehicle-actuated control on the net's programs,
 envs.actuated), iqld
 (IQL with DeepQPolicy) or any other name, e.g. iqll (IQL with LRQPolicy).  The controllers ignore
@@ -25,8 +25,7 @@ import sys
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
-from deeprl_signal_control_b200.envs import (actuated_controller, fixedtime_controller,  # noqa: E402
-                                             greedy_controller, make_env, maxpressure_controller)
+from deeprl_signal_control_b200.envs import make_env  # noqa: E402
 
 
 def parse_args(argv=None):
@@ -39,12 +38,6 @@ def parse_args(argv=None):
     p.add_argument("--output-dir", default=None)
     p.add_argument("--policy", default="lstm", choices=["lstm", "fc"])
     return p.parse_args(argv)
-
-
-def iql_model_type(agent):
-    """main.py:185-190: 'iqld' is the DeepQPolicy IQL, every other agent name that is not an A2C variant or a controller
-    (greedy, maxpressure, fixedtime, actuated) the LRQPolicy one."""
-    return 'dqn' if agent == 'iqld' else 'lr'
 
 
 def main(argv=None):
@@ -70,30 +63,8 @@ def main(argv=None):
     os.makedirs(out, exist_ok=True)
     out = out.rstrip("/") + "/"
     env = make_env(cfg, len(seeds), out)
-    if agent == "greedy":
-        model = greedy_controller(env)
-    elif agent == "maxpressure":
-        model = maxpressure_controller(env)
-    elif agent == "fixedtime":
-        model = fixedtime_controller(env)
-    elif agent == "actuated":
-        model = actuated_controller(env)
-    else:
-        from deeprl_signal_control_b200.agents.models import IA2C, IQL, MA2C
-        mc = config["MODEL_CONFIG"]
-        kw = dict(n_replicas=1, obs_off=env._tables.node_obs_off, policy=a.policy)
-        if agent == "ma2c":
-            model = MA2C(env.n_s_ls, env.n_a_ls, env.n_w_ls, env.n_f_ls, 0, mc, **kw)
-        elif agent == "ia2c":
-            model = IA2C(env.n_s_ls, env.n_a_ls, env.n_w_ls, 0, mc, **kw)
-        elif agent == "a2c":
-            raise SystemExit("batched evaluation covers greedy, maxpressure, fixedtime, actuated, ia2c, ma2c and IQL "
-                             "(got %r)" % agent)
-        else:
-            model = IQL(env.n_s_ls, env.n_a_ls, env.n_w_ls, 0, mc, seed=0, model_type=iql_model_type(agent))
-        if not model.load(os.path.join(agent_dir, "model") + "/"):
-            raise SystemExit("no checkpoint under %s/model/" % agent_dir)
-    from deeprl_signal_control_b200.agents.evaluator import Evaluator
+    from deeprl_signal_control_b200.agents.evaluator import Evaluator, build_model, entry_model
+    model = build_model(entry_model(agent), agent_dir, env, config, a.policy)
     ev = Evaluator(env, model, out, policy_type=a.evaluation_policy_type)
     mean, std = ev.run()
     control, traffic, trip = ev.recorded

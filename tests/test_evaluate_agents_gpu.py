@@ -8,6 +8,8 @@
 * End to end: a base directory with greedy, ia2c, ma2c, iqll, iqld, two ma2c seed members and two ma2c coop_gamma members
   (short episodes, the reference's widths): every entry's three CSVs and <agent>_summary.json are byte-identical to
   scripts/evaluate.py on that directory alone, for the policy types default, deterministic and stochastic.
+* Two iqld directories of different widths (num_fc / num_h) on one simulator, one Q launch per layout: each entry's
+  CSVs and summary byte-identical to scripts/evaluate.py on that directory alone.
 """
 import configparser
 import ctypes as C
@@ -206,18 +208,18 @@ def _load(name):
     return mod
 
 
-def _make_base(base):
+def _make_base(base, entries):
     from tests.test_train_driver_gpu import A2C_MODEL, GRID, IQL_MODEL, TRAIN
     from deeprl_signal_control_b200.envs import make_env
     from deeprl_signal_control_b200.agents.models import IA2C, IQL, MA2C
-    for entry, changes, wseed in ENTRIES:
+    for entry, changes, wseed in entries:
         agent = os.path.basename(entry)
         model = A2C_MODEL if agent in ("ia2c", "ma2c", "greedy") else IQL_MODEL
         c = configparser.ConfigParser()
         c.read_string(model + TRAIN % (120, 120) + GRID % (agent, ",".join(map(str, SEEDS))))
         c["ENV_CONFIG"]["episode_length_sec"] = str(EPISODE_SEC)
-        for k, v in changes.items():
-            c["ENV_CONFIG"][k] = v
+        for k, v in changes.items():                    # a [MODEL_CONFIG] key where it names one, else [ENV_CONFIG]
+            c["MODEL_CONFIG" if k in c["MODEL_CONFIG"] else "ENV_CONFIG"][k] = v
         d = os.path.join(base, entry)
         for sub in ("data", "model"):
             os.makedirs(os.path.join(d, sub))
@@ -246,16 +248,16 @@ def _bytes(path):
         return f.read()
 
 
-@pytest.mark.parametrize("policy_type", ["default", "deterministic", "stochastic"])
-def test_evaluate_agents_equals_one_directory_at_a_time(tmp_path, policy_type):
+def _evaluate_against_solo(tmp_path, entries, policy_type):
+    """evaluate_agents.py on `entries`, then evaluate.py on each directory alone: the same bytes in every output."""
     base = str(tmp_path / "B")
-    _make_base(base)
+    _make_base(base, entries)
     seeds = ",".join(map(str, SEEDS))
-    out = _load("evaluate_agents").main(["--base-dir", base, "--agents", ",".join(e for e, _, _ in ENTRIES),
+    out = _load("evaluate_agents").main(["--base-dir", base, "--agents", ",".join(e for e, _, _ in entries),
                                          "--evaluation-policy-type", policy_type, "--evaluation-seeds", seeds])
-    assert [lab for lab, _ in out] == [e for e, _, _ in ENTRIES]
+    assert [lab for lab, _ in out] == [e for e, _, _ in entries]
     solo = _load("evaluate")
-    for entry, _, _ in ENTRIES:
+    for entry, _, _ in entries:
         agent = os.path.basename(entry)
         x = str(tmp_path / "solo" / entry)
         solo.main(["--agent-dir", os.path.join(base, entry), "--output-dir", x, "--evaluation-seeds", seeds,
@@ -265,5 +267,15 @@ def test_evaluate_agents_equals_one_directory_at_a_time(tmp_path, policy_type):
         for n in names:
             assert _bytes(os.path.join(got_dir, n)) == _bytes(os.path.join(x, n)), (entry, n)
     rows = open(os.path.join(base, "eva_data", "summary.csv")).read().splitlines()
-    assert len(rows) == 1 + len(ENTRIES) and rows[0].startswith("entry,mean_reward")
+    assert len(rows) == 1 + len(entries) and rows[0].startswith("entry,mean_reward")
     assert os.listdir(os.path.join(base, "eva_log"))
+
+
+@pytest.mark.parametrize("policy_type", ["default", "deterministic", "stochastic"])
+def test_evaluate_agents_equals_one_directory_at_a_time(tmp_path, policy_type):
+    _evaluate_against_solo(tmp_path, ENTRIES, policy_type)
+
+
+def test_iql_entries_of_two_layouts_equal_one_directory_at_a_time(tmp_path):
+    """Two iqld directories that share a simulator but not a Q layout: each layout has its own grouped launch."""
+    _evaluate_against_solo(tmp_path, [("w128/iqld", {}, 3), ("w64/iqld", {"num_fc": "64", "num_h": "32"}, 4)], "default")

@@ -323,7 +323,8 @@ def _read(path):
 CASES = {("large_grid", "ma2c", "lstm", 128): "v2", ("large_grid", "ia2c", "fc", 128): "fc",
          ("large_grid", "ia2c", "lstm", 64): "v1",
          ("real_net", "ma2c", "lstm", 128): "v2", ("real_net", "ia2c", "lstm", 128): "v2",
-         ("real_net", "ia2c", "lstm", 160): "v2", ("large_grid", "greedy", None, 0): None, ("real_net", "greedy", None, 0): None}
+         ("real_net", "ia2c", "lstm", 160): "v2", ("large_grid", "greedy", None, 0): "greedy",
+         ("real_net", "greedy", None, 0): "greedy"}
 
 
 @pytest.mark.parametrize("scenario,agent,policy,fw", list(CASES))

@@ -1,12 +1,11 @@
 """CPU: the pieces of batched IQL evaluation that need no GPU — a float64 restatement of the LRQPolicy / DeepQPolicy
 forward (agents/policies.py:341-389) against the reference graph's own q-values (tests/golden/learner_iql.npz), the
 flat Q parameter layout (agents/layout.py:QLayout) against IQL.nets and IQL checkpoints, the Monaco tables of the IQL
-agents, and the agent-name -> model-type map of scripts/evaluate.py (main.py:179-190)."""
+agents, and the agent-name -> model-type map both evaluation scripts use (evaluator.entry_model, main.py:179-190)."""
 import configparser
 import gzip
 import os
 import shutil
-import sys
 
 import numpy as np
 import pytest
@@ -148,12 +147,8 @@ def test_monaco_tables_of_iql_agents_equal_the_net_file(agent, tmp_path):
     assert a.n_w_ls == [0] * 28 and a.n_f_ls == [0] * 28
 
 
-def test_evaluate_script_maps_agent_names_like_main():
-    sys.path.insert(0, os.path.join(ROOT, "scripts"))
-    try:
-        import evaluate
-    finally:
-        sys.path.pop(0)
-    assert evaluate.iql_model_type("iqld") == "dqn"
-    assert evaluate.iql_model_type("iqll") == "lr"
-    assert evaluate.iql_model_type("iql") == "lr"            # main.py: every other name is IQL-LR
+def test_entry_model_maps_iql_agent_names_like_main():
+    from deeprl_signal_control_b200.agents.evaluator import entry_model
+    assert entry_model("iqld") == "dqn"
+    assert entry_model("iqll") == "lr"
+    assert entry_model("iql") == "lr"                        # main.py: every other name is IQL-LR
