@@ -17,7 +17,9 @@ A member's model is an IA2C / MA2C wrapper (agents/models.py; only its parameter
 (`model.name == 'greedy'`), the max-pressure controller (`model.name == 'maxpressure'`, envs.maxpressure_controller;
 nothing of it is read), the fixed-time controller (`model.name == 'fixedtime'`, envs.fixedtime_controller) or the
 vehicle-actuated controller (`model.name == 'actuated'`, envs.actuated_controller); the last two have their `program`
-set on the simulator, which runs it with no action launch and action = NULL.  The parameters are copied into the
+set on the simulator, which runs it with no action launch and action = NULL.  Fixed-time members read their `program`
+at the start of every episode: one program for all is set as it is, different ones as one plan per member on its
+replicas (tsc_set_replica_signal_programs).  The parameters are copied into the
 group's own buffers at the start of every episode, so a live learner evaluated mid-training is read at its current
 weights, and its parameters, optimiser slot, recurrent states, rollout and counters are left as they were.
 
@@ -426,9 +428,8 @@ def _program_key(env, model):
         return actuated_program(env).key()
     if model != 'fixedtime':
         return None
-    from ..envs.fixedtime import env_program
-    p = env_program(env)
-    return tuple(np.asarray(getattr(p, f)).tobytes() for f in ('n_phases', 'dur', 'open', 'major', 'yellow', 'offset'))
+    from ..envs.fixedtime import env_program, program_key
+    return program_key(env_program(env))
 
 
 def forward_family(model, net, label):
@@ -545,8 +546,6 @@ class _Group:
             max_cand, off, idx, act = (int(prog[0]),) + tuple(np.ascontiguousarray(a, np.int32) for a in prog[1:])
             _lib.check(lib.tsc_set_greedy_program(
                 self.sim._h, max_cand, off.ctypes.data, idx.ctypes.data, act.ctypes.data))
-        elif kind == 'fixedtime':                       # every member runs the one program of the group
-            self.sim.set_signal_program(m0.program)
         elif kind == 'actuated':
             self.sim.set_actuated_program(m0.program)
         elif kind == 'q':
@@ -575,6 +574,18 @@ class _Group:
             if kind == 'q' and st['h'].value:
                 _lib.lib().tscl_q_destroy(st['h'])
                 st['h'] = C.c_void_p()
+
+    def _set_programs(self, programs, i):
+        """The fixed-time family's programs, one per member from position i on: set_signal_program when they are all
+        the same program, else plan p on the replicas of position i + p (set_replica_signal_programs)."""
+        from ..envs.fixedtime import program_key
+        if len(set(program_key(p) for p in programs)) == 1:
+            self.sim.set_signal_program(programs[0])
+            return
+        plan = np.zeros(self.R, np.int64)
+        for p in range(len(programs)):
+            plan[(i + p) * self.S:(i + p + 1) * self.S] = p
+        self.sim.set_replica_signal_programs(programs, plan)
 
     def _actions(self, t, stream):
         lib, done, stp = _lib.lib(), 1 if t == 0 else 0, t
@@ -632,6 +643,8 @@ class _Group:
                 for k, m in enumerate(members):
                     st['params'][k].copy_(st['qlay'].pack(m.nets))
                 st['bad'].fill_(-1)
+            elif kind == 'fixedtime':
+                self._set_programs([m.program for m in members], st['i'])
             if kind in ('v1', 'v2'):
                 st['c'].zero_(); st['h'].zero_()
         fp = self.fp0 if self.ma2c else None

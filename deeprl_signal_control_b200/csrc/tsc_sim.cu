@@ -101,10 +101,11 @@ struct StepArgs {
   const float* cg;    // [R] per-replica coop_gamma (tsc_set_replica_coop_gamma) or null: cfg.coop_gamma / obs_scale_val
   const int32_t* dlevel;  // [R] demand level of each replica (tsc_set_replica_demand) or null.  When set, launch() points
                           // net.src_due / src_plo / src_phi at the level stack [n_levels][..] and the CTA offsets them
-  // fixed-time signal program (tsc_set_signal_program), read only by the FIXED instantiations.  Appended last so that
-  // the parameter offsets of every field above stay those of the action-driven kernels.
-  const int4* fx_node;    // [n_nodes] {n_phases, cycle, offset, 0}
-  const uint4* fx_phase;  // [n_nodes][fx_max_phases] {duration, open, major, yellow}
+  // fixed-time signal programs (tsc_set_signal_program / tsc_set_replica_signal_programs), read only by the FIXED
+  // instantiations.  Appended last so that the parameter offsets of every field above stay those of the action-driven
+  // kernels.  A stack of plans: replica r runs plan fx_plan[r] (plan 0 when fx_plan is null).
+  const int4* fx_node;    // [n_plans][n_nodes] {n_phases, cycle, offset, 0}
+  const uint4* fx_phase;  // [n_plans][n_nodes][fx_max_phases] {duration, open, major, yellow}
   int32_t fx_max_phases;
   // actuated signal program (tsc_set_actuated_program), read only by the ACTUATED instantiations; appended last too
   const int4* ac_node;      // [n_nodes] {n_phases, max_gap, first, end} of the node's loop-link list ac_link
@@ -115,6 +116,7 @@ struct StepArgs {
   int2* ac_state;           // [R][n_nodes] {phase, seconds the phase has run before the next simulated second}
   uint8_t* ac_gap;          // [R][lpad] seconds since the lane's loop was last covered, saturating at 255
   int32_t ac_max_phases;
+  const int32_t* fx_plan;   // [R] plan of each replica in the fixed-time stacks, or null: plan 0 (appended last too)
 };
 
 // ------------------------------------------------------------------------------------------------
@@ -333,13 +335,17 @@ __device__ __forceinline__ void node_signal(const DevNet& n, int i, int a, int p
   open[i] = o; major[i] = m; ymask[i] = y;
 }
 
-// fixed-time program: the phase of node i in force during simulated second `sec`, the k whose window
-// [start_k, start_k + d_k) holds (sec - offset) mod cycle (envs/fixedtime.py:phase_at)
-__device__ __forceinline__ int program_phase(const StepArgs& A, int i, int sec) {
-  const int4 nd = __ldg(&A.fx_node[i]);
+// fixed-time program: the phase of node i of replica `rep` in force during simulated second `sec`, the k whose window
+// [start_k, start_k + d_k) holds (sec - offset) mod cycle (envs/fixedtime.py:phase_at), in the replica's plan
+__device__ __forceinline__ int program_row(const StepArgs& A, int rep, int i) {
+  return (A.fx_plan ? __ldg(&A.fx_plan[rep]) : 0) * A.net.n_nodes + i;
+}
+__device__ __forceinline__ int program_phase(const StepArgs& A, int rep, int i, int sec) {
+  const int row = program_row(A, rep, i);
+  const int4 nd = __ldg(&A.fx_node[row]);
   int t = (sec - nd.z) % nd.y;
   if (t < 0) t += nd.y;
-  const uint4* ph = A.fx_phase + (size_t)i * A.fx_max_phases;
+  const uint4* ph = A.fx_phase + (size_t)row * A.fx_max_phases;
   int k = 0;
   for (; k < nd.x - 1; ++k) {
     const int d = (int)__ldg(&ph[k].x);
@@ -349,9 +355,9 @@ __device__ __forceinline__ int program_phase(const StepArgs& A, int i, int sec) 
   return k;
 }
 // ... and its signal state: the program's link masks replace node_signal's action / yellow derivation
-__device__ __forceinline__ void program_signal(const StepArgs& A, int i, int sec, uint32_t* open, uint32_t* major,
-                                               uint32_t* ymask) {
-  const uint4 p = __ldg(&A.fx_phase[(size_t)i * A.fx_max_phases + program_phase(A, i, sec)]);
+__device__ __forceinline__ void program_signal(const StepArgs& A, int rep, int i, int sec, uint32_t* open,
+                                               uint32_t* major, uint32_t* ymask) {
+  const uint4 p = __ldg(&A.fx_phase[(size_t)program_row(A, rep, i) * A.fx_max_phases + program_phase(A, rep, i, sec)]);
   open[i] = p.y; major[i] = p.z; ymask[i] = p.w;
 }
 
@@ -447,7 +453,7 @@ tsc_step_kernel(const StepArgs A) {
   if (tid < CTL_FIXED) s_misc[tid] = g_ctl[tid];
   for (int i = tid; i < N; i += TSC_THREADS) {
     s_prev[i] = g_ctl[CTL_FIXED + i];
-    if constexpr (FIXED) s_act[i] = program_phase(A, i, g_ctl[0] - A.sub0);
+    if constexpr (FIXED) s_act[i] = program_phase(A, rep, i, g_ctl[0] - A.sub0);
     else if constexpr (ACT) {
       const int2 st = A.ac_state[(size_t)rep * N + i];
       s_aph[i] = st.x; s_ael[i] = st.y;
@@ -476,7 +482,7 @@ tsc_step_kernel(const StepArgs A) {
     }
   }
   for (int i = tid; i < N; i += TSC_THREADS) {
-    if constexpr (FIXED) program_signal(A, i, s_misc[0], s_opn, s_maj, s_yel);
+    if constexpr (FIXED) program_signal(A, rep, i, s_misc[0], s_opn, s_maj, s_yel);
     else if constexpr (ACT) actuated_signal(A, i, s_aph[i], s_opn, s_maj, s_yel);
     else node_signal(n, i, s_act[i], s_prev[i], A.sub0 < c.yellow_interval_sec, s_opn, s_maj, s_yel);
   }
@@ -705,7 +711,7 @@ tsc_step_kernel(const StepArgs A) {
     for (int i = tid; i < N; i += TSC_THREADS) {
       s_appr[i] = 0;
       // green part starts after the yellow sub-steps (envs/env.py:571-573); a program sets the next second's signal
-      if constexpr (FIXED) program_signal(A, i, cur_sec + 1, s_opn, s_maj, s_yel);
+      if constexpr (FIXED) program_signal(A, rep, i, cur_sec + 1, s_opn, s_maj, s_yel);
       else if constexpr (ACT) {
         // phase k has run e seconds including this one: it ends at max_dur, or from min_dur on once every loop on the
         // from-lane of an open link has a gap of at least max_gap
@@ -989,7 +995,7 @@ __global__ void tsc_program_phase_kernel(const StepArgs A, int64_t RN, int32_t* 
   if (t >= RN) return;
   const int N = A.net.n_nodes;
   const int64_t r = t / N;
-  phase[t] = A.ac_state ? A.ac_state[t].x : program_phase(A, (int)(t - r * N), A.ctl[r * A.ctl_words]);
+  phase[t] = A.ac_state ? A.ac_state[t].x : program_phase(A, (int)r, (int)(t - r * N), A.ctl[r * A.ctl_words]);
 }
 
 // _measure_traffic_step (envs/env.py:409-437) for every replica: one CTA per replica over the compact state.
@@ -1090,8 +1096,9 @@ struct tsc_handle {
   std::vector<uint32_t> mp_green;
   int mp_max_phases = 0;
   int32_t* d_mp_off = nullptr; uint32_t* d_mp_link = nullptr; int32_t* d_mp_nph = nullptr; uint32_t* d_mp_green = nullptr;
-  // fixed-time signal program (tsc_set_signal_program): while set, every step launch is a FIXED instantiation
-  int4* d_fx_node = nullptr; uint4* d_fx_phase = nullptr; int fx_max_phases = 0;
+  // fixed-time signal programs (tsc_set_signal_program / tsc_set_replica_signal_programs): while set, every step launch
+  // is a FIXED instantiation.  The plan stacks and, when set per replica, each replica's plan index.
+  int4* d_fx_node = nullptr; uint4* d_fx_phase = nullptr; int32_t* d_fx_plan = nullptr; int fx_max_phases = 0;
   // actuated signal program (tsc_set_actuated_program): while set, every step launch is an ACTUATED instantiation with
   // smem_act / smem_rec_act bytes of shared memory.  Tables, each node's initial state, and the per-replica state.
   int4* d_ac_node = nullptr; uint4* d_ac_phase = nullptr; uint32_t* d_ac_yel = nullptr; uint32_t* d_ac_link = nullptr;
@@ -1100,6 +1107,11 @@ struct tsc_handle {
 };
 
 static bool has_program(const tsc_handle* h) { return h->d_fx_node != nullptr || h->d_ac_state != nullptr; }
+
+static void free_fixed(tsc_handle* h) {
+  cudaFree(h->d_fx_node); cudaFree(h->d_fx_phase); cudaFree(h->d_fx_plan);
+  h->d_fx_node = nullptr; h->d_fx_phase = nullptr; h->d_fx_plan = nullptr; h->fx_max_phases = 0;
+}
 
 static void free_actuated(tsc_handle* h) {
   cudaFree(h->d_ac_node); cudaFree(h->d_ac_phase); cudaFree(h->d_ac_yel); cudaFree(h->d_ac_link);
@@ -1268,7 +1280,7 @@ extern "C" int tsc_destroy(tsc_handle* h) {
   cudaFree(h->d_gp_off); cudaFree(h->d_gp_idx); cudaFree(h->d_gp_act);
   cudaFree(h->d_level); cudaFree(h->d_lv_due); cudaFree(h->d_lv_plo); cudaFree(h->d_lv_phi);
   cudaFree(h->d_mp_off); cudaFree(h->d_mp_link); cudaFree(h->d_mp_nph); cudaFree(h->d_mp_green);
-  cudaFree(h->d_fx_node); cudaFree(h->d_fx_phase);
+  free_fixed(h);
   free_actuated(h);
   delete h;
   return 0;
@@ -1351,52 +1363,83 @@ extern "C" int tsc_set_replica_demand(tsc_handle* h, int32_t n_levels, const uin
   return 0;
 }
 
-extern "C" int tsc_set_signal_program(tsc_handle* h, int32_t max_phases, const int32_t* n_phases_host,
-                                      const int32_t* dur_host, const uint32_t* open_host, const uint32_t* major_host,
-                                      const uint32_t* yellow_host, const int32_t* offset_host) {
-  if (!h) return fail("tsc_set_signal_program: null handle");
-  const int N = h->n_nodes;
-  std::vector<int4> node(N > 0 ? N : 1);
+// the one validation and upload path of fixed-time programs: n_plans plans, replica r running plan plan_host[r] (null:
+// every replica runs plan 0).  Nothing is replaced until every plan and every plan index has passed.
+static int set_fixed_programs(tsc_handle* h, const char* fn, int32_t n_plans, int32_t max_phases,
+                              const int32_t* n_phases_host, const int32_t* dur_host, const uint32_t* open_host,
+                              const uint32_t* major_host, const uint32_t* yellow_host, const int32_t* offset_host,
+                              const int32_t* plan_host) {
+  if (!h) return fail(std::string(fn) + ": null handle");
+  const int N = h->n_nodes, R = h->R;
+  const size_t NN = N > 0 ? N : 1;
+  std::vector<int4> node;
   std::vector<uint4> phase;
   if (n_phases_host) {          // every check before the current program is touched
-    if (max_phases <= 0 || !dur_host || !open_host || !major_host || !yellow_host || !offset_host)
-      return fail("tsc_set_signal_program: bad argument");
-    phase.resize((size_t)(N > 0 ? N : 1) * max_phases);
-    for (int i = 0; i < N; ++i) {
-      const int np_ = n_phases_host[i];
-      const std::string who = "tsc_set_signal_program: node " + std::to_string(i);
-      if (np_ < 1 || np_ > max_phases) return fail(who + " has " + std::to_string(np_) + " phases, outside [1, max_phases]");
-      if (offset_host[i] < -(1 << 30) || offset_host[i] > (1 << 30)) return fail(who + ": offset out of range");
-      int64_t cycle = 0;
-      for (int k = 0; k < np_; ++k) {
-        const size_t e = (size_t)i * max_phases + k;
-        if (dur_host[e] < 1) return fail(who + ": phase " + std::to_string(k) + " lasts less than 1 s");
-        if (yellow_host[e] & open_host[e]) return fail(who + ": phase " + std::to_string(k) + " has a link open and yellow");
-        if (major_host[e] & ~open_host[e]) return fail(who + ": phase " + std::to_string(k) + " has a major link not open");
-        cycle += dur_host[e];
-        phase[e] = make_uint4((uint32_t)dur_host[e], open_host[e], major_host[e], yellow_host[e]);
+    if (n_plans < 1 || max_phases <= 0 || !dur_host || !open_host || !major_host || !yellow_host || !offset_host)
+      return fail(std::string(fn) + ": bad argument");
+    node.resize((size_t)n_plans * NN);
+    phase.resize((size_t)n_plans * NN * max_phases);
+    for (int p = 0; p < n_plans; ++p)
+      for (int i = 0; i < N; ++i) {
+        const size_t row = (size_t)p * N + i;
+        const int np_ = n_phases_host[row];
+        const std::string who = std::string(fn) + (plan_host ? ": plan " + std::to_string(p) : std::string()) +
+                                ": node " + std::to_string(i);
+        if (np_ < 1 || np_ > max_phases) return fail(who + " has " + std::to_string(np_) + " phases, outside [1, max_phases]");
+        if (offset_host[row] < -(1 << 30) || offset_host[row] > (1 << 30)) return fail(who + ": offset out of range");
+        int64_t cycle = 0;
+        for (int k = 0; k < np_; ++k) {
+          const size_t e = row * max_phases + k;
+          if (dur_host[e] < 1) return fail(who + ": phase " + std::to_string(k) + " lasts less than 1 s");
+          if (yellow_host[e] & open_host[e]) return fail(who + ": phase " + std::to_string(k) + " has a link open and yellow");
+          if (major_host[e] & ~open_host[e]) return fail(who + ": phase " + std::to_string(k) + " has a major link not open");
+          cycle += dur_host[e];
+          phase[e] = make_uint4((uint32_t)dur_host[e], open_host[e], major_host[e], yellow_host[e]);
+        }
+        if (cycle > (1 << 30)) return fail(who + ": cycle longer than 2^30 s");
+        node[row] = make_int4(np_, (int)cycle, offset_host[row], 0);
       }
-      if (cycle > (1 << 30)) return fail(who + ": cycle longer than 2^30 s");
-      node[i] = make_int4(np_, (int)cycle, offset_host[i], 0);
-    }
+    if (plan_host)
+      for (int r = 0; r < R; ++r)
+        if (plan_host[r] < 0 || plan_host[r] >= n_plans)
+          return fail(std::string(fn) + ": replica " + std::to_string(r) + " has plan index " +
+                      std::to_string(plan_host[r]) + ", outside [0, " + std::to_string(n_plans) + ")");
   }
   CK(cudaSetDevice(h->device));
   CK(cudaDeviceSynchronize());          // no launch in flight still reads the previous program
-  cudaFree(h->d_fx_node); cudaFree(h->d_fx_phase);
-  h->d_fx_node = nullptr; h->d_fx_phase = nullptr; h->fx_max_phases = 0;
+  free_fixed(h);
   if (!n_phases_host) return 0;
   free_actuated(h);             // one signal program at a time
-  int4* dn = nullptr; uint4* dp = nullptr;
+  int4* dn = nullptr; uint4* dp = nullptr; int32_t* dl = nullptr;
   cudaError_t e = cudaMalloc(&dn, node.size() * sizeof(int4));
   if (e == cudaSuccess) e = cudaMalloc(&dp, phase.size() * sizeof(uint4));
+  if (e == cudaSuccess && plan_host) e = cudaMalloc(&dl, (size_t)(R > 0 ? R : 1) * sizeof(int32_t));
   if (e == cudaSuccess) e = cudaMemcpy(dn, node.data(), node.size() * sizeof(int4), cudaMemcpyHostToDevice);
   if (e == cudaSuccess) e = cudaMemcpy(dp, phase.data(), phase.size() * sizeof(uint4), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess && plan_host) e = cudaMemcpy(dl, plan_host, (size_t)R * sizeof(int32_t), cudaMemcpyHostToDevice);
   if (e != cudaSuccess) {       // the program stays off
-    cudaFree(dn); cudaFree(dp);
-    return fail(std::string("tsc_set_signal_program: ") + cudaGetErrorString(e));
+    cudaFree(dn); cudaFree(dp); cudaFree(dl);
+    return fail(std::string(fn) + ": " + cudaGetErrorString(e));
   }
-  h->d_fx_node = dn; h->d_fx_phase = dp; h->fx_max_phases = max_phases;
+  h->d_fx_node = dn; h->d_fx_phase = dp; h->d_fx_plan = dl; h->fx_max_phases = max_phases;
   return 0;
+}
+
+extern "C" int tsc_set_signal_program(tsc_handle* h, int32_t max_phases, const int32_t* n_phases_host,
+                                      const int32_t* dur_host, const uint32_t* open_host, const uint32_t* major_host,
+                                      const uint32_t* yellow_host, const int32_t* offset_host) {
+  return set_fixed_programs(h, "tsc_set_signal_program", 1, max_phases, n_phases_host, dur_host, open_host, major_host,
+                            yellow_host, offset_host, nullptr);
+}
+
+extern "C" int tsc_set_replica_signal_programs(tsc_handle* h, int32_t n_plans, int32_t max_phases,
+                                               const int32_t* n_phases_host, const int32_t* dur_host,
+                                               const uint32_t* open_host, const uint32_t* major_host,
+                                               const uint32_t* yellow_host, const int32_t* offset_host,
+                                               const int32_t* plan_host) {
+  if (n_phases_host && !plan_host) return fail("tsc_set_replica_signal_programs: bad argument");
+  return set_fixed_programs(h, "tsc_set_replica_signal_programs", n_plans, max_phases, n_phases_host, dur_host,
+                            open_host, major_host, yellow_host, offset_host, plan_host);
 }
 
 extern "C" int tsc_set_actuated_program(tsc_handle* h, int32_t max_phases, const int32_t* n_phases_host,
@@ -1461,8 +1504,7 @@ extern "C" int tsc_set_actuated_program(tsc_handle* h, int32_t max_phases, const
   CK(cudaDeviceSynchronize());          // no launch in flight still reads the previous program
   free_actuated(h);
   if (!n_phases_host) return 0;
-  cudaFree(h->d_fx_node); cudaFree(h->d_fx_phase);     // one signal program at a time
-  h->d_fx_node = nullptr; h->d_fx_phase = nullptr; h->fx_max_phases = 0;
+  free_fixed(h);                // one signal program at a time
   CK(cudaFuncSetAttribute(tsc_step_kernel<false, CTL_ACTUATED>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                           h->smem_act));
   if (h->smem_rec_act <= 232448)      // else record mode is refused while this program is set
@@ -1503,7 +1545,7 @@ extern "C" int tsc_get_program_phase(tsc_handle* h, int32_t* phase_dev, void* st
   if (!has_program(h)) return fail("tsc_get_program_phase: no signal program is set");
   CK(cudaSetDevice(h->device));
   StepArgs a = h->args;
-  a.fx_node = h->d_fx_node; a.fx_phase = h->d_fx_phase; a.fx_max_phases = h->fx_max_phases;
+  a.fx_node = h->d_fx_node; a.fx_phase = h->d_fx_phase; a.fx_plan = h->d_fx_plan; a.fx_max_phases = h->fx_max_phases;
   a.ac_state = h->d_ac_state;
   const int64_t RN = (int64_t)h->R * h->n_nodes;
   if (RN == 0) return 0;
@@ -1522,7 +1564,9 @@ static int launch(tsc_handle* h, int n_sub, const int32_t* action, const float* 
   a.n_sub = n_sub; a.action = action; a.fp = fp; a.obs = obs; a.reward = reward; a.greward = greward; a.done = done;
   a.rep0 = rep0;
   const bool fixed = h->d_fx_node != nullptr, act = h->d_ac_state != nullptr;
-  if (fixed) { a.fx_node = h->d_fx_node; a.fx_phase = h->d_fx_phase; a.fx_max_phases = h->fx_max_phases; }
+  if (fixed) {
+    a.fx_node = h->d_fx_node; a.fx_phase = h->d_fx_phase; a.fx_plan = h->d_fx_plan; a.fx_max_phases = h->fx_max_phases;
+  }
   if (act) {
     a.ac_node = h->d_ac_node; a.ac_phase = h->d_ac_phase; a.ac_yel = h->d_ac_yel; a.ac_link = h->d_ac_link;
     a.ac_loop = h->d_ac_loop; a.ac_state = h->d_ac_state; a.ac_gap = h->d_ac_gap; a.ac_max_phases = h->ac_max_phases;

@@ -147,14 +147,48 @@ def scenario_programs(env):
     raise ValueError('no fixed-time programs for scenario %r' % env.name)
 
 
-def env_program(env) -> SignalProgram:
-    """The SignalProgram of a scenario env: its scenario's programs, those named by its `tll_file` replaced."""
+def env_programs(env):
+    """The programs ({tlLogic id: program}) a scenario env runs: its scenario's, those named by its `tll_file`
+    replaced."""
     from ..net import sumo_ingest
     programs = dict(scenario_programs(env))
     if env.tll_file:
         programs.update(sumo_ingest.read_signal_programs(env.tll_file))
+    return programs
+
+
+def env_program(env) -> SignalProgram:
+    """The SignalProgram of a scenario env: its scenario's programs, those named by its `tll_file` replaced."""
     net = env._tables
-    return program_tables(net.node_names, [len(net.phases[n][0]) for n in net.node_names], programs)
+    return program_tables(net.node_names, [len(net.phases[n][0]) for n in net.node_names], env_programs(env))
+
+
+def program_key(program: SignalProgram):
+    """Equal for two SignalPrograms with the same tables (padding included)."""
+    return tuple(np.asarray(getattr(program, f)).tobytes() for f in ('n_phases', 'dur', 'open', 'major', 'yellow', 'offset'))
+
+
+def write_tll(programs, path) -> str:
+    """Write `programs` ({tlLogic id: {'offset', 'phases': [[duration, state], ...]}}) as a SUMO additional file of
+    static programs, in the given id order: `<additional><tlLogic id type="static" programID="tuned" offset><phase
+    duration state/>...`, durations and offsets as whole-second integers.  The inverse of
+    net.sumo_ingest.read_signal_programs for static programs: program_tables of what it reads back gives the tables of
+    `programs`.  Returns `path`."""
+    from xml.sax.saxutils import quoteattr
+    lines = ['<additional>']
+    for tl_id, prog in programs.items():
+        if prog.get('type', 'static') != 'static':
+            raise ValueError('tlLogic %r: type %r is not static (only static programs are written)' % (tl_id, prog['type']))
+        lines.append('    <tlLogic id=%s type="static" programID="tuned" offset="%d">'
+                     % (quoteattr(str(tl_id)), _whole(tl_id, 'offset', prog.get('offset', 0))))
+        for dur, state in prog['phases']:
+            lines.append('        <phase duration="%d" state=%s/>' % (_whole(tl_id, 'duration', dur, least=1),
+                                                                       quoteattr(str(state))))
+        lines.append('    </tlLogic>')
+    lines.append('</additional>')
+    with open(path, 'w') as f:
+        f.write('\n'.join(lines) + '\n')
+    return path
 
 
 class FixedTimeController:

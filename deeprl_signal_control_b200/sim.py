@@ -210,6 +210,43 @@ class BatchedSim:
                                                     (program.yellow, np.uint32), (program.offset, np.int32))]
         _lib.check(lib.tsc_set_signal_program(self._h, program.max_phases, *(x.ctypes.data for x in a)))
 
+    def set_replica_signal_programs(self, programs=None, plan_of=None) -> None:
+        """Fixed-time control per replica (`tsc_set_replica_signal_programs`): `programs` a list of
+        envs.fixedtime.SignalProgram in the net's node order, `plan_of` [R] ints; replica r then runs programs[plan_of[r]]
+        as a simulator under set_signal_program(programs[plan_of[r]]) would.  The programs are padded to the largest
+        max_phases, and identical programs are uploaded once.  None returns to action-driven stepping."""
+        lib = _lib.lib()
+        if programs is None:
+            _lib.check(lib.tsc_set_replica_signal_programs(self._h, 0, 0, *([None] * 7)))
+            return
+        plan_of = np.ascontiguousarray(plan_of, dtype=np.int64)
+        if plan_of.shape != (self.R,):
+            raise ValueError("set_replica_signal_programs takes %d plans of replicas (got shape %s)"
+                             % (self.R, plan_of.shape))
+        if len(programs) == 0 or plan_of.min() < 0 or plan_of.max() >= len(programs):
+            raise ValueError("set_replica_signal_programs: every replica's plan must index the %d programs" % len(programs))
+        N = self.net.n_nodes
+        for k, p in enumerate(programs):
+            if len(p.n_phases) != N:
+                raise ValueError("set_replica_signal_programs: program %d has %d node programs for %d nodes"
+                                 % (k, len(p.n_phases), N))
+        P = max(p.max_phases for p in programs)
+        uniq, index = {}, []                  # tables -> (plan index, tables)
+        for p in programs:
+            rows = tuple(np.pad(np.asarray(x, t), ((0, 0), (0, P - p.max_phases))) for x, t in
+                         ((p.dur, np.int32), (p.open, np.uint32), (p.major, np.uint32), (p.yellow, np.uint32)))
+            plan = (np.asarray(p.n_phases, np.int32), np.asarray(p.offset, np.int32)) + rows
+            key = tuple(x.tobytes() for x in plan)
+            if key not in uniq:
+                uniq[key] = (len(uniq), plan)
+            index.append(uniq[key][0])
+        n_phases, offset, dur, opn, major, yellow = (
+            np.ascontiguousarray(np.stack([u[1][f] for u in uniq.values()])) for f in range(6))
+        plan = np.ascontiguousarray(np.asarray(index, np.int32)[plan_of])
+        _lib.check(lib.tsc_set_replica_signal_programs(self._h, len(uniq), P, n_phases.ctypes.data, dur.ctypes.data,
+                                                       opn.ctypes.data, major.ctypes.data, yellow.ctypes.data,
+                                                       offset.ctypes.data, plan.ctypes.data))
+
     def set_actuated_program(self, program=None, max_gap=None) -> None:
         """Actuated control (`tsc_set_actuated_program`): every replica runs `program` (an envs.actuated.ActuatedProgram
         in the net's node order) second by second from its initial state, which reset() restores; the steps read no
@@ -230,8 +267,8 @@ class BatchedSim:
         _lib.check(lib.tsc_set_actuated_program(self._h, program.max_phases, *(x.ctypes.data for x in a)))
 
     def program_phase(self, out: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """`tsc_get_program_phase`: int32 [R, n_nodes] on the device, the phase every node's signal program shows in
-        the next simulated second (into `out` when given)."""
+        """`tsc_get_program_phase`: int32 [R, n_nodes] on the device, the phase every node's signal program (each
+        replica's own under set_replica_signal_programs) shows in the next simulated second (into `out` when given)."""
         ph = torch.empty(self.R, self.net.n_nodes, dtype=torch.int32, device=self.device) if out is None else out
         assert ph.dtype == torch.int32 and ph.is_contiguous() and ph.numel() == self.R * self.net.n_nodes
         _lib.check(_lib.lib().tsc_get_program_phase(self._h, ptr(ph), self._stream()))

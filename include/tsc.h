@@ -167,6 +167,17 @@ int tsc_set_signal_program(tsc_handle* h, int32_t max_phases, const int32_t* n_p
                            const uint32_t* open_host, const uint32_t* major_host, const uint32_t* yellow_host,
                            const int32_t* offset_host);
 
+/* Fixed-time signal control with one program per replica (synchronous, like tsc_set_signal_program).  n_plans >= 1
+ * programs, stacked: n_phases_host and offset_host [n_plans][n_nodes], dur_host, open_host, major_host and yellow_host
+ * [n_plans][n_nodes][max_phases]; plan p is a program as tsc_set_signal_program takes it.  plan_host [R]: replica r runs
+ * plan plan_host[r] (0 <= plan_host[r] < n_plans), bit-identical to a handle that runs that plan alone through
+ * tsc_set_signal_program.  Every plan and every plan index is checked before anything is replaced; the error names the
+ * plan.  The setting persists over tsc_reset, replaces the current fixed-time program and turns an actuated program off;
+ * tsc_set_signal_program is the case of one plan run by every replica.  n_phases_host NULL turns it off. */
+int tsc_set_replica_signal_programs(tsc_handle* h, int32_t n_plans, int32_t max_phases, const int32_t* n_phases_host,
+                                    const int32_t* dur_host, const uint32_t* open_host, const uint32_t* major_host,
+                                    const uint32_t* yellow_host, const int32_t* offset_host, const int32_t* plan_host);
+
 /* Vehicle-actuated signal control (synchronous, like tsc_set_signal_program; validates every table before it replaces
  * anything).  Node i runs n_phases_host[i] phases in order (1 <= n <= max_phases); phase k (entry [i][k] of the
  * [n_nodes][max_phases] host arrays) shows the link masks open_host, major_host and yellow_host as in
