@@ -32,6 +32,20 @@ csrc/tsc_learn.cu (loss / head gradients, returns, clip + RMSProp).  No library 
 `use_tc=False` selects the plain fp32 twin kernels (fc_embed, lstm_seq_fwd / bwd, heads, fc_bwd) that the reference
 goldens pin at 2e-4; only on that path do the three plain batched products (X.Wx, dZ.Wx^T, [X|H]^T.dZ) go through
 `torch.baddbmm / bmm` (fp32, TF32 only when `allow_tf32`).
+
+Imitation (`teacher`, DESIGN §5 Imitation): A2C guided by a signal controller in DAgger form.  The student drives the
+simulator; at every control step the trainer has the teacher label the state the student is in, into `teach_hist[t]`
+(int32 [T][R][A], next to act_hist).  For every row (t, r) and agent i with pi the softmax over the agent's n_a_i
+logits, a the sampled action, A the advantage, b the teacher's action and lam the update's imitation coefficient (one
+float per update, one per member in a sweep), the loss gains  -lam * log clip(pi_b, 1e-10, 1), summed with the A2C
+terms' scale = 1 / (n_step * R_total).  Its gradient at the logits is  scale * lam * (pi_j - [j == b])  when pi_b is not
+clipped and 0 when it is: the policy-gradient term with A := lam and a := b, added in the same pass of the kernels that
+compute the head gradients (tscl_lstm_seq_bwd_tc_heads_imit, tscl_heads_loss_imit).  The value head and the entropy
+term do not change; at lam = 0 the update is plain A2C.  stats[3] receives agent 0's unweighted cross-entropy
+sum -log clip(pi_b, 1e-10, 1) * scale.  Teachers (TEACHERS): 'maxpressure' (tsc_pressure_actions on the simulator's lane
+counts) and 'greedy' (tsc_greedy_actions on obs_hist[t] with the training env's greedy program: the greedy rule on the
+own-wave entries the student sees, normalised and clipped by the training config).  Without a teacher the learner
+allocates and launches exactly what it does without the feature.
 """
 from __future__ import annotations
 
@@ -63,6 +77,32 @@ def check_population(seeds, seed, n_replicas, chunk, process_group):
     if len(set(seeds)) != len(seeds):
         raise ValueError("population seeds must be distinct (got %s)" % seeds)
     return _check_members(seeds, n_replicas, chunk, process_group)
+
+
+# controllers that can label a student's state with one action per agent (BatchedA2C(teacher=...)).  Fixed-time, tuned
+# fixed-time and actuated control cannot: their program phases include yellow and all-red, a phase may change inside a
+# control interval, so there is no action label to give.
+TEACHERS = ("maxpressure", "greedy")
+NO_LABEL_CONTROLLERS = ("fixedtime", "actuated")
+
+
+def check_teacher(teacher):
+    """`teacher` if it is None or one of TEACHERS, else ValueError naming it (and why, for the program controllers)."""
+    if teacher is None or teacher in TEACHERS:
+        return teacher
+    if teacher in NO_LABEL_CONTROLLERS:
+        raise ValueError("teacher %r cannot label states: its signal program's phases include yellow and all-red and "
+                         "a phase can change inside a control interval, so there is no action to imitate (teachers: %s)"
+                         % (teacher, ", ".join(TEACHERS)))
+    raise ValueError("unknown teacher %r (teachers: %s)" % (teacher, ", ".join(TEACHERS)))
+
+
+def check_imit(v, name="imitation coefficient"):
+    """An imitation coefficient as a float: finite and >= 0, else ValueError."""
+    v = float(v)
+    if not np.isfinite(v) or v < 0:
+        raise ValueError("the %s must be finite and >= 0 (got %r)" % (name, v))
+    return v
 
 
 # the learner values a sweep member sets for itself (BatchedA2C(hparams=...)); lr and beta come with each backward
@@ -175,7 +215,9 @@ class BatchedA2C:
                  chunk: int = 1024, replica0: int = 0, total_replicas: Optional[int] = None,
                  process_group=None, allow_tf32: bool = True, use_tc: bool = True,
                  store_acts: Optional[bool] = None, seeds: Optional[Sequence[int]] = None,
-                 hparams: Optional[Sequence[dict]] = None, deterministic: bool = False):
+                 hparams: Optional[Sequence[dict]] = None, deterministic: bool = False,
+                 teacher: Optional[str] = None):
+        self.teacher = check_teacher(teacher)
         if deterministic:       # the layout / switch refusals, before any device work
             why = deterministic_refusal(learner_paths(layout, use_tc, 1 if seeds is None else len(seeds),
                                                       os.environ.get("TSC_DX_LIBRARY", "0") == "1"),
@@ -244,6 +286,8 @@ class BatchedA2C:
         self.rew_hist = torch.zeros(T, R, A, **f32)
         self.val_hist = torch.zeros(T, R, A, **f32)
         self.Rs = torch.zeros(T, R, A, **f32); self.Adv = torch.zeros(T, R, A, **f32)
+        # the teacher's action of every rollout row (written by the trainer before each simulator step)
+        self.teach_hist = torch.zeros(T, R, A, dtype=torch.int32, device=self.dev) if self.teacher else None
         self.done_pre = [0.0] * T
         self.done_post = [0.0] * T
         self.last_done = False      # OnPolicyBuffer.reset(done) carries the last done (agents/utils.py:187-193)
@@ -333,7 +377,7 @@ class BatchedA2C:
                              "differ in them; use the device-resident loop (add_transition_device)" % what)
 
     def _per_member(self, v, name):
-        """lr / beta of backward(): one value for every member, or a sequence of K"""
+        """lr / beta / imit of backward(): one value for every member, or a sequence of K"""
         if isinstance(v, (list, tuple, np.ndarray)):
             if len(v) != self.K:
                 raise ValueError("%s takes one value per member (%d, got %d)" % (name, self.K, len(v)))
@@ -561,22 +605,36 @@ class BatchedA2C:
             self._dz_all = torch.empty(nc, L.U, self.T * self.chunk, 4 * L.h, dtype=torch.bfloat16, device=self.dev)
         return self._dz_all
 
-    def _bwd_heads(self, P, G, Wt, stats, r0, n_chunks, v_coef, beta, scale, dpre, dZb):
+    def _bwd_heads(self, P, G, Wt, stats, r0, n_chunks, v_coef, beta, scale, dpre, dZb, imit=0.0):
         """tscl_lstm_seq_bwd_tc_heads over `n_chunks` chunks of the store from replica r0: loss gradients at the heads and
-        BPTT in one kernel, dZ (bf16) into dZb, head weight gradients into G, agent 0's loss sums into stats."""
+        BPTT in one kernel, dZ (bf16) into dZb, head weight gradients into G, agent 0's loss sums into stats; with a
+        teacher the _imit form, toward teach_hist with coefficient `imit`."""
         ci, R, A = r0 // self.chunk, self.R, self.lay.A
-        _lib.check(_lib.lib().tscl_lstm_seq_bwd_tc_heads(
-            self._h, _p(Wt), _p(P), _p(self.st_g[ci]), _p(self.st_c[ci]), _p(self.st_h[ci]), _p(self.c_bw), _p(dpre),
-            _p(self.act_hist[0, r0:]), _p(self.Rs[0, r0:]), _p(self.Adv[0, r0:]), self.T, self.chunk, n_chunks, R, r0,
-            R * A, v_coef, beta, scale, _p(dZb), _p(stats), _p(G), self._st()))
+        args = (self._h, _p(Wt), _p(P), _p(self.st_g[ci]), _p(self.st_c[ci]), _p(self.st_h[ci]), _p(self.c_bw), _p(dpre),
+                _p(self.act_hist[0, r0:]), _p(self.Rs[0, r0:]), _p(self.Adv[0, r0:]), self.T, self.chunk, n_chunks, R, r0,
+                R * A, v_coef, beta, scale, _p(dZb), _p(stats), _p(G))
+        if self.teacher:
+            _lib.check(_lib.lib().tscl_lstm_seq_bwd_tc_heads_imit(*args, _p(self.teach_hist[0, r0:]), imit, self._st()))
+        else:
+            _lib.check(_lib.lib().tscl_lstm_seq_bwd_tc_heads(*args, self._st()))
 
-    def backward(self, boot: Optional[torch.Tensor], lr: float, beta: float):
+    def _imits(self, imit):
+        """The update's imitation coefficient per member: with a teacher, `imit` (one value or one per member, each
+        finite and >= 0); without one, `imit` must be 0."""
+        imits = [check_imit(v) for v in self._per_member(imit, "imit")]
+        if not self.teacher and any(imits):
+            raise ValueError("an imitation coefficient (%s) needs a teacher (BatchedA2C(teacher=...))" % imits)
+        return imits
+
+    def backward(self, boot: Optional[torch.Tensor], lr: float, beta: float, imit=0.0):
         """One A2C update from the stored n_step rollout (agents/models.py:174-183).  `boot` is the
         bootstrap value [R, A] (None / zeros when the episode ended, utils.py:186-190).  `lr` / `beta`: one value, or one
-        per member (a sweep's schedules)."""
+        per member (a sweep's schedules).  `imit`: the imitation coefficient lam of a learner with a teacher, likewise
+        (module docstring); 0 without one."""
         assert self.t == self.T, "rollout buffer not full"
         L, R, T, U, A, lib = self.lay, self.R, self.T, self.lay.U, self.lay.A, _lib.lib()
         lrs, betas = self._per_member(lr, "lr"), self._per_member(beta, "beta")
+        imits = self._imits(imit)
         self._mm()
         st = self._st
         f32 = dict(dtype=torch.float32, device=self.dev)
@@ -613,7 +671,8 @@ class BatchedA2C:
         # one BPTT launch over every chunk (one member, and the all-chunk dZ fits); else one per chunk, the same bits
         dz_all = self._dz_all_buf() if heads_bptt and self.K == 1 and R > self.chunk else None
         if dz_all is not None:
-            self._bwd_heads(P, G, Wt, stats, 0, R // self.chunk, self.hp[0]["v_coef"], betas[0], scale, dpre, dz_all)
+            self._bwd_heads(P, G, Wt, stats, 0, R // self.chunk, self.hp[0]["v_coef"], betas[0], scale, dpre, dz_all,
+                            imits[0])
             self.kernel_launches += 1
         for r0 in range(0, R, self.chunk):
             if self.K > 1:        # the member of this chunk: its weights, images, gradient and loss terms
@@ -660,14 +719,17 @@ class BatchedA2C:
             hb = _p(self.st_h[ci]) if use_store else None
             if heads_bptt:      # heads + BPTT in one kernel (already run for every chunk when dz_all is set)
                 if dz_all is None:
-                    self._bwd_heads(P, G, Wt, stats, r0, 1, self.hp[k]["v_coef"], betas[k], scale, dpre, dZb)
+                    self._bwd_heads(P, G, Wt, stats, r0, 1, self.hp[k]["v_coef"], betas[k], scale, dpre, dZb, imits[k])
                     self.kernel_launches += 1
             else:
-                _lib.check(lib.tscl_heads_loss(self._h, _p(P), None if all_tc else _p(H), _p(self.act_hist[0, r0:]),
-                                               _p(self.Rs[0, r0:]), _p(self.Adv[0, r0:]), M, rc, R * A,
-                                               self.hp[k]["v_coef"], betas[k], scale,
-                                               None if self.fused_heads else _p(dlog), _p(dH), _p(stats),
-                                               hb if all_tc else None, _p(G) if self.fused_heads else None, st()))
+                args = (self._h, _p(P), None if all_tc else _p(H), _p(self.act_hist[0, r0:]), _p(self.Rs[0, r0:]),
+                        _p(self.Adv[0, r0:]), M, rc, R * A, self.hp[k]["v_coef"], betas[k], scale,
+                        None if self.fused_heads else _p(dlog), _p(dH), _p(stats), hb if all_tc else None,
+                        _p(G) if self.fused_heads else None)
+                if self.teacher:
+                    _lib.check(lib.tscl_heads_loss_imit(*args, _p(self.teach_hist[0, r0:]), imits[k], st()))
+                else:
+                    _lib.check(lib.tscl_heads_loss(*args, st()))
                 self.kernel_launches += 2
             if not self.fused_heads:
                 # head weight / bias gradients (plain batched GEMM + column sums)

@@ -46,9 +46,10 @@ class BatchedFcA2C(BatchedA2C):
         return self.pi, self.val, (self.act if want_act else None)
 
     # ------------------------------------------------------------------------------------------
-    def backward(self, boot: Optional[torch.Tensor], lr: float, beta: float):
+    def backward(self, boot: Optional[torch.Tensor], lr: float, beta: float, imit=0.0):
         assert self.t == self.T, "rollout buffer not full"
         L, R, T, U, A, lib = self.lay, self.R, self.T, self.lay.U, self.lay.A, _lib.lib()
+        imit = self._imits(imit)[0]
         self._mm()
         st = self._st
         f32 = dict(dtype=torch.float32, device=self.dev)
@@ -72,9 +73,12 @@ class BatchedFcA2C(BatchedA2C):
             obs0 = self.obs_hist[0, r0:]
             _lib.check(lib.tscl_fc_embed(self._h, _p(self.P), _p(obs0), M, rc, R * n_obs, _p(X), st()))
             _lib.check(lib.tscl_fc_hidden_fwd(self._h, _p(self.P), _p(X), M, _p(H), st()))
-            _lib.check(lib.tscl_heads_loss(self._h, _p(self.P), _p(H), _p(self.act_hist[0, r0:]), _p(self.Rs[0, r0:]),
-                                           _p(self.Adv[0, r0:]), M, rc, R * A, self.v_coef, beta, scale, None, _p(dH),
-                                           _p(self.stats), None, _p(self.G), st()))
+            args = (self._h, _p(self.P), _p(H), _p(self.act_hist[0, r0:]), _p(self.Rs[0, r0:]), _p(self.Adv[0, r0:]), M,
+                    rc, R * A, self.v_coef, beta, scale, None, _p(dH), _p(self.stats), None, _p(self.G))
+            if self.teacher:            # the imitation term (learner.py's module docstring)
+                _lib.check(lib.tscl_heads_loss_imit(*args, _p(self.teach_hist[0, r0:]), imit, st()))
+            else:
+                _lib.check(lib.tscl_heads_loss(*args, st()))
             dX = torch.empty(U, M, L.dx, **f32)
             # relu', dX = dH . W^T, dW += X^T dH, db += 1^T dH: own kernels (no library GEMM on this path)
             _lib.check(lib.tscl_fc_hidden_bwd(self._h, _p(self.P), _p(X), _p(H), _p(dH), M, _p(dX), _p(self.G), st()))

@@ -44,6 +44,60 @@ def a2c_schedulers(model_config, total_step):
     return lr, beta
 
 
+# [MODEL_CONFIG] keys of imitation (learner.py's module docstring): `teacher = maxpressure | greedy` and the schedule of
+# the imitation coefficient lam, which may differ between the members of a sweep
+IMITATION_KEYS = ('imitation_coef_init', 'imitation_decay', 'imitation_coef_min', 'imitation_ratio')
+IMITATION_DECAYS = ('constant', 'linear')
+
+
+def check_imitation(model_config, agent):
+    """The teacher of an agent's [MODEL_CONFIG] (None without one), every imitation key checked; raises ValueError
+    naming the key: an unknown teacher (or a controller that has no action labels), imitation keys without a teacher, a
+    teacher without imitation_coef_init, an imitation_decay other than constant / linear, an imitation_coef_init or
+    imitation_coef_min that is negative or not finite, an imitation_ratio that is not finite and > 0, and a teacher for
+    an IQL agent (iqll / iqld).  Reads nothing but the section: call it before any directory or device work."""
+    from .learner import check_imit, check_teacher
+    teacher = model_config.get('teacher', fallback=None)
+    given = [k for k in IMITATION_KEYS if model_config.get(k, fallback=None) is not None]
+    if teacher is None:
+        if given:
+            raise ValueError('[MODEL_CONFIG] %s: imitation keys need a teacher (teacher = maxpressure | greedy)'
+                             % ', '.join(given))
+        return None
+    try:
+        check_teacher(teacher)
+    except ValueError as e:
+        raise ValueError('[MODEL_CONFIG] teacher: %s' % e)
+    if agent not in ('ia2c', 'ma2c'):
+        raise ValueError('[MODEL_CONFIG] teacher = %s: imitation trains the A2C agents (ia2c, ma2c), not %r (IQL with '
+                         'demonstrations is not built)' % (teacher, agent))
+    if 'imitation_coef_init' not in given:
+        raise ValueError('[MODEL_CONFIG] imitation_coef_init is required with teacher = %s' % teacher)
+    decay = model_config.get('imitation_decay', fallback='constant')
+    if decay not in IMITATION_DECAYS:
+        raise ValueError('[MODEL_CONFIG] imitation_decay must be one of %s (got %r)' % (', '.join(IMITATION_DECAYS), decay))
+    for key in ('imitation_coef_init', 'imitation_coef_min'):
+        try:
+            check_imit(model_config.get(key, fallback='0'), key)
+        except ValueError as e:
+            raise ValueError('[MODEL_CONFIG] %s' % e)
+    ratio = model_config.getfloat('imitation_ratio', fallback=1.0)
+    if not np.isfinite(ratio) or ratio <= 0:
+        raise ValueError('[MODEL_CONFIG] imitation_ratio must be finite and > 0 (got %r)' % ratio)
+    return teacher
+
+
+def imitation_scheduler(model_config, total_step):
+    """The schedule of the imitation coefficient lam (a `Scheduler`, as the entropy coefficient's): imitation_coef_init,
+    'constant', or 'linear' down to imitation_coef_min (default 0) over total_step * imitation_ratio (default 1)."""
+    lam0 = model_config.getfloat('imitation_coef_init')
+    decay = model_config.get('imitation_decay', fallback='constant')
+    if decay == 'constant':
+        return Scheduler(lam0, decay=decay)
+    return Scheduler(lam0, model_config.getfloat('imitation_coef_min', fallback=0.0),
+                     total_step * model_config.getfloat('imitation_ratio', fallback=1.0), decay=decay)
+
+
 def a2c_hparams(model_config):
     """The `BatchedA2C` values of one [MODEL_CONFIG] section, keyed by learner.SWEEP_KEYS."""
     return dict(gamma=model_config.getfloat('gamma'), v_coef=model_config.getfloat('value_coef'),
@@ -80,6 +134,10 @@ class IA2C:
         if seeds is not None:
             learner_kw['seeds'] = seeds
             seed = int(seeds[0])
+        # imitation of a signal controller (learner.py's module docstring): refused by key before any device work
+        self.teacher = check_imitation(model_config, self.name)
+        if self.teacher:
+            learner_kw['teacher'] = self.teacher
         self.n_agent = len(n_s_ls)
         self._pre_done = False
         self.reward_clip = model_config.getfloat('reward_clip')
@@ -111,6 +169,10 @@ class IA2C:
             if member_configs is not None:
                 self.lr_schedulers, self.beta_schedulers = (
                     list(s) for s in zip(*(a2c_schedulers(c, total_step) for c in member_configs)))
+            if self.teacher:
+                self.imit_scheduler = imitation_scheduler(model_config, total_step)
+                if member_configs is not None:
+                    self.imit_schedulers = [imitation_scheduler(c, total_step) for c in member_configs]
         self._rng = np.random.RandomState(seed)
         self._obs_dev = torch.zeros(n_replicas, n_obs, device=self.batched.dev)
 

@@ -235,14 +235,19 @@ def summary_name(agent: str, policy: str = 'lstm', model_type: str | None = None
 
 def a2c_values(name: str, rec):
     """The four scalars of one A2C update from its record (policy, value, entropy loss, pre-clip gradient norm)
-    (agents/policies.py:62-72): total_loss = policy + value + entropy in float32, as the TF graph adds them."""
+    (agents/policies.py:62-72): total_loss = policy + value + entropy in float32, as the TF graph adds them.  A record of
+    a run with a teacher has a 5th entry, agent 0's unweighted imitation cross-entropy: one more scalar,
+    `loss/<name>_imitation_loss`, which total_loss does not include."""
     p, v, e, g = (np.float32(x) for x in rec[:4])
-    return {'loss/%s_policy_loss' % name: p, 'loss/%s_value_loss' % name: v,
-            'loss/%s_total_loss' % name: np.float32(np.float32(p + v) + e), 'train/%s_gradnorm' % name: g}
+    out = {'loss/%s_policy_loss' % name: p, 'loss/%s_value_loss' % name: v,
+           'loss/%s_total_loss' % name: np.float32(np.float32(p + v) + e), 'train/%s_gradnorm' % name: g}
+    if len(rec) > 4:
+        out['loss/%s_imitation_loss' % name] = np.float32(rec[4])
+    return out
 
 
 def a2c_events(name: str, rec, first_step: int, n_step: int):
-    """[(step, values)] of one episode set's A2C updates: rec [n_updates, 4], update j at first_step + j * n_step (the
+    """[(step, values)] of one episode set's A2C updates: rec [n_updates, 4] (5 with a teacher), update j at first_step + j * n_step (the
     global step of its backward, utils.py:288-291)."""
     return [(int(first_step + j * n_step), a2c_values(name, rec[j])) for j in range(len(rec))]
 

@@ -128,7 +128,8 @@ class Counter:
 
 class Summaries:
     """The reference's TensorBoard log of a training run (utils.py:129-140, 255-306; agents/policies.py:62-72, 331-338):
-    agent 0's scalars of every update (A2C: policy / value / total loss and gradient norm at the step of the backward;
+    agent 0's scalars of every update (A2C: policy / value / total loss and gradient norm at the step of the backward,
+    and with a teacher the imitation loss;
     IQL: loss, mean q, mean target and gradient norm of round k at that step + k), `train_reward` once per episode set
     (the training row's avg_reward, at the step of its last update) and `test_reward` once per in-training test (the
     mean over test seeds of the per-seed means, at the step of the test).
@@ -149,10 +150,12 @@ class Summaries:
             return None if self.writer is None else trainer.summary_rec[:, :, 0, :].cpu().numpy()
         rec = trainer.summary_rec.cpu().numpy()
         if group is not None:
-            loss = _dist.sum_partials(rec[:, :3], group)
+            cols = [0, 1, 2] + ([4] if rec.shape[1] > 4 else [])      # loss terms (with a teacher also imitation)
+            loss = _dist.sum_partials(rec[:, cols], group)
             if loss is None:
                 return None
-            rec = np.concatenate([loss, rec[:, 3:]], 1)
+            rec = rec.astype(np.float64)
+            rec[:, cols] = loss
         return rec
 
     def episode_set(self, rec, ran, prev_step, step, train_reward):
@@ -471,6 +474,7 @@ def train(config, base_dir, test_mode='no_test', n_replicas=1, policy='lstm', de
     data/<label>/.  Not with `seeds`."""
     if deterministic and policy != 'lstm':
         raise ValueError("deterministic=True needs the LSTM policy's lean update (got policy=%r)" % (policy,))
+    _check_imitation([_read_config(config)[0]])
     mix = None
     if demand_mix is not None:
         if seeds is not None:
@@ -555,6 +559,27 @@ def check_ranks_agree(model, group):
                            'model' % differ)
 
 
+def teacher_kwargs(model, env, sweep=False):
+    """The `BatchedTrainer` arguments of a model with a teacher ({} without one): the imitation coefficient's schedule
+    (one per member in a sweep) and, for the greedy teacher, the training env's greedy program: the greedy rule on the
+    own-wave entries of the observation the student sees, normalised and clipped by the training config."""
+    teacher = getattr(model, 'teacher', None)
+    if not teacher:
+        return {}
+    kw = dict(imit=model.imit_schedulers if sweep else model.imit_scheduler)
+    if teacher == 'greedy':
+        from ..envs import greedy_controller
+        kw['greedy_program'] = greedy_controller(env).greedy_program(env._tables.node_obs_off)
+    return kw
+
+
+def _check_imitation(cfgs):
+    """check_imitation on the [MODEL_CONFIG] of every config (before any directory or device work)."""
+    from .models import check_imitation
+    for c in cfgs:
+        check_imitation(c['MODEL_CONFIG'], c['ENV_CONFIG'].get('agent'))
+
+
 def _schedule(config, env):
     """(total_step, Counter, episode length T) of a run; T must be a multiple of batch_size (utils.py:121)."""
     total_step = int(config.getfloat('TRAIN_CONFIG', 'total_step'))
@@ -603,7 +628,7 @@ def _train(config, dirs, in_test, post_test, R_total, policy, device, pg, summar
                 from .learner_iql import N_ROUNDS
                 shape = (-(-T // n_step), N_ROUNDS, model.n_agent, 4)
             else:
-                shape = (T // n_step, 4)
+                shape = (T // n_step, 5 if getattr(model, 'teacher', None) else 4)
             srec = dict(summary_rec=torch.zeros(shape, dtype=torch.float32, device=sim.device))
             if rank == 0:
                 writer = SummaryWriter(dirs['log'])
@@ -619,7 +644,8 @@ def _train(config, dirs, in_test, post_test, R_total, policy, device, pg, summar
         else:
             from .trainer import BatchedTrainer
             trainer = BatchedTrainer(sim, model.batched, agent, model.lr_scheduler, model.beta_scheduler, seed0=seed,
-                                     replica0=replica0, greward_trace=trace, demand_mix=mix_nets, **srec)
+                                     replica0=replica0, greward_trace=trace, demand_mix=mix_nets, **srec,
+                                     **teacher_kwargs(model, env))
         evaluator = None
         levels = None if mix is None else [(label, None) for label in mix.labels]
         if (in_test or post_test) and rank == 0:
@@ -708,6 +734,7 @@ def train_population(config, base_dir, seeds, test_mode='no_test', n_replicas=1,
     if policy != 'lstm':
         raise ValueError("a population trains the LSTM policy only (got policy=%r)" % policy)
     check_population(seeds, 0, n_replicas, 1024, None)               # before any directory or device work
+    _check_imitation([config])
     cfgs, dirs = [], []
     for s in seeds:
         cfg = copy.deepcopy(config)
@@ -756,13 +783,13 @@ def _train_members(cfgs, dirs, agent, seeds, R_m, in_test, post_test, policy, de
         srec, summ = {}, None
         if summaries:
             from .summary import SummaryWriter, summary_name
-            shape = (T // model.n_step,) + ((K,) if K > 1 else ()) + (4,)
+            shape = (T // model.n_step,) + ((K,) if K > 1 else ()) + (5 if model.teacher else 4,)
             srec = dict(summary_rec=torch.zeros(shape, dtype=torch.float32, device=sim.device))
             writers = [SummaryWriter(d['log']) for d in dirs]
             summ = [Summaries(w, summary_name(agent, policy), 'a2c', model.n_step) for w in writers]
         lr, beta = (model.lr_schedulers, model.beta_schedulers) if sweep else (model.lr_scheduler, model.beta_scheduler)
         trainer = BatchedTrainer(sim, model.batched, agent, lr, beta, seed0=seeds[0], greward_trace=trace,
-                                 coop_gamma=cg, demand=demand, **srec)
+                                 coop_gamma=cg, demand=demand, **srec, **teacher_kwargs(model, env, sweep))
         drivers = []
         for k in range(K):                  # one driver per member, over its view of the shared trainer
             evaluator = None
@@ -798,6 +825,8 @@ SWEEP_CONFIG_KEYS = {
     'MODEL_CONFIG': ('lr_init', 'lr_decay', 'lr_min', 'entropy_coef_init', 'entropy_decay', 'entropy_coef_min',
                      'entropy_ratio', 'value_coef', 'max_grad_norm', 'rmsp_alpha', 'rmsp_epsilon', 'gamma',
                      'reward_norm', 'reward_clip')}
+# the imitation keys the members of an A2C sweep may set for themselves as well (`train_sweep`); `teacher` must be the same
+IMITATION_SWEEP_KEYS = ('imitation_coef_init', 'imitation_decay', 'imitation_coef_min', 'imitation_ratio')
 # the same for an IQL sweep (`train_iql_sweep`): IQL reads no coop_gamma, and its ring and networks are shared
 IQL_SWEEP_CONFIG_KEYS = {
     'ENV_CONFIG': ('seed',),
@@ -893,7 +922,8 @@ def sweep_dir(base_dir, name, agent):
 def train_sweep(configs, base_dir, test_mode='no_test', n_replicas=64, device=0, summaries=False, policy='lstm',
                 process_group=None, deterministic=False, vary_demand=False):
     """Train a hyperparameter sweep of one A2C agent (ia2c / ma2c, LSTM policy) in one process: one member per config
-    (`sweep_members`: the configs may differ only in SWEEP_CONFIG_KEYS), each on `n_replicas` replicas (a multiple of
+    (`sweep_members`: the configs may differ only in SWEEP_CONFIG_KEYS and IMITATION_SWEEP_KEYS, with one teacher for
+    all), each on `n_replicas` replicas (a multiple of
     64).  One simulator launch and one grouped policy forward per control step cover all K * n_replicas replicas;
     member k runs with its own seed, coop_gamma (ma2c), learner values and lr / entropy schedules, and trains what
     `train(config_k, n_replicas=n_replicas)` trains alone.  Its directory `sweep_dir(base_dir, name_k, agent)` holds
@@ -908,7 +938,8 @@ def train_sweep(configs, base_dir, test_mode='no_test', n_replicas=64, device=0,
     in_test, post_test = init_test_flag(test_mode)
     if process_group is not None:
         raise ValueError('a sweep trains in one process: it takes no process_group')
-    items = sweep_members(configs, demand=vary_demand)
+    keys = dict(SWEEP_CONFIG_KEYS, MODEL_CONFIG=SWEEP_CONFIG_KEYS['MODEL_CONFIG'] + IMITATION_SWEEP_KEYS)
+    items = sweep_members(configs, keys, demand=vary_demand)
     agent = items[0][1]['ENV_CONFIG'].get('agent')
     kind, _ = model_spec(agent)
     if kind == 'iql':
@@ -916,6 +947,7 @@ def train_sweep(configs, base_dir, test_mode='no_test', n_replicas=64, device=0,
     if policy != 'lstm':
         raise ValueError("a sweep trains the LSTM policy only (got policy=%r)" % policy)
     cfgs = [c for _, c, _ in items]
+    _check_imitation(cfgs)
     seeds = [c['ENV_CONFIG'].getint('seed') for c in cfgs]
     check_sweep(seeds, [a2c_hparams(c['MODEL_CONFIG']) for c in cfgs], n_replicas, 1024, None)
     demand = member_demand(cfgs) if vary_demand else None
@@ -967,6 +999,7 @@ def train_iql_population(config, base_dir, seeds, test_mode='no_test', n_replica
     seeds = parse_seeds(seeds if isinstance(seeds, str) else ','.join(str(int(x)) for x in seeds))
     config, name = _read_config(config)
     agent = _iql_agent(config, 'train_iql_population')
+    _check_imitation([config])
     cfgs = []
     for s in seeds:
         cfg = copy.deepcopy(config)
@@ -995,6 +1028,7 @@ def train_iql_sweep(configs, base_dir, test_mode='no_test', n_replicas=1, device
     items = sweep_members(configs, IQL_SWEEP_CONFIG_KEYS, demand=vary_demand)
     agent = _iql_agent(items[0][1], 'train_iql_sweep')
     cfgs = [c for _, c, _ in items]
+    _check_imitation(cfgs)
     seeds = [c['ENV_CONFIG'].getint('seed') for c in cfgs]
     names = [n for n, _, _ in items]
     paths = [sweep_dir(base_dir, n, agent) for n in names]

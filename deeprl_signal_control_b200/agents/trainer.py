@@ -106,7 +106,8 @@ def set_mix_demand(sim, demand_mix, replica0=0):
 class BatchedTrainer:
     def __init__(self, sim: BatchedSim, model: BatchedA2C, agent: str, lr, beta,
                  seed0: int = 12, replica0: int = 0, greward_trace: Optional[torch.Tensor] = None,
-                 summary_rec: Optional[torch.Tensor] = None, coop_gamma=None, demand=None, demand_mix=None):
+                 summary_rec: Optional[torch.Tensor] = None, coop_gamma=None, demand=None, demand_mix=None,
+                 imit=None, greedy_program=None):
         """lr / beta: floats (the 'constant' schedules of every shipped A2C config) or objects with the reference's
         `Scheduler.get(n_step)` (agents/utils.py:268-281, agents/models.py:175-176); a schedule advances by n_step per
         update exactly as in the reference (its unit is control steps of ONE environment).
@@ -123,7 +124,13 @@ class BatchedTrainer:
         (BatchedSim.set_replica_coop_gamma), and `demand`, one NetTables per member: member k's replicas then take
         their traffic demand from demand[k] (BatchedSim.set_replica_demand).
         demand_mix: one agent trained on a mixture of demand levels, a list of L NetTables; global replica g (this
-        simulator's replica g - replica0) runs at level g mod L (`set_mix_demand`)."""
+        simulator's replica g - replica0) runs at level g mod L (`set_mix_demand`).
+        A learner with a teacher (`BatchedA2C(teacher=...)`): every control step labels the student's state into
+        model.teach_hist[t] before the simulator step (one tsc_pressure_actions or tsc_greedy_actions launch), and every
+        update passes the imitation coefficient `imit` (a float, a schedule, or one per sweep member, as lr / beta) to
+        backward().  `greedy_program`: the greedy teacher's table, greedy_controller(env).greedy_program(node_obs_off)
+        of the training env, set on the simulator once here.  summary_rec then has a 5th column, agent 0's imitation
+        loss (model.stats[3])."""
         set_member_demand(sim, demand, int(getattr(model, "K", 1)))
         set_mix_demand(sim, demand_mix, replica0)
         if coop_gamma is not None:
@@ -133,6 +140,21 @@ class BatchedTrainer:
             sim.set_replica_coop_gamma(np.repeat(np.asarray(coop_gamma, np.float32), R_m))
         self.sim, self.model, self.agent = sim, model, agent
         self.lr, self.beta = lr, beta
+        self.teacher = getattr(model, "teacher", None)
+        if self.teacher is None and (imit is not None or greedy_program is not None):
+            raise ValueError("imit / greedy_program need a learner with a teacher (BatchedA2C(teacher=...))")
+        if self.teacher is not None and imit is None:
+            raise ValueError("a learner with teacher %r needs the imitation coefficient `imit`" % self.teacher)
+        self.imit = imit
+        if self.teacher == "greedy":
+            if greedy_program is None:
+                raise ValueError("the greedy teacher needs the training env's greedy_program")
+            max_cand, off, idx, act = (int(greedy_program[0]),) + tuple(np.ascontiguousarray(a, np.int32)
+                                                                       for a in greedy_program[1:])
+            _lib.check(_lib.lib().tsc_set_greedy_program(sim._h, max_cand, off.ctypes.data, idx.ctypes.data,
+                                                         act.ctypes.data))
+        elif greedy_program is not None:
+            raise ValueError("greedy_program is the greedy teacher's (the teacher is %r)" % self.teacher)
         self.seed0, self.replica0 = int(seed0), int(replica0)
         self.total_replicas = int(getattr(model, "total_replicas", sim.R))
         self.K = int(getattr(model, "K", 1))
@@ -140,8 +162,8 @@ class BatchedTrainer:
         self.T_episode = int(np.ceil(sim.params.episode_length_sec / sim.params.control_interval_sec))
         assert self.T_episode % model.T == 0                      # utils.py:121
         self.greward_trace = _check_trace(greward_trace, self.T_episode, sim)
-        self.summary_rec = _check_rec(summary_rec, (self.T_episode // model.T,) + ((self.K,) if self.K > 1 else ()) + (4,),
-                                      sim.device)
+        self.summary_rec = _check_rec(summary_rec, (self.T_episode // model.T,) + ((self.K,) if self.K > 1 else ()) +
+                                      (5 if self.teacher else 4,), sim.device)
         self.summary_ran = np.ones(self.T_episode // model.T, bool)       # every A2C update runs
         self.step_in_episode = 0
         self.done = True
@@ -191,6 +213,8 @@ class BatchedTrainer:
         fused = bool(getattr(m, 'tc_v2', False))      # fused tensor-core forward: one-launch transition hand-over
         pi, val, act = m.forward(m.obs_slot(t), self.done, to_hist=True) if fused else m.forward(m.obs_slot(t), self.done)
         fp = pi if self.agent == 'ma2c' else None                 # env.update_fingerprint(policy)
+        if self.teacher is not None:
+            self.label(t)
         if self.sim_events is not None:
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
@@ -212,10 +236,27 @@ class BatchedTrainer:
         if m.t == m.T:
             self.update()
 
+    def label(self, t: int):
+        """The teacher's action for the state the student is in at step t (the one obs_hist[t] describes) into
+        teach_hist[t]: max-pressure from the lane counts the last simulator step / observe left, greedy from
+        obs_hist[t].  Issued before that step's simulator launch."""
+        sim, m = self.sim, self.model
+        st = sim._stream()
+        if self.teacher == "maxpressure":
+            _lib.check(_lib.lib().tsc_pressure_actions(sim._h, _lib.ptr(m.teach_hist[t]), st))
+        else:
+            _lib.check(_lib.lib().tsc_greedy_actions(sim._h, _lib.ptr(m.obs_hist[t]), _lib.ptr(m.teach_hist[t]), st))
+
+    def _no_teacher(self, what):
+        if self.teacher is not None:
+            raise ValueError("%s does not label states for a teacher (teacher %r): train with control_step()"
+                             % (what, self.teacher))
+
     def control_step_host(self):
         """Same step with the environment driven through the HOST-buffer C-ABI call (tsc_step_host),
         i.e. the way a reference-style caller holds numpy arrays: actions / fingerprints D2H, env step
-        (H2D + kernel + D2H inside), observation / reward H2D into the learner."""
+        (H2D + kernel + D2H inside), observation / reward H2D into the learner.  Not with a teacher."""
+        self._no_teacher("control_step_host")
         sim, m = self.sim, self.model
         t = m.t
         pi, val, act = m.forward(m.obs_slot(t), self.done)
@@ -245,7 +286,9 @@ class BatchedTrainer:
         the PCIe link (tsc_step_host_range: actions H2D, kernel, observations D2H; then observations H2D into the
         learner), the other ranges run their policy forward / simulator kernels.  Same results as control_step_host():
         ranges are independent and the sampling RNG is keyed by the absolute replica.  The host still receives every
-        range's observations / rewards in page-locked numpy buffers before the learner consumes them."""
+        range's observations / rewards in page-locked numpy buffers before the learner consumes them.  Not with a
+        teacher."""
+        self._no_teacher("control_step_host_pipelined")
         sim, m = self.sim, self.model
         m._one_reward_scaling("the host-range pipeline")
         R, A, L = sim.R, m.lay.A, m.lay
@@ -333,11 +376,17 @@ class BatchedTrainer:
         boot = None
         if not self.done:
             _, boot, _ = m.forward(m.obs_slot(m.T), False, out_type='v')    # utils.py:190
-        m.backward(boot, schedule_values(self.lr, m.T), schedule_values(self.beta, m.T))
+        if self.teacher is None:
+            m.backward(boot, schedule_values(self.lr, m.T), schedule_values(self.beta, m.T))
+        else:
+            m.backward(boot, schedule_values(self.lr, m.T), schedule_values(self.beta, m.T),
+                       schedule_values(self.imit, m.T))
         if self.summary_rec is not None:
             j = self.step_in_episode // m.T - 1
             self.summary_rec[j, ..., :3].copy_(m.stats[..., :3])
-            self.summary_rec[j, ..., 3:].copy_(m.norms[..., :1])
+            self.summary_rec[j, ..., 3:4].copy_(m.norms[..., :1])
+            if self.teacher is not None:
+                self.summary_rec[j, ..., 4:].copy_(m.stats[..., 3:4])
         self.n_updates += 1
         if self.done and self.K > 1:
             R_m = m.R_m

@@ -14,6 +14,7 @@
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <cmath>
 
 #include <string>
 #include <map>
@@ -359,12 +360,16 @@ __global__ void returns_g_kernel(const float* __restrict__ rew, const float* __r
 #define HL_DL 12                       // dlog (8) | dv | pad
 // Shared-memory traffic bounds this kernel: rows and the head
 // weights are therefore moved with 128-bit accesses only (Wp padded to 8 logits per hidden unit = two broadcast loads).
+// IMIT (tscl_heads_loss_imit): the imitation term  -imit * log clip(pi_b, 1e-10, 1)  toward the teacher's action
+// b = teach[row] joins the loss, the policy-gradient term with adv := imit and a := b, added in the same pass; agent
+// 0's unweighted sum of -log clip(pi_b) goes to stats[3].
+template <bool IMIT>
 __global__ void __launch_bounds__(128)
 heads_loss_kernel(const DDims d, const float* __restrict__ P, const float* __restrict__ Hm,
                   const __nv_bfloat16* __restrict__ Hb, const int32_t* __restrict__ act, const float* __restrict__ Rs,
                   const float* __restrict__ Adv, int64_t M, int64_t Rc, int64_t stride_t, float v_coef, float beta,
                   float scale, float* __restrict__ dlog, float* __restrict__ dH, float* __restrict__ stats,
-                  float* __restrict__ G) {
+                  float* __restrict__ G, const int32_t* __restrict__ teach, float imit) {
   extern __shared__ __align__(16) float sm[];
   const int a = blockIdx.y, tid = threadIdx.x, na = d.n_a[a], mna = d.max_na;
   float* sWp = sm;                     // [64][8]
@@ -379,7 +384,7 @@ heads_loss_kernel(const DDims d, const float* __restrict__ P, const float* __res
   for (int i = tid; i < mna; i += 128) sb[i] = P[d.off_bo + (int64_t)(2 * a) * mna + i];
   if (tid == 0) sb[mna] = P[d.off_bo + (int64_t)(2 * a + 1) * mna];
   __syncthreads();
-  float pl = 0.f, vl = 0.f, el = 0.f;
+  float pl = 0.f, vl = 0.f, el = 0.f, il = 0.f;
   float accp[4] = {0.f, 0.f, 0.f, 0.f}, accv = 0.f, accb = 0.f;
   const int kk = tid & 63, hh = tid >> 6;
   const int64_t n_tiles = (M + 127) / 128;
@@ -472,12 +477,13 @@ heads_loss_kernel(const DDims d, const float* __restrict__ P, const float* __res
       const float inv = 1.0f / s;
       const int at = act[io];
       const float adv = Adv[io];
+      const int bt = IMIT ? teach[io] : -1;
       // log(clip(pi, 1e-10, 1)) (agents/policies.py:47) has zero derivative where the clip is active: a taken action
       // with pi < 1e-10 contributes no policy gradient, and a clipped pi_k drops its "+1" from the entropy gradient
       // beta * pi_j * (lp_j + m_j + ent - sum_k pi_k m_k),  m_k = [1e-10 <= pi_k <= 1],  written with
       // sum_k pi_k m_k = 1 - clip_mass so that nothing changes when no pi is clipped
       float lp[8], ent = 0.f, clip_mass = 0.f;
-      bool in_at = true;
+      bool in_at = true, in_bt = true;
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
         lg[j] *= inv;                                             // pi_j
@@ -486,13 +492,15 @@ heads_loss_kernel(const DDims d, const float* __restrict__ P, const float* __res
         const bool clipped = j < na && !(lg[j] >= 1e-10f && lg[j] <= 1.0f);
         if (clipped) clip_mass += lg[j];
         if (clipped && j == at) in_at = false;
+        if (IMIT && clipped && j == bt) in_bt = false;
       }
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
         float g = 0.f;
         if (j < na) {
           const bool clipped = !(lg[j] >= 1e-10f && lg[j] <= 1.0f);
-          const float pg = in_at ? -adv * ((j == at ? 1.f : 0.f) - lg[j]) : 0.f;
+          float pg = in_at ? -adv * ((j == at ? 1.f : 0.f) - lg[j]) : 0.f;
+          if (IMIT) pg += in_bt ? -imit * ((j == bt ? 1.f : 0.f) - lg[j]) : 0.f;
           g = scale * (pg + beta * lg[j] * (lp[j] + ent + clip_mass - (clipped ? 1.f : 0.f)));
         }
         dl[j] = g;
@@ -521,6 +529,10 @@ heads_loss_kernel(const DDims d, const float* __restrict__ P, const float* __res
         for (int j = 0; j < 8; ++j) if (j == at) pl += -lp[j] * adv;
         vl += 0.5f * v_coef * (ret - v) * (ret - v);
         el += -beta * ent;
+        if (IMIT) {
+#pragma unroll
+          for (int j = 0; j < 8; ++j) if (j == bt) il += -lp[j];
+        }
       }
     } else {
 #pragma unroll
@@ -555,9 +567,11 @@ heads_loss_kernel(const DDims d, const float* __restrict__ P, const float* __res
       pl += __shfl_down_sync(0xffffffffu, pl, o);
       vl += __shfl_down_sync(0xffffffffu, vl, o);
       el += __shfl_down_sync(0xffffffffu, el, o);
+      if (IMIT) il += __shfl_down_sync(0xffffffffu, il, o);
     }
     if ((tid & 31) == 0) {
       atomicAdd(&stats[0], pl * scale); atomicAdd(&stats[1], vl * scale); atomicAdd(&stats[2], el * scale);
+      if (IMIT) atomicAdd(&stats[3], il * scale);
     }
   }
 }
@@ -1237,8 +1251,30 @@ extern "C" int tscl_heads_loss(tscl_handle* h, const float* params, const float*
   const int64_t n_tiles = (M + 127) / 128;
   dim3 grid((unsigned)(grads ? (n_tiles < HL_GX ? n_tiles : HL_GX) : n_tiles), h->d.A);
   const int smem = (H64 * 8 + H64 + 16 + 128 * HL_LD + 128 * HL_DL) * 4;
-  heads_loss_kernel<<<grid, 128, smem, (cudaStream_t)stream>>>(h->d, params, H, (const __nv_bfloat16*)h_bf16, act, Rs, Adv,
-                                                               M, Rc, stride_t, v_coef, beta, scale, dlog, dH, stats, grads);
+  heads_loss_kernel<false><<<grid, 128, smem, (cudaStream_t)stream>>>(h->d, params, H, (const __nv_bfloat16*)h_bf16, act,
+                                                                      Rs, Adv, M, Rc, stride_t, v_coef, beta, scale, dlog,
+                                                                      dH, stats, grads, nullptr, 0.f);
+  LCK(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int tscl_heads_loss_imit(tscl_handle* h, const float* params, const float* H, const int32_t* act,
+                                    const float* Rs, const float* Adv, int64_t M, int64_t Rc, int64_t stride_t,
+                                    float v_coef, float beta, float scale, float* dlog, float* dH, float* stats,
+                                    const void* h_bf16, float* grads, const int32_t* teach, float imit_coef,
+                                    void* stream) {
+  if (!h || M <= 0 || (!H && !h_bf16) || !dH || !teach) return tsc_set_error("tscl_heads_loss_imit: bad argument");
+  if (!(std::isfinite(imit_coef) && imit_coef >= 0.f))
+    return tsc_set_error("tscl_heads_loss_imit: the imitation coefficient must be finite and >= 0");
+  NO_DET("tscl_heads_loss_imit");
+  if (h->d.max_na > 8) return tsc_set_error("tscl_heads_loss_imit: more than 8 actions");
+  LCK(cudaSetDevice(h->device));
+  const int64_t n_tiles = (M + 127) / 128;
+  dim3 grid((unsigned)(grads ? (n_tiles < HL_GX ? n_tiles : HL_GX) : n_tiles), h->d.A);
+  const int smem = (H64 * 8 + H64 + 16 + 128 * HL_LD + 128 * HL_DL) * 4;
+  heads_loss_kernel<true><<<grid, 128, smem, (cudaStream_t)stream>>>(h->d, params, H, (const __nv_bfloat16*)h_bf16, act,
+                                                                     Rs, Adv, M, Rc, stride_t, v_coef, beta, scale, dlog,
+                                                                     dH, stats, grads, teach, imit_coef);
   LCK(cudaGetLastError());
   return 0;
 }

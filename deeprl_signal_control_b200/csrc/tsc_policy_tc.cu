@@ -16,6 +16,7 @@
 //   A tile  [KC][128 rows][16 B]   : LBO = 2048 (next K chunk of 8 bf16), SBO = 128 (next 8 rows)
 //   B tile  [KC][256 cols][16 B]   : LBO = 4096,                          SBO = 128
 #include <cuda.h>
+#include <cmath>
 #include <cstdlib>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -1368,8 +1369,15 @@ struct BwdTC {
 // atomic instantiations.
 struct DetTC {
   float* part;               // [slab rows][floats per row]
-  float* part_st;            // BPTT: agent 0's loss sums per (item, warp) [items][8][3]
+  float* part_st;            // BPTT: agent 0's loss sums per (item, warp) [items][8][3] ([..][4] with the imitation term)
   int64_t seg_tiles, n_seg;
+};
+
+// The imitation term of lstm_bwd_tc_regs_kernel<., true, ., true> (tscl_lstm_seq_bwd_tc_heads_imit): the teacher's
+// action of every row, laid out like BwdTC::act, and its coefficient.  The last kernel argument, unused without IMIT.
+struct ImitTC {
+  const int32_t* teach;
+  float coef;
 };
 
 // NT = 512: thread = (replica row, 16 hidden units), one CTA per SM.
@@ -1619,11 +1627,13 @@ __device__ __forceinline__ void tma_store_3d(const CUtensorMap* m, int x, int y,
 // Loss gradients at the heads for one step of a warpgroup of lstm_bwd_tc_regs_kernel<., true>: the thread's rows
 // rr0, rr0 + 8 of the chunk (rg0, rg0 + 8 of the update), h_t in the swizzled tile sH.  Writes dht = dH + dhc for the
 // thread's 16 units (the register layout of the kernel), the rows' dlog into sDl (value unit: dv in slot 0) and adds
-// agent 0's loss terms.  The per-row arithmetic is heads_loss_kernel's (tsc_learn.cu), expression for expression.
+// agent 0's loss terms.  The per-row arithmetic is heads_loss_kernel's (tsc_learn.cu), expression for expression, with
+// and without its IMIT term (the teacher's action from im.teach, agent 0's cross-entropy sum in il).
+template <bool IMIT>
 __device__ __forceinline__ void heads_step(const DDimsTC& d, const BwdTC& a, const unsigned char* sH, const float* sHW,
                                            float* sDl, bool pol, int ag, int na, int rq, int rr0, int lane, int q,
                                            int64_t rg0, int t, const float (&dhc)[8][4], float (&dht)[8][4], float& pl,
-                                           float& vl, float& el) {
+                                           float& vl, float& el, const ImitTC& im, float& il) {
   constexpr int HB_DL = 12;
   const float* sWp = sHW;                  // [64][8]
   const float* sWv = sHW + 512;            // [64]
@@ -1675,9 +1685,10 @@ __device__ __forceinline__ void heads_step(const DDimsTC& d, const BwdTC& a, con
         const float inv = 1.0f / s;
         const int at = a.act[io[h]];
         const float adv = a.Adv[io[h]];
+        const int bt = IMIT ? im.teach[io[h]] : -1;
         // log(clip(pi, 1e-10, 1)) and its gradient: see heads_loss_kernel
         float lp[8], ent = 0.f, clip_mass = 0.f;
-        bool in_at = true;
+        bool in_at = true, in_bt = true;
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
           lg[j] *= inv;                                             // pi_j
@@ -1686,13 +1697,15 @@ __device__ __forceinline__ void heads_step(const DDimsTC& d, const BwdTC& a, con
           const bool clipped = j < na && !(lg[j] >= 1e-10f && lg[j] <= 1.0f);
           if (clipped) clip_mass += lg[j];
           if (clipped && j == at) in_at = false;
+          if (IMIT && clipped && j == bt) in_bt = false;
         }
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
           float g = 0.f;
           if (j < na) {
             const bool clipped = !(lg[j] >= 1e-10f && lg[j] <= 1.0f);
-            const float pg = in_at ? -adv * ((j == at ? 1.f : 0.f) - lg[j]) : 0.f;
+            float pg = in_at ? -adv * ((j == at ? 1.f : 0.f) - lg[j]) : 0.f;
+            if (IMIT) pg += in_bt ? -im.coef * ((j == bt ? 1.f : 0.f) - lg[j]) : 0.f;
             g = a.scale * (pg + a.beta * lg[j] * (lp[j] + ent + clip_mass - (clipped ? 1.f : 0.f)));
           }
           dl[h][j] = g;
@@ -1701,6 +1714,10 @@ __device__ __forceinline__ void heads_step(const DDimsTC& d, const BwdTC& a, con
 #pragma unroll
           for (int j = 0; j < 8; ++j) if (j == at) pl += -lp[j] * adv;
           el += -a.beta * ent;
+          if (IMIT) {
+#pragma unroll
+            for (int j = 0; j < 8; ++j) if (j == bt) il += -lp[j];
+          }
         }
       }
       float s0 = 0.f, s1 = 0.f;              // this thread's share of the staging row: dlog 2 q, 2 q + 1
@@ -1773,11 +1790,13 @@ __device__ __forceinline__ void heads_step(const DDimsTC& d, const BwdTC& a, con
 // Items run over n_chunks consecutive chunks (chunk-outermost, the activation store's order).
 // DET (with HEADS): at the end of every item each thread stores its head sums into det.part [item][256 threads][5] and
 // each warp of a unit of agent 0 its loss sums into det.part_st [item][8 warps][3]; det_heads_reduce_kernel adds them.
-template <bool PROF, bool HEADS = false, bool DET = false>
+// IMIT (with HEADS): the imitation term of heads_loss_kernel<true> (tscl_lstm_seq_bwd_tc_heads_imit) toward im.teach,
+// agent 0's cross-entropy sum as a 4th loss sum (stats[3]; det.part_st rows of 4).
+template <bool PROF, bool HEADS = false, bool DET = false, bool IMIT = false>
 __global__ void __launch_bounds__(256, 1)
 lstm_bwd_tc_regs_kernel(const DDimsTC d, const BwdTC a, const __grid_constant__ CUtensorMap mapG,
                         const __grid_constant__ CUtensorMap mapC, const __grid_constant__ CUtensorMap mapD,
-                        const __grid_constant__ CUtensorMap mapZ, const DetTC det) {
+                        const __grid_constant__ CUtensorMap mapZ, const DetTC det, const ImitTC im) {
   const int tid = threadIdx.x, wg = tid >> 7, w = (tid >> 5) & 3, lane = tid & 31, q = lane & 3;
   const bool lead = (tid & 127) == 0;
   long long bp[4] = {0, 0, 0, 0}, pc = 0;
@@ -1812,7 +1831,7 @@ lstm_bwd_tc_regs_kernel(const DDimsTC d, const BwdTC a, const __grid_constant__ 
   uint32_t ldpar = 0, hpar = 0;
   // HEADS: head weight / bias gradient sums of the current unit, thread = (hidden unit hk, logits 4 hh .. 4 hh + 3)
   const int hk = tid & 63, hh = (tid >> 6) & 1;
-  float gw[4] = {0.f, 0.f, 0.f, 0.f}, gb = 0.f, pl = 0.f, vl = 0.f, el = 0.f;
+  float gw[4] = {0.f, 0.f, 0.f, 0.f}, gb = 0.f, pl = 0.f, vl = 0.f, el = 0.f, il = 0.f;
   auto flush = [&](int uu) {
     const int nl = (uu & 1) ? 1 : d.max_na;                          // value units have one output
 #pragma unroll
@@ -1884,7 +1903,8 @@ lstm_bwd_tc_regs_kernel(const DDimsTC d, const BwdTC a, const __grid_constant__ 
       if (HEADS) { mbar_wait(hbar, hpar); hpar ^= 1; }               // and h_t
       BR_MARK(0);
       float dht[8][4];                                               // dH + dh carry
-      if constexpr (HEADS) heads_step(d, a, sH, sHW, sDl, pol, ag, na, rq, rw0 + rq, lane, q, rg0, t, dhc, dht, pl, vl, el);
+      if constexpr (HEADS)
+        heads_step<IMIT>(d, a, sH, sHW, sDl, pol, ag, na, rq, rw0 + rq, lane, q, rg0, t, dhc, dht, pl, vl, el, im, il);
       // shared memory -> registers; bf16 pairs [j][h]: row rq + 8 h, units 8 j + 2 q + {0 (low half), 1}
       uint32_t gr[4][8][2], cr[8][2], pr[8][2];
 #pragma unroll
@@ -2017,12 +2037,14 @@ lstm_bwd_tc_regs_kernel(const DDimsTC d, const BwdTC a, const __grid_constant__ 
           pl += __shfl_down_sync(0xffffffffu, pl, o);
           vl += __shfl_down_sync(0xffffffffu, vl, o);
           el += __shfl_down_sync(0xffffffffu, el, o);
+          if (IMIT) il += __shfl_down_sync(0xffffffffu, il, o);
         }
         if (lane == 0) {
-          float* ps = det.part_st + (it * 8 + (tid >> 5)) * 3;
+          float* ps = det.part_st + (it * 8 + (tid >> 5)) * (IMIT ? 4 : 3);
           ps[0] = pl; ps[1] = vl; ps[2] = el;
+          if (IMIT) ps[3] = il;
         }
-        pl = vl = el = 0.f;
+        pl = vl = el = il = 0.f;
       }
     }
   }
@@ -2035,9 +2057,11 @@ lstm_bwd_tc_regs_kernel(const DDimsTC d, const BwdTC a, const __grid_constant__ 
         pl += __shfl_down_sync(0xffffffffu, pl, o);
         vl += __shfl_down_sync(0xffffffffu, vl, o);
         el += __shfl_down_sync(0xffffffffu, el, o);
+        if (IMIT) il += __shfl_down_sync(0xffffffffu, il, o);
       }
-      if (lane == 0 && (pl != 0.f || vl != 0.f || el != 0.f)) {
+      if (lane == 0 && (pl != 0.f || vl != 0.f || el != 0.f || il != 0.f)) {
         atomicAdd(&a.stats[0], pl * a.scale); atomicAdd(&a.stats[1], vl * a.scale); atomicAdd(&a.stats[2], el * a.scale);
+        if (IMIT) atomicAdd(&a.stats[3], il * a.scale);
       }
     }
   }
@@ -2156,8 +2180,8 @@ extern "C" int tscl_lstm_seq_bwd_tc_dx(tscl_handle* h, const void* wt_bf16, floa
       }
       const int grid_r = (int)(n_items < n_sm ? n_items : n_sm);
       a.prof = g_bptt_prof;
-      if (a.prof) lstm_bwd_tc_regs_kernel<true><<<grid_r, 256, BR_SMEM, (cudaStream_t)stream>>>(d, a, mG, mC, mD, mZ, DetTC{});
-      else lstm_bwd_tc_regs_kernel<false><<<grid_r, 256, BR_SMEM, (cudaStream_t)stream>>>(d, a, mG, mC, mD, mZ, DetTC{});
+      if (a.prof) lstm_bwd_tc_regs_kernel<true><<<grid_r, 256, BR_SMEM, (cudaStream_t)stream>>>(d, a, mG, mC, mD, mZ, DetTC{}, ImitTC{});
+      else lstm_bwd_tc_regs_kernel<false><<<grid_r, 256, BR_SMEM, (cudaStream_t)stream>>>(d, a, mG, mC, mD, mZ, DetTC{}, ImitTC{});
       PCK(cudaGetLastError());
       return 0;
     }
@@ -2172,7 +2196,9 @@ extern "C" int tscl_lstm_seq_bwd_tc_dx(tscl_handle* h, const void* wt_bf16, floa
 // each chunk's sum over its tiles and warpgroups in that order (thread k = (hidden unit k & 63, logits 4 (k >> 6) ..));
 // block 2A adds agent 0's loss sums chunk by chunk: lane l takes the chunk's (unit, tile, warp) entries l, l + 32, .. in
 // order, then a fixed shuffle tree.  Adding per chunk makes one launch over n chunks give the bits of n one-chunk
-// launches.  A warpgroup whose first row is past Rc stored nothing and is skipped.
+// launches.  A warpgroup whose first row is past Rc stored nothing and is skipped.  NS: loss sums per warp entry (3, or
+// 4 with the imitation term's cross-entropy into stats[3]).
+template <int NS>
 __global__ void __launch_bounds__(128)
 det_heads_reduce_kernel(const DDimsTC d, const DetTC det, float* __restrict__ G, float* __restrict__ stats, float scale,
                         int n_chunks, int64_t n_tiles, int64_t Rc) {
@@ -2198,46 +2224,59 @@ det_heads_reduce_kernel(const DDimsTC d, const DetTC det, float* __restrict__ G,
   if (!stats || k >= 32) return;
   const int64_t n = 2 * n_tiles * 8;                          // (unit 0 / 1, tile, warp) of one chunk
   for (int ci = 0; ci < n_chunks; ++ci) {
-    float s[3] = {0.f, 0.f, 0.f};
+    float s[NS] = {};
     for (int64_t e = k; e < n; e += 32) {
       const int w8 = (int)(e & 7);
       const int64_t tl = (e >> 3) % n_tiles, uu = (e >> 3) / n_tiles;
       if (tl * TC_M + 64 * (w8 >> 2) >= Rc) continue;
-      const float* p = det.part_st + (((ci * 2 * d.A + uu) * n_tiles + tl) * 8 + w8) * 3;
-      s[0] += p[0]; s[1] += p[1]; s[2] += p[2];
+      const float* p = det.part_st + (((ci * 2 * d.A + uu) * n_tiles + tl) * 8 + w8) * NS;
+#pragma unroll
+      for (int i = 0; i < NS; ++i) s[i] += p[i];
     }
 #pragma unroll
     for (int o = 16; o; o >>= 1)
 #pragma unroll
-      for (int i = 0; i < 3; ++i) s[i] += __shfl_down_sync(0xffffffffu, s[i], o);
-    if (k == 0) { stats[0] += s[0] * scale; stats[1] += s[1] * scale; stats[2] += s[2] * scale; }
+      for (int i = 0; i < NS; ++i) s[i] += __shfl_down_sync(0xffffffffu, s[i], o);
+    if (k == 0) {
+#pragma unroll
+      for (int i = 0; i < NS; ++i) stats[i] += s[i] * scale;
+    }
   }
 }
 
-extern "C" int tscl_lstm_seq_bwd_tc_heads(tscl_handle* h, const void* wt_bf16, const float* params, const void* gates_bf16,
-                                          const void* c_bf16, const void* h_bf16, const float* c0, const float* done,
-                                          const int32_t* act, const float* Rs, const float* Adv, int32_t T, int64_t Rc,
-                                          int32_t n_chunks, int64_t ld_state, int64_t r0, int64_t stride_t, float v_coef,
-                                          float beta, float scale, void* dz_bf16, float* stats, float* grads, void* stream) {
+// tscl_lstm_seq_bwd_tc_heads (teach == nullptr) and tscl_lstm_seq_bwd_tc_heads_imit (the IMIT instantiations)
+static int bwd_tc_heads(const char* name, tscl_handle* h, const void* wt_bf16, const float* params, const void* gates_bf16,
+                        const void* c_bf16, const void* h_bf16, const float* c0, const float* done, const int32_t* act,
+                        const float* Rs, const float* Adv, int32_t T, int64_t Rc, int32_t n_chunks, int64_t ld_state,
+                        int64_t r0, int64_t stride_t, float v_coef, float beta, float scale, void* dz_bf16, float* stats,
+                        float* grads, const int32_t* teach, float imit_coef, void* stream) {
+  const std::string nm(name);
   if (!h || !wt_bf16 || !params || !gates_bf16 || !c_bf16 || !h_bf16 || !c0 || !done || !act || !Rs || !Adv || !dz_bf16 ||
       !grads || T <= 0 || Rc <= 0 || n_chunks <= 0)
-    return tsc_set_error("tscl_lstm_seq_bwd_tc_heads: bad argument");
+    return tsc_set_error(nm + ": bad argument");
+  const bool imit = teach != nullptr;
+  if (imit && !(std::isfinite(imit_coef) && imit_coef >= 0.f))
+    return tsc_set_error(nm + ": the imitation coefficient must be finite and >= 0");
   PCK(cudaSetDevice(tscl_device_of(h)));
   const DDimsTC& d = *tscl_dims_of(h);
-  if (d.max_na > 8) return tsc_set_error("tscl_lstm_seq_bwd_tc_heads: more than 8 actions");
-  if ((uint64_t)n_chunks * 2 * d.A * T > 0x7fffffffu) return tsc_set_error("tscl_lstm_seq_bwd_tc_heads: too many planes");
+  if (d.max_na > 8) return tsc_set_error(nm + ": more than 8 actions");
+  if ((uint64_t)n_chunks * 2 * d.A * T > 0x7fffffffu) return tsc_set_error(nm + ": too many planes");
   CUtensorMap mG, mC, mH, mZ;
   const uint64_t planes = (uint64_t)n_chunks * 2 * d.A * T;
   if (!(make_tmap_3d(&mG, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, gates_bf16, planes, Rc, TC_N, 64, 64) &&
         make_tmap_3d(&mC, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, c_bf16, planes, Rc, TC_H, 64, 64) &&
         make_tmap_3d(&mH, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, h_bf16, planes, Rc, TC_H, 64, 64) &&
         make_tmap_3d(&mZ, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, dz_bf16, planes, Rc, TC_N, 64, 64)))
-    return tsc_set_error("tscl_lstm_seq_bwd_tc_heads: cannot encode the tensor maps (cuTensorMapEncodeTiled)");
+    return tsc_set_error(nm + ": cannot encode the tensor maps (cuTensorMapEncodeTiled)");
   static int attr_r = -1;
   if (attr_r != tscl_device_of(h)) {
     PCK(cudaFuncSetAttribute(lstm_bwd_tc_regs_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, BR_SMEM));
     PCK(cudaFuncSetAttribute(lstm_bwd_tc_regs_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, BR_SMEM));
     PCK(cudaFuncSetAttribute(lstm_bwd_tc_regs_kernel<false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, BR_SMEM));
+    PCK(cudaFuncSetAttribute(lstm_bwd_tc_regs_kernel<false, true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                             BR_SMEM));
+    PCK(cudaFuncSetAttribute(lstm_bwd_tc_regs_kernel<false, true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                             BR_SMEM));
     attr_r = tscl_device_of(h);
   }
   int n_sm = 0;
@@ -2252,21 +2291,58 @@ extern "C" int tscl_lstm_seq_bwd_tc_heads(tscl_handle* h, const void* wt_bf16, c
   a.P = params; a.act = act; a.Rs = Rs; a.Adv = Adv; a.stride_t = stride_t; a.v_coef = v_coef; a.beta = beta;
   a.scale = scale; a.stats = stats; a.G = grads; a.n_chunks = n_chunks;
   a.prof = g_bptt_prof;
+  const ImitTC im = {teach, imit_coef};
   if (det_ctas >= 0) {
+    const int ns = imit ? 4 : 3;                                     // loss sums per (item, warp)
     DetTC det = {};
-    det.part = tscl_det_slab(h, 0, (size_t)n_items * (256 * 5 + 8 * 3) * sizeof(float), stream);
-    if (!det.part) return tsc_set_error("tscl_lstm_seq_bwd_tc_heads: cudaMalloc of the deterministic slab failed");
+    det.part = tscl_det_slab(h, 0, (size_t)n_items * (256 * 5 + 8 * ns) * sizeof(float), stream);
+    if (!det.part) return tsc_set_error(nm + ": cudaMalloc of the deterministic slab failed");
     det.part_st = det.part + n_items * 256 * 5;
-    lstm_bwd_tc_regs_kernel<false, true, true><<<grid, 256, BR_SMEM, (cudaStream_t)stream>>>(d, a, mG, mC, mH, mZ, det);
-    PCK(cudaGetLastError());
-    det_heads_reduce_kernel<<<2 * d.A + 1, 128, 0, (cudaStream_t)stream>>>(d, det, grads, stats, scale, n_chunks, n_tiles, Rc);
+    if (imit) {
+      lstm_bwd_tc_regs_kernel<false, true, true, true><<<grid, 256, BR_SMEM, (cudaStream_t)stream>>>(d, a, mG, mC, mH, mZ,
+                                                                                                    det, im);
+      PCK(cudaGetLastError());
+      det_heads_reduce_kernel<4><<<2 * d.A + 1, 128, 0, (cudaStream_t)stream>>>(d, det, grads, stats, scale, n_chunks,
+                                                                                n_tiles, Rc);
+    } else {
+      lstm_bwd_tc_regs_kernel<false, true, true><<<grid, 256, BR_SMEM, (cudaStream_t)stream>>>(d, a, mG, mC, mH, mZ, det, im);
+      PCK(cudaGetLastError());
+      det_heads_reduce_kernel<3><<<2 * d.A + 1, 128, 0, (cudaStream_t)stream>>>(d, det, grads, stats, scale, n_chunks,
+                                                                                n_tiles, Rc);
+    }
+  } else if (imit) {                                                 // (no profiling instantiation of the IMIT form)
+    lstm_bwd_tc_regs_kernel<false, true, false, true><<<grid, 256, BR_SMEM, (cudaStream_t)stream>>>(d, a, mG, mC, mH, mZ,
+                                                                                                   DetTC{}, im);
   } else if (a.prof) {
-    lstm_bwd_tc_regs_kernel<true, true><<<grid, 256, BR_SMEM, (cudaStream_t)stream>>>(d, a, mG, mC, mH, mZ, DetTC{});
+    lstm_bwd_tc_regs_kernel<true, true><<<grid, 256, BR_SMEM, (cudaStream_t)stream>>>(d, a, mG, mC, mH, mZ, DetTC{}, im);
   } else {
-    lstm_bwd_tc_regs_kernel<false, true><<<grid, 256, BR_SMEM, (cudaStream_t)stream>>>(d, a, mG, mC, mH, mZ, DetTC{});
+    lstm_bwd_tc_regs_kernel<false, true><<<grid, 256, BR_SMEM, (cudaStream_t)stream>>>(d, a, mG, mC, mH, mZ, DetTC{}, im);
   }
   PCK(cudaGetLastError());
   return 0;
+}
+
+extern "C" int tscl_lstm_seq_bwd_tc_heads(tscl_handle* h, const void* wt_bf16, const float* params, const void* gates_bf16,
+                                          const void* c_bf16, const void* h_bf16, const float* c0, const float* done,
+                                          const int32_t* act, const float* Rs, const float* Adv, int32_t T, int64_t Rc,
+                                          int32_t n_chunks, int64_t ld_state, int64_t r0, int64_t stride_t, float v_coef,
+                                          float beta, float scale, void* dz_bf16, float* stats, float* grads, void* stream) {
+  return bwd_tc_heads("tscl_lstm_seq_bwd_tc_heads", h, wt_bf16, params, gates_bf16, c_bf16, h_bf16, c0, done, act, Rs, Adv,
+                      T, Rc, n_chunks, ld_state, r0, stride_t, v_coef, beta, scale, dz_bf16, stats, grads, nullptr, 0.f,
+                      stream);
+}
+
+extern "C" int tscl_lstm_seq_bwd_tc_heads_imit(tscl_handle* h, const void* wt_bf16, const float* params,
+                                               const void* gates_bf16, const void* c_bf16, const void* h_bf16,
+                                               const float* c0, const float* done, const int32_t* act, const float* Rs,
+                                               const float* Adv, int32_t T, int64_t Rc, int32_t n_chunks, int64_t ld_state,
+                                               int64_t r0, int64_t stride_t, float v_coef, float beta, float scale,
+                                               void* dz_bf16, float* stats, float* grads, const int32_t* teach,
+                                               float imit_coef, void* stream) {
+  if (!teach) return tsc_set_error("tscl_lstm_seq_bwd_tc_heads_imit: bad argument (teach is NULL)");
+  return bwd_tc_heads("tscl_lstm_seq_bwd_tc_heads_imit", h, wt_bf16, params, gates_bf16, c_bf16, h_bf16, c0, done, act, Rs,
+                      Adv, T, Rc, n_chunks, ld_state, r0, stride_t, v_coef, beta, scale, dz_bf16, stats, grads, teach,
+                      imit_coef, stream);
 }
 
 // ===================================================================================================

@@ -106,6 +106,16 @@ int tscl_heads_loss(tscl_handle* h, const float* params, const float* H, const i
                     const float* Adv, int64_t M, int64_t Rc, int64_t stride_t, float v_coef, float beta,
                     float scale, float* dlog, float* dH, float* stats, const void* h_bf16, float* grads,
                     void* stream);
+/* tscl_heads_loss with the imitation term of a teacher (DAgger on the student's own states): per row m and agent the
+ * loss gains  -imit_coef * log clip(pi_b, 1e-10, 1)  toward the teacher's action b = teach[row] (int32, rows laid out
+ * like `act`), so the logits' gradient gains  scale * imit_coef * (pi_j - [j == b])  when pi_b is not clipped (0 when
+ * it is): the policy-gradient term with Adv := imit_coef and act := b, added in the same pass.  stats [4] must hold 4
+ * floats: stats[3] += agent 0's unweighted  sum -log clip(pi_b, 1e-10, 1) * scale.  imit_coef finite and >= 0; at 0
+ * the gradients equal tscl_heads_loss's. */
+int tscl_heads_loss_imit(tscl_handle* h, const float* params, const float* H, const int32_t* act, const float* Rs,
+                         const float* Adv, int64_t M, int64_t Rc, int64_t stride_t, float v_coef, float beta,
+                         float scale, float* dlog, float* dH, float* stats, const void* h_bf16, float* grads,
+                         const int32_t* teach, float imit_coef, void* stream);
 
 /* BPTT through the LSTM (reverse of tscl_lstm_seq_fwd).  ZG holds gate activations on entry and
  * dZ (pre-activation gate gradients) on exit; dH holds head gradients on entry. */
@@ -167,6 +177,16 @@ int tscl_lstm_seq_bwd_tc_heads(tscl_handle* h, const void* wt_bf16, const float*
                                const int32_t* act, const float* Rs, const float* Adv, int32_t T, int64_t Rc,
                                int32_t n_chunks, int64_t ld_state, int64_t r0, int64_t stride_t, float v_coef, float beta,
                                float scale, void* dz_bf16, float* stats, float* grads, void* stream);
+/* tscl_lstm_seq_bwd_tc_heads with tscl_heads_loss_imit's imitation term (teach rows laid out like `act`, imit_coef
+ * finite and >= 0): dz_bf16 is bit-identical to tscl_heads_loss_imit followed by the store-path tscl_lstm_seq_bwd_tc;
+ * agent 0's cross-entropy sum goes to stats[3].  Deterministic mode as tscl_lstm_seq_bwd_tc_heads (4 loss sums per
+ * slab entry). */
+int tscl_lstm_seq_bwd_tc_heads_imit(tscl_handle* h, const void* wt_bf16, const float* params, const void* gates_bf16,
+                                    const void* c_bf16, const void* h_bf16, const float* c0, const float* done,
+                                    const int32_t* act, const float* Rs, const float* Adv, int32_t T, int64_t Rc,
+                                    int32_t n_chunks, int64_t ld_state, int64_t r0, int64_t stride_t, float v_coef,
+                                    float beta, float scale, void* dz_bf16, float* stats, float* grads,
+                                    const int32_t* teach, float imit_coef, void* stream);
 /* Host-buffer loop, one call per replica range and control step (replaces the reference's per-step numpy hand-over of
  * ob / reward into `model.add_transition`, agents/models.py:222-229, main.py / utils.py:272-286): observations
  * host -> obs_dev (the rollout slot), rewards host -> rew_hist_dev = clip(reward / reward_norm) (0 = off for either),
@@ -221,7 +241,7 @@ int tscl_debug_bptt_prof(void* counters_dev);
 int tscl_clip_rmsprop(tscl_handle* h, float* params, float* grads, float* ms, const uint8_t* agent_of,
                       float max_norm, float lr, float alpha, float eps, float* norms, void* stream);
 
-/* Deterministic mode of the lean A2C update (on != 0): later calls of tscl_lstm_seq_bwd_tc_heads, tscl_wgrad_tc (the
+/* Deterministic mode of the lean A2C update (on != 0): later calls of tscl_lstm_seq_bwd_tc_heads[_imit], tscl_wgrad_tc (the
  * all-bf16 store form), tscl_dx_fc_bwd_tc and tscl_clip_rmsprop on this handle add their gradients, loss sums and clip
  * norms in a fixed order instead of with atomics, so that equal inputs give equal bits from run to run and on any
  * H100.  Each kernel stores its accumulator fragments into a partial slab row per work item (BPTT: chunk, unit,
@@ -229,7 +249,7 @@ int tscl_clip_rmsprop(tscl_handle* h, float* params, float* grads, float* ms, co
  * a reduce kernel adds the rows into grads in item order; the clip norm is summed per 8192-element block, then over
  * blocks in order.  The sums therefore depend on the shapes only, not on the grid: n_ctas = 0 keeps each kernel's
  * device-sized grid, n_ctas > 0 caps it (the same bits).  The slabs are owned by the handle, allocated on first use.
- * While the mode is on, the update entry points without a deterministic form (tscl_heads_loss,
+ * While the mode is on, the update entry points without a deterministic form (tscl_heads_loss[_imit],
  * tscl_lstm_seq_bwd_tc[_dx], tscl_fc_bwd_tc, tscl_dx_tc, the other tscl_wgrad_tc forms, tscl_lstm_seq_bwd, tscl_fc_bwd,
  * tscl_fc_hidden_bwd) return an error naming themselves.  on = 0 restores the atomic kernels. */
 int tscl_set_deterministic(tscl_handle* h, int32_t on, int32_t n_ctas);
