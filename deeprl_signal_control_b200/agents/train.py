@@ -3,9 +3,14 @@
 
     train(config, base_dir, test_mode='no_test', n_replicas=1, policy='lstm', device=0, process_group=None,
           summaries=False)
-    train_sweep([a.ini, b.ini, ...], base_dir, ...)   (one member per config in one process, `train_sweep`)
+    train_population(config, base_dir, seeds, ...) / train_sweep([a.ini, b.ini, ...], base_dir, ...)   (ia2c / ma2c
+                                                        members, one per seed or config, in one process)
     train_iql_population(config, base_dir, seeds, ...) / train_iql_sweep([a.ini, ...], base_dir, ...)   (the same for
                                                         iqll / iqld)
+
+The four member fronts refuse what they cannot train and then run one members driver (`_train_members`), built from
+the solo run's parts: the same trainer construction (`_trainer`), summary set-up (`_summaries`) and log set-up
+(`init_log`).
 
 leaves the reference's agent directory: `data/` with a copy of the config and `train_reward.csv`, `model/checkpoint-<step>`
 and `log/<time>.log`; with `after_train_test` / `all_test` also `data/<scenario>_<agent>_{control,traffic,trip}.csv`;
@@ -33,6 +38,7 @@ the device and leaves the training sim and the learner's recurrent state alone.
 from __future__ import annotations
 
 import configparser
+import copy
 import hashlib
 import json
 import logging
@@ -57,11 +63,17 @@ def init_dir(base_dir, pathes=('log', 'data', 'model')):
     return dirs
 
 
-def init_log(log_dir):
-    """utils.py:42-48: INFO records to `<log_dir>/<time>.log` and to stderr.  The handlers are added to the root logger
-    and returned, so that a caller that trains more than once in a process can remove them."""
+def init_log(log_dirs):
+    """utils.py:42-48: INFO records to `<log_dir>/<time>.log` of every directory in `log_dirs` and to stderr.  File k
+    takes the records of member k (`extra={'member': k}`, a population's) and those of no member in particular, so one
+    directory takes every record.  The handlers are added to the root logger and returned, so that a caller that trains
+    more than once in a process can remove them."""
     fmt = logging.Formatter('%(asctime)s [%(levelname)s] %(message)s')
-    handlers = [logging.FileHandler(os.path.join(log_dir, '%d.log' % time.time())), logging.StreamHandler()]
+    handlers = []
+    for k, d in enumerate(log_dirs):
+        handlers.append(logging.FileHandler(os.path.join(d, '%d.log' % time.time())))
+        handlers[-1].addFilter(lambda rec, k=k: getattr(rec, 'member', k) == k)
+    handlers.append(logging.StreamHandler())
     root = logging.getLogger()
     for h in handlers:
         h.setFormatter(fmt)
@@ -395,7 +407,6 @@ def demand_mix_levels(config, demand_mix, n_replicas):
     a key outside the scenario's envs.DEMAND_KEYS, a level that repeats another (same values of every demand key), a
     level whose net differs from the config's in more than its demand tables (`check_demand_tables`), and a replica
     count that is not a multiple of L (each level weighs the same in every gradient)."""
-    import copy
     from ..envs import check_demand_tables, demand_keys, demand_label, make_env
     levels = [dict((str(k), str(v)) for k, v in dict(lv).items()) for lv in demand_mix]
     if not levels:
@@ -474,12 +485,13 @@ def train(config, base_dir, test_mode='no_test', n_replicas=1, policy='lstm', de
     data/<label>/.  Not with `seeds`."""
     if deterministic and policy != 'lstm':
         raise ValueError("deterministic=True needs the LSTM policy's lean update (got policy=%r)" % (policy,))
-    _check_imitation([_read_config(config)[0]])
+    cfg, path = _read_config(config)
+    _check_imitation([cfg])
     mix = None
     if demand_mix is not None:
         if seeds is not None:
             raise ValueError('demand_mix trains one agent: it does not combine with seeds (a population)')
-        mix = demand_mix_levels(_read_config(config)[0], demand_mix, n_replicas)
+        mix = demand_mix_levels(cfg, demand_mix, n_replicas)
     if seeds is not None:
         if process_group is not None:
             raise ValueError('a population trains in one process: seeds and process_group exclude each other')
@@ -495,25 +507,17 @@ def train(config, base_dir, test_mode='no_test', n_replicas=1, policy='lstm', de
     _dist.replica_range(rank, world, int(n_replicas))                 # every rank rejects an uneven split alike
     if rank == 0:
         dirs = init_dir(base_dir)
-        handlers = init_log(dirs['log'])
+        handlers = init_log([dirs['log']])
     else:
         dirs = {k: os.path.join(base_dir, k) + os.sep for k in ('log', 'data', 'model')}
         handlers = init_rank_log(rank)
     try:
-        if isinstance(config, configparser.ConfigParser):
-            if rank == 0:
-                with open(os.path.join(dirs['data'], 'config.ini'), 'w') as f:
-                    config.write(f)
-        else:
-            if rank == 0:
-                shutil.copy(config, dirs['data'])
-            path, config = config, configparser.ConfigParser()
-            if not config.read(path):
-                raise FileNotFoundError(path)
-        if mix is not None and rank == 0:
-            with open(os.path.join(dirs['data'], 'demand_mix.json'), 'w') as f:
-                json.dump({'levels': mix.levels, 'labels': mix.labels}, f, indent=1)
-        out = _train(config, dirs, in_test, post_test, int(n_replicas), policy, device, pg, bool(summaries),
+        if rank == 0:
+            _save_config(dirs['data'], cfg, path)
+            if mix is not None:
+                with open(os.path.join(dirs['data'], 'demand_mix.json'), 'w') as f:
+                    json.dump({'levels': mix.levels, 'labels': mix.labels}, f, indent=1)
+        out = _train(cfg, dirs, in_test, post_test, int(n_replicas), policy, device, pg, bool(summaries),
                      bool(deterministic), mix)
     finally:
         for h in handlers:
@@ -591,11 +595,74 @@ def _schedule(config, env):
     return total_step, counter, T
 
 
+def _read_config(config):
+    """(ConfigParser, its path or None) of a config path or a parsed ConfigParser."""
+    if isinstance(config, configparser.ConfigParser):
+        return config, None
+    c = configparser.ConfigParser()
+    if not c.read(config):
+        raise FileNotFoundError(config)
+    return c, config
+
+
+def _save_config(data_dir, cfg, path=None, name='config.ini'):
+    """A run's config into its data/: a copy of the file `path` (as main.py copies it), else `cfg` written as `name`."""
+    if path is not None:
+        shutil.copy(path, data_dir)
+        return
+    with open(os.path.join(data_dir, name), 'w') as f:
+        cfg.write(f)
+
+
+def _summaries(model, agent, policy, T, log_dirs, device):
+    """(summary_rec, [Summaries]) of a run with summaries over K = len(log_dirs) members: the record the trainer fills
+    (A2C [T / n_step, 4], 5 columns with a teacher; IQL [ceil(T / n_step), N_ROUNDS, n_agent, 4]; with K > 1 a member
+    axis after the first) and one `Summaries` per log directory, with no writer for a directory of None."""
+    import torch
+    from .summary import SummaryWriter, summary_name
+    n_step, K = int(model.n_step), len(log_dirs)
+    if model.name == 'iql':
+        from .learner_iql import N_ROUNDS
+        tail = (N_ROUNDS, model.n_agent, 4)
+    else:
+        tail = (5 if getattr(model, 'teacher', None) else 4,)
+    rec = torch.zeros((-(-T // n_step),) + ((K,) if K > 1 else ()) + tail, dtype=torch.float32, device=device)
+    name = summary_name(agent, policy, getattr(model, 'model_type', None))
+    kind = 'iql' if model.name == 'iql' else 'a2c'
+    return rec, [Summaries(None if d is None else SummaryWriter(d), name, kind, n_step) for d in log_dirs]
+
+
+def _trainer(model, env, cfgs, total_step, T, rec, seed0, replica0=0, demand=None, demand_mix=None, coop_gamma=None,
+             sweep=False):
+    """The batched trainer of `model` on env's simulator, keeping a [T, R] reward trace: `BatchedIQLTrainer` with one
+    lr / ε schedule pair per config of cfgs (`member_schedulers`), or `BatchedTrainer` with the model's lr / β
+    schedules (one per member in a sweep), its teacher's arguments and the members' coop_gamma."""
+    import torch
+    sim = env._ensure_sim()
+    kw = dict(seed0=seed0, replica0=replica0, summary_rec=rec, demand=demand, demand_mix=demand_mix,
+              greward_trace=torch.zeros(T, sim.R, dtype=torch.float32, device=sim.device))
+    if model.name == 'iql':
+        from .learner_iql import BatchedIQLTrainer
+        lr, eps = member_schedulers([c['MODEL_CONFIG'] for c in cfgs], total_step)
+        return BatchedIQLTrainer(sim, model, lr, eps, **kw)
+    from .trainer import BatchedTrainer
+    lr, beta = (model.lr_schedulers, model.beta_schedulers) if sweep else (model.lr_scheduler, model.beta_scheduler)
+    return BatchedTrainer(sim, model.batched, model.name, lr, beta, coop_gamma=coop_gamma, **kw,
+                          **teacher_kwargs(model, env, sweep))
+
+
+def _evaluator(env_cfg, n_seeds, path, model, device):
+    """The batched Evaluator of `model` on a test env of its own (n_seeds test seeds), writing into `path`."""
+    from ..envs import make_env
+    from .evaluator import Evaluator
+    return Evaluator(make_env(env_cfg, n_seeds, path, is_record=False, device=device), model, path,
+                     policy_type='default')
+
+
 def _train(config, dirs, in_test, post_test, R_total, policy, device, pg, summaries=False, deterministic=False,
            mix=None):
     import torch
     from ..envs import make_env
-    from .evaluator import Evaluator
     env_cfg, mc = config['ENV_CONFIG'], config['MODEL_CONFIG']
     agent = env_cfg.get('agent')
     model_spec(agent)                                                 # reject greedy / a2c before any device work
@@ -610,55 +677,31 @@ def _train(config, dirs, in_test, post_test, R_total, policy, device, pg, summar
     if mix is not None:
         logging.info('Training: %d demand levels %s, replica g at level g mod %d'
                      % (len(mix.labels), mix.labels, len(mix.labels)))
-    mix_nets = None if mix is None else mix.nets
     total_step, counter, T = _schedule(config, env)
     seed = env_cfg.getint('seed')
     group, own_group = host_group(pg) if pg is not None else (None, False)
-    writer = None
+    summ = []
     try:
         model = build_model(agent, env, mc, total_step, R, policy=policy, seed=seed, device=device, replica0=replica0,
                             total_replicas=R_total, process_group=pg, deterministic=deterministic)
         sim = env._ensure_sim()
-        trace = torch.zeros(T, R, dtype=torch.float32, device=sim.device)
-        summary, srec = None, {}
+        rec = None
         if summaries:
-            from .summary import SummaryWriter, summary_name
-            n_step = int(model.n_step)
-            if model.name == 'iql':
-                from .learner_iql import N_ROUNDS
-                shape = (-(-T // n_step), N_ROUNDS, model.n_agent, 4)
-            else:
-                shape = (T // n_step, 5 if getattr(model, 'teacher', None) else 4)
-            srec = dict(summary_rec=torch.zeros(shape, dtype=torch.float32, device=sim.device))
+            rec, summ = _summaries(model, agent, policy, T, [dirs['log'] if rank == 0 else None], sim.device)
             if rank == 0:
-                writer = SummaryWriter(dirs['log'])
-                logging.info('Summaries: TensorBoard events into %s' % writer.path)
-            summary = Summaries(writer, summary_name(agent, policy, getattr(model, 'model_type', None)),
-                                'iql' if model.name == 'iql' else 'a2c', n_step)
-        if model.name == 'iql':
-            from .learner_iql import BatchedIQLTrainer
-            from .models import iql_schedulers
-            lr_s, eps_s = iql_schedulers(mc, total_step)
-            trainer = BatchedIQLTrainer(sim, model, lr_s, eps_s, seed0=seed, replica0=replica0, greward_trace=trace,
-                                        demand_mix=mix_nets, **srec)
-        else:
-            from .trainer import BatchedTrainer
-            trainer = BatchedTrainer(sim, model.batched, agent, model.lr_scheduler, model.beta_scheduler, seed0=seed,
-                                     replica0=replica0, greward_trace=trace, demand_mix=mix_nets, **srec,
-                                     **teacher_kwargs(model, env))
+                logging.info('Summaries: TensorBoard events into %s' % summ[0].writer.path)
+        trainer = _trainer(model, env, [config], total_step, T, rec, seed, replica0=replica0,
+                           demand_mix=None if mix is None else mix.nets)
         evaluator = None
         levels = None if mix is None else [(label, None) for label in mix.labels]
         if (in_test or post_test) and rank == 0:
-            test_env = make_env(env_cfg, len(env.test_seeds), dirs['data'], is_record=False, device=device)
-            evaluator = Evaluator(test_env, model, dirs['data'], policy_type='default')
+            n = len(env.test_seeds)
+            evaluator = _evaluator(env_cfg, n, dirs['data'], model, device)
             if mix is not None:                     # one evaluator per level, on the config edited to that level
-                levels = []
-                for label, c in zip(mix.labels, mix.configs):
-                    path = os.path.join(dirs['data'], label) + os.sep
-                    lv_env = make_env(c['ENV_CONFIG'], len(env.test_seeds), path, is_record=False, device=device)
-                    levels.append((label, Evaluator(lv_env, model, path, policy_type='default')))
-        driver = Trainer(trainer, evaluator, counter, agent, in_test, dirs['data'], group=group, summary=summary,
-                         levels=levels)
+                levels = [(label, _evaluator(c['ENV_CONFIG'], n, os.path.join(dirs['data'], label) + os.sep, model,
+                                             device)) for label, c in zip(mix.labels, mix.configs)]
+        driver = Trainer(trainer, evaluator, counter, agent, in_test, dirs['data'], group=group,
+                         summary=summ[0] if summ else None, levels=levels)
         driver.run()
         final_step = counter.cur_step
         if group is not None:
@@ -669,8 +712,9 @@ def _train(config, dirs, in_test, post_test, R_total, policy, device, pg, summar
         post = driver.run_offline() if post_test else None
         torch.cuda.synchronize(sim.device)
     finally:
-        if writer is not None:
-            writer.close()
+        for s in summ:
+            if s.writer is not None:
+                s.writer.close()
         if own_group:
             import torch.distributed as dist
             dist.destroy_process_group(group)
@@ -681,27 +725,37 @@ def _train(config, dirs, in_test, post_test, R_total, policy, device, pg, summar
                                  demand_post_test=driver.level_post)
 
 
-def _member_filter(k):
-    """Log records of member k, and those of no member in particular, go to member k's log file."""
-    return lambda rec: getattr(rec, 'member', k) == k
+def _a2c_agent(config, what, policy):
+    """The agent of an A2C population or sweep (`what`): refused for IQL agents and for the FC policy."""
+    agent = config['ENV_CONFIG'].get('agent')
+    if model_spec(agent)[0] == 'iql':
+        raise ValueError("a %s trains an A2C agent (ia2c or ma2c), not %r; train_iql_%s trains IQL members"
+                         % (what, agent, what))
+    if policy != 'lstm':
+        raise ValueError("a %s trains the LSTM policy only (got policy=%r)" % (what, policy))
+    return agent
 
 
-def _member_logs(dirs):
-    """One log file per member directory (`_member_filter`) and stderr, added to the root logger and returned."""
-    handlers = []
-    fmt = logging.Formatter('%(asctime)s [%(levelname)s] %(message)s')
-    for k, d in enumerate(dirs):
-        h = logging.FileHandler(os.path.join(d['log'], '%d.log' % time.time()))
-        h.setFormatter(fmt)
-        h.addFilter(_member_filter(k))
-        handlers.append(h)
-    handlers.append(logging.StreamHandler())
-    handlers[-1].setFormatter(fmt)
-    root = logging.getLogger()
-    for h in handlers:
-        root.addHandler(h)
-    root.setLevel(logging.INFO)
-    return handlers
+def _iql_agent(config, what):
+    agent = config['ENV_CONFIG'].get('agent')
+    if model_spec(agent)[0] != 'iql':
+        raise ValueError("%s trains an IQL agent (iqll or iqld), not %r; train(seeds=) and train_sweep train A2C "
+                         "members" % (what, agent))
+    return agent
+
+
+def _population(config, base_dir, seeds, agent_of):
+    """(seeds, member configs, member directories, name of their configs in data/) of a population: the seeds parsed,
+    the config read and its agent checked by agent_of(config), which returns it; member k's config is the config with
+    `[ENV_CONFIG] seed = seeds[k]` and its directory `member_dir(base_dir, seeds[k], agent)`."""
+    seeds = parse_seeds(seeds if isinstance(seeds, str) else ','.join(str(int(x)) for x in seeds))
+    config, path = _read_config(config)
+    agent = agent_of(config)
+    cfgs = []
+    for s in seeds:
+        cfgs.append(copy.deepcopy(config))
+        cfgs[-1]['ENV_CONFIG']['seed'] = str(s)
+    return seeds, cfgs, [member_dir(base_dir, s, agent) for s in seeds], os.path.basename(path) if path else 'config.ini'
 
 
 def train_population(config, base_dir, seeds, test_mode='no_test', n_replicas=1, policy='lstm', device=0,
@@ -715,108 +769,32 @@ def train_population(config, base_dir, seeds, test_mode='no_test', n_replicas=1,
     log/<time>.log and, with `summaries`, the member's event file.  Returns a namespace like train()'s with per-member
     lists `dirs`, `data`, `post_test` and `members`.  `deterministic`: as in train(); member k then equals its solo
     deterministic run bit for bit."""
-    import copy
     from .learner import check_population
     t0 = time.time()
     in_test, post_test = init_test_flag(test_mode)
-    seeds = parse_seeds(','.join(str(int(x)) for x in seeds)) if not isinstance(seeds, str) else parse_seeds(seeds)
-    if isinstance(config, configparser.ConfigParser):
-        name = 'config.ini'
-    else:
-        path, name, config = config, os.path.basename(config), configparser.ConfigParser()
-        if not config.read(path):
-            raise FileNotFoundError(path)
-    agent = config['ENV_CONFIG'].get('agent')
-    kind, _ = model_spec(agent)
-    if kind == 'iql':
-        raise ValueError("a population trains an A2C agent (ia2c or ma2c), not %r; train_iql_population trains IQL "
-                         "members" % agent)
-    if policy != 'lstm':
-        raise ValueError("a population trains the LSTM policy only (got policy=%r)" % policy)
+    seeds, cfgs, paths, name = _population(config, base_dir, seeds, lambda c: _a2c_agent(c, 'population', policy))
     check_population(seeds, 0, n_replicas, 1024, None)               # before any directory or device work
-    _check_imitation([config])
-    cfgs, dirs = [], []
-    for s in seeds:
-        cfg = copy.deepcopy(config)
-        cfg['ENV_CONFIG']['seed'] = str(s)
-        d = init_dir(member_dir(base_dir, s, agent))
-        with open(os.path.join(d['data'], name), 'w') as f:
-            cfg.write(f)
-        cfgs.append(cfg); dirs.append(d)
-    out = _train_members(cfgs, dirs, agent, seeds, int(n_replicas), in_test, post_test, policy, device, summaries,
-                         'population of %d seeds %s' % (len(seeds), seeds), deterministic=deterministic)
-    out.dirs, out.wall_sec = [member_dir(base_dir, s, agent) for s in seeds], time.time() - t0
+    _check_imitation(cfgs[:1])
+    out = _train_members(cfgs, paths, int(n_replicas), in_test, post_test, device, summaries, policy=policy,
+                         deterministic=deterministic, config_name=name)
+    out.wall_sec = time.time() - t0
     return out
 
 
-def _train_members(cfgs, dirs, agent, seeds, R_m, in_test, post_test, policy, device, summaries, what, sweep=False,
-                   deterministic=False, demand=None):
-    """The training run of a population or a sweep, member k from cfgs[k] (seed seeds[k]) into the agent directory
-    dirs[k] (init_dir's dict): member-tagged log files, one simulator and one learner for all K * R_m replicas, one
-    driver per member.  A sweep gives each member its own learner values and schedules (`IA2C(member_configs=...)`)
-    and, for ma2c, its own coop_gamma in the simulator; `demand` (member_demand) gives member k the demand of
-    demand[k]."""
-    import torch
-    from ..envs import make_env
-    from .evaluator import Evaluator
-    from .trainer import BatchedTrainer
-    K = len(cfgs)
-    root, handlers = logging.getLogger(), _member_logs(dirs)
-    writers = []
-    cg = [c['ENV_CONFIG'].getfloat('coop_gamma') for c in cfgs] if sweep and agent == 'ma2c' else None
-    if cg is not None and len(set(cg)) == 1:
-        cg = None                                                     # one coop_gamma: the simulator's own
-    # the training simulator marks the observation entries it scales only when built with a coop_gamma other than 1
-    base = next((k for k in range(K) if cg[k] != 1.0), 0) if cg is not None else 0
-    try:
-        env_cfg, mc = cfgs[base]['ENV_CONFIG'], cfgs[0]['MODEL_CONFIG']
-        env = make_env(env_cfg, K * R_m, dirs[0]['data'], is_record=False, device=device)
-        logging.info('Training: s dim: %d, s dim ls: %r, a dim ls: %r, %s x %d replicas'
-                     % (env.n_s, env.n_s_ls, env.n_a_ls, what, R_m))
-        total_step, counter, T = _schedule(cfgs[0], env)
-        model = build_model(agent, env, mc, total_step, R_m, seeds=seeds, device=device,
-                            member_configs=[c['MODEL_CONFIG'] for c in cfgs] if sweep else None,
-                            deterministic=deterministic)
-        members = model.members()
-        sim = env._ensure_sim()
-        trace = torch.zeros(T, K * R_m, dtype=torch.float32, device=sim.device)
-        srec, summ = {}, None
-        if summaries:
-            from .summary import SummaryWriter, summary_name
-            shape = (T // model.n_step,) + ((K,) if K > 1 else ()) + (5 if model.teacher else 4,)
-            srec = dict(summary_rec=torch.zeros(shape, dtype=torch.float32, device=sim.device))
-            writers = [SummaryWriter(d['log']) for d in dirs]
-            summ = [Summaries(w, summary_name(agent, policy), 'a2c', model.n_step) for w in writers]
-        lr, beta = (model.lr_schedulers, model.beta_schedulers) if sweep else (model.lr_scheduler, model.beta_scheduler)
-        trainer = BatchedTrainer(sim, model.batched, agent, lr, beta, seed0=seeds[0], greward_trace=trace,
-                                 coop_gamma=cg, demand=demand, **srec, **teacher_kwargs(model, env, sweep))
-        drivers = []
-        for k in range(K):                  # one driver per member, over its view of the shared trainer
-            evaluator = None
-            if in_test or post_test:
-                test_env = make_env(cfgs[k]['ENV_CONFIG'], len(env.test_seeds), dirs[k]['data'], is_record=False,
-                                    device=device)
-                evaluator = Evaluator(test_env, members[k], dirs[k]['data'], policy_type='default')
-            drivers.append(Trainer(trainer.member(k), evaluator, counter, agent, in_test, dirs[k]['data'],
-                                   summary=summ[k] if summ else None, log_extra={'member': k}))
-        run_schedule(drivers)
-        post = [None] * K
-        for k, d in enumerate(drivers):
-            logging.info('Training: save final model at step %d ...' % counter.cur_step, extra=d.log_extra)
-            members[k].save(dirs[k]['model'], counter.cur_step)
-            if post_test:
-                post[k] = d.run_offline()
-        torch.cuda.synchronize(sim.device)
-    finally:
-        for w in writers:
-            w.close()
-        for h in handlers:
-            root.removeHandler(h)
-            h.close()
-    return types.SimpleNamespace(final_step=counter.cur_step, episode_sets=drivers[0].n_episode_sets,
-                                 env_samples=counter.cur_step * K * R_m, world=1, rank=0, seeds=seeds,
-                                 data=[d.data for d in drivers], post_test=post, model=model, members=members,
-                                 trainer=trainer)
+def train_iql_population(config, base_dir, seeds, test_mode='no_test', n_replicas=1, device=0, summaries=False):
+    """Train K = len(seeds) members of one IQL agent (iqll / iqld) in one process, member k with `[ENV_CONFIG] seed =
+    seeds[k]` on `n_replicas` replicas.  One simulator launch, one grouped ε-greedy forward per control step and one
+    grouped TD / Adam update per round cover all K * n_replicas replicas (`BatchedIQL` with seeds); the schedules, the
+    tests and every file are per member.  Member k's directory `member_dir(base_dir, seeds[k], agent)` is, bit for bit,
+    what `train(config with seed seeds[k], n_replicas=n_replicas)` leaves (the log's times aside).  Everything is
+    checked before any directory is made.  Returns a namespace like train_population's."""
+    t0 = time.time()
+    in_test, post_test = init_test_flag(test_mode)
+    seeds, cfgs, paths, name = _population(config, base_dir, seeds, lambda c: _iql_agent(c, 'train_iql_population'))
+    _check_imitation(cfgs[:1])
+    out = _train_members(cfgs, paths, int(n_replicas), in_test, post_test, device, summaries, config_name=name)
+    out.wall_sec = time.time() - t0
+    return out
 
 
 # the config keys a sweep's members may set for themselves; every other key must be equal in all of them
@@ -940,79 +918,15 @@ def train_sweep(configs, base_dir, test_mode='no_test', n_replicas=64, device=0,
         raise ValueError('a sweep trains in one process: it takes no process_group')
     keys = dict(SWEEP_CONFIG_KEYS, MODEL_CONFIG=SWEEP_CONFIG_KEYS['MODEL_CONFIG'] + IMITATION_SWEEP_KEYS)
     items = sweep_members(configs, keys, demand=vary_demand)
-    agent = items[0][1]['ENV_CONFIG'].get('agent')
-    kind, _ = model_spec(agent)
-    if kind == 'iql':
-        raise ValueError("a sweep trains an A2C agent (ia2c or ma2c), not %r; train_iql_sweep trains IQL members" % agent)
-    if policy != 'lstm':
-        raise ValueError("a sweep trains the LSTM policy only (got policy=%r)" % policy)
-    cfgs = [c for _, c, _ in items]
+    agent = _a2c_agent(items[0][1], 'sweep', policy)
+    cfgs, names = [c for _, c, _ in items], [n for n, _, _ in items]
     _check_imitation(cfgs)
-    seeds = [c['ENV_CONFIG'].getint('seed') for c in cfgs]
-    check_sweep(seeds, [a2c_hparams(c['MODEL_CONFIG']) for c in cfgs], n_replicas, 1024, None)
-    demand = member_demand(cfgs) if vary_demand else None
-    names, dirs = [n for n, _, _ in items], []
-    for name, cfg, path in items:
-        d = init_dir(sweep_dir(base_dir, name, agent))
-        if path is not None:
-            shutil.copy(path, d['data'])                              # as train() copies its config
-        else:
-            with open(os.path.join(d['data'], 'config.ini'), 'w') as f:
-                cfg.write(f)
-        dirs.append(d)
-    out = _train_members(cfgs, dirs, agent, seeds, int(n_replicas), in_test, post_test, policy, device, summaries,
-                         'sweep of %d configs %s' % (len(cfgs), names), sweep=True, deterministic=deterministic,
-                         demand=demand)
-    out.names, out.dirs = names, [sweep_dir(base_dir, n, agent) for n in names]
+    check_sweep([c['ENV_CONFIG'].getint('seed') for c in cfgs], [a2c_hparams(c['MODEL_CONFIG']) for c in cfgs],
+                n_replicas, 1024, None)
+    out = _train_members(cfgs, [sweep_dir(base_dir, n, agent) for n in names], int(n_replicas), in_test, post_test,
+                         device, summaries, policy=policy, deterministic=deterministic, names=names,
+                         srcs=[p for _, _, p in items], demand=member_demand(cfgs) if vary_demand else None)
     out.wall_sec = time.time() - t0
-    return out
-
-
-def _read_config(config):
-    """(ConfigParser, name of its copy in data/) of a config path or a parsed ConfigParser."""
-    if isinstance(config, configparser.ConfigParser):
-        return config, 'config.ini'
-    c = configparser.ConfigParser()
-    if not c.read(config):
-        raise FileNotFoundError(config)
-    return c, os.path.basename(config)
-
-
-def _iql_agent(config, what):
-    agent = config['ENV_CONFIG'].get('agent')
-    if model_spec(agent)[0] != 'iql':
-        raise ValueError("%s trains an IQL agent (iqll or iqld), not %r; train(seeds=) and train_sweep train A2C "
-                         "members" % (what, agent))
-    return agent
-
-
-def train_iql_population(config, base_dir, seeds, test_mode='no_test', n_replicas=1, device=0, summaries=False):
-    """Train K = len(seeds) members of one IQL agent (iqll / iqld) in one process, member k with `[ENV_CONFIG] seed =
-    seeds[k]` on `n_replicas` replicas.  One simulator launch, one grouped ε-greedy forward per control step and one
-    grouped TD / Adam update per round cover all K * n_replicas replicas (`BatchedIQL` with seeds); the schedules, the
-    tests and every file are per member.  Member k's directory `member_dir(base_dir, seeds[k], agent)` is, bit for bit,
-    what `train(config with seed seeds[k], n_replicas=n_replicas)` leaves (the log's times aside).  Everything is
-    checked before any directory is made.  Returns a namespace like train_population's."""
-    import copy
-    t0 = time.time()
-    in_test, post_test = init_test_flag(test_mode)
-    seeds = parse_seeds(seeds if isinstance(seeds, str) else ','.join(str(int(x)) for x in seeds))
-    config, name = _read_config(config)
-    agent = _iql_agent(config, 'train_iql_population')
-    _check_imitation([config])
-    cfgs = []
-    for s in seeds:
-        cfg = copy.deepcopy(config)
-        cfg['ENV_CONFIG']['seed'] = str(s)
-        cfgs.append(cfg)
-    paths = [member_dir(base_dir, s, agent) for s in seeds]
-
-    def write(k, d):
-        with open(os.path.join(d['data'], name), 'w') as f:
-            cfgs[k].write(f)
-    out = _train_iql_members(cfgs, paths, write, agent, seeds, int(n_replicas), in_test, post_test, device, summaries,
-                             'population of %d seeds %s' % (len(seeds), seeds), sweep=False)
-    out.dirs, out.wall_sec = paths, time.time() - t0
     return out
 
 
@@ -1027,22 +941,12 @@ def train_iql_sweep(configs, base_dir, test_mode='no_test', n_replicas=1, device
     in_test, post_test = init_test_flag(test_mode)
     items = sweep_members(configs, IQL_SWEEP_CONFIG_KEYS, demand=vary_demand)
     agent = _iql_agent(items[0][1], 'train_iql_sweep')
-    cfgs = [c for _, c, _ in items]
+    cfgs, names = [c for _, c, _ in items], [n for n, _, _ in items]
     _check_imitation(cfgs)
-    seeds = [c['ENV_CONFIG'].getint('seed') for c in cfgs]
-    names = [n for n, _, _ in items]
-    paths = [sweep_dir(base_dir, n, agent) for n in names]
-    demand = member_demand(cfgs) if vary_demand else None
-
-    def write(k, d):
-        if items[k][2] is not None:
-            shutil.copy(items[k][2], d['data'])                       # as train() copies its config
-        else:
-            with open(os.path.join(d['data'], 'config.ini'), 'w') as f:
-                cfgs[k].write(f)
-    out = _train_iql_members(cfgs, paths, write, agent, seeds, int(n_replicas), in_test, post_test, device, summaries,
-                             'sweep of %d configs %s' % (len(cfgs), names), sweep=True, demand=demand)
-    out.names, out.dirs, out.wall_sec = names, paths, time.time() - t0
+    out = _train_members(cfgs, [sweep_dir(base_dir, n, agent) for n in names], int(n_replicas), in_test, post_test,
+                         device, summaries, names=names, srcs=[p for _, _, p in items],
+                         demand=member_demand(cfgs) if vary_demand else None)
+    out.wall_sec = time.time() - t0
     return out
 
 
@@ -1056,50 +960,49 @@ def member_schedulers(model_configs, total_step):
     return [p[0] for p in pairs], [p[1] for p in pairs]
 
 
-def _train_iql_members(cfgs, paths, write_config, agent, seeds, R_m, in_test, post_test, device, summaries, what,
-                       sweep, demand=None):
-    """The training run of IQL members: member k from cfgs[k] into the agent directory paths[k].  The environment and
-    the learner (which refuses what it cannot train) are built before any directory is made; then the directories, their
-    configs (write_config(k, dirs)), member-tagged log files, one simulator and one learner for all K * R_m replicas, and
-    one driver per member."""
+def _train_members(cfgs, paths, R_m, in_test, post_test, device, summaries, policy='lstm', deterministic=False,
+                   config_name='config.ini', names=None, srcs=None, demand=None):
+    """The training run of a population, or with `names` a sweep, of A2C or IQL members: member k from cfgs[k] into the
+    agent directory paths[k].  The env and the learner (which refuses what it cannot train) are built before any
+    directory is made; then the directories with their configs (a copy of srcs[k], else cfgs[k] written as
+    `config_name`), member-tagged log files, and one driver per member over one simulator, learner and trainer for all
+    K * R_m replicas.  A sweep gives each member its own learner values and schedules and, for ma2c, its own coop_gamma
+    in the simulator; `demand` (member_demand) gives member k the demand of demand[k]."""
     import torch
     from ..envs import make_env
-    from .evaluator import Evaluator
-    from .learner_iql import N_ROUNDS, BatchedIQLTrainer
-    K = len(cfgs)
-    mc = cfgs[0]['MODEL_CONFIG']
-    data0 = os.path.join(paths[0], 'data') + os.sep
-    env = make_env(cfgs[0]['ENV_CONFIG'], K * R_m, data0, is_record=False, device=device)
+    K, sweep = len(cfgs), names is not None
+    agent = cfgs[0]['ENV_CONFIG'].get('agent')
+    seeds = [c['ENV_CONFIG'].getint('seed') for c in cfgs]
+    cg = [c['ENV_CONFIG'].getfloat('coop_gamma') for c in cfgs] if sweep and agent == 'ma2c' else None
+    if cg is not None and len(set(cg)) == 1:
+        cg = None                                                     # one coop_gamma: the simulator's own
+    # the training simulator marks the observation entries it scales only when built with a coop_gamma other than 1
+    base = next((k for k in range(K) if cg[k] != 1.0), 0) if cg is not None else 0
+    env = make_env(cfgs[base]['ENV_CONFIG'], K * R_m, os.path.join(paths[0], 'data') + os.sep, is_record=False,
+                   device=device)
     total_step, counter, T = _schedule(cfgs[0], env)
-    model = build_model(agent, env, mc, total_step, R_m, seeds=seeds, device=device,
-                        member_configs=[c['MODEL_CONFIG'] for c in cfgs] if sweep else None)
+    model = build_model(agent, env, cfgs[0]['MODEL_CONFIG'], total_step, R_m, seeds=seeds, device=device,
+                        member_configs=[c['MODEL_CONFIG'] for c in cfgs] if sweep else None,
+                        deterministic=deterministic)
     dirs = [init_dir(p) for p in paths]
     for k, d in enumerate(dirs):
-        write_config(k, d)
-    root, handlers = logging.getLogger(), _member_logs(dirs)
-    writers = []
+        _save_config(d['data'], cfgs[k], srcs[k] if srcs else None, config_name)
+    handlers, summ = init_log([d['log'] for d in dirs]), []
     try:
+        what = 'sweep of %d configs %s' % (K, names) if sweep else 'population of %d seeds %s' % (K, seeds)
         logging.info('Training: s dim: %d, s dim ls: %r, a dim ls: %r, %s x %d replicas'
                      % (env.n_s, env.n_s_ls, env.n_a_ls, what, R_m))
-        members = [model.member(k) for k in range(K)]
+        members = [model.member(k) for k in range(K)] if model.name == 'iql' else model.members()
         sim = env._ensure_sim()
-        trace = torch.zeros(T, K * R_m, dtype=torch.float32, device=sim.device)
-        srec, summ = {}, None
+        rec = None
         if summaries:
-            from .summary import SummaryWriter, summary_name
-            shape = (-(-T // model.n_step),) + ((K,) if K > 1 else ()) + (N_ROUNDS, model.n_agent, 4)
-            srec = dict(summary_rec=torch.zeros(shape, dtype=torch.float32, device=sim.device))
-            writers = [SummaryWriter(d['log']) for d in dirs]
-            summ = [Summaries(w, summary_name(agent, 'lstm', model.model_type), 'iql', model.n_step) for w in writers]
-        lr_s, eps_s = member_schedulers([c['MODEL_CONFIG'] for c in cfgs], total_step)
-        trainer = BatchedIQLTrainer(sim, model, lr_s, eps_s, seed0=seeds[0], greward_trace=trace, demand=demand, **srec)
+            rec, summ = _summaries(model, agent, policy, T, [d['log'] for d in dirs], sim.device)
+        trainer = _trainer(model, env, cfgs, total_step, T, rec, seeds[0], demand=demand, coop_gamma=cg, sweep=sweep)
         drivers = []
         for k in range(K):                  # one driver per member, over its view of the shared trainer
             evaluator = None
             if in_test or post_test:
-                test_env = make_env(cfgs[k]['ENV_CONFIG'], len(env.test_seeds), dirs[k]['data'], is_record=False,
-                                    device=device)
-                evaluator = Evaluator(test_env, members[k], dirs[k]['data'], policy_type='default')
+                evaluator = _evaluator(cfgs[k]['ENV_CONFIG'], len(env.test_seeds), dirs[k]['data'], members[k], device)
             drivers.append(Trainer(trainer.member(k), evaluator, counter, agent, in_test, dirs[k]['data'],
                                    summary=summ[k] if summ else None, log_extra={'member': k}))
         run_schedule(drivers)
@@ -1111,13 +1014,15 @@ def _train_iql_members(cfgs, paths, write_config, agent, seeds, R_m, in_test, po
                 post[k] = d.run_offline()
         torch.cuda.synchronize(sim.device)
     finally:
-        for w in writers:
-            w.close()
+        for s in summ:
+            s.writer.close()
         for h in handlers:
-            root.removeHandler(h)
+            logging.getLogger().removeHandler(h)
             h.close()
-    return types.SimpleNamespace(final_step=counter.cur_step, episode_sets=drivers[0].n_episode_sets,
-                                 env_samples=counter.cur_step * K * R_m, world=1, rank=0, seeds=seeds,
-                                 data=[d.data for d in drivers], post_test=post, model=model, members=members,
-                                 trainer=trainer)
-
+    out = types.SimpleNamespace(final_step=counter.cur_step, episode_sets=drivers[0].n_episode_sets,
+                                env_samples=counter.cur_step * K * R_m, world=1, rank=0, seeds=seeds,
+                                data=[d.data for d in drivers], post_test=post, model=model, members=members,
+                                trainer=trainer, dirs=paths)
+    if sweep:
+        out.names = names
+    return out
